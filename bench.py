@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — formula-images/sec of one full im2latex train step (BASELINE.json metric).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--precision bf16|fp32]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--precision bf16|fp32] [--dump-outputs DIR]
 
 N=1 workload = BASELINE.json configs[1]: batch 64, 1x128x512 images, 6-conv encoder + 512-d attention LSTM
 decoder, vocab 500, every caption padded to T=150 decode steps (the reference trains on PADs,
@@ -13,6 +13,11 @@ skipped.  `value` times K steps with inputs resident in HBM (CUDA events, max ov
 K steps through Img2SeqModel.train_step with PINNED HOST inputs (H2D inside) and a D2H read of the loss.
 `--impl reference` times the reference's CPU algorithm (oracle port, un-hoisted exactly as the reference
 executes it) on the host cores of rank 0.
+`--dump-outputs DIR` writes what the last timed step computed as DIR/<name>.npy (float64 loss vector, float32 parameters
+after its Adam update; a fixed sample of the larger ones): weights, inputs and dropout draws are seeded, so two builds
+can be compared output for output.  It also turns on the library's "deterministic" option (cross-CTA reductions in a fixed
+order instead of fp32 atomics; slower), so that two runs of one build write identical arrays; timings taken with it are
+those of that mode.
 """
 import argparse
 import json
@@ -37,7 +42,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], tf=d["bf16_tflops"], tf_sustained=d.get("bf16_tflops_sustained", d["bf16_tflops"]), src="measured")
-    return dict(hbm=6650.0, tf=1590.0, tf_sustained=1400.0, src="fallback")
+    return dict(hbm=3350.0, tf=989.0, tf_sustained=989.0, src="fallback: H100 SXM data sheet (dense bf16), not measured")
 
 
 class ClockSampler:
@@ -129,12 +134,15 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours")
     ap.add_argument("--precision", default="bf16")
-    ap.add_argument("--kernels", default=os.environ.get("LO_IMPL", "tc"), help="simt | tc (tcgen05 convs/GEMMs)")
+    ap.add_argument("--kernels", default=os.environ.get("LO_IMPL", "tc"), help="simt | tc (wgmma convs/GEMMs)")
     ap.add_argument("--batch", type=int, default=CFG2["B"])
     ap.add_argument("--no-graph", action="store_true")
     ap.add_argument("--skip-cpu-baseline", action="store_true")
     ap.add_argument("--skip-decode", action="store_true", help="omit the cfg #5 decode probe (N=1 only)")
     ap.add_argument("--workload", default="cfg2", choices=["cfg2", "cfg4"], help="cfg4 = the row-encoder / two-layer EXTENSION")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the loss and updated parameters of the last timed step as DIR/<name>.npy (runs in the "
+                         "library's deterministic mode)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -167,7 +175,10 @@ def main():
         cuda_graph = (not args.no_graph) and (world == 1 or os.environ.get("LO_DP_GRAPH", "1") == "1")
     kernels = args.kernels
     if kernels == "tc" and not bs.tc_ready():
-        kernels = "simt"
+        raise SystemExit("bench: --kernels tc needs the wgmma/TMA kernels (sm_90 device); lo_tc_available() is 0")
+    torch.manual_seed(1234 + rank)             # parameter init and the dropout seed: identical from run to run
+    if args.dump_outputs:
+        _lib.set_option("deterministic", 1)    # the dumped step must not depend on the arrival order of fp32 atomics
     if args.workload == "cfg4":
         from latex_ocr_b200.ext import Img2SeqRowModel as ModelCls
     else:
@@ -205,6 +216,7 @@ def main():
     e1.record()
     barrier()
     ms = e0.elapsed_time(e1) / args.steps
+    dump = bs.step_outputs(model, loss) if args.dump_outputs and rank == 0 else None
     clocks = sampler.stop() if rank == 0 else None
     launches_eager = _lib.launch_count() - l0
     final_loss = float(loss[0].item())
@@ -225,6 +237,8 @@ def main():
     ms, ms_e2e = t[0].item(), t[1].item()
     log("e2e: %.2f ms/step" % ms_e2e)
     per_step_launches = bs.launches_per_step(model, img_dev, formula_dev)
+    if dump is not None:
+        bs.write_outputs(args.dump_outputs, dump)
 
     def finish():
         """N > 1: every rank waits here until rank 0 has printed its line, then the process leaves WITHOUT tearing the NCCL
@@ -268,7 +282,8 @@ def main():
         "config": {"workload": "cfg2: batch %d/GPU, 1x128x512 images, 6-conv encoder + 512-d attention LSTM decoder, vocab 500, "
                                "T=150 teacher-forced steps (PADs trained on, as the reference)" % c["B"],
                    "global_batch": total_imgs, "parallelism": "dp%d" % world, "kernels": kernels, "cuda_graph": bool(Cfg.cuda_graph),
-                   "l2": "per-step working set (>1 GB of feature maps + 114 MB attention stream) exceeds the 126 MB L2; no explicit flush",
+                   "deterministic": bool(args.dump_outputs),
+                   "l2": "per-step working set (>1 GB of feature maps + 114 MB attention stream) exceeds the 50 MB L2; no explicit flush",
                    "loss_after": final_loss},
         "e2e": {"value": total_imgs / (ms_e2e / 1e3), "unit": "images/s", "ms_per_step": ms_e2e,
                 "h2d_bytes_per_step": int(img.numel() * 1 + formula.numel() * 8), "d2h_bytes_per_step": 4,

@@ -29,6 +29,34 @@ def synthetic_batch(B, H, W, V, T, seed):
     return img, formula
 
 
+DUMP_SAMPLE = 1 << 20     # parameters larger than this are dumped as a fixed sample: a dump of either workload stays < 64 MB
+
+
+def step_outputs(model, loss):
+    """Host copies of what one train step hands its caller: the loss vector [total, ce, reg, n_valid] (float64) and every
+    parameter after the step's Adam update (float32; tensors above DUMP_SAMPLE elements as a fixed, seeded sample of
+    their flattened values).  Taken right after the timed steps, before anything else updates the parameters."""
+    out = {"loss": loss.detach().double().cpu().numpy()}
+    for mod in ("encoder", "decoder", "row_encoder", "layer2"):
+        m = getattr(model, mod, None)
+        if m is None:
+            continue
+        for name, t in m.state_dict().items():
+            flat = t.detach().float().reshape(-1)
+            if flat.numel() > DUMP_SAMPLE:
+                idx = torch.randperm(flat.numel(), generator=torch.Generator().manual_seed(0))[:DUMP_SAMPLE].sort().values
+                flat = flat[idx.to(flat.device)]
+            out["%s.%s" % (mod, name)] = flat.cpu().numpy()
+    return out
+
+
+def write_outputs(directory, arrays):
+    import numpy as np
+    os.makedirs(directory, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(directory, name + ".npy"), a)
+
+
 def launches_per_step(model, img_dev, formula_dev):
     """Kernels launched by ONE train step (counted on an eager replay of the same step body)."""
     from latex_ocr_b200 import _lib
@@ -95,21 +123,8 @@ def kernel_probes(model, c, pk):
     _lib.set_option("att_abi_pdl", 1)
     ms_att = _time_ms(att_steps_mask if maskbits else att_steps, 3) / T
     att_bytes = B * R * (A + C) * bpe + B * R * 4 + (B * R * A // 8 if maskbits else 0)
-    traffic_tab = {}
-    try:
-        import json
-        traffic_tab = json.load(open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "profiles", "r2_traffic.json")))
-    except Exception:
-        pass
-
-    def traffic_of(kernel):
-        """dram__bytes_read + dram__bytes_write per launch of `kernel` from this round's `ncu --set full` capture (profiles/
-        r2_traffic.json is written by tools/ncu_traffic.py from the committed raw CSVs); null off the profiled shape."""
-        e = traffic_tab.get(kernel)
-        return e["bytes"] if (e and B == 64 and R == 868 and bpe == 2) else None
-
     att = {"kernel": "attention_fwd_pipe_kernel (score + softmax + context + gate, one decode step, TMA ring)", "bound": "hbm",
-           "achieved": att_bytes / (ms_att * 1e-3) / 1e9, "peak": pk["hbm"], "unit": "GB/s", "traffic": traffic_of("attention_fwd_pipe_kernel"),
+           "achieved": att_bytes / (ms_att * 1e-3) / 1e9, "peak": pk["hbm"], "unit": "GB/s", "traffic": None,
            "us_per_launch": ms_att * 1e3, "algorithmic_bytes": att_bytes, "peak_source": pk["src"]}
     att["frac"] = att["achieved"] / att["peak"]
 
@@ -137,7 +152,7 @@ def kernel_probes(model, c, pk):
                       + ("; streams enc + the forward's mask bits instead of enc + att1" if maskbits else "")
                       + ("; both contractions on mma.sync)" if mma else ")"), "bound": "hbm",
             "achieved": attb_bytes / (ms_attb * 1e-3) / 1e9, "peak": pk["hbm"], "unit": "GB/s",
-            "traffic": traffic_of(kname), "us_per_launch": ms_attb * 1e3, "algorithmic_bytes": attb_bytes,
+            "traffic": None, "us_per_launch": ms_attb * 1e3, "algorithmic_bytes": attb_bytes,
             "peak_source": pk["src"]}
     attb["frac"] = attb["achieved"] / attb["peak"]
 
@@ -152,10 +167,10 @@ def kernel_probes(model, c, pk):
     flops = B * 56.0e9
     conv = {"kernel": "conv stack fwd+dgrad+wgrad (6 layers, incl. pools/ReLU masks)", "bound": "tensor",
             "achieved": flops / (ms_conv * 1e-3) / 1e12, "peak": pk["tf_sustained"], "unit": "TFLOP/s", "traffic": None,
-            "ms": ms_conv, "algorithmic_flops": flops, "peak_source": pk["src"] + " (sustained cuBLAS bf16)"}
+            "ms": ms_conv, "algorithmic_flops": flops, "peak_source": pk["src"]}
     conv["frac"] = conv["achieved"] / conv["peak"]
 
-    # the tcgen05 kernels alone (layers 2-6: forward, data gradient, weight gradient) — what SURVEY §8-d calls the tensor-pipe
+    # the wgmma kernels alone (layers 2-6: forward, data gradient, weight gradient) — what SURVEY §8-d calls the tensor-pipe
     # figure (conv1 / pools / masks / bias-gradient column sums are memory-bound CUDA-core kernels and are excluded here)
     from latex_ocr_b200.encoder import _LAYERS
     Aa, Gg, S = enc_ws["acts"], enc_ws["grads"], enc.store
@@ -181,11 +196,11 @@ def kernel_probes(model, c, pk):
 
     ms_tc = _time_ms(conv_tc, 3)
     flops_tc = B * 3 * 2 * 9.296e9     # layers 2-6: 9.296 GMAC/image, x3 passes (fwd, dgrad, wgrad)
-    conv_tc_r = {"kernel": "tcgen05 conv kernels only: tc_conv_p_kernel (persistent, 128x256 tiles, fwd + dgrad) and tc_wgrad_kernel, "
+    conv_tc_r = {"kernel": "wgmma conv kernels only: tc_conv_p_kernel (persistent, 128x256 tiles, fwd + dgrad) and tc_wgrad_kernel, "
                            "layers 2-6 (15 launches)", "bound": "tensor",
                  "achieved": flops_tc / (ms_tc * 1e-3) / 1e12, "peak": pk["tf_sustained"], "unit": "TFLOP/s",
-                 "traffic": traffic_of("tc_conv_p_kernel"), "traffic_note": "mean DRAM bytes per tc_conv_p_kernel launch (ncu)", "ms": ms_tc,
-                 "algorithmic_flops": flops_tc, "peak_source": pk["src"] + " (sustained cuBLAS bf16)"}
+                 "traffic": None, "ms": ms_tc,
+                 "algorithmic_flops": flops_tc, "peak_source": pk["src"]}
     conv_tc_r["frac"] = conv_tc_r["achieved"] / conv_tc_r["peak"]
 
     def dec_all():

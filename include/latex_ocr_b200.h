@@ -1,5 +1,5 @@
 /*
- * latex_ocr_b200 — C ABI of the B200-native (sm_100a) im2latex hot path.
+ * latex_ocr_b200 — C ABI of the H100-native (sm_90a) im2latex hot path.
  *
  * The reference (LinXueyuanStdio/LaTeX_OCR) has no FFI: its boundary is the Python class surface
  * (SURVEY.md §8-b).  Each entry point below replaces the library call(s) the reference makes at the
@@ -37,10 +37,10 @@ extern "C" {
 #define LO_OK 0
 #define LO_EINVAL (-1)   /* bad argument / unsupported shape */
 #define LO_ECUDA (-2)    /* a CUDA runtime call or launch failed */
-#define LO_ENOTSUP (-3)  /* path not available on this device (needs sm_100) */
+#define LO_ENOTSUP (-3)  /* path not available on this device (needs sm_90) */
 
 #define LO_IMPL_SIMT 0   /* CUDA-core kernels (fp32 or bf16 storage) — the tight-parity path */
-#define LO_IMPL_TC 1     /* tcgen05 + TMA kernels (bf16 storage only) */
+#define LO_IMPL_TC 1     /* wgmma + TMA kernels (bf16 storage only) */
 
 int lo_version(void);
 const char* lo_last_error(void);
@@ -50,7 +50,9 @@ int64_t lo_launch_count(void);
  * "att_policy_att1" (L2 policy 0 normal, 1 evict_last, 2 evict_first), "att_nsplit" (0 = automatic), "pdl", "att_abi_pdl" (above);
  * schedule variants, each parity-tested against the default (tests/test_gpu_tc.py, DESIGN.md §8): "att_maskbits", "att_bwd_mma",
  * "skinny_mma", "skinny_tma", "fuse_lstm", "dec_streams", "dec_fuse", "dec_fuse_bwd", "dec_cl", "dec_cl_bwd", "conv_persist",
- * "conv_mt2", "conv_mc", "wgrad256"; "dbg_skip" is a timing-dissection aid (results are garbage).  LO_OPTS=name=value,... in the
+ * "conv_mt2", "conv_mc", "wgrad256"; "deterministic" (1: every cross-CTA reduction of the train step
+ * adds its partial sums in a fixed order, so a seeded run is bit-reproducible — slower; 0, default: fp32 atomics whose rounding
+ * depends on arrival order); "dbg_skip" is a timing-dissection aid (results are garbage).  LO_OPTS=name=value,... in the
  * environment sets them at load time (Python side). */
 int lo_set_option(const char* name, int value);
 /* current value of a tuning knob (-1: unknown name) */
@@ -59,10 +61,10 @@ int lo_get_option(const char* name);
  * persisting carve-out sized to fit; bytes = 0 resets.  The attention kernels honour it with att_policy_enc/att1 = 3
  * (bulk copies without an explicit cache hint). */
 int lo_set_l2_window(const void* base, int64_t bytes, float hit_ratio, void* stream);
-/* development aid: device buffer (>= 16 int64) that CTA (0,0,0) of the tcgen05 NT GEMM stamps with clock64 at its
+/* development aid: device buffer (>= 16 int64) that CTA (0,0,0) of the wgmma NT GEMM stamps with clock64 at its
  * pipeline milestones; NULL disables */
 int lo_debug_buffer(void* p);
-/* 1 if the tcgen05/TMA kernels are built in and the current device is sm_100 */
+/* 1 if the wgmma/TMA kernels are built in and the current device is sm_90 */
 int lo_tc_available(void);
 
 /* ------------------------------------------------------------------------------------------------
@@ -96,7 +98,9 @@ int lo_conv1_pool_forward_u8(const uint8_t* img, const float* w, const float* bi
 int lo_conv1_pool_wgrad_u8(const uint8_t* img, const float* w, const float* bias, const void* dpool, int dt,
                            float* dw, float* db, int N, int H, int W, void* stream);
 /* conv1 weight/bias gradient from the POOLED output gradient; recomputes conv1 to find the
- * ReLU mask and pool argmax (first maximum in window scan order, as PyTorch) */
+ * ReLU mask and pool argmax (first maximum in window scan order, as PyTorch).  All conv1 weight-gradient entry points write dw / db
+ * (no accumulation).  With lo_set_option("deterministic", 1) their per-block partial sums go through a device buffer of the
+ * library (summed in block order), so two of them must not then run concurrently on the same device. */
 int lo_conv1_pool_wgrad(const float* img, const float* w, const float* bias, const void* dpool, int dt,
                         float* dw, float* db, int N, int H, int W, void* stream);
 /* the same two kernels with the pixel normalisation x' = x * scale + offset applied to in-bounds pixels (zero padding stays
@@ -197,7 +201,7 @@ typedef struct lo_decoder_args {
   int32_t has_dropout;     /* 0: eval ; 1: multiply h by dropout_mask before fc (injected mask: parity tests) ;
                               2: draw the inverted-dropout mask inside the LSTM kernels (Philox4x32-10 keyed by dropout_state,
                                  regenerated in the backward; nothing is stored) */
-  int32_t ldl;             /* row stride of logits/dlogits (>= V; a multiple of 64 enables the tcgen05 fc GEMMs); 0 -> V */
+  int32_t ldl;             /* row stride of logits/dlogits (>= V; a multiple of 64 enables the wgmma fc GEMMs); 0 -> V */
   float alpha_c;           /* doubly-stochastic regulariser weight (img2seq_torch.py:157) */
   int32_t rows_per_img;    /* decode only: consecutive rows that share one image (beam size); 0/1 for training */
   int32_t phase;           /* 0: whole call (default).  EXTENSION (a second decoder layer between the cell and fc): 1 = time loop
@@ -268,7 +272,7 @@ typedef struct lo_decoder_args {
   float* g_w_init; float* g_b_init;
   float* g_w_fc; float* g_b_fc;
   void* work;              /* lo_decoder_workspace_bytes(B, max(A,C)), zero-initialised once */
-  void* bfwork;            /* optional (impl=TC, dt=bf16): bf16 staging for the hoisted tcgen05 GEMMs,
+  void* bfwork;            /* optional (impl=TC, dt=bf16): bf16 staging for the hoisted wgmma GEMMs,
                               lo_decoder_bfwork_bytes(args) bytes */
 } lo_decoder_args;
 

@@ -1,4 +1,4 @@
-"""In-tree build of the C-ABI library: nvcc -> latex_ocr_b200/_C/liblatex_ocr_b200.so (sm_100a only)."""
+"""In-tree build of the C-ABI library: nvcc -> latex_ocr_b200/_C/liblatex_ocr_b200.so (sm_90a only)."""
 import os
 import subprocess
 import sys
@@ -9,7 +9,7 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, os.environ.get("LO_LIB_DIR", "_C"))      # LO_LIB_DIR: build a tuning variant next to the product library
 LIB = os.path.join(OUT, "liblatex_ocr_b200.so")
 SOURCES = ["lo_gemm.cu", "lo_conv.cu", "lo_decoder.cu", "lo_attention.cu", "lo_skinny.cu", "lo_cluster.cu", "lo_optim.cu", "lo_tc.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xptxas", "-v"] + os.environ.get("LO_NVCC_EXTRA", "").split()
 
 
@@ -55,7 +55,7 @@ def build(force=False, verbose=False):
                     print("compiled", s)
     objs = [os.path.join(OUT, s.replace(".cu", ".o")) for s in SOURCES]
     if force or jobs or _stale(LIB, objs):
-        cmd = [_nvcc(), "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"]
+        cmd = [_nvcc(), "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError("link failed:\n" + r.stderr[-4000:])

@@ -862,9 +862,9 @@ __global__ void __launch_bounds__(AP_THREADS, LO_ATT_MINB) attention_bwd_mask_ke
 
 // ------------------------------------------------------------------------------------------------------------------------------
 // [r2b] Tensor-core backward for the 512-wide torch flavour (bf16): the two contractions of the step run on mma.sync instead of
-// CUDA-core FMAs / predicated adds (2.5x fewer warp instructions).  Measured: the launch was NOT issue-bound — 17.35 vs 17.44 us
-// (run 60); what it loses it loses at its ends (DESIGN.md section 4) — but the tensor-core version frees the issue slots and,
-// with alpha / d reg staged in shared memory and the tail operands fetched up front, runs at 15.7 us:
+// CUDA-core FMAs / predicated adds (2.5x fewer warp instructions).  The launch is not issue-bound — what it loses it loses at its
+// ends — but the tensor-core version frees the issue slots, and alpha / d reg are staged in shared memory and the tail operands
+// fetched up front:
 //   d[r]     = sum_c enc[r][c] * dctx[c]          A = 16 enc rows straight from the ring (ldmatrix), B = dctx split into bf16 hi+lo
 //                                                  (columns 0/1 of B, products exact, fp32 accumulation)
 //   datt2[a] = sum_r bit[r][a] * de[r]            A = mask bits expanded to bf16 {0, 2.0} with ONE shift + ONE and per register,
@@ -1004,8 +1004,8 @@ __global__ void __launch_bounds__(AP_THREADS, 2) attention_bwd_mma_kernel(
     }
     const float sreg_b = sreg ? sreg[(int64_t)b * sreg_stride] : 0.f;
     // alpha and the regulariser gradient of this CTA's rows are forward-pass results: ALL of them are staged in shared memory before
-    // the wait.  (Fetching them stage by stage with a one-stage lookahead made every 16-row stage cost one L2 round trip, ~0.8 us: the
-    // main loop then ran at 3.5 TB/s whatever the arithmetic was — run 62 timeline.)
+    // the wait.  (Fetching them stage by stage with a one-stage lookahead makes every 16-row stage cost one L2 round trip, which then
+    // bounds the main loop whatever the arithmetic is.)
     const float* alb = alpha + (int64_t)b * alpha_stride;
     float* deb = de + (int64_t)b * alpha_stride;
     const float* drb = dreg + (int64_t)b * dreg_stride;
@@ -1165,10 +1165,8 @@ __global__ void __launch_bounds__(AP_THREADS, 2) attention_bwd_mma_kernel(
 int att_pipe_splits(int B, int hint = 0) {
   if (g_opt_att_nsplit > 0) return g_opt_att_nsplit > AP_MAXSPLIT ? AP_MAXSPLIT : g_opt_att_nsplit;      // explicit option wins
   if (hint > 0) return hint > 8 ? 8 : hint;
-  // two CTAs per SM are resident (smem): one full wave of <= 296 CTAs.  Measured at B=64, R=868 (bf16): 4 splits
-  // (256 CTAs, 14 stages each) 25.9 us vs 9 splits (576 CTAs = 2 waves) 32.8 us — per-CTA start-up/combine
-  // costs dominate short CTAs (profiles/r1_attention_nsplit_sweep.txt)
-  int s = (148 * LO_ATT_MINB) / B;
+  // two CTAs per SM are resident (smem): aim for one full wave — per-CTA start-up/combine costs dominate short CTAs
+  int s = (LO_NUM_SMS * LO_ATT_MINB) / B;
   if (s < 1) s = 1;
   if (s > AP_MAXSPLIT) s = AP_MAXSPLIT;
   if (g_opt_att_cluster && s > 8) s = 8;       // portable cluster size limit
@@ -1416,6 +1414,7 @@ extern "C" int lo_get_option(const char* name) {
   if (!strcmp(name, "conv_persist")) return lo::g_opt_conv_persist;
   if (!strcmp(name, "wgrad256")) return lo::g_opt_wgrad256;
   if (!strcmp(name, "conv_mt2")) return lo::g_opt_conv_mt2;
+  if (!strcmp(name, "deterministic")) return lo::g_opt_det;
   if (!strcmp(name, "dec_fuse")) return lo::g_opt_dec_fuse;
   if (!strcmp(name, "dec_cl")) return lo::g_opt_dec_cl;
   if (!strcmp(name, "dec_cl_bwd")) return lo::g_opt_dec_cl_bwd;
@@ -1443,6 +1442,7 @@ extern "C" int lo_set_option(const char* name, int value) {
   else if (!strcmp(name, "conv_persist")) lo::g_opt_conv_persist = value;
   else if (!strcmp(name, "wgrad256")) lo::g_opt_wgrad256 = value;
   else if (!strcmp(name, "conv_mt2")) lo::g_opt_conv_mt2 = value;
+  else if (!strcmp(name, "deterministic")) lo::g_opt_det = value;
   else if (!strcmp(name, "dec_streams")) { lo::g_opt_dec_streams = value; lo::g_opt_skinny8 = value >= 2 ? 0 : 1; }
   else if (!strcmp(name, "skinny8")) lo::g_opt_skinny8 = value;
   else if (!strcmp(name, "fuse_lstm")) lo::g_opt_fuse_lstm = value;

@@ -3,10 +3,9 @@
 //
 // Why a cluster and not the grid: batch rows are independent in the recurrence (seq2seq_torch.py:304-316), so a block of 16 rows
 // (one mma M tile) can be carried through [gates GEMM -> LSTM cell -> next projection] by 16 CTAs that split the OUTPUT columns
-// and exchange the 16 x 512 state through DSMEM behind a hardware cluster barrier (~0.3 us).  The grid-wide versions
+// and exchange the 16 x 512 state through DSMEM behind a hardware cluster barrier.  The grid-wide versions
 // (dec_step_fwd_kernel / dec_step_bwd_kernel, lo_skinny.cu) needed an all-to-all through L2 — a kernel boundary or a 192-CTA
-// atomic barrier, ~3 us each, three per direction and step: run 61 measured 16.3 us (forward) / 13.0 us (backward) per step for the
-// three small launches against ~1 us of math.  Here 4 clusters (64 rows) x 16 CTAs stream each their 320 KB slice of the weights
+// atomic barrier, three per direction and step, each costing more than the step's math.  Here 4 clusters (64 rows) x 16 CTAs stream each their 320 KB slice of the weights
 // from L2 through a cp.async ring (weights are parameters: the ring is filled before griddepcontrol.wait).
 //
 // forward  (after attention(t)):   gates = (gate*ctx)_t W_ih[:, E:]^T (+ table row + hh) -> LSTM cell -> h_{t+1}, c_{t+1}
@@ -24,8 +23,8 @@ namespace cg = cooperative_groups;
 
 namespace lo {
 
-// measured (runs 63-65): 16.3 / 18.3 us per launch against 15.6 / 13.0 us for the three separate launches — each CTA has to pull its
-// 320 KB weight slice through ONE SM's load path (~30 GB/s with cp.async), and 4 clusters use only 64 of the 148 SMs.  Off by default.
+// Off by default: each CTA has to pull its 320 KB weight slice through ONE SM's load path, and 4 clusters use only 64 of the
+// 132 SMs, so the fused step was slower than the three separate launches it replaces.
 int g_opt_dec_cl = 0;       // cluster-fused forward step
 int g_opt_dec_cl_bwd = 0;   // cluster-fused backward step
 

@@ -1,4 +1,4 @@
-// Shared device/host helpers for the latex_ocr_b200 kernels (sm_100a only).
+// Shared device/host helpers for the latex_ocr_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -50,6 +50,9 @@ inline int fail(int code, const char* fmt, const char* a = "", long b = 0, long 
 
 inline int cdiv(long a, long b) { return (int)((a + b - 1) / b); }
 
+// SMs of the H100 SXM: caps the grids of the grid-stride kernels and sets the split-K / split-count targets
+constexpr int LO_NUM_SMS = 132;
+
 // kernel launch with (optionally) the programmatic-dependent-launch attribute; kernels launched this way call
 // pdl_wait() before touching global memory
 extern int g_opt_pdl;
@@ -65,6 +68,32 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = g_opt_pdl ? 1 : 0;
+  return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
+}
+// the same with a thread-block cluster of `cl` CTAs (a divisor of the grid; <= 8, or <= 16 for kernels that allow the
+// non-portable size) and optional PDL
+template <typename... KArgs, typename... Args>
+inline cudaError_t launch_cluster(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, dim3 cl, bool pdl,
+                                  Args... args) {
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = grid;
+  cfg.blockDim = block;
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = st;
+  cudaLaunchAttribute attr[2];
+  int n = 0;
+  attr[n].id = cudaLaunchAttributeClusterDimension;
+  attr[n].val.clusterDim.x = cl.x;
+  attr[n].val.clusterDim.y = cl.y;
+  attr[n].val.clusterDim.z = cl.z;
+  n++;
+  if (pdl && g_opt_pdl) {
+    attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[n].val.programmaticStreamSerializationAllowed = 1;
+    n++;
+  }
+  cfg.attrs = attr;
+  cfg.numAttrs = n;
   return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
 }
 
@@ -228,12 +257,15 @@ extern int g_opt_conv_mc;
 extern int g_opt_conv_persist;
 extern int g_opt_wgrad256;
 extern int g_opt_conv_mt2;
+// 1: every cross-CTA reduction of the train step adds its partial sums in a fixed order (thread-block clusters / per-block slots,
+// lo_ptx.cuh:cl_sum) so that a run is bit-reproducible; 0 (default): fp32 atomics, faster, rounding depends on arrival order
+extern int g_opt_det;
 extern int g_opt_dec_streams;
 extern int g_opt_skinny8;
 int attention_fwd_pipe(const AttFwdArgs& x, int dt, int C, cudaStream_t st);
 int attention_bwd_pipe(const AttBwdArgs& x, int dt, int C, cudaStream_t st);
 
-// tcgen05 paths (lo_tc.cu)
+// wgmma paths (lo_tc.cu)
 bool tc_available();
 int tc_gemm_nt(const bf16* A, int64_t lda, const bf16* W, int64_t ldw, void* C, int dtC, int64_t ldc,
                int M, int N, int K, const float* bias, int accumulate, int relu, cudaStream_t st);

@@ -1,6 +1,6 @@
 // Encoder kernels, CUDA-core versions (fp32 or bf16 storage, fp32 accumulate): the 6-conv "vanilla"
 // stack of seq2seq_torch.py:31-57 in NHWC with [Cout][3][3][Cin] weights, its data/weight gradients,
-// the max-pools and the timing-signal add.  The tcgen05/TMA implicit-GEMM convolution is in lo_tc.cu.
+// the max-pools and the timing-signal add.  The wgmma/TMA implicit-GEMM convolution is in lo_tc.cu.
 #include "lo_common.cuh"
 
 namespace lo {
@@ -69,6 +69,45 @@ __global__ void __launch_bounds__(256) conv1_pool_fwd_kernel(const TI* __restric
   }
 }
 
+// conv1 weight / bias gradient: every block adds its partial sums (64 channels x (9 taps + bias)) onto the zeroed dw / db with fp32
+// atomics.  Option "deterministic": it stores them in its own slot of g_conv1_part instead and conv1_wgrad_reduce_kernel adds the
+// slots in block order; the slots are a device buffer of the library, so with that option two conv1 weight-gradient calls must not
+// run concurrently on one device.
+constexpr int C1_PART = 64 * 10;
+constexpr int C1_MAXBLOCKS = LO_NUM_SMS * 4;
+__device__ float g_conv1_part[C1_MAXBLOCKS][C1_PART];
+
+__device__ __forceinline__ void conv1_wgrad_block_partial(const float (&gw)[8][9], const float (&gb)[8], int cg, int lane, float* dw,
+                                                          float* db, int ordered) {
+  float* part = g_conv1_part[blockIdx.x];
+#pragma unroll
+  for (int c = 0; c < 8; c++) {
+    const float s = warp_sum(gb[c]);
+    if (lane == 0) {
+      if (ordered) part[(cg * 8 + c) * 10 + 9] = s;
+      else atomicAdd(db + cg * 8 + c, s);
+    }
+#pragma unroll
+    for (int k = 0; k < 9; k++) {
+      const float t = warp_sum(gw[c][k]);
+      if (lane == 0) {
+        if (ordered) part[(cg * 8 + c) * 10 + k] = t;
+        else atomicAdd(dw + (cg * 8 + c) * 9 + k, t);
+      }
+    }
+  }
+}
+
+__global__ void conv1_wgrad_reduce_kernel(float* __restrict__ dw, float* __restrict__ db, int nblocks) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= C1_PART) return;
+  float s = 0.f;
+  for (int b = 0; b < nblocks; b++) s += g_conv1_part[b][i];
+  const int c = i / 10, k = i % 10;
+  if (k == 9) db[c] = s;
+  else dw[c * 9 + k] = s;
+}
+
 // conv1 weight gradient from the arg-max / ReLU codes the forward kernel saved: no recomputation of conv1 (36 of the 84 FMA slots
 // per pooled output and channel), the 3x3 window of the winning position is selected with 21 selects instead of 27 masked FMAs.
 // warp <-> 8 channels, lane <-> pooled position (as conv1_pool_wgrad_kernel below).
@@ -76,7 +115,7 @@ template <typename T, typename TI>
 __global__ void __launch_bounds__(256) conv1_pool_wgrad_code_kernel(const TI* __restrict__ img, const uint8_t* __restrict__ code,
                                                                      const T* __restrict__ dpool, float* __restrict__ dw,
                                                                      float* __restrict__ db, int N, int H, int W, float pscale,
-                                                                     float poff) {
+                                                                     float poff, int ordered) {
   const int Hp = H / 2, Wp = W / 2;
   const int lane = threadIdx.x & 31, cg = threadIdx.x >> 5;
   const int64_t npos = (int64_t)N * Hp * Wp;
@@ -127,16 +166,7 @@ __global__ void __launch_bounds__(256) conv1_pool_wgrad_code_kernel(const TI* __
         for (int q = 0; q < 3; q++) gw[c][r * 3 + q] = fmaf(gg, py ? xc[r + 1][q] : xc[r][q], gw[c][r * 3 + q]);
     }
   }
-#pragma unroll
-  for (int c = 0; c < 8; c++) {
-    float s = warp_sum(gb[c]);
-    if (lane == 0) atomicAdd(db + cg * 8 + c, s);
-#pragma unroll
-    for (int k = 0; k < 9; k++) {
-      float t = warp_sum(gw[c][k]);
-      if (lane == 0) atomicAdd(dw + (cg * 8 + c) * 9 + k, t);
-    }
-  }
+  conv1_wgrad_block_partial(gw, gb, cg, lane, dw, db, ordered);
 }
 
 // conv1 weight gradient from the pooled-output gradient (recompute conv1 -> argmax + ReLU mask).
@@ -145,7 +175,7 @@ template <typename T, typename TI>
 __global__ void __launch_bounds__(256) conv1_pool_wgrad_kernel(const TI* __restrict__ img, const float* __restrict__ w,
                                                                 const float* __restrict__ bias, const T* __restrict__ dpool,
                                                                 float* __restrict__ dw, float* __restrict__ db,
-                                                                int N, int H, int W, float pscale, float poff) {
+                                                                int N, int H, int W, float pscale, float poff, int ordered) {
   __shared__ float sw[64 * 9];
   __shared__ float sb[64];
   for (int i = threadIdx.x; i < 64 * 9; i += blockDim.x) sw[i] = w[i];
@@ -212,16 +242,7 @@ __global__ void __launch_bounds__(256) conv1_pool_wgrad_kernel(const TI* __restr
         }
     }
   }
-#pragma unroll
-  for (int c = 0; c < 8; c++) {
-    float s = warp_sum(gb[c]);
-    if (lane == 0) atomicAdd(db + cg * 8 + c, s);
-#pragma unroll
-    for (int k = 0; k < 9; k++) {
-      float t = warp_sum(gw[c][k]);
-      if (lane == 0) atomicAdd(dw + (cg * 8 + c) * 9 + k, t);
-    }
-  }
+  conv1_wgrad_block_partial(gw, gb, cg, lane, dw, db, ordered);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -478,7 +499,7 @@ __global__ void relu_mask_cast_kernel(const float* __restrict__ g, const T* __re
 
 static inline int grid_for(int64_t work, int threads) {
   int64_t b = (work + threads - 1) / threads;
-  const int64_t cap = 148 * 16;
+  const int64_t cap = LO_NUM_SMS * 16;
   return (int)(b < 1 ? 1 : (b > cap ? cap : b));
 }
 
@@ -580,26 +601,32 @@ static int conv1_fwd(const void* img, int u8, const float* w, const float* bias,
 static int conv1_wgrad(const void* img, int u8, const float* w, const float* bias, const void* dpool, int dt, float* dw, float* db,
                        int N, int H, int W, cudaStream_t st, float pscale = 1.f, float poff = 0.f, const uint8_t* code = nullptr) {
   LO_CHECK_ARG(img && w && bias && dpool && dw && db, "null pointer");
-  LO_CUDA(cudaMemsetAsync(dw, 0, 64 * 9 * sizeof(float), st));
-  LO_CUDA(cudaMemsetAsync(db, 0, 64 * sizeof(float), st));
+  const int ordered = g_opt_det;
+  if (!ordered) {
+    LO_CUDA(cudaMemsetAsync(dw, 0, 64 * 9 * sizeof(float), st));
+    LO_CUDA(cudaMemsetAsync(db, 0, 64 * sizeof(float), st));
+  }
   const int64_t npos = (int64_t)N * (H / 2) * (W / 2);
   int grid = (int)((npos + 31) / 32);
-  if (grid > 148 * 4) grid = 148 * 4;
+  if (grid > C1_MAXBLOCKS) grid = C1_MAXBLOCKS;
   if (code) {
     if (u8) {
-      LO_DISPATCH_DT(dt, T, (conv1_pool_wgrad_code_kernel<T, uint8_t><<<grid, 256, 0, st>>>((const uint8_t*)img, code, (const T*)dpool, dw, db, N, H, W, pscale, poff)));
+      LO_DISPATCH_DT(dt, T, (conv1_pool_wgrad_code_kernel<T, uint8_t><<<grid, 256, 0, st>>>((const uint8_t*)img, code, (const T*)dpool, dw, db, N, H, W, pscale, poff, ordered)));
     } else {
-      LO_DISPATCH_DT(dt, T, (conv1_pool_wgrad_code_kernel<T, float><<<grid, 256, 0, st>>>((const float*)img, code, (const T*)dpool, dw, db, N, H, W, pscale, poff)));
+      LO_DISPATCH_DT(dt, T, (conv1_pool_wgrad_code_kernel<T, float><<<grid, 256, 0, st>>>((const float*)img, code, (const T*)dpool, dw, db, N, H, W, pscale, poff, ordered)));
     }
     LO_LAUNCH_OK();
-    return LO_OK;
-  }
-  if (u8) {
-    LO_DISPATCH_DT(dt, T, (conv1_pool_wgrad_kernel<T, uint8_t><<<grid, 256, 0, st>>>((const uint8_t*)img, w, bias, (const T*)dpool, dw, db, N, H, W, pscale, poff)));
+  } else if (u8) {
+    LO_DISPATCH_DT(dt, T, (conv1_pool_wgrad_kernel<T, uint8_t><<<grid, 256, 0, st>>>((const uint8_t*)img, w, bias, (const T*)dpool, dw, db, N, H, W, pscale, poff, ordered)));
+    LO_LAUNCH_OK();
   } else {
-    LO_DISPATCH_DT(dt, T, (conv1_pool_wgrad_kernel<T, float><<<grid, 256, 0, st>>>((const float*)img, w, bias, (const T*)dpool, dw, db, N, H, W, pscale, poff)));
+    LO_DISPATCH_DT(dt, T, (conv1_pool_wgrad_kernel<T, float><<<grid, 256, 0, st>>>((const float*)img, w, bias, (const T*)dpool, dw, db, N, H, W, pscale, poff, ordered)));
+    LO_LAUNCH_OK();
   }
-  LO_LAUNCH_OK();
+  if (ordered) {
+    conv1_wgrad_reduce_kernel<<<cdiv(C1_PART, 128), 128, 0, st>>>(dw, db, grid);
+    LO_LAUNCH_OK();
+  }
   return LO_OK;
 }
 
@@ -677,8 +704,8 @@ int lo_conv3x3(const void* x, const void* w, const float* bias, const void* mask
   LO_CHECK_ARG(H + 2 * pad - 2 > 0 && W + 2 * pad - 2 > 0, "output would be empty");
   cudaStream_t st = (cudaStream_t)stream;
   if (impl == LO_IMPL_TC) {
-    LO_CHECK_ARG(dt == LO_BF16, "tcgen05 path needs bf16 storage");
-    if (!tc_available()) return fail(LO_ENOTSUP, "%s: tcgen05 path requires an sm_100 device", __func__);
+    LO_CHECK_ARG(dt == LO_BF16, "wgmma path needs bf16 storage");
+    if (!tc_available()) return fail(LO_ENOTSUP, "%s: wgmma path requires an sm_90 device", __func__);
     return tc_conv3x3((const bf16*)x, (const bf16*)w, bias, (const bf16*)mask, (bf16*)y, N, H, W, Cin, Cout, pad, relu, st);
   }
   const int Ho = H + 2 * pad - 2, Wo = W + 2 * pad - 2;
@@ -703,7 +730,7 @@ int lo_conv3x3_wgrad(const void* x, const void* dy, float* dw, float* db, int dt
     return LO_OK;
   }
   const int tiles = 9 * cdiv(Cin, 64) * cdiv(Cout, 64);
-  int splits = cdiv(148 * 4, tiles);
+  int splits = cdiv(LO_NUM_SMS * 4, tiles);
   const int maxs = (int)((P + 511) / 512);
   if (splits > maxs) splits = maxs;
   if (splits < 1) splits = 1;

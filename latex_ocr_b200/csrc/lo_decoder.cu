@@ -287,7 +287,9 @@ __global__ void __launch_bounds__(LO_ATT_THREADS) attention_bwd_kernel(
 // hoisted d att1 / d w_full: ONE sweep over att1 after the time loop.
 //   datt1[b,r,a] = wf[a] * sum_t de[b,t,r] * [att1[b,r,a] + att2[t,b,a] > 0]
 //   dwf[a]      += sum_{b,r,t} de[b,t,r] * relu(att1[b,r,a] + att2[t,b,a])
-// grid (A/64, ceil(R/32), B), 128 threads, thread tile 4(r) x 4(a), time chunks of 32 staged in smem.
+// grid (A/64, ceil(R/(32 nchunk)), B), 128 threads, thread tile 4(r) x 4(a), time chunks of 32 staged in smem.  d w_full: each
+// block adds its sums onto dwf[A] with fp32 atomics, or (dwf_rows, option "deterministic") the row blocks of a batch row (<= 16)
+// form one cluster and dwf is a [B][A] scratch (row b += that batch row's sum, added in block order).
 // ------------------------------------------------------------------------------------------------
 // WACC: 0 = d att1 only; 1 = also all of d w_full; 2 = only the `x * (sum_t on * de)` term of d w_full (ReLU): the other term,
 // sum_{t,b} att2_t[b,a] * sum_r on * de_t[b,r], was accumulated per step by the mask-bit attention backward kernels (dwf_part)
@@ -295,17 +297,20 @@ template <typename T, int WACC, int ACT = 0>
 __global__ void __launch_bounds__(128) datt1_kernel(const T* __restrict__ att1, const float* __restrict__ out1,
                                                      int64_t o1_row, int64_t o1_step, const float* __restrict__ de,
                                                      const float* __restrict__ wf, T* __restrict__ datt1,
-                                                     float* __restrict__ dwf, int Tn, int R, int A) {
+                                                     float* __restrict__ dwf, int Tn, int R, int A, int nchunk, int dwf_rows) {
   constexpr int TT = 32;
   __shared__ __align__(16) float s_a2[TT][64];
   __shared__ __align__(16) float s_de[TT][32];
   __shared__ float s_w[8][64];
-  const int b = blockIdx.z, r0 = blockIdx.y * 32, a0 = blockIdx.x * 64;
+  const int b = blockIdx.z, a0 = blockIdx.x * 64;
   const int tx = threadIdx.x % 16, ty = threadIdx.x / 16;   // a = a0 + tx*4.., r = r0 + ty*4..
-  float x[4][4], nx[4][4], acc[4][4], wacc[4];
+  float wacc[4] = {0.f, 0.f, 0.f, 0.f};
+  for (int ch = 0; ch < nchunk; ch++) {                     // 32-row chunks of this block, in order
+  const int r0 = (blockIdx.y * nchunk + ch) * 32;
+  if (r0 >= R) break;
+  float x[4][4], nx[4][4], acc[4][4];
 #pragma unroll
   for (int i = 0; i < 4; i++) {
-    wacc[i] = 0.f;
     const int r = r0 + ty * 4 + i;
 #pragma unroll
     for (int j = 0; j < 4; j++) {
@@ -372,8 +377,7 @@ __global__ void __launch_bounds__(128) datt1_kernel(const T* __restrict__ att1, 
 #pragma unroll
     for (int j = 0; j < 4; j++) stf(datt1 + ((int64_t)b * R + r) * A + a0 + tx * 4 + j, acc[i][j] * wv[j]);
   }
-  if (!WACC) return;
-  if constexpr (ACT == 0) {
+  if constexpr (WACC != 0 && ACT == 0) {
 #pragma unroll
     for (int i = 0; i < 4; i++)
       if (r0 + ty * 4 + i < R) {
@@ -381,6 +385,8 @@ __global__ void __launch_bounds__(128) datt1_kernel(const T* __restrict__ att1, 
         for (int j = 0; j < 4; j++) wacc[j] = fmaf(x[i][j], acc[i][j], wacc[j]);      // the x * (sum_t on * de) term
       }
   }
+  }
+  if (!WACC) return;
 #pragma unroll
   for (int j = 0; j < 4; j++) s_w[ty][tx * 4 + j] = wacc[j];
   __syncthreads();
@@ -388,8 +394,17 @@ __global__ void __launch_bounds__(128) datt1_kernel(const T* __restrict__ att1, 
     float t = 0.f;
 #pragma unroll
     for (int k = 0; k < 8; k++) t += s_w[k][threadIdx.x];
-    atomicAdd(dwf + a0 + threadIdx.x, t);
+    s_w[0][threadIdx.x] = t;
   }
+  if (!dwf_rows) {
+    if (threadIdx.x < 64) atomicAdd(dwf + a0 + threadIdx.x, s_w[0][threadIdx.x]);
+    return;
+  }
+  // ordered: the row blocks of batch row b are one cluster; rank 0 adds their sums in order onto the row's [B][A] scratch (one
+  // writer per element; the caller sums the rows over b with colsum)
+  cl_sync();
+  if (cl_rank() == 0 && threadIdx.x < 64) dwf[(int64_t)b * A + a0 + threadIdx.x] += cl_sum(&s_w[0][threadIdx.x]);
+  cl_sync();
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -494,7 +509,7 @@ __global__ void lstm_pw_bwd_kernel(const float* __restrict__ dhd, int64_t dhd_st
     q[3 * D + j] = __float2bfloat16_rn(d[3 * D + j]);
   }
   if (dxh_zero) {
-    // the tcgen05 split-K GEMMs that follow accumulate with atomics: clear [dgctx | dh] (dh_next was consumed above;
+    // the wgmma split-K GEMMs that follow accumulate with atomics: clear [dgctx | dh] (dh_next was consumed above;
     // entry C+j is this thread's own read location, entries < C are never read here)
     float* z = dxh_zero + (int64_t)b * (C + D);
     z[C + j] = 0.f;
@@ -859,7 +874,7 @@ static inline Dims dims(const lo_decoder_args* a) {
   return Dims{a->B, a->T, a->R, a->C, a->A, a->D, a->E, a->V, a->A + a->C + 4 * a->D, 4 * a->D, a->ldl > 0 ? a->ldl : a->V};
 }
 
-// bf16 staging used when impl == TC: mirrors written by the step kernels feed the tcgen05 GEMMs directly
+// bf16 staging used when impl == TC: mirrors written by the step kernels feed the wgmma GEMMs directly
 struct BfViews {
   bool on;
   bf16 *dcat, *hall, *gctx, *wet, *onehot, *hd, *dlogits, *wfct, *wil, *alphas, *dctx, *dptab, *wihT;
@@ -971,10 +986,10 @@ __global__ void split_bf16_kernel(const float* __restrict__ x, bf16* __restrict_
   }
 }
 
-int g_opt_fuse_lstm = 0;   // measured slower (23.0 vs 20.1 ms/step): 128 epilogue threads cannot hide the dependent global loads
+int g_opt_fuse_lstm = 0;   // off: the epilogue threads cannot hide the dependent global loads
                            // (tok -> table row, recurrent projection, c) that 32 K threads of lstm_pw_fwd_kernel hide
 // wil[4*j + g][c] = w_ih[g*D + j][E + c]: gate-interleaved copy of the context half of weight_ih, so that one 32-column
-// accumulator chunk of the tcgen05 GEMM holds whole hidden units and the LSTM cell can run in its epilogue
+// accumulator chunk of the wgmma GEMM holds whole hidden units and the LSTM cell can run in its epilogue
 __global__ void interleave_wih_kernel(const bf16* __restrict__ w_ih, bf16* __restrict__ wil, int D, int E, int C) {
   const int64_t total = (int64_t)4 * D * (C / 8);
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
@@ -1027,7 +1042,7 @@ static int forward_prologue(const lo_decoder_args* a, const Dims& d, cudaStream_
   if (bv.on) {
     LO_TRY(lo_cast(a->hall, LO_F32, bv.hall, LO_BF16, (int64_t)d.B * d.D, (void*)st));
     if ((g_opt_fuse_lstm || g_opt_dec_fuse || g_opt_dec_cl) && d.E % 8 == 0 && d.C % 8 == 0) {
-      interleave_wih_kernel<<<148 * 2, 256, 0, st>>>((const bf16*)a->w_ih, bv.wil, d.D, d.E, d.C);
+      interleave_wih_kernel<<<LO_NUM_SMS * 2, 256, 0, st>>>((const bf16*)a->w_ih, bv.wil, d.D, d.E, d.C);
       LO_LAUNCH_OK();
     }
   }
@@ -1136,7 +1151,7 @@ static inline Rows chain_rows(const lo_decoder_args* a, const Dims& d, int chain
   r.nrows = hi - r.row0 > 0 ? hi - r.row0 : 0;
   if (chain == 0 && nchains == 1) r.nrows = active;
   r.work = (char*)a->work + (size_t)chain * lo_attention_workspace_bytes(d.B, d.C);
-  r.nsplit = nchains == 2 ? (148 / (half > 0 ? half : 1) > 0 ? 148 / half : 1) : 0;   // each chain fills one CTA slot per SM
+  r.nsplit = nchains == 2 ? (LO_NUM_SMS / (half > 0 ? half : 1) > 0 ? LO_NUM_SMS / half : 1) : 0;   // each chain fills one CTA slot per SM
   return r;
 }
 
@@ -1603,7 +1618,7 @@ int lo_decoder_backward(const lo_decoder_args* a, void* stream) {
   // embedding path through the projection table
   if (tc) {
     const int Vp = (d.V + 7) / 8 * 8;
-    onehot_kernel<<<148 * 8, 256, 0, st>>>(a->caps, a->caps_stride, work_dlen(a), bv.onehot, d.B, d.T, Vp);
+    onehot_kernel<<<LO_NUM_SMS * 8, 256, 0, st>>>(a->caps, a->caps_stride, work_dlen(a), bv.onehot, d.B, d.T, Vp);
     LO_LAUNCH_OK();
     LO_CUDA(cudaMemsetAsync(a->dptab, 0, (size_t)d.V * d.G * 4, st));
     LO_TRY(tc_gemm_tn(bv.onehot, Vp, dcat_bf + d.A + d.C, d.O1, a->dptab, d.G, d.V, d.G, d.T * d.B, st));
@@ -1614,7 +1629,7 @@ int lo_decoder_backward(const lo_decoder_args* a, void* stream) {
     LO_LAUNCH_OK();
   }
   if (tc && d.E % 64 == 0 && d.G % 64 == 0 && d.V >= 64) {
-    // g_emb = dptab W_ih[:, :E] and g_W_ih[:, :E] = dptab^T emb on tcgen05 (bf16 copy of dptab, transposed weight slice)
+    // g_emb = dptab W_ih[:, :E] and g_W_ih[:, :E] = dptab^T emb on wgmma (bf16 copy of dptab, transposed weight slice)
     LO_TRY(lo_cast(a->dptab, LO_F32, bv.dptab, LO_BF16, (int64_t)d.V * d.G, stream));
     transpose_kernel<bf16><<<dim3(cdiv(d.E, 32), cdiv(d.G, 32)), dim3(32, 8), 0, st>>>((const bf16*)a->w_ih, d.E + d.C, bv.wihT, d.G, d.G, d.E);
     LO_LAUNCH_OK();
@@ -1626,25 +1641,56 @@ int lo_decoder_backward(const lo_decoder_args* a, void* stream) {
     LO_TRY(gemm_tn(a->dptab, LO_F32, d.G, a->emb, dt, d.E, a->g_w_ih, LO_F32, d.E + d.C, d.G, d.E, d.V, 0, LO_IMPL_SIMT, st));
   }
   // d att1 + d w_full in one sweep over att1
-  LO_CUDA(cudaMemsetAsync(a->g_w_full, 0, (size_t)d.A * 4, st));
   LO_CUDA(cudaMemsetAsync(a->g_b_full, 0, 4, st));   // sum_r de = 0 exactly (softmax); reference value is rounding noise
-  {
+  const bool pipe_dwf = g_opt_att_pipe && !att_mask_at(a, 0, 0);   // d w_full accumulated per batch row by the attention backward
+  if (!g_opt_det) {
     dim3 grid(d.A / 64, cdiv(d.R, 32), d.B);
-    if (g_opt_att_pipe && !att_mask_at(a, 0, 0)) {
-      // d w_full was accumulated per batch row by the attention backward kernels (dmean doubles as the [B][A] scratch)
+    if (g_opt_att_pipe) {
+      // the per-step kernels' part of d w_full (all of it without mask bits, the att2 term with them) sits in dmean ([B][A] scratch)
       LO_TRY(colsum(a->dmean, LO_F32, a->g_w_full, d.B, d.A, d.A, 0, st));
+    } else {
+      LO_CUDA(cudaMemsetAsync(a->g_w_full, 0, (size_t)d.A * 4, st));
+    }
+    if (pipe_dwf) {
       LO_DISPATCH_DT(dt, T, (datt1_kernel<T, 0><<<grid, 128, 0, st>>>((const T*)a->att1, a->out1, d.O1, (int64_t)d.B * d.O1, a->de,
-                                                                       a->w_full, (T*)a->datt1, a->g_w_full, d.T, d.R, d.A)));
+                                                                       a->w_full, (T*)a->datt1, nullptr, d.T, d.R, d.A, 1, 0)));
     } else if (g_opt_att_pipe) {
-      // mask-bit scheme: the att2 term of d w_full came out of the per-step kernels (dmean scratch), the sweep adds the x term
-      LO_TRY(colsum(a->dmean, LO_F32, a->g_w_full, d.B, d.A, d.A, 0, st));
+      // mask-bit scheme: the sweep adds the x term
       LO_DISPATCH_DT(dt, T, (datt1_kernel<T, 2><<<grid, 128, 0, st>>>((const T*)a->att1, a->out1, d.O1, (int64_t)d.B * d.O1, a->de,
-                                                                       a->w_full, (T*)a->datt1, a->g_w_full, d.T, d.R, d.A)));
+                                                                       a->w_full, (T*)a->datt1, a->g_w_full, d.T, d.R, d.A, 1, 0)));
     } else {
       LO_DISPATCH_DT(dt, T, (datt1_kernel<T, 1><<<grid, 128, 0, st>>>((const T*)a->att1, a->out1, d.O1, (int64_t)d.B * d.O1, a->de,
-                                                                       a->w_full, (T*)a->datt1, a->g_w_full, d.T, d.R, d.A)));
+                                                                       a->w_full, (T*)a->datt1, a->g_w_full, d.T, d.R, d.A, 1, 0)));
     }
     LO_LAUNCH_OK();
+  } else {
+    // ordered: the sweep adds its d w_full part per batch row onto the dmean rows, then one colsum over b
+    const int nch = cdiv(cdiv(d.R, 32), 16);            // row chunks per block: <= 16 row blocks (one cluster) per batch row
+    static bool attr = false;
+    if (!attr) {
+      LO_CUDA(cudaFuncSetAttribute(datt1_kernel<float, 1>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+      LO_CUDA(cudaFuncSetAttribute(datt1_kernel<bf16, 1>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+      LO_CUDA(cudaFuncSetAttribute(datt1_kernel<float, 2>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+      LO_CUDA(cudaFuncSetAttribute(datt1_kernel<bf16, 2>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+      attr = true;
+    }
+    dim3 grid(d.A / 64, cdiv(d.R, 32 * nch), d.B);
+    const dim3 cl(1, grid.y, 1);
+    if (pipe_dwf) {
+      LO_DISPATCH_DT(dt, T, (datt1_kernel<T, 0><<<grid, 128, 0, st>>>((const T*)a->att1, a->out1, d.O1, (int64_t)d.B * d.O1, a->de,
+                                                                       a->w_full, (T*)a->datt1, nullptr, d.T, d.R, d.A, nch, 0)));
+    } else if (g_opt_att_pipe) {
+      LO_DISPATCH_DT(dt, T, LO_CUDA(launch_cluster(datt1_kernel<T, 2>, grid, dim3(128), 0, st, cl, false, (const T*)a->att1,
+                                                   (const float*)a->out1, (int64_t)d.O1, (int64_t)d.B * d.O1, (const float*)a->de,
+                                                   (const float*)a->w_full, (T*)a->datt1, a->dmean, d.T, d.R, d.A, nch, 1)));
+    } else {
+      LO_CUDA(cudaMemsetAsync(a->dmean, 0, (size_t)d.B * d.A * 4, st));
+      LO_DISPATCH_DT(dt, T, LO_CUDA(launch_cluster(datt1_kernel<T, 1>, grid, dim3(128), 0, st, cl, false, (const T*)a->att1,
+                                                   (const float*)a->out1, (int64_t)d.O1, (int64_t)d.B * d.O1, (const float*)a->de,
+                                                   (const float*)a->w_full, (T*)a->datt1, a->dmean, d.T, d.R, d.A, nch, 1)));
+    }
+    LO_LAUNCH_OK();
+    LO_TRY(colsum(a->dmean, LO_F32, a->g_w_full, d.B, d.A, d.A, 0, st));
   }
   // encoder_att: g_W = datt1^T enc ; g_b = colsum(datt1) ; denc = datt1 @ W_e
   if (tc) {
@@ -1660,11 +1706,11 @@ int lo_decoder_backward(const lo_decoder_args* a, void* stream) {
   LO_TRY(colsum(a->datt1, dt, a->g_b_enc_att, d.B * d.R, d.A, d.A, 0, st));
   // denc[b] += alphas[b]^T @ dctx[:, b, :]   (the context read, summed over time — a batched GEMM instead of a per-step RMW)
   if (tc && d.C % 8 == 0) {
-    // tcgen05, one launch (3-D tensor maps, grid.y = batch); bf16 operands cast once after the loop
+    // wgmma, one launch (3-D tensor maps, grid.y = batch); bf16 operands cast once after the loop
     const int Rp = (int)rpad8(d.R);
-    cast_pad_rows_kernel<<<148 * 8, 256, 0, st>>>(a->alphas, bv.alphas, BT, d.R, Rp);
+    cast_pad_rows_kernel<<<LO_NUM_SMS * 8, 256, 0, st>>>(a->alphas, bv.alphas, BT, d.R, Rp);
     LO_LAUNCH_OK();
-    cast_tb_to_bt_kernel<<<148 * 8, 256, 0, st>>>(a->dctx, bv.dctx, d.T, d.B, d.C);
+    cast_tb_to_bt_kernel<<<LO_NUM_SMS * 8, 256, 0, st>>>(a->dctx, bv.dctx, d.T, d.B, d.C);
     LO_LAUNCH_OK();
     LO_TRY(tc_gemm_tn_batched(bv.alphas, Rp, (int64_t)d.T * Rp, bv.dctx, d.C, (int64_t)d.T * d.C, a->denc, d.C, (int64_t)d.R * d.C, d.R,
                               d.C, d.T, d.B, st));
@@ -1678,7 +1724,7 @@ int lo_decoder_backward(const lo_decoder_args* a, void* stream) {
   LO_TRY(gemm_nn(a->dinit, LO_F32, 2 * d.D, a->w_init, dt, d.C, a->dmean, LO_F32, d.C, d.B, d.C, 2 * d.D, 0, LO_IMPL_SIMT, st));
   {
     const int64_t total = (int64_t)d.B * d.R * d.C;
-    add_rowbcast_kernel<<<148 * 8, 256, 0, st>>>(a->denc, a->dmean, d.R, d.C, 1.0f / (float)d.R, total);
+    add_rowbcast_kernel<<<LO_NUM_SMS * 8, 256, 0, st>>>(a->denc, a->dmean, d.R, d.C, 1.0f / (float)d.R, total);
     LO_LAUNCH_OK();
   }
   if (a->has_dropout == 2) {

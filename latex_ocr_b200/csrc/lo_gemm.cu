@@ -1,7 +1,8 @@
 // CUDA-core (SIMT) strided batched GEMM with fp32 accumulation — the tight-parity path and the
-// fallback for shapes the tcgen05 kernels (lo_tc.cu) do not take.  Replaces the torch.mm / nn.Linear
+// fallback for shapes the wgmma kernels (lo_tc.cu) do not take.  Replaces the torch.mm / nn.Linear
 // library calls behind seq2seq_torch.py:172-176, :223-227 (and their autograd twins).
 #include "lo_common.cuh"
+#include "lo_ptx.cuh"
 
 namespace lo {
 
@@ -112,30 +113,31 @@ int gemm(const void* A, int dtA, const void* B, int dtB, void* C, int dtC, const
   if (impl == LO_IMPL_TC && dtA == LO_BF16 && dtB == LO_BF16 && d.sak == 1 && d.sbk == 1 && d.batch == 1 && d.sam % 8 == 0 &&
       d.sbn % 8 == 0 && tc_available()) {
     // few rows, fp32 result: the latency-optimised mma.sync kernel (lo_skinny.cu) — same path as the decoder's per-step GEMMs;
-    // up to 512 rows (row blocks of 64) when the shape does not qualify for tcgen05 (e.g. beam-search logits with V % 8 != 0)
+    // up to 512 rows (row blocks of 64) when the shape does not qualify for wgmma (e.g. beam-search logits with V % 8 != 0)
     const bool tc_ok = d.K % 64 == 0 && d.N % 8 == 0 && d.ldc % 8 == 0;
     if (g_opt_skinny_mma && (d.M <= 64 || (!tc_ok && d.M <= 512)) && dtC == LO_F32 && !d.relu && d.K % 16 == 0 && d.N % 2 == 0 &&
         d.ldc % 2 == 0)
       return skinny_gemm_nt((const bf16*)A, d.sam, (const bf16*)B, d.sbn, (float*)C, d.ldc, d.M, d.N, d.K, d.bias, 1, d.accumulate, st);
-    // otherwise tcgen05; few rows -> 64-wide N tiles (twice the CTAs)
+    // otherwise wgmma; few rows -> 64-wide N tiles (twice the CTAs)
     if (tc_ok)
       return tc_gemm_nt_ex((const bf16*)A, d.sam, (const bf16*)B, d.sbn, C, dtC, d.ldc, d.M, d.N, d.K, d.bias, d.accumulate, d.relu, 1, 0,
                            d.M <= 64 ? 1 : 0, st);
   }
-  // C = A^T B with both operands stored [K][.] (weight gradients): tcgen05 MN-major kernel, split-K atomics onto a cleared C
+  // C = A^T B with both operands stored [K][.] (weight gradients): wgmma MN-major kernel, split-K atomics onto a cleared C
   if (impl == LO_IMPL_TC && dtA == LO_BF16 && dtB == LO_BF16 && dtC == LO_F32 && d.sam == 1 && d.sbn == 1 && d.batch == 1 && !d.bias &&
       !d.relu && !d.accumulate && d.sak % 8 == 0 && d.sbk % 8 == 0 && d.M >= 64 && d.N >= 64 && ((uintptr_t)A & 15) == 0 &&
       ((uintptr_t)B & 15) == 0 && tc_available()) {
     LO_CUDA(cudaMemset2DAsync(C, (size_t)d.ldc * 4, 0, (size_t)d.N * 4, (size_t)d.M, st));
     return tc_gemm_tn((const bf16*)A, d.sak, (const bf16*)B, d.sbk, (float*)C, d.ldc, d.M, d.N, d.K, st);
   }
-  // split-K only for fp32 outputs without ReLU when the tile grid would leave most SMs idle and K is long
+  // split-K only for fp32 outputs without ReLU when the tile grid would leave most SMs idle and K is long.  Option
+  // "deterministic": at most two splits, onto a zeroed C only — two addends onto 0 sum the same in either order
   int splitk = 1;
-  if (dtC == LO_F32 && !d.relu && d.K >= 2048) {
+  if (dtC == LO_F32 && !d.relu && d.K >= 2048 && !(g_opt_det && d.accumulate)) {
     const long tiles = (long)cdiv(d.M, 64) * cdiv(d.N, 64) * d.batch;
-    if (tiles < 296) {
-      splitk = (int)((296 + tiles - 1) / tiles);
-      const int maxs = d.K / 256;
+    if (tiles < 2 * LO_NUM_SMS) {
+      splitk = (int)((2 * LO_NUM_SMS + tiles - 1) / tiles);
+      const int maxs = g_opt_det ? 2 : d.K / 256;
       if (splitk > maxs) splitk = maxs;
       if (splitk < 1) splitk = 1;
     }
@@ -176,37 +178,39 @@ int gemm_nn(const void* A, int dtA, int64_t lda, const void* B, int dtB, int64_t
   return gemm(A, dtA, B, dtB, C, dtC, d, impl, st);
 }
 
-// out[n] (+)= sum_m X[m][n].  grid (N/32, row splits): each block reduces a row range for 32 columns (8 row lanes,
-// fixed tree) and adds its partial with one fp32 atomic per column; `out` is zeroed first unless accumulating.
-template <typename T>
-__global__ void colsum_kernel(const T* __restrict__ X, float* __restrict__ out, int M, int N, int64_t ld, int rows_per_block) {
-  __shared__ float red[8][33];
-  const int n = blockIdx.x * 32 + threadIdx.x;
-  const int m0 = blockIdx.y * rows_per_block, m1 = min(M, m0 + rows_per_block);
-  float s = 0.f;
-  if (n < N)
-    for (int m = m0 + threadIdx.y; m < m1; m += 8) s += ldf(X + (int64_t)m * ld + n);
-  red[threadIdx.y][threadIdx.x] = s;
-  __syncthreads();
-  if (threadIdx.y == 0 && n < N) {
-    float t = 0.f;
-#pragma unroll
-    for (int i = 0; i < 8; i++) t += red[i][threadIdx.x];
-    atomicAdd(out + n, t);
-  }
-}
+// out[n] (+)= sum_m X[m][n]: every row split of a column block adds its partial sums with one fp32 atomic per column.  Option
+// "deterministic": the row splits of a column block form one thread-block cluster whose rank 0 adds their partial sums in rank
+// order (lo_ptx.cuh:cl_sum); without `accumulate` up to two clusters cover a column block and add onto the zeroed `out` with one
+// fp32 atomic each — two addends onto 0 give the same sum in either order.  Without a cluster launch the kernels' cluster is
+// the block itself.
+int g_opt_det = 0;
 
-// vectorised variant: a warp reads 256 consecutive columns of one row (8 per lane, 16 B for bf16), 8 warps stride the rows
+constexpr int CS_MAXCL = 16;          // non-portable cluster size (H100)
+constexpr int CS_THREADS = 1024;
+
+// a warp reads 256 consecutive columns of one row (8 per lane, 16 B for bf16), the block's 32 warps stride the rows, 4 rows in flight
 template <typename T>
-__global__ void __launch_bounds__(256) colsum_vec_kernel(const T* __restrict__ X, float* __restrict__ out, int M, int N, int64_t ld,
-                                                          int rows_per_block) {
-  __shared__ float red[8][256 + 8];
+__global__ void __launch_bounds__(CS_THREADS) colsum_vec_kernel(const T* __restrict__ X, float* __restrict__ out, int M, int N, int64_t ld,
+                                                                 int rows_per_block, int atomic) {
+  constexpr int NW = CS_THREADS / 32;
+  __shared__ float red[NW][256 + 8];
+  __shared__ float part[256];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int n = blockIdx.x * 256 + lane * 8;
   const int m0 = blockIdx.y * rows_per_block, m1 = min(M, m0 + rows_per_block);
   float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
   if (n < N) {
-    for (int m = m0 + warp; m < m1; m += 8) {
+    int m = m0 + warp;
+    for (; m + 3 * NW < m1; m += 4 * NW) {
+      float v[4][8];
+#pragma unroll
+      for (int u = 0; u < 4; u++) ld8(X + (int64_t)(m + u * NW) * ld + n, v[u]);
+#pragma unroll
+      for (int u = 0; u < 4; u++)
+#pragma unroll
+        for (int k = 0; k < 8; k++) acc[k] += v[u][k];
+    }
+    for (; m < m1; m += NW) {
       float v[8];
       ld8(X + (int64_t)m * ld + n, v);
 #pragma unroll
@@ -217,36 +221,89 @@ __global__ void __launch_bounds__(256) colsum_vec_kernel(const T* __restrict__ X
   for (int k = 0; k < 8; k++) red[warp][lane * 8 + k] = acc[k];
   __syncthreads();
   const int c = threadIdx.x;
-  if (blockIdx.x * 256 + c < N) {
+  if (c < 256) {
     float t = 0.f;
 #pragma unroll
-    for (int w = 0; w < 8; w++) t += red[w][c];
-    atomicAdd(out + blockIdx.x * 256 + c, t);
+    for (int w = 0; w < NW; w++) t += red[w][c];
+    part[c] = t;
   }
+  cl_sync();
+  if (cl_rank() == 0 && c < 256 && blockIdx.x * 256 + c < N) {
+    const float t = cl_sum(&part[c]);
+    if (atomic) atomicAdd(out + blockIdx.x * 256 + c, t);
+    else out[blockIdx.x * 256 + c] += t;
+  }
+  cl_sync();
+}
+
+// any N / ld / alignment: 32 columns per block, 32 row lanes
+template <typename T>
+__global__ void __launch_bounds__(CS_THREADS) colsum_kernel(const T* __restrict__ X, float* __restrict__ out, int M, int N, int64_t ld,
+                                                             int rows_per_block, int atomic) {
+  __shared__ float red[32][33];
+  const int n = blockIdx.x * 32 + threadIdx.x;
+  const int m0 = blockIdx.y * rows_per_block, m1 = min(M, m0 + rows_per_block);
+  float s = 0.f;
+  if (n < N)
+    for (int m = m0 + threadIdx.y; m < m1; m += 32) s += ldf(X + (int64_t)m * ld + n);
+  red[threadIdx.y][threadIdx.x] = s;
+  __syncthreads();
+  if (threadIdx.y == 0) {
+    float t = 0.f;
+#pragma unroll
+    for (int i = 0; i < 32; i++) t += red[i][threadIdx.x];
+    red[0][threadIdx.x] = t;
+  }
+  cl_sync();
+  if (cl_rank() == 0 && threadIdx.y == 0 && n < N) {
+    const float t = cl_sum(&red[0][threadIdx.x]);
+    if (atomic) atomicAdd(out + n, t);
+    else out[n] += t;
+  }
+  cl_sync();
 }
 
 int colsum(const void* X, int dt, float* out, int M, int N, int64_t ld, int accumulate, cudaStream_t st) {
   LO_CHECK_ARG(M > 0 && N > 0, "empty colsum");
+  static bool attr = false;
+  if (!attr) {
+    LO_CUDA(cudaFuncSetAttribute(colsum_vec_kernel<float>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+    LO_CUDA(cudaFuncSetAttribute(colsum_vec_kernel<bf16>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+    LO_CUDA(cudaFuncSetAttribute(colsum_kernel<float>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+    LO_CUDA(cudaFuncSetAttribute(colsum_kernel<bf16>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+    attr = true;
+  }
   if (!accumulate) LO_CUDA(cudaMemsetAsync(out, 0, (size_t)N * sizeof(float), st));
   const size_t es = dt == LO_F32 ? 4 : 2;
-  if (N % 8 == 0 && ld % 8 == 0 && ((uintptr_t)X % (8 * es)) == 0 && M >= 256) {
-    const int cb = cdiv(N, 256);
-    int splits = cdiv(148 * 4, cb);
-    if (splits > cdiv(M, 64)) splits = cdiv(M, 64);
+  const bool vec = N % 8 == 0 && ld % 8 == 0 && ((uintptr_t)X % (8 * es)) == 0;
+  const int cb = vec ? cdiv(N, 256) : cdiv(N, 32);
+  if (!g_opt_det) {
+    int splits = cdiv(LO_NUM_SMS * 2, cb);
+    if (splits > cdiv(M, 128)) splits = cdiv(M, 128);
     if (splits < 1) splits = 1;
     const int rpb = cdiv(M, splits);
-    dim3 grid(cb, cdiv(M, rpb));
-    LO_DISPATCH_DT(dt, T, (colsum_vec_kernel<T><<<grid, 256, 0, st>>>((const T*)X, out, M, N, ld, rpb)));
+    const dim3 grid(cb, cdiv(M, rpb));
+    if (vec) {
+      LO_DISPATCH_DT(dt, T, (colsum_vec_kernel<T><<<grid, CS_THREADS, 0, st>>>((const T*)X, out, M, N, ld, rpb, 1)));
+    } else {
+      LO_DISPATCH_DT(dt, T, (colsum_kernel<T><<<grid, dim3(32, 32), 0, st>>>((const T*)X, out, M, N, ld, rpb, 1)));
+    }
     LO_LAUNCH_OK();
     return LO_OK;
   }
-  const int cb = cdiv(N, 32);
-  int splits = cdiv(148 * 8, cb);
-  if (splits > cdiv(M, 64)) splits = cdiv(M, 64);
-  if (splits < 1) splits = 1;
-  const int rpb = cdiv(M, splits);
-  dim3 grid(cb, cdiv(M, rpb));
-  LO_DISPATCH_DT(dt, T, (colsum_kernel<T><<<grid, dim3(32, 8), 0, st>>>((const T*)X, out, M, N, ld, rpb)));
+  // ordered: one cluster of up to 16 row splits (>= 256 rows each), a second one only onto the zeroed output
+  int cs = cdiv(M, 256);
+  if (cs > CS_MAXCL) cs = CS_MAXCL;
+  const int groups = (!accumulate && cs == CS_MAXCL && M >= 2 * CS_MAXCL * 256) ? 2 : 1;
+  const int rpb = cdiv(M, cs * groups);
+  const dim3 grid(cb, cs * groups), cl(1, cs, 1);
+  if (vec) {
+    LO_DISPATCH_DT(dt, T, LO_CUDA(launch_cluster(colsum_vec_kernel<T>, grid, dim3(CS_THREADS), 0, st, cl, false, (const T*)X, out, M, N, ld,
+                                                  rpb, groups > 1 ? 1 : 0)));
+  } else {
+    LO_DISPATCH_DT(dt, T, LO_CUDA(launch_cluster(colsum_kernel<T>, grid, dim3(32, 32), 0, st, cl, false, (const T*)X, out, M, N, ld, rpb,
+                                                  groups > 1 ? 1 : 0)));
+  }
   LO_LAUNCH_OK();
   return LO_OK;
 }

@@ -2,7 +2,7 @@
 // independent sequences and the hand-derived backward.  EXTENSION beyond the reference (BASELINE.json configs[3]: row-encoder
 // biLSTM over the CNN feature rows + a second decoder layer; the reference only links the paper, model/decoder.py:16): there is no
 // reference code to restate — the oracle is torch.nn.LSTM itself (oracle/ref_ext.py).  Part of the lo_decoder.cu translation unit
-// (reuses its transpose / cast kernels and the GEMM dispatcher: tcgen05 for the hoisted products and the M > 64 per-step
+// (reuses its transpose / cast kernels and the GEMM dispatcher: wgmma for the hoisted products and the M > 64 per-step
 // projections, the mma.sync kernel for M <= 64, CUDA cores in fp32 mode).
 //
 // Schedule (same ideas as the decoder, DESIGN.md §4): the input projection x W_ih^T + b of ALL steps is one hoisted GEMM; the time
@@ -185,7 +185,7 @@ int lo_lstm_seq_forward(const lo_lstm_seq_args* a, void* stream) {
   const SeqWs w = seq_carve(a);
   const bool bf = dt == LO_BF16;
   const int impl = (a->impl == LO_IMPL_TC && bf) ? LO_IMPL_TC : LO_IMPL_SIMT;
-  LO_DISPATCH_DT(dt, T, (seq_gather_kernel<T><<<148 * 8, 256, 0, st>>>((const T*)a->x, a->x_row, a->x_step, (T*)w.xt, S, M, I, a->reverse)));
+  LO_DISPATCH_DT(dt, T, (seq_gather_kernel<T><<<LO_NUM_SMS * 8, 256, 0, st>>>((const T*)a->x, a->x_row, a->x_step, (T*)w.xt, S, M, I, a->reverse)));
   LO_LAUNCH_OK();
   seq_bias_sum_kernel<<<cdiv(G, 256), 256, 0, st>>>(a->b_ih, a->b_hh, w.bsum, G);
   LO_LAUNCH_OK();
@@ -250,7 +250,7 @@ int lo_lstm_seq_backward(const lo_lstm_seq_args* a, void* stream) {
   LO_CUDA(cudaMemcpyAsync(a->g_b_hh, a->g_b_ih, (size_t)G * 4, cudaMemcpyDeviceToDevice, st));
   if (a->dx) {
     LO_TRY(gemm_nt(dGs, dt, G, w.wihT, dt, G, w.dxt, LO_F32, I, S * M, I, G, nullptr, 0, 0, impl, st));
-    seq_scatter_kernel<<<148 * 8, 256, 0, st>>>(w.dxt, a->dx, a->dx_row, a->dx_step, S, M, I, a->reverse, a->dx_accumulate);
+    seq_scatter_kernel<<<LO_NUM_SMS * 8, 256, 0, st>>>(w.dxt, a->dx, a->dx_row, a->dx_step, S, M, I, a->reverse, a->dx_accumulate);
     LO_LAUNCH_OK();
   }
   return LO_OK;

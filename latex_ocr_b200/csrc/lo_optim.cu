@@ -81,7 +81,7 @@ int lo_adam_step(float* p, const float* g, float* m, float* v, void* shadow_bf16
   LO_CHECK_ARG(p && g && m && v && state_dev && n > 0, "null pointer / n");
   cudaStream_t st = (cudaStream_t)stream;
   int grid = (int)((n + 1023) / 1024);
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > LO_NUM_SMS * 8) grid = LO_NUM_SMS * 8;
   adam_kernel<<<grid, 256, 0, st>>>(p, g, m, v, (bf16*)shadow_bf16, n, state_dev, beta1, beta2, eps, grad_scale);
   LO_LAUNCH_OK();
   adam_bump_kernel<<<1, 1, 0, st>>>(state_dev);
@@ -97,7 +97,7 @@ int lo_adam_step_ranges(float* p, const float* g, float* m, float* v, void* shad
     const int64_t off = ranges[2 * r], n = ranges[2 * r + 1];
     LO_CHECK_ARG(off >= 0 && n > 0, "range");
     int grid = (int)((n + 1023) / 1024);
-    if (grid > 148 * 8) grid = 148 * 8;
+    if (grid > LO_NUM_SMS * 8) grid = LO_NUM_SMS * 8;
     adam_kernel<<<grid, 256, 0, st>>>(p + off, g + off, m + off, v + off, shadow_bf16 ? (bf16*)shadow_bf16 + off : nullptr, n, state_dev, beta1,
                                       beta2, eps, grad_scale);
     LO_LAUNCH_OK();
@@ -114,7 +114,7 @@ int lo_tf_optim_step(int kind, float* p, const float* g, float* s1, float* s2, v
   LO_CHECK_ARG((kind != 1 || (s1 && s2)) && (kind < 3 || s1), "slot buffers");
   cudaStream_t st = (cudaStream_t)stream;
   int grid = (int)((n + 1023) / 1024);
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > LO_NUM_SMS * 8) grid = LO_NUM_SMS * 8;
   tf_optim_kernel<<<grid, 256, 0, st>>>(kind, p, g, s1, s2, (bf16*)shadow_bf16, n, state_dev, beta1, beta2, eps, grad_scale);
   LO_LAUNCH_OK();
   adam_bump_kernel<<<1, 1, 0, st>>>(state_dev);
@@ -126,7 +126,7 @@ int lo_cast(const void* src, int dt_src, void* dst, int dt_dst, int64_t n, void*
   LO_CHECK_ARG(src && dst && n > 0, "null pointer / n");
   cudaStream_t st = (cudaStream_t)stream;
   int grid = (int)((n + 1023) / 1024);
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > LO_NUM_SMS * 8) grid = LO_NUM_SMS * 8;
   if (dt_src == LO_F32 && dt_dst == LO_BF16) cast_kernel<float, bf16><<<grid, 256, 0, st>>>((const float*)src, (bf16*)dst, n);
   else if (dt_src == LO_BF16 && dt_dst == LO_F32) cast_kernel<bf16, float><<<grid, 256, 0, st>>>((const bf16*)src, (float*)dst, n);
   else if (dt_src == LO_F32 && dt_dst == LO_F32) cast_kernel<float, float><<<grid, 256, 0, st>>>((const float*)src, (float*)dst, n);

@@ -75,4 +75,56 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
+// Deterministic cross-CTA sums: the CTAs that contribute to the same outputs form one thread-block cluster, each stages its
+// partial sums at the same shared-memory offset, and rank 0 adds them in rank order (distributed shared memory) before the
+// single write to global memory — no fp32 atomics whose order, and so whose rounding, changes from run to run.
+// Every thread of every CTA of the cluster must call cl_sync() (no early exit before the last one).
+__device__ __forceinline__ uint32_t cl_rank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+__device__ __forceinline__ uint32_t cl_size() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(r));
+  return r;
+}
+__device__ __forceinline__ void cl_sync() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+// the float at the same shared-memory offset as `p` in CTA `rank` of the cluster
+__device__ __forceinline__ float cl_ld(const float* p, uint32_t rank) {
+  uint32_t a;
+  float v;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(a) : "r"(smem_u32(p)), "r"(rank));
+  asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(v) : "r"(a) : "memory");
+  return v;
+}
+// sum over the cluster's CTAs (<= 16), in rank order, of the float at `p`; all loads are issued before the first add
+__device__ __forceinline__ float cl_sum(const float* p) {
+  const uint32_t n = cl_size();
+  float v[16];
+#pragma unroll
+  for (uint32_t r = 0; r < 16; r++) v[r] = r < n ? cl_ld(p, r) : 0.f;
+  float s = v[0];
+#pragma unroll
+  for (uint32_t r = 1; r < 16; r++)
+    if (r < n) s += v[r];
+  return s;
+}
+// out[i] = the same sum for the K floats at p + i * stride; the K loads of one rank are in flight together
+template <int K>
+__device__ __forceinline__ void cl_sum_n(const float* p, int stride, float* out) {
+  const uint32_t n = cl_size();
+#pragma unroll
+  for (int i = 0; i < K; i++) out[i] = cl_ld(p + i * stride, 0);
+  for (uint32_t r = 1; r < n; r++) {
+    float v[K];
+#pragma unroll
+    for (int i = 0; i < K; i++) v[i] = cl_ld(p + i * stride, r);
+#pragma unroll
+    for (int i = 0; i < K; i++) out[i] += v[i];
+  }
+}
+
 }  // namespace lo

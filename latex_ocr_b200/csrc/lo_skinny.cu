@@ -1,11 +1,11 @@
 // Latency-optimised GEMM for the decoder's per-step projections: C[M <= 64][N] (+)= A[M][K] * W[N][K]^T + bias.
 //
-// These GEMMs are 33-134 MFLOP with M = batch = 64 rows: nothing about them is throughput bound.  The tcgen05 path
-// (lo_tc.cu, kept and selectable with lo_set_option("skinny_mma", 0)) pays ~5.6 us per launch in fixed pipeline latency
-// (TMEM allocation, single-thread TMA issue at ~430 cycles per K block, accumulator drain through 128 threads).  Here
+// These GEMMs are 33-134 MFLOP with M = batch = 64 rows: nothing about them is throughput bound.  The wgmma path
+// (lo_tc.cu, kept and selectable with lo_set_option("skinny_mma", 0)) pays a fixed pipeline latency per launch
+// (barrier setup, a TMA round trip per K block, the accumulator epilogue).  Here
 // every CTA (16 output columns x all 64 rows x one K slice) issues ALL of its loads at once with cp.async (one L2
 // round trip), then runs warp-level mma.sync from shared memory and stores straight from the accumulator registers.
-// The FLOP-heavy work (convolutions, att1, weight gradients, logits) stays on tcgen05.
+// The FLOP-heavy work (convolutions, att1, weight gradients, logits) stays on wgmma.
 #include "lo_common.cuh"
 #include "lo_ptx.cuh"
 
@@ -36,12 +36,11 @@ __device__ __forceinline__ void mma_bf16_16816(float* c, uint32_t a0, uint32_t a
 
 // grid (N/16, ksplit, row blocks of 64), 128 threads (warp w owns rows 16w..16w+15 of its row block)
 // TMA = true: both operands arrive as 1-D bulk copies (cp.async.bulk, one per row, issued by warp 0, completion on two mbarriers)
-// instead of 16-byte cp.async: the fused-step timeline (run 70) showed the post-wait 64 KB activation load taking ~3 us per CTA at
-// the ~30 GB/s an SM sustains with LDGSTS.
+// instead of 16-byte cp.async, which moves the post-wait 64 KB activation load through one SM's LDGSTS path far more slowly.
 template <bool TMA>
 __global__ void __launch_bounds__(128) skinny_mma_kernel(const bf16* __restrict__ A, int64_t lda, const bf16* __restrict__ W, int64_t ldw,
                                                           float* __restrict__ C, int64_t ldc, int M, int N, int K, int kc,
-                                                          const float* __restrict__ bias, int atomic) {
+                                                          const float* __restrict__ bias, int mode) {
   A += (int64_t)blockIdx.z * 64 * lda;
   C += (int64_t)blockIdx.z * 64 * ldc;
   M = min(64, M - (int)blockIdx.z * 64);
@@ -139,21 +138,41 @@ __global__ void __launch_bounds__(128) skinny_mma_kernel(const bf16* __restrict_
 #pragma unroll
   for (int j = 0; j < 2; j++)
 #pragma unroll
-    for (int q = 0; q < 4; q++) acc[j][q] += acd[j][q];
+    for (int q = 0; q < 4; q++) acc[j][q] += acd[j][q] + bpre[j][q & 1];
+  if (gridDim.y > 1 && mode != 1) {
+    // ordered split K: the K slices of this tile are one cluster; rank 0 (slice 0) adds the partials in slice order, alone writes C
+    __syncthreads();                                         // every ldmatrix read of sA is done: it stages the partials
+    float* part = reinterpret_cast<float*>(sk_smem);
+#pragma unroll
+    for (int i = 0; i < 8; i++) part[i * 128 + tid] = acc[i >> 2][i & 3];
+    cl_sync();
+    if (cl_rank() == 0) {
+      float s[8];
+      cl_sum_n<8>(part + tid, 128, s);
+#pragma unroll
+      for (int i = 0; i < 8; i++) acc[i >> 2][i & 3] = s[i];
+    }
+    cl_sync();
+    if (cl_rank() != 0) return;
+  }
   const int g = lane >> 2, t = lane & 3;
 #pragma unroll
   for (int j = 0; j < 2; j++) {
     const int n = n0 + j * 8 + 2 * t;
     if (n >= N) continue;
-    const float bx = bpre[j][0], by = bpre[j][1];
 #pragma unroll
     for (int h = 0; h < 2; h++) {
       const int r = warp * 16 + g + h * 8;
       if (r >= M) continue;
       float* o = C + (int64_t)r * ldc + n;
-      const float x = acc[j][2 * h] + bx, y = acc[j][2 * h + 1] + by;
-      if (atomic) { atomicAdd(o, x); atomicAdd(o + 1, y); }
-      else *reinterpret_cast<float2*>(o) = make_float2(x, y);
+      float x = acc[j][2 * h], y = acc[j][2 * h + 1];
+      if (mode == 1) {
+        atomicAdd(o, x);
+        atomicAdd(o + 1, y);
+        continue;
+      }
+      if (mode == 2) { const float2 old = *reinterpret_cast<float2*>(o); x += old.x; y += old.y; }
+      *reinterpret_cast<float2*>(o) = make_float2(x, y);
     }
   }
 }
@@ -162,7 +181,7 @@ __global__ void __launch_bounds__(128) skinny_mma_kernel(const bf16* __restrict_
 // LSTM cell (nn.LSTMCell, gates i,f,g,o: seq2seq_torch.py:313) in the epilogue: a CTA's 16 columns are 4 whole hidden units, lane
 // pairs (t, t^1) hold (i,f) and (g,o) of one unit for rows g and g+8 and swap halves with one shuffle, so every thread finalises
 // one (row, unit).  The table row, the recurrent projection and c_{t-1} are fetched BEFORE the MMA loop (they do not depend on
-// it), which is what the 128-thread tcgen05 epilogue could not hide.  K <= 512 (one slice).  Replaces gemm + lstm_pw_fwd_kernel.
+// it), which a separate GEMM epilogue could not hide.  K <= 512 (one slice).  Replaces gemm + lstm_pw_fwd_kernel.
 __global__ void __launch_bounds__(128) skinny_lstm_kernel(const bf16* __restrict__ A, int64_t lda, const bf16* __restrict__ Wil, int64_t ldw,
                                                            int M, int K, TcLstmEpi e) {
   extern __shared__ __align__(16) uint8_t sk_smem[];
@@ -269,10 +288,10 @@ __global__ void __launch_bounds__(128) skinny_lstm_kernel(const bf16* __restrict
 // ------------------------------------------------------------------------------------------------------------------------------
 // Fused decoder forward step: one launch per time step instead of three.
 //   phase 1 (CTAs 0 .. 4D/16-1): gates = (gate*ctx)_t W_ih[:, E:]^T with the LSTM cell in the epilogue -> h_{t+1}, c_{t+1}
-//   grid barrier (all CTAs are co-resident: <= 2 per SM by shared memory, grid <= 296)
+//   grid barrier (all CTAs are co-resident: <= 2 per SM by shared memory, grid <= 2 x LO_NUM_SMS)
 //   phase 2 (CTAs 0 .. N2/16-1): [att2 | gate_pre | hh_pre]_{t+1} = h_{t+1} [W_d; W_beta; W_hh]^T + b
-// The time loop is a chain of dependent 64-row GEMMs: each separate launch costs ~6-7 us of pure latency (launch, cold loads,
-// drain) for ~1 us of math.  Here both weight slices are fetched before griddepcontrol.wait, the barrier costs one L2 atomic
+// The time loop is a chain of dependent 64-row GEMMs: each separate launch costs several times its math in pure
+// latency (launch, cold loads, drain).  Here both weight slices are fetched before griddepcontrol.wait, the barrier costs one L2 atomic
 // round trip, and h_{t+1} is re-read from L2 where the other CTAs just put it.  griddepcontrol.launch_dependents is issued only
 // AFTER the barrier: by then every CTA of this grid is resident, so the early-starting attention kernel of the next step
 // cannot take a slot a not-yet-resident CTA of this grid needs (no deadlock).
@@ -283,9 +302,9 @@ __device__ __forceinline__ unsigned int ld_acquire_u32(const unsigned int* p) {
   return v;
 }
 // Arrival counters are spread over GB_NC cache lines (one L2 atomic unit each): a CTA adds 1 to counter (blockIdx.x % GB_NC) with a
-// fire-and-forget red.release, warp 0 polls all GB_NC counters with ONE acquire load per lane and sums them with a warp reduce.  192
-// arrivals on a single counter serialise in the L2 atomic unit (~27 cycles each: 2.7 us, as much as a kernel boundary, which is why
-// the fused step kernels first measured no faster, run 42); 12 arrivals per counter cost ~0.2 us.  Counters are monotonic: `target` is the
+// fire-and-forget red.release, warp 0 polls all GB_NC counters with ONE acquire load per lane and sums them with a warp reduce.  Arrivals
+// on a single counter serialise in the L2 atomic unit (as much as a kernel boundary for a full grid); spread over GB_NC counters
+// they cost a small fraction of that.  Counters are monotonic: `target` is the
 // total number of arrivals after this barrier.
 constexpr int GB_NC = 16;
 __device__ __forceinline__ void grid_barrier(unsigned int* ctr, unsigned int target) {
@@ -471,7 +490,7 @@ __global__ void __launch_bounds__(128) dec_step_fwd_kernel(DecStepFwd p) {
   SK_TS(7);
 }
 
-int g_opt_dec_fuse = 0;       // run 42 (single-counter barrier): 13.46 vs 13.35 ms decoder fwd+bwd; see grid_barrier for the spread counters
+int g_opt_dec_fuse = 0;       // fused forward step: off, it measured no faster than the separate launches; see grid_barrier
 
 int dec_step_fwd(const DecStepFwd& p, cudaStream_t st) {
   LO_CHECK_ARG(p.M >= 1 && p.M <= 64 && p.K % 16 == 0 && p.K <= SK_KC && p.e.D == p.K && p.e.D % 4 == 0 && p.N2 % 2 == 0, "M<=64, K=D<=512");
@@ -614,7 +633,7 @@ __global__ void __launch_bounds__(128) dec_step_bwd_kernel(DecStepBwd p) {
   skinny_tile_atomic(sA, sWc, SK_KC, p.dxh, CD, c_n0, CD, p.Mb);
 }
 
-int g_opt_dec_fuse_bwd = 0;   // measured: 13.78 vs 13.46 ms (run 42): two grid barriers cost more than two PDL boundaries
+int g_opt_dec_fuse_bwd = 0;   // off: two grid barriers cost more than two PDL boundaries
 
 int dec_step_bwd(const DecStepBwd& p, cudaStream_t st) {
   LO_CHECK_ARG(p.K2 % SK_KC == 0 && p.K1 % SK_KC == 0 && p.D % SK_NT == 0 && (p.C + p.D) % SK_NT == 0 && p.C == p.D, "K1, K2 multiples of 512, C == D");
@@ -644,7 +663,9 @@ int skinny_gemm_nt_lstm(const bf16* A, int64_t lda, const bf16* Wil, int64_t ldw
   return LO_OK;
 }
 
-// splits > 1 or atomic_acc: partial sums are added onto C with fp32 atomics (C holds the base values)
+// atomic_acc: the product is added onto C (C holds the base values).  splits > 1: the K slices add their partial sums onto C with
+// fp32 atomics, or — option "deterministic" — groups of up to 8 slices run as one thread-block cluster each, summed in slice order
+// and added onto C group after group in stream order (run-to-run identical results)
 int skinny_gemm_nt(const bf16* A, int64_t lda, const bf16* W, int64_t ldw, float* C, int64_t ldc, int M, int N, int K, const float* bias,
                    int splits, int atomic_acc, cudaStream_t st) {
   LO_CHECK_ARG(M >= 1 && M <= 64 * 1024 && K % 16 == 0 && N % 2 == 0 && lda % 8 == 0 && ldw % 8 == 0 && ldc % 2 == 0, "K%16, ld%8");
@@ -659,16 +680,32 @@ int skinny_gemm_nt(const bf16* A, int64_t lda, const bf16* W, int64_t ldw, float
   int kc = cdiv(cdiv(K, ks), 16) * 16;
   if (kc > SK_KC) kc = SK_KC;
   ks = cdiv(K, kc);
-  const int atomic = (ks > 1 || atomic_acc) ? 1 : 0;
-  if (ks > 1 && !atomic_acc) LO_CUDA(cudaMemset2DAsync(C, (size_t)ldc * 4, 0, (size_t)N * 4, (size_t)M, st));
-  if (g_opt_skinny_tma) {
-    LO_CUDA(launch_pdl(skinny_mma_kernel<true>, dim3(cdiv(N, SK_NT), ks, cdiv(M, 64)), dim3(128), (size_t)SK_SMEM + 16, st, A, lda, W, ldw, C,
-                       ldc, M, N, K, kc, bias, atomic));
-  } else {
-    LO_CUDA(launch_pdl(skinny_mma_kernel<false>, dim3(cdiv(N, SK_NT), ks, cdiv(M, 64)), dim3(128), (size_t)SK_SMEM, st, A, lda, W, ldw, C, ldc,
-                       M, N, K, kc, bias, atomic));
+  if (!g_opt_det || ks == 1) {
+    const int mode = (ks > 1 || atomic_acc) ? 1 : 0;
+    if (ks > 1 && !atomic_acc) LO_CUDA(cudaMemset2DAsync(C, (size_t)ldc * 4, 0, (size_t)N * 4, (size_t)M, st));
+    const dim3 grid(cdiv(N, SK_NT), ks, cdiv(M, 64));
+    if (g_opt_skinny_tma) {
+      LO_CUDA(launch_pdl(skinny_mma_kernel<true>, grid, dim3(128), (size_t)SK_SMEM + 16, st, A, lda, W, ldw, C, ldc, M, N, K, kc, bias, mode));
+    } else {
+      LO_CUDA(launch_pdl(skinny_mma_kernel<false>, grid, dim3(128), (size_t)SK_SMEM, st, A, lda, W, ldw, C, ldc, M, N, K, kc, bias, mode));
+    }
+    LO_LAUNCH_OK();
+    return LO_OK;
   }
-  LO_LAUNCH_OK();
+  for (int k0 = 0; k0 < K; k0 += 8 * kc) {
+    const int kg = K - k0 < 8 * kc ? K - k0 : 8 * kc, ng = cdiv(kg, kc);
+    const int mode = (k0 > 0 || atomic_acc) ? 2 : 0;
+    const float* bg = k0 == 0 ? bias : nullptr;
+    const dim3 grid(cdiv(N, SK_NT), ng, cdiv(M, 64)), cl(1, ng, 1);
+    if (g_opt_skinny_tma) {
+      LO_CUDA(launch_cluster(skinny_mma_kernel<true>, grid, dim3(128), (size_t)SK_SMEM + 16, st, cl, true, A + k0, lda, W + k0, ldw, C, ldc, M,
+                             N, kg, kc, bg, mode));
+    } else {
+      LO_CUDA(launch_cluster(skinny_mma_kernel<false>, grid, dim3(128), (size_t)SK_SMEM, st, cl, true, A + k0, lda, W + k0, ldw, C, ldc, M, N,
+                             kg, kc, bg, mode));
+    }
+    LO_LAUNCH_OK();
+  }
   return LO_OK;
 }
 

@@ -1,13 +1,13 @@
-// tcgen05 + TMA kernels (sm_100a): NHWC 3x3 implicit-GEMM convolution and the K-major "NT" GEMM.
+// wgmma + TMA kernels (sm_90a): NHWC 3x3 implicit-GEMM convolution and the K-major "NT" GEMM.
 //
-//   D[128 x NT] (TMEM, fp32) += A[128 x 64] (smem, bf16, K-major, SWIZZLE_128B) * B[NT x 64]^T (smem, bf16, K-major)
+//   D[128 x NT] (registers, fp32) += A[128 x 64] (smem, bf16, K-major, SWIZZLE_128B) * B[NT x 64]^T (smem, bf16, K-major)
 //
 // A tiles come from TMA: for the convolution a 4-D tiled map over the NHWC feature map {C, W, H, N} with box
 // {64, BW, BH, 1} (BW*BH = 128 output positions); tap (r,s) is just a coordinate shift and the halo / zero padding
 // falls out of TMA's out-of-bounds zero fill — no im2col buffer, no predicates.  B tiles are rows of the
-// [Cout][9*Cin] weight matrix.  Warp roles: warp 0 = TMA producer, warp 1 = TMEM allocator + single-thread MMA
-// issuer, warps 2..5 = epilogue (tcgen05.ld -> bias/ReLU/mask -> global).  3-4 stage mbarrier ring, one output
-// tile per CTA, 2 CTAs per SM so one CTA's epilogue overlaps the other's main loop.
+// [Cout][9*Cin] weight matrix.  Warp roles: warps 0..7 = two consumer warpgroups (warpgroup g owns rows [64g, 64g+64)
+// of the tile: wgmma into registers, then the epilogue straight from the accumulators), warp 8 = A-tile TMA producer,
+// warp 9 = B-tile TMA producer.  3-8 stage mbarrier ring.
 #include <cuda.h>
 
 #include <mutex>
@@ -15,15 +15,13 @@
 
 #include "lo_common.cuh"
 #include "lo_ptx.cuh"
+#include "lo_wgmma.cuh"
 
 namespace lo {
 
 // ------------------------------------------------------------------------------------------------
-// PTX wrappers (strings follow cute/arch/{copy_sm90_tma,mma_sm100_umma,tmem_allocator_sm100}.hpp)
+// PTX wrappers (strings follow cute/arch/copy_sm90_tma.hpp, cutlass/arch/barrier.h)
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
 __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1) {
   asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(
                    smem_u32(dst)),
@@ -67,10 +65,11 @@ __device__ __forceinline__ void tma_load_4d_mc(void* dst, const CUtensorMap* map
       "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "h"(mask), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
-__device__ __forceinline__ void umma_commit_mc(uint64_t* bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(smem_u32(bar)),
-               "h"(mask)
-               : "memory");
+// arrive on the mbarrier at the same shared-memory offset in CTA `cta` of the cluster (may be this CTA)
+__device__ __forceinline__ void mbar_arrive_cta(uint64_t* bar, uint32_t cta) {
+  uint32_t remote;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(cta));
+  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
 }
 __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
@@ -84,57 +83,15 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
 }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t* slot, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]^T, bf16 x bf16 -> fp32, issued by ONE thread
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on an mbarrier once every previously issued tcgen05.mma of this thread has completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// 32 lanes x 32 columns of fp32: thread i of the warp gets row (quadrant base + i), columns [col, col+32)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* v) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-        "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]),
-        "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-        "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): rows of 128 B, 8-row groups
-// 1024 B apart (SBO), LBO unused for swizzled K-major (=1), version 1 (Blackwell), layout type 2 (SWIZZLE_128B).
+// K-major, SWIZZLE_128B wgmma shared-memory descriptor (cute::GMMA::GmmaDescriptor): rows of 128 B, 8-row groups
+// 1024 B apart (SBO), LBO unused for swizzled K-major (=1), layout type 1 (SWIZZLE_128B).  Tiles start 1024-aligned.
 __device__ __forceinline__ uint64_t make_kmajor_sw128_desc(uint32_t saddr) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFF) >> 4);          // start address   bits [0,14)
   d |= (uint64_t)1 << 16;                           // leading byte offset (16 B units) bits [16,30)
   d |= (uint64_t)(1024 >> 4) << 32;                 // stride byte offset  bits [32,46)
-  d |= (uint64_t)1 << 46;                           // version = 1         bits [46,48)
-  d |= (uint64_t)2 << 61;                           // SWIZZLE_128B        bits [61,64)
+  d |= (uint64_t)1 << 62;                           // SWIZZLE_128B        bits [62,64)
   return d;
-}
-// kind::f16 instruction descriptor (cute::UMMA::InstrDescriptor): D=f32, A=B=bf16, both K-major, M x N
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
 }
 
 struct TcParams {
@@ -164,7 +121,8 @@ struct TcParams {
 };
 
 constexpr int TC_BM = 128, TC_BK = 64;
-constexpr int TC_THREADS = 224;   // warp 0: A-tile TMA producer, 1: TMEM + MMA issuer, 2..5: epilogue, 6: B-tile TMA producer
+constexpr int TC_CWARPS = 8;                          // two consumer warpgroups
+constexpr int TC_THREADS = (TC_CWARPS + 2) * 32;      // + warp 8: A-tile TMA producer, warp 9: B-tile TMA producer
 
 template <int NT, int STAGES>
 struct TcSmem {
@@ -174,19 +132,52 @@ struct TcSmem {
   static constexpr int TOTAL = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
 };
 
+// One K block (64 wide) of a consumer warpgroup: its 64 rows of the A stage (rows 64 * wg.., 8 KB apart) times the B stage.
+template <int NT>
+__device__ __forceinline__ void tc_mma_kblock(float* acc, uint32_t sa, uint32_t sb, bool first) {
+  const uint64_t da = make_kmajor_sw128_desc(sa), db = make_kmajor_sw128_desc(sb);
+#pragma unroll
+  for (int k = 0; k < TC_BK / 16; k++)
+    // advance 16 elements (32 B) along K inside the 128 B swizzle row: +2 in the 16 B-unit address field
+    Wgmma<NT, 0, 0>::mma(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (first && k == 0) ? 0u : 1u);
+}
+
+// bias (+ReLU) (+bf16 mask) epilogue of two adjacent accumulator columns of one output row, written to bf16 or fp32;
+// `atomic` adds onto fp32 (split-K partial sums)
+__device__ __forceinline__ void tc_store_pair(const TcParams& p, int64_t off, float f0, float f1, bool use_mask) {
+  if (p.atomic) {
+    float* o = reinterpret_cast<float*>(p.out) + off;
+    atomicAdd(o, f0);
+    atomicAdd(o + 1, f1);
+  } else if (p.out_f32) {
+    float2* o = reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + off);
+    if (p.accumulate) { const float2 old = *o; f0 += old.x; f1 += old.y; }
+    if (p.relu) { f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f); }
+    *o = make_float2(f0, f1);
+  } else {
+    uint32_t* o = reinterpret_cast<uint32_t*>(reinterpret_cast<bf16*>(p.out) + off);
+    if (p.accumulate) { const uint32_t old = *o; f0 += __uint_as_float(old << 16); f1 += __uint_as_float(old & 0xffff0000u); }
+    if (p.relu) { f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f); }
+    if (use_mask) {
+      const uint32_t w = *reinterpret_cast<const uint32_t*>(p.mask + off);
+      if (!(__uint_as_float(w << 16) > 0.f)) f0 = 0.f;
+      if (!(__uint_as_float(w & 0xffff0000u) > 0.f)) f1 = 0.f;
+    }
+    __nv_bfloat162 h = __floats2bfloat162_rn(f0, f1);
+    *o = *reinterpret_cast<uint32_t*>(&h);
+  }
+}
+
 // MC = 1: the two CTAs of a (2,1,1) cluster compute neighbouring N tiles of the SAME 128-row A tile; each loads one
-// 64-row half of A and multicasts it to both (halves the L2 -> SM traffic of A; the kernel is L2-bandwidth bound at
-// 128x128 tiles).  mapA then describes HALF boxes.
+// 64-row half of A and multicasts it to both (halves the L2 -> SM traffic of A).  mapA then describes HALF boxes.
 template <int NT, int STAGES, int MC>
-__global__ void __launch_bounds__(TC_THREADS) tc_gemm_conv_kernel(const __grid_constant__ CUtensorMap mapA,
-                                                                   const __grid_constant__ CUtensorMap mapB, TcParams p) {
+__global__ void __launch_bounds__(TC_THREADS, 1) tc_gemm_conv_kernel(const __grid_constant__ CUtensorMap mapA,
+                                                                      const __grid_constant__ CUtensorMap mapB, TcParams p) {
   using SM = TcSmem<NT, STAGES>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * SM::STAGE_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full_bar = empty_bar + STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
   __shared__ __align__(16) float s_bias[NT];
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -208,28 +199,22 @@ __global__ void __launch_bounds__(TC_THREADS) tc_gemm_conv_kernel(const __grid_c
 
   const bool dbg = p.dbg && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0;
   if (dbg && threadIdx.x == 0) p.dbg[0] = clock64();
-  if (warp == 0 && lane == 0) {
+  if (warp == TC_CWARPS && lane == 0) {
     tma_prefetch_desc(&mapA);
     tma_prefetch_desc(&mapB);
     for (int s = 0; s < STAGES; s++) {
-      mbar_init(full_bar + s, 2);                 // two producer threads (A tiles / B tiles): one TMA issue costs ~200 cycles,
-                                                  // a single producer (~410 cycles per K block) could not feed the 256-cycle MMAs
-      mbar_init(empty_bar + s, MC ? 2 : 1);       // MC: the slot is also written by the peer -> both MMA threads release it
+      mbar_init(full_bar + s, 2);                 // two producer threads (A tiles / B tiles)
+      mbar_init(empty_bar + s, MC ? 2 * TC_CWARPS : TC_CWARPS);   // MC: the slot is also written by the peer -> both CTAs' consumers release it
     }
-    mbar_init(tmem_full_bar, 1);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, NT);
-  pdl_wait();          // everything above touched only shared memory / TMEM / kernel parameters
+  pdl_wait();          // everything above touched only shared memory / kernel parameters
   pdl_trigger();
-  tc_fence_before();
   if (MC) cluster_sync_all(); else __syncthreads();   // peer barriers must be initialised before any multicast lands
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   const uint32_t crank = MC ? cluster_ctarank() : 0;
   if (dbg && threadIdx.x == 0) p.dbg[1] = clock64();
 
-  if (warp == 0) {
+  if (warp == TC_CWARPS) {
     if (lane == 0) {
       // ===== TMA producer, A tiles =====
       const int cpb = p.conv ? p.Cin / TC_BK : 1;
@@ -263,7 +248,7 @@ __global__ void __launch_bounds__(TC_THREADS) tc_gemm_conv_kernel(const __grid_c
       if (dbg) p.dbg[3] = clock64();
     }
     __syncwarp();
-  } else if (warp == 6) {
+  } else if (warp == TC_CWARPS + 1) {
     if (lane == 0) {
       // ===== TMA producer, B tiles (weights) =====
       const uint64_t polB = p.w_evict_last ? l2_policy_evict_last() : l2_policy_evict_normal();
@@ -277,87 +262,56 @@ __global__ void __launch_bounds__(TC_THREADS) tc_gemm_conv_kernel(const __grid_c
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // ===== MMA issuer (one thread) =====
-      constexpr uint32_t idesc = make_idesc_bf16(TC_BM, NT);
-      for (int kb = 0; kb < KB; kb++) {
-        const int s = kb % STAGES;
-        const uint32_t ph = (kb / STAGES) & 1;
-        mbar_wait(full_bar + s, ph);
-        if (dbg && kb == 0) p.dbg[4] = clock64();
-        if (dbg && kb < 40) p.dbg[16 + kb] = clock64();          // MMA thread: K block kb landed
-        tc_fence_after();
-        const uint32_t sa = smem_u32(smem + s * SM::STAGE_BYTES);
-        const uint32_t sb = sa + SM::A_BYTES;
-        const uint64_t da = make_kmajor_sw128_desc(sa);
-        const uint64_t db = make_kmajor_sw128_desc(sb);
-#pragma unroll
-        for (int k = 0; k < TC_BK / 16; k++) {
-          // advance 16 elements (32 B) along K inside the 128 B swizzle row: +2 in the 16 B-unit address field
-          umma_bf16(tmem_base, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (kb | k) != 0 ? 1u : 0u);
-        }
-        if (MC) umma_commit_mc(empty_bar + s, (uint16_t)3);   // frees the slot in BOTH CTAs
-        else umma_commit(empty_bar + s);                       // frees the smem stage when these MMAs retire
-      }
-      umma_commit(tmem_full_bar);             // accumulator complete
-      if (dbg) p.dbg[5] = clock64();
-    }
-    __syncwarp();
   } else {
-    // ===== epilogue: warps 2..5 ; warp w may touch TMEM lanes [32*(w%4), 32*(w%4)+32) =====
-    const int quad = warp & 3;
-    const int row = quad * 32 + lane;          // row inside the 128-row tile == TMEM lane
-    // while the main loop runs: stage the bias slice of this N tile in shared memory (a dependent global load per
-    // 8 columns inside the drain loop cost ~6 us per tile before)
-    {
-      const int te = threadIdx.x - 64;
-      if (te < NT) s_bias[te] = (p.bias && blockIdx.z == 0 && n0 + te < p.N) ? __ldg(p.bias + n0 + te) : 0.f;
-      asm volatile("bar.sync 1, 128;" ::: "memory");
+    // ===== consumers: warpgroup wg accumulates rows [64 wg, 64 wg + 64) of the tile =====
+    const int wg = warp >> 2;
+    for (int c = threadIdx.x; c < NT; c += TC_CWARPS * 32)
+      s_bias[c] = (p.bias && blockIdx.z == 0 && n0 + c < p.N) ? __ldg(p.bias + n0 + c) : 0.f;
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+    float acc[NT / 2];
+    for (int kb = 0; kb < KB; kb++) {
+      const int s = kb % STAGES;
+      const uint32_t ph = (kb / STAGES) & 1;
+      mbar_wait(full_bar + s, ph);
+      if (dbg && threadIdx.x == 0 && kb == 0) p.dbg[4] = clock64();
+      if (dbg && threadIdx.x == 0 && kb < 40) p.dbg[16 + kb] = clock64();          // consumer: K block kb landed
+      const uint32_t sa = smem_u32(smem + s * SM::STAGE_BYTES);
+      wgmma_fence();
+      tc_mma_kblock<NT>(acc, sa + wg * (SM::A_BYTES / 2), sa + SM::A_BYTES, kb == 0);
+      wgmma_commit();
+      wgmma_wait0();
+      wgmma_acc_fence<NT / 2>(acc);
+      __syncwarp();
+      if (lane == 0) {
+        if (MC) { mbar_arrive_cta(empty_bar + s, 0); mbar_arrive_cta(empty_bar + s, 1); }   // frees the slot in BOTH CTAs
+        else mbar_arrive(empty_bar + s);
+      }
     }
-    bool row_ok;
-    int64_t row_off;
-    if (p.conv) {
-      const int h = h0 + row / p.BW, w = w0 + row % p.BW;
-      row_ok = (h < p.Ho) && (w < p.Wo);
-      row_off = (((int64_t)img * p.Ho + h) * p.Wo + w) * p.ldc;
-    } else {
-      row_ok = (m0 + row) < p.M;
-      row_off = (int64_t)(m0 + row) * p.ldc;
-    }
-    const bool use_mask = p.mask && !p.out_f32 && !p.atomic;
-    mbar_wait(tmem_full_bar, 0);
-    if (dbg && warp == 2 && lane == 0) p.dbg[6] = clock64();
-    tc_fence_after();
+    if (dbg && threadIdx.x == 0) p.dbg[5] = clock64();
+    // ===== epilogue from the accumulators (layout: lo_wgmma.cuh) =====
+    const int rbase = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int cq = 2 * (lane & 3);
     if (p.lstm) {
-      // ---- fused LSTM cell (nn.LSTMCell, gate order i,f,g,o).  The 32x32 accumulator chunk is transposed through the idle
-      // pipeline ring so that a lane owns one hidden unit (4 interleaved gate columns) and consecutive lanes consecutive units
-      float* stg = reinterpret_cast<float*>(smem) + quad * (32 * 36);
+      // ---- fused LSTM cell (nn.LSTMCell, gate order i,f,g,o).  Columns 4u..4u+3 hold the gates of hidden unit u: the even
+      // lane of a pair holds (i, f), the odd one (g, o)
       const int D = p.l_D;
-#pragma unroll 1
-      for (int c = 0; c < NT; c += 32) {
-        uint32_t v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)c, v);
 #pragma unroll
-        for (int g = 0; g < 8; g++)
-          *reinterpret_cast<uint4*>(&stg[lane * 36 + g * 4]) = make_uint4(v[g * 4], v[g * 4 + 1], v[g * 4 + 2], v[g * 4 + 3]);
-        __syncwarp();
-        const int u = lane & 7;
-        const int j = (n0 + c) / 4 + u;
-#pragma unroll 2
-        for (int i = 0; i < 8; i++) {
-          const int rl = i * 4 + (lane >> 3);
-          const int b = m0 + quad * 32 + rl;
-          if (b >= p.M || j >= D) continue;
-          const float4 a = *reinterpret_cast<const float4*>(&stg[rl * 36 + 4 * u]);
+      for (int h = 0; h < 2; h++) {
+        const int b = m0 + rbase + 8 * h;
+#pragma unroll
+        for (int i = 0; i < NT / 8; i++) {
+          const float a0 = acc[4 * i + 2 * h], a1 = acc[4 * i + 2 * h + 1];
+          const float o0 = __shfl_xor_sync(0xffffffffu, a0, 1), o1 = __shfl_xor_sync(0xffffffffu, a1, 1);
+          const int j = (n0 + 8 * i + cq) / 4;
+          if ((lane & 1) || b >= p.M || j >= D) continue;
           int64_t tk = p.l_tok[(int64_t)b * p.l_tok_stride];
           tk = tk < 0 ? 0 : (tk >= p.l_V ? p.l_V - 1 : tk);
           const float* pt = p.l_ptab + tk * 4 * D;
           const float* hh = p.l_hh + (int64_t)b * p.l_hh_stride;
-          const float pi = a.x + pt[j] + hh[j];
-          const float pf = a.y + pt[D + j] + hh[D + j];
-          const float pg = a.z + pt[2 * D + j] + hh[2 * D + j];
-          const float po = a.w + pt[3 * D + j] + hh[3 * D + j];
+          const float pi = a0 + pt[j] + hh[j];
+          const float pf = a1 + pt[D + j] + hh[D + j];
+          const float pg = o0 + pt[2 * D + j] + hh[2 * D + j];
+          const float po = o1 + pt[3 * D + j] + hh[3 * D + j];
           const float ig = sigmoidf_(pi), fg = sigmoidf_(pf), gg = tanhf(pg), og = sigmoidf_(po);
           const float cn = fg * p.l_cprev[(int64_t)b * D + j] + ig * gg;
           const float hn = og * tanhf(cn);
@@ -368,85 +322,42 @@ __global__ void __launch_bounds__(TC_THREADS) tc_gemm_conv_kernel(const __grid_c
           if (p.l_hbf) p.l_hbf[(int64_t)b * D + j] = __float2bfloat16_rn(hn);
           if (p.l_hd) p.l_hd[(int64_t)b * p.l_hd_stride + j] = p.l_dmask ? hn * p.l_dmask[(int64_t)b * p.l_hd_stride + j] : hn;
         }
-        __syncwarp();
       }
-    } else
-#pragma unroll 1
-    for (int c = 0; c < NT; c += 32) {
-      uint4 mk4[4];
-      if (use_mask && row_ok) {                 // issue the mask loads of the whole chunk before the TMEM read
+    } else {
+      const bool use_mask = p.mask && !p.out_f32 && !p.atomic;
 #pragma unroll
-        for (int g = 0; g < 4; g++)
-          if (n0 + c + g * 8 < p.N) mk4[g] = *reinterpret_cast<const uint4*>(p.mask + row_off + n0 + c + g * 8);
-      }
-      uint32_t v[32];
-      tmem_ld32(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)c, v);   // warp-collective: no divergence around it
-      if (!row_ok) continue;
-#pragma unroll
-      for (int g = 0; g < 4; g++) {
-        const int n = n0 + c + g * 8;
-        if (n >= p.N) continue;
-        float f[8];
-        const float4 b0 = *reinterpret_cast<const float4*>(&s_bias[c + g * 8]);
-        const float4 b1 = *reinterpret_cast<const float4*>(&s_bias[c + g * 8 + 4]);
-        const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-#pragma unroll
-        for (int i = 0; i < 8; i++) f[i] = __uint_as_float(v[g * 8 + i]) + bb[i];
-        if (p.atomic) {
-          float* o = reinterpret_cast<float*>(p.out) + row_off + n;
-#pragma unroll
-          for (int i = 0; i < 8; i++) atomicAdd(o + i, f[i]);
-        } else if (p.out_f32) {
-          float* o = reinterpret_cast<float*>(p.out) + row_off + n;
-          if (p.accumulate) {
-            float old[8];
-            ld8(o, old);
-#pragma unroll
-            for (int i = 0; i < 8; i++) f[i] += old[i];
-          }
-          if (p.relu) {
-#pragma unroll
-            for (int i = 0; i < 8; i++) f[i] = fmaxf(f[i], 0.f);
-          }
-          st8(o, f);
+      for (int h = 0; h < 2; h++) {
+        const int row = rbase + 8 * h;
+        bool row_ok;
+        int64_t row_off;
+        if (p.conv) {
+          const int hh = h0 + row / p.BW, ww = w0 + row % p.BW;
+          row_ok = (hh < p.Ho) && (ww < p.Wo);
+          row_off = (((int64_t)img * p.Ho + hh) * p.Wo + ww) * p.ldc;
         } else {
-          bf16* o = reinterpret_cast<bf16*>(p.out) + row_off + n;
-          if (p.accumulate) {
-            float old[8];
-            ld8(o, old);
+          row_ok = (m0 + row) < p.M;
+          row_off = (int64_t)(m0 + row) * p.ldc;
+        }
+        if (!row_ok) continue;
 #pragma unroll
-            for (int i = 0; i < 8; i++) f[i] += old[i];
-          }
-          if (p.relu) {
-#pragma unroll
-            for (int i = 0; i < 8; i++) f[i] = fmaxf(f[i], 0.f);
-          }
-          if (use_mask) {
-            const uint32_t w[4] = {mk4[g].x, mk4[g].y, mk4[g].z, mk4[g].w};
-#pragma unroll
-            for (int i = 0; i < 4; i++) {
-              if (!(__uint_as_float(w[i] << 16) > 0.f)) f[2 * i] = 0.f;
-              if (!(__uint_as_float(w[i] & 0xffff0000u) > 0.f)) f[2 * i + 1] = 0.f;
-            }
-          }
-          st8(o, f);
+        for (int i = 0; i < NT / 8; i++) {
+          if (n0 + 8 * i >= p.N) continue;       // 8-column groups: columns up to roundup8(N) are written (ldc allows it)
+          const int c = 8 * i + cq;
+          tc_store_pair(p, row_off + n0 + c, acc[4 * i + 2 * h] + s_bias[c], acc[4 * i + 2 * h + 1] + s_bias[c + 1], use_mask);
         }
       }
     }
+    if (dbg && threadIdx.x == 0) p.dbg[6] = clock64();
   }
-  tc_fence_before();
-  if (MC) cluster_sync_all(); else __syncthreads();   // a CTA may not exit while its peer can still multicast into it
+  if (MC) cluster_sync_all();   // a CTA may not exit while its peer can still multicast into it or arrive on its barriers
   if (dbg && threadIdx.x == 0) p.dbg[7] = clock64();
-  if (warp == 1) tmem_dealloc(tmem_base, NT);
-  if (dbg && threadIdx.x == 32) p.dbg[8] = clock64();
 }
 
 // ------------------------------------------------------------------------------------------------
-// Persistent 3x3 convolution (forward and data gradient): one CTA per SM walks over output tiles of 128 positions x NT
-// channels; TWO TMEM accumulators (2 x NT columns) so that the 128-thread epilogue of tile i drains while the MMA thread
-// already accumulates tile i+1; the TMA ring runs ahead across tile boundaries.  NT = 256 for the 256/512-channel layers:
-// per 64-wide K block a CTA pulls 16 KB of A + 32 KB of B from L2 for 4.2 MFLOP = 85 FLOP per L2 byte (128 x 128 tiles: 64).
-// The one-tile-per-CTA kernel above is L2-bandwidth bound at 45-56 % tensor-pipe activity (profiles/r1_tc_conv_r1_raw.csv).
+// Persistent 3x3 convolution (forward and data gradient): one CTA per SM walks over output tiles of MT x 128 positions x NT
+// channels.  The TMA ring runs ahead across tile boundaries, so the next tile's operands stream in while the consumer
+// warpgroups run the epilogue of the current one.  NT = 256 for the 256/512-channel layers: per 64-wide K block a CTA
+// pulls 16 KB of A + 32 KB of B from L2 for 4.2 MFLOP = 85 FLOP per L2 byte (128 x 128 tiles: 64).
 // ------------------------------------------------------------------------------------------------
 template <int NT, int STAGES, int MT>
 struct TcPSmem {
@@ -464,14 +375,11 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_conv_p_kernel(const __grid_c
                                                                  const __grid_constant__ CUtensorMap mapB, TcParams p, int ntiles_n,
                                                                  int total_tiles, int mtiles) {
   using SM = TcPSmem<NT, STAGES, MT>;
-  static_assert(2 * MT * NT <= 512, "TMEM columns");
+  static_assert(MT * NT <= 256, "accumulator registers");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * SM::STAGE_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tfull_bar = empty_bar + STAGES;        // [2] accumulator complete
-  uint64_t* tempty_bar = tfull_bar + 2;            // [2] accumulator drained
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
   float* s_bias = reinterpret_cast<float*>(smem + STAGES * SM::STAGE_BYTES + 256);      // [2][NT]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -479,28 +387,20 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_conv_p_kernel(const __grid_c
   const int cpb = p.Cin / TC_BK;
   const int per_img = p.tiles_w * p.tiles_h;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == TC_CWARPS && lane == 0) {
     tma_prefetch_desc(&mapA);
     tma_prefetch_desc(&mapB);
     for (int s = 0; s < STAGES; s++) {
       mbar_init(full_bar + s, 2);                // A producer + B producer
-      mbar_init(empty_bar + s, 1);
-    }
-    for (int b = 0; b < 2; b++) {
-      mbar_init(tfull_bar + b, 1);
-      mbar_init(tempty_bar + b, 4);              // one arrival per epilogue warp
+      mbar_init(empty_bar + s, TC_CWARPS);       // one arrival per consumer warp
     }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 2 * MT * NT);
   pdl_wait();
   pdl_trigger();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == TC_CWARPS) {
     if (lane == 0) {
       // ===== TMA producer, A tiles (implicit im2col: tap = coordinate shift, halo = out-of-bounds zero fill) =====
       uint32_t it = 0;
@@ -532,7 +432,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_conv_p_kernel(const __grid_c
       }
     }
     __syncwarp();
-  } else if (warp == 6) {
+  } else if (warp == TC_CWARPS + 1) {
     if (lane == 0) {
       // ===== TMA producer, B tiles (weights: re-read by every CTA -> keep them in L2) =====
       const uint64_t polB = l2_policy_evict_last();
@@ -549,125 +449,84 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_conv_p_kernel(const __grid_c
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // ===== MMA issuer =====
-      constexpr uint32_t idesc = make_idesc_bf16(TC_BM, NT);
-      uint32_t it = 0, lt = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, lt++) {
-        const uint32_t buf = lt & 1;
-        const int nsub = min(MT, mtiles - (tile / ntiles_n) * MT);
-        mbar_wait(tempty_bar + buf, ((lt >> 1) & 1) ^ 1);       // the epilogue has drained this accumulator set (2 tiles ago)
-        tc_fence_after();
-        const uint32_t tacc = tmem_base + buf * (MT * NT);
-        for (int kb = 0; kb < KB; kb++, it++) {
-          const int s = it % STAGES;
-          const uint32_t ph = (it / STAGES) & 1;
-          mbar_wait(full_bar + s, ph);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + s * SM::STAGE_BYTES);
-          const uint64_t db = make_kmajor_sw128_desc(sa + MT * SM::A_BYTES);
-#pragma unroll
-          for (int j = 0; j < MT; j++) {
-            if (j < nsub) {
-              const uint64_t da = make_kmajor_sw128_desc(sa + j * SM::A_BYTES);
-#pragma unroll
-              for (int k = 0; k < TC_BK / 16; k++)
-                umma_bf16(tacc + j * NT, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (kb | k) != 0 ? 1u : 0u);
-            }
-          }
-          umma_commit(empty_bar + s);
-        }
-        umma_commit(tfull_bar + buf);
-      }
-    }
-    __syncwarp();
   } else {
-    // ===== epilogue: warps 2..5 ; warp w may touch TMEM lanes [32*(w%4), 32*(w%4)+32) =====
-    const int quad = warp & 3;
-    const int row = quad * 32 + lane;
-    const int te = threadIdx.x - 64;                               // 0..127
+    // ===== consumers: warpgroup wg owns rows [64 wg, 64 wg + 64) of every sub-tile =====
+    const int wg = warp >> 2;
+    const int rbase = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int cq = 2 * (lane & 3);
     const bool use_mask = p.mask != nullptr;
-    uint32_t lt = 0;
+    uint32_t it = 0, lt = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, lt++) {
-      const uint32_t buf = lt & 1;
       const int n0 = (tile % ntiles_n) * NT;
       const int mt0 = (tile / ntiles_n) * MT;
       const int nsub = min(MT, mtiles - mt0);
-      float* sb = s_bias + buf * NT;
-      for (int c = te; c < NT; c += 128) sb[c] = (p.bias && n0 + c < p.N) ? __ldg(p.bias + n0 + c) : 0.f;
-      asm volatile("bar.sync 1, 128;" ::: "memory");               // bias of this tile staged (buffer last read 2 tiles ago)
-      mbar_wait(tfull_bar + buf, (lt >> 1) & 1);
-      tc_fence_after();
-#pragma unroll 1
-      for (int j = 0; j < nsub; j++) {
+      float* sb = s_bias + (lt & 1) * NT;        // double buffered: a slower thread may still read the previous tile's
+      for (int c = threadIdx.x; c < NT; c += TC_CWARPS * 32) sb[c] = (p.bias && n0 + c < p.N) ? __ldg(p.bias + n0 + c) : 0.f;
+      asm volatile("bar.sync 1, 256;" ::: "memory");
+      float acc[MT][NT / 2];
+      for (int kb = 0; kb < KB; kb++, it++) {
+        const int s = it % STAGES;
+        const uint32_t ph = (it / STAGES) & 1;
+        mbar_wait(full_bar + s, ph);
+        const uint32_t sa = smem_u32(smem + s * SM::STAGE_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int j = 0; j < MT; j++)
+          // issued for every sub-tile, also the missing last one of an odd tile count (its slot holds stale data; that
+          // accumulator is never stored): a predicate here makes ptxas serialise the warpgroup MMAs
+          tc_mma_kblock<NT>(acc[j], sa + j * SM::A_BYTES + wg * (SM::A_BYTES / 2), sa + MT * SM::A_BYTES, kb == 0);
+        wgmma_commit();
+        wgmma_wait0();
+#pragma unroll
+        for (int j = 0; j < MT; j++) wgmma_acc_fence<NT / 2>(acc[j]);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(empty_bar + s);
+      }
+#pragma unroll
+      for (int j = 0; j < MT; j++) {
+        if (j >= nsub) continue;
         const int mt = mt0 + j;
         const int img = mt / per_img, rem = mt % per_img;
-        const int h = (rem / p.tiles_w) * p.BH + row / p.BW, w = (rem % p.tiles_w) * p.BW + row % p.BW;
-        const bool row_ok = (h < p.Ho) && (w < p.Wo);
-        const int64_t row_off = (((int64_t)img * p.Ho + h) * p.Wo + w) * p.ldc;
-        const uint32_t tacc = tmem_base + buf * (MT * NT) + j * NT + ((uint32_t)(quad * 32) << 16);
-#pragma unroll 1
-        for (int c = 0; c < NT; c += 32) {
-          uint4 mk4[4];
-          if (use_mask && row_ok) {
 #pragma unroll
-            for (int g = 0; g < 4; g++)
-              if (n0 + c + g * 8 < p.N) mk4[g] = *reinterpret_cast<const uint4*>(p.mask + row_off + n0 + c + g * 8);
-          }
-          uint32_t v[32];
-          tmem_ld32(tacc + (uint32_t)c, v);
-          if (!row_ok) continue;
+        for (int h = 0; h < 2; h++) {
+          const int row = rbase + 8 * h;
+          const int hh = (rem / p.tiles_w) * p.BH + row / p.BW, ww = (rem % p.tiles_w) * p.BW + row % p.BW;
+          if (hh >= p.Ho || ww >= p.Wo) continue;
+          const int64_t row_off = (((int64_t)img * p.Ho + hh) * p.Wo + ww) * p.ldc;
 #pragma unroll
-          for (int g = 0; g < 4; g++) {
-            const int n = n0 + c + g * 8;
-            if (n >= p.N) continue;
-            float f[8];
-            const float4 b0 = *reinterpret_cast<const float4*>(&sb[c + g * 8]);
-            const float4 b1 = *reinterpret_cast<const float4*>(&sb[c + g * 8 + 4]);
-            const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-#pragma unroll
-            for (int i = 0; i < 8; i++) f[i] = __uint_as_float(v[g * 8 + i]) + bb[i];
-            if (p.relu) {
-#pragma unroll
-              for (int i = 0; i < 8; i++) f[i] = fmaxf(f[i], 0.f);
-            }
+          for (int i = 0; i < NT / 8; i++) {
+            if (n0 + 8 * i >= p.N) continue;
+            const int c = 8 * i + cq;
+            float f0 = acc[j][4 * i + 2 * h] + sb[c], f1 = acc[j][4 * i + 2 * h + 1] + sb[c + 1];
+            if (p.relu) { f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f); }
             if (use_mask) {
-              const uint32_t wv[4] = {mk4[g].x, mk4[g].y, mk4[g].z, mk4[g].w};
-#pragma unroll
-              for (int i = 0; i < 4; i++) {
-                if (!(__uint_as_float(wv[i] << 16) > 0.f)) f[2 * i] = 0.f;
-                if (!(__uint_as_float(wv[i] & 0xffff0000u) > 0.f)) f[2 * i + 1] = 0.f;
-              }
+              const uint32_t w = *reinterpret_cast<const uint32_t*>(p.mask + row_off + n0 + c);
+              if (!(__uint_as_float(w << 16) > 0.f)) f0 = 0.f;
+              if (!(__uint_as_float(w & 0xffff0000u) > 0.f)) f1 = 0.f;
             }
-            st8(reinterpret_cast<bf16*>(p.out) + row_off + n, f);
+            __nv_bfloat162 hv = __floats2bfloat162_rn(f0, f1);
+            *reinterpret_cast<__nv_bfloat162*>(reinterpret_cast<bf16*>(p.out) + row_off + n0 + c) = hv;
           }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar + buf);                  // this warp's quarter of the accumulators is free again
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, 2 * MT * NT);
 }
 
 // ------------------------------------------------------------------------------------------------
-// Weight gradient on tcgen05:  dW[co][tap][ci] += sum_p dY[p][co] * X[p + tap][ci]
+// Weight gradient on wgmma:  dW[co][tap][ci] += sum_p dY[p][co] * X[p + tap][ci]
 // GEMM view: M = co (128), N = ci (NT), K = output positions.  Both operands are "MN-major" (the channel index is
-// contiguous in NHWC), which UMMA takes directly: smem tile = [128 positions][64 channels] (one TMA box, SWIZZLE_128B),
-// descriptor LBO = distance between 64-channel boxes, SBO = 1024 B (8 positions), 16 positions (2048 B) per MMA.
-// grid: (co tiles * ci tiles, 9 taps, K splits); epilogue = fp32 atomics into dW (split-K partial sums).
+// contiguous in NHWC), which wgmma takes directly (transpose flags): smem tile = [128 positions][64 channels] (one TMA
+// box, SWIZZLE_128B), descriptor LBO = distance between 64-channel boxes, SBO = 1024 B (8 positions), 16 positions
+// (2048 B) per MMA.  grid: (co tiles * ci tiles, 9 taps, K splits); the splits add their partial sums onto dW with fp32 atomics,
+// or — option "deterministic" — form one cluster (<= 8) whose rank 0 adds them in split order and alone adds the result.
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint64_t make_mnmajor_sw128_desc(uint32_t saddr, uint32_t lbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;   // next 64-element block along M/N
   d |= (uint64_t)(1024 >> 4) << 32;                   // next 8 rows along K
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;                             // SWIZZLE_128B
   return d;
 }
 
@@ -679,19 +538,18 @@ struct WgParams {
                       // 2: the same, batched over blockIdx.y (3-D maps {M|N, K, batch}; C of batch b at dw + b * batch_c)
   int64_t ldc;
   int64_t batch_c;
+  int ordered;        // 1: the K splits of a tile are one cluster, summed in split order (option "deterministic")
 };
 
 template <int NT, int STAGES>
-__global__ void __launch_bounds__(TC_THREADS) tc_wgrad_kernel(const __grid_constant__ CUtensorMap mapDY,
-                                                               const __grid_constant__ CUtensorMap mapX, WgParams p) {
+__global__ void __launch_bounds__(TC_THREADS, 1) tc_wgrad_kernel(const __grid_constant__ CUtensorMap mapDY,
+                                                                  const __grid_constant__ CUtensorMap mapX, WgParams p) {
   constexpr int BOX = 128 * 64 * 2;                 // one [128 pos][64 ch] box
   constexpr int A_BYTES = 2 * BOX, B_BYTES = (NT / 64) * BOX, STAGE_BYTES = A_BYTES + B_BYTES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full_bar = empty_bar + STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int co0 = (blockIdx.x / p.ci_tiles) * 128, ci0 = (blockIdx.x % p.ci_tiles) * NT;
   const int tap = p.plain == 2 ? 0 : blockIdx.y, r = tap / 3, q = tap % 3;
@@ -699,121 +557,118 @@ __global__ void __launch_bounds__(TC_THREADS) tc_wgrad_kernel(const __grid_const
   const int ks0 = blockIdx.z * p.per_split;
   const int ks1 = min(p.kstages, ks0 + p.per_split);
   const int KS = ks1 - ks0;
-  if (warp == 0 && lane == 0) {
+  if (warp == TC_CWARPS && lane == 0) {
     tma_prefetch_desc(&mapDY);
     tma_prefetch_desc(&mapX);
-    for (int s = 0; s < STAGES; s++) { mbar_init(full_bar + s, 2); mbar_init(empty_bar + s, 1); }   // two producers
-    mbar_init(tmem_full_bar, 1);
+    for (int s = 0; s < STAGES; s++) { mbar_init(full_bar + s, 2); mbar_init(empty_bar + s, TC_CWARPS); }   // two producers
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, NT);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  if (KS > 0) {
-    if (warp == 0) {
-      if (lane == 0) {
-        const int per_img = p.tiles_w * p.tiles_h;
-        for (int i = 0; i < KS; i++) {
-          const int s = i % STAGES;
-          const uint32_t ph = (i / STAGES) & 1;
-          mbar_wait(empty_bar + s, ph ^ 1);
-          const int ks = ks0 + i;
-          const int img = ks / per_img, rem = ks % per_img;
-          const int h0 = (rem / p.tiles_w) * p.BH, w0 = (rem % p.tiles_w) * p.BW;
-          uint8_t* sa = smem + s * STAGE_BYTES;
-          mbar_expect_tx(full_bar + s, A_BYTES);
-          if (p.plain == 2) {
-            tma_load_3d(sa, &mapDY, full_bar + s, co0, ks * 128, bz);
-            tma_load_3d(sa + BOX, &mapDY, full_bar + s, co0 + 64, ks * 128, bz);
-          } else if (p.plain) {
-            tma_load_2d(sa, &mapDY, full_bar + s, co0, ks * 128);
-            tma_load_2d(sa + BOX, &mapDY, full_bar + s, co0 + 64, ks * 128);
-          } else {
-            tma_load_4d(sa, &mapDY, full_bar + s, co0, w0, h0, img);
-            tma_load_4d(sa + BOX, &mapDY, full_bar + s, co0 + 64, w0, h0, img);
-          }
+  float acc[NT / 2];
+  if (warp == TC_CWARPS) {
+    if (lane == 0) {
+      const int per_img = p.tiles_w * p.tiles_h;
+      for (int i = 0; i < KS; i++) {
+        const int s = i % STAGES;
+        const uint32_t ph = (i / STAGES) & 1;
+        mbar_wait(empty_bar + s, ph ^ 1);
+        const int ks = ks0 + i;
+        const int img = ks / per_img, rem = ks % per_img;
+        const int h0 = (rem / p.tiles_w) * p.BH, w0 = (rem % p.tiles_w) * p.BW;
+        uint8_t* sa = smem + s * STAGE_BYTES;
+        mbar_expect_tx(full_bar + s, A_BYTES);
+        if (p.plain == 2) {
+          tma_load_3d(sa, &mapDY, full_bar + s, co0, ks * 128, bz);
+          tma_load_3d(sa + BOX, &mapDY, full_bar + s, co0 + 64, ks * 128, bz);
+        } else if (p.plain) {
+          tma_load_2d(sa, &mapDY, full_bar + s, co0, ks * 128);
+          tma_load_2d(sa + BOX, &mapDY, full_bar + s, co0 + 64, ks * 128);
+        } else {
+          tma_load_4d(sa, &mapDY, full_bar + s, co0, w0, h0, img);
+          tma_load_4d(sa + BOX, &mapDY, full_bar + s, co0 + 64, w0, h0, img);
         }
       }
-      __syncwarp();
-    } else if (warp == 6) {
-      if (lane == 0) {            // second producer: the X (B operand) boxes
-        const int per_img = p.tiles_w * p.tiles_h;
-        for (int i = 0; i < KS; i++) {
-          const int s = i % STAGES;
-          const uint32_t ph = (i / STAGES) & 1;
-          mbar_wait(empty_bar + s, ph ^ 1);
-          const int ks = ks0 + i;
-          const int img = ks / per_img, rem = ks % per_img;
-          const int h0 = (rem / p.tiles_w) * p.BH, w0 = (rem % p.tiles_w) * p.BW;
-          uint8_t* sb = smem + s * STAGE_BYTES + A_BYTES;
-          mbar_expect_tx(full_bar + s, B_BYTES);
-          if (p.plain == 2) {
+    }
+    __syncwarp();
+  } else if (warp == TC_CWARPS + 1) {
+    if (lane == 0) {            // second producer: the X (B operand) boxes
+      const int per_img = p.tiles_w * p.tiles_h;
+      for (int i = 0; i < KS; i++) {
+        const int s = i % STAGES;
+        const uint32_t ph = (i / STAGES) & 1;
+        mbar_wait(empty_bar + s, ph ^ 1);
+        const int ks = ks0 + i;
+        const int img = ks / per_img, rem = ks % per_img;
+        const int h0 = (rem / p.tiles_w) * p.BH, w0 = (rem % p.tiles_w) * p.BW;
+        uint8_t* sb = smem + s * STAGE_BYTES + A_BYTES;
+        mbar_expect_tx(full_bar + s, B_BYTES);
+        if (p.plain == 2) {
 #pragma unroll
-            for (int j = 0; j < NT / 64; j++) tma_load_3d(sb + j * BOX, &mapX, full_bar + s, ci0 + 64 * j, ks * 128, bz);
-          } else if (p.plain) {
+          for (int j = 0; j < NT / 64; j++) tma_load_3d(sb + j * BOX, &mapX, full_bar + s, ci0 + 64 * j, ks * 128, bz);
+        } else if (p.plain) {
 #pragma unroll
-            for (int j = 0; j < NT / 64; j++) tma_load_2d(sb + j * BOX, &mapX, full_bar + s, ci0 + 64 * j, ks * 128);
-          } else {
+          for (int j = 0; j < NT / 64; j++) tma_load_2d(sb + j * BOX, &mapX, full_bar + s, ci0 + 64 * j, ks * 128);
+        } else {
 #pragma unroll
-            for (int j = 0; j < NT / 64; j++)
-              tma_load_4d(sb + j * BOX, &mapX, full_bar + s, ci0 + 64 * j, w0 + q - p.pad, h0 + r - p.pad, img);
-          }
+          for (int j = 0; j < NT / 64; j++)
+            tma_load_4d(sb + j * BOX, &mapX, full_bar + s, ci0 + 64 * j, w0 + q - p.pad, h0 + r - p.pad, img);
         }
       }
-      __syncwarp();
-    } else if (warp == 1) {
-      if (lane == 0) {
-        constexpr uint32_t idesc = make_idesc_bf16(128, NT) | (1u << 15) | (1u << 16);   // A and B MN-major
-        for (int i = 0; i < KS; i++) {
-          const int s = i % STAGES;
-          const uint32_t ph = (i / STAGES) & 1;
-          mbar_wait(full_bar + s, ph);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + s * STAGE_BYTES);
-          const uint32_t sb = sa + A_BYTES;
+    }
+    __syncwarp();
+  } else {
+    // ===== consumers: warpgroup wg accumulates co rows [64 wg, 64 wg + 64) = A box wg =====
+    const int wg = warp >> 2;
 #pragma unroll
-          for (int k = 0; k < 8; k++) {
-            const uint64_t da = make_mnmajor_sw128_desc(sa + k * 2048, BOX);
-            const uint64_t db = make_mnmajor_sw128_desc(sb + k * 2048, BOX);
-            umma_bf16(tmem_base, da, db, idesc, (i | k) != 0 ? 1u : 0u);
-          }
-          umma_commit(empty_bar + s);
-        }
-        umma_commit(tmem_full_bar);
-      }
-      __syncwarp();
-    } else {
-      const int quad = warp & 3;
-      float* stg = reinterpret_cast<float*>(smem) + quad * (32 * 36);    // transpose staging in the (now idle) ring
-      mbar_wait(tmem_full_bar, 0);
-      tc_fence_after();
-#pragma unroll 1
-      for (int c = 0; c < NT; c += 32) {
-        uint32_t v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)c, v);
+    for (int i = 0; i < NT / 2; i++) acc[i] = 0.f;
+    for (int i = 0; i < KS; i++) {
+      const int s = i % STAGES;
+      const uint32_t ph = (i / STAGES) & 1;
+      mbar_wait(full_bar + s, ph);
+      const uint32_t sa = smem_u32(smem + s * STAGE_BYTES) + wg * BOX;
+      const uint32_t sb = smem_u32(smem + s * STAGE_BYTES) + A_BYTES;
+      wgmma_fence();
 #pragma unroll
-        for (int g = 0; g < 8; g++)
-          *reinterpret_cast<uint4*>(&stg[lane * 36 + g * 4]) = make_uint4(v[g * 4], v[g * 4 + 1], v[g * 4 + 2], v[g * 4 + 3]);
-        __syncwarp();
-        // one warp instruction = one 128 B row segment of dW -> coalesced red.global.add
-#pragma unroll 4
-        for (int rr = 0; rr < 32; rr++) {
-          const int co = co0 + quad * 32 + rr;
-          const int ci = ci0 + c + lane;
-          if (co < p.Cout && ci < p.Cin) {
-            float* o = p.plain ? p.dw + (int64_t)bz * p.batch_c + (int64_t)co * p.ldc + ci : p.dw + ((int64_t)co * 9 + tap) * p.Cin + ci;
-            atomicAdd(o, stg[rr * 36 + lane]);
-          }
-        }
-        __syncwarp();
+      for (int k = 0; k < 8; k++)
+        Wgmma<NT, 1, 1>::mma(acc, make_mnmajor_sw128_desc(sa + k * 2048, BOX), make_mnmajor_sw128_desc(sb + k * 2048, BOX), 1u);
+      wgmma_commit();
+      wgmma_wait0();
+      wgmma_acc_fence<NT / 2>(acc);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(empty_bar + s);
+    }
+  }
+  if (p.ordered && gridDim.z > 1) {
+    // ordered split K: the splits of this tile are one cluster; rank 0 adds the partials in split order and alone writes dW
+    float* part = reinterpret_cast<float*>(smem);      // the ring is idle once every consumer is past its last K block
+    if (warp < TC_CWARPS) {
+      asm volatile("bar.sync 1, 256;" ::: "memory");
+#pragma unroll
+      for (int i = 0; i < NT / 2; i++) part[i * 256 + threadIdx.x] = acc[i];
+    }
+    cl_sync();
+    if (cl_rank() == 0 && warp < TC_CWARPS) {
+#pragma unroll
+      for (int i = 0; i < NT / 2; i += 16) cl_sum_n<16>(part + i * 256 + threadIdx.x, 256, acc + i);
+    }
+    cl_sync();
+    if (cl_rank() != 0) return;
+  }
+  if (warp < TC_CWARPS) {
+    const int wg = warp >> 2, cq = 2 * (lane & 3);
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      const int co = co0 + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+      if (co >= p.Cout) continue;
+      float* orow = p.plain ? p.dw + (int64_t)bz * p.batch_c + (int64_t)co * p.ldc : p.dw + ((int64_t)co * 9 + tap) * p.Cin;
+#pragma unroll
+      for (int i = 0; i < NT / 8; i++) {                 // split-K partial sums (or, ordered, the tile's sum) onto C
+        const int ci = ci0 + 8 * i + cq;
+        if (ci < p.Cin) atomicAdd(orow + ci, acc[4 * i + 2 * h]);
+        if (ci + 1 < p.Cin) atomicAdd(orow + ci + 1, acc[4 * i + 2 * h + 1]);
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, NT);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -830,7 +685,7 @@ bool tc_available() {
   g_tc_state = 0;
   int dev = 0, major = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) return false;
-  if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess || major != 10) return false;
+  if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess || major != 9) return false;
   void* fn = nullptr;
   cudaDriverEntryPointQueryResult qres;
   if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) != cudaSuccess || fn == nullptr ||
@@ -941,7 +796,7 @@ static bool g_lstm_epi_on = false;
 // splits > 1 (or atomic_acc): fp32 C only, partial sums are ADDED onto C with atomics (C must hold the base values)
 int tc_gemm_nt_ex(const bf16* A, int64_t lda, const bf16* W, int64_t ldw, void* C, int dtC, int64_t ldc, int M, int N, int K,
                   const float* bias, int accumulate, int relu, int splits, int atomic_acc, int small_n_tile, cudaStream_t st) {
-  if (!tc_available()) return fail(LO_ENOTSUP, "%s: needs an sm_100 device", __func__);
+  if (!tc_available()) return fail(LO_ENOTSUP, "%s: needs an sm_90 device", __func__);
   LO_CHECK_ARG(K % 64 == 0 && lda % 8 == 0 && ldw % 8 == 0 && ldc % 8 == 0 && ldc >= (N + 7) / 8 * 8, "K%64, ld%8, ldc >= roundup8(N)");
   LO_CHECK_ARG(((uintptr_t)A & 15) == 0 && ((uintptr_t)W & 15) == 0 && ((uintptr_t)C & 15) == 0, "16-byte alignment");
   CUtensorMap mA, mB;
@@ -990,8 +845,8 @@ int tc_gemm_nt(const bf16* A, int64_t lda, const bf16* W, int64_t ldw, void* C, 
   return tc_gemm_nt_ex(A, lda, W, ldw, C, dtC, ldc, M, N, K, bias, accumulate, relu, 1, 0, 0, st);
 }
 
-int g_opt_wgrad256 = 0;       // conv weight gradient with 128 x 256 tiles when Cin % 256 == 0: measured slower (two 96 KB stages
-                              // cannot hide the loads: 3.64 vs 3.42 ms for the conv tensor kernels, run 50)
+int g_opt_wgrad256 = 0;       // conv weight gradient with 128 x 256 tiles when Cin % 256 == 0: off, two 96 KB stages
+                              // cannot hide the loads
 int g_opt_conv_persist = 1;   // persistent double-accumulator kernel (tc_conv_p_kernel); 0 = one tile per CTA (tc_gemm_conv_kernel)
 
 int g_opt_conv_mt2 = 1;       // layers with <= 128 output channels: two 128-position sub-tiles per CTA tile share each weight stage
@@ -1018,7 +873,7 @@ static int launch_conv_p(const CUtensorMap& mA, const CUtensorMap& mB, const TcP
 
 int tc_conv3x3(const bf16* x, const bf16* w, const float* bias, const bf16* mask, bf16* y, int N, int H, int W, int Cin, int Cout,
                int pad, int relu, cudaStream_t st) {
-  if (!tc_available()) return fail(LO_ENOTSUP, "%s: needs an sm_100 device", __func__);
+  if (!tc_available()) return fail(LO_ENOTSUP, "%s: needs an sm_90 device", __func__);
   LO_CHECK_ARG(Cin % 64 == 0 && Cout % 8 == 0, "Cin%64==0, Cout%8==0");
   const int Ho = H + 2 * pad - 2, Wo = W + 2 * pad - 2;
   int BW = 128;
@@ -1089,14 +944,17 @@ static int launch_wgrad(const CUtensorMap& mDY, const CUtensorMap& mX, const WgP
     LO_CUDA(cudaFuncSetAttribute(tc_wgrad_kernel<NT, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, TOTAL));
     attr_set = true;
   }
-  tc_wgrad_kernel<NT, STAGES><<<grid, TC_THREADS, TOTAL, st>>>(mDY, mX, p);
+  if (p.ordered)
+    LO_CUDA(launch_cluster(tc_wgrad_kernel<NT, STAGES>, grid, dim3(TC_THREADS), (size_t)TOTAL, st, dim3(1, 1, grid.z), false, mDY, mX, p));
+  else
+    tc_wgrad_kernel<NT, STAGES><<<grid, TC_THREADS, TOTAL, st>>>(mDY, mX, p);
   LO_LAUNCH_OK();
   return LO_OK;
 }
 
-// dw must be zeroed by the caller (split-K partial sums are accumulated with atomics)
+// the weight gradient is ADDED onto dw (zero it for a plain product)
 int tc_conv3x3_wgrad(const bf16* x, const bf16* dy, float* dw, int N, int H, int W, int Cin, int Cout, int pad, cudaStream_t st) {
-  if (!tc_available()) return fail(LO_ENOTSUP, "%s: needs an sm_100 device", __func__);
+  if (!tc_available()) return fail(LO_ENOTSUP, "%s: needs an sm_90 device", __func__);
   LO_CHECK_ARG(Cin % 64 == 0 && Cout % 128 == 0, "Cin%64==0, Cout%128==0");
   const int Ho = H + 2 * pad - 2, Wo = W + 2 * pad - 2;
   int BW = 128;
@@ -1124,11 +982,13 @@ int tc_conv3x3_wgrad(const bf16* x, const bf16* dy, float* dw, int N, int H, int
   const int NT = (g_opt_wgrad256 && Cin % 256 == 0) ? 256 : (Cin >= 128 ? 128 : 64);
   p.ci_tiles = Cin / NT;
   const int tiles = (Cout / 128) * p.ci_tiles * 9;
-  int splits = cdiv(NT == 256 ? 148 : 148 * 2, tiles);
+  int splits = cdiv(NT == 256 ? LO_NUM_SMS : LO_NUM_SMS * 2, tiles);
+  if (g_opt_det && splits > 8) splits = 8;      // ordered: the splits of a tile are summed inside one (portable) cluster
   if (splits > p.kstages) splits = p.kstages;
   if (splits < 1) splits = 1;
   p.per_split = cdiv(p.kstages, splits);
   splits = cdiv(p.kstages, p.per_split);
+  p.ordered = g_opt_det && splits > 1;
   dim3 grid((Cout / 128) * p.ci_tiles, 9, splits);
   if (NT == 256) return launch_wgrad<256, 2>(mDY, mX, p, grid, st);
   if (NT == 128) return launch_wgrad<128, 3>(mDY, mX, p, grid, st);
@@ -1136,9 +996,9 @@ int tc_conv3x3_wgrad(const bf16* x, const bf16* dy, float* dw, int N, int H, int
 }
 
 // C[M][N] (fp32, ldc) += A[K][M]^T * B[K][N]; A, B bf16 row-major.  C must hold the values to accumulate onto
-// (zero it for a plain product): split-K partial sums land with fp32 atomics.
+// (zero it for a plain product): split-K partial sums land with fp32 atomics (in split order with option "deterministic").
 int tc_gemm_tn(const bf16* A, int64_t lda, const bf16* B, int64_t ldb, float* C, int64_t ldc, int M, int N, int K, cudaStream_t st) {
-  if (!tc_available()) return fail(LO_ENOTSUP, "%s: needs an sm_100 device", __func__);
+  if (!tc_available()) return fail(LO_ENOTSUP, "%s: needs an sm_90 device", __func__);
   LO_CHECK_ARG(lda % 8 == 0 && ldb % 8 == 0, "lda%8, ldb%8");
   LO_CHECK_ARG(((uintptr_t)A & 15) == 0 && ((uintptr_t)B & 15) == 0, "16-byte alignment");
   CUtensorMap mA, mB;
@@ -1162,22 +1022,24 @@ int tc_gemm_tn(const bf16* A, int64_t lda, const bf16* B, int64_t ldb, float* C,
   p.ci_tiles = cdiv(N, NT);
   const int mt = cdiv(M, 128);
   const int tiles = mt * p.ci_tiles;
-  int splits = cdiv(148 * 2, tiles);
+  int splits = cdiv(LO_NUM_SMS * 2, tiles);
+  if (g_opt_det && splits > 8) splits = 8;
   if (splits > p.kstages) splits = p.kstages;
   if (splits < 1) splits = 1;
   p.per_split = cdiv(p.kstages, splits);
   splits = cdiv(p.kstages, p.per_split);
+  p.ordered = g_opt_det && splits > 1;
   dim3 grid(mt * p.ci_tiles, 1, splits);
   if (NT == 128) return launch_wgrad<128, 3>(mA, mB, p, grid, st);
   return launch_wgrad<64, 4>(mA, mB, p, grid, st);
 }
 
-// Batched C[b][M][N] (fp32, += with atomics) += A[b][K][M]^T * B[b][K][N]; A, B bf16 with arbitrary (16-byte multiple) strides:
+// Batched C[b][M][N] (fp32) += A[b][K][M]^T * B[b][K][N]; A, B bf16 with arbitrary (16-byte multiple) strides:
 // element (b, k, m) of A at A + b * sAb + k * sAk + m, likewise B.  One launch, grid.y = batch.  (decoder backward:
 // d enc[b] += alphas[b]^T dctx[:, b, :], the context read summed over time.)
 int tc_gemm_tn_batched(const bf16* A, int64_t sAk, int64_t sAb, const bf16* B, int64_t sBk, int64_t sBb, float* C, int64_t ldc,
                        int64_t sCb, int M, int N, int K, int batch, cudaStream_t st) {
-  if (!tc_available()) return fail(LO_ENOTSUP, "%s: needs an sm_100 device", __func__);
+  if (!tc_available()) return fail(LO_ENOTSUP, "%s: needs an sm_90 device", __func__);
   LO_CHECK_ARG(sAk % 8 == 0 && sAb % 8 == 0 && sBk % 8 == 0 && sBb % 8 == 0, "strides must be multiples of 8 elements");
   LO_CHECK_ARG(((uintptr_t)A & 15) == 0 && ((uintptr_t)B & 15) == 0 && batch >= 1 && batch <= 65535, "alignment / batch");
   CUtensorMap mA, mB;

@@ -325,14 +325,14 @@ static int tf_check(const lo_tfdec_args* a) {
 }
 
 // activations live in fp32 with a bf16 mirror (bf16 mode): C (+)= A W^T through the dispatcher (mma.sync kernel for M <= 64,
-// tcgen05 otherwise, CUDA cores when the shape does not qualify)
+// wgmma otherwise, CUDA cores when the shape does not qualify)
 static int tf_nt(const lo_tfdec_args* a, const float* A32, const bf16* Abf, int64_t lda, const void* W, int64_t ldw, float* C,
                  int64_t ldc, int M, int N, int K, const float* bias, int acc, cudaStream_t st) {
   if (a->dt == LO_BF16 && Abf && a->impl == LO_IMPL_TC)
     return gemm_nt(Abf, LO_BF16, lda, W, LO_BF16, ldw, C, LO_F32, ldc, M, N, K, bias, acc, 0, LO_IMPL_TC, st);
   return gemm_nt(A32, LO_F32, lda, W, a->dt, ldw, C, LO_F32, ldc, M, N, K, bias, acc, 0, LO_IMPL_SIMT, st);
 }
-// C[M][N] = A[K][M]^T B[K][N]   (hoisted weight gradients; tcgen05 when both operands have bf16 mirrors)
+// C[M][N] = A[K][M]^T B[K][N]   (hoisted weight gradients; wgmma when both operands have bf16 mirrors)
 static int tf_tn(const lo_tfdec_args* a, const float* A32, const bf16* Abf, int64_t lda, const float* B32, const bf16* Bbf,
                  int64_t ldb, float* C, int64_t ldc, int M, int N, int K, cudaStream_t st) {
   if (a->dt == LO_BF16 && a->impl == LO_IMPL_TC && Abf && Bbf && tc_available() && lda % 8 == 0 && ldb % 8 == 0 &&
@@ -513,7 +513,7 @@ int lo_tfdec_backward(const lo_tfdec_args* a, void* stream) {
   // LSTM kernel, [o ; h] rows: dz^T xh[0..T-1]
   LO_TRY(tf_tn(a, w.dz, w.dz_bf, d.G, w.xh, w.xh_bf, d.XH, a->g_w_lstm + d.E, d.LW, d.G, d.XH, TB, st));
   // embedding rows through the table: d ptab (scatter), then d emb = d ptab K[:E]^T..., d K[:E] = d ptab^T emb, d b = colsum
-  tf_dptab_scatter_kernel<<<148 * 8, 256, 0, st>>>(w.dz, a->formula, a->formula_stride, w.dptab, d.B, d.T, d.G, d.V);
+  tf_dptab_scatter_kernel<<<LO_NUM_SMS * 8, 256, 0, st>>>(w.dz, a->formula, a->formula_stride, w.dptab, d.B, d.T, d.G, d.V);
   LO_LAUNCH_OK();
   LO_TRY(gemm_nn(w.dptab, LO_F32, d.G, a->w_lstm, dt, d.LW, a->g_emb, LO_F32, d.E, d.V + 1, d.E, d.G, 0, LO_IMPL_SIMT, st));
   LO_TRY(gemm_tn(w.dptab, LO_F32, d.G, a->emb, dt, d.E, a->g_w_lstm, LO_F32, d.LW, d.G, d.E, d.V + 1, 0, LO_IMPL_SIMT, st));
@@ -530,7 +530,7 @@ int lo_tfdec_backward(const lo_tfdec_args* a, void* stream) {
   {
     dim3 grid(d.A / 64, cdiv(d.R, 32), d.B);
     LO_DISPATCH_DT(dt, T, (datt1_kernel<T, 0, 1><<<grid, 128, 0, st>>>((const T*)w.att_img, w.out2, d.N2, (int64_t)d.B * d.N2, w.de, a->beta,
-                                                                            (T*)w.datt_img, nullptr, d.T, d.R, d.A)));
+                                                                            (T*)w.datt_img, nullptr, d.T, d.R, d.A, 1, 0)));
     LO_LAUNCH_OK();
   }
   const int BR = d.B * d.R;
@@ -556,7 +556,7 @@ int lo_tfdec_backward(const lo_tfdec_args* a, void* stream) {
   LO_TRY(gemm_nn(w.dinit, LO_F32, IW, a->w_init, dt, d.C, w.dmean, LO_F32, d.C, d.B, d.C, IW, 0, LO_IMPL_SIMT, st));
   {
     const int64_t total = (int64_t)d.B * d.R * d.C;
-    add_rowbcast_kernel<<<148 * 8, 256, 0, st>>>(a->denc, w.dmean, d.R, d.C, 1.0f / (float)d.R, total);
+    add_rowbcast_kernel<<<LO_NUM_SMS * 8, 256, 0, st>>>(a->denc, w.dmean, d.R, d.C, 1.0f / (float)d.R, total);
     LO_LAUNCH_OK();
   }
   (void)es;

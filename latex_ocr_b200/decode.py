@@ -1,4 +1,4 @@
-"""Greedy / beam-search decoding on the B200 step kernels — the decode row of SURVEY.md §8 (a8).
+"""Greedy / beam-search decoding on the H100 step kernels — the decode row of SURVEY.md §8 (a8).
 
 Loop semantics follow the reference's TF decode loop, which is framework independent:
   dynamic_decode (model/components/dynamic_decode.py:38-61): run until every row is finished, at most

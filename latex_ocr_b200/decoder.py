@@ -1,5 +1,5 @@
 """Attention / DecoderWithAttention — drop-ins for model/components/seq2seq_torch.py:160-320 on the
-sm_100a kernels (lo_decoder.cu) through the C ABI.  Same constructors, forward signatures, return
+sm_90a kernels (lo_decoder.cu) through the C ABI.  Same constructors, forward signatures, return
 tuples and ``state_dict`` keys:
   attention.{encoder_att,decoder_att,full_att}.{weight,bias}, embedding.weight,
   decode_step.{weight_ih,weight_hh,bias_ih,bias_hh}, init_h.*, init_c.*, f_beta.*, fc.*

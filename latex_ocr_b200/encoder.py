@@ -1,5 +1,5 @@
 """EncoderCNN — drop-in for model/components/seq2seq_torch.py:24-157 ('vanilla' stack) running on
-hand-written sm_100a kernels through the C ABI.  Same constructor, ``forward(img[N,1,H,W]) ->
+hand-written sm_90a kernels through the C ABI.  Same constructor, ``forward(img[N,1,H,W]) ->
 [N,H',W',512]``, ``fine_tune`` and ``state_dict`` keys ``cnn.{0,3,6,8,11,14}.{weight,bias}``.
 
 Layout in HBM: feature maps NHWC, conv weights [Cout][3][3][Cin] (exposed to ``state_dict`` as OIHW

@@ -1,5 +1,5 @@
 """Img2SeqModel — the trainer surface of model/img2seq_torch.py:64-172 + model/base_torch.py:45-206
-(build_train / getLoss / _run_train_epoch / train) on the B200-native encoder and decoder.
+(build_train / getLoss / _run_train_epoch / train) on the H100-native encoder and decoder.
 
 ``getLoss`` keeps the reference semantics exactly (img2seq_torch.py:136-172): every row's caption
 length is the padded length (:144), targets are captions[:, 1:] (:147), loss = CE(mean over packed
@@ -31,7 +31,7 @@ class Img2SeqModel:
             raise _lib.LatexOcrB200Error("latex_ocr_b200 runs on CUDA devices only (device=%r)" % (dev,))
         self.device = torch.device(dev)
         self.precision = precision or getattr(config, "precision", "bf16")
-        # kernels: "tc" = tcgen05/TMA convolutions and GEMMs (bf16 storage only), "simt" = CUDA-core twins (fp32 tight-parity mode)
+        # kernels: "tc" = wgmma/TMA convolutions and GEMMs (bf16 storage only), "simt" = CUDA-core twins (fp32 tight-parity mode)
         self.impl = impl or getattr(config, "impl", "tc" if self.precision == "bf16" else "simt")
         self._n_tok = n_tok if n_tok is not None else (vocab.n_tok if vocab is not None else None)
         self.encoder = None

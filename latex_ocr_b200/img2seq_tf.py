@@ -1,4 +1,4 @@
-"""TensorFlow-flavour ``Img2SeqModel`` — the surface of model/img2seq.py on the sm_100a kernels: ``build_train`` /
+"""TensorFlow-flavour ``Img2SeqModel`` — the surface of model/img2seq.py on the sm_90a kernels: ``build_train`` /
 ``build_pred``, ``_run_train(config, train_set, val_set, epoch, lr_schedule)`` (:144-196), ``write_prediction`` /
 ``_run_evaluate`` semantics (:198-254, perplexity negated like :252), ``predict_batch(images)`` / ``predict(img)`` (:256-285).
 

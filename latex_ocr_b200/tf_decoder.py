@@ -1,6 +1,6 @@
 """TensorFlow-flavour decoder — drop-in for the path of model/decoder.py:15-72 (``Decoder(config, n_tok, id_end)``),
 model/components/attention_mechanism.py, attention_cell.py, greedy_decoder_cell.py and beam_search_decoder_cell.py on
-the sm_100a kernels (csrc/lo_tfdecoder.cuh) through the C ABI (``lo_tfdec_*``).
+the sm_90a kernels (csrc/lo_tfdecoder.cuh) through the C ABI (``lo_tfdec_*``).
 
 The reference builds a TF graph; here the same three things the graph offers are methods:
   * ``train_logits(enc, formula)``            -> pred_train  [N,T,V]                      (decoder.py:48-57)

@@ -131,6 +131,28 @@ def run_cnn_variant():
     print("cnn_variant", tuple(out.shape), "bytes", os.path.getsize(os.path.join(OUT, "cnn_variant.pt")))
 
 
+LIVE_CASE = dict(V=50, pseed=21, B=2, H=32, W=96, tmin=3, tmax=6, dseed=22, lengths=[[7], [4]])
+
+
+def run_live_case():
+    """The reference's eval-mode getLoss outputs and a ragged-length DecoderWithAttention.forward, stored in full
+    (tests/test_oracle_pinned.py::test_restatement_matches_live_reference)."""
+    c = LIVE_CASE
+    pe, pd = rm.init_params(c["V"], seed=c["pseed"])
+    enc, dec = ref_shim.build_reference_models(c["V"])
+    enc.load_state_dict(pe)
+    dec.load_state_dict(pd)
+    dec.eval()
+    img, formula = rm.synthetic_batch(c["B"], c["H"], c["W"], c["V"], c["tmin"], c["tmax"], seed=c["dseed"])
+    with torch.no_grad():
+        loss, scores, alphas = ref_shim.ref_get_loss(enc, dec, img, formula)
+        out = dec(enc(img), formula, torch.tensor(c["lengths"]))
+    rec = dict(case=c, torch=torch.__version__, loss=loss.item(), scores=scores.clone(), alphas=alphas.clone(),
+               ragged_predictions=out[0].clone(), ragged_decode_lengths=list(out[2]), ragged_alphas=out[3].clone())
+    torch.save(rec, os.path.join(OUT, "live_reference.pt"))
+    print("live_reference bytes", os.path.getsize(os.path.join(OUT, "live_reference.pt")))
+
+
 def main():
     if not ref_shim.reference_available():
         sys.exit("reference tree not available; golden files can only be regenerated in the build container")
@@ -143,6 +165,8 @@ def main():
         run_case(name, c)
     if not only or "cnn_variant" in only:
         run_cnn_variant()
+    if not only or "live_reference" in only:
+        run_live_case()
 
 
 if __name__ == "__main__":

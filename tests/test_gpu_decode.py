@@ -145,7 +145,7 @@ def test_train_epoch_and_evaluate_surface(tmp_path):
 
 
 def test_bf16_greedy_token_match_rate_at_cfg5_widths():
-    """BASELINE.json configs[4] shapes (height 64, widths 64..1024): greedy tokens of the bf16 / tcgen05 path against the fp32 CPU
+    """BASELINE.json configs[4] shapes (height 64, widths 64..1024): greedy tokens of the bf16 / wgmma path against the fp32 CPU
     oracle.  bf16 rounding can legitimately flip an argmax whose top-2 margin is at rounding level, so the comparison is made
     where it is well defined: teacher-forced on the oracle's own tokens, on the steps whose fp32 top-2 logit margin exceeds
     5e-2 (logits are O(1)).  Stated bar: >= 0.99 of those steps agree; the free-running exact-match rate is reported."""

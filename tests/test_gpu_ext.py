@@ -62,7 +62,7 @@ def test_lstm_seq_fp32_matches_torch(S, M, I, H, reverse):
 
 @pytest.mark.parametrize("S,M,I,H", [(6, 48, 128, 64), (7, 200, 512, 256)])
 def test_lstm_seq_bf16_tensor_core_path(S, M, I, H):
-    """bf16 storage + tcgen05 / mma.sync GEMMs (M <= 64 and M > 64 both), inputs pre-rounded so only the kernels' own
+    """bf16 storage + wgmma / mma.sync GEMMs (M <= 64 and M > 64 both), inputs pre-rounded so only the kernels' own
     rounding (bf16 mirrors of h and d pre-activations) shows: STATED tolerance 2e-2 of max-abs."""
     hs, out, dx, dxr, g, gr = _seq_case(torch.bfloat16, S, M, I, H, False, seed=S * 3 + M)
     assert relerr(hs, out) < 2e-2
@@ -123,7 +123,7 @@ def test_ext_train_step_fp32_vs_oracle_all_gradients():
 
 
 def test_ext_bf16_close_to_oracle_and_trains():
-    """bf16 / tcgen05 path of the extension: STATED tolerance loss 5e-3 relative; repeated steps on one batch reduce the loss;
+    """bf16 / wgmma path of the extension: STATED tolerance loss 5e-3 relative; repeated steps on one batch reduce the loss;
     the CUDA-graph step equals the eager one."""
     from oracle import ref_ext as rx
     from oracle import ref_model as rm

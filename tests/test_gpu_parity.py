@@ -216,7 +216,7 @@ def test_cfg2_shape_fp32_vs_golden():
 
 
 def test_cfg2_shape_bf16_tc_vs_golden():
-    """Same shapes on the bf16 / tcgen05 + mma.sync path the bench runs.  STATED bf16 tolerances (bf16 storage of feature maps,
+    """Same shapes on the bf16 / wgmma + mma.sync path the bench runs.  STATED bf16 tolerances (bf16 storage of feature maps,
     att1/enc and weight shadows, fp32 accumulation, 150 recurrent steps): loss 2e-3 relative; per-tensor relative gradient NORM
     error 3e-2 (measured on the golden's strided samples; small tensors in full)."""
     rec = load_golden("cfg2")
@@ -324,7 +324,7 @@ def test_uint8_image_upload_equals_float_path():
 def test_cnn_variant_encoder_vs_golden():
     """encoder_cnn='cnn' (seq2seq_torch.py:58-86: Conv2d(512,512,(2,4),stride 2,padding 1) instead of the two asymmetric pools):
     output and the gradients of sum(out * G) against the reference's own run (tests/golden/cnn_variant.pt); fp32 tight, and the
-    bf16/tcgen05 path (im2col + tensor-core GEMMs) against the fp32 one."""
+    bf16/wgmma path (im2col + tensor-core GEMMs) against the fp32 one."""
     from latex_ocr_b200.encoder import EncoderCNN
     from util import Cfg
     rm = _oracle()

@@ -63,7 +63,7 @@ def test_tf_decoder_fp32_matches_oracle(dropout):
 
 
 def test_tf_decoder_bf16_close_to_oracle():
-    """bf16 storage / fp32 accumulate, tcgen05 + mma.sync GEMMs, tanh.approx in the attention score: loss within 2e-2 relative,
+    """bf16 storage / fp32 accumulate, wgmma + mma.sync GEMMs, tanh.approx in the attention score: loss within 2e-2 relative,
     gradients within 6e-2 of their max."""
     tfm, p, dec, enc, formula = _setup(N=4, R=40, T=9, precision="bf16", impl="tc")
     lengths = torch.tensor([9, 9, 6, 2])

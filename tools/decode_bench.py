@@ -40,4 +40,4 @@ for mode, beam in (("greedy", 1), ("beam5", 5)):
             torch.cuda.synchronize(); dt = time.perf_counter() - t0
         toks += nt; secs += dt
     out[mode] = {"tokens_per_s": toks / secs, "images_per_s": 256 / secs, "seconds": secs}
-print(json.dumps({"workload": "cfg5: 256 images 64 x {64..1024}, 152 steps, bf16, 1 x B200", **out}))
+print(json.dumps({"workload": "cfg5: 256 images 64 x {64..1024}, 152 steps, bf16, 1 x H100", **out}))

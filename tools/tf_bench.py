@@ -1,5 +1,5 @@
 """Times the TensorFlow-flavour decoder (Genthial cell) forward + loss + backward at the cfg #2 shape (B=64, R=868, T=150,
-V=500, bf16) and its greedy / beam-2 decode on one B200.  Prints one JSON line."""
+V=500, bf16) and its greedy / beam-2 decode on one H100.  Prints one JSON line."""
 import json
 import os
 import sys

@@ -5,7 +5,8 @@
 //   forward : e_r = w . relu(att1_r + att2) ; online softmax ; ctx = sum_r alpha_r enc_r      (seq2seq_torch.py:186-190)
 //   backward: dalpha_r = <dctx, enc_r> + dreg_r ; de_r = alpha_r (dalpha_r - s) ; datt2 = w * sum_r de_r [att1_r + att2 > 0]
 // L2 policy: enc is read again by the next step (and by the backward) -> evict_last; att1 likewise is re-read every
-// step; which of the two to pin is a run-time option (lo_set_option) because together they are as large as the L2.
+// step; which of the two to pin is a run-time option (lo_set_option) because together they are larger than the L2.  The
+// tensor-core backward streams enc evict_first (attention_bwd_mma_kernel launch).
 #include <cooperative_groups.h>
 
 #include "lo_common.cuh"
@@ -879,7 +880,18 @@ __global__ void __launch_bounds__(AP_THREADS, LO_ATT_MINB) attention_bwd_mask_ke
 // [even(q) | even(q+4) | odd(q) | odd(q+4)] (q = lane % 4: fragment k index = region row).  Fragment row m = g + 8h of block j
 // stands for attention column 64w + 8g + 2j + h (g = lane / 4): any bijection works, this one makes a lane's 8 columns one byte.
 // ------------------------------------------------------------------------------------------------------------------------------
-constexpr int ABM_STAGES = 5;
+// Ring depth and CTAs per SM.  The grid stays one wave at 2 CTAs per SM (att_pipe_splits: 4 splits at B = 64, the same row
+// partition and so the same sums as before), but the ring is sized so that 3 CTAs fit per SM.  On the H100 a one-wave grid of
+// 4-CTA clusters with exactly 2 slots per SM did not become resident at once: about an eighth of the CTAs entered only when others
+// exited and the launch ended in a second wave of full-length CTAs.  The spare slot lets every cluster be placed at launch.
+// Backward time loop at B = 64 (H100 SXM, 400 W), us per step: 5 stages / 2 per SM 53.2, 4 / 3 48.0, 3 / 3 47.6.
+#ifndef LO_ABM_STAGES
+#define LO_ABM_STAGES 3
+#endif
+#ifndef LO_ABM_MINB
+#define LO_ABM_MINB 3
+#endif
+constexpr int ABM_STAGES = LO_ABM_STAGES;
 constexpr int ABM_ROWS = 16;
 constexpr int ABM_CH = 512;
 constexpr int ABM_PITCH = ABM_CH * 2 + 16;                    // bytes per ring row
@@ -911,7 +923,7 @@ __device__ __forceinline__ uint32_t pack_split(float x, float y, int sel) {
 }
 
 template <bool CL>
-__global__ void __launch_bounds__(AP_THREADS, 2) attention_bwd_mma_kernel(
+__global__ void __launch_bounds__(AP_THREADS, LO_ABM_MINB) attention_bwd_mma_kernel(
     const uint8_t* __restrict__ mask, const bf16* __restrict__ enc, const float* __restrict__ gate, int64_t o1_stride,
     const float* __restrict__ wf, const float* __restrict__ alpha, int64_t alpha_stride, const float* __restrict__ ctx,
     const float* __restrict__ dgctx, int64_t dg_stride, const float* __restrict__ dreg, int64_t dreg_stride,
@@ -1125,18 +1137,29 @@ __global__ void __launch_bounds__(AP_THREADS, 2) attention_bwd_mma_kernel(
   __syncthreads();
   if constexpr (CL) {
     cg::cluster_group cluster = cg::this_cluster();
+    // the running d w_full sum of this thread's column (last written by an earlier step): its load overlaps the cluster barrier
+    const float dwf_pf = dwf_part && (int)threadIdx.x < cps_pf && c_pf < CH ? dwf_part[(int64_t)b * CH + c_pf] : 0.f;
     cluster.sync();
     const int cps = (CH + nsplit - 1) / nsplit;
+    // gather the peers' sums first (into the ring behind s_part, which no peer reads), arrive, then the global read-modify-writes
+    // overlap the barrier
+    float* s_sum = s_part + CH;
     for (int c = sp * cps + threadIdx.x; c < min(CH, (sp + 1) * cps); c += AP_THREADS) {
       float t = 0.f;
       for (int qq = 0; qq < nsplit; qq++) t += cluster.map_shared_rank(s_part, qq)[c];      // fixed order -> deterministic
+      s_sum[c - sp * cps] = t;
+    }
+    cl_arrive_release();
+    for (int c = sp * cps + threadIdx.x; c < min(CH, (sp + 1) * cps); c += AP_THREADS) {
+      const float t = s_sum[c - sp * cps];
       const bool pf = c == c_pf;
       const float wfc = pf ? wf_pf : wf[c];
-      if (dwf_part) dwf_part[(int64_t)b * CH + c] += t * (pf ? a2_pf : att2[(int64_t)b * o1_stride + c]);      // att2 term of d w_full (one owner per (b, c))
+      if (dwf_part)      // att2 term of d w_full (one owner per (b, c))
+        dwf_part[(int64_t)b * CH + c] = (pf ? dwf_pf : dwf_part[(int64_t)b * CH + c]) + t * (pf ? a2_pf : att2[(int64_t)b * o1_stride + c]);
       datt2[(int64_t)b * dcat_stride + c] = t * wfc;
       if (datt2_bf) datt2_bf[(int64_t)b * dcat_stride + c] = __float2bfloat16_rn(t * wfc);
     }
-    cluster.sync();
+    cl_wait_acquire();                                           // peers may still be reading this CTA's s_part
     ATT_TS(5, threadIdx.x == 0);
     return;
   }
@@ -1295,7 +1318,9 @@ static int bwd_launch_a(const AttBwdArgs& x, cudaStream_t st) {
 #define LO_BWDT_ARGS                                                                                                                  \
   x.mask_in, (const bf16*)x.enc, x.gate, x.o1_stride, x.wf, x.alpha, x.alpha_stride, x.ctx, x.dgctx, x.dg_stride, x.dreg,            \
       x.dreg_stride, x.sreg, x.sreg_stride, x.de, x.datt2, x.dgp, x.dcat_stride, x.datt2_bf, x.dgp_bf, x.dctx_out, x.R, ns,           \
-      (int*)x.work, (float*)((char*)x.work + 4096), g_opt_att_policy_enc, x.att2, x.dwf_part
+      (int*)x.work, (float*)((char*)x.work + 4096), 2, x.att2, x.dwf_part
+    // enc evict_first (policy 2) whatever att_policy_enc says: the 57 MB of enc do not fit the H100's 50 MB L2 and are read once per
+    // launch; measured faster than evict_last in the backward loop (47.0 vs 48.1 us per step; in the forward loop it was slower)
     const size_t smem_t = (size_t)ABM_SMEM + (size_t)att_rows_per_split(x.R, ns) * 8;      // + alpha / d reg of the CTA's rows
     if (use_cluster(ns, x.R)) {
       LO_CUDA(launch_att(attention_bwd_mma_kernel<true>, dim3(ns, x.B), smem_t, ns, st, att_pdl_ok(x.abi), LO_BWDT_ARGS));

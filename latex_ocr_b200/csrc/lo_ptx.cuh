@@ -92,6 +92,9 @@ __device__ __forceinline__ uint32_t cl_size() {
 __device__ __forceinline__ void cl_sync() {
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
+// the two halves of cl_sync(), for work in between that touches no peer's shared memory
+__device__ __forceinline__ void cl_arrive_release() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
+__device__ __forceinline__ void cl_wait_acquire() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
 // the float at the same shared-memory offset as `p` in CTA `rank` of the cluster
 __device__ __forceinline__ float cl_ld(const float* p, uint32_t rank) {
   uint32_t a;

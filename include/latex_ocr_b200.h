@@ -251,7 +251,9 @@ typedef struct lo_decoder_args {
   float* dlogits;          /* [B][T][ldl] */
   float* dhd;              /* [B][T][D] */
   float* dreg;             /* [B][R] gradient of the regulariser w.r.t. alpha (same for every t) */
-  const float* dalpha_ext; /* optional external d loss/d alphas [B][T][R] (generic autograd mode); overrides dreg */
+  const float* dalpha_ext; /* optional external d loss/d alphas [B][T][R] (generic mode, below); overrides dreg */
+  const float* dpred_ext;  /* generic mode: upstream gradient of predictions, fp32 rows (b, t) in sorted-row order */
+  int64_t dpred_stride;    /* elements between consecutive (b, t) rows of dpred_ext (>= V) */
   float* sreg;             /* [B][T] */
   float* dcat;             /* [T][B][A+C+4D]: datt2 | dgate_pre | dgates_pre */
   float* dxh;              /* [B][C+D] scratch: dgctx | dh_prev */
@@ -281,7 +283,18 @@ int64_t lo_decoder_bfwork_bytes(const lo_decoder_args* a);
 int64_t lo_sizeof_decoder_args(void);
 /* forward through all T steps + logits ; if with_loss, also CE + regulariser into loss[] */
 int lo_decoder_forward(const lo_decoder_args* a, int with_loss, void* stream);
-/* backward of loss[0]; fills every g_* and denc.  Requires lo_decoder_forward(with_loss=1) state. */
+/* backward of loss[0]; fills every g_* and denc.  Requires lo_decoder_forward(with_loss=1) state.
+ * Generic mode (dpred_ext != NULL): the backward of an arbitrary loss of predictions and alphas (the autograd path of
+ * DecoderWithAttention).  Contract:
+ *   - the forward ran with with_loss = 0 and the backward buffers (dlogits, dhd, dreg, ..., g_*) allocated;
+ *   - dpred_ext holds d loss / d predictions [B][T] rows of V (dpred_stride >= V apart) and dalpha_ext d loss / d alphas
+ *     [B][T][R] (NULL: zero).  The first launch copies dpred_ext into dlogits (and its bf16 mirror when the wgmma fc backward
+ *     runs), writing zeros for rows t >= the row's decode length and for the padding columns [V, ldl): the forward zeroes those
+ *     predictions, so their gradient reaches neither g_w_fc, g_b_fc nor dhd;
+ *   - dreg and loss are not touched;
+ *   - the attention backward reads its d alpha rows before it waits on the preceding launch (programmatic dependent launch):
+ *     dalpha_ext must be complete before the call, which stream order gives for anything enqueued before it.
+ * Without dpred_ext, dalpha_ext only replaces the regulariser's d alpha of a with_loss = 1 forward (dlogits from its loss). */
 int lo_decoder_backward(const lo_decoder_args* a, void* stream);
 int lo_decoder_pack_bwd_weights(const lo_decoder_args* a, void* stream);
 

@@ -553,6 +553,19 @@ __global__ void ce_kernel(const float* __restrict__ logits, const int64_t* __res
     }
 }
 
+// generic backward: dlogits (+ bf16 mirror) = the caller's d predictions; rows with t >= dlen[b] and columns [V, ld) get zeros
+// (same rule as ce_kernel).  grid (ld / 128 blocks, B*T rows)
+__global__ void dpred_kernel(const float* __restrict__ dpred, int64_t dpred_stride, const int32_t* __restrict__ dlen,
+                             float* __restrict__ dlogits, bf16* __restrict__ dlogits_bf, int Tn, int V, int ld) {
+  const int row = blockIdx.y;
+  const int v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= ld) return;
+  const int b = row / Tn, t = row % Tn;
+  const float g = (v < V && t < dlen[b]) ? dpred[(int64_t)row * dpred_stride + v] : 0.f;
+  dlogits[(int64_t)row * ld + v] = g;
+  if (dlogits_bf) dlogits_bf[(int64_t)row * ld + v] = __float2bfloat16_rn(g);
+}
+
 // doubly-stochastic regulariser: S = sum_t alpha ; sq -> row_loss tail ; dreg = -2 alpha_c (1-S)/(B R)
 __global__ void reg_kernel(const float* __restrict__ alphas, float* __restrict__ sq, float* __restrict__ dreg, int B, int Tn,
                            int R, float alpha_c) {
@@ -1363,27 +1376,41 @@ int lo_decoder_pack_bwd_weights(const lo_decoder_args* a, void* stream) {
 
 int lo_decoder_backward(const lo_decoder_args* a, void* stream) {
   LO_TRY(check_args(a));
+  LO_CHECK_ARG(!a->dpred_ext || a->dlogits, "dpred_ext needs dlogits");
+  LO_CHECK_ARG(!a->dpred_ext || a->dpred_stride >= a->V, "dpred_stride >= V");
   cudaStream_t st = (cudaStream_t)stream;
   const Dims d = dims(a);
   const int dt = a->dt;
   const bool ragged = a->bt_host[d.T - 1] < d.B;
   const int ns = att_splits(d.B);
   const int64_t BT = (int64_t)d.B * d.T;
-  const float* dal = a->dalpha_ext ? a->dalpha_ext : a->dreg;
-  const int64_t dal_b = a->dalpha_ext ? (int64_t)d.T * d.R : d.R, dal_t = a->dalpha_ext ? d.R : 0;
+  // d alpha rows: the regulariser's (one row per b), the caller's (one per (b, t)), or none (generic mode without dalpha_ext)
+  const bool generic = a->dpred_ext != nullptr;
+  const float* dal = a->dalpha_ext ? a->dalpha_ext : (generic ? nullptr : a->dreg);
+  const int64_t dal_b = a->dalpha_ext ? (int64_t)d.T * d.R : (dal ? d.R : 0), dal_t = a->dalpha_ext ? d.R : 0;
+  const BfViews bvf = bf_views(a, d);
+  const bool fc_tc = bvf.on && d.Vl % 64 == 0 && d.D % 64 == 0;
+  if (generic && a->phase != 1) {
+    // plain launch (no overlap with the preceding one); everything after it that reads dlogits waits for it
+    dpred_kernel<<<dim3(cdiv(d.Vl, 128), (unsigned)BT), 128, 0, st>>>(a->dpred_ext, a->dpred_stride, work_dlen(a), a->dlogits,
+                                                                      fc_tc ? bvf.dlogits : nullptr, d.T, d.V, d.Vl);
+    LO_LAUNCH_OK();
+  }
   if (a->phase != 2) {
     LO_TRY(lo_decoder_pack_bwd_weights(a, stream));
     // sreg[b,t] = sum_r alpha dreg
-    sreg_kernel<<<cdiv(BT, 8), 256, 0, st>>>(a->alphas, dal, dal_b, dal_t, a->sreg, d.B, d.T, d.R);
-    LO_LAUNCH_OK();
+    if (dal) {
+      sreg_kernel<<<cdiv(BT, 8), 256, 0, st>>>(a->alphas, dal, dal_b, dal_t, a->sreg, d.B, d.T, d.R);
+      LO_LAUNCH_OK();
+    } else {
+      LO_CUDA(cudaMemsetAsync(a->sreg, 0, (size_t)BT * 4, st));
+    }
   }
   // fc backward (hoisted): g_w_fc = dlogits^T hd ; g_b_fc ; dhd = dlogits @ W_fc (* dropout mask)
-  const BfViews bvf = bf_views(a, d);
-  const bool fc_tc = bvf.on && d.Vl % 64 == 0 && d.D % 64 == 0 && !a->dalpha_ext;
   if (a->phase == 1) {
     // extension: d hd was put there by the caller (backward of the layer between the cell and fc)
   } else if (fc_tc) {
-    // (dlogits bf16 mirror was written by ce_kernel; generic-autograd callers that fill dlogits themselves use the SIMT path)
+    // (the dlogits bf16 mirror was written by ce_kernel or, in the generic mode, by dpred_kernel)
     LO_CUDA(cudaMemsetAsync(a->g_w_fc, 0, (size_t)d.V * d.D * 4, st));
     LO_TRY(tc_gemm_tn(bvf.dlogits, d.Vl, bvf.hd, d.D, a->g_w_fc, d.D, d.V, d.D, (int)BT, st));
     transpose_kernel<bf16><<<dim3(cdiv(d.D, 32), cdiv(d.V, 32)), dim3(32, 8), 0, st>>>((const bf16*)a->w_fc, d.D, bvf.wfct, d.Vl, d.V, d.D);

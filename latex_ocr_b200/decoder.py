@@ -12,11 +12,30 @@ import torch.nn as nn
 
 from . import _lib
 from ._lib import check, ptr, stream_ptr
-from .params import FlatStore, LRUCache, ParamHolder
+from .params import FlatStore, LRUCache, ParamHolder, grad_view, unbind_grads
 
 
 def _dt(precision):
     return _lib.LO_F32 if precision == "fp32" else _lib.LO_BF16
+
+
+class _DecoderFunction(torch.autograd.Function):
+    """Autograd node of DecoderWithAttention.forward: inputs (module, side-output dict, encoder_out, captions, lengths,
+    *parameters), differentiable outputs (predictions, alphas)."""
+
+    @staticmethod
+    def forward(ctx, dec, rest, encoder_out, encoded_captions, caption_lengths, *params):
+        preds, caps, decode_lengths, alphas, sort_ind, saved = dec._forward_impl(encoder_out, encoded_captions, caption_lengths,
+                                                                                 need_grad=True)
+        rest["out"] = (caps, decode_lengths, sort_ind)
+        ctx.dec, ctx.saved = dec, saved
+        return preds, alphas
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, dpreds, dalphas):
+        dx, grads = ctx.dec._backward_impl(ctx.saved, dpreds, dalphas, ctx.needs_input_grad[5:])
+        return (None, None, dx if ctx.needs_input_grad[2] else None, None, None) + tuple(grads)
 
 
 def decoder_specs(A, E, D, V, C):
@@ -120,6 +139,7 @@ class DecoderWithAttention(nn.Module):
         self.reset_parameters()
         self._ws = LRUCache()     # bounded: see params.LRUCache
         self._shadow_fresh = False
+        self._shadow_version = -1
         # in-kernel dropout (has_dropout=2): device {seed, call counter}; the counter is advanced by lo_decoder_backward, so
         # CUDA-graph replays draw a fresh mask every step
         self.dropout_state = torch.tensor([int(torch.initial_seed()) & 0x7FFFFFFFFFFFFFFF, 0], dtype=torch.int64, device=device)
@@ -172,9 +192,13 @@ class DecoderWithAttention(nn.Module):
         self._shadow_fresh = False
 
     def sync_shadow(self):
-        if not self._shadow_fresh:
+        # in-place edits of the parameters (torch.optim steps, load_state_dict, p.copy_) move the version counter that the
+        # views share with store.master; the fused Adam writes the shadow itself and leaves the counter alone
+        v = self.store.master._version
+        if not self._shadow_fresh or v != self._shadow_version:
             self.store.sync_shadow()
             self._shadow_fresh = True
+            self._shadow_version = v
 
     # ---------------------------------------------------------------------------------------------
     def workspace(self, B, T, R, need_grad):
@@ -212,7 +236,9 @@ class DecoderWithAttention(nn.Module):
             t["work"] = z(int(_lib.lib().lo_decoder_workspace_bytes(B, max(A, C))), dtype=torch.uint8)
             t["dropout_mask"] = None             # [B,T,D] allocated on first use of an injected mask
             ws["bt"] = (ctypes.c_int32 * T)(*([B] * T))
+            ws["gen"] = 0
             self._ws[key] = ws
+        ws["gen"] += 1         # every caller overwrites the forward state: a pending autograd backward of it must refuse to run
         if need_grad and not ws["need_grad"]:
             t = ws["t"]
             t["wbwd1"] = z(C + D, G, dtype=self.tdtype)
@@ -373,28 +399,74 @@ class DecoderWithAttention(nn.Module):
 
     def forward(self, encoder_out, encoded_captions, caption_lengths):
         """Reference signature and return tuple (seq2seq_torch.py:267-320): (predictions[B,maxT,V],
-        sorted captions, decode_lengths(list), alphas[B,maxT,R], sort_ind).  Inference-style call (no
-        autograd graph); training goes through Img2SeqModel.getLoss which fuses loss and backward."""
+        sorted captions, decode_lengths(list), alphas[B,maxT,R], sort_ind).  With grad mode on and ``encoder_out`` or a
+        parameter requiring grad, an autograd graph is recorded: ``predictions`` and ``alphas`` are differentiable (any loss of
+        them), and their backward runs lo_decoder_backward in its generic mode.  The outputs are the same either way."""
         if not encoder_out.is_cuda:
             raise _lib.LatexOcrB200Error("DecoderWithAttention runs on CUDA tensors only (no CPU fallback)")
+        params = list(self.parameters())
+        if torch.is_grad_enabled() and (encoder_out.requires_grad or any(p.requires_grad for p in params)):
+            rest = {}
+            preds, alphas = _DecoderFunction.apply(self, rest, encoder_out, encoded_captions, caption_lengths, *params)
+            caps, decode_lengths, sort_ind = rest["out"]
+            return preds, caps, decode_lengths, alphas, sort_ind
         with torch.no_grad():
-            B = encoder_out.size(0)
-            C = encoder_out.size(-1)
-            enc = encoder_out.reshape(B, -1, C)
-            lens, sort_ind = caption_lengths.squeeze(1).sort(dim=0, descending=True)     # :286
-            sort_ind_dev = sort_ind.to(enc.device)
-            enc = enc[sort_ind_dev].contiguous().to(self.tdtype)
-            caps = encoded_captions.to(enc.device)[sort_ind_dev].contiguous()
-            decode_lengths = (lens - 1).tolist()                                           # :298
-            T = max(decode_lengths)
-            mask = self.make_dropout_mask(B, T)
-            ws = self.run_forward(enc, caps, decode_lengths, with_loss=False, need_grad=False, dropout_mask=mask)
-            if isinstance(mask, str):
-                self.dropout_state[1] += 1       # forward-only call: no lo_decoder_backward to advance the Philox call counter
-            preds = ws["t"]["logits"][:, :, :self.vocab_size].clone()
-            alphas = ws["t"]["alphas"].clone()
-            if min(decode_lengths) < T:      # rows that stopped decoding keep zeros (:301-302, :317-318)
-                act = torch.arange(T, device=enc.device)[None, :] < torch.tensor(decode_lengths, device=enc.device)[:, None]
-                preds = preds * act[:, :, None]
-                alphas = alphas * act[:, :, None]
-            return preds, caps, decode_lengths, alphas, sort_ind_dev
+            return self._forward_impl(encoder_out, encoded_captions, caption_lengths, need_grad=False)[:5]
+
+    def _forward_impl(self, encoder_out, encoded_captions, caption_lengths, need_grad):
+        """The forward outputs, plus (need_grad) what the backward of this call needs."""
+        B = encoder_out.size(0)
+        C = encoder_out.size(-1)
+        enc = encoder_out.reshape(B, -1, C)
+        lens, sort_ind = caption_lengths.squeeze(1).sort(dim=0, descending=True)     # :286
+        sort_ind_dev = sort_ind.to(enc.device)
+        enc = enc[sort_ind_dev].contiguous().to(self.tdtype)
+        caps = encoded_captions.to(enc.device)[sort_ind_dev].contiguous()
+        decode_lengths = (lens - 1).tolist()                                           # :298
+        T = max(decode_lengths)
+        mask = self.make_dropout_mask(B, T)
+        # the Philox {seed, call} this forward draws its dropout mask from; the backward regenerates the mask from this copy
+        dstate = self.dropout_state.clone() if need_grad and mask is not None else None
+        ws = self.run_forward(enc, caps, decode_lengths, with_loss=False, need_grad=need_grad, dropout_mask=mask)
+        if isinstance(mask, str):
+            self.dropout_state[1] += 1       # forward-only call: no lo_decoder_backward to advance the Philox call counter
+        preds = ws["t"]["logits"][:, :, :self.vocab_size].clone()
+        alphas = ws["t"]["alphas"].clone()
+        if min(decode_lengths) < T:      # rows that stopped decoding keep zeros (:301-302, :317-318)
+            act = torch.arange(T, device=enc.device)[None, :] < torch.tensor(decode_lengths, device=enc.device)[:, None]
+            preds = preds * act[:, :, None]
+            alphas = alphas * act[:, :, None]
+        saved = None
+        if need_grad:
+            saved = {"ws": ws, "gen": ws["gen"], "enc": enc, "sort_ind": sort_ind_dev, "shape": tuple(encoder_out.shape),
+                     "dtype": encoder_out.dtype, "has_do": 0 if mask is None else 2, "dstate": dstate}
+        return preds, caps, decode_lengths, alphas, sort_ind_dev, saved
+
+    def _backward_impl(self, saved, dpreds, dalphas, need_params):
+        """lo_decoder_backward in its generic mode: returns (d encoder_out in the caller's row order and shape, [gradient or
+        None per parameter])."""
+        ws = saved["ws"]
+        enc = saved["enc"]
+        B, R, _ = enc.shape
+        T = ws["t"]["hd"].shape[1]
+        if ws["gen"] != saved["gen"]:
+            raise _lib.LatexOcrB200Error(
+                "DecoderWithAttention backward: the saved forward state (B=%d, T=%d, R=%d) was overwritten by a later forward of "
+                "the same shape; run backward before the next forward of that shape" % (B, T, R))
+        V = self.vocab_size
+        dpred = dpreds.float().contiguous() if dpreds is not None else torch.zeros(B, T, V, device=enc.device)
+        dal = dalphas.float().contiguous() if dalphas is not None else None
+        unbind_grads(self, self.store)           # the kernels overwrite store.grad
+        a = self.fill_args(ws, enc, B, T, R, saved["has_do"], dalpha_ext=dal)
+        dstate = None
+        if saved["dstate"] is not None:
+            dstate = saved["dstate"].clone()     # lo_decoder_backward advances the counter it is given
+            a.dropout_state = dstate.data_ptr()
+        a.dpred_ext = dpred.data_ptr()
+        a.dpred_stride = V
+        check(_lib.lib().lo_decoder_backward(ctypes.byref(a), stream_ptr()))
+        denc = ws["t"]["denc"]
+        dx = torch.empty_like(denc).index_copy_(0, saved["sort_ind"], denc)
+        dx = dx.view(saved["shape"]).to(saved["dtype"])
+        grads = [grad_view(self.store, p).clone() if need else None for p, need in zip(self.parameters(), need_params)]
+        return dx, grads

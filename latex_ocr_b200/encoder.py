@@ -13,7 +13,7 @@ import torch.nn as nn
 
 from . import _lib
 from ._lib import check, ptr, stream_ptr
-from .params import FlatStore, LRUCache, ParamHolder
+from .params import FlatStore, LRUCache, ParamHolder, grad_view, unbind_grads
 
 # (sequential index, Cin, Cout, pad, pool after)    seq2seq_torch.py:35-56
 _LAYERS = (("0", 1, 64, 1, (2, 2)), ("3", 64, 128, 1, (2, 2)), ("6", 128, 256, 1, None),
@@ -82,6 +82,7 @@ class EncoderCNN(nn.Module):
         self.reset_parameters()
         self._ws = LRUCache()     # bounded: see params.LRUCache
         self._shadow_fresh = False
+        self._shadow_version = -1
 
     # nn.Conv2d default init (kaiming_uniform(a=sqrt(5)) == U(-1/sqrt(fan_in), 1/sqrt(fan_in)))
     def reset_parameters(self):
@@ -159,9 +160,12 @@ class EncoderCNN(nn.Module):
         return _lib.LO_IMPL_TC if (self.impl == "tc" and self.precision == "bf16") else _lib.LO_IMPL_SIMT
 
     def sync_shadow(self):
-        if not self._shadow_fresh:
+        # resync after in-place edits of the parameters (see DecoderWithAttention.sync_shadow)
+        v = self.store.master._version
+        if not self._shadow_fresh or v != self._shadow_version:
             self.store.sync_shadow()
             self._shadow_fresh = True
+            self._shadow_version = v
 
     def forward_raw(self, img, need_grad=False):
         """img: CUDA float32 or uint8 [N,1,H,W] (raw 0..255 like img2seq_torch.py:115-117; uint8 = 4x less H2D traffic).  Returns the
@@ -176,6 +180,7 @@ class EncoderCNN(nn.Module):
         img = img.contiguous()
         N, _, H, W = img.shape
         ws = self._workspace(N, H, W, need_grad)
+        ws["gen"] = ws.get("gen", 0) + 1      # this call overwrites the forward state: a pending autograd backward of it must refuse
         self.sync_shadow()
         st, dt, impl, S = stream_ptr(), _dt(self.precision), self._impl(), self.store
         A = ws["acts"]
@@ -225,13 +230,14 @@ class EncoderCNN(nn.Module):
         ob, nb, _ = self.store.offsets["cnn.%s.bias" % idx]
         return ow, ob + nb - ow
 
-    def backward_raw(self, img_shape, denc, on_layer_grad=None):
+    def backward_raw(self, img_shape, denc, on_layer_grad=None, ws=None):
         """denc: fp32 [N,H',W',512] gradient w.r.t. the encoder output.  Fills self.store.grad.  ``on_layer_grad(idx)`` is
         called right after the kernels that complete layer idx's weight/bias gradient have been enqueued (last conv first):
-        the data-parallel path fires that layer's gradient all-reduce there, overlapping the rest of the backward."""
+        the data-parallel path fires that layer's gradient all-reduce there, overlapping the rest of the backward.  ``ws``: the
+        workspace of the forward (default: the cached one of this image shape)."""
         L = _lib.lib()
         N, _, H, W = img_shape
-        ws = self._workspace(N, H, W, True)
+        ws = ws if ws is not None else self._workspace(N, H, W, True)
         st, dt, impl, S = stream_ptr(), _dt(self.precision), self._impl(), self.store
         A, G = ws["acts"], ws["grads"]
         for l in self.layers[1:]:
@@ -295,6 +301,38 @@ class EncoderCNN(nn.Module):
             on_layer_grad("0")
 
     def forward(self, img):
-        """Reference signature (seq2seq_torch.py:88-100): returns a new fp32 tensor [N,H',W',512]."""
+        """Reference signature (seq2seq_torch.py:88-100): returns a new fp32 tensor [N,H',W',512].  With grad mode on and a
+        parameter requiring grad, an autograd graph is recorded whose backward runs ``backward_raw``; the output is the same
+        either way.  There is no gradient for the image."""
+        if img.requires_grad and torch.is_grad_enabled():
+            raise NotImplementedError("EncoderCNN computes no gradient for the input image")
+        params = list(self.parameters())
+        if torch.is_grad_enabled() and any(p.requires_grad for p in params):
+            return _EncoderFunction.apply(self, img, *params)
         with torch.no_grad():
             return self.forward_raw(img, need_grad=False).float()
+
+
+class _EncoderFunction(torch.autograd.Function):
+    """Autograd node of EncoderCNN.forward: inputs (module, img, *parameters), output the encoder output."""
+
+    @staticmethod
+    def forward(ctx, enc, img, *params):
+        out = enc.forward_raw(img, need_grad=True)
+        N, _, H, W = img.shape
+        ctx.enc, ctx.ws, ctx.shape = enc, enc._ws.get((N, H, W)), tuple(img.shape)
+        ctx.gen = ctx.ws["gen"]
+        return out.to(torch.float32, copy=True)        # never the workspace buffer itself: each call's output has its own node
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, dout):
+        enc, S = ctx.enc, ctx.enc.store
+        if ctx.ws["gen"] != ctx.gen:
+            raise _lib.LatexOcrB200Error("EncoderCNN backward: the saved forward state (image batch %s) was overwritten by a later "
+                                         "forward of the same shape; run backward before the next forward of that shape"
+                                         % (ctx.shape,))
+        unbind_grads(enc, S)                      # the kernels overwrite store.grad
+        enc.backward_raw(ctx.shape, dout.float().contiguous(), ws=ctx.ws)
+        return (None, None) + tuple(grad_view(S, p).clone() if need else None
+                                    for p, need in zip(enc.parameters(), ctx.needs_input_grad[2:]))

@@ -18,7 +18,7 @@ from . import _lib
 from ._lib import check, ptr, stream_ptr
 from .decoder import DecoderWithAttention
 from .encoder import EncoderCNN
-from .params import LRUCache
+from .params import LRUCache, bind_grads
 
 
 class Img2SeqModel:
@@ -149,6 +149,9 @@ class Img2SeqModel:
         """img: float tensor [N,1,H,W] (CPU pinned or CUDA); formula: int64 [N,L] (CPU or CUDA).
         Returns the device loss vector [total, ce, reg, n_valid] (no host sync unless sync=True)."""
         N, L = formula.shape
+        # the step writes the flat gradient buffers; autograd use or zero_grad(set_to_none=True) may have re-pointed p.grad
+        for m_ in (self.encoder, self.decoder):
+            bind_grads(m_, m_.store)
         lengths = torch.full((N, 1), L, dtype=torch.long)                       # img2seq_torch.py:144
         lens, sort_ind = lengths.squeeze(1).sort(dim=0, descending=True)        # seq2seq_torch.py:286 (host, tiny)
         decode_lengths = (lens - 1).tolist()
@@ -193,6 +196,8 @@ class Img2SeqModel:
             for S, sn in zip(stores, snap):
                 for k, v in sn.items():
                     getattr(S, k).copy_(v)
+            for m_ in (self.encoder, self.decoder):
+                m_._shadow_version = m_.store.master._version    # the restore put the shadows back too: no resync in the capture
             graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(graph):
                 mask = self.decoder.make_dropout_mask(N, T)
@@ -306,8 +311,9 @@ class Img2SeqModel:
         """(sum of CE over the real tokens incl. END, number of such tokens) of one padded batch — ``ce_words`` / ``n_words`` of
         img2seq.py:72-75 on the torch-flavour decoder (inputs prefixed with START, targets = tokens then END)."""
         inp = torch.cat([torch.full((formula_t.shape[0], 1), start_id, dtype=torch.int64), formula_t], dim=1)
-        enc = self.encoder(img.to(self.device))
-        preds, caps, dl, _, _ = self.decoder(enc, inp.to(self.device), lens + 1)
+        with torch.no_grad():
+            enc = self.encoder(img.to(self.device))
+            preds, caps, dl, _, _ = self.decoder(enc, inp.to(self.device), lens + 1)
         tgt = caps[:, 1:]
         ce_sum, n_tok = 0.0, 0
         for b, n in enumerate(dl):

@@ -108,4 +108,29 @@ class ParamHolder(nn.Module):
         p = nn.Parameter(v, requires_grad=True)
         p.grad = gv
         p._lo_store_name = sname
+        p._lo_permute = permute
         self.register_parameter(pname, p)
+
+
+def grad_view(store, p):
+    """The slice of ``store.grad`` that holds parameter ``p``'s gradient, in ``p``'s shape."""
+    gv = store.view(store.grad, p._lo_store_name)
+    return gv.permute(*p._lo_permute) if p._lo_permute is not None else gv
+
+
+def bind_grads(module, store):
+    """Point every parameter's ``.grad`` at its slice of ``store.grad``, which the fused train step overwrites: after that step
+    ``p.grad`` reads its gradients.  A no-op when they already point there."""
+    base = store.grad.data_ptr()
+    for p in module.parameters():
+        if p.grad is None or p.grad.data_ptr() != base + 4 * store.offsets[p._lo_store_name][0]:
+            p.grad = grad_view(store, p)
+
+
+def unbind_grads(module, store):
+    """Give every ``.grad`` that aliases ``store.grad`` memory of its own (same values), so that kernels may overwrite
+    ``store.grad`` while autograd accumulates into ``p.grad``."""
+    sp = store.grad.untyped_storage().data_ptr()
+    for p in module.parameters():
+        if p.grad is not None and p.grad.untyped_storage().data_ptr() == sp:
+            p.grad = p.grad.clone()

@@ -371,13 +371,27 @@ typedef struct lo_tfdec_args {
   float* loss;             /* [4]: mean CE over valid tokens (x2), 0, n_words — ce_words (img2seq.py:74) = loss[0] * loss[3] */
   float* denc;             /* f32 [B][R][C] gradient w.r.t. the encoder output */
   void* ws;                /* lo_tfdec_workspace_bytes(args) bytes, zero-initialised once by the caller */
+  const float* dlogits_ext; /* generic backward (below): d loss / d logits, fp32 rows (b, t) batch-major, dlogits_stride apart */
+  int64_t dlogits_stride;  /* elements between consecutive (b, t) rows of dlogits_ext (>= V) */
+  const float* dalpha_ext; /* generic backward, optional: d loss / d alphas [B][T][R] (NULL: zero) */
 } lo_tfdec_args;
 
 int64_t lo_sizeof_tfdec_args(void);
 int64_t lo_tfdec_workspace_bytes(const lo_tfdec_args* a);
 /* all T steps + logits; with_loss: masked CE into loss[] (and d logits kept for the backward) */
 int lo_tfdec_forward(const lo_tfdec_args* a, int with_loss, void* stream);
-/* backward of loss[0]: fills every g_* and denc (requires lo_tfdec_forward(with_loss=1) state in ws) */
+/* backward of loss[0]: fills every g_* and denc (requires lo_tfdec_forward(with_loss=1) state in ws).
+ * Generic mode (dlogits_ext != NULL): the backward of an arbitrary loss of the train logits and the alphas (the autograd path of
+ * tf_decoder.Decoder).  Contract:
+ *   - the forward ran with with_loss = 0 or 1 on the same args (lengths, inv_n_words and the CE's d logits are not used);
+ *   - dlogits_ext holds d loss / d logits, batch-major [B][T] rows of V floats (dlogits_stride >= V apart); every one of the T
+ *     positions carries its gradient (the forward computes logits for all of them, no row is masked).  The first launch copies it
+ *     into the workspace's time-major d logits (and their bf16 mirror when the wgmma GEMMs read it), zeros in columns [V, ldl);
+ *   - dalpha_ext holds d loss / d alphas [B][T][R] (NULL: zero).  The attention backward reads its d alpha rows before it waits on
+ *     the preceding launch (programmatic dependent launch): dalpha_ext must be complete before the call, which stream order gives
+ *     for anything enqueued before it;
+ *   - loss is not touched.
+ * dalpha_ext without dlogits_ext and dlogits_stride < V are refused (LO_EINVAL) before any GPU work. */
 int lo_tfdec_backward(const lo_tfdec_args* a, void* stream);
 /* greedy decode (greedy_decoder_cell.py:38-66 + dynamic_decode.py:38-61): tokens [B][max_steps], fin_hist (optional)
  * [B][max_steps] finished flags after each step; max_steps <= T */

@@ -553,17 +553,21 @@ __global__ void ce_kernel(const float* __restrict__ logits, const int64_t* __res
     }
 }
 
-// generic backward: dlogits (+ bf16 mirror) = the caller's d predictions; rows with t >= dlen[b] and columns [V, ld) get zeros
-// (same rule as ce_kernel).  grid (ld / 128 blocks, B*T rows)
+// generic backward: dlogits (+ bf16 mirror) = the caller's d predictions, source rows (b, t) batch-major; rows with t >= dlen[b]
+// (dlen NULL: none) and columns [V, ld) get zeros (same rule as ce_kernel).  Destination row: the same (b * Tn + t), or with
+// tm_B > 0 the time-major t * tm_B + b (TF flavour).  grid (ld / 128 blocks, up to nrows rows; y strides over the rest)
 __global__ void dpred_kernel(const float* __restrict__ dpred, int64_t dpred_stride, const int32_t* __restrict__ dlen,
-                             float* __restrict__ dlogits, bf16* __restrict__ dlogits_bf, int Tn, int V, int ld) {
-  const int row = blockIdx.y;
+                             float* __restrict__ dlogits, bf16* __restrict__ dlogits_bf, int Tn, int V, int ld, int64_t nrows,
+                             int tm_B) {
   const int v = blockIdx.x * blockDim.x + threadIdx.x;
   if (v >= ld) return;
-  const int b = row / Tn, t = row % Tn;
-  const float g = (v < V && t < dlen[b]) ? dpred[(int64_t)row * dpred_stride + v] : 0.f;
-  dlogits[(int64_t)row * ld + v] = g;
-  if (dlogits_bf) dlogits_bf[(int64_t)row * ld + v] = __float2bfloat16_rn(g);
+  for (int64_t row = blockIdx.y; row < nrows; row += gridDim.y) {
+    const int b = (int)(row / Tn), t = (int)(row % Tn);
+    const float g = (v < V && (!dlen || t < dlen[b])) ? dpred[row * dpred_stride + v] : 0.f;
+    const int64_t drow = tm_B > 0 ? (int64_t)t * tm_B + b : row;
+    dlogits[drow * ld + v] = g;
+    if (dlogits_bf) dlogits_bf[drow * ld + v] = __float2bfloat16_rn(g);
+  }
 }
 
 // doubly-stochastic regulariser: S = sum_t alpha ; sq -> row_loss tail ; dreg = -2 alpha_c (1-S)/(B R)
@@ -1392,8 +1396,8 @@ int lo_decoder_backward(const lo_decoder_args* a, void* stream) {
   const bool fc_tc = bvf.on && d.Vl % 64 == 0 && d.D % 64 == 0;
   if (generic && a->phase != 1) {
     // plain launch (no overlap with the preceding one); everything after it that reads dlogits waits for it
-    dpred_kernel<<<dim3(cdiv(d.Vl, 128), (unsigned)BT), 128, 0, st>>>(a->dpred_ext, a->dpred_stride, work_dlen(a), a->dlogits,
-                                                                      fc_tc ? bvf.dlogits : nullptr, d.T, d.V, d.Vl);
+    dpred_kernel<<<dim3(cdiv(d.Vl, 128), (unsigned)(BT < 65535 ? BT : 65535)), 128, 0, st>>>(
+        a->dpred_ext, a->dpred_stride, work_dlen(a), a->dlogits, fc_tc ? bvf.dlogits : nullptr, d.T, d.V, d.Vl, BT, 0);
     LO_LAUNCH_OK();
   }
   if (a->phase != 2) {

@@ -237,7 +237,7 @@ struct TfWs {
   void *att_img, *datt_img;                       // dt [nimg*R][A]
   float *dbeta_acc, *ptab, *dptab;
   float *xh, *call, *gates, *ztmp, *out2, *ctx, *oc, *dologit, *dout2, *dhc, *dz, *dxh, *dc, *de, *dctx, *mean, *initpre, *sinit,
-      *dinit, *dmean, *dlogits, *row_loss, *gtmp, *hd;
+      *dinit, *dmean, *dlogits, *row_loss, *gtmp, *hd, *sreg;
   bf16 *xh_bf, *ctx_bf, *dout2_bf, *dz_bf, *dlogits_bf, *hd_bf;
   void *wb4, *wb5, *wb6, *wbY, *wimgT;            // dt: transposed weights for the backward GEMMs
   void* attwork;
@@ -303,6 +303,7 @@ static TfWs tf_carve(const lo_tfdec_args* a) {
   w.next_tok = (int64_t*)take((size_t)d.B * 8);
   w.finished = (int32_t*)take((size_t)d.B * 4);
   w.parent_rows = (int32_t*)take((size_t)d.B * 4);
+  w.sreg = (float*)take(TB * 4);                                      // generic backward: [B][T] sum_r alpha d alpha
   w.bytes = off;
   return w;
 }
@@ -448,6 +449,8 @@ int lo_tfdec_forward(const lo_tfdec_args* a, int with_loss, void* stream) {
 
 int lo_tfdec_backward(const lo_tfdec_args* a, void* stream) {
   LO_TRY(tf_check(a));
+  LO_CHECK_ARG(a->dlogits_ext || !a->dalpha_ext, "dalpha_ext needs dlogits_ext (generic mode)");
+  LO_CHECK_ARG(!a->dlogits_ext || a->dlogits_stride >= a->V, "dlogits_stride >= V");
   LO_CHECK_ARG(a->formula && a->denc, "formula / denc");
   LO_CHECK_ARG(a->g_w_img && a->g_w_cat2 && a->g_beta && a->g_w_lstm && a->g_b_lstm && a->g_w_oc && a->g_w_y && a->g_w_init &&
                    a->g_b_init && a->g_emb, "null gradient buffer");
@@ -458,6 +461,19 @@ int lo_tfdec_backward(const lo_tfdec_args* a, void* stream) {
   const size_t es = dt == LO_F32 ? 4 : 2;
   const int TB = d.T * d.B;
   const dim3 tb(32, 8);
+  // generic mode: d logits from the caller (batch-major -> the time-major workspace rows; every position carries gradient), and
+  // sreg[b,t] = sum_r alpha d alpha for the attention backward.  Plain launches: everything after them waits for them.
+  if (a->dlogits_ext) {
+    const bool bf_mirror = dt == LO_BF16 && a->impl == LO_IMPL_TC;            // the wgmma GEMMs read d logits in bf16 (tf_nt / tf_tn)
+    dpred_kernel<<<dim3(cdiv(d.Vl, 128), (unsigned)(TB < 65535 ? TB : 65535)), 128, 0, st>>>(
+        a->dlogits_ext, a->dlogits_stride, nullptr, w.dlogits, bf_mirror ? w.dlogits_bf : nullptr, d.T, d.V, d.Vl, (int64_t)TB, d.B);
+    LO_LAUNCH_OK();
+    if (a->dalpha_ext) {
+      sreg_kernel<<<cdiv(TB, 8), 256, 0, st>>>(a->alphas, a->dalpha_ext, (int64_t)d.T * d.R, d.R, w.sreg, d.B, d.T, d.R);
+      LO_LAUNCH_OK();
+    }
+  }
+  const float* dal = a->dalpha_ext;          // d alpha rows [B][T][R] (generic mode only, checked above) or none
   // transposed shadows for the backward GEMMs (dX = dY W needs W as [in][out] = the TF layout); out[n][k] = in[k][n]
   auto transpose = [&](const void* in, int64_t off_in, int64_t ld_in, void* out, int64_t off_out, int64_t ld_out, int K, int N) -> int {
     LO_DISPATCH_DT(dt, T, (transpose_kernel<T><<<dim3(cdiv(N, 32), cdiv(K, 32)), tb, 0, st>>>((const T*)in + off_in, ld_in, (T*)out + off_out,
@@ -489,7 +505,8 @@ int lo_tfdec_backward(const lo_tfdec_args* a, void* stream) {
     LO_TRY(tf_nt(a, dout2 + d.A, dout2b ? dout2b + d.A : nullptr, d.DW, w.wb4, d.O, w.dhc, d.D + d.C, d.B, d.D + d.C, d.O, nullptr, 0, st));
     {
       AttBwdArgs x{w.att_img, a->enc, w.out2 + rowt * d.N2, nullptr, d.N2, a->beta, a->alphas + (int64_t)t * d.R, (int64_t)d.T * d.R,
-                   w.ctx + rowt * d.C, w.dhc + d.D, d.D + d.C, nullptr, 0, nullptr, 0, w.de + (int64_t)t * d.R, dout2, nullptr, d.DW,
+                   w.ctx + rowt * d.C, w.dhc + d.D, d.D + d.C, dal ? dal + (int64_t)t * d.R : nullptr, dal ? (int64_t)d.T * d.R : 0,
+                   dal ? w.sreg + t : nullptr, dal ? d.T : 0, w.de + (int64_t)t * d.R, dout2, nullptr, d.DW,
                    dout2b, nullptr, w.dctx + rowt * d.C, d.B, d.R, w.attwork, w.dbeta_acc, 0, 1, d.A};
       LO_TRY(attention_bwd_pipe(x, dt, d.C, st));
     }

@@ -17,6 +17,7 @@ from . import _lib
 from ._lib import check, ptr, stream_ptr
 from .data import minibatches, pad_batch_formulas, pad_batch_images
 from .encoder import EncoderCNN
+from .params import bind_grads
 from .tf_decoder import Decoder
 
 
@@ -106,6 +107,9 @@ class Img2SeqModel:
         length_t = torch.as_tensor(np.asarray(length), dtype=torch.int32)
         img = self._to_device_images(images)
         N = img.shape[0]
+        # the step writes the flat gradient buffers; autograd use or zero_grad(set_to_none=True) may have re-pointed p.grad
+        for m_ in (self.encoder, self.decoder):
+            bind_grads(m_, m_.store)
         enc = self.encoder.forward_raw(img, need_grad=True)
         keep_h = keep_o = None
         if dropout is not None and float(dropout) < 1.0:
@@ -148,6 +152,7 @@ class Img2SeqModel:
             check(fn(kind, ptr(S.master), ptr(S.grad), ptr(S.m), ptr(S.v), ptr(S.shadow), S.numel, ptr(S.adam_state), b1, b2, eps,
                      float(scale), stream_ptr()))
             m._shadow_fresh = True                                          # the fused update refreshed the bf16 shadow
+            m._shadow_version = m.store.master._version                     # ... and left the version counter alone: no resync
 
     def train_step(self, images, formulas, dropout=1.0):
         """One update (img2seq.py:163-170).  Returns the device loss vector [mean CE, mean CE, 0, n_words]."""

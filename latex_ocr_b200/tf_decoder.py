@@ -4,6 +4,8 @@ the sm_90a kernels (csrc/lo_tfdecoder.cuh) through the C ABI (``lo_tfdec_*``).
 
 The reference builds a TF graph; here the same three things the graph offers are methods:
   * ``train_logits(enc, formula)``            -> pred_train  [N,T,V]                      (decoder.py:48-57)
+  * ``train_outputs(enc, formula)``           -> (pred_train, alphas [N,T,R]), differentiable: any loss of them trains
+                                                 through ``loss.backward()`` (lo_tfdec_backward in its generic mode)
   * ``loss_and_backward(enc, formula, len)``  -> masked CE of img2seq.py:68-71 + every gradient (+ d enc)
   * ``decode(enc)``                           -> DecoderOutput(logits=None, ids)          (decoder.py:59-70; greedy ids [N,time],
                                                  beam ids [N,time,beam] like the TF cell before img2seq.py:241 transposes them)
@@ -23,9 +25,27 @@ import torch.nn as nn
 
 from . import _lib
 from ._lib import check, stream_ptr
-from .params import FlatStore, LRUCache, ParamHolder
+from .params import FlatStore, LRUCache, ParamHolder, bind_grads, grad_view, unbind_grads
 
 DecoderOutput = collections.namedtuple("DecoderOutput", ("logits", "ids"))      # greedy_decoder_cell.py:5-6
+
+
+class _TfDecoderFunction(torch.autograd.Function):
+    """Autograd node of Decoder.train_outputs: inputs (module, enc, formula, keep_h, keep_o, *parameters), differentiable outputs
+    (logits, alphas)."""
+
+    @staticmethod
+    def forward(ctx, dec, enc, formula, keep_h, keep_o, *params):
+        logits, alphas, saved = dec._train_outputs_impl(enc, formula, keep_h, keep_o, need_grad=True)
+        ctx.dec, ctx.saved = dec, saved
+        ctx.set_materialize_grads(False)         # an output the loss does not use arrives as None: no d alpha pass for it
+        return logits, alphas
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, dlogits, dalphas):
+        dx, grads = ctx.dec._backward_impl(ctx.saved, dlogits, dalphas, ctx.needs_input_grad[5:])
+        return (None, dx if ctx.needs_input_grad[1] else None, None, None, None) + tuple(grads)
 
 
 def _make_args_struct():
@@ -121,6 +141,7 @@ class Decoder(nn.Module):
         self.reset_parameters()
         self._ws = LRUCache()     # bounded: see params.LRUCache
         self._shadow_fresh = False
+        self._shadow_version = -1
 
     # tf.get_variable / tf.layers.dense default: glorot_uniform; LSTMCell bias zeros; embeddings decoder.py:98-105
     def reset_parameters(self):
@@ -154,14 +175,20 @@ class Decoder(nn.Module):
         self._shadow_fresh = False
 
     def sync_shadow(self):
-        if not self._shadow_fresh:
+        # in-place edits of the parameters (torch.optim steps, load_state_dict, p.copy_) move the version counter that the views
+        # share with store.master; the fused optimizer step writes the shadow itself and records the version
+        v = self.store.master._version
+        if not self._shadow_fresh or v != self._shadow_version:
             self.store.sync_shadow()
             self._shadow_fresh = True
+            self._shadow_version = v
 
     # ---------------------------------------------------------------------------------------------
-    def _args(self, enc, B, T, R, rows_per_img=1):
+    def _args(self, enc, B, T, R, rows_per_img=1, decode=False):
+        """Args and workspace of one shape.  Decoding has workspaces of its own, so a decode never overwrites the saved state of
+        a teacher-forced pass whose autograd backward is still to run (Decoder.forward runs both)."""
         L = _bind()
-        key = (B, T, R, rows_per_img)
+        key = (B, T, R, rows_per_img, "decode") if decode else (B, T, R, rows_per_img)
         ws = self._ws.get(key)
         dev = self.store.device
         if ws is None:
@@ -172,7 +199,9 @@ class Decoder(nn.Module):
             ws["denc"] = torch.zeros(B // rows_per_img, R, self.C, dtype=torch.float32, device=dev)
             ws["formula"] = torch.zeros(B, T, dtype=torch.int64, device=dev)
             ws["lengths"] = torch.zeros(B, dtype=torch.int32, device=dev)
+            ws["gen"] = 0
             self._ws[key] = ws
+        ws["gen"] += 1         # every caller overwrites the forward state: a pending autograd backward of it must refuse to run
         S = self.store
         a = TfDecArgs()
         a.B, a.T, a.R, a.C, a.A, a.D, a.O, a.E, a.V = B, T, R, self.C, self.A, self.D, self.O, self.E, self.V
@@ -243,9 +272,56 @@ class Decoder(nn.Module):
             ws = self.run_forward(enc, formula, None, keep_h, keep_o)
             return ws["logits"][:, :, :self.V].permute(1, 0, 2).contiguous()
 
+    def train_outputs(self, enc, formula, keep_h=None, keep_o=None):
+        """Teacher-forced pass: (logits [N,T,V], alphas [N,T,R]).  With grad mode on and ``enc`` or a parameter requiring grad, an
+        autograd graph is recorded: both outputs are differentiable (any loss of them), d enc comes back in ``enc``'s shape and
+        dtype, and the backward runs lo_tfdec_backward in its generic mode with the same keep masks.  The outputs are the same
+        either way."""
+        params = list(self.parameters())
+        if torch.is_grad_enabled() and (enc.requires_grad or any(p.requires_grad for p in params)):
+            return _TfDecoderFunction.apply(self, enc, formula, keep_h, keep_o, *params)
+        with torch.no_grad():
+            return self._train_outputs_impl(enc, formula, keep_h, keep_o, need_grad=False)[:2]
+
+    def _train_outputs_impl(self, enc, formula, keep_h, keep_o, need_grad):
+        """The outputs of train_outputs, plus (need_grad) what the backward of this call needs."""
+        ws = self.run_forward(enc, formula, None, keep_h, keep_o)
+        logits = ws["logits"][:, :, :self.V].permute(1, 0, 2).contiguous()
+        alphas = ws["alphas"].clone()
+        saved = None
+        if need_grad:
+            # ws["args"] points at ws["enc"] and the keep masks of this call; holding them keeps them alive even if the workspace
+            # leaves the cache
+            saved = {"ws": ws, "gen": ws["gen"], "args": ws["args"], "enc": ws["enc"],
+                     "keep": (ws["keep_h"] if keep_h is not None else None, ws["keep_o"] if keep_o is not None else None),
+                     "shape": tuple(enc.shape), "dtype": enc.dtype}
+        return logits, alphas, saved
+
+    def _backward_impl(self, saved, dlogits, dalphas, need_params):
+        """lo_tfdec_backward in its generic mode: returns (d enc in the caller's shape and dtype, [gradient or None per
+        parameter])."""
+        ws = saved["ws"]
+        B, T, R = ws["alphas"].shape
+        if ws["gen"] != saved["gen"]:
+            raise _lib.LatexOcrB200Error(
+                "Decoder backward: the saved forward state (N=%d, T=%d, R=%d) was overwritten by a later call of the same shape; "
+                "run backward before the next forward of that shape" % (B, T, R))
+        dev = self.store.device
+        dl = dlogits.float().contiguous() if dlogits is not None else torch.zeros(B, T, self.V, device=dev)
+        dal = dalphas.float().contiguous() if dalphas is not None else None
+        unbind_grads(self, self.store)           # the kernels overwrite store.grad
+        a = TfDecArgs.from_buffer_copy(saved["args"])
+        a.dlogits_ext, a.dlogits_stride = dl.data_ptr(), self.V
+        a.dalpha_ext = dal.data_ptr() if dal is not None else None
+        check(_bind().lo_tfdec_backward(ctypes.byref(a), stream_ptr()))
+        dx = ws["denc"].reshape(saved["shape"]).to(saved["dtype"], copy=True)
+        grads = [grad_view(self.store, p).clone() if need else None for p, need in zip(self.parameters(), need_params)]
+        return dx, grads
+
     def loss_and_backward(self, enc, formula, lengths, keep_h=None, keep_o=None, n_words=None):
         """Returns (loss tensor [4] on the device: mean CE, mean CE, 0, n_words; d loss / d enc [N,R,C] fp32).  Parameter
         gradients land in ``self.store.grad`` (the ``.grad`` of every parameter)."""
+        bind_grads(self, self.store)             # autograd use or zero_grad(set_to_none=True) may have re-pointed p.grad
         with torch.no_grad():
             ws = self.run_forward(enc, formula, lengths, keep_h, keep_o, n_words)
             denc = self.run_backward(ws)
@@ -263,7 +339,7 @@ class Decoder(nn.Module):
         B = N * beam
         self.sync_shadow()
         with torch.no_grad():
-            L, ws, a = self._args(enc, B, steps, R, rows_per_img=beam)
+            L, ws, a = self._args(enc, B, steps, R, rows_per_img=beam, decode=True)
             ws["enc"] = enc
             dev = self.store.device
             if self.decoding == "greedy":
@@ -299,7 +375,8 @@ class Decoder(nn.Module):
 
     def forward(self, img, formula=None, dropout=1.0):
         """Decoder.__call__(img, formula, dropout) (decoder.py:24): (pred_train, pred_test).  dropout is the TF keep_prob; the
-        shipped training config uses 1 (training.json:7) — other values draw masks here."""
+        shipped training config uses 1 (training.json:7) — other values draw masks here.  pred_train comes from train_outputs, so
+        it is differentiable under the same rule (its backward reuses the masks drawn here)."""
         keep_h = keep_o = None
         train = None
         if formula is not None:
@@ -309,5 +386,5 @@ class Decoder(nn.Module):
                 dev = self.store.device
                 keep_h = (torch.rand(N, T, self.D, device=dev) < kp).float() / kp
                 keep_o = (torch.rand(N, T, self.O, device=dev) < kp).float() / kp
-            train = self.train_logits(img, formula, keep_h, keep_o)
+            train = self.train_outputs(img, formula, keep_h, keep_o)[0]
         return train, self.decode(img)

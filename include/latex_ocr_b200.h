@@ -206,7 +206,13 @@ typedef struct lo_decoder_args {
   int32_t rows_per_img;    /* decode only: consecutive rows that share one image (beam size); 0/1 for training */
   int32_t phase;           /* 0: whole call (default).  EXTENSION (a second decoder layer between the cell and fc): 1 = time loop
                               only — lo_decoder_forward stops after writing hd, lo_decoder_backward starts from the dhd the caller
-                              put there; 2 = head only — logits + loss from whatever the caller left in hd, backward of fc -> dhd */
+                              put there; 2 = head only — logits + loss from whatever the caller left in hd, backward of fc -> dhd.
+                              A split backward runs phase 2, then the caller's layer (dhd in place), then phase 1; phase 1
+                              bumps the dropout call counter, phase 2 does not.  Generic mode across phases: dpred_ext is the
+                              mode flag and must be set in BOTH calls — phase 2 reads it (dpred_kernel -> dlogits, fc backward
+                              -> dhd, g_w_fc, g_b_fc), phase 1 does not read it but takes d alpha from dalpha_ext (NULL: zero)
+                              instead of the regulariser's dreg, which a with_loss = 0 forward never wrote.  dalpha_ext in a
+                              phase-2 call and a phase outside 0..2 are refused (LO_EINVAL) before any GPU work. */
   const int32_t* bt_host;  /* HOST int[T]: rows active at step t (seq2seq_torch.py:308); non-increasing */
   const int64_t* caps;     /* [B][caps_stride] token ids (sorted rows) */
   int64_t caps_stride;
@@ -252,7 +258,8 @@ typedef struct lo_decoder_args {
   float* dhd;              /* [B][T][D] */
   float* dreg;             /* [B][R] gradient of the regulariser w.r.t. alpha (same for every t) */
   const float* dalpha_ext; /* optional external d loss/d alphas [B][T][R] (generic mode, below); overrides dreg */
-  const float* dpred_ext;  /* generic mode: upstream gradient of predictions, fp32 rows (b, t) in sorted-row order */
+  const float* dpred_ext;  /* generic mode: upstream gradient of predictions, fp32 rows (b, t) in sorted-row order.  Non-NULL
+                              selects the generic mode, also in a phase-1 call, which does not read it (see phase) */
   int64_t dpred_stride;    /* elements between consecutive (b, t) rows of dpred_ext (>= V) */
   float* sreg;             /* [B][T] */
   float* dcat;             /* [T][B][A+C+4D]: datt2 | dgate_pre | dgates_pre */

@@ -927,6 +927,7 @@ static int check_args(const lo_decoder_args* a) {
   LO_CHECK_ARG(a->dt == LO_F32 || a->dt == LO_BF16, "dt");
   LO_CHECK_ARG(a->ldl == 0 || a->ldl >= a->V, "ldl >= V");
   LO_CHECK_ARG(a->rows_per_img <= 1 || a->B % a->rows_per_img == 0, "B must be a multiple of rows_per_img");
+  LO_CHECK_ARG(a->phase >= 0 && a->phase <= 2, "phase in 0..2");
   LO_CHECK_ARG(a->bt_host && a->caps && a->enc && a->work, "null pointer");
   LO_CHECK_ARG(a->has_dropout != 2 || (a->dropout_state && a->dropout_p >= 0.f && a->dropout_p < 1.f &&
                                        (!g_opt_fuse_lstm || g_opt_skinny_mma)),
@@ -1382,6 +1383,7 @@ int lo_decoder_backward(const lo_decoder_args* a, void* stream) {
   LO_TRY(check_args(a));
   LO_CHECK_ARG(!a->dpred_ext || a->dlogits, "dpred_ext needs dlogits");
   LO_CHECK_ARG(!a->dpred_ext || a->dpred_stride >= a->V, "dpred_stride >= V");
+  LO_CHECK_ARG(a->phase != 2 || !a->dalpha_ext, "phase 2 reads no d alpha: pass dalpha_ext to the phase-1 call");
   cudaStream_t st = (cudaStream_t)stream;
   const Dims d = dims(a);
   const int dt = a->dt;

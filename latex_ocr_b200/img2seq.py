@@ -141,16 +141,20 @@ class Img2SeqModel:
         """Everything a captured graph replays on (the bounded workspace caches may evict their entries later)."""
         return [list(self.decoder._ws.values()), list(self.encoder._ws.values())]
 
+    def _param_modules(self):
+        """Every module with a flat parameter store that the step updates."""
+        return tuple(getattr(self, n) for n in ("encoder", "decoder", "row_encoder", "layer2") if getattr(self, n, None) is not None)
+
     def _stores(self):
         """Every flat parameter store the step updates (snapshotted around the pre-capture warm-up steps)."""
-        return tuple(getattr(self, n).store for n in ("encoder", "decoder", "row_encoder", "layer2") if getattr(self, n, None) is not None)
+        return tuple(m_.store for m_ in self._param_modules())
 
     def train_step(self, img, formula, sync=False):
         """img: float tensor [N,1,H,W] (CPU pinned or CUDA); formula: int64 [N,L] (CPU or CUDA).
         Returns the device loss vector [total, ce, reg, n_valid] (no host sync unless sync=True)."""
         N, L = formula.shape
         # the step writes the flat gradient buffers; autograd use or zero_grad(set_to_none=True) may have re-pointed p.grad
-        for m_ in (self.encoder, self.decoder):
+        for m_ in self._param_modules():
             bind_grads(m_, m_.store)
         lengths = torch.full((N, 1), L, dtype=torch.long)                       # img2seq_torch.py:144
         lens, sort_ind = lengths.squeeze(1).sort(dim=0, descending=True)        # seq2seq_torch.py:286 (host, tiny)
@@ -196,7 +200,7 @@ class Img2SeqModel:
             for S, sn in zip(stores, snap):
                 for k, v in sn.items():
                     getattr(S, k).copy_(v)
-            for m_ in (self.encoder, self.decoder):
+            for m_ in self._param_modules():
                 m_._shadow_version = m_.store.master._version    # the restore put the shadows back too: no resync in the capture
             graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(graph):

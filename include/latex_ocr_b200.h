@@ -119,6 +119,15 @@ int lo_conv1_pool_forward_code(const void* img, int img_is_u8, float scale, floa
                                void* out, uint8_t* code, int dt, int N, int H, int W, void* stream);
 int lo_conv1_pool_wgrad_code(const void* img, int img_is_u8, float scale, float offset, const uint8_t* code, const void* dpool,
                              int dt, float* dw, float* db, int N, int H, int W, void* stream);
+/* conv1 data gradient (d image) through the ReLU and the 2x2 max-pool, from those codes and dpool [N][H/2][W/2][64] (dt):
+ * dpre[n,oy,ox,c] = dpool[n,oy/2,ox/2,c] where the code has its ReLU bit set and window index (oy&1)*2+(ox&1), else 0 (an odd
+ * H / W's last conv row / column, which the pool drops, gets none); dimg[n,y,x] = scale * sum_{r,q<3} sum_c w[c][r][q] *
+ * dpre[n,y+1-r,x+1-q,c] over in-bounds conv positions.  w: the fp32 conv1 weights [64][9]; scale: the pixel scale of the
+ * forward (1, or 1/128 for the TF flavour; the offset does not enter).  dimg fp32 [N][H][W] is written, not accumulated.  Each
+ * pixel is summed by one thread in a fixed order (no atomics), so the result is bit-reproducible without "deterministic".
+ * Null pointers, dt other than LO_F32 / LO_BF16, N < 1, H < 2 or W < 2 are refused before any GPU work. */
+int lo_conv1_pool_dgrad_code(const uint8_t* code, const void* dpool, int dt, const float* w, float scale, float* dimg,
+                             int N, int H, int W, void* stream);
 /* General strided convolution = im2col + lo_gemm: the 'cnn' encoder variant's Conv2d(512,512,(2,4),stride=2,padding=1)
  * (seq2seq_torch.py:80).  col [N*Ho*Wo][R*S*C], taps-major, C % 8 == 0; forward y = relu(col W^T + b) with W [Cout][R][S][C];
  * weight gradient dW = dy^T col; data gradient dcol = dy W then lo_col2im (a gather over the windows covering each input

@@ -108,6 +108,15 @@ __global__ void conv1_wgrad_reduce_kernel(float* __restrict__ dw, float* __restr
   else dw[c * 9 + k] = s;
 }
 
+// Decodes one arg-max / ReLU code byte of conv1_pool_fwd_kernel: returns the gradient of the winning conv position (g, or 0 when
+// the ReLU bit is clear: relu'(0) = 0) and its window position (py, px).  The weight and the data gradient both decode through
+// this, so they agree on the arg-max and on relu'(0).
+__device__ __forceinline__ float conv1_code_decode(uint32_t cd, float g, bool& py, bool& px) {
+  px = cd & 1u;
+  py = cd & 2u;
+  return (cd & 4u) ? g : 0.f;
+}
+
 // conv1 weight gradient from the arg-max / ReLU codes the forward kernel saved: no recomputation of conv1 (36 of the 84 FMA slots
 // per pooled output and channel), the 3x3 window of the winning position is selected with 21 selects instead of 27 masked FMAs.
 // warp <-> 8 channels, lane <-> pooled position (as conv1_pool_wgrad_kernel below).
@@ -152,8 +161,8 @@ __global__ void __launch_bounds__(256) conv1_pool_wgrad_code_kernel(const TI* __
 #pragma unroll
     for (int c = 0; c < 8; c++) {
       const uint32_t cd = (cw[c >> 2] >> (8 * (c & 3))) & 0xffu;
-      const float gg = (cd & 4u) ? g[c] : 0.f;
-      const bool px = cd & 1u, py = cd & 2u;
+      bool py, px;
+      const float gg = conv1_code_decode(cd, g[c], py, px);
       gb[c] += gg;
       float xc[4][3];
 #pragma unroll
@@ -167,6 +176,92 @@ __global__ void __launch_bounds__(256) conv1_pool_wgrad_code_kernel(const TI* __
     }
   }
   conv1_wgrad_block_partial(gw, gb, cg, lane, dw, db, ordered);
+}
+
+// conv1 data gradient through its ReLU and 2x2 max-pool, from the same codes:
+//   dimg[n,y,x] = scale * sum_{r,q} sum_c w[c][r][q] * dpre[n, y+1-r, x+1-q, c]
+// with dpre = dpool at the winning conv position of each pooled output (0 elsewhere, and 0 where the ReLU bit is clear).
+// A block owns C1D_TH x C1D_TW pooled positions of one image and computes them plus a ring of one position (C1D_EH x C1D_EW,
+// two per thread; the ring is computed again by the neighbouring block).  A thread sums the 64 channels of its pooled position,
+// in channel order, into the 4x4 pixel patch their winning conv positions touch: 9 products per channel, placed by selects on
+// the window position.  The patches go to shared memory; each owned pixel then adds the (up to) four patches that cover it in a
+// fixed order and is written by that one thread.  No atomics: the result is bit-reproducible.
+constexpr int C1D_EH = 16, C1D_EW = 32, C1D_TH = C1D_EH - 2, C1D_TW = C1D_EW - 2;
+constexpr int C1D_PS = 17;                // patch stride in shared memory (16 + 1: neighbouring patches fall in different banks)
+
+template <typename T>
+__global__ void __launch_bounds__(256) conv1_pool_dgrad_code_kernel(const uint8_t* __restrict__ code, const T* __restrict__ dpool,
+                                                                     const float* __restrict__ w, float scale,
+                                                                     float* __restrict__ dimg, int H, int W) {
+  __shared__ float sw[64 * 9];
+  __shared__ float patch[C1D_EH * C1D_EW * C1D_PS];
+  for (int i = threadIdx.x; i < 64 * 9; i += blockDim.x) sw[i] = w[i];
+  __syncthreads();
+  const int Hp = H / 2, Wp = W / 2;
+  const int n = blockIdx.z;
+  const int h0 = blockIdx.y * C1D_TH, w0 = blockIdx.x * C1D_TW;     // first owned pooled position
+  for (int e = threadIdx.x; e < C1D_EH * C1D_EW; e += blockDim.x) {
+    const int ho = h0 - 1 + e / C1D_EW, wo = w0 - 1 + e % C1D_EW;
+    if (ho < 0 || ho >= Hp || wo < 0 || wo >= Wp) continue;        // outside the image: never read below
+    const int64_t pp = (((int64_t)n * Hp + ho) * Wp + wo) * 64;
+    float acc[4][4];
+#pragma unroll
+    for (int i = 0; i < 16; i++) acc[i >> 2][i & 3] = 0.f;
+#pragma unroll 1
+    for (int cg = 0; cg < 8; cg++) {
+      float g[8];
+      ld8(dpool + pp + cg * 8, g);
+      const uint2 cw2 = *reinterpret_cast<const uint2*>(code + pp + cg * 8);
+      const uint32_t cw[2] = {cw2.x, cw2.y};
+#pragma unroll
+      for (int c = 0; c < 8; c++) {
+        bool py, px;
+        const float gg = conv1_code_decode((cw[c >> 2] >> (8 * (c & 3))) & 0xffu, g[c], py, px);
+        const float* wc = sw + (cg * 8 + c) * 9;
+        float u[3][4];                    // row r of the tap products, shifted right by px
+#pragma unroll
+        for (int r = 0; r < 3; r++) {
+          const float t0 = gg * wc[r * 3], t1 = gg * wc[r * 3 + 1], t2 = gg * wc[r * 3 + 2];
+          u[r][0] = px ? 0.f : t0;
+          u[r][1] = px ? t0 : t1;
+          u[r][2] = px ? t1 : t2;
+          u[r][3] = px ? t2 : 0.f;
+        }
+#pragma unroll
+        for (int dx = 0; dx < 4; dx++) {  // ... and down by py
+          acc[0][dx] += py ? 0.f : u[0][dx];
+          acc[1][dx] += py ? u[0][dx] : u[1][dx];
+          acc[2][dx] += py ? u[1][dx] : u[2][dx];
+          acc[3][dx] += py ? u[2][dx] : 0.f;
+        }
+      }
+    }
+    float* ps = patch + e * C1D_PS;       // patch pixel (dy, dx) is image pixel (2ho-1+dy, 2wo-1+dx)
+#pragma unroll
+    for (int i = 0; i < 16; i++) ps[i] = acc[i >> 2][i & 3];
+  }
+  __syncthreads();
+  // owned pixels: the 2x2 blocks under the owned pooled positions; the last tile row / column also owns the image row / column an
+  // odd H / W leaves outside every pool window (it receives taps of the conv row / column before it, but no gradient of its own)
+  const int y0 = 2 * h0, x0 = 2 * w0;
+  const int y1 = (h0 + C1D_TH >= Hp) ? H : 2 * (h0 + C1D_TH), x1 = (w0 + C1D_TW >= Wp) ? W : 2 * (w0 + C1D_TW);
+  const int tw = x1 - x0, npix = (y1 - y0) * tw;
+  for (int i = threadIdx.x; i < npix; i += blockDim.x) {
+    const int y = y0 + i / tw, x = x0 + i % tw;
+    float s = 0.f;
+#pragma unroll
+    for (int a = 0; a < 2; a++) {
+      const int ho = ((y + 1) >> 1) - 1 + a;                       // the two pooled rows whose patches (rows 2ho-1..2ho+2) hold y
+      if (ho < 0 || ho >= Hp) continue;
+#pragma unroll
+      for (int b = 0; b < 2; b++) {
+        const int wo = ((x + 1) >> 1) - 1 + b;
+        if (wo < 0 || wo >= Wp) continue;
+        s += patch[((ho - h0 + 1) * C1D_EW + (wo - w0 + 1)) * C1D_PS + (y - 2 * ho + 1) * 4 + (x - 2 * wo + 1)];
+      }
+    }
+    dimg[((int64_t)n * H + y) * W + x] = s * scale;
+  }
 }
 
 // conv1 weight gradient from the pooled-output gradient (recompute conv1 -> argmax + ReLU mask).
@@ -664,6 +759,18 @@ int lo_conv1_pool_wgrad_code(const void* img, int img_is_u8, float scale, float 
 int lo_conv1_pool_wgrad_norm(const void* img, int img_is_u8, float scale, float offset, const float* w, const float* bias,
                              const void* dpool, int dt, float* dw, float* db, int N, int H, int W, void* stream) {
   return conv1_wgrad(img, img_is_u8, w, bias, dpool, dt, dw, db, N, H, W, (cudaStream_t)stream, scale, offset);
+}
+int lo_conv1_pool_dgrad_code(const uint8_t* code, const void* dpool, int dt, const float* w, float scale, float* dimg, int N, int H,
+                             int W, void* stream) {
+  LO_CHECK_ARG(code && dpool && w && dimg, "null pointer");
+  LO_CHECK_ARG(dt == LO_F32 || dt == LO_BF16, "dt must be LO_F32 or LO_BF16");
+  LO_CHECK_ARG(N >= 1 && H >= 2 && W >= 2, "shape (N >= 1, H >= 2, W >= 2)");
+  LO_CHECK_ARG(N <= 65535 && (H / 2 + C1D_TH - 1) / C1D_TH <= 65535, "shape (N or H too large for the grid)");
+  cudaStream_t st = (cudaStream_t)stream;
+  const dim3 grid(cdiv(W / 2, C1D_TW), cdiv(H / 2, C1D_TH), N);
+  LO_DISPATCH_DT(dt, T, (conv1_pool_dgrad_code_kernel<T><<<grid, 256, 0, st>>>(code, (const T*)dpool, w, scale, dimg, H, W)));
+  LO_LAUNCH_OK();
+  return LO_OK;
 }
 
 int lo_im2col(const void* x, void* col, int dt, int N, int H, int W, int C, int R, int S, int stride, int pad, void* stream) {

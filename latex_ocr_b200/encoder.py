@@ -230,14 +230,22 @@ class EncoderCNN(nn.Module):
         ob, nb, _ = self.store.offsets["cnn.%s.bias" % idx]
         return ow, ob + nb - ow
 
-    def backward_raw(self, img_shape, denc, on_layer_grad=None, ws=None):
+    def backward_raw(self, img_shape, denc, on_layer_grad=None, ws=None, dimg=None):
         """denc: fp32 [N,H',W',512] gradient w.r.t. the encoder output.  Fills self.store.grad.  ``on_layer_grad(idx)`` is
         called right after the kernels that complete layer idx's weight/bias gradient have been enqueued (last conv first):
         the data-parallel path fires that layer's gradient all-reduce there, overlapping the rest of the backward.  ``ws``: the
-        workspace of the forward (default: the cached one of this image shape)."""
+        workspace of the forward (default: the cached one of this image shape).  ``dimg``: an fp32 CUDA tensor of N*H*W
+        elements that receives the gradient w.r.t. the image (written, not accumulated); it needs the arg-max codes of a training
+        forward (``forward_raw(..., need_grad=True)``).  Without it, no image gradient is computed."""
         L = _lib.lib()
         N, _, H, W = img_shape
         ws = ws if ws is not None else self._workspace(N, H, W, True)
+        if dimg is not None:
+            if ws.get("code0") is None:
+                raise _lib.LatexOcrB200Error("EncoderCNN.backward_raw: the image gradient needs the arg-max codes of a training "
+                                             "forward (forward_raw(img, need_grad=True)); this workspace has none")
+            if dimg.dtype != torch.float32 or not dimg.is_contiguous() or dimg.numel() != N * H * W:
+                raise ValueError("dimg must be a contiguous float32 tensor of N*H*W elements")
         st, dt, impl, S = stream_ptr(), _dt(self.precision), self._impl(), self.store
         A, G = ws["acts"], ws["grads"]
         for l in self.layers[1:]:
@@ -299,15 +307,17 @@ class EncoderCNN(nn.Module):
                       ptr(S.g("cnn.0.weight")), ptr(S.g("cnn.0.bias")), N, H, W, st))
         if on_layer_grad is not None:
             on_layer_grad("0")
+        if dimg is not None:
+            # conv1's data gradient through its ReLU and max-pool, from the forward's codes and G["P0"] (complete above)
+            check(L.lo_conv1_pool_dgrad_code(ptr(ws["code0"]), ptr(G["P0"]), dt, ptr(S.f32("cnn.0.weight")), sc, ptr(dimg),
+                                             N, H, W, st))
 
     def forward(self, img):
-        """Reference signature (seq2seq_torch.py:88-100): returns a new fp32 tensor [N,H',W',512].  With grad mode on and a
-        parameter requiring grad, an autograd graph is recorded whose backward runs ``backward_raw``; the output is the same
-        either way.  There is no gradient for the image."""
-        if img.requires_grad and torch.is_grad_enabled():
-            raise NotImplementedError("EncoderCNN computes no gradient for the input image")
+        """Reference signature (seq2seq_torch.py:88-100): returns a new fp32 tensor [N,H',W',512].  With grad mode on and the
+        image or a parameter requiring grad, an autograd graph is recorded whose backward runs ``backward_raw``; the output is
+        the same either way.  The image gradient is returned in the image's shape and dtype."""
         params = list(self.parameters())
-        if torch.is_grad_enabled() and any(p.requires_grad for p in params):
+        if torch.is_grad_enabled() and (img.requires_grad or any(p.requires_grad for p in params)):
             return _EncoderFunction.apply(self, img, *params)
         with torch.no_grad():
             return self.forward_raw(img, need_grad=False).float()
@@ -320,7 +330,7 @@ class _EncoderFunction(torch.autograd.Function):
     def forward(ctx, enc, img, *params):
         out = enc.forward_raw(img, need_grad=True)
         N, _, H, W = img.shape
-        ctx.enc, ctx.ws, ctx.shape = enc, enc._ws.get((N, H, W)), tuple(img.shape)
+        ctx.enc, ctx.ws, ctx.shape, ctx.img_dtype = enc, enc._ws.get((N, H, W)), tuple(img.shape), img.dtype
         ctx.gen = ctx.ws["gen"]
         return out.to(torch.float32, copy=True)        # never the workspace buffer itself: each call's output has its own node
 
@@ -333,6 +343,9 @@ class _EncoderFunction(torch.autograd.Function):
                                          "forward of the same shape; run backward before the next forward of that shape"
                                          % (ctx.shape,))
         unbind_grads(enc, S)                      # the kernels overwrite store.grad
-        enc.backward_raw(ctx.shape, dout.float().contiguous(), ws=ctx.ws)
-        return (None, None) + tuple(grad_view(S, p).clone() if need else None
+        dimg = torch.empty(ctx.shape, dtype=torch.float32, device=dout.device) if ctx.needs_input_grad[1] else None
+        enc.backward_raw(ctx.shape, dout.float().contiguous(), ws=ctx.ws, dimg=dimg)
+        if dimg is not None and dimg.dtype != ctx.img_dtype:
+            dimg = dimg.to(ctx.img_dtype)
+        return (None, dimg) + tuple(grad_view(S, p).clone() if need else None
                                     for p, need in zip(enc.parameters(), ctx.needs_input_grad[2:]))

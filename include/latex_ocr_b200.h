@@ -196,6 +196,31 @@ int lo_attention_backward(const void* att1, const void* enc, int dt, const float
                           float* de, float* datt2, float* dgp, int64_t dcat_stride, float* dctx_out, float* dwf_part,
                           const uint8_t* relu_mask, int B, int R, int A, int C, void* work, void* stream);
 
+/* Whole backward of ONE stand-alone Attention.forward call (autograd of seq2seq_torch.py:185-190: encoder_att, decoder_att,
+ * full_att, softmax and the context sum), where lo_decoder_backward hoists d att1 and d enc out of its time loop:
+ *   s = <dctx, ctx> + sum_r alpha_r dalpha_r ; de_r = alpha_r (<dctx, enc_r> + dalpha_r - s) ; on_ra = att1_ra + att2_a > 0
+ *   datt1_ra = wf_a de_r on_ra ; datt2_a = wf_a sum_r de_r on_ra ; g_w_full_a = sum_b sum_r de_r relu(att1_ra + att2_a) ; g_b_full = 0
+ *   denc = alpha (x) dctx + datt1 W_enc ; g_w_enc = datt1^T enc ; g_b_enc = colsum(datt1)
+ *   dh = datt2 W_dec ; g_w_dec = datt2^T h ; g_b_dec = colsum(datt2)
+ * One pass of the TMA-ring backward kernel reads att1 and enc once and writes de, datt2, the per-row g_w_full partials and datt1.
+ * Inputs (required): enc / att1 [B][R][C|A] (dt) and h [B][D] fp32 as the forward used them, att2 [B][A] fp32 (= h W_dec^T + b_dec),
+ * w_enc [A][C] and w_dec [A][D] (dt: the weights the forward read), wf [A] fp32, alpha [B][R] and ctx [B][C] fp32 (forward results),
+ * dctx [B][C] fp32; dalpha [B][R] fp32 may be NULL (zero).  Outputs, all fp32 except datt1 (dt), all written (never accumulated),
+ * each optional — NULL means not needed and skips the work only it needs: denc [B][R][C], dh [B][D], g_w_enc [A][C], g_b_enc [A],
+ * g_w_dec [A][D], g_b_dec [A], g_w_full [A], g_b_full [1], de [B][R], datt2 [B][A], datt1 [B][R][A].  Without denc, g_w_enc,
+ * g_b_enc and datt1, d att1 is not written and neither of its GEMMs runs.  impl = LO_IMPL_TC with dt = LO_BF16: the two
+ * [B*R, A] x [A, C] products run on the wgmma GEMMs (fp32 storage ignores it).  work: lo_attention_step_workspace_bytes(B, R, A, C,
+ * dt) bytes, zero-initialised once by the caller.  With lo_set_option("deterministic", 1) every cross-CTA sum adds in a fixed
+ * order, so two identical calls give identical bits.  Launched stream-ordered unless "att_abi_pdl" (above).  Null inputs, a bad
+ * dt or impl, A != C, C not in {256, 512, 1024}, B outside 1..512, R < 1, D < 1 and enc, att1 or datt1 not 16-byte aligned are
+ * refused (LO_EINVAL) before any GPU work. */
+int64_t lo_attention_step_workspace_bytes(int B, int R, int A, int C, int dt);
+int lo_attention_step_backward(const void* enc, const void* att1, int dt, const float* h, const float* att2, const void* w_enc,
+                               const void* w_dec, const float* wf, const float* alpha, const float* ctx, const float* dctx,
+                               const float* dalpha, float* denc, float* dh, float* g_w_enc, float* g_b_enc, float* g_w_dec,
+                               float* g_b_dec, float* g_w_full, float* g_b_full, float* de, float* datt2, void* datt1,
+                               int B, int R, int A, int C, int D, int impl, void* work, void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Whole teacher-forced decoder: DecoderWithAttention.forward seq2seq_torch.py:267-320 (+ the loss of
  * img2seq_torch.py:147-159) and its hand-derived backward.  One struct carries every buffer; the

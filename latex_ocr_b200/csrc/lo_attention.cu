@@ -379,7 +379,11 @@ __global__ void __launch_bounds__(AP_THREADS, LO_ATT_MINB) attention_fwd_pipe_ke
   for (int r = threadIdx.x; r < R; r += AP_THREADS) alb[r] = expf(__ldcg(alb + r) - Mg) * invL;
 }
 
-template <typename T, int NVA, int NVC, bool CL, int ACT>
+// DA1 (lo_attention_step_backward, a single Attention.forward call): while a stage is resident the consumer warps also store
+//   datt1[b][r][a] = wf[a] * de[b][r] * act'(att1[b][r][a] + att2[b][a])
+// in the storage type, so the att1 rows are read once for de, datt2, the d w_full partial and d att1.  Without DA1 the datt1
+// argument (last, so the other parameters keep their offsets) is unused.
+template <typename T, int NVA, int NVC, bool CL, int ACT, bool DA1 = false>
 __global__ void __launch_bounds__(AP_THREADS) attention_bwd_pipe_kernel(
     const T* __restrict__ att1, const T* __restrict__ enc, const float* __restrict__ att2, const float* __restrict__ gate,
     int64_t o1_stride, const float* __restrict__ wf, const float* __restrict__ alpha, int64_t alpha_stride,
@@ -387,7 +391,7 @@ __global__ void __launch_bounds__(AP_THREADS) attention_bwd_pipe_kernel(
     int64_t dreg_stride, const float* __restrict__ sreg, int64_t sreg_stride, float* __restrict__ de, float* __restrict__ datt2,
     float* __restrict__ dgp, int64_t dcat_stride, bf16* __restrict__ datt2_bf, bf16* __restrict__ dgp_bf,
     float* __restrict__ dctx_out, int R, int nsplit, int* __restrict__ counters, float* __restrict__ partials, int pol_enc,
-    int pol_att1, float* __restrict__ dwf_part) {
+    int pol_att1, float* __restrict__ dwf_part, T* __restrict__ datt1) {
   using C = ApCfg<T, NVA, NVC>;
   constexpr int CHA = C::CHA, CHC = C::CHC;
   extern __shared__ __align__(128) uint8_t ap_smem[];
@@ -402,6 +406,12 @@ __global__ void __launch_bounds__(AP_THREADS) attention_bwd_pipe_kernel(
   const int nst = r1 > r0 ? (r1 - r0 + C::ROWS - 1) / C::ROWS : 0;
   const T* a1b = att1 + (int64_t)b * R * CHA;
   const T* eb = enc + (int64_t)b * R * CHC;
+  const float* s_wf = nullptr;           // DA1, NVA > 2: full_att.weight in shared memory (in registers it would spill)
+  if constexpr (DA1 && NVA > 2) {
+    __shared__ __align__(16) float s_wbuf[CHA];       // read 8 floats at a time (two 16-byte loads)
+    for (int c = threadIdx.x; c < CHA; c += AP_THREADS) s_wbuf[c] = wf[c];
+    s_wf = s_wbuf;
+  }
   if (threadIdx.x == 0) {
     for (int s = 0; s < AP_STAGES; s++) {
       mbar_init(full_bar + s, 1);
@@ -438,6 +448,11 @@ __global__ void __launch_bounds__(AP_THREADS) attention_bwd_pipe_kernel(
     pdl_wait();          // the producer warp joins the combine below, which reads the preceding kernel's results
   } else {
     float a2[NVA * 8], dc[NVC * 8];
+    float wv[NVA * 8];                 // DA1, NVA <= 2: full_att.weight in registers
+    if constexpr (DA1 && NVA <= 2) {
+#pragma unroll
+      for (int j = 0; j < NVA; j++) ld8(wf + (j * 32 + lane) * 8, wv + j * 8);
+    }
     float sdot = 0.f;
     // att2 / gate / ctx / sreg were saved by the forward pass: they are fetched BEFORE griddepcontrol.wait (overlapping the tail of
     // the preceding launch); only d gctx comes from the preceding kernel
@@ -531,7 +546,10 @@ __global__ void __launch_bounds__(AP_THREADS) attention_bwd_pipe_kernel(
         }
 #pragma unroll
         for (int j = 0; j < NVA; j++) {
-          float v[8];
+          float v[8], g[8], w8[8];
+          const float* wj = w8;
+          if constexpr (DA1 && NVA > 2) ld8(s_wf + (j * 32 + lane) * 8, w8);
+          else wj = wv + j * 8;
           ld8(sa + (size_t)ra * CHA + (j * 32 + lane) * 8, v);
 #pragma unroll
           for (int q = 0; q < 8; q++) {
@@ -539,7 +557,9 @@ __global__ void __launch_bounds__(AP_THREADS) attention_bwd_pipe_kernel(
             const float post = att_act<ACT, sizeof(T) == 2>(pre);
             macc[j * 8 + q] = fmaf(de0, att_dact<ACT>(pre, post), macc[j * 8 + q]);
             wacc[j * 8 + q] = fmaf(de0, post, wacc[j * 8 + q]);
+            if constexpr (DA1) g[q] = wj[q] * (de0 * att_dact<ACT>(pre, post));
           }
+          if constexpr (DA1) st8(datt1 + ((int64_t)b * R + row + ra) * CHA + (j * 32 + lane) * 8, g);
           if (two) {
             ld8(sa + (size_t)rb * CHA + (j * 32 + lane) * 8, v);
 #pragma unroll
@@ -548,7 +568,9 @@ __global__ void __launch_bounds__(AP_THREADS) attention_bwd_pipe_kernel(
               const float post = att_act<ACT, sizeof(T) == 2>(pre);
               macc[j * 8 + q] = fmaf(de1, att_dact<ACT>(pre, post), macc[j * 8 + q]);
               wacc[j * 8 + q] = fmaf(de1, post, wacc[j * 8 + q]);
+              if constexpr (DA1) g[q] = wj[q] * (de1 * att_dact<ACT>(pre, post));
             }
+            if constexpr (DA1) st8(datt1 + ((int64_t)b * R + row + rb) * CHA + (j * 32 + lane) * 8, g);
           }
         }
       }
@@ -1307,6 +1329,34 @@ static int bwd_launch_a(const AttBwdArgs& x, cudaStream_t st) {
     attr = true;
   }
   const int ns = att_pipe_splits(x.B, x.nsplit_hint);
+  if (x.datt1) {
+    if constexpr (ACT == 0) {
+      LO_CHECK_ARG(!x.mask_in, "d att1 is computed from att1, not from the mask bits");
+      static bool attr_d = false;
+      if (!attr_d) {
+        LO_CUDA(cudaFuncSetAttribute(attention_bwd_pipe_kernel<T, NVA, NVC, false, ACT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM));
+        LO_CUDA(cudaFuncSetAttribute(attention_bwd_pipe_kernel<T, NVA, NVC, true, ACT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM));
+        attr_d = true;
+      }
+      // without a cluster the splits of a batch row add their d w_full partials with atomics: one split keeps the order fixed
+      const int nsd = (x.ordered_dwf && x.dwf_part && !use_cluster(ns, x.R)) ? 1 : ns;
+#define LO_BWDD_ARGS                                                                                                             \
+  (const T*)x.att1, (const T*)x.enc, x.att2, x.gate, x.o1_stride, x.wf, x.alpha, x.alpha_stride, x.ctx, x.dgctx, x.dg_stride, x.dreg, \
+      x.dreg_stride, x.sreg, x.sreg_stride, x.de, x.datt2, x.dgp, x.dcat_stride, x.datt2_bf, x.dgp_bf, x.dctx_out, x.R, nsd,      \
+      (int*)x.work, (float*)((char*)x.work + 4096), g_opt_att_policy_enc, g_opt_att_policy_att1, x.dwf_part, (T*)x.datt1
+      if (use_cluster(nsd, x.R)) {
+        LO_CUDA(launch_att(attention_bwd_pipe_kernel<T, NVA, NVC, true, ACT, true>, dim3(nsd, x.B), (size_t)C::SMEM, nsd, st, att_pdl_ok(x.abi),
+                           LO_BWDD_ARGS));
+      } else {
+        LO_CUDA(launch_att(attention_bwd_pipe_kernel<T, NVA, NVC, false, ACT, true>, dim3(nsd, x.B), (size_t)C::SMEM, 1, st, att_pdl_ok(x.abi),
+                           LO_BWDD_ARGS));
+      }
+#undef LO_BWDD_ARGS
+      LO_LAUNCH_OK();
+      return LO_OK;
+    }
+    return fail(LO_EINVAL, "%s: d att1 is only produced for the ReLU score", __func__);
+  }
   if constexpr (ACT == 0 && sizeof(T) == 2 && NVA == 2 && NVC == 2)
   if (x.mask_in && g_opt_att_bwd_mma && att_rows_per_split(x.R, ns) <= 2048) {
     static bool attr_t = false;
@@ -1355,7 +1405,7 @@ static int bwd_launch_a(const AttBwdArgs& x, cudaStream_t st) {
 #define LO_BWD_ARGS                                                                                                              \
   (const T*)x.att1, (const T*)x.enc, x.att2, x.gate, x.o1_stride, x.wf, x.alpha, x.alpha_stride, x.ctx, x.dgctx, x.dg_stride, x.dreg, \
       x.dreg_stride, x.sreg, x.sreg_stride, x.de, x.datt2, x.dgp, x.dcat_stride, x.datt2_bf, x.dgp_bf, x.dctx_out, x.R, ns,       \
-      (int*)x.work, (float*)((char*)x.work + 4096), g_opt_att_policy_enc, g_opt_att_policy_att1, x.dwf_part
+      (int*)x.work, (float*)((char*)x.work + 4096), g_opt_att_policy_enc, g_opt_att_policy_att1, x.dwf_part, (T*)nullptr
   if (use_cluster(ns, x.R)) {
     LO_CUDA(launch_att(attention_bwd_pipe_kernel<T, NVA, NVC, true, ACT>, dim3(ns, x.B), (size_t)C::SMEM, ns, st, att_pdl_ok(x.abi), LO_BWD_ARGS));
   } else {

@@ -249,6 +249,8 @@ struct AttBwdArgs {
   const uint8_t* mask_in;   // optional (ReLU score only): the forward's mask bits; the kernel then streams enc + 1 bit per att1
                             // element instead of enc + att1 (d w_full must then come from the post-loop sweep: dwf_part unused)
   int abi = 0;         // as in AttFwdArgs
+  void* datt1 = nullptr;   // optional (ReLU score, no mask_in): [B][R][A] storage-type d att1, written by the same pass
+  int ordered_dwf = 0;     // 1: dwf_part must be summed in a fixed order (one split per batch row unless the splits form a cluster)
 };
 extern int g_opt_att_pipe;
 extern int g_opt_att_maskbits;

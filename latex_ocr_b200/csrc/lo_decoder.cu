@@ -702,6 +702,16 @@ __global__ void add_rowbcast_kernel(float* __restrict__ denc, const float* __res
   }
 }
 
+// denc[b][r][c] += alpha[b][r] * dctx[b][c]   (the context read of one attention step, seq2seq_torch.py:190)
+__global__ void add_outer_kernel(float* __restrict__ denc, const float* __restrict__ alpha, const float* __restrict__ dctx, int R, int C,
+                                 int64_t total) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int c = (int)(i % C);
+    const int64_t br = i / C;
+    denc[i] = fmaf(alpha[br], dctx[(br / R) * C + c], denc[i]);
+  }
+}
+
 // out[n][k] = in[k][n]  (in [K][ld_in] -> out [N][ld_out]), generic small transpose with dtype
 template <typename T>
 __global__ void transpose_kernel(const T* __restrict__ in, int64_t ld_in, T* __restrict__ out, int64_t ld_out, int K, int N) {
@@ -1232,6 +1242,89 @@ int lo_attention_backward(const void* att1, const void* enc, int dt, const float
                de, datt2, dgp, dcat_stride, nullptr, nullptr, dctx_out, B, R, work, dwf_part, 0, 0, 0, relu_mask};
   x.abi = 1;
   return attention_bwd_pipe(x, dt, C, (cudaStream_t)stream);
+}
+
+// work of lo_attention_step_backward: attention split workspace | d w_full partials [B][A] | de [B][R] | datt2 [B][A] | sreg [B] |
+// d att1 [B][R][A] (dt) | W_enc^T [C][A] bf16, each region 256-byte aligned
+static inline int64_t step_ws_align(int64_t n) { return (n + 255) & ~(int64_t)255; }
+
+int64_t lo_attention_step_workspace_bytes(int B, int R, int A, int C, int dt) {
+  if (B < 1 || R < 1 || A < 1 || C < 1) return 0;
+  const int64_t es = dt == LO_F32 ? 4 : 2;
+  return step_ws_align(lo_attention_workspace_bytes(B, C)) + 2 * step_ws_align((int64_t)B * A * 4) + step_ws_align((int64_t)B * R * 4) +
+         step_ws_align((int64_t)B * 4) + step_ws_align((int64_t)B * R * A * es) + step_ws_align((int64_t)A * C * 2);
+}
+
+int lo_attention_step_backward(const void* enc, const void* att1, int dt, const float* h, const float* att2, const void* w_enc,
+                               const void* w_dec, const float* wf, const float* alpha, const float* ctx, const float* dctx,
+                               const float* dalpha, float* denc, float* dh, float* g_w_enc, float* g_b_enc, float* g_w_dec, float* g_b_dec,
+                               float* g_w_full, float* g_b_full, float* de, float* datt2, void* datt1, int B, int R, int A, int C, int D,
+                               int impl, void* work, void* stream) {
+  LO_CHECK_ARG(enc && att1 && h && att2 && w_enc && w_dec && wf && alpha && ctx && dctx && work, "null pointer");
+  LO_CHECK_ARG(dt == LO_F32 || dt == LO_BF16, "dt must be LO_F32 or LO_BF16");
+  LO_CHECK_ARG(impl == LO_IMPL_SIMT || impl == LO_IMPL_TC, "impl must be LO_IMPL_SIMT or LO_IMPL_TC");
+  LO_CHECK_ARG(A == C && (C == 256 || C == 512 || C == 1024), "attention_dim == encoder_dim in {256,512,1024}");
+  LO_CHECK_ARG(B > 0 && B <= 512 && R > 0 && D > 0, "B in 1..512, R > 0, D > 0");
+  LO_CHECK_ARG((((uintptr_t)enc | (uintptr_t)att1 | (uintptr_t)datt1) & 15) == 0,
+               "enc, att1 and datt1 must be 16-byte aligned (bulk copies, 16-byte stores)");
+  LO_CHECK_ARG(g_opt_att_pipe, "stand-alone attention backward runs on the TMA-ring kernel (option att_pipe=1)");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int64_t es = dt == LO_F32 ? 4 : 2;
+  const int64_t BR = (int64_t)B * R;
+  char* w = (char*)work + step_ws_align(lo_attention_workspace_bytes(B, C));
+  float* ws_dwf = (float*)w;     w += step_ws_align((int64_t)B * A * 4);
+  float* ws_de = (float*)w;      w += step_ws_align(BR * 4);
+  float* ws_datt2 = (float*)w;   w += step_ws_align((int64_t)B * A * 4);
+  float* ws_sreg = (float*)w;    w += step_ws_align((int64_t)B * 4);
+  void* ws_datt1 = w;            w += step_ws_align(BR * A * es);
+  bf16* ws_wet = (bf16*)w;
+  float* de_ = de ? de : ws_de;
+  float* datt2_ = datt2 ? datt2 : ws_datt2;
+  // d att1 is written only when something reads it: d enc, the encoder_att gradients, or the caller
+  const bool need_d1 = denc || g_w_enc || g_b_enc || datt1;
+  void* d1 = datt1 ? datt1 : ws_datt1;
+  const bool tc = impl == LO_IMPL_TC && dt == LO_BF16 && tc_available();
+  // s = <dctx, ctx> + sum_r alpha_r dalpha_r: the second term per batch row (one warp each, fixed order)
+  if (dalpha) {
+    sreg_kernel<<<cdiv(B, 8), 256, 0, st>>>(alpha, dalpha, R, 0, ws_sreg, B, 1, R);
+    LO_LAUNCH_OK();
+  }
+  if (g_w_full) LO_CUDA(cudaMemsetAsync(ws_dwf, 0, (size_t)B * A * 4, st));
+  AttBwdArgs x{att1, enc, att2, nullptr, A, wf, alpha, R, ctx, dctx, C, dalpha, R, dalpha ? ws_sreg : nullptr, 1, de_, datt2_, nullptr, A,
+               nullptr, nullptr, nullptr, B, R, work, g_w_full ? ws_dwf : nullptr, 0, 0, 0, nullptr};
+  x.abi = 1;
+  x.datt1 = need_d1 ? d1 : nullptr;
+  x.ordered_dwf = g_opt_det;
+  LO_TRY(attention_bwd_pipe(x, dt, C, st));
+  // full_att: d weight = sum_b of the per-row partials; d bias = 0 exactly (sum_r de_r = 0), as lo_decoder_backward
+  if (g_w_full) LO_TRY(colsum(ws_dwf, LO_F32, g_w_full, B, A, A, 0, st));
+  if (g_b_full) LO_CUDA(cudaMemsetAsync(g_b_full, 0, 4, st));
+  // decoder_att: dh = datt2 W_d ; d W_d = datt2^T h ; d b_d = colsum(datt2)
+  if (dh) LO_TRY(gemm_nn(datt2_, LO_F32, A, w_dec, dt, D, dh, LO_F32, D, B, D, A, 0, LO_IMPL_SIMT, st));
+  if (g_w_dec) LO_TRY(gemm_tn(datt2_, LO_F32, A, h, LO_F32, D, g_w_dec, LO_F32, D, A, D, B, 0, LO_IMPL_SIMT, st));
+  if (g_b_dec) LO_TRY(colsum(datt2_, LO_F32, g_b_dec, B, A, A, 0, st));
+  // encoder_att: d W_e = datt1^T enc ; d b_e = colsum(datt1) ; denc = datt1 W_e + alpha (x) dctx
+  if (g_w_enc) {
+    if (tc) {
+      LO_CUDA(cudaMemsetAsync(g_w_enc, 0, (size_t)A * C * 4, st));
+      LO_TRY(tc_gemm_tn((const bf16*)d1, A, (const bf16*)enc, C, g_w_enc, C, A, C, (int)BR, st));
+    } else {
+      LO_TRY(gemm_tn(d1, dt, A, enc, dt, C, g_w_enc, LO_F32, C, A, C, (int)BR, 0, LO_IMPL_SIMT, st));
+    }
+  }
+  if (g_b_enc) LO_TRY(colsum(d1, dt, g_b_enc, (int)BR, A, A, 0, st));
+  if (denc) {
+    if (tc) {
+      transpose_kernel<bf16><<<dim3(cdiv(C, 32), cdiv(A, 32)), dim3(32, 8), 0, st>>>((const bf16*)w_enc, C, ws_wet, A, A, C);
+      LO_LAUNCH_OK();
+      LO_TRY(tc_gemm_nt((const bf16*)d1, A, ws_wet, A, denc, LO_F32, C, (int)BR, C, A, nullptr, 0, 0, st));
+    } else {
+      LO_TRY(gemm_nn(d1, dt, A, w_enc, dt, C, denc, LO_F32, C, (int)BR, C, A, 0, LO_IMPL_SIMT, st));
+    }
+    add_outer_kernel<<<LO_NUM_SMS * 8, 256, 0, st>>>(denc, alpha, dctx, R, C, BR * C);
+    LO_LAUNCH_OK();
+  }
+  return LO_OK;
 }
 
 int lo_decoder_forward(const lo_decoder_args* a, int with_loss, void* stream) {

@@ -38,6 +38,26 @@ class _DecoderFunction(torch.autograd.Function):
         return (None, None, dx if ctx.needs_input_grad[2] else None, None, None) + tuple(grads)
 
 
+class _AttentionFunction(torch.autograd.Function):
+    """Autograd node of Attention.forward: inputs (module, encoder_out, decoder_hidden, *parameters), differentiable outputs
+    (context, alpha)."""
+
+    @staticmethod
+    def forward(ctx, att, encoder_out, decoder_hidden, *params):
+        c, alpha, saved = att._forward_impl(encoder_out, decoder_hidden, need_grad=True)
+        ctx.att, ctx.meta = att, saved.pop("meta")
+        ctx.save_for_backward(saved["enc"], saved["h"], saved["att1"], saved["att2"], c, alpha)
+        ctx.set_materialize_grads(False)          # an unused output's gradient stays None (no zero tensor, no d alpha pass)
+        return c, alpha
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, dctx, dalpha):
+        need = ctx.needs_input_grad
+        denc, dh, grads = ctx.att._backward_impl(ctx.saved_tensors, ctx.meta, dctx, dalpha, need[1], need[2], need[3:])
+        return (None, denc, dh) + tuple(grads)
+
+
 def decoder_specs(A, E, D, V, C):
     """Flat order: [decoder_att.W; f_beta.W; weight_hh] and their biases are contiguous so the per-step
     GEMM h -> (att2 | gate_pre | hh) and its weight gradient are single launches."""
@@ -58,10 +78,12 @@ class Attention(nn.Module):
     -> (context[B,C], alpha[B,R]).  Inside DecoderWithAttention the parameters are views into the
     decoder's flat store."""
 
-    def __init__(self, encoder_dim, decoder_dim, attention_dim, device="cuda", precision="bf16", _store=None):
+    def __init__(self, encoder_dim, decoder_dim, attention_dim, device="cuda", precision="bf16", _store=None, impl=None):
         super().__init__()
         self.encoder_dim, self.decoder_dim, self.attention_dim = encoder_dim, decoder_dim, attention_dim
         self.precision = precision
+        # GEMMs of the backward's two [B*R, A] x [A, C] products: wgmma in bf16 ("tc"), CUDA cores otherwise
+        self.impl = impl if impl is not None else ("tc" if precision == "bf16" else "simt")
         self.tdtype = torch.float32 if precision == "fp32" else torch.bfloat16
         own = _store is None
         if own:
@@ -82,11 +104,25 @@ class Attention(nn.Module):
                     getattr(self, sub).weight.uniform_(-b, b)
                     getattr(self, sub).bias.uniform_(-b, b)
         self._work = None
+        self._bwork = None
 
     def forward(self, encoder_out, decoder_hidden):
-        L = _lib.lib()
+        """With grad mode on and ``encoder_out``, ``decoder_hidden`` or a parameter requiring grad, an autograd graph is
+        recorded: ``context`` and ``alpha`` are differentiable, and their backward is lo_attention_step_backward.  The outputs
+        are the same either way."""
         if not encoder_out.is_cuda:
             raise _lib.LatexOcrB200Error("Attention runs on CUDA tensors only (no CPU fallback)")
+        params = list(self.parameters())
+        if torch.is_grad_enabled() and (encoder_out.requires_grad or decoder_hidden.requires_grad
+                                        or any(p.requires_grad for p in params)):
+            return _AttentionFunction.apply(self, encoder_out, decoder_hidden, *params)
+        with torch.no_grad():
+            return self._forward_impl(encoder_out, decoder_hidden, need_grad=False)[:2]
+
+    def _forward_impl(self, encoder_out, decoder_hidden, need_grad):
+        """(context, alpha, what the backward of this call needs or None).  att1 is computed per call, as the reference does
+        (seq2seq_torch.py:186), and kept with att2 for the backward."""
+        L = _lib.lib()
         with torch.no_grad():
             S, st, dt = self.store, stream_ptr(), _dt(self.precision)
             S.sync_shadow()
@@ -107,7 +143,58 @@ class Attention(nn.Module):
             ctx = torch.empty(B, C, dtype=torch.float32, device=enc.device)
             check(L.lo_attention_forward(ptr(att1), ptr(enc), dt, ptr(att2), A, ptr(S.f32("attention.full_att.weight")),
                                          ptr(alpha), R, ptr(ctx), None, 0, None, B, R, A, C, ptr(self._work), st))
-            return ctx, alpha
+            saved = None
+            if need_grad:
+                # the caller's tensors are kept, not the storage-dtype / fp32 copies the kernels read: in a per-step loop the
+                # enc[:bt] slices share one tensor, whereas a bf16 copy per call (57 MB at cfg #2) would double what the loop
+                # holds; the backward redoes the same deterministic conversion (one cast per call)
+                saved = {"enc": encoder_out, "h": decoder_hidden, "att1": att1, "att2": att2,
+                         "meta": {"version": S.master._version, "enc_shape": tuple(encoder_out.shape), "enc_dtype": encoder_out.dtype,
+                                  "h_shape": tuple(decoder_hidden.shape), "h_dtype": decoder_hidden.dtype}}
+            return ctx, alpha, saved
+
+    _GRAD_NAMES = ("encoder_att.weight", "encoder_att.bias", "decoder_att.weight", "decoder_att.bias", "full_att.weight",
+                   "full_att.bias")
+
+    def _backward_impl(self, saved_tensors, meta, dctx, dalpha, need_enc, need_h, need_params):
+        """lo_attention_step_backward: returns (d encoder_out or None, d decoder_hidden or None, [gradient or None per
+        parameter]), each in the shape and dtype of what it is the gradient of."""
+        enc, h, att1, att2, ctx, alpha = saved_tensors
+        S = self.store
+        if S.master._version != meta["version"]:
+            raise _lib.LatexOcrB200Error("Attention backward: a parameter was modified in place after the forward; run backward "
+                                         "before the optimizer step")
+        enc = enc.contiguous().to(self.tdtype)         # exactly what the forward's kernels read
+        h = h.contiguous().float()
+        B, R, C = enc.shape
+        A, D = self.attention_dim, self.decoder_dim
+        dev = enc.device
+        named = dict(self.named_parameters())
+        if dctx is None and dalpha is None:
+            return None, None, [None] * len(need_params)
+        f32 = torch.float32
+        dctx = dctx.float().contiguous() if dctx is not None else torch.zeros(B, C, dtype=f32, device=dev)
+        dal = dalpha.float().contiguous() if dalpha is not None else None
+        grads = [torch.empty(named[n].shape, dtype=f32, device=dev) if need else None
+                 for n, need in zip(self._GRAD_NAMES, need_params)]
+        denc = torch.empty(B, R, C, dtype=f32, device=dev) if need_enc else None
+        dh = torch.empty(B, D, dtype=f32, device=dev) if need_h else None
+        L = _lib.lib()
+        dt = _dt(self.precision)
+        nbytes = L.lo_attention_step_workspace_bytes(B, R, A, C, dt)
+        if self._bwork is None or self._bwork.numel() < nbytes:
+            self._bwork = torch.zeros(nbytes, dtype=torch.uint8, device=dev)
+        impl = _lib.LO_IMPL_TC if (self.impl == "tc" and self.precision == "bf16") else _lib.LO_IMPL_SIMT
+        check(L.lo_attention_step_backward(
+            ptr(enc), ptr(att1), dt, ptr(h), ptr(att2), ptr(S.w("attention.encoder_att.weight")),
+            ptr(S.w("attention.decoder_att.weight")), ptr(S.f32("attention.full_att.weight")), ptr(alpha), ptr(ctx), ptr(dctx),
+            ptr(dal), ptr(denc), ptr(dh), *[ptr(g) for g in grads], None, None, None, B, R, A, C, D, impl, ptr(self._bwork),
+            stream_ptr()))
+        if denc is not None:
+            denc = denc.view(meta["enc_shape"]).to(meta["enc_dtype"])
+        if dh is not None:
+            dh = dh.view(meta["h_shape"]).to(meta["h_dtype"])
+        return denc, dh, grads
 
 
 class DecoderWithAttention(nn.Module):
@@ -124,7 +211,7 @@ class DecoderWithAttention(nn.Module):
         A, E, D, V, C = attention_dim, embed_dim, decoder_dim, vocab_size, encoder_dim
         self.store = FlatStore(decoder_specs(A, E, D, V, C), device, bf16_shadow=(precision == "bf16"))
         S = self.store
-        self.attention = Attention(C, D, A, device, precision, _store=S)
+        self.attention = Attention(C, D, A, device, precision, _store=S, impl=self.impl)
         self.embedding = ParamHolder()
         self.embedding.bind("weight", S, "embedding.weight")
         self.dropout = nn.Dropout(p=dropout)    # kept for train()/eval() semantics and p

@@ -34,7 +34,7 @@ def _prepare(model, img, rows_per_img, max_steps):
     dec = model.decoder
     B = N * rows_per_img
     ws = dec.workspace(B, max_steps, R, need_grad=False)
-    dec.sync_shadow()
+    dec.store.refresh_shadow()
     for t in range(max_steps):
         ws["bt"][t] = B
     a = dec.fill_args(ws, enc_flat, B, max_steps, R, has_dropout=False)

@@ -11,51 +11,9 @@ import torch
 import torch.nn as nn
 
 from . import _lib
-from ._lib import check, ptr, stream_ptr
-from .params import FlatStore, LRUCache, ParamHolder, grad_view, unbind_grads
-
-
-def _dt(precision):
-    return _lib.LO_F32 if precision == "fp32" else _lib.LO_BF16
-
-
-class _DecoderFunction(torch.autograd.Function):
-    """Autograd node of DecoderWithAttention.forward: inputs (module, side-output dict, encoder_out, captions, lengths,
-    *parameters), differentiable outputs (predictions, alphas)."""
-
-    @staticmethod
-    def forward(ctx, dec, rest, encoder_out, encoded_captions, caption_lengths, *params):
-        preds, caps, decode_lengths, alphas, sort_ind, saved = dec._forward_impl(encoder_out, encoded_captions, caption_lengths,
-                                                                                 need_grad=True)
-        rest["out"] = (caps, decode_lengths, sort_ind)
-        ctx.dec, ctx.saved = dec, saved
-        return preds, alphas
-
-    @staticmethod
-    @torch.autograd.function.once_differentiable
-    def backward(ctx, dpreds, dalphas):
-        dx, grads = ctx.dec._backward_impl(ctx.saved, dpreds, dalphas, ctx.needs_input_grad[5:])
-        return (None, None, dx if ctx.needs_input_grad[2] else None, None, None) + tuple(grads)
-
-
-class _AttentionFunction(torch.autograd.Function):
-    """Autograd node of Attention.forward: inputs (module, encoder_out, decoder_hidden, *parameters), differentiable outputs
-    (context, alpha)."""
-
-    @staticmethod
-    def forward(ctx, att, encoder_out, decoder_hidden, *params):
-        c, alpha, saved = att._forward_impl(encoder_out, decoder_hidden, need_grad=True)
-        ctx.att, ctx.meta = att, saved.pop("meta")
-        ctx.save_for_backward(saved["enc"], saved["h"], saved["att1"], saved["att2"], c, alpha)
-        ctx.set_materialize_grads(False)          # an unused output's gradient stays None (no zero tensor, no d alpha pass)
-        return c, alpha
-
-    @staticmethod
-    @torch.autograd.function.once_differentiable
-    def backward(ctx, dctx, dalpha):
-        need = ctx.needs_input_grad
-        denc, dh, grads = ctx.att._backward_impl(ctx.saved_tensors, ctx.meta, dctx, dalpha, need[1], need[2], need[3:])
-        return (None, denc, dh) + tuple(grads)
+from ._lib import check, dtype_code, impl_code, ptr, stream_ptr
+from .kernel_module import kernel_forward, stamp
+from .params import FlatStore, LRUCache, ParamHolder, grad_view
 
 
 def decoder_specs(A, E, D, V, C):
@@ -110,22 +68,15 @@ class Attention(nn.Module):
         """With grad mode on and ``encoder_out``, ``decoder_hidden`` or a parameter requiring grad, an autograd graph is
         recorded: ``context`` and ``alpha`` are differentiable, and their backward is lo_attention_step_backward.  The outputs
         are the same either way."""
-        if not encoder_out.is_cuda:
-            raise _lib.LatexOcrB200Error("Attention runs on CUDA tensors only (no CPU fallback)")
-        params = list(self.parameters())
-        if torch.is_grad_enabled() and (encoder_out.requires_grad or decoder_hidden.requires_grad
-                                        or any(p.requires_grad for p in params)):
-            return _AttentionFunction.apply(self, encoder_out, decoder_hidden, *params)
-        with torch.no_grad():
-            return self._forward_impl(encoder_out, decoder_hidden, need_grad=False)[:2]
+        return kernel_forward(self, (encoder_out, decoder_hidden), (encoder_out, decoder_hidden))[0]
 
     def _forward_impl(self, encoder_out, decoder_hidden, need_grad):
-        """(context, alpha, what the backward of this call needs or None).  att1 is computed per call, as the reference does
-        (seq2seq_torch.py:186), and kept with att2 for the backward."""
+        """((context, alpha), None, what the backward of this call needs or None).  att1 is computed per call, as the reference
+        does (seq2seq_torch.py:186), and kept with att2 for the backward."""
         L = _lib.lib()
         with torch.no_grad():
-            S, st, dt = self.store, stream_ptr(), _dt(self.precision)
-            S.sync_shadow()
+            S, st, dt = self.store, stream_ptr(), dtype_code(self.precision)
+            S.refresh_shadow()
             B, R, C = encoder_out.shape
             A, D = self.attention_dim, self.decoder_dim
             enc = encoder_out.contiguous().to(self.tdtype)
@@ -148,18 +99,20 @@ class Attention(nn.Module):
                 # the caller's tensors are kept, not the storage-dtype / fp32 copies the kernels read: in a per-step loop the
                 # enc[:bt] slices share one tensor, whereas a bf16 copy per call (57 MB at cfg #2) would double what the loop
                 # holds; the backward redoes the same deterministic conversion (one cast per call)
-                saved = {"enc": encoder_out, "h": decoder_hidden, "att1": att1, "att2": att2,
+                saved = {"tensors": (encoder_out, decoder_hidden, att1, att2, ctx, alpha),
                          "meta": {"version": S.master._version, "enc_shape": tuple(encoder_out.shape), "enc_dtype": encoder_out.dtype,
                                   "h_shape": tuple(decoder_hidden.shape), "h_dtype": decoder_hidden.dtype}}
-            return ctx, alpha, saved
+            return (ctx, alpha), None, saved
 
+    # the parameters in the order of lo_attention_step_backward's gradient arguments (and of self.parameters())
     _GRAD_NAMES = ("encoder_att.weight", "encoder_att.bias", "decoder_att.weight", "decoder_att.bias", "full_att.weight",
                    "full_att.bias")
 
-    def _backward_impl(self, saved_tensors, meta, dctx, dalpha, need_enc, need_h, need_params):
-        """lo_attention_step_backward: returns (d encoder_out or None, d decoder_hidden or None, [gradient or None per
-        parameter]), each in the shape and dtype of what it is the gradient of."""
-        enc, h, att1, att2, ctx, alpha = saved_tensors
+    def _backward_impl(self, saved, dctx, dalpha, need):
+        """lo_attention_step_backward: returns (d encoder_out or None, d decoder_hidden or None), each in the shape and dtype of
+        what it is the gradient of; the parameter gradients ``need`` asks for land in ``store.grad``."""
+        enc, h, att1, att2, ctx, alpha = saved["tensors"]
+        meta = saved["meta"]
         S = self.store
         if S.master._version != meta["version"]:
             raise _lib.LatexOcrB200Error("Attention backward: a parameter was modified in place after the forward; run backward "
@@ -169,32 +122,28 @@ class Attention(nn.Module):
         B, R, C = enc.shape
         A, D = self.attention_dim, self.decoder_dim
         dev = enc.device
-        named = dict(self.named_parameters())
-        if dctx is None and dalpha is None:
-            return None, None, [None] * len(need_params)
         f32 = torch.float32
         dctx = dctx.float().contiguous() if dctx is not None else torch.zeros(B, C, dtype=f32, device=dev)
         dal = dalpha.float().contiguous() if dalpha is not None else None
-        grads = [torch.empty(named[n].shape, dtype=f32, device=dev) if need else None
-                 for n, need in zip(self._GRAD_NAMES, need_params)]
-        denc = torch.empty(B, R, C, dtype=f32, device=dev) if need_enc else None
-        dh = torch.empty(B, D, dtype=f32, device=dev) if need_h else None
+        named = dict(self.named_parameters())
+        grads = [ptr(grad_view(S, named[n])) if nd else None for n, nd in zip(self._GRAD_NAMES, need[2:])]
+        denc = torch.empty(B, R, C, dtype=f32, device=dev) if need[0] else None
+        dh = torch.empty(B, D, dtype=f32, device=dev) if need[1] else None
         L = _lib.lib()
-        dt = _dt(self.precision)
+        dt = dtype_code(self.precision)
         nbytes = L.lo_attention_step_workspace_bytes(B, R, A, C, dt)
         if self._bwork is None or self._bwork.numel() < nbytes:
             self._bwork = torch.zeros(nbytes, dtype=torch.uint8, device=dev)
-        impl = _lib.LO_IMPL_TC if (self.impl == "tc" and self.precision == "bf16") else _lib.LO_IMPL_SIMT
         check(L.lo_attention_step_backward(
             ptr(enc), ptr(att1), dt, ptr(h), ptr(att2), ptr(S.w("attention.encoder_att.weight")),
             ptr(S.w("attention.decoder_att.weight")), ptr(S.f32("attention.full_att.weight")), ptr(alpha), ptr(ctx), ptr(dctx),
-            ptr(dal), ptr(denc), ptr(dh), *[ptr(g) for g in grads], None, None, None, B, R, A, C, D, impl, ptr(self._bwork),
-            stream_ptr()))
+            ptr(dal), ptr(denc), ptr(dh), *grads, None, None, None, B, R, A, C, D, impl_code(self.impl, self.precision),
+            ptr(self._bwork), stream_ptr()))
         if denc is not None:
             denc = denc.view(meta["enc_shape"]).to(meta["enc_dtype"])
         if dh is not None:
             dh = dh.view(meta["h_shape"]).to(meta["h_dtype"])
-        return denc, dh, grads
+        return denc, dh
 
 
 class DecoderWithAttention(nn.Module):
@@ -225,8 +174,6 @@ class DecoderWithAttention(nn.Module):
             setattr(self, n, h)
         self.reset_parameters()
         self._ws = LRUCache()     # bounded: see params.LRUCache
-        self._shadow_fresh = False
-        self._shadow_version = -1
         # in-kernel dropout (has_dropout=2): device {seed, call counter}; the counter is advanced by lo_decoder_backward, so
         # CUDA-graph replays draw a fresh mask every step
         self.dropout_state = torch.tensor([int(torch.initial_seed()) & 0x7FFFFFFFFFFFFFFF, 0], dtype=torch.int64, device=device)
@@ -253,7 +200,6 @@ class DecoderWithAttention(nn.Module):
             self.embedding.weight.normal_(0, 1)
             lin(self.fc, D)
         self.init_weights()
-        self._shadow_fresh = False
 
     def init_weights(self):
         """seq2seq_torch.py:230-236."""
@@ -261,31 +207,16 @@ class DecoderWithAttention(nn.Module):
             self.embedding.weight.uniform_(-0.1, 0.1)
             self.fc.bias.fill_(0)
             self.fc.weight.uniform_(-0.1, 0.1)
-        self._shadow_fresh = False
 
     def load_pretrained_embeddings(self, embeddings):
         """seq2seq_torch.py:238-244 (copies into the flat store instead of re-pointing the Parameter)."""
         with torch.no_grad():
             self.embedding.weight.copy_(embeddings)
-        self._shadow_fresh = False
 
     def fine_tune_embeddings(self, fine_tune=True):
         """seq2seq_torch.py:246-253."""
         for p in self.embedding.parameters():
             p.requires_grad = fine_tune
-
-    def _load_from_state_dict(self, *a, **k):
-        super()._load_from_state_dict(*a, **k)
-        self._shadow_fresh = False
-
-    def sync_shadow(self):
-        # in-place edits of the parameters (torch.optim steps, load_state_dict, p.copy_) move the version counter that the
-        # views share with store.master; the fused Adam writes the shadow itself and leaves the counter alone
-        v = self.store.master._version
-        if not self._shadow_fresh or v != self._shadow_version:
-            self.store.sync_shadow()
-            self._shadow_fresh = True
-            self._shadow_version = v
 
     # ---------------------------------------------------------------------------------------------
     def workspace(self, B, T, R, need_grad):
@@ -323,9 +254,8 @@ class DecoderWithAttention(nn.Module):
             t["work"] = z(int(_lib.lib().lo_decoder_workspace_bytes(B, max(A, C))), dtype=torch.uint8)
             t["dropout_mask"] = None             # [B,T,D] allocated on first use of an injected mask
             ws["bt"] = (ctypes.c_int32 * T)(*([B] * T))
-            ws["gen"] = 0
             self._ws[key] = ws
-        ws["gen"] += 1         # every caller overwrites the forward state: a pending autograd backward of it must refuse to run
+        stamp(ws)              # every caller overwrites the forward state: a pending autograd backward of it must refuse to run
         if need_grad and not ws["need_grad"]:
             t = ws["t"]
             t["wbwd1"] = z(C + D, G, dtype=self.tdtype)
@@ -357,8 +287,8 @@ class DecoderWithAttention(nn.Module):
         a = _lib.DecoderArgs()
         a.B, a.T, a.R = B, T, R
         a.C, a.A, a.D, a.E, a.V = self.encoder_dim, self.attention_dim, self.decoder_dim, self.embed_dim, self.vocab_size
-        a.dt = _dt(self.precision)
-        a.impl = _lib.LO_IMPL_TC if (self.impl == "tc" and self.precision == "bf16") else _lib.LO_IMPL_SIMT
+        a.dt = dtype_code(self.precision)
+        a.impl = impl_code(self.impl, self.precision)
         a.has_dropout = int(has_dropout)           # 0 eval, 1 injected mask, 2 in-kernel Philox
         a.dropout_state = self.dropout_state.data_ptr()
         a.dropout_p = float(self.dropout_p)
@@ -419,8 +349,8 @@ class DecoderWithAttention(nn.Module):
         """seq2seq_torch.py:255-265 (stand-alone; the fused path computes it inside lo_decoder_forward)."""
         L = _lib.lib()
         with torch.no_grad():
-            S, st, dt = self.store, stream_ptr(), _dt(self.precision)
-            self.sync_shadow()
+            S, st, dt = self.store, stream_ptr(), dtype_code(self.precision)
+            S.refresh_shadow()
             m = encoder_out.float().mean(dim=1).contiguous()      # plumbing; the hot path uses mean_rows_kernel
             B, C, D = m.shape[0], self.encoder_dim, self.decoder_dim
             hc = torch.empty(2, B, D, dtype=torch.float32, device=m.device)
@@ -452,7 +382,7 @@ class DecoderWithAttention(nn.Module):
         B, R, _ = enc_flat.shape
         T = max(decode_lengths)
         ws = self.workspace(B, T, R, need_grad)
-        self.sync_shadow()
+        self.store.refresh_shadow()
         ws["t"]["caps"].copy_(caps_sorted[:, :T + 1])
         self.set_lengths(ws, decode_lengths, B, T)
         has_do = 0 if dropout_mask is None else (2 if isinstance(dropout_mask, str) else 1)
@@ -490,33 +420,46 @@ class DecoderWithAttention(nn.Module):
         sorted captions, decode_lengths(list), alphas[B,maxT,R], sort_ind).  With grad mode on and ``encoder_out`` or a
         parameter requiring grad, an autograd graph is recorded: ``predictions`` and ``alphas`` are differentiable (any loss of
         them), and their backward runs lo_decoder_backward in its generic mode.  The outputs are the same either way."""
-        if not encoder_out.is_cuda:
-            raise _lib.LatexOcrB200Error("DecoderWithAttention runs on CUDA tensors only (no CPU fallback)")
-        params = list(self.parameters())
-        if torch.is_grad_enabled() and (encoder_out.requires_grad or any(p.requires_grad for p in params)):
-            rest = {}
-            preds, alphas = _DecoderFunction.apply(self, rest, encoder_out, encoded_captions, caption_lengths, *params)
-            caps, decode_lengths, sort_ind = rest["out"]
-            return preds, caps, decode_lengths, alphas, sort_ind
-        with torch.no_grad():
-            return self._forward_impl(encoder_out, encoded_captions, caption_lengths, need_grad=False)[:5]
+        (preds, alphas), (caps, decode_lengths, sort_ind) = kernel_forward(self, (encoder_out, encoded_captions, caption_lengths),
+                                                                           (encoder_out,))
+        return preds, caps, decode_lengths, alphas, sort_ind
 
     def _forward_impl(self, encoder_out, encoded_captions, caption_lengths, need_grad):
-        """The forward outputs, plus (need_grad) what the backward of this call needs."""
+        """((predictions, alphas), (captions, decode_lengths, sort_ind), what the backward of this call needs or None)."""
+        enc, caps, decode_lengths, sort_ind = self._sorted_inputs(encoder_out, encoded_captions, caption_lengths)
+        mask = self.make_dropout_mask(enc.shape[0], max(decode_lengths))
+        ws = self.run_forward(enc, caps, decode_lengths, with_loss=False, need_grad=need_grad, dropout_mask=mask)
+        return self._outputs(ws, encoder_out, enc, caps, decode_lengths, sort_ind, mask, need_grad)
+
+    def _backward_impl(self, saved, dpreds, dalphas, need):
+        """lo_decoder_backward in its generic mode: returns (d encoder_out in the caller's row order and shape,)."""
+        a, keep = self._generic_backward_args(saved, dpreds)
+        dal = dalphas.float().contiguous() if dalphas is not None else None
+        if dal is not None:
+            a.dalpha_ext = dal.data_ptr()
+        check(_lib.lib().lo_decoder_backward(ctypes.byref(a), stream_ptr()))
+        return (self._scatter_denc(saved),)
+
+    # shared with ext.TwoLayerDecoder, which runs its second layer between phase 1 (time loop) and phase 2 (fc head)
+    def _sorted_inputs(self, encoder_out, encoded_captions, caption_lengths):
+        """seq2seq_torch.py:284-298: (encoder_out as [B,R,C] in storage dtype, captions, decode_lengths, sort_ind), rows sorted by
+        decreasing caption length."""
         B = encoder_out.size(0)
         C = encoder_out.size(-1)
         enc = encoder_out.reshape(B, -1, C)
         lens, sort_ind = caption_lengths.squeeze(1).sort(dim=0, descending=True)     # :286
-        sort_ind_dev = sort_ind.to(enc.device)
-        enc = enc[sort_ind_dev].contiguous().to(self.tdtype)
-        caps = encoded_captions.to(enc.device)[sort_ind_dev].contiguous()
-        decode_lengths = (lens - 1).tolist()                                           # :298
+        sort_ind = sort_ind.to(enc.device)
+        enc = enc[sort_ind].contiguous().to(self.tdtype)
+        caps = encoded_captions.to(enc.device)[sort_ind].contiguous()
+        return enc, caps, (lens - 1).tolist(), sort_ind                             # :298
+
+    def _outputs(self, ws, encoder_out, enc, caps, decode_lengths, sort_ind, mask, need_grad):
+        """The return value of _forward_impl once the logits and alphas of the forward are in ``ws``."""
         T = max(decode_lengths)
-        mask = self.make_dropout_mask(B, T)
-        # the Philox {seed, call} this forward draws its dropout mask from; the backward regenerates the mask from this copy
-        dstate = self.dropout_state.clone() if need_grad and mask is not None else None
-        ws = self.run_forward(enc, caps, decode_lengths, with_loss=False, need_grad=need_grad, dropout_mask=mask)
-        if isinstance(mask, str):
+        philox = isinstance(mask, str)
+        # the Philox {seed, call} this forward drew its dropout mask from; the backward regenerates the mask from this copy
+        dstate = self.dropout_state.clone() if need_grad and philox else None
+        if philox:
             self.dropout_state[1] += 1       # forward-only call: no lo_decoder_backward to advance the Philox call counter
         preds = ws["t"]["logits"][:, :, :self.vocab_size].clone()
         alphas = ws["t"]["alphas"].clone()
@@ -526,35 +469,29 @@ class DecoderWithAttention(nn.Module):
             alphas = alphas * act[:, :, None]
         saved = None
         if need_grad:
-            saved = {"ws": ws, "gen": ws["gen"], "enc": enc, "sort_ind": sort_ind_dev, "shape": tuple(encoder_out.shape),
-                     "dtype": encoder_out.dtype, "has_do": 0 if mask is None else 2, "dstate": dstate}
-        return preds, caps, decode_lengths, alphas, sort_ind_dev, saved
+            saved = {"entries": [ws], "ws": ws, "enc": enc, "sort_ind": sort_ind, "shape": tuple(encoder_out.shape),
+                     "dtype": encoder_out.dtype, "has_do": 0 if mask is None else (2 if philox else 1), "dstate": dstate}
+        return (preds, alphas), (caps, decode_lengths, sort_ind), saved
 
-    def _backward_impl(self, saved, dpreds, dalphas, need_params):
-        """lo_decoder_backward in its generic mode: returns (d encoder_out in the caller's row order and shape, [gradient or
-        None per parameter])."""
-        ws = saved["ws"]
-        enc = saved["enc"]
+    def _generic_backward_args(self, saved, dpreds):
+        """The argument block of a generic-mode lo_decoder_backward of the forward ``saved`` describes: d predictions and the
+        forward's Philox state.  Returns (args, the tensors it points at, to be kept referenced until the launches)."""
+        ws, enc = saved["ws"], saved["enc"]
         B, R, _ = enc.shape
         T = ws["t"]["hd"].shape[1]
-        if ws["gen"] != saved["gen"]:
-            raise _lib.LatexOcrB200Error(
-                "DecoderWithAttention backward: the saved forward state (B=%d, T=%d, R=%d) was overwritten by a later forward of "
-                "the same shape; run backward before the next forward of that shape" % (B, T, R))
         V = self.vocab_size
         dpred = dpreds.float().contiguous() if dpreds is not None else torch.zeros(B, T, V, device=enc.device)
-        dal = dalphas.float().contiguous() if dalphas is not None else None
-        unbind_grads(self, self.store)           # the kernels overwrite store.grad
-        a = self.fill_args(ws, enc, B, T, R, saved["has_do"], dalpha_ext=dal)
+        a = self.fill_args(ws, enc, B, T, R, saved["has_do"])
         dstate = None
         if saved["dstate"] is not None:
             dstate = saved["dstate"].clone()     # lo_decoder_backward advances the counter it is given
             a.dropout_state = dstate.data_ptr()
-        a.dpred_ext = dpred.data_ptr()
+        a.dpred_ext = dpred.data_ptr()           # also the generic-mode flag
         a.dpred_stride = V
-        check(_lib.lib().lo_decoder_backward(ctypes.byref(a), stream_ptr()))
-        denc = ws["t"]["denc"]
+        return a, (dpred, dstate)
+
+    def _scatter_denc(self, saved):
+        """d encoder_out in the caller's row order, shape and dtype."""
+        denc = saved["ws"]["t"]["denc"]
         dx = torch.empty_like(denc).index_copy_(0, saved["sort_ind"], denc)
-        dx = dx.view(saved["shape"]).to(saved["dtype"])
-        grads = [grad_view(self.store, p).clone() if need else None for p, need in zip(self.parameters(), need_params)]
-        return dx, grads
+        return dx.view(saved["shape"]).to(saved["dtype"])

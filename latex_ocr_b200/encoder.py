@@ -12,8 +12,9 @@ import torch
 import torch.nn as nn
 
 from . import _lib
-from ._lib import check, ptr, stream_ptr
-from .params import FlatStore, LRUCache, ParamHolder, grad_view, unbind_grads
+from ._lib import check, dtype_code, impl_code, ptr, stream_ptr
+from .kernel_module import kernel_forward, stamp
+from .params import FlatStore, LRUCache, ParamHolder
 
 # (sequential index, Cin, Cout, pad, pool after)    seq2seq_torch.py:35-56
 _LAYERS = (("0", 1, 64, 1, (2, 2)), ("3", 64, 128, 1, (2, 2)), ("6", 128, 256, 1, None),
@@ -42,10 +43,6 @@ def timing_signal_table(channels, height, width, device):
         lo = dim * 2 * nts
         table[lo:lo + 2 * nts] += sig[:, :, None] if dim == 0 else sig[:, None, :]
     return table.permute(1, 2, 0).contiguous().to(device)
-
-
-def _dt(precision):
-    return _lib.LO_F32 if precision == "fp32" else _lib.LO_BF16
 
 
 class EncoderCNN(nn.Module):
@@ -81,8 +78,6 @@ class EncoderCNN(nn.Module):
             self.cnn[idx] = h
         self.reset_parameters()
         self._ws = LRUCache()     # bounded: see params.LRUCache
-        self._shadow_fresh = False
-        self._shadow_version = -1
 
     # nn.Conv2d default init (kaiming_uniform(a=sqrt(5)) == U(-1/sqrt(fan_in), 1/sqrt(fan_in)))
     def reset_parameters(self):
@@ -93,7 +88,6 @@ class EncoderCNN(nn.Module):
                 b = 1.0 / math.sqrt(cin * R * S_)
                 self.cnn[idx].weight.uniform_(-b, b)
                 self.cnn[idx].bias.uniform_(-b, b)
-        self._shadow_fresh = False
 
     def fine_tune(self, fine_tune=True):
         """seq2seq_torch.py:102-113."""
@@ -102,10 +96,6 @@ class EncoderCNN(nn.Module):
         for idx in list(self.cnn.keys())[2:]:      # children()[5:] of the Sequential == convs from index 6 on
             for p in self.cnn[idx].parameters():
                 p.requires_grad = fine_tune
-
-    def _load_from_state_dict(self, *a, **k):
-        super()._load_from_state_dict(*a, **k)
-        self._shadow_fresh = False
 
     def out_hw(self, H, W):
         h, w = H, W
@@ -157,15 +147,7 @@ class EncoderCNN(nn.Module):
         return ws
 
     def _impl(self):
-        return _lib.LO_IMPL_TC if (self.impl == "tc" and self.precision == "bf16") else _lib.LO_IMPL_SIMT
-
-    def sync_shadow(self):
-        # resync after in-place edits of the parameters (see DecoderWithAttention.sync_shadow)
-        v = self.store.master._version
-        if not self._shadow_fresh or v != self._shadow_version:
-            self.store.sync_shadow()
-            self._shadow_fresh = True
-            self._shadow_version = v
+        return impl_code(self.impl, self.precision)
 
     def forward_raw(self, img, need_grad=False):
         """img: CUDA float32 or uint8 [N,1,H,W] (raw 0..255 like img2seq_torch.py:115-117; uint8 = 4x less H2D traffic).  Returns the
@@ -179,10 +161,9 @@ class EncoderCNN(nn.Module):
             img = img.float()
         img = img.contiguous()
         N, _, H, W = img.shape
-        ws = self._workspace(N, H, W, need_grad)
-        ws["gen"] = ws.get("gen", 0) + 1      # this call overwrites the forward state: a pending autograd backward of it must refuse
-        self.sync_shadow()
-        st, dt, impl, S = stream_ptr(), _dt(self.precision), self._impl(), self.store
+        ws = stamp(self._workspace(N, H, W, need_grad))     # this call overwrites the forward state of a pending backward
+        self.store.refresh_shadow()
+        st, dt, impl, S = stream_ptr(), dtype_code(self.precision), self._impl(), self.store
         A = ws["acts"]
         ws["img"] = img
         sc, of = (1.0 / 128.0, -1.0) if self.input_norm == "tf" else (1.0, 0.0)
@@ -246,7 +227,7 @@ class EncoderCNN(nn.Module):
                                              "forward (forward_raw(img, need_grad=True)); this workspace has none")
             if dimg.dtype != torch.float32 or not dimg.is_contiguous() or dimg.numel() != N * H * W:
                 raise ValueError("dimg must be a contiguous float32 tensor of N*H*W elements")
-        st, dt, impl, S = stream_ptr(), _dt(self.precision), self._impl(), self.store
+        st, dt, impl, S = stream_ptr(), dtype_code(self.precision), self._impl(), self.store
         A, G = ws["acts"], ws["grads"]
         for l in self.layers[1:]:
             idx, cin, cout = l[:3]
@@ -316,36 +297,20 @@ class EncoderCNN(nn.Module):
         """Reference signature (seq2seq_torch.py:88-100): returns a new fp32 tensor [N,H',W',512].  With grad mode on and the
         image or a parameter requiring grad, an autograd graph is recorded whose backward runs ``backward_raw``; the output is
         the same either way.  The image gradient is returned in the image's shape and dtype."""
-        params = list(self.parameters())
-        if torch.is_grad_enabled() and (img.requires_grad or any(p.requires_grad for p in params)):
-            return _EncoderFunction.apply(self, img, *params)
-        with torch.no_grad():
-            return self.forward_raw(img, need_grad=False).float()
+        return kernel_forward(self, (img,), (img,))[0][0]
 
-
-class _EncoderFunction(torch.autograd.Function):
-    """Autograd node of EncoderCNN.forward: inputs (module, img, *parameters), output the encoder output."""
-
-    @staticmethod
-    def forward(ctx, enc, img, *params):
-        out = enc.forward_raw(img, need_grad=True)
+    def _forward_impl(self, img, need_grad):
+        """((encoder output,), None, what the backward of this call needs or None)."""
+        out = self.forward_raw(img, need_grad=need_grad)
+        if not need_grad:
+            return (out.float(),), None, None
         N, _, H, W = img.shape
-        ctx.enc, ctx.ws, ctx.shape, ctx.img_dtype = enc, enc._ws.get((N, H, W)), tuple(img.shape), img.dtype
-        ctx.gen = ctx.ws["gen"]
-        return out.to(torch.float32, copy=True)        # never the workspace buffer itself: each call's output has its own node
+        ws = self._ws.get((N, H, W))
+        # a copy, never the workspace buffer itself: each call's output has its own node
+        return (out.to(torch.float32, copy=True),), None, {"entries": [ws], "ws": ws, "shape": tuple(img.shape), "dtype": img.dtype}
 
-    @staticmethod
-    @torch.autograd.function.once_differentiable
-    def backward(ctx, dout):
-        enc, S = ctx.enc, ctx.enc.store
-        if ctx.ws["gen"] != ctx.gen:
-            raise _lib.LatexOcrB200Error("EncoderCNN backward: the saved forward state (image batch %s) was overwritten by a later "
-                                         "forward of the same shape; run backward before the next forward of that shape"
-                                         % (ctx.shape,))
-        unbind_grads(enc, S)                      # the kernels overwrite store.grad
-        dimg = torch.empty(ctx.shape, dtype=torch.float32, device=dout.device) if ctx.needs_input_grad[1] else None
-        enc.backward_raw(ctx.shape, dout.float().contiguous(), ws=ctx.ws, dimg=dimg)
-        if dimg is not None and dimg.dtype != ctx.img_dtype:
-            dimg = dimg.to(ctx.img_dtype)
-        return (None, dimg) + tuple(grad_view(S, p).clone() if need else None
-                                    for p, need in zip(enc.parameters(), ctx.needs_input_grad[2:]))
+    def _backward_impl(self, saved, dout, need):
+        """backward_raw on the workspace of the forward: returns (d img in the image's shape and dtype, or None,)."""
+        dimg = torch.empty(saved["shape"], dtype=torch.float32, device=dout.device) if need[0] else None
+        self.backward_raw(saved["shape"], dout.float().contiguous(), ws=saved["ws"], dimg=dimg)
+        return (dimg.to(saved["dtype"]) if dimg is not None else None,)

@@ -200,8 +200,7 @@ class Img2SeqModel:
             for S, sn in zip(stores, snap):
                 for k, v in sn.items():
                     getattr(S, k).copy_(v)
-            for m_ in self._param_modules():
-                m_._shadow_version = m_.store.master._version    # the restore put the shadows back too: no resync in the capture
+                S.mark_shadow_current()          # the restore put the shadow back too: no re-cast inside the capture
             graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(graph):
                 mask = self.decoder.make_dropout_mask(N, T)
@@ -377,8 +376,6 @@ class Img2SeqModel:
         self.encoder.load_state_dict(sd["encoder"])
         self.decoder.load_state_dict(sd["decoder"])
         self._graphs.clear()                         # captured steps hold the old bf16 shadows' VALUES only through memory
-        self.encoder._shadow_fresh = False           # that stays valid, but force the shadows to be rebuilt from the masters
-        self.decoder._shadow_fresh = False
 
     def save(self, path=None):
         path = path or os.path.join(self._dir_output or ".", "model.pt")

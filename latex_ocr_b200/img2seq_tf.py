@@ -151,8 +151,6 @@ class Img2SeqModel:
             S = m.store
             check(fn(kind, ptr(S.master), ptr(S.grad), ptr(S.m), ptr(S.v), ptr(S.shadow), S.numel, ptr(S.adam_state), b1, b2, eps,
                      float(scale), stream_ptr()))
-            m._shadow_fresh = True                                          # the fused update refreshed the bf16 shadow
-            m._shadow_version = m.store.master._version                     # ... and left the version counter alone: no resync
 
     def train_step(self, images, formulas, dropout=1.0):
         """One update (img2seq.py:163-170).  Returns the device loss vector [mean CE, mean CE, 0, n_words]."""

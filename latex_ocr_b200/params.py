@@ -54,6 +54,7 @@ class FlatStore:
         self.v = None
         self.shadow = torch.zeros(off, dtype=torch.bfloat16, device=self.device) if bf16_shadow else None
         self.adam_state = None   # device float[2]: step, lr
+        self._shadow_version = None   # master._version the shadow was last cast from (None: never, or stale)
 
     def view(self, buf, name):
         off, n, shape = self.offsets[name]
@@ -79,8 +80,21 @@ class FlatStore:
         self.adam_state[1] = float(lr)
 
     def sync_shadow(self):
+        """Re-cast the bf16 shadow from the fp32 master (e.g. after the master was written behind torch's back by NCCL)."""
         if self.shadow is not None:
             self.shadow.copy_(self.master)   # plumbing cast (fp32 -> bf16, round-to-nearest-even)
+        self._shadow_version = self.master._version
+
+    def refresh_shadow(self):
+        """Re-cast the shadow if the master changed since the last cast; every kernel-backed forward calls this.  In-place edits
+        of the parameters (``p.mul_``, ``load_state_dict``, ``torch.optim`` steps) move the version counter that the parameter
+        views share with ``master``.  The fused optimisers write the shadow themselves and leave the counter alone."""
+        if self._shadow_version != self.master._version:
+            self.sync_shadow()
+
+    def mark_shadow_current(self):
+        """Master and shadow were just written together (restored from a snapshot): the shadow needs no re-cast."""
+        self._shadow_version = self.master._version
 
     def to_(self, device):
         device = torch.device(device)
@@ -91,6 +105,7 @@ class FlatStore:
             if t is not None:
                 setattr(self, k, t.to(device))
         self.device = device
+        self._shadow_version = None
 
 
 class ParamHolder(nn.Module):
@@ -107,6 +122,7 @@ class ParamHolder(nn.Module):
             gv = gv.permute(*permute)
         p = nn.Parameter(v, requires_grad=True)
         p.grad = gv
+        p._lo_store = store
         p._lo_store_name = sname
         p._lo_permute = permute
         self.register_parameter(pname, p)
@@ -127,10 +143,13 @@ def bind_grads(module, store):
             p.grad = grad_view(store, p)
 
 
-def unbind_grads(module, store):
-    """Give every ``.grad`` that aliases ``store.grad`` memory of its own (same values), so that kernels may overwrite
-    ``store.grad`` while autograd accumulates into ``p.grad``."""
-    sp = store.grad.untyped_storage().data_ptr()
-    for p in module.parameters():
-        if p.grad is not None and p.grad.untyped_storage().data_ptr() == sp:
+def kernel_grads(params, need, backward):
+    """Runs ``backward()``, whose kernels write the gradients of ``params`` (from one or several stores) into their stores' flat
+    ``grad`` buffers, and returns (its result, [a copy of the gradient of each parameter, None where ``need`` is false]).  Every
+    ``p.grad`` that aliases a store's buffer first gets memory of its own (same values), so what autograd has accumulated there
+    survives the kernels."""
+    for p in params:
+        if p.grad is not None and p.grad.untyped_storage().data_ptr() == p._lo_store.grad.untyped_storage().data_ptr():
             p.grad = p.grad.clone()
+    out = backward()
+    return out, [grad_view(p._lo_store, p).clone() if n else None for p, n in zip(params, need)]

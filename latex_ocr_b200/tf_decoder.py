@@ -24,65 +24,12 @@ import torch
 import torch.nn as nn
 
 from . import _lib
-from ._lib import check, stream_ptr
-from .params import FlatStore, LRUCache, ParamHolder, bind_grads, grad_view, unbind_grads
+from ._lib import TfDecArgs, check, dtype_code, impl_code, stream_ptr
+from .kernel_module import kernel_forward, stamp
+from .params import FlatStore, LRUCache, ParamHolder, bind_grads
 
 DecoderOutput = collections.namedtuple("DecoderOutput", ("logits", "ids"))      # greedy_decoder_cell.py:5-6
-
-
-class _TfDecoderFunction(torch.autograd.Function):
-    """Autograd node of Decoder.train_outputs: inputs (module, enc, formula, keep_h, keep_o, *parameters), differentiable outputs
-    (logits, alphas)."""
-
-    @staticmethod
-    def forward(ctx, dec, enc, formula, keep_h, keep_o, *params):
-        logits, alphas, saved = dec._train_outputs_impl(enc, formula, keep_h, keep_o, need_grad=True)
-        ctx.dec, ctx.saved = dec, saved
-        ctx.set_materialize_grads(False)         # an output the loss does not use arrives as None: no d alpha pass for it
-        return logits, alphas
-
-    @staticmethod
-    @torch.autograd.function.once_differentiable
-    def backward(ctx, dlogits, dalphas):
-        dx, grads = ctx.dec._backward_impl(ctx.saved, dlogits, dalphas, ctx.needs_input_grad[5:])
-        return (None, dx if ctx.needs_input_grad[1] else None, None, None, None) + tuple(grads)
-
-
-def _make_args_struct():
-    with open(_lib.HEADER) as f:
-        text = f.read()
-
-    class TfDecArgs(ctypes.Structure):
-        _fields_ = _lib._parse_struct(text, "lo_tfdec_args")
-
-    return TfDecArgs
-
-
-TfDecArgs = _make_args_struct()
-_bound = False
-
-
-def _bind():
-    global _bound
-    L = _lib.lib()
-    if _bound:
-        return L
-    vp, i32, i64 = ctypes.c_void_p, ctypes.c_int, ctypes.c_int64
-    P = ctypes.POINTER(TfDecArgs)
-    L.lo_sizeof_tfdec_args.restype = i64
-    if L.lo_sizeof_tfdec_args() != ctypes.sizeof(TfDecArgs):
-        raise _lib.LatexOcrB200Error("lo_tfdec_args layout mismatch: library %d bytes, ctypes mirror %d bytes — rebuild"
-                                     % (L.lo_sizeof_tfdec_args(), ctypes.sizeof(TfDecArgs)))
-    L.lo_tfdec_workspace_bytes.restype = i64
-    L.lo_tfdec_workspace_bytes.argtypes = [P]
-    for name, argtypes in (("lo_tfdec_forward", [P, i32, vp]), ("lo_tfdec_backward", [P, vp]),
-                           ("lo_tfdec_greedy", [P, i64, i32, vp, vp, vp]), ("lo_tfdec_beam", [P, i64, i32, vp, vp, vp, vp, vp]),
-                           ("lo_tfdec_beam_div", [P, i64, i32, vp, vp, vp, vp, ctypes.c_float, ctypes.c_float, vp, vp, vp])):
-        fn = getattr(L, name)
-        fn.argtypes = argtypes
-        fn.restype = ctypes.c_int
-    _bound = True
-    return L
+_bind = _lib.lib          # the library with the lo_tfdec_* signatures set (lib() binds them along with the rest)
 
 
 def tf_decoder_specs(V, C, A, D, O, E):
@@ -140,8 +87,6 @@ class Decoder(nn.Module):
             bind(self, n, S, n)
         self.reset_parameters()
         self._ws = LRUCache()     # bounded: see params.LRUCache
-        self._shadow_fresh = False
-        self._shadow_version = -1
 
     # tf.get_variable / tf.layers.dense default: glorot_uniform; LSTMCell bias zeros; embeddings decoder.py:98-105
     def reset_parameters(self):
@@ -160,7 +105,6 @@ class Decoder(nn.Module):
             for p in (self.embedding_table, self.start_token):
                 p.uniform_(-1.0, 1.0)
                 p.copy_(torch.nn.functional.normalize(p, dim=-1))
-        self._shadow_fresh = False
 
     def load_tf_variables(self, d):
         """d: name -> tensor in the TF shapes (module docstring); ``att_beta`` may be [A,1]."""
@@ -168,26 +112,12 @@ class Decoder(nn.Module):
         with torch.no_grad():
             for k, v in d.items():
                 sd[k].copy_(v.reshape(sd[k].shape))
-        self._shadow_fresh = False
-
-    def _load_from_state_dict(self, *a, **k):
-        super()._load_from_state_dict(*a, **k)
-        self._shadow_fresh = False
-
-    def sync_shadow(self):
-        # in-place edits of the parameters (torch.optim steps, load_state_dict, p.copy_) move the version counter that the views
-        # share with store.master; the fused optimizer step writes the shadow itself and records the version
-        v = self.store.master._version
-        if not self._shadow_fresh or v != self._shadow_version:
-            self.store.sync_shadow()
-            self._shadow_fresh = True
-            self._shadow_version = v
 
     # ---------------------------------------------------------------------------------------------
     def _args(self, enc, B, T, R, rows_per_img=1, decode=False):
         """Args and workspace of one shape.  Decoding has workspaces of its own, so a decode never overwrites the saved state of
         a teacher-forced pass whose autograd backward is still to run (Decoder.forward runs both)."""
-        L = _bind()
+        L = _lib.lib()
         key = (B, T, R, rows_per_img, "decode") if decode else (B, T, R, rows_per_img)
         ws = self._ws.get(key)
         dev = self.store.device
@@ -199,14 +129,13 @@ class Decoder(nn.Module):
             ws["denc"] = torch.zeros(B // rows_per_img, R, self.C, dtype=torch.float32, device=dev)
             ws["formula"] = torch.zeros(B, T, dtype=torch.int64, device=dev)
             ws["lengths"] = torch.zeros(B, dtype=torch.int32, device=dev)
-            ws["gen"] = 0
             self._ws[key] = ws
-        ws["gen"] += 1         # every caller overwrites the forward state: a pending autograd backward of it must refuse to run
+        stamp(ws)              # every caller overwrites the forward state: a pending autograd backward of it must refuse to run
         S = self.store
         a = TfDecArgs()
         a.B, a.T, a.R, a.C, a.A, a.D, a.O, a.E, a.V = B, T, R, self.C, self.A, self.D, self.O, self.E, self.V
-        a.dt = _lib.LO_F32 if self.precision == "fp32" else _lib.LO_BF16
-        a.impl = _lib.LO_IMPL_TC if (self.impl == "tc" and self.precision == "bf16") else _lib.LO_IMPL_SIMT
+        a.dt = dtype_code(self.precision)
+        a.impl = impl_code(self.impl, self.precision)
         a.ldl = ws["ldl"]
         a.rows_per_img = rows_per_img
         a.enc = enc.data_ptr()
@@ -249,7 +178,7 @@ class Decoder(nn.Module):
         enc = self._enc(enc)
         B, R, _ = enc.shape
         T = formula.shape[1]
-        self.sync_shadow()
+        self.store.refresh_shadow()
         L, ws, a = self._args(enc, B, T, R)
         ws["enc"] = enc
         ws["formula"].copy_(formula)
@@ -264,7 +193,7 @@ class Decoder(nn.Module):
         return ws
 
     def run_backward(self, ws):
-        check(_bind().lo_tfdec_backward(ctypes.byref(ws["args"]), stream_ptr()))
+        check(_lib.lib().lo_tfdec_backward(ctypes.byref(ws["args"]), stream_ptr()))
         return ws["denc"]
 
     def train_logits(self, enc, formula, keep_h=None, keep_o=None):
@@ -277,14 +206,10 @@ class Decoder(nn.Module):
         autograd graph is recorded: both outputs are differentiable (any loss of them), d enc comes back in ``enc``'s shape and
         dtype, and the backward runs lo_tfdec_backward in its generic mode with the same keep masks.  The outputs are the same
         either way."""
-        params = list(self.parameters())
-        if torch.is_grad_enabled() and (enc.requires_grad or any(p.requires_grad for p in params)):
-            return _TfDecoderFunction.apply(self, enc, formula, keep_h, keep_o, *params)
-        with torch.no_grad():
-            return self._train_outputs_impl(enc, formula, keep_h, keep_o, need_grad=False)[:2]
+        return kernel_forward(self, (enc, formula, keep_h, keep_o), (enc,))[0]
 
-    def _train_outputs_impl(self, enc, formula, keep_h, keep_o, need_grad):
-        """The outputs of train_outputs, plus (need_grad) what the backward of this call needs."""
+    def _forward_impl(self, enc, formula, keep_h, keep_o, need_grad):
+        """((logits, alphas), None, what the backward of this call needs or None)."""
         ws = self.run_forward(enc, formula, None, keep_h, keep_o)
         logits = ws["logits"][:, :, :self.V].permute(1, 0, 2).contiguous()
         alphas = ws["alphas"].clone()
@@ -292,31 +217,23 @@ class Decoder(nn.Module):
         if need_grad:
             # ws["args"] points at ws["enc"] and the keep masks of this call; holding them keeps them alive even if the workspace
             # leaves the cache
-            saved = {"ws": ws, "gen": ws["gen"], "args": ws["args"], "enc": ws["enc"],
+            saved = {"entries": [ws], "ws": ws, "args": ws["args"], "enc": ws["enc"],
                      "keep": (ws["keep_h"] if keep_h is not None else None, ws["keep_o"] if keep_o is not None else None),
                      "shape": tuple(enc.shape), "dtype": enc.dtype}
-        return logits, alphas, saved
+        return (logits, alphas), None, saved
 
-    def _backward_impl(self, saved, dlogits, dalphas, need_params):
-        """lo_tfdec_backward in its generic mode: returns (d enc in the caller's shape and dtype, [gradient or None per
-        parameter])."""
+    def _backward_impl(self, saved, dlogits, dalphas, need):
+        """lo_tfdec_backward in its generic mode: returns (d enc in the caller's shape and dtype,)."""
         ws = saved["ws"]
         B, T, R = ws["alphas"].shape
-        if ws["gen"] != saved["gen"]:
-            raise _lib.LatexOcrB200Error(
-                "Decoder backward: the saved forward state (N=%d, T=%d, R=%d) was overwritten by a later call of the same shape; "
-                "run backward before the next forward of that shape" % (B, T, R))
         dev = self.store.device
         dl = dlogits.float().contiguous() if dlogits is not None else torch.zeros(B, T, self.V, device=dev)
         dal = dalphas.float().contiguous() if dalphas is not None else None
-        unbind_grads(self, self.store)           # the kernels overwrite store.grad
         a = TfDecArgs.from_buffer_copy(saved["args"])
         a.dlogits_ext, a.dlogits_stride = dl.data_ptr(), self.V
         a.dalpha_ext = dal.data_ptr() if dal is not None else None
-        check(_bind().lo_tfdec_backward(ctypes.byref(a), stream_ptr()))
-        dx = ws["denc"].reshape(saved["shape"]).to(saved["dtype"], copy=True)
-        grads = [grad_view(self.store, p).clone() if need else None for p, need in zip(self.parameters(), need_params)]
-        return dx, grads
+        check(_lib.lib().lo_tfdec_backward(ctypes.byref(a), stream_ptr()))
+        return (ws["denc"].reshape(saved["shape"]).to(saved["dtype"], copy=True),)
 
     def loss_and_backward(self, enc, formula, lengths, keep_h=None, keep_o=None, n_words=None):
         """Returns (loss tensor [4] on the device: mean CE, mean CE, 0, n_words; d loss / d enc [N,R,C] fp32).  Parameter
@@ -337,7 +254,7 @@ class Decoder(nn.Module):
         beam = self._tiles
         steps = int(max_steps) if max_steps is not None else self.max_length_formula + 2
         B = N * beam
-        self.sync_shadow()
+        self.store.refresh_shadow()
         with torch.no_grad():
             L, ws, a = self._args(enc, B, steps, R, rows_per_img=beam, decode=True)
             ws["enc"] = enc

@@ -46,17 +46,41 @@ int lo_version(void);
 const char* lo_last_error(void);
 /* number of kernels launched through this library since load (bench.py's gpu_launches) */
 int64_t lo_launch_count(void);
-/* tuning knobs: "att_pipe" (1: TMA-pipelined attention kernels, 0: register-streaming), "att_policy_enc" /
- * "att_policy_att1" (L2 policy 0 normal, 1 evict_last, 2 evict_first), "att_nsplit" (0 = automatic), "pdl", "att_abi_pdl" (above);
- * schedule variants, each parity-tested against the default (tests/test_gpu_tc.py, DESIGN.md §8): "att_maskbits", "att_bwd_mma",
- * "skinny_mma", "skinny_tma", "fuse_lstm", "dec_streams", "dec_fuse", "dec_fuse_bwd", "dec_cl", "dec_cl_bwd", "conv_persist",
- * "conv_mt2", "conv_mc", "wgrad256"; "deterministic" (1: every cross-CTA reduction of the train step
- * adds its partial sums in a fixed order, so a seeded run is bit-reproducible — slower; 0, default: fp32 atomics whose rounding
- * depends on arrival order); "dbg_skip" is a timing-dissection aid (results are garbage).  LO_OPTS=name=value,... in the
- * environment sets them at load time (Python side). */
+/* Run-time options.  lo_set_option sets one by name and accepts any int value (an unknown name is refused with LO_EINVAL);
+ * lo_get_option reads it back (-1: unknown name); lo_option_name(i) is the i-th name, NULL past the last.  From Python,
+ * LO_OPTS=name=value,... in the environment sets them when the library is loaded.  [p]: parity-tested, tests/test_gpu_tc.py or
+ * tests/test_gpu_parity.py runs the other value against the default and requires the same results (measured A/B: DESIGN.md §8).
+ *
+ *   name             default  meaning
+ *   att_pipe         1 [p]    attention step kernels: 1 TMA bulk-copy -> shared-memory ring, 0 register-streaming
+ *   pdl              1        programmatic dependent launch (above); 0 turns it off everywhere
+ *   att_abi_pdl      0        1: the stand-alone attention entry points use it too (the caller vouches for their inputs, above)
+ *   att_policy_enc   1        L2 policy of the attention kernels' enc stream: 0 normal, 1 evict_last, 2 evict_first, 3 no hint
+ *   att_policy_att1  2        the same for their att1 stream
+ *   att_nsplit       0        splits of one batch row in the attention kernels; 0: automatic
+ *   att_cluster      1        1: the splits of a batch row form a thread-block cluster and combine through distributed shared memory
+ *   att_maskbits     1 [p]    1: the forward attention kernel stores the ReLU mask bits, the backward streams them instead of att1
+ *   att_bwd_mma      1 [p]    1: the 512-wide bf16 attention backward runs both contractions on mma.sync
+ *   dec_streams      1 [p]    >= 2: the decoder time loop runs as two half-batch chains on two streams; also sets skinny8 = value < 2
+ *   dec_fuse         0 [p]    1: grid-barrier fused forward step; off: measured no faster than the separate launches
+ *   dec_fuse_bwd     0 [p]    1: grid-barrier fused backward step; off: two grid barriers cost more than two PDL boundaries
+ *   dec_cl           0 [p]    1: cluster-fused forward step; off: slower, each CTA pulls its 320 KB weight slice through one SM
+ *   dec_cl_bwd       0 [p]    1: cluster-fused backward step; off for the same reason
+ *   fuse_lstm        0 [p]    1: LSTM cell in the gates GEMM's epilogue; off: it cannot hide the dependent loads the pointwise kernel hides
+ *   skinny_mma       1 [p]    decoder per-step GEMMs (M <= 64) on mma.sync; 0: on wgmma
+ *   skinny_tma       1 [p]    1: their operands by cp.async.bulk, one copy per row; 0: 16-byte cp.async
+ *   skinny8          1        1: 8-stage (198 KB shared memory) wgmma config for GEMMs with M <= 128; rewritten by dec_streams
+ *   conv_persist     1 [p]    1: persistent double-accumulator convolution kernel; 0: one tile per CTA
+ *   conv_mt2         1 [p]    1: layers with <= 128 output channels: two 128-position sub-tiles per CTA share each weight stage
+ *   conv_mc          1        1: cluster-of-2 multicast of the A tile in the wgmma GEMM
+ *   wgrad256         0 [p]    1: conv weight gradient with 128 x 256 tiles when Cin % 256 == 0; off: two 96 KB stages cannot hide the loads
+ *   deterministic    0        1: cross-CTA sums of the train step add in a fixed order, bit-reproducible but slower; 0: fp32 atomics
+ *   dbg_skip         0        timing aid, results garbage: skips bwd hoisted part (1), loop attention (2), loop GEMM/LSTM (4), fwd hoisted (8)
+ *   l2_persist_mb    0        an action: sets the persisting-L2 set-aside to value MiB (0: driver default); reads back the last value set
+ */
 int lo_set_option(const char* name, int value);
-/* current value of a tuning knob (-1: unknown name) */
 int lo_get_option(const char* name);
+const char* lo_option_name(int i);
 /* L2 persistence: access-policy window of `stream` over [base, base+bytes) (hits persist, misses stream) with the
  * persisting carve-out sized to fit; bytes = 0 resets.  The attention kernels honour it with att_policy_enc/att1 = 3
  * (bulk copies without an explicit cache hint). */

@@ -16,16 +16,6 @@ namespace cg = cooperative_groups;
 
 namespace lo {
 
-int g_opt_att_pipe = 1;
-int g_opt_pdl = 1;               // programmatic dependent launch for the per-step kernels
-int g_opt_att_policy_enc = 1;    // 0 normal, 1 evict_last, 2 evict_first
-int g_opt_att_policy_att1 = 2;
-int g_opt_att_nsplit = 0;        // 0 = automatic
-int g_opt_att_cluster = 1;
-int g_opt_att_abi_pdl = 0;       // 1: the stand-alone attention entry points may use programmatic dependent launch too (bench probes)
-int g_opt_att_bwd_mma = 1;       // 1: 512-wide bf16 backward with both contractions on mma.sync (attention_bwd_mma_kernel)
-int g_opt_att_maskbits = 1;      // 1: the forward attention kernel stores the ReLU mask bits, the backward streams them instead of att1       // 1: the splits of one batch row form a thread-block cluster and combine through DSMEM
-
 #ifndef LO_ATT_RPW
 #define LO_ATT_RPW 2          // rows per consumer warp per stage (bf16): 2 -> 32 KB stages, 2 CTAs/SM ; 1 -> 16 KB stages, 3 CTAs/SM
 #endif
@@ -1473,65 +1463,5 @@ extern "C" int lo_set_l2_window(const void* base, int64_t bytes, float hit_ratio
   lo::g_att_window = v.accessPolicyWindow;
   LO_CUDA(cudaStreamSetAttribute((cudaStream_t)stream, cudaStreamAttributeAccessPolicyWindow, &v));
   lo::fail(LO_OK, "l2 window%s: carve %ld B (device max %ld B)", "", (long)carve, (long)max_persist);      // readable via lo_last_error()
-  return LO_OK;
-}
-
-extern "C" int lo_get_option(const char* name) {
-  if (!name) return -1;
-  if (!strcmp(name, "att_pipe")) return lo::g_opt_att_pipe;
-  if (!strcmp(name, "att_maskbits")) return lo::g_opt_att_maskbits;
-  if (!strcmp(name, "att_bwd_mma")) return lo::g_opt_att_bwd_mma;
-  if (!strcmp(name, "att_abi_pdl")) return lo::g_opt_att_abi_pdl;
-  if (!strcmp(name, "dbg_skip")) return lo::g_opt_dbg_skip;
-  if (!strcmp(name, "conv_mc")) return lo::g_opt_conv_mc;
-  if (!strcmp(name, "att_cluster")) return lo::g_opt_att_cluster;
-  if (!strcmp(name, "pdl")) return lo::g_opt_pdl;
-  if (!strcmp(name, "conv_persist")) return lo::g_opt_conv_persist;
-  if (!strcmp(name, "wgrad256")) return lo::g_opt_wgrad256;
-  if (!strcmp(name, "conv_mt2")) return lo::g_opt_conv_mt2;
-  if (!strcmp(name, "deterministic")) return lo::g_opt_det;
-  if (!strcmp(name, "dec_fuse")) return lo::g_opt_dec_fuse;
-  if (!strcmp(name, "dec_cl")) return lo::g_opt_dec_cl;
-  if (!strcmp(name, "dec_cl_bwd")) return lo::g_opt_dec_cl_bwd;
-  if (!strcmp(name, "dec_fuse_bwd")) return lo::g_opt_dec_fuse_bwd;
-  if (!strcmp(name, "fuse_lstm")) return lo::g_opt_fuse_lstm;
-  if (!strcmp(name, "skinny_mma")) return lo::g_opt_skinny_mma;
-  if (!strcmp(name, "skinny_tma")) return lo::g_opt_skinny_tma;
-  if (!strcmp(name, "dec_streams")) return lo::g_opt_dec_streams;
-  return -1;
-}
-
-extern "C" int lo_set_option(const char* name, int value) {
-  if (!name) return LO_EINVAL;
-  if (!strcmp(name, "att_pipe")) lo::g_opt_att_pipe = value;
-  else if (!strcmp(name, "att_policy_enc")) lo::g_opt_att_policy_enc = value;
-  else if (!strcmp(name, "att_policy_att1")) lo::g_opt_att_policy_att1 = value;
-  else if (!strcmp(name, "att_nsplit")) lo::g_opt_att_nsplit = value;
-  else if (!strcmp(name, "pdl")) lo::g_opt_pdl = value;
-  else if (!strcmp(name, "att_cluster")) lo::g_opt_att_cluster = value;
-  else if (!strcmp(name, "att_maskbits")) lo::g_opt_att_maskbits = value;
-  else if (!strcmp(name, "att_bwd_mma")) lo::g_opt_att_bwd_mma = value;
-  else if (!strcmp(name, "att_abi_pdl")) lo::g_opt_att_abi_pdl = value;
-  else if (!strcmp(name, "dbg_skip")) lo::g_opt_dbg_skip = value;
-  else if (!strcmp(name, "conv_mc")) lo::g_opt_conv_mc = value;
-  else if (!strcmp(name, "conv_persist")) lo::g_opt_conv_persist = value;
-  else if (!strcmp(name, "wgrad256")) lo::g_opt_wgrad256 = value;
-  else if (!strcmp(name, "conv_mt2")) lo::g_opt_conv_mt2 = value;
-  else if (!strcmp(name, "deterministic")) lo::g_opt_det = value;
-  else if (!strcmp(name, "dec_streams")) { lo::g_opt_dec_streams = value; lo::g_opt_skinny8 = value >= 2 ? 0 : 1; }
-  else if (!strcmp(name, "skinny8")) lo::g_opt_skinny8 = value;
-  else if (!strcmp(name, "fuse_lstm")) lo::g_opt_fuse_lstm = value;
-  else if (!strcmp(name, "dec_fuse")) lo::g_opt_dec_fuse = value;
-  else if (!strcmp(name, "dec_cl")) lo::g_opt_dec_cl = value;
-  else if (!strcmp(name, "dec_cl_bwd")) lo::g_opt_dec_cl_bwd = value;
-  else if (!strcmp(name, "dec_fuse_bwd")) lo::g_opt_dec_fuse_bwd = value;
-  else if (!strcmp(name, "skinny_mma")) lo::g_opt_skinny_mma = value;
-  else if (!strcmp(name, "skinny_tma")) lo::g_opt_skinny_tma = value;
-  else if (!strcmp(name, "l2_persist_mb")) {
-    // size of the L2 set-aside that evict_last / persisting accesses may occupy (0 = driver default)
-    cudaError_t e = cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, (size_t)value << 20);
-    if (e != cudaSuccess) return lo::fail(LO_ECUDA, "lo_set_option(l2_persist_mb): %s (%ld)", cudaGetErrorString(e), (long)e);
-  }
-  else return lo::fail(LO_EINVAL, "lo_set_option: unknown option %s", name);
   return LO_OK;
 }

@@ -23,11 +23,6 @@ namespace cg = cooperative_groups;
 
 namespace lo {
 
-// Off by default: each CTA has to pull its 320 KB weight slice through ONE SM's load path, and 4 clusters use only 64 of the
-// 132 SMs, so the fused step was slower than the three separate launches it replaces.
-int g_opt_dec_cl = 0;       // cluster-fused forward step
-int g_opt_dec_cl_bwd = 0;   // cluster-fused backward step
-
 constexpr int CLS = 16;           // CTAs per cluster (non-portable size)
 constexpr int CL_ROWS = 16;       // batch rows per cluster = one mma M tile
 constexpr int CL_THREADS = 256;

@@ -53,9 +53,42 @@ inline int cdiv(long a, long b) { return (int)((a + b - 1) / b); }
 // SMs of the H100 SXM: caps the grids of the grid-stride kernels and sets the split-K / split-count targets
 constexpr int LO_NUM_SMS = 132;
 
+// ---- run-time options ---------------------------------------------------------------------------
+// One entry per option: variable, name taken by lo_set_option / lo_get_option, default.  include/latex_ocr_b200.h documents
+// each one; lo_gemm.cu defines the variables and the name table from this list.
+#define LO_OPTIONS(X)                                                                                           \
+  X(g_opt_att_pipe, "att_pipe", 1)                /* TMA-pipelined attention kernels; 0: register-streaming */ \
+  X(g_opt_pdl, "pdl", 1)                          /* programmatic dependent launch */                         \
+  X(g_opt_att_abi_pdl, "att_abi_pdl", 0)          /* ... also for the stand-alone attention entry points */   \
+  X(g_opt_att_policy_enc, "att_policy_enc", 1)    /* L2 policy of the enc stream */                            \
+  X(g_opt_att_policy_att1, "att_policy_att1", 2)  /* L2 policy of the att1 stream */                           \
+  X(g_opt_att_nsplit, "att_nsplit", 0)            /* attention splits per batch row; 0: automatic */           \
+  X(g_opt_att_cluster, "att_cluster", 1)          /* splits of a batch row combine through DSMEM */            \
+  X(g_opt_att_maskbits, "att_maskbits", 1)        /* ReLU mask bits instead of att1 in the backward */         \
+  X(g_opt_att_bwd_mma, "att_bwd_mma", 1)          /* 512-wide bf16 attention backward on mma.sync */           \
+  X(g_opt_dec_streams, "dec_streams", 1)          /* decoder time loop as two half-batch chains when >= 2 */   \
+  X(g_opt_dec_fuse, "dec_fuse", 0)                /* grid-barrier fused forward step */                        \
+  X(g_opt_dec_fuse_bwd, "dec_fuse_bwd", 0)        /* grid-barrier fused backward step */                       \
+  X(g_opt_dec_cl, "dec_cl", 0)                    /* cluster-fused forward step */                             \
+  X(g_opt_dec_cl_bwd, "dec_cl_bwd", 0)            /* cluster-fused backward step */                            \
+  X(g_opt_fuse_lstm, "fuse_lstm", 0)              /* LSTM cell in the gates GEMM's epilogue */                 \
+  X(g_opt_skinny_mma, "skinny_mma", 1)            /* per-step GEMMs on mma.sync; 0: wgmma */                   \
+  X(g_opt_skinny_tma, "skinny_tma", 1)            /* their operands by cp.async.bulk */                        \
+  X(g_opt_skinny8, "skinny8", 1)                  /* 8-stage wgmma config for M <= 128 */                      \
+  X(g_opt_conv_persist, "conv_persist", 1)        /* persistent double-accumulator conv kernel */              \
+  X(g_opt_conv_mt2, "conv_mt2", 1)                /* two position sub-tiles share a weight stage */            \
+  X(g_opt_conv_mc, "conv_mc", 1)                  /* cluster-of-2 multicast of the A tile */                   \
+  X(g_opt_wgrad256, "wgrad256", 0)                /* 128 x 256 conv weight-gradient tiles */                   \
+  X(g_opt_det, "deterministic", 0)                /* fixed-order cross-CTA sums */                             \
+  X(g_opt_dbg_skip, "dbg_skip", 0)                /* timing dissection: skip launch groups */                  \
+  X(g_opt_l2_persist_mb, "l2_persist_mb", 0)      /* last persisting-L2 set-aside set, MiB */
+
+#define LO_OPTION_EXTERN(var, name, def) extern int var;
+LO_OPTIONS(LO_OPTION_EXTERN)
+#undef LO_OPTION_EXTERN
+
 // kernel launch with (optionally) the programmatic-dependent-launch attribute; kernels launched this way call
 // pdl_wait() before touching global memory
-extern int g_opt_pdl;
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args... args) {
   cudaLaunchConfig_t cfg{};
@@ -252,18 +285,6 @@ struct AttBwdArgs {
   void* datt1 = nullptr;   // optional (ReLU score, no mask_in): [B][R][A] storage-type d att1, written by the same pass
   int ordered_dwf = 0;     // 1: dwf_part must be summed in a fixed order (one split per batch row unless the splits form a cluster)
 };
-extern int g_opt_att_pipe;
-extern int g_opt_att_maskbits;
-extern int g_opt_dbg_skip;
-extern int g_opt_conv_mc;
-extern int g_opt_conv_persist;
-extern int g_opt_wgrad256;
-extern int g_opt_conv_mt2;
-// 1: every cross-CTA reduction of the train step adds its partial sums in a fixed order (thread-block clusters / per-block slots,
-// lo_ptx.cuh:cl_sum) so that a run is bit-reproducible; 0 (default): fp32 atomics, faster, rounding depends on arrival order
-extern int g_opt_det;
-extern int g_opt_dec_streams;
-extern int g_opt_skinny8;
 int attention_fwd_pipe(const AttFwdArgs& x, int dt, int C, cudaStream_t st);
 int attention_bwd_pipe(const AttBwdArgs& x, int dt, int C, cudaStream_t st);
 
@@ -312,11 +333,8 @@ struct DecStepBwd {
   unsigned int* bar; unsigned int bar_target;      // target of the FIRST barrier of this launch (the second is + gridDim.x)
 };
 int dec_step_bwd(const DecStepBwd& p, cudaStream_t st);
-extern int g_opt_dec_fuse_bwd;
-extern int g_opt_dec_fuse;
 // cluster-fused step kernels (lo_cluster.cu): the same DecStepFwd / DecStepBwd contracts, rows split into blocks of 16 (one 16-CTA cluster
 // each), no grid barrier (bar / bar_target unused), dxh written instead of accumulated
-extern int g_opt_dec_cl, g_opt_dec_cl_bwd;
 bool dec_cl_fwd_ok(int D, int C, int N2);
 bool dec_cl_bwd_ok(int D, int C, int A);
 int dec_cl_fwd(const DecStepFwd& p, cudaStream_t st);
@@ -324,9 +342,6 @@ int dec_cl_bwd(const DecStepBwd& p, cudaStream_t st);
 int cl_set_ts(long long* p);      // timing build only
 int sk_set_ts(long long* p);      // timing build only
 int tc_gemm_nt_lstm(const bf16* A, int64_t lda, const bf16* Wil, int64_t ldw, int M, int D, int K, const TcLstmEpi& e, cudaStream_t st);
-extern int g_opt_fuse_lstm;
-extern int g_opt_skinny_mma;
-extern int g_opt_skinny_tma;
 int skinny_gemm_nt_lstm(const bf16* A, int64_t lda, const bf16* Wil, int64_t ldw, int M, int D, int K, const TcLstmEpi& e, cudaStream_t st);
 int skinny_gemm_nt(const bf16* A, int64_t lda, const bf16* W, int64_t ldw, float* C, int64_t ldc, int M, int N, int K, const float* bias,
                    int splits, int atomic_acc, cudaStream_t st);

@@ -1014,8 +1014,6 @@ __global__ void split_bf16_kernel(const float* __restrict__ x, bf16* __restrict_
   }
 }
 
-int g_opt_fuse_lstm = 0;   // off: the epilogue threads cannot hide the dependent global loads
-                           // (tok -> table row, recurrent projection, c) that 32 K threads of lstm_pw_fwd_kernel hide
 // wil[4*j + g][c] = w_ih[g*D + j][E + c]: gate-interleaved copy of the context half of weight_ih, so that one 32-column
 // accumulator chunk of the wgmma GEMM holds whole hidden units and the LSTM cell can run in its epilogue
 __global__ void interleave_wih_kernel(const bf16* __restrict__ w_ih, bf16* __restrict__ wil, int D, int E, int C) {
@@ -1085,10 +1083,6 @@ struct Rows {
   void* work;       // attention workspace of this chain
   int nsplit;       // attention split hint (0 = automatic)
 };
-int g_opt_dec_streams = 1;
-// timing dissection only (tools/dec_breakdown.py; results are garbage): 1 = skip the hoisted part of the backward, 2 = skip the
-// attention launches of the time loops, 4 = skip the per-step GEMM / LSTM launches, 8 = skip the hoisted part of the forward
-int g_opt_dbg_skip = 0;
 
 // one decoder step t for the rows of `rs`; tok: token ids consumed at this step (row 0 of the batch)
 static int forward_step(const lo_decoder_args* a, const Dims& d, int t, const Rows& rs, const int64_t* tok, int64_t tok_stride,

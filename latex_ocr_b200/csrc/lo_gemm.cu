@@ -183,8 +183,6 @@ int gemm_nn(const void* A, int dtA, int64_t lda, const void* B, int dtB, int64_t
 // order (lo_ptx.cuh:cl_sum); without `accumulate` up to two clusters cover a column block and add onto the zeroed `out` with one
 // fp32 atomic each — two addends onto 0 give the same sum in either order.  Without a cluster launch the kernels' cluster is
 // the block itself.
-int g_opt_det = 0;
-
 constexpr int CS_MAXCL = 16;          // non-portable cluster size (H100)
 constexpr int CS_THREADS = 1024;
 
@@ -308,6 +306,26 @@ int colsum(const void* X, int dt, float* out, int M, int N, int64_t ld, int accu
   return LO_OK;
 }
 
+// the run-time options of lo_common.cuh's LO_OPTIONS and the name table lo_set_option / lo_get_option / lo_option_name walk
+#define LO_OPTION_DEFINE(var, name, def) int var = def;
+LO_OPTIONS(LO_OPTION_DEFINE)
+#undef LO_OPTION_DEFINE
+
+struct Option {
+  const char* name;
+  int* var;
+};
+#define LO_OPTION_ENTRY(var, name, def) {name, &var},
+static const Option g_options[] = {LO_OPTIONS(LO_OPTION_ENTRY)};
+#undef LO_OPTION_ENTRY
+constexpr int NUM_OPTIONS = sizeof(g_options) / sizeof(g_options[0]);
+
+static int* find_option(const char* name) {
+  for (int i = 0; name && i < NUM_OPTIONS; i++)
+    if (!strcmp(name, g_options[i].name)) return g_options[i].var;
+  return nullptr;
+}
+
 }  // namespace lo
 
 extern "C" {
@@ -316,6 +334,28 @@ int lo_version(void) { return 100; }
 const char* lo_last_error(void) { return lo::g_err; }
 int64_t lo_launch_count(void) { return lo::g_launches; }
 int lo_tc_available(void) { return lo::tc_available() ? 1 : 0; }
+
+const char* lo_option_name(int i) { return i >= 0 && i < lo::NUM_OPTIONS ? lo::g_options[i].name : nullptr; }
+
+int lo_get_option(const char* name) {
+  const int* v = lo::find_option(name);
+  return v ? *v : -1;
+}
+
+int lo_set_option(const char* name, int value) {
+  int* v = lo::find_option(name);
+  if (!v) return lo::fail(LO_EINVAL, "lo_set_option: unknown option %s", name ? name : "(null)");
+  if (v == &lo::g_opt_l2_persist_mb) {
+    // an action: size of the L2 set-aside that evict_last / persisting accesses may occupy (0 = driver default)
+    cudaError_t e = cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, (size_t)value << 20);
+    if (e != cudaSuccess) return lo::fail(LO_ECUDA, "lo_set_option(l2_persist_mb): %s (%ld)", cudaGetErrorString(e), (long)e);
+  }
+  *v = value;
+  // the 8-stage skinny wgmma config takes 198 KB of shared memory, a whole SM: with two decoder chains (dec_streams >= 2) it
+  // would keep the other chain's kernels off the SMs it runs on
+  if (v == &lo::g_opt_dec_streams) lo::g_opt_skinny8 = value >= 2 ? 0 : 1;
+  return LO_OK;
+}
 
 int lo_gemm(const void* A, int dtA, const void* B, int dtB, void* C, int dtC, int M, int N, int K, int64_t sam,
             int64_t sak, int64_t sbk, int64_t sbn, int64_t ldc, int batch, int64_t sA, int64_t sB, int64_t sC,

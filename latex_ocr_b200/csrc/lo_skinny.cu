@@ -11,9 +11,6 @@
 
 namespace lo {
 
-int g_opt_skinny_mma = 1;
-int g_opt_skinny_tma = 1;       // operands of skinny_mma_kernel by cp.async.bulk (one copy per row) instead of 16-byte cp.async
-
 constexpr int SK_KC = 512;        // K elements per CTA
 constexpr int SK_NT = 16;         // output columns per CTA
 constexpr int SK_PITCH = SK_KC + 8;   // bf16 elements per smem row (+16 B: conflict-free ldmatrix)
@@ -490,8 +487,6 @@ __global__ void __launch_bounds__(128) dec_step_fwd_kernel(DecStepFwd p) {
   SK_TS(7);
 }
 
-int g_opt_dec_fuse = 0;       // fused forward step: off, it measured no faster than the separate launches; see grid_barrier
-
 int dec_step_fwd(const DecStepFwd& p, cudaStream_t st) {
   LO_CHECK_ARG(p.M >= 1 && p.M <= 64 && p.K % 16 == 0 && p.K <= SK_KC && p.e.D == p.K && p.e.D % 4 == 0 && p.N2 % 2 == 0, "M<=64, K=D<=512");
   LO_CHECK_ARG(p.e.h_bf && p.bar, "bf16 mirror of h and the barrier counter are required");
@@ -632,8 +627,6 @@ __global__ void __launch_bounds__(128) dec_step_bwd_kernel(DecStepBwd p) {
   __syncthreads();
   skinny_tile_atomic(sA, sWc, SK_KC, p.dxh, CD, c_n0, CD, p.Mb);
 }
-
-int g_opt_dec_fuse_bwd = 0;   // off: two grid barriers cost more than two PDL boundaries
 
 int dec_step_bwd(const DecStepBwd& p, cudaStream_t st) {
   LO_CHECK_ARG(p.K2 % SK_KC == 0 && p.K1 % SK_KC == 0 && p.D % SK_NT == 0 && (p.C + p.D) % SK_NT == 0 && p.C == p.D, "K1, K2 multiples of 512, C == D");

@@ -737,9 +737,7 @@ static int make_map(CUtensorMap* m, const void* base, int rank, const cuuint64_t
   return LO_OK;
 }
 
-int g_opt_conv_mc = 1;    // cluster-of-2 multicast of the A tile
 long long* g_tc_dbg = nullptr;
-int g_opt_skinny8 = 1;    // 8-stage (198 KB smem) config for M <= 128 GEMMs; off when two decoder chains share the SMs
 
 template <int NT, int STAGES, int MC>
 static int launch_tc(const CUtensorMap& mA, const CUtensorMap& mB, const TcParams& p, int mtiles, int splits, cudaStream_t st) {
@@ -844,12 +842,6 @@ int tc_gemm_nt(const bf16* A, int64_t lda, const bf16* W, int64_t ldw, void* C, 
                const float* bias, int accumulate, int relu, cudaStream_t st) {
   return tc_gemm_nt_ex(A, lda, W, ldw, C, dtC, ldc, M, N, K, bias, accumulate, relu, 1, 0, 0, st);
 }
-
-int g_opt_wgrad256 = 0;       // conv weight gradient with 128 x 256 tiles when Cin % 256 == 0: off, two 96 KB stages
-                              // cannot hide the loads
-int g_opt_conv_persist = 1;   // persistent double-accumulator kernel (tc_conv_p_kernel); 0 = one tile per CTA (tc_gemm_conv_kernel)
-
-int g_opt_conv_mt2 = 1;       // layers with <= 128 output channels: two 128-position sub-tiles per CTA tile share each weight stage
 
 template <int NT, int STAGES, int MT>
 static int launch_conv_p(const CUtensorMap& mA, const CUtensorMap& mB, const TcParams& p, int mtiles, cudaStream_t st) {

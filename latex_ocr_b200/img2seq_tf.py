@@ -140,16 +140,12 @@ class Img2SeqModel:
         if self.clip > 0:                                                   # tf.clip_by_global_norm (img2seq.py:116-121)
             gn = float(torch.sqrt(self.encoder.store.grad.pow(2).sum() + self.decoder.store.grad.pow(2).sum()))
             scale = min(1.0, self.clip / max(gn, 1e-30))
-        import ctypes
-        fn = L.lo_tf_optim_step
-        fn.restype = ctypes.c_int
-        fn.argtypes = [ctypes.c_int] + [ctypes.c_void_p] * 5 + [ctypes.c_int64, ctypes.c_void_p] + [ctypes.c_float] * 4 + [ctypes.c_void_p]
         kind = getattr(self, "_opt_kind", 1)
         # TF defaults: Adam beta1 0.9, beta2 0.999, epsilon 1e-8 (outside the bias correction); RMSProp decay 0.9, epsilon 1e-10
         b1, b2, eps = (0.9, 0.9, 1e-10) if kind == 4 else (0.9, 0.999, 1e-8)
         for m in (self.decoder, self.encoder):
             S = m.store
-            check(fn(kind, ptr(S.master), ptr(S.grad), ptr(S.m), ptr(S.v), ptr(S.shadow), S.numel, ptr(S.adam_state), b1, b2, eps,
+            check(L.lo_tf_optim_step(kind, ptr(S.master), ptr(S.grad), ptr(S.m), ptr(S.v), ptr(S.shadow), S.numel, ptr(S.adam_state), b1, b2, eps,
                      float(scale), stream_ptr()))
 
     def train_step(self, images, formulas, dropout=1.0):

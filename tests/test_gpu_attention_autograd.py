@@ -137,23 +137,6 @@ def test_step_kernel_shares_the_attention_backward_arithmetic(dtype, A, R, B):
     assert torch.equal(de, de2) and torch.equal(datt2, datt2b)
 
 
-class _options:
-    """Library options set for a block and restored after it."""
-
-    def __init__(self, **kv):
-        self.kv = kv
-
-    def __enter__(self):
-        L = _lib.lib()
-        self.prev = {k: L.lo_get_option(k.encode()) for k in self.kv}
-        for k, v in self.kv.items():
-            _lib.set_option(k, v)
-
-    def __exit__(self, *exc):
-        for k, v in self.prev.items():
-            _lib.set_option(k, v)
-
-
 def _check_vs_float64(dtype, A, R, B, seed):
     enc, att1, att2, wf, alpha, ctx, dctx, dalpha = _kernel_inputs(B, R, A, dtype, seed=seed)
     outs = _step_backward(enc, att1, att2, wf, alpha, ctx, dctx, dalpha)
@@ -174,9 +157,9 @@ def test_step_kernel_without_cluster(dtype, A, R, B, opts):
     """The non-cluster launches of the d att1 kernel: B >= 133 gives one split per batch row; att_cluster=0 gives several splits
     whose d w_full partials meet with atomics.  With "deterministic" the splits of a row are folded into one (fixed order) and two
     calls give the same bits."""
-    with _options(**opts):
+    with _lib.option(**opts):
         _check_vs_float64(dtype, A, R, B, seed=3 * A + B)
-        with _options(deterministic=1):
+        with _lib.option(deterministic=1):
             first = _check_vs_float64(dtype, A, R, B, seed=5 * A + B)
             second = _check_vs_float64(dtype, A, R, B, seed=5 * A + B)
     for a, b in zip(first, second):
@@ -469,16 +452,12 @@ def test_deterministic_backward_is_bit_reproducible():
     enc = (torch.randn(8, 868, 512, generator=g) * 0.5).cuda()
     h = torch.randn(8, 512, generator=g).cuda()
     gc, ga = torch.randn(8, 512, generator=g).cuda(), torch.randn(8, 868, generator=g).cuda()
-    prev = _lib.lib().lo_get_option(b"deterministic")
-    _lib.set_option("deterministic", 1)
-    try:
+    with _lib.option(deterministic=1):
         runs = []
         for _ in range(2):
             att.zero_grad(set_to_none=True)
             x, y = enc.clone().requires_grad_(True), h.clone().requires_grad_(True)
             _loss(*att(x, y), gc, ga, "both").backward()
             runs.append([x.grad, y.grad] + [p.grad.clone() for p in att.parameters()])
-    finally:
-        _lib.set_option("deterministic", prev)
     for a, b in zip(*runs):
         assert torch.equal(a, b)

@@ -134,32 +134,28 @@ def test_generic_backward_bit_identical_to_fused(precision):
     m = build_model(V, pe, pd, precision, train=True, impl="tc" if precision == "bf16" else "simt")
     dec = m.decoder
     B, T = formula.shape[0], formula.shape[1] - 1
-    _lib.set_option("deterministic", 1)
-    try:
-        with torch.no_grad():
-            enc = m.encoder.forward_raw(img.cuda(), need_grad=True)
-            enc = enc.reshape(B, -1, enc.shape[3])
-            R = enc.shape[1]
-            caps = formula.cuda()
-            dec.seed_dropout(1234)
-            ws = dec.run_forward(enc, caps, [T] * B, with_loss=True, need_grad=True, dropout_mask="philox")
-            dec.run_backward(ws)
-            want_g = dec.store.grad.clone()
-            want_denc = ws["t"]["denc"].clone()
-            dlogits = ws["t"]["dlogits"].clone()                 # [B][T][ldl]: rows ldl apart
-            dalpha = ws["t"]["dreg"][:, None, :].expand(B, T, R).contiguous()
-            dec.store.grad.zero_()
-            ws["t"]["denc"].zero_()
-            dec.seed_dropout(1234)
-            ws = dec.run_forward(enc, caps, [T] * B, with_loss=False, need_grad=True, dropout_mask="philox")
-            a = ws["args"]
-            a.dpred_ext, a.dpred_stride, a.dalpha_ext = dlogits.data_ptr(), dlogits.shape[2], dalpha.data_ptr()
-            dec.run_backward(ws)
-            torch.cuda.synchronize()
-            assert torch.equal(dec.store.grad, want_g)
-            assert torch.equal(ws["t"]["denc"], want_denc)
-    finally:
-        _lib.set_option("deterministic", 0)
+    with _lib.option(deterministic=1), torch.no_grad():
+        enc = m.encoder.forward_raw(img.cuda(), need_grad=True)
+        enc = enc.reshape(B, -1, enc.shape[3])
+        R = enc.shape[1]
+        caps = formula.cuda()
+        dec.seed_dropout(1234)
+        ws = dec.run_forward(enc, caps, [T] * B, with_loss=True, need_grad=True, dropout_mask="philox")
+        dec.run_backward(ws)
+        want_g = dec.store.grad.clone()
+        want_denc = ws["t"]["denc"].clone()
+        dlogits = ws["t"]["dlogits"].clone()                 # [B][T][ldl]: rows ldl apart
+        dalpha = ws["t"]["dreg"][:, None, :].expand(B, T, R).contiguous()
+        dec.store.grad.zero_()
+        ws["t"]["denc"].zero_()
+        dec.seed_dropout(1234)
+        ws = dec.run_forward(enc, caps, [T] * B, with_loss=False, need_grad=True, dropout_mask="philox")
+        a = ws["args"]
+        a.dpred_ext, a.dpred_stride, a.dalpha_ext = dlogits.data_ptr(), dlogits.shape[2], dalpha.data_ptr()
+        dec.run_backward(ws)
+        torch.cuda.synchronize()
+        assert torch.equal(dec.store.grad, want_g)
+        assert torch.equal(ws["t"]["denc"], want_denc)
 
 
 # 3 ---------------------------------------------------------------------------------------------------------------------------
@@ -214,13 +210,9 @@ def test_custom_loss_under_backward_schedules(option):
     L = _lib.lib()
     m = build_model(V, pe, pd, "bf16", impl="tc")
     want_dx, want = _run_custom(m, formula, lengths, enc)
-    old = L.lo_get_option(option.encode())
-    _lib.set_option(option, 1 - old)
-    try:
+    with _lib.option(**{option: 1 - L.lo_get_option(option.encode())}):
         m.decoder.zero_grad()
         dx, got = _run_custom(m, formula, lengths, enc)
-    finally:
-        _lib.set_option(option, old)
     _close(dx, want_dx, 1e-2, "d encoder_out")
     for k in want:
         if k != "attention.full_att.bias":

@@ -258,8 +258,7 @@ def test_image_grad_changes_nothing_else_and_works_on_a_frozen_model(precision):
     m = _torch_model(pe, pd, precision)
     params = list(m.encoder.parameters()) + list(m.decoder.parameters())
     f = formula.cuda()
-    _lib.set_option("deterministic", 1)
-    try:
+    with _lib.option(deterministic=1):
         with torch.no_grad():
             want_out = m.encoder(img.cuda())
 
@@ -297,8 +296,6 @@ def test_image_grad_changes_nothing_else_and_works_on_a_frozen_model(precision):
         custom_loss(preds, caps, dl, alphas).backward()
         assert torch.equal(x2.grad, dimg)
         assert all(p.grad is None for p in params)
-    finally:
-        _lib.set_option("deterministic", 0)
 
 
 # 6 ---------------------------------------------------------------------------------------------------------------------------

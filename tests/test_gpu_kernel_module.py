@@ -3,8 +3,6 @@ use gets no gradient pass: an unused ``alphas`` reaches lo_decoder_backward as `
 bits explicit zeros give.  A backward reads the forward state its node holds, so it still runs, with the same bits, after a forward
 of another shape evicted that state from the bounded workspace caches.  bf16 with the tensor-core kernels, option
 ``deterministic``."""
-import contextlib
-
 import pytest
 import torch
 import torch.nn.functional as F
@@ -15,16 +13,6 @@ from util import Cfg
 pytestmark = pytest.mark.gpu
 
 V = 50
-
-
-@contextlib.contextmanager
-def _deterministic():
-    prev = _lib.lib().lo_get_option(b"deterministic")
-    _lib.set_option("deterministic", 1)
-    try:
-        yield
-    finally:
-        _lib.set_option("deterministic", prev)
 
 
 def _row_model():
@@ -73,7 +61,7 @@ def test_unused_alphas_give_the_bits_of_explicit_zeros(two_layer):
         loss.backward()
         return [x.grad] + [p.grad.clone() for p in dec.parameters()]
 
-    with _deterministic():
+    with _lib.option(deterministic=1):
         unused, zeros = grads(False), grads(True)
     names = ["d encoder_out"] + [k for k, _ in dec.named_parameters()]
     for name, a, b in zip(names, unused, zeros):
@@ -153,7 +141,7 @@ def test_backward_after_eviction_gives_the_same_bits(name):
         loss.backward()
         return [x.grad for x in inputs] + [p.grad.clone() for p in module.parameters()]
 
-    with _deterministic():
+    with _lib.option(deterministic=1):
         want, got = run(False), run(True)
     names = ["d input"] + [k for k, _ in module.named_parameters()]
     for k, a, b in zip(names, want, got):

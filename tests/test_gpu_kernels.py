@@ -194,7 +194,6 @@ def test_maxpool(k):
 def test_attention_forward(dtype, B, R, pipe):
     """pipe=1: TMA bulk-copy -> smem ring version (lo_attention.cu); pipe=0: register-streaming version."""
     _lib, L = _L()
-    _lib.set_option("att_pipe", pipe)
     torch.manual_seed(6)
     C = A = 512
     enc = torch.randn(B, R, C, device="cuda").to(dtype)
@@ -207,12 +206,13 @@ def test_attention_forward(dtype, B, R, pipe):
     ctx = torch.zeros(B, C, device="cuda")
     gctx = torch.zeros(B, C, device="cuda")
     work = torch.zeros(int(L.lo_attention_workspace_bytes(B, C)), dtype=torch.uint8, device="cuda")
-    for _ in range(2):     # second launch checks that the ticket counters were reset
-        gate_pre.copy_(gp0)
-        _lib.check(L.lo_attention_forward(_lib.ptr(att1), _lib.ptr(enc), _lib.dt_of(enc), _lib.ptr(att2), att2.stride(0), _lib.ptr(wf),
-                                          _lib.ptr(alpha), R, _lib.ptr(ctx), _lib.ptr(gate_pre), C, _lib.ptr(gctx), B, R, A, C,
-                                          _lib.ptr(work), _lib.stream_ptr()))
-        torch.cuda.synchronize()
+    with _lib.option(att_pipe=pipe):
+        for _ in range(2):     # second launch checks that the ticket counters were reset
+            gate_pre.copy_(gp0)
+            _lib.check(L.lo_attention_forward(_lib.ptr(att1), _lib.ptr(enc), _lib.dt_of(enc), _lib.ptr(att2), att2.stride(0), _lib.ptr(wf),
+                                              _lib.ptr(alpha), R, _lib.ptr(ctx), _lib.ptr(gate_pre), C, _lib.ptr(gctx), B, R, A, C,
+                                              _lib.ptr(work), _lib.stream_ptr()))
+            torch.cuda.synchronize()
     e = (torch.relu(att1.double() + att2.double()[:, None, :]) * wf.double()).sum(-1)
     al = torch.softmax(e, dim=1)
     cx = torch.einsum("br,brc->bc", al, enc.double())
@@ -220,7 +220,6 @@ def test_attention_forward(dtype, B, R, pipe):
     assert relerr(ctx, cx.float()) < 2e-5
     assert relerr(gate_pre, torch.sigmoid(gp0)) < 1e-6
     assert relerr(gctx, (torch.sigmoid(gp0.double()) * cx).float()) < 2e-5
-    _lib.set_option("att_pipe", 1)
 
 
 def test_adam_matches_torch():
@@ -290,11 +289,8 @@ def test_tf_optimisers_follow_tf_update_rules(kind):
     """lo_tf_optim_step: the four optimisers of model/img2seq.py:98-111 with TensorFlow 1.12's update rules restated in fp64
     (parity unpinned: TF cannot run here).  1 Adam (epsilon outside the bias correction), 2 SGD, 3 Adagrad (accumulator starts at
     0.1), 4 RMSProp (rms slot starts at 1, decay 0.9, epsilon 1e-10, momentum 0)."""
-    import ctypes
     _lib, L = _L()
     fn = L.lo_tf_optim_step
-    fn.restype = ctypes.c_int
-    fn.argtypes = [ctypes.c_int] + [ctypes.c_void_p] * 5 + [ctypes.c_int64, ctypes.c_void_p] + [ctypes.c_float] * 4 + [ctypes.c_void_p]
     torch.manual_seed(kind)
     n, lr = 5003, 1e-2
     p = torch.randn(n, device="cuda")

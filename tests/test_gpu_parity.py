@@ -292,15 +292,12 @@ def test_attention_kernel_versions_agree_on_a_full_step():
     img, formula = rm.synthetic_batch(3, 40, 72, V, 4, 9, seed=16)
     B, T = formula.shape[0], formula.shape[1] - 1
     res = {}
-    try:
-        for pipe in (0, 1):
-            _lib.set_option("att_pipe", pipe)
+    for pipe in (0, 1):
+        with _lib.option(att_pipe=pipe):
             m = build_model(V, pe, pd, "fp32")
             loss = m._step_body(img.cuda(), formula.cuda(), [T] * B, None)
             torch.cuda.synchronize()
             res[pipe] = (loss[0].item(), m.decoder.store.grad.clone(), m.encoder.store.grad.clone())
-    finally:
-        _lib.set_option("att_pipe", 1)
     assert abs(res[0][0] - res[1][0]) / abs(res[0][0]) < 1e-6
     for i in (1, 2):
         assert (res[0][i] - res[1][i]).abs().max().item() <= 1e-4 * res[0][i].abs().max().item() + 1e-8

@@ -45,18 +45,15 @@ def test_skinny_mma_gemm(M, N, K, acc):
     b = torch.randn(N, device="cuda")
     base = torch.randn(M, N, device="cuda")
     ref = (A.double() @ W.double().t() + b.double() + (base.double() if acc else 0)).float()
-    try:
-        for opt in (1, 0):
-            if opt == 0 and (K % 64 or N % 8):
-                continue                                   # wgmma path constraints
-            _lib.set_option("skinny_mma", opt)
+    for opt in (1, 0):
+        if opt == 0 and (K % 64 or N % 8):
+            continue                                   # wgmma path constraints
+        with _lib.option(skinny_mma=opt):
             C = base.clone()
             _lib.check(L.lo_gemm(_lib.ptr(A), 1, _lib.ptr(W), 1, _lib.ptr(C), _lib.dt_of(C), M, N, K, K, 1, 1, K, N, 1, 0, 0, 0, _lib.ptr(b), acc, 0,
                                  1, _lib.stream_ptr()))
             torch.cuda.synchronize()
-            assert relerr(C, ref) < 1e-5, opt
-    finally:
-        _lib.set_option("skinny_mma", 1)
+        assert relerr(C, ref) < 1e-5, opt
 
 
 @pytest.mark.parametrize("N,H,W,Cin,Cout,pad", [(2, 8, 128, 64, 128, 1), (2, 16, 64, 128, 256, 1), (3, 16, 64, 512, 512, 0),
@@ -151,16 +148,12 @@ def test_optional_decoder_schedules_match_default(opt):
     img, formula = rm.synthetic_batch(40, 32, 64, V, 4, 6, seed=42)     # B >= 32 so that the two-chain loop engages
     B, T = formula.shape[0], formula.shape[1] - 1
     res = {}
-    try:
-        for val in _SCHEDULE_OPTS[opt]:
-            _lib.set_option(opt, val)
+    for val in _SCHEDULE_OPTS[opt]:
+        with _lib.option(**{opt: val}):
             m = build_model(V, pe, pd, "bf16", impl="tc")
             loss = m._step_body(img.cuda(), formula.cuda(), [T] * B, None)
             torch.cuda.synchronize()
             res[val] = (loss[0].item(), m.decoder.store.grad.clone())
-    finally:
-        for name, (default, _) in _SCHEDULE_OPTS.items():
-            _lib.set_option(name, default)
     (l0, g0), (l1, g1) = res.values()
     assert abs(l0 - l1) / abs(l0) < 1e-4
     assert (g0 - g1).norm().item() / g0.norm().item() < 2e-2
@@ -185,20 +178,17 @@ def test_deterministic_option_gives_bit_identical_steps():
     base = torch.randn(64, 256, device="cuda")
     ref = (A.double() @ W.double().t() + base.double()).float()
     runs = {}
-    try:
-        for det in (1, 1, 0):
-            _lib.set_option("deterministic", det)
+    for det in (1, 1, 0):
+        with _lib.option(deterministic=det):
             m = build_model(c["V"], pe, pd, "bf16", impl="tc")
             m._step_body(img.cuda(), formula.cuda(), [T] * B, None)
             C = base.clone()
             _lib.check(L.lo_gemm(_lib.ptr(A), 1, _lib.ptr(W), 1, _lib.ptr(C), 0, 64, 256, 4608, 4608, 1, 1, 4608, 256, 1, 0, 0, 0, None, 1,
                                  0, 1, _lib.stream_ptr()))
             torch.cuda.synchronize()
-            assert relerr(C, ref) < 1e-5, det
-            stores = (m.encoder.store, m.decoder.store)
-            runs.setdefault(det, []).append([t.clone() for s_ in stores for t in (s_.grad, s_.master)] + [C])
-    finally:
-        _lib.set_option("deterministic", 0)
+        assert relerr(C, ref) < 1e-5, det
+        stores = (m.encoder.store, m.decoder.store)
+        runs.setdefault(det, []).append([t.clone() for s_ in stores for t in (s_.grad, s_.master)] + [C])
     first, second = runs[1]
     for a, b in zip(first, second):
         assert torch.equal(a, b)

@@ -3,7 +3,6 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 from latex_ocr_b200 import _lib
 L = _lib.lib()
-L.lo_debug_buffer.argtypes = [ctypes.c_void_p]
 dbg = torch.zeros(128, dtype=torch.int64, device="cuda")
 N, H, W, Cin, Cout = 64, 32, 128, 256, 256
 x = torch.randn(N, H, W, Cin, device="cuda").bfloat16(); w = (torch.randn(Cout, 3, 3, Cin, device="cuda") * 0.02).bfloat16()

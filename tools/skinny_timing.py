@@ -3,7 +3,6 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 from latex_ocr_b200 import _lib
 L = _lib.lib()
-L.lo_debug_buffer.argtypes = [ctypes.c_void_p]
 dbg = torch.zeros(16, dtype=torch.int64, device="cuda")
 for (M, N, K) in ((64, 3072, 512), (64, 2048, 512)):
     A = torch.randn(M, K, device="cuda").bfloat16(); W = torch.randn(N, K, device="cuda").bfloat16()

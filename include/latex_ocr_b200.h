@@ -274,6 +274,24 @@ typedef struct lo_decoder_args {
   const int32_t* bt_host;  /* HOST int[T]: rows active at step t (seq2seq_torch.py:308); non-increasing */
   const int64_t* caps;     /* [B][caps_stride] token ids (sorted rows) */
   int64_t caps_stride;
+  /* scheduled sampling (Bengio et al. 2015).  ss_prob != NULL selects the mode; it must then be set in BOTH the forward and the
+   * backward call, as dpred_ext is.  Step t >= 1 of an active row b feeds
+   *     fed[b][t] = argmax_v logits[b][t-1][v]  if u[b][t] < p   (lowest index wins ties, as torch.argmax)
+   *               = caps[b][t]                  otherwise ;       fed[b][0] = caps[b][0]
+   * where logits[b][t-1] is the returned prediction row (fc(dropout(h)) with the dropout of this call), p = *ss_prob.  The choice
+   * is not differentiated: given fed, forward and backward are teacher forcing on the input sequence fed (the embedding and
+   * weight_ih[:, :E] gradients go to the rows of the tokens fed); ce_kernel's targets stay caps[b][t+1].  In this mode the head
+   * fc(hd_t) runs inside the time loop (one GEMM per step, writing only the rows active at step t) instead of once after it, and
+   * the forward always runs the default single-chain step loop: dec_fuse, dec_cl, fuse_lstm and dec_streams >= 2 are ignored.
+   * Refused (LO_EINVAL) before any GPU work: ss_prob without fed, without ss_u and dropout_state, with phase != 0, with
+   * rows_per_img > 1, and on the greedy / beam entry points. */
+  int64_t* fed;            /* [B][T] tokens fed at each step: written by the forward (positions past a row's decode length get
+                              caps[b][t]), read by the backward */
+  const float* ss_prob;    /* DEVICE scalar p, read inside the kernels (a captured graph stays valid when p changes); NULL: off */
+  const float* ss_u;       /* optional injected uniforms [B][T] (parity tests); NULL: u = (x >> 8) * 2^-24 with x the first word
+                              of Philox4x32-10(counter = (0xFFFFFFFF, t, b, call), key = seed) of dropout_state {seed, call} — a
+                              counter the dropout stream (j >> 2, t, b, call) never uses.  lo_decoder_backward advances the
+                              call counter in this mode as it does for has_dropout = 2 */
   /* inputs */
   const void* enc;         /* big [B][R][C] */
   /* parameters: weight shadows in `dt`, biases fp32.  Wcat1 = [decoder_att; f_beta; weight_hh] rows

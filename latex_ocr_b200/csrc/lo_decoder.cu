@@ -419,13 +419,27 @@ __global__ void mean_rows_kernel(const T* __restrict__ enc, float* __restrict__ 
   mean[(int64_t)b * C + c] = s / (float)R;
 }
 
+// scheduled-sampling operands of lstm_pw_fwd_kernel<true> (row pointers at the first row of the launch, step t)
+struct SsStep {
+  const float* prev_logits;   // logits of step t-1 (NULL at t = 0), rows lstride apart
+  int64_t lstride;
+  const float* prob;          // device scalar p
+  const float* u;             // injected uniforms of step t, rows ustride apart, or NULL: Philox keyed by coin_state
+  const unsigned long long* coin_state;   // {seed, call} (lo_decoder_args.dropout_state)
+  int64_t ustride;
+  int64_t* fed;               // fed tokens of step t, rows ustride apart
+  bf16* hd_bf;                // bf16 mirror of hd (A operand of the per-step fc GEMM in bf16), NULL otherwise
+};
+
 // LSTM cell pointwise (nn.LSTMCell, gate order i,f,g,o).  pre = gtmp + ptab[tok] + hh_pre.
+// SS (scheduled sampling): tok is the teacher token; the token fed is chosen here (lo_decoder_args.ss_prob) and recorded.
+template <bool SS>
 __global__ void lstm_pw_fwd_kernel(const float* __restrict__ gtmp, const float* __restrict__ ptab,
                                    const int64_t* __restrict__ tok, int64_t tok_stride, const float* __restrict__ hh,
                                    int64_t hh_stride, const float* __restrict__ c_prev, float* __restrict__ gates,
                                    float* __restrict__ c_out, float* __restrict__ h_out, bf16* __restrict__ h_bf,
                                    float* __restrict__ hd, int64_t hd_stride, const float* __restrict__ dmask, int nrows, int D,
-                                   int V, const unsigned long long* __restrict__ dstate, float dp, int row0, int t_idx) {
+                                   int V, const unsigned long long* __restrict__ dstate, float dp, int row0, int t_idx, SsStep ss) {
   // Everything but the gates GEMM result is at least two launches old (token -> table row, the recurrent projection of this step,
   // c_t; the dropout draw depends on nothing): fetched / computed BEFORE griddepcontrol.wait, so only one L2 round trip (gtmp) is left
   // on the critical path of the time loop instead of two dependent ones.
@@ -433,8 +447,53 @@ __global__ void lstm_pw_fwd_kernel(const float* __restrict__ gtmp, const float* 
   const bool live = idx < nrows * D;
   const int b = live ? idx / D : 0, j = live ? idx % D : 0;
   float a4[4] = {0.f, 0.f, 0.f, 0.f}, cp = 0.f, mult = 1.f;
+  int64_t tk_ss = 0;
+  if constexpr (SS) {
+    // The logits of step t-1 come from the fc GEMM launched right after lstm_pw_fwd_kernel(t-1); the o1 GEMM, the attention and
+    // the gates GEMM of step t come in between, so they are three launches old and safe to read before griddepcontrol.wait (as
+    // the teacher token is).  The forward keeps that launch order.  One warp per row of the block: coin, then (only when it
+    // says "sample") the lowest-index argmax of the row's V logits.
+    __shared__ int64_t s_tok[256 / 8 + 2];            // rows a 256-thread block touches: <= 256 / D + 1, D % 8 == 0
+    const int first = (int)(blockIdx.x * blockDim.x) / D;
+    const int last = min(nrows - 1, (int)(blockIdx.x * blockDim.x + blockDim.x - 1) / D);
+    const int lane = threadIdx.x & 31;
+    for (int r = first + (int)(threadIdx.x >> 5); r <= last; r += (int)(blockDim.x >> 5)) {
+      int64_t pick = tok[(int64_t)r * tok_stride];
+      if (ss.prev_logits) {
+        float u;
+        if (ss.u) u = ss.u[(int64_t)r * ss.ustride];
+        else {
+          const unsigned long long seed = ss.coin_state[0], call = ss.coin_state[1];
+          u = u01(philox4x32_10(make_uint4(0xFFFFFFFFu, (uint32_t)t_idx, (uint32_t)(row0 + r), (uint32_t)call),
+                                make_uint2((uint32_t)seed, (uint32_t)(seed >> 32))).x);
+        }
+        if (u < *ss.prob) {                           // warp-uniform
+          const float* lg = ss.prev_logits + (int64_t)r * ss.lstride;
+          float best = -INFINITY;
+          int bi = 0;
+          for (int v = lane; v < V; v += 32) {
+            const float x = lg[v];
+            if (x > best) { best = x; bi = v; }
+          }
+#pragma unroll
+          for (int o = 16; o > 0; o >>= 1) {
+            const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+            const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+            if (ob > best || (ob == best && oi < bi)) { best = ob; bi = oi; }   // the rule of argmax_kernel (greedy decode)
+          }
+          pick = bi;
+        }
+      }
+      if (lane == 0) {
+        s_tok[r - first] = pick;
+        if ((int64_t)r * D >= (int64_t)blockIdx.x * blockDim.x) ss.fed[(int64_t)r * ss.ustride] = pick;   // the block holding j = 0
+      }
+    }
+    __syncthreads();
+    if (live) tk_ss = s_tok[b - first];
+  }
   if (live) {
-    int64_t tk = tok[(int64_t)b * tok_stride];
+    int64_t tk = SS ? tk_ss : tok[(int64_t)b * tok_stride];
     if (tk < 0) tk = 0;
     if (tk >= V) tk = V - 1;
     const float* pt = ptab + tk * 4 * D;
@@ -464,6 +523,9 @@ __global__ void lstm_pw_fwd_kernel(const float* __restrict__ gtmp, const float* 
   h_out[(int64_t)b * D + j] = h;
   if (h_bf) h_bf[(int64_t)b * D + j] = __float2bfloat16_rn(h);
   if (hd) hd[(int64_t)b * hd_stride + j] = h * mult;
+  if constexpr (SS) {
+    if (ss.hd_bf) ss.hd_bf[(int64_t)b * hd_stride + j] = __float2bfloat16_rn(h * mult);
+  }
 }
 
 // backward of the cell pointwise part: dh = dhd[b,t] + dh_next ; writes d(pre-activations), dc_prev in place
@@ -942,6 +1004,12 @@ static int check_args(const lo_decoder_args* a) {
   LO_CHECK_ARG(a->has_dropout != 2 || (a->dropout_state && a->dropout_p >= 0.f && a->dropout_p < 1.f &&
                                        (!g_opt_fuse_lstm || g_opt_skinny_mma)),
                "has_dropout=2 needs dropout_state, 0 <= dropout_p < 1 (and the mma.sync kernel when fuse_lstm=1)");
+  if (a->ss_prob) {
+    LO_CHECK_ARG(a->fed, "scheduled sampling (ss_prob) needs fed");
+    LO_CHECK_ARG(a->ss_u || a->dropout_state, "scheduled sampling (ss_prob) needs ss_u or dropout_state for its coin");
+    LO_CHECK_ARG(a->phase == 0, "scheduled sampling (ss_prob) needs phase 0: no per-step head when a layer sits between h and fc");
+    LO_CHECK_ARG(a->rows_per_img <= 1, "scheduled sampling (ss_prob) needs rows_per_img <= 1");
+  }
   for (int t = 0; t < a->T; t++) {
     LO_CHECK_ARG(a->bt_host[t] >= 1 && a->bt_host[t] <= a->B, "bt_host out of range");
     if (t) LO_CHECK_ARG(a->bt_host[t] <= a->bt_host[t - 1], "bt_host must be non-increasing");
@@ -1090,6 +1158,7 @@ static int forward_step(const lo_decoder_args* a, const Dims& d, int t, const Ro
   const int dt = a->dt;
   const int nrows = rs.nrows;
   const int64_t r0 = rs.row0;
+  const bool sampling = a->ss_prob && hd_t;     // scheduled sampling: token chosen in the cell, head inside the loop
   if (nrows <= 0) return LO_OK;
   const size_t es = dt == LO_F32 ? 4 : 2;
   float* h_prev = a->hall + ((int64_t)t * d.B + r0) * d.D;
@@ -1118,7 +1187,7 @@ static int forward_step(const lo_decoder_args* a, const Dims& d, int t, const Ro
                                   a->rows_per_img, rs.nsplit, hd_t ? att_mask_at(a, t, r0) : nullptr));
   if (g_opt_dbg_skip & 4) return LO_OK;
   // gates_x = (gate*ctx) @ W_ih[:, E:]^T
-  if (bv.on && g_opt_fuse_lstm) {
+  if (bv.on && g_opt_fuse_lstm && !sampling) {
     // ... with the LSTM cell fused into the GEMM epilogue (no gates_x round trip, one launch less per step)
     TcLstmEpi e{a->ptab, tok + r0 * tok_stride, tok_stride, o1 + d.A + d.C, d.O1, c_prev, a->gates + ((int64_t)t * d.B + r0) * d.G,
                 a->call + ((int64_t)(t + 1) * d.B + r0) * d.D, a->hall + ((int64_t)(t + 1) * d.B + r0) * d.D,
@@ -1139,15 +1208,39 @@ static int forward_step(const lo_decoder_args* a, const Dims& d, int t, const Ro
     LO_TRY(gemm_nt(a->gctx + ((int64_t)t * d.B + r0) * d.C, LO_F32, d.C, (const char*)a->w_ih + (size_t)d.E * es, dt, d.E + d.C, gtmp,
                    LO_F32, d.G, nrows, d.G, d.C, nullptr, 0, 0, LO_IMPL_SIMT, st));
   }
-  LO_CUDA(launch_pdl(lstm_pw_fwd_kernel, dim3(cdiv((long)nrows * d.D, 256)), dim3(256), (size_t)0, st, (const float*)gtmp,
+  SsStep ss{};
+  if (sampling) {
+    ss.prev_logits = t > 0 ? a->logits + (r0 * d.T + t - 1) * d.Vl : nullptr;
+    ss.lstride = (int64_t)d.T * d.Vl;
+    ss.prob = a->ss_prob;
+    ss.u = a->ss_u ? a->ss_u + r0 * d.T + t : nullptr;
+    ss.coin_state = (const unsigned long long*)a->dropout_state;
+    ss.ustride = d.T;
+    ss.fed = a->fed + r0 * d.T + t;
+    ss.hd_bf = bv.on ? bv.hd + r0 * hd_stride + t * d.D : nullptr;
+  }
+  LO_CUDA(launch_pdl(sampling ? lstm_pw_fwd_kernel<true> : lstm_pw_fwd_kernel<false>, dim3(cdiv((long)nrows * d.D, 256)), dim3(256),
+                     (size_t)0, st, (const float*)gtmp,
                      (const float*)a->ptab, tok + r0 * tok_stride, tok_stride, (const float*)(o1 + d.A + d.C), (int64_t)d.O1,
                      (const float*)c_prev, a->gates + ((int64_t)t * d.B + r0) * d.G, a->call + ((int64_t)(t + 1) * d.B + r0) * d.D,
                      a->hall + ((int64_t)(t + 1) * d.B + r0) * d.D,
                      bv.on ? bv.hall + ((int64_t)(t + 1) * d.B + r0) * d.D : (bf16*)nullptr,
                      hd_t ? hd_t + r0 * hd_stride : (float*)nullptr, hd_stride,
                      dmask_t ? dmask_t + r0 * hd_stride : (const float*)nullptr, nrows, d.D, d.V,
-                     (const unsigned long long*)((hd_t && a->has_dropout == 2) ? a->dropout_state : nullptr), a->dropout_p, (int)r0, t));
+                     (const unsigned long long*)((hd_t && a->has_dropout == 2) ? a->dropout_state : nullptr), a->dropout_p, (int)r0, t,
+                     ss));
   LO_LAUNCH_OK();
+  if (sampling) {
+    // the head of step t, right after the cell (the next step's cell reads these logits, see lstm_pw_fwd_kernel): the returned
+    // predictions of this mode.  The dispatcher of greedy decode: mma.sync for <= 64 bf16 rows, CUDA cores in fp32
+    float* lg = a->logits + (r0 * d.T + t) * d.Vl;
+    if (bv.on)
+      LO_TRY(gemm_nt(ss.hd_bf, LO_BF16, hd_stride, a->w_fc, LO_BF16, d.D, lg, LO_F32, (int64_t)d.T * d.Vl, nrows, d.V, d.D, a->b_fc, 0, 0,
+                     LO_IMPL_TC, st));
+    else
+      LO_TRY(gemm_nt(hd_t + r0 * hd_stride, LO_F32, hd_stride, a->w_fc, dt, d.D, lg, LO_F32, (int64_t)d.T * d.Vl, nrows, d.V, d.D, a->b_fc,
+                     0, 0, LO_IMPL_SIMT, st));
+  }
   return LO_OK;
 }
 
@@ -1326,23 +1419,29 @@ int lo_decoder_forward(const lo_decoder_args* a, int with_loss, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   const Dims d = dims(a);
   const bool ragged = a->bt_host[d.T - 1] < d.B;
+  const bool sampling = a->ss_prob != nullptr;
   if (ragged && a->phase != 2) {
     LO_CUDA(cudaMemsetAsync(a->alphas, 0, (size_t)d.B * d.T * d.R * 4, st));
     LO_CUDA(cudaMemsetAsync(a->hd, 0, (size_t)d.B * d.T * d.D * 4, st));
+    const BfViews bz = bf_views(a, d);
+    if (sampling && bz.on) LO_CUDA(cudaMemsetAsync(bz.hd, 0, (size_t)d.B * d.T * d.D * 2, st));   // written by the cell in this mode
   }
+  if (sampling)     // the steps overwrite the positions they decode; the others keep the teacher token
+    LO_CUDA(cudaMemcpy2DAsync(a->fed, (size_t)d.T * 8, a->caps, (size_t)a->caps_stride * 8, (size_t)d.T * 8, d.B,
+                              cudaMemcpyDeviceToDevice, st));
   LO_TRY(upload_dlen(a, st));
   if (a->phase != 2) {
   LO_TRY(forward_prologue(a, d, st));
-  const int nchains = two_chains(a, d) ? 2 : 1;
+  const int nchains = two_chains(a, d) && !sampling ? 2 : 1;
   if (nchains == 2) {
     LO_TRY(side_stream_init());
     LO_CUDA(cudaEventRecord(g_ev_fork, st));
     LO_CUDA(cudaStreamWaitEvent(g_side, g_ev_fork, 0));
   }
   const BfViews bvs = bf_views(a, d);
-  const bool fused = bvs.on && g_opt_dec_fuse && g_opt_skinny_mma && !g_opt_fuse_lstm && g_opt_att_pipe && nchains == 1 && d.B <= 64 &&
+  const bool fused = bvs.on && !sampling && g_opt_dec_fuse && g_opt_skinny_mma && !g_opt_fuse_lstm && g_opt_att_pipe && nchains == 1 && d.B <= 64 &&
                      d.C == d.D && d.D <= 512 && d.D % 16 == 0 && d.O1 % 16 == 0 && d.E % 8 == 0 && a->rows_per_img <= 1;
-  const bool clf = bvs.on && !fused && !(g_opt_dbg_skip & 4) && g_opt_skinny_mma && !g_opt_fuse_lstm && g_opt_att_pipe && nchains == 1 && d.E % 8 == 0 &&
+  const bool clf = bvs.on && !sampling && !fused && !(g_opt_dbg_skip & 4) && g_opt_skinny_mma && !g_opt_fuse_lstm && g_opt_att_pipe && nchains == 1 && d.E % 8 == 0 &&
                    a->rows_per_img <= 1 && dec_cl_fwd_ok(d.D, d.C, d.O1);
   if (clf) {
     // two launches per step: attention(t) -> dec_cl_fwd(t) = [gates GEMM + LSTM cell | cluster all-gather | projection of h_{t+1}],
@@ -1418,7 +1517,9 @@ int lo_decoder_forward(const lo_decoder_args* a, int with_loss, void* stream) {
   // predictions = fc(dropout(h))  (seq2seq_torch.py:316), hoisted out of the loop
   const BfViews bvf = bf_views(a, d);
   const bool fc_tc = bvf.on && d.Vl % 64 == 0 && d.D % 64 == 0;
-  if (fc_tc) {
+  if (sampling) {
+    // the time loop wrote the logits (and, in bf16, the hd mirror the fc weight gradient reads)
+  } else if (fc_tc) {
     LO_TRY(lo_cast(a->hd, LO_F32, bvf.hd, LO_BF16, (int64_t)d.B * d.T * d.D, stream));
     LO_TRY(tc_gemm_nt_ex(bvf.hd, d.D, (const bf16*)a->w_fc, d.D, a->logits, LO_F32, d.Vl, d.B * d.T, d.V, d.D, a->b_fc, 0, 0, 1, 0, 0, st));
   } else {
@@ -1735,16 +1836,18 @@ int lo_decoder_backward(const lo_decoder_args* a, void* stream) {
                    LO_IMPL_SIMT, st));
   }
   LO_TRY(colsum(a->dcat + d.A + d.C, LO_F32, a->g_b_ih, d.T * d.B, d.G, d.O1, 0, st));
-  // embedding path through the projection table
+  // embedding path through the projection table, scattered by the tokens the forward fed (scheduled sampling: fed, else caps)
+  const int64_t* in_tok = a->ss_prob ? a->fed : a->caps;
+  const int64_t in_stride = a->ss_prob ? (int64_t)d.T : a->caps_stride;
   if (tc) {
     const int Vp = (d.V + 7) / 8 * 8;
-    onehot_kernel<<<LO_NUM_SMS * 8, 256, 0, st>>>(a->caps, a->caps_stride, work_dlen(a), bv.onehot, d.B, d.T, Vp);
+    onehot_kernel<<<LO_NUM_SMS * 8, 256, 0, st>>>(in_tok, in_stride, work_dlen(a), bv.onehot, d.B, d.T, Vp);
     LO_LAUNCH_OK();
     LO_CUDA(cudaMemsetAsync(a->dptab, 0, (size_t)d.V * d.G * 4, st));
     LO_TRY(tc_gemm_tn(bv.onehot, Vp, dcat_bf + d.A + d.C, d.O1, a->dptab, d.G, d.V, d.G, d.T * d.B, st));
   } else {
     dim3 grid(cdiv(d.G, 256), d.V);
-    dptab_kernel<<<grid, 256, 0, st>>>(a->dcat, d.O1, (int64_t)d.B * d.O1, d.A + d.C, a->caps, a->caps_stride, work_dlen(a), a->dptab,
+    dptab_kernel<<<grid, 256, 0, st>>>(a->dcat, d.O1, (int64_t)d.B * d.O1, d.A + d.C, in_tok, in_stride, work_dlen(a), a->dptab,
                                        d.B, d.T, d.G);
     LO_LAUNCH_OK();
   }
@@ -1847,8 +1950,9 @@ int lo_decoder_backward(const lo_decoder_args* a, void* stream) {
     add_rowbcast_kernel<<<LO_NUM_SMS * 8, 256, 0, st>>>(a->denc, a->dmean, d.R, d.C, 1.0f / (float)d.R, total);
     LO_LAUNCH_OK();
   }
-  if (a->has_dropout == 2) {
-    // forward and backward of this step drew the same Philox stream; the next step (also a graph replay) gets a new one
+  if (a->has_dropout == 2 || (a->ss_prob && a->dropout_state)) {
+    // forward and backward of this step drew the same Philox stream (dropout, sampling coins); the next step (also a graph
+    // replay) gets a new one
     bump_counter_kernel<<<1, 1, 0, st>>>((unsigned long long*)a->dropout_state + 1);
     LO_LAUNCH_OK();
   }
@@ -1858,6 +1962,7 @@ int lo_decoder_backward(const lo_decoder_args* a, void* stream) {
 int lo_decoder_greedy_hist(const lo_decoder_args* a, int64_t start_id, int64_t end_id, int max_steps, int64_t* tokens,
                            int32_t* finished, int32_t* fin_hist, void* stream) {
   LO_TRY(check_args(a));
+  LO_CHECK_ARG(!a->ss_prob, "scheduled sampling (ss_prob) is a training mode: greedy decode feeds its own argmax already");
   LO_CHECK_ARG(tokens && finished && max_steps > 0 && max_steps <= a->T, "tokens/finished/max_steps (<= T capacity)");
   cudaStream_t st = (cudaStream_t)stream;
   const Dims d = dims(a);
@@ -1900,6 +2005,7 @@ int lo_decoder_beam_div(const lo_decoder_args* a, int64_t start_id, int64_t end_
                         int32_t* fin_hist, float* logp, float div_gamma, float div_prob, const float* div_u,
                         const uint64_t* div_state, void* stream) {
   LO_TRY(check_args(a));
+  LO_CHECK_ARG(!a->ss_prob, "scheduled sampling (ss_prob) is a training mode: not available in beam search");
   const bool div_on = !(div_gamma == 1.f || div_prob == 0.f);               // beam_search_decoder_cell.py:270-273
   LO_CHECK_ARG(!div_on || (div_gamma > 0.f && (div_u || div_state)), "diversity penalty needs gamma > 0 and div_u or div_state");
   const int beam = a->rows_per_img;

@@ -177,6 +177,11 @@ class DecoderWithAttention(nn.Module):
         # in-kernel dropout (has_dropout=2): device {seed, call counter}; the counter is advanced by lo_decoder_backward, so
         # CUDA-graph replays draw a fresh mask every step
         self.dropout_state = torch.tensor([int(torch.initial_seed()) & 0x7FFFFFFFFFFFFFFF, 0], dtype=torch.int64, device=device)
+        # scheduled sampling (forward(..., sampling_prob=p)): the device scalar p the kernels read, created on first use; the
+        # tokens fed by the last forward ([B, T], sorted rows); injected coins [B, T] for parity tests (None: Philox)
+        self._ss_prob = None
+        self.last_fed_tokens = None
+        self._ss_u = None
 
     def seed_dropout(self, seed, call=0):
         self.dropout_state.copy_(torch.tensor([int(seed) & 0x7FFFFFFFFFFFFFFF, int(call)], dtype=torch.int64))
@@ -278,11 +283,18 @@ class DecoderWithAttention(nn.Module):
             ws["need_grad"] = True
         return ws
 
+    def _fed_buffer(self, ws):
+        """[B, T] int64 tokens fed by a scheduled-sampling forward (allocated on first use of the mode for this shape)."""
+        t = ws["t"]
+        if t.get("fed") is None:
+            t["fed"] = torch.zeros(t["hd"].shape[0], t["hd"].shape[1], dtype=torch.int64, device=self.store.device)
+        return t["fed"]
+
     def _ws_for(self, B, T, R):
         """The cached workspace of an exact shape (tests / bench probes)."""
         return self._ws[(B, T, R)]
 
-    def fill_args(self, ws, enc, B, T, R, has_dropout, dalpha_ext=None):
+    def fill_args(self, ws, enc, B, T, R, has_dropout, dalpha_ext=None, ss_prob=None):
         S, t = self.store, ws["t"]
         a = _lib.DecoderArgs()
         a.B, a.T, a.R = B, T, R
@@ -333,6 +345,11 @@ class DecoderWithAttention(nn.Module):
             a.g_w_fc, a.g_b_fc = Gd("fc.weight"), Gd("fc.bias")
         if dalpha_ext is not None:
             a.dalpha_ext = dalpha_ext.data_ptr()
+        if ss_prob is not None:                    # scheduled sampling: device p, the fed-token record, injected coins if any
+            a.ss_prob = ss_prob.data_ptr()
+            a.fed = self._fed_buffer(ws).data_ptr()
+            if self._ss_u is not None:
+                a.ss_u = self._ss_u.data_ptr()
         if a.impl == _lib.LO_IMPL_TC:
             if "bfwork" not in t:
                 t["bfwork"] = torch.zeros(int(_lib.lib().lo_decoder_bfwork_bytes(ctypes.byref(a))), dtype=torch.uint8, device=S.device)
@@ -374,10 +391,11 @@ class DecoderWithAttention(nn.Module):
         finally:
             a.phase = 0
 
-    def run_forward(self, enc_flat, caps_sorted, decode_lengths, with_loss, need_grad, dropout_mask=None, phase=0):
+    def run_forward(self, enc_flat, caps_sorted, decode_lengths, with_loss, need_grad, dropout_mask=None, phase=0, ss_prob=None):
         """enc_flat: storage-dtype CUDA [B,R,C] (sorted rows); caps_sorted: CUDA int64 [B,T+1].
         dropout_mask: None (no dropout), a [B,T,D] tensor of multipliers (injected, parity tests) or the string "philox"
-        (mask drawn inside the kernels)."""
+        (mask drawn inside the kernels).  ss_prob: None (teacher forcing) or a CUDA float32 scalar p: scheduled sampling, the
+        tokens fed land in ``ws["t"]["fed"]`` (the same argument block serves the backward, run_backward)."""
         L = _lib.lib()
         B, R, _ = enc_flat.shape
         T = max(decode_lengths)
@@ -391,7 +409,7 @@ class DecoderWithAttention(nn.Module):
                 ws["t"]["dropout_mask"] = torch.zeros(B, T, self.decoder_dim, dtype=torch.float32, device=self.store.device)
                 ws.pop("args", None)
             ws["t"]["dropout_mask"].copy_(dropout_mask)
-        a = self.fill_args(ws, enc_flat, B, T, R, has_do)
+        a = self.fill_args(ws, enc_flat, B, T, R, has_do, ss_prob=ss_prob)
         a.phase = int(phase)
         try:
             check(L.lo_decoder_forward(ctypes.byref(a), 1 if with_loss else 0, stream_ptr()))
@@ -415,21 +433,39 @@ class DecoderWithAttention(nn.Module):
         keep = torch.rand(B, T, self.decoder_dim, device=self.store.device) >= p
         return keep.float() / (1.0 - p)
 
-    def forward(self, encoder_out, encoded_captions, caption_lengths):
+    def forward(self, encoder_out, encoded_captions, caption_lengths, sampling_prob=0.0):
         """Reference signature and return tuple (seq2seq_torch.py:267-320): (predictions[B,maxT,V],
         sorted captions, decode_lengths(list), alphas[B,maxT,R], sort_ind).  With grad mode on and ``encoder_out`` or a
         parameter requiring grad, an autograd graph is recorded: ``predictions`` and ``alphas`` are differentiable (any loss of
-        them), and their backward runs lo_decoder_backward in its generic mode.  The outputs are the same either way."""
-        (preds, alphas), (caps, decode_lengths, sort_ind) = kernel_forward(self, (encoder_out, encoded_captions, caption_lengths),
-                                                                           (encoder_out,))
+        them), and their backward runs lo_decoder_backward in its generic mode.  The outputs are the same either way.
+
+        ``sampling_prob`` = p > 0: scheduled sampling (Bengio et al. 2015) inside the CUDA time loop.  Step t >= 1 of a row feeds
+        the argmax of the row's returned prediction of step t-1 (lowest index on ties) where a coin u ~ U[0,1) is below p, the
+        teacher token ``captions[b][t]`` otherwise; step 0 feeds ``captions[b][0]``.  The coins come from Philox keyed by the
+        dropout seed (one call counter per forward, also in eval mode; ``seed_dropout`` reproduces them).  Targets of a loss stay
+        ``captions[:, 1:]``; the choice is not differentiated: the backward is teacher forcing on the tokens fed, which
+        ``last_fed_tokens`` holds ([B, T] in sorted-row order, the teacher token past a row's length).  p = 0 runs the teacher-forced
+        path unchanged (``last_fed_tokens`` is then ``captions[:, :T]``)."""
+        (preds, alphas), (caps, decode_lengths, sort_ind) = kernel_forward(
+            self, (encoder_out, encoded_captions, caption_lengths, float(sampling_prob)), (encoder_out,))
         return preds, caps, decode_lengths, alphas, sort_ind
 
-    def _forward_impl(self, encoder_out, encoded_captions, caption_lengths, need_grad):
+    def _forward_impl(self, encoder_out, encoded_captions, caption_lengths, sampling_prob=0.0, need_grad=False):
         """((predictions, alphas), (captions, decode_lengths, sort_ind), what the backward of this call needs or None)."""
+        if not 0.0 <= sampling_prob <= 1.0:
+            raise ValueError("sampling_prob must lie in [0, 1] (got %r)" % (sampling_prob,))
         enc, caps, decode_lengths, sort_ind = self._sorted_inputs(encoder_out, encoded_captions, caption_lengths)
-        mask = self.make_dropout_mask(enc.shape[0], max(decode_lengths))
-        ws = self.run_forward(enc, caps, decode_lengths, with_loss=False, need_grad=need_grad, dropout_mask=mask)
-        return self._outputs(ws, encoder_out, enc, caps, decode_lengths, sort_ind, mask, need_grad)
+        T = max(decode_lengths)
+        mask = self.make_dropout_mask(enc.shape[0], T)
+        ss = None
+        if sampling_prob > 0.0:
+            if self._ss_prob is None:
+                self._ss_prob = torch.zeros((), dtype=torch.float32, device=self.store.device)
+            ss = self._ss_prob
+            ss.fill_(sampling_prob)
+        ws = self.run_forward(enc, caps, decode_lengths, with_loss=False, need_grad=need_grad, dropout_mask=mask, ss_prob=ss)
+        self.last_fed_tokens = ws["t"]["fed"].clone() if ss is not None else caps[:, :T]
+        return self._outputs(ws, encoder_out, enc, caps, decode_lengths, sort_ind, mask, need_grad, sampling=ss is not None)
 
     def _backward_impl(self, saved, dpreds, dalphas, need):
         """lo_decoder_backward in its generic mode: returns (d encoder_out in the caller's row order and shape,)."""
@@ -453,13 +489,14 @@ class DecoderWithAttention(nn.Module):
         caps = encoded_captions.to(enc.device)[sort_ind].contiguous()
         return enc, caps, (lens - 1).tolist(), sort_ind                             # :298
 
-    def _outputs(self, ws, encoder_out, enc, caps, decode_lengths, sort_ind, mask, need_grad):
+    def _outputs(self, ws, encoder_out, enc, caps, decode_lengths, sort_ind, mask, need_grad, sampling=False):
         """The return value of _forward_impl once the logits and alphas of the forward are in ``ws``."""
         T = max(decode_lengths)
         philox = isinstance(mask, str)
-        # the Philox {seed, call} this forward drew its dropout mask from; the backward regenerates the mask from this copy
-        dstate = self.dropout_state.clone() if need_grad and philox else None
-        if philox:
+        # the Philox {seed, call} this forward drew its dropout mask (and sampling coins) from; the backward regenerates the mask
+        # from this copy and advances the copy, not the live counter
+        dstate = self.dropout_state.clone() if need_grad and (philox or sampling) else None
+        if philox or sampling:
             self.dropout_state[1] += 1       # forward-only call: no lo_decoder_backward to advance the Philox call counter
         preds = ws["t"]["logits"][:, :, :self.vocab_size].clone()
         alphas = ws["t"]["alphas"].clone()
@@ -470,7 +507,8 @@ class DecoderWithAttention(nn.Module):
         saved = None
         if need_grad:
             saved = {"entries": [ws], "ws": ws, "enc": enc, "sort_ind": sort_ind, "shape": tuple(encoder_out.shape),
-                     "dtype": encoder_out.dtype, "has_do": 0 if mask is None else (2 if philox else 1), "dstate": dstate}
+                     "dtype": encoder_out.dtype, "has_do": 0 if mask is None else (2 if philox else 1), "dstate": dstate,
+                     "sampling": sampling}
         return (preds, alphas), (caps, decode_lengths, sort_ind), saved
 
     def _generic_backward_args(self, saved, dpreds):
@@ -481,7 +519,9 @@ class DecoderWithAttention(nn.Module):
         T = ws["t"]["hd"].shape[1]
         V = self.vocab_size
         dpred = dpreds.float().contiguous() if dpreds is not None else torch.zeros(B, T, V, device=enc.device)
-        a = self.fill_args(ws, enc, B, T, R, saved["has_do"])
+        # scheduled sampling: ss_prob is the mode flag of the backward (its value is not read), which scatters the embedding
+        # gradient by the recorded fed tokens
+        a = self.fill_args(ws, enc, B, T, R, saved["has_do"], ss_prob=self._ss_prob if saved.get("sampling") else None)
         dstate = None
         if saved["dstate"] is not None:
             dstate = saved["dstate"].clone()     # lo_decoder_backward advances the counter it is given

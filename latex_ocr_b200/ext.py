@@ -217,6 +217,12 @@ class DecoderLayer2(nn.Module):
         check(_lib.lib().lo_lstm_seq_backward(ctypes.byref(a), stream_ptr()))
 
 
+def _refuse_sampling(p):
+    if p:
+        raise _lib.LatexOcrB200Error("scheduled sampling is not available with the second decoder layer: the layer sits between the "
+                                     "LSTM cell and fc, so layer 1's time loop has no per-step prediction to feed back")
+
+
 class TwoLayerDecoder(nn.Module):
     """The whole two-layer decoder as one module over an existing DecoderWithAttention (layer 1, attention, fc) and
     DecoderLayer2, whose parameters and state_dict entries stay where they are.  ``forward`` has DecoderWithAttention.forward's
@@ -226,11 +232,13 @@ class TwoLayerDecoder(nn.Module):
         super().__init__()
         self.decoder, self.layer2 = decoder, layer2
 
-    def forward(self, encoder_out, encoded_captions, caption_lengths):
+    def forward(self, encoder_out, encoded_captions, caption_lengths, sampling_prob=0.0):
         """encoder_out [B,H',W',C] or [B,R,C]; returns (predictions [B,T,V], sorted captions, decode_lengths (list),
         alphas [B,T,R], sort_ind), rows sorted by length and outputs past a row's length zero.  With grad mode on and
         ``encoder_out`` or a parameter requiring grad, ``predictions`` and ``alphas`` are differentiable; the outputs are the
-        same either way."""
+        same either way.  Scheduled sampling (``sampling_prob`` > 0) is refused: the second layer sits between the cell and fc,
+        so the time loop of layer 1 has no per-step prediction to feed back."""
+        _refuse_sampling(sampling_prob)
         (preds, alphas), (caps, decode_lengths, sort_ind) = kernel_forward(self, (encoder_out, encoded_captions, caption_lengths),
                                                                            (encoder_out,))
         return preds, caps, decode_lengths, alphas, sort_ind
@@ -288,6 +296,9 @@ class Img2SeqRowModel(Img2SeqModel):
 
     def predict_batch(self, *a, **k):
         raise NotImplementedError("the row-encoder / two-layer extension offers the training path only")
+
+    def set_sampling_prob(self, p):
+        _refuse_sampling(float(p))
 
     def _keepalive(self):
         keep = super()._keepalive()

@@ -40,6 +40,10 @@ class Img2SeqModel:
         self._graphs = LRUCache()  # captured train-step graphs, one per (shapes, mode): bounded like the workspaces
         self.dist = None          # set by latex_ocr_b200.dist.attach(model)
         self.lr = float(getattr(config, "lr_init", 1e-3))
+        # scheduled sampling in the fused step: p (host copy) and the device scalar the kernels read (created when p first > 0)
+        self.sampling_prob = 0.0
+        self._ss_prob_dev = None
+        self.set_sampling_prob(getattr(config, "sampling_prob", 0.0) or 0.0)
 
     # --- model/base_torch.py:45-71 -------------------------------------------------------------
     def build_train(self, config=None):
@@ -74,6 +78,21 @@ class Img2SeqModel:
         self.lr = float(lr)
         self.encoder.store.set_lr(lr)
         self.decoder.store.set_lr(lr)
+
+    def set_sampling_prob(self, p):
+        """Scheduled sampling (Bengio et al. 2015) in the fused train step: from the next step on, each decoder step t >= 1 feeds
+        the model's own argmax prediction of step t-1 with probability p instead of the teacher token (DecoderWithAttention.forward
+        documents the rule).  p is a device scalar read by the kernels, so a captured step graph picks up a new p without
+        re-capture; p = 0 runs the teacher-forced step (its own graph).  No schedule is built in: set p per epoch.  The tokens fed
+        by the last step are ``self.decoder.last_fed_tokens`` (a view of the step's buffer)."""
+        p = float(p)
+        if not 0.0 <= p <= 1.0:
+            raise ValueError("sampling_prob must lie in [0, 1] (got %r)" % (p,))
+        self.sampling_prob = p
+        if p > 0.0:
+            if self._ss_prob_dev is None:
+                self._ss_prob_dev = torch.zeros((), dtype=torch.float32, device=self.device)
+            self._ss_prob_dev.fill_(p)
 
     def train_mode(self, flag=True):
         self.encoder.train(flag)
@@ -119,7 +138,10 @@ class Img2SeqModel:
         enc_out = self.encoder.forward_raw(img, need_grad=True)
         R = enc_out.shape[1] * enc_out.shape[2]
         enc_flat = enc_out.view(N, R, enc_out.shape[3])
-        ws = self.decoder.run_forward(enc_flat, caps, decode_lengths, with_loss=True, need_grad=True, dropout_mask=dropout_mask)
+        ss = self._ss_prob_dev if self.sampling_prob > 0.0 else None
+        ws = self.decoder.run_forward(enc_flat, caps, decode_lengths, with_loss=True, need_grad=True, dropout_mask=dropout_mask,
+                                      ss_prob=ss)
+        self.decoder.last_fed_tokens = ws["t"]["fed"] if ss is not None else None
         self.decoder.run_backward(ws)
         scale = 1.0
         if self.dist is not None:
@@ -176,7 +198,7 @@ class Img2SeqModel:
 
     def _graph_step(self, img_d, caps_d, decode_lengths):
         frozen = tuple(p_._lo_store_name for m_ in (self.encoder, self.decoder) for p_ in m_.parameters() if not p_.requires_grad)
-        key = (tuple(img_d.shape), img_d.dtype, tuple(caps_d.shape), self.decoder.training, frozen)
+        key = (tuple(img_d.shape), img_d.dtype, tuple(caps_d.shape), self.decoder.training, frozen, self.sampling_prob > 0.0)
         g = self._graphs.get(key)
         if g is None:
             N, T = caps_d.shape[0], caps_d.shape[1] - 1

@@ -4,6 +4,10 @@ dropout masks and beam-search diversity draws, and documenting the stream layout
   dropout multiplier of (row b, step t, unit j), call counter n, 64-bit seed s:
       words = philox4x32_10(counter = (j >> 2, t, b, n), key = (s & 0xffffffff, s >> 32));  u = (words[j & 3] >> 8) * 2**-24
       multiplier = 1/(1-p) if u >= p else 0                                   (nn.Dropout semantics, seq2seq_torch.py:316)
+
+  scheduled-sampling coin of (row b, step t) under the same {seed s, call n} (lo_decoder_args.ss_prob without ss_u):
+      u = (philox4x32_10(counter = (0xFFFFFFFF, t, b, n), key = (s & 0xffffffff, s >> 32))[0] >> 8) * 2**-24
+  a first counter word the dropout stream (j >> 2 < D / 4) never reaches; the model's own argmax is fed where u < p
 """
 import numpy as np
 
@@ -38,3 +42,12 @@ def dropout_multipliers(seed, call, B, T, D, p):
     w = philox4x32_10(j4 + 0 * b + 0 * t, t + 0 * b + 0 * j4, b + 0 * t + 0 * j4, np.uint64(call), seed & 0xFFFFFFFF, (seed >> 32) & 0xFFFFFFFF)
     u = np.stack([u01(x) for x in w], axis=-1).reshape(B, T, -1)[:, :, :D]
     return np.where(u >= np.float32(p), np.float32(1.0 / (1.0 - p)), np.float32(0.0)).astype(np.float32)
+
+
+def sampling_uniforms(seed, call, B, T):
+    """[B, T] float32 coins exactly as lstm_pw_fwd_kernel draws them in scheduled-sampling mode (row b, step t)."""
+    b = np.arange(B, dtype=np.uint64)[:, None]
+    t = np.arange(T, dtype=np.uint64)[None, :]
+    w = philox4x32_10(np.uint64(0xFFFFFFFF) + 0 * b + 0 * t, t + 0 * b, b + 0 * t, np.uint64(call), seed & 0xFFFFFFFF,
+                      (seed >> 32) & 0xFFFFFFFF)
+    return u01(w[0]).reshape(B, T)

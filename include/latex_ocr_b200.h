@@ -48,8 +48,9 @@ const char* lo_last_error(void);
 int64_t lo_launch_count(void);
 /* Run-time options.  lo_set_option sets one by name and accepts any int value (an unknown name is refused with LO_EINVAL);
  * lo_get_option reads it back (-1: unknown name); lo_option_name(i) is the i-th name, NULL past the last.  From Python,
- * LO_OPTS=name=value,... in the environment sets them when the library is loaded.  [p]: parity-tested, tests/test_gpu_tc.py or
- * tests/test_gpu_parity.py runs the other value against the default and requires the same results (measured A/B: DESIGN.md §8).
+ * LO_OPTS=name=value,... in the environment sets them when the library is loaded.  [p]: parity-tested, tests/test_gpu_tc.py,
+ * tests/test_gpu_parity.py or tests/test_gpu_attention_grid.py runs the other value against the default and requires the same
+ * results (measured A/B: DESIGN.md §8).
  *
  *   name             default  meaning
  *   att_pipe         1 [p]    attention step kernels: 1 TMA bulk-copy -> shared-memory ring, 0 register-streaming
@@ -58,7 +59,10 @@ int64_t lo_launch_count(void);
  *   att_policy_enc   1        L2 policy of the attention kernels' enc stream: 0 normal, 1 evict_last, 2 evict_first, 3 no hint
  *   att_policy_att1  2        the same for their att1 stream
  *   att_nsplit       0        splits of one batch row in the attention kernels; 0: automatic
- *   att_cluster      1        1: the splits of a batch row form a thread-block cluster and combine through distributed shared memory
+ *   att_cluster      1 [p]    how the splits of a batch row meet.  Forward kernel and 512-wide tensor-core backward: 1 launches them
+ *                             without a cluster (the last CTA of a row combines the partials in split order) when that grid is one
+ *                             resident wave, else as a thread-block cluster combining through distributed shared memory; 2 always
+ *                             as a cluster; 0 never.  The other attention kernels: cluster unless 0.  Same results for 1 and 2
  *   att_maskbits     1 [p]    1: the forward attention kernel stores the ReLU mask bits, the backward streams them instead of att1
  *   att_bwd_mma      1 [p]    1: the 512-wide bf16 attention backward runs both contractions on mma.sync
  *   dec_streams      1 [p]    >= 2: the decoder time loop runs as two half-batch chains on two streams; also sets skinny8 = value < 2

@@ -9,6 +9,9 @@
 // tensor-core backward streams enc evict_first (attention_bwd_mma_kernel launch).
 #include <cooperative_groups.h>
 
+#include <mutex>
+#include <vector>
+
 #include "lo_common.cuh"
 #include "lo_ptx.cuh"
 
@@ -96,8 +99,7 @@ __global__ void __launch_bounds__(AP_THREADS, LO_ATT_MINB) attention_fwd_pipe_ke
   uint64_t* empty_bar = full_bar + AP_STAGES;
   float* s_e = reinterpret_cast<float*>(ap_smem + AP_STAGES * C::STAGE_BYTES + 128);   // cluster mode: raw scores of this CTA's rows
   __shared__ float s_m[AP_CWARPS], s_l[AP_CWARPS];
-  __shared__ float s_scale[AP_MAXSPLIT];
-  __shared__ float s_ML[2];
+  __shared__ float s_msplit[AP_MAXSPLIT], s_lsplit[AP_MAXSPLIT];     // cluster-free combine: (M, L) of every split
   __shared__ int s_last;
 
   const int b = blockIdx.y, sp = blockIdx.x;
@@ -244,6 +246,18 @@ __global__ void __launch_bounds__(AP_THREADS, LO_ATT_MINB) attention_fwd_pipe_ke
     }
   }
   ATT_TS(4, threadIdx.x == 0);
+  // cluster-free: the gate pre-activations of the channels this thread finalises should its CTA combine last (channel c = tid +
+  // k * AP_THREADS, below).  Fetched here, so that the load hides behind the CTA combine and the ticket instead of sitting on the
+  // last CTA's tail; only that CTA uses them.  Nothing else writes gate_pre before that CTA's ticket.
+  constexpr int NCI = (CHC + AP_THREADS - 1) / AP_THREADS;
+  float gpf[NCI];
+  if constexpr (!CL) {
+#pragma unroll
+    for (int k = 0; k < NCI; k++) {
+      const int c = threadIdx.x + k * AP_THREADS;
+      gpf[k] = (gate_pre && c < CHC) ? gate_pre[(int64_t)b * gate_stride + c] : 0.f;
+    }
+  }
   __syncthreads();     // every TMA write has landed and been consumed: the ring can be reused for the combine
   ATT_TS(8, threadIdx.x == 0);
   float* s_acc = reinterpret_cast<float*>(ap_smem);          // [AP_CWARPS][CHC]
@@ -334,39 +348,72 @@ __global__ void __launch_bounds__(AP_THREADS, LO_ATT_MINB) attention_fwd_pipe_ke
     if (s_last) counters[b] = 0;
   }
   __syncthreads();
-  if (!s_last) return;
+  if (!s_last) {
+    ATT_TS(5, threadIdx.x == 0);
+    return;
+  }
   __threadfence();
+  ATT_TS(9, threadIdx.x == 0);
+  // ===== ordered combine by the CTA that took the last ticket: the same operations in the same split order as the cluster combine.
+  // Every load it needs is issued before the first use: the splits' (M, L) into shared memory, this thread's partial sums of its
+  // first channel and its first raw scores into registers, so the tail costs about one L2 round trip instead of a chain of them.
   const float* pb = partials + (int64_t)b * nsplit * (CHC + 2);
-  if (threadIdx.x == 0) {
-    float Mg = -INFINITY;
-    for (int s = 0; s < nsplit; s++) Mg = fmaxf(Mg, __ldcg(pb + (int64_t)s * (CHC + 2)));
-    float Lg = 0.f;
-    for (int s = 0; s < nsplit; s++) {
-      const float ms = __ldcg(pb + (int64_t)s * (CHC + 2));
-      const float scl = (ms == -INFINITY) ? 0.f : expf(ms - Mg);
-      s_scale[s] = scl;
-      Lg += __ldcg(pb + (int64_t)s * (CHC + 2) + 1) * scl;
-    }
-    s_ML[0] = Mg;
-    s_ML[1] = 1.0f / Lg;
+  constexpr int PS = 8;      // partial sums of a channel held in registers; splits beyond PS are read in the loop
+  constexpr int RB = 4;      // raw scores per thread held in registers; rows beyond RB * AP_THREADS are read in the loop
+  if ((int)threadIdx.x < nsplit) {
+    s_msplit[threadIdx.x] = __ldcg(pb + (int64_t)threadIdx.x * (CHC + 2));          // M of split tid
+    s_lsplit[threadIdx.x] = __ldcg(pb + (int64_t)threadIdx.x * (CHC + 2) + 1);       // L of split tid
+  }
+  float pv[PS], ev[RB];
+  auto load_parts = [&](int c) {
+#pragma unroll
+    for (int s = 0; s < PS; s++) pv[s] = s < nsplit ? __ldcg(pb + (int64_t)s * (CHC + 2) + 2 + c) : 0.f;
+  };
+  if ((int)threadIdx.x < CHC) load_parts(threadIdx.x);
+#pragma unroll
+  for (int k = 0; k < RB; k++) {
+    const int r = threadIdx.x + k * AP_THREADS;
+    ev[k] = r < R ? __ldcg(alb + r) : 0.f;
   }
   __syncthreads();
-  const float Mg = s_ML[0], invL = s_ML[1];
-  for (int c = threadIdx.x; c < CHC; c += AP_THREADS) {
-    float t = 0.f;
-    for (int s = 0; s < nsplit; s++) t = fmaf(__ldcg(pb + (int64_t)s * (CHC + 2) + 2 + c), s_scale[s], t);
-    t *= invL;
-    ctx[(int64_t)b * CHC + c] = t;
-    if (gate_pre) {
-      const float g = sigmoidf_(gate_pre[(int64_t)b * gate_stride + c]);
-      gate_pre[(int64_t)b * gate_stride + c] = g;
-      gctx[(int64_t)b * CHC + c] = g * t;
-      if (gctx_bf) gctx_bf[(int64_t)b * CHC + c] = __float2bfloat16_rn(g * t);
-    } else if (gctx_bf) {
-      gctx_bf[(int64_t)b * CHC + c] = __float2bfloat16_rn(t);
+  float Mg = -INFINITY;
+  for (int s = 0; s < nsplit; s++) Mg = fmaxf(Mg, s_msplit[s]);
+  auto split_scale = [&](int s) {
+    const float ms = s_msplit[s];
+    return (ms == -INFINITY) ? 0.f : expf(ms - Mg);
+  };
+  float Lg = 0.f;
+  for (int s = 0; s < nsplit; s++) Lg += s_lsplit[s] * split_scale(s);
+  const float invL = 1.0f / Lg;
+#pragma unroll
+  for (int k = 0; k < NCI; k++) {
+    const int c = threadIdx.x + k * AP_THREADS;
+    if (c < CHC) {
+      if (k > 0) load_parts(c);
+      float t = 0.f;
+#pragma unroll
+      for (int s = 0; s < PS; s++)
+        if (s < nsplit) t = fmaf(pv[s], split_scale(s), t);
+      for (int s = PS; s < nsplit; s++) t = fmaf(__ldcg(pb + (int64_t)s * (CHC + 2) + 2 + c), split_scale(s), t);
+      t *= invL;
+      ctx[(int64_t)b * CHC + c] = t;
+      if (gate_pre) {
+        const float g = sigmoidf_(gpf[k]);
+        gate_pre[(int64_t)b * gate_stride + c] = g;
+        gctx[(int64_t)b * CHC + c] = g * t;
+        if (gctx_bf) gctx_bf[(int64_t)b * CHC + c] = __float2bfloat16_rn(g * t);
+      } else if (gctx_bf) {
+        gctx_bf[(int64_t)b * CHC + c] = __float2bfloat16_rn(t);
+      }
     }
   }
-  for (int r = threadIdx.x; r < R; r += AP_THREADS) alb[r] = expf(__ldcg(alb + r) - Mg) * invL;
+#pragma unroll
+  for (int k = 0; k < RB; k++) {
+    const int r = threadIdx.x + k * AP_THREADS;
+    if (r < R) alb[r] = expf(ev[k] - Mg) * invL;
+  }
+  for (int r = threadIdx.x + RB * AP_THREADS; r < R; r += AP_THREADS) alb[r] = expf(__ldcg(alb + r) - Mg) * invL;
+  ATT_TS(5, threadIdx.x == 0);
 }
 
 // DA1 (lo_attention_step_backward, a single Attention.forward call): while a stage is resident the consumer warps also store
@@ -892,16 +939,17 @@ __global__ void __launch_bounds__(AP_THREADS, LO_ATT_MINB) attention_bwd_mask_ke
 // [even(q) | even(q+4) | odd(q) | odd(q+4)] (q = lane % 4: fragment k index = region row).  Fragment row m = g + 8h of block j
 // stands for attention column 64w + 8g + 2j + h (g = lane / 4): any bijection works, this one makes a lane's 8 columns one byte.
 // ------------------------------------------------------------------------------------------------------------------------------
-// Ring depth and CTAs per SM.  The grid stays one wave at 2 CTAs per SM (att_pipe_splits: 4 splits at B = 64, the same row
-// partition and so the same sums as before), but the ring is sized so that 3 CTAs fit per SM.  On the H100 a one-wave grid of
-// 4-CTA clusters with exactly 2 slots per SM did not become resident at once: about an eighth of the CTAs entered only when others
-// exited and the launch ended in a second wave of full-length CTAs.  The spare slot lets every cluster be placed at launch.
-// Backward time loop at B = 64 (H100 SXM, 400 W), us per step: 5 stages / 2 per SM 53.2, 4 / 3 48.0, 3 / 3 47.6.
+// Ring depth and CTAs per SM.  The grid is one wave at 2 CTAs per SM (att_pipe_splits: 4 splits at B = 64).  On the H100 a
+// one-wave grid of 4-CTA clusters with exactly 2 slots per SM did not become resident at once: about an eighth of the CTAs entered
+// only when others exited and the launch ended in a second wave of full-length CTAs.  With clusters, a 3-stage ring that lets 3
+// CTAs share an SM was the cure (backward time loop at B = 64, H100 SXM, 400 W, us per step: 5 stages / 2 per SM 53.2, 4 / 3 48.0,
+// 3 / 3 47.6).  The default launch has no cluster (att_grid_cluster): 256 independent CTAs fill 264 slots, and the deeper ring at
+// 2 per SM wins (same card, cluster-free: 3 / 3 45.4, 4 / 2 42.8, 5 / 2 41.7).
 #ifndef LO_ABM_STAGES
-#define LO_ABM_STAGES 3
+#define LO_ABM_STAGES 5
 #endif
 #ifndef LO_ABM_MINB
-#define LO_ABM_MINB 3
+#define LO_ABM_MINB 2
 #endif
 constexpr int ABM_STAGES = LO_ABM_STAGES;
 constexpr int ABM_ROWS = 16;
@@ -1136,6 +1184,20 @@ __global__ void __launch_bounds__(AP_THREADS, LO_ABM_MINB) attention_bwd_mma_ker
     }
   }
   ATT_TS(4, threadIdx.x == 0);
+  // cluster-free: full_att weight, att2 and the running d w_full sum of the columns this thread finalises should its CTA combine
+  // last (column c = tid + k * AP_THREADS, below): fetched now, behind the CTA combine and the ticket.  Only the last CTA of this
+  // batch row writes its d w_full row, after its ticket.
+  constexpr int NCB = (CH + AP_THREADS - 1) / AP_THREADS;
+  float wf_t[NCB], a2_t[NCB], dwf_t[NCB];
+  if constexpr (!CL) {
+#pragma unroll
+    for (int k = 0; k < NCB; k++) {
+      const int c = threadIdx.x + k * AP_THREADS;
+      wf_t[k] = c < CH ? wf[c] : 0.f;
+      a2_t[k] = (dwf_part && c < CH) ? att2[(int64_t)b * o1_stride + c] : 0.f;
+      dwf_t[k] = (dwf_part && c < CH) ? dwf_part[(int64_t)b * CH + c] : 0.f;
+    }
+  }
   __syncthreads();
   ATT_TS(8, threadIdx.x == 0);
   float* s_part = reinterpret_cast<float*>(ap_smem);             // [CH] mask sums of this CTA (every column has ONE owner lane)
@@ -1185,16 +1247,33 @@ __global__ void __launch_bounds__(AP_THREADS, LO_ABM_MINB) attention_bwd_mma_ker
     if (s_last) counters[b] = 0;
   }
   __syncthreads();
-  if (!s_last) return;
-  __threadfence();
-  const float* pb = partials + (int64_t)b * nsplit * (CH + 2);
-  for (int c = threadIdx.x; c < CH; c += AP_THREADS) {
-    float t = 0.f;
-    for (int sidx = 0; sidx < nsplit; sidx++) t += __ldcg(pb + (int64_t)sidx * (CH + 2) + 2 + c);
-    if (dwf_part) dwf_part[(int64_t)b * CH + c] += t * att2[(int64_t)b * o1_stride + c];
-    datt2[(int64_t)b * dcat_stride + c] = t * wf[c];
-    if (datt2_bf) datt2_bf[(int64_t)b * dcat_stride + c] = __float2bfloat16_rn(t * wf[c]);
+  if (!s_last) {
+    ATT_TS(5, threadIdx.x == 0);
+    return;
   }
+  __threadfence();
+  ATT_TS(9, threadIdx.x == 0);
+  // ordered combine, split order 0..nsplit-1 as in the cluster combine; the partial sums of a column are loaded together
+  const float* pb = partials + (int64_t)b * nsplit * (CH + 2);
+  constexpr int PS = 8;
+#pragma unroll
+  for (int k = 0; k < NCB; k++) {
+    const int c = threadIdx.x + k * AP_THREADS;
+    if (c < CH) {
+      float pv[PS];
+#pragma unroll
+      for (int s = 0; s < PS; s++) pv[s] = s < nsplit ? __ldcg(pb + (int64_t)s * (CH + 2) + 2 + c) : 0.f;
+      float t = 0.f;
+#pragma unroll
+      for (int s = 0; s < PS; s++)
+        if (s < nsplit) t += pv[s];
+      for (int s = PS; s < nsplit; s++) t += __ldcg(pb + (int64_t)s * (CH + 2) + 2 + c);
+      if (dwf_part) dwf_part[(int64_t)b * CH + c] = dwf_t[k] + t * a2_t[k];
+      datt2[(int64_t)b * dcat_stride + c] = t * wf_t[k];
+      if (datt2_bf) datt2_bf[(int64_t)b * dcat_stride + c] = __float2bfloat16_rn(t * wf_t[k]);
+    }
+  }
+  ATT_TS(5, threadIdx.x == 0);
 }
 
 int att_pipe_splits(int B, int hint = 0) {
@@ -1255,6 +1334,38 @@ static inline bool use_cluster(int ns, int R) {
   return g_opt_att_cluster && ns >= 2 && ns <= 8 && ((R + ns - 1) / ns) * 4 <= 16 * 1024;
 }
 
+// Resident CTAs of `kernel` at `smem` bytes of dynamic shared memory on the whole device.  Queried once per (device, kernel,
+// shared memory) and cached: the launch paths call this on every step, also while a CUDA graph is being captured.
+static int att_resident_ctas(const void* kernel, size_t smem) {
+  struct Entry { int dev; const void* k; size_t smem; int ctas; };
+  static std::mutex mu;
+  static std::vector<Entry> cache;
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 0;
+  std::lock_guard<std::mutex> lock(mu);
+  for (const Entry& e : cache)
+    if (e.dev == dev && e.k == kernel && e.smem == smem) return e.ctas;
+  int per_sm = 0, sms = 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, AP_THREADS, smem) != cudaSuccess ||
+      cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) {
+    cudaGetLastError();
+    return 0;                    // unknown: the caller keeps the cluster launch
+  }
+  cache.push_back({dev, kernel, smem, per_sm * sms});
+  return per_sm * sms;
+}
+
+// Grid choice of the forward pipe kernel and the tensor-core backward (att_cluster): 2 always launches the splits of a batch row as
+// a thread-block cluster, 0 never; 1 (default) launches without a cluster whenever the cluster-free grid of ns * B CTAs is one
+// resident wave.  Both combines add the nsplit partials in split order with the same operations, so the choice changes timing only.
+// Why: cluster placement could not fill the last slots of a 2-CTA-per-SM grid (4 x 64 CTAs in 2 x 132 slots on the H100), and
+// about an eighth of the CTAs ran as a second wave; 256 independent CTAs are all resident at launch.
+static bool att_grid_cluster(const void* free_kernel, size_t free_smem, int ns, int B, int R) {
+  if (!use_cluster(ns, R)) return false;
+  if (g_opt_att_cluster != 1) return true;
+  return att_resident_ctas(free_kernel, free_smem) < ns * B;
+}
+
 template <typename T, int NVA, int NVC, int ACT, bool MK>
 static int fwd_launch_m(const AttFwdArgs& x, cudaStream_t st) {
   using C = ApCfg<T, NVA, NVC>;
@@ -1267,7 +1378,7 @@ static int fwd_launch_m(const AttFwdArgs& x, cudaStream_t st) {
   }
   const int ns = att_pipe_splits(x.B, x.nsplit_hint);
   const int rpi = x.rows_per_img > 1 ? x.rows_per_img : 1;
-  if (use_cluster(ns, x.R)) {
+  if (att_grid_cluster((const void*)attention_fwd_pipe_kernel<T, NVA, NVC, false, ACT, MK>, (size_t)C::SMEM, ns, x.B, x.R)) {
     const size_t smem = C::SMEM + (size_t)((x.R + ns - 1) / ns) * 4;
     LO_CUDA(launch_att(attention_fwd_pipe_kernel<T, NVA, NVC, true, ACT, MK>, dim3(ns, x.B), smem, ns, st, att_pdl_ok(x.abi), (const T*)x.att1, (const T*)x.enc,
                        x.att2, x.att2_stride, x.wf, x.alpha, x.alpha_stride, x.ctx, x.gate_pre, x.gate_stride, x.gctx, x.gctx_bf, x.R, ns,
@@ -1362,7 +1473,7 @@ static int bwd_launch_a(const AttBwdArgs& x, cudaStream_t st) {
     // enc evict_first (policy 2) whatever att_policy_enc says: the 57 MB of enc do not fit the H100's 50 MB L2 and are read once per
     // launch; measured faster than evict_last in the backward loop (47.0 vs 48.1 us per step; in the forward loop it was slower)
     const size_t smem_t = (size_t)ABM_SMEM + (size_t)att_rows_per_split(x.R, ns) * 8;      // + alpha / d reg of the CTA's rows
-    if (use_cluster(ns, x.R)) {
+    if (att_grid_cluster((const void*)attention_bwd_mma_kernel<false>, smem_t, ns, x.B, x.R)) {
       LO_CUDA(launch_att(attention_bwd_mma_kernel<true>, dim3(ns, x.B), smem_t, ns, st, att_pdl_ok(x.abi), LO_BWDT_ARGS));
     } else {
       LO_CUDA(launch_att(attention_bwd_mma_kernel<false>, dim3(ns, x.B), smem_t, 1, st, att_pdl_ok(x.abi), LO_BWDT_ARGS));

@@ -1,7 +1,10 @@
 """(build the timing variant first: LO_LIB_DIR=_C_timing LO_NVCC_EXTRA=-DLO_ATT_TIMING python -m latex_ocr_b200.build)
 Per-CTA timeline of the attention step kernels (timing build: LO_LIB_DIR=_C_timing, built with -DLO_ATT_TIMING).
 Stamps (%globaltimer, ns): 0 entry, 1 consumer past griddepcontrol.wait, 2 consumer prologue done, 3 first stage landed,
-4 main loop done, 8 after the CTA barrier, 5 exit; producer: 6 first stage issued, 7 last stage issued."""
+4 main loop done, 8 after the CTA barrier, 9 last ticket taken (cluster-free combine), 5 exit; producer: 6 first stage issued,
+7 last stage issued.  Both grids of the forward and the tensor-core backward are timed in one run: att_cluster=2 (every launch a
+cluster) and att_cluster=1 (the default: cluster-free when that grid is one resident wave); per launch it reports the CTAs that
+enter more than 5 us after the first one (a second wave), the launch span and the median main loop."""
 import ctypes, os, sys
 os.environ.setdefault("LO_LIB_DIR", "_C_timing")
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -58,6 +61,10 @@ def bwd(s):
 def report(name, n=256):
     x = buf.cpu().numpy().reshape(-1, 16)[:n].astype(np.float64)
     t0 = x[:, 0].min()
+    late = int(((x[:, 0] - t0) > 5e3).sum())
+    wave2 = int((x[:, 0] > x[:, 5].min()).sum())        # entered only after a CTA of the same launch had exited
+    loop = np.median(x[:, 4] - x[:, 3]) / 1e3
+    span = (x[:, 5].max() - t0) / 1e3
     def col(k):
         v = (x[:, k] - t0) / 1e3
         return "%6.2f / %6.2f / %6.2f" % (v.min(), np.median(v), v.max())
@@ -65,18 +72,26 @@ def report(name, n=256):
     for k, lab in ((0, "entry"), (6, "producer: first stage issued"), (1, "consumer past griddepcontrol.wait"), (2, "consumer prologue done"),
                    (3, "first stage landed"), (7, "producer: last stage issued"), (4, "main loop done"), (8, "after CTA barrier"), (5, "exit")):
         print("  %-36s %s" % (lab, col(k)))
-    print("  span first entry -> last exit: %.2f us" % ((x[:, 5].max() - t0) / 1e3), flush=True)
+    print("  span first entry -> last exit: %.2f us" % span, flush=True)
+    print("  summary: %d of %d CTAs enter > 5 us after the first (under PDL the first ones enter during the preceding launch), "
+          "%d after a CTA of this launch exited (second wave), span %.2f us, median main loop (first stage -> loop done) %.2f us" % (
+              late, n, wave2, span, loop), flush=True)
 
 
-for name, fn in (("forward (mask emission), back-to-back launches", fwd), ("backward (mma), back-to-back launches", bwd)):
-    for rep in range(2):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for s in range(40):
-            fn(s)
-        e1.record(); torch.cuda.synchronize()
-    print("%s: %.2f us per launch" % (name, e0.elapsed_time(e1) / 40 * 1e3))
-    report(name)
+for cl in (2, 1):
+    _lib.set_option("att_cluster", cl)
+    for name, fn in (("forward (mask emission), back-to-back launches", fwd), ("backward (mma), back-to-back launches", bwd)):
+        name = "%s, att_cluster=%d" % (name, cl)
+        for rep in range(2):
+            buf.zero_()
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            for s in range(40):
+                fn(s)
+            e1.record(); torch.cuda.synchronize()
+        print("%s: %.2f us per launch" % (name, e0.elapsed_time(e1) / 40 * 1e3))
+        report(name)
+_lib.set_option("att_cluster", 1)
 # in situ: one eager train step; the last attention launch is the backward of step 0
 m.train_step(img, formula); torch.cuda.synchronize()
 report("backward of step 0 inside a train step (eager launches)")

@@ -265,7 +265,8 @@ typedef struct lo_decoder_args {
                                  regenerated in the backward; nothing is stored) */
   int32_t ldl;             /* row stride of logits/dlogits (>= V; a multiple of 64 enables the wgmma fc GEMMs); 0 -> V */
   float alpha_c;           /* doubly-stochastic regulariser weight (img2seq_torch.py:157) */
-  int32_t rows_per_img;    /* decode only: consecutive rows that share one image (beam size); 0/1 for training */
+  int32_t rows_per_img;    /* decode only: consecutive rows that share one image (beam size); 0/1 for training.  Images of
+                              different sizes: reg_off / reg_off_host below */
   int32_t phase;           /* 0: whole call (default).  EXTENSION (a second decoder layer between the cell and fc): 1 = time loop
                               only — lo_decoder_forward stops after writing hd, lo_decoder_backward starts from the dhd the caller
                               put there; 2 = head only — logits + loss from whatever the caller left in hd, backward of fc -> dhd.
@@ -360,6 +361,15 @@ typedef struct lo_decoder_args {
   float* g_w_ih; float* g_b_ih;
   float* g_w_init; float* g_b_init;
   float* g_w_fc; float* g_b_fc;
+  /* decode of images of different sizes (lo_decoder_greedy[_hist] and lo_decoder_beam[_div] only): prefix offsets of the images'
+   * regions, [B / rows_per_img + 1] each, the same values on the device and on the host.  Image i owns regions [reg_off[i],
+   * reg_off[i+1]) of a PACKED enc [reg_off[n]][C] and att1 [reg_off[n]][A] (n = B / rows_per_img; beam rows share their image's
+   * regions).  R is then the largest count: the row stride of alphas [B][T][R], whose entries past an image's own count are left
+   * untouched.  Every image attends over its own regions only, so its tokens are those it gets when decoded alone.  Both NULL:
+   * every image has R regions ([n][R][.]).  Refused (LO_EINVAL) before any GPU work: one set without the other, either on
+   * lo_decoder_forward / lo_decoder_backward, reg_off_host[0] != 0, a count below 1 or above R, and att_pipe = 0. */
+  const int32_t* reg_off;
+  const int32_t* reg_off_host;
   void* work;              /* lo_decoder_workspace_bytes(B, max(A,C)), zero-initialised once */
   void* bfwork;            /* optional (impl=TC, dt=bf16): bf16 staging for the hoisted wgmma GEMMs,
                               lo_decoder_bfwork_bytes(args) bytes */

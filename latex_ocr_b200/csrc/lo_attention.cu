@@ -85,12 +85,17 @@ struct ApCfg {
   static constexpr int SMEM = AP_STAGES * STAGE_BYTES + 128;
 };
 
+// The work of one CTA: split sp of the nsplit splits of batch row b, which attends over the R regions of its image, rows g0.. of
+// att1 / enc.  The CTA streams regions [sp * ceil(R / nsplit), ...) and, cluster-free, writes its partial sums to split slot
+// pbase + sp of `partials` (pbase: the row's first slot) and takes a ticket at counters[b].  Called by the dense kernel (every row has
+// R regions and nsplit splits) and by the ragged one (per-row R and nsplit from its CTA map).
 template <typename T, int NVA, int NVC, bool CL, int ACT, bool MK>
-__global__ void __launch_bounds__(AP_THREADS, LO_ATT_MINB) attention_fwd_pipe_kernel(
+__device__ __forceinline__ void attention_fwd_pipe_cta(
     const T* __restrict__ att1, const T* __restrict__ enc, const float* __restrict__ att2, int64_t att2_stride,
     const float* __restrict__ wf, float* __restrict__ alpha, int64_t alpha_stride, float* __restrict__ ctx,
     float* __restrict__ gate_pre, int64_t gate_stride, float* __restrict__ gctx, bf16* __restrict__ gctx_bf, int R, int nsplit,
-    int* __restrict__ counters, float* __restrict__ partials, int pol_enc, int pol_att1, int rpi, uint8_t* __restrict__ mask_out) {
+    int* __restrict__ counters, float* __restrict__ partials, int pol_enc, int pol_att1, uint8_t* __restrict__ mask_out, int b, int sp,
+    int64_t g0, int64_t pbase) {
   using C = ApCfg<T, NVA, NVC>;
   constexpr int CHA = C::CHA, CHC = C::CHC;
   extern __shared__ __align__(128) uint8_t ap_smem[];
@@ -102,13 +107,12 @@ __global__ void __launch_bounds__(AP_THREADS, LO_ATT_MINB) attention_fwd_pipe_ke
   __shared__ float s_msplit[AP_MAXSPLIT], s_lsplit[AP_MAXSPLIT];     // cluster-free combine: (M, L) of every split
   __shared__ int s_last;
 
-  const int b = blockIdx.y, sp = blockIdx.x;
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const int rps = (R + nsplit - 1) / nsplit;
   const int r0 = sp * rps, r1 = min(R, r0 + rps);
   const int nst = r1 > r0 ? (r1 - r0 + C::ROWS - 1) / C::ROWS : 0;
-  const T* a1b = att1 + (int64_t)(b / rpi) * R * CHA;      // beam search: rpi consecutive rows attend over one image
-  const T* eb = enc + (int64_t)(b / rpi) * R * CHC;
+  const T* a1b = att1 + g0 * CHA;
+  const T* eb = enc + g0 * CHC;
   float* alb = alpha + (int64_t)b * alpha_stride;
   ATT_TS(0, threadIdx.x == 0);
 
@@ -332,7 +336,7 @@ __global__ void __launch_bounds__(AP_THREADS, LO_ATT_MINB) attention_fwd_pipe_ke
     ATT_TS(5, threadIdx.x == 0);
     return;
   }
-  float* part = partials + ((int64_t)b * nsplit + sp) * (CHC + 2);
+  float* part = partials + (pbase + sp) * (CHC + 2);
   for (int c = threadIdx.x; c < CHC; c += AP_THREADS) {
     float t = 0.f;
 #pragma unroll
@@ -357,7 +361,7 @@ __global__ void __launch_bounds__(AP_THREADS, LO_ATT_MINB) attention_fwd_pipe_ke
   // ===== ordered combine by the CTA that took the last ticket: the same operations in the same split order as the cluster combine.
   // Every load it needs is issued before the first use: the splits' (M, L) into shared memory, this thread's partial sums of its
   // first channel and its first raw scores into registers, so the tail costs about one L2 round trip instead of a chain of them.
-  const float* pb = partials + (int64_t)b * nsplit * (CHC + 2);
+  const float* pb = partials + pbase * (CHC + 2);
   constexpr int PS = 8;      // partial sums of a channel held in registers; splits beyond PS are read in the loop
   constexpr int RB = 4;      // raw scores per thread held in registers; rows beyond RB * AP_THREADS are read in the loop
   if ((int)threadIdx.x < nsplit) {
@@ -414,6 +418,68 @@ __global__ void __launch_bounds__(AP_THREADS, LO_ATT_MINB) attention_fwd_pipe_ke
   }
   for (int r = threadIdx.x + RB * AP_THREADS; r < R; r += AP_THREADS) alb[r] = expf(__ldcg(alb + r) - Mg) * invL;
   ATT_TS(5, threadIdx.x == 0);
+}
+
+// Dense layout: grid (nsplit, B), every image R regions, att1 / enc [B / rpi][R][.].
+template <typename T, int NVA, int NVC, bool CL, int ACT, bool MK>
+__global__ void __launch_bounds__(AP_THREADS, LO_ATT_MINB) attention_fwd_pipe_kernel(
+    const T* __restrict__ att1, const T* __restrict__ enc, const float* __restrict__ att2, int64_t att2_stride,
+    const float* __restrict__ wf, float* __restrict__ alpha, int64_t alpha_stride, float* __restrict__ ctx,
+    float* __restrict__ gate_pre, int64_t gate_stride, float* __restrict__ gctx, bf16* __restrict__ gctx_bf, int R, int nsplit,
+    int* __restrict__ counters, float* __restrict__ partials, int pol_enc, int pol_att1, int rpi, uint8_t* __restrict__ mask_out) {
+  const int b = blockIdx.y, sp = blockIdx.x;
+  // beam search: rpi consecutive rows attend over one image
+  attention_fwd_pipe_cta<T, NVA, NVC, CL, ACT, MK>(att1, enc, att2, att2_stride, wf, alpha, alpha_stride, ctx, gate_pre, gate_stride, gctx,
+                                                  gctx_bf, R, nsplit, counters, partials, pol_enc, pol_att1, mask_out, b, sp,
+                                                  (int64_t)(b / rpi) * R, (int64_t)b * nsplit);
+}
+
+// Ragged layout (decode of images of different sizes): image i owns regions [reg_off[i], reg_off[i+1]) of the packed att1 / enc.
+// One-dimensional cluster-free grid; CTA x does the work cta_map[x] = {row b, split, splits of row b, first partial slot of row b}
+// says (attention_ragged_map_kernel).  Decode only: ReLU score, no mask bits.
+template <typename T, int NVA, int NVC>
+__global__ void __launch_bounds__(AP_THREADS, LO_ATT_MINB) attention_fwd_ragged_kernel(
+    const T* __restrict__ att1, const T* __restrict__ enc, const float* __restrict__ att2, int64_t att2_stride,
+    const float* __restrict__ wf, float* __restrict__ alpha, int64_t alpha_stride, float* __restrict__ ctx,
+    float* __restrict__ gate_pre, int64_t gate_stride, float* __restrict__ gctx, bf16* __restrict__ gctx_bf,
+    const int4* __restrict__ cta_map, const int32_t* __restrict__ reg_off, int rpi, int* __restrict__ counters,
+    float* __restrict__ partials, int pol_enc, int pol_att1) {
+  // the map and the offsets were written by the decode call's prologue, long before the preceding launch: read before its wait
+  const int4 e = cta_map[blockIdx.x];
+  const int img = e.x / rpi;
+  const int g0 = reg_off[img];
+  attention_fwd_pipe_cta<T, NVA, NVC, false, 0, false>(att1, enc, att2, att2_stride, wf, alpha, alpha_stride, ctx, gate_pre, gate_stride,
+                                                      gctx, gctx_bf, reg_off[img + 1] - g0, e.z, counters, partials, pol_enc, pol_att1,
+                                                      nullptr, e.x, e.y, (int64_t)g0, (int64_t)e.w);
+}
+
+// Splits of one row of the ragged launch: its share of ns * B splits in proportion to its region count, at least 1 and at most
+// AP_MAXSPLIT; `fixed` (the att_nsplit option) gives every row ns.  Equal counts give every row exactly ns, the dense partition.
+__host__ __device__ __forceinline__ int att_ragged_row_splits(int ns, int B, int Ri, int64_t sumR, bool fixed) {
+  if (fixed) return ns;
+  const int64_t q = (int64_t)ns * B * Ri / sumR;
+  return q < 1 ? 1 : (q > AP_MAXSPLIT ? AP_MAXSPLIT : (int)q);
+}
+
+// One block: cta_map of the ragged launch (row-major: the splits of row 0, then row 1, ...) and zeroed ticket counters.
+__global__ void attention_ragged_map_kernel(const int32_t* __restrict__ reg_off, int B, int rpi, int ns, int64_t sumR, int fixed,
+                                            int4* __restrict__ cta_map, int* __restrict__ counters) {
+  extern __shared__ int s_rows[];          // [B] splits of each row, then [B] first slot of each row
+  for (int b = threadIdx.x; b < B; b += blockDim.x) {
+    s_rows[b] = att_ragged_row_splits(ns, B, reg_off[b / rpi + 1] - reg_off[b / rpi], sumR, fixed != 0);
+    counters[b] = 0;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    int p = 0;
+    for (int b = 0; b < B; b++) {
+      s_rows[B + b] = p;
+      p += s_rows[b];
+    }
+  }
+  __syncthreads();
+  for (int b = threadIdx.x; b < B; b += blockDim.x)
+    for (int s = 0; s < s_rows[b]; s++) cta_map[s_rows[B + b] + s] = make_int4(b, s, s_rows[b], s_rows[B + b]);
 }
 
 // DA1 (lo_attention_step_backward, a single Attention.forward call): while a stage is resident the consumer warps also store
@@ -1418,6 +1484,57 @@ static int fwd_dispatch(const AttFwdArgs& x, int C, cudaStream_t st) {
 }
 int attention_fwd_pipe(const AttFwdArgs& x, int dt, int C, cudaStream_t st) {
   return dt == LO_F32 ? fwd_dispatch<float>(x, C, st) : fwd_dispatch<bf16>(x, C, st);
+}
+
+// ---- ragged layout: per-image region counts (decode of images of different sizes)
+// rg.map: [B * AP_MAXSPLIT] int4 CTA map, then [B] ticket counters
+int64_t attention_ragged_map_bytes(int B) { return (int64_t)B * AP_MAXSPLIT * 16 + (int64_t)B * 4; }
+
+// The split counts follow the dense rule's total: att_pipe_splits(B) per row on average, so equal counts reproduce the dense
+// partition and the dense kernel's bits.  Host side: the grid size; device side (one launch per decode call): the map itself.
+int attention_ragged_prepare(AttRagged& rg, int B, int rpi, cudaStream_t st) {
+  LO_CHECK_ARG(B >= 1 && B <= 6144, "ragged attention: 1 <= rows <= 6144 (shared memory of the map kernel)");
+  const int n_img = B / rpi;
+  const int ns = att_pipe_splits(B);
+  const bool fixed = g_opt_att_nsplit > 0;
+  const int64_t sumR = (int64_t)rpi * rg.reg_off_host[n_img];
+  int ctas = 0;
+  for (int b = 0; b < B; b++)
+    ctas += att_ragged_row_splits(ns, B, rg.reg_off_host[b / rpi + 1] - rg.reg_off_host[b / rpi], sumR, fixed);
+  rg.ctas = ctas;
+  int4* map = (int4*)rg.map;
+  attention_ragged_map_kernel<<<1, 512, (size_t)B * 8, st>>>(rg.reg_off, B, rpi, ns, sumR, fixed ? 1 : 0, map,
+                                                             (int*)(map + (int64_t)B * AP_MAXSPLIT));
+  LO_LAUNCH_OK();
+  return LO_OK;
+}
+
+template <typename T, int NV>
+static int fwd_ragged_launch(const AttFwdArgs& x, const AttRagged& rg, cudaStream_t st) {
+  using C = ApCfg<T, NV, NV>;
+  static bool attr = false;
+  if (!attr) {
+    LO_CUDA(cudaFuncSetAttribute(attention_fwd_ragged_kernel<T, NV, NV>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM));
+    attr = true;
+  }
+  const int4* map = (const int4*)rg.map;
+  LO_CUDA(launch_att(attention_fwd_ragged_kernel<T, NV, NV>, dim3(rg.ctas), (size_t)C::SMEM, 1, st, true, (const T*)x.att1,
+                     (const T*)x.enc, x.att2, x.att2_stride, x.wf, x.alpha, x.alpha_stride, x.ctx, x.gate_pre, x.gate_stride, x.gctx,
+                     x.gctx_bf, map, rg.reg_off, x.rows_per_img > 1 ? x.rows_per_img : 1, (int*)(map + (int64_t)x.B * AP_MAXSPLIT),
+                     (float*)((char*)x.work + 4096), g_opt_att_policy_enc, g_opt_att_policy_att1));
+  LO_LAUNCH_OK();
+  return LO_OK;
+}
+
+template <typename T>
+static int fwd_ragged_dispatch(const AttFwdArgs& x, const AttRagged& rg, int C, cudaStream_t st) {
+  if (C == 256) return fwd_ragged_launch<T, 1>(x, rg, st);
+  if (C == 512) return fwd_ragged_launch<T, 2>(x, rg, st);
+  if (C == 1024) return fwd_ragged_launch<T, 4>(x, rg, st);
+  return fail(LO_EINVAL, "%s: attention width %ld not instantiated", __func__, (long)C);
+}
+int attention_fwd_ragged(const AttFwdArgs& x, const AttRagged& rg, int dt, int C, cudaStream_t st) {
+  return dt == LO_F32 ? fwd_ragged_dispatch<float>(x, rg, C, st) : fwd_ragged_dispatch<bf16>(x, rg, C, st);
 }
 
 template <typename T, int NVA, int NVC, int ACT>

@@ -287,6 +287,18 @@ struct AttBwdArgs {
 };
 int attention_fwd_pipe(const AttFwdArgs& x, int dt, int C, cudaStream_t st);
 int attention_bwd_pipe(const AttBwdArgs& x, int dt, int C, cudaStream_t st);
+// ragged layout (lo_decoder_args.reg_off): image i owns regions [reg_off[i], reg_off[i+1]) of the packed att1 / enc
+struct AttRagged {
+  const int32_t* reg_off;        // device [n_img + 1]
+  const int32_t* reg_off_host;   // host copy
+  void* map;                     // device, attention_ragged_map_bytes(B): CTA -> (row, split) map and ticket counters
+  int ctas;                      // grid size, set by attention_ragged_prepare
+};
+int64_t attention_ragged_map_bytes(int B);
+// once per decode call: the grid size (host) and the CTA map (device, stream-ordered)
+int attention_ragged_prepare(AttRagged& rg, int B, int rpi, cudaStream_t st);
+// x.B rows (x.R unused, x.alpha_stride >= the largest count), x.work as for attention_fwd_pipe; ReLU score, A == C, no mask bits
+int attention_fwd_ragged(const AttFwdArgs& x, const AttRagged& rg, int dt, int C, cudaStream_t st);
 
 // wgmma paths (lo_tc.cu)
 bool tc_available();

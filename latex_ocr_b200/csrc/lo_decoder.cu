@@ -418,6 +418,17 @@ __global__ void mean_rows_kernel(const T* __restrict__ enc, float* __restrict__ 
   for (int r = 0; r < R; r++) s += ldf(enc + ((int64_t)(b / rpi) * R + r) * C + c);
   mean[(int64_t)b * C + c] = s / (float)R;
 }
+// the same over the packed layout (lo_decoder_args.reg_off): row b averages its image's own regions, in mean_rows_kernel's order
+template <typename T>
+__global__ void mean_segments_kernel(const T* __restrict__ enc, float* __restrict__ mean, const int32_t* __restrict__ reg_off, int C,
+                                     int rpi) {
+  const int b = blockIdx.y, c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  const int g0 = reg_off[b / rpi], R = reg_off[b / rpi + 1] - g0;
+  float s = 0.f;
+  for (int r = 0; r < R; r++) s += ldf(enc + ((int64_t)g0 + r) * C + c);
+  mean[(int64_t)b * C + c] = s / (float)R;
+}
 
 // scheduled-sampling operands of lstm_pw_fwd_kernel<true> (row pointers at the first row of the launch, step t)
 struct SsStep {
@@ -1017,6 +1028,28 @@ static int check_args(const lo_decoder_args* a) {
   return LO_OK;
 }
 
+// per-image region counts (reg_off / reg_off_host): decode entry points only
+static int check_reg_off(const lo_decoder_args* a) {
+  if (!a->reg_off && !a->reg_off_host) return LO_OK;
+  LO_CHECK_ARG(a->reg_off && a->reg_off_host, "reg_off and reg_off_host must be set together");
+  LO_CHECK_ARG(g_opt_att_pipe, "per-image region counts (reg_off) need the pipelined attention kernels (att_pipe = 1)");
+  const int rpi = a->rows_per_img > 1 ? a->rows_per_img : 1;
+  LO_CHECK_ARG(a->reg_off_host[0] == 0, "reg_off_host[0] must be 0");
+  for (int i = 0; i < a->B / rpi; i++) {
+    const int n = a->reg_off_host[i + 1] - a->reg_off_host[i];
+    LO_CHECK_ARG(n >= 1 && n <= a->R, "region count of every image in 1..R (reg_off_host)");
+  }
+  return LO_OK;
+}
+static int refuse_reg_off(const lo_decoder_args* a) {
+  LO_CHECK_ARG(!a->reg_off && !a->reg_off_host, "reg_off / reg_off_host (per-image region counts) are for the decode entry points only");
+  return LO_OK;
+}
+// the ragged attention state of a decode call: map in the second attention region of `work` (the decode loop runs one row chain)
+static AttRagged ragged_of(const lo_decoder_args* a) {
+  return AttRagged{a->reg_off, a->reg_off_host, (char*)a->work + lo_attention_workspace_bytes(a->B, a->C), 0};
+}
+
 static int* work_counters(const lo_decoder_args* a) { return (int*)a->work; }
 // ReLU mask bits of step t, first row r0 (NULL when the scheme is off)
 static inline uint8_t* att_mask_at(const lo_decoder_args* a, int t, int64_t r0) {
@@ -1098,8 +1131,10 @@ __global__ void interleave_wih_kernel(const bf16* __restrict__ w_ih, bf16* __res
 static int forward_prologue(const lo_decoder_args* a, const Dims& d, cudaStream_t st) {
   const int dt = a->dt;
   const int rpi = a->rows_per_img > 1 ? a->rows_per_img : 1;
-  // att1 = enc @ W_e^T + b_e   (hoisted: the reference recomputes it every step, seq2seq_torch.py:186)
-  LO_TRY(gemm_nt(a->enc, dt, d.C, a->w_enc_att, dt, d.C, a->att1, dt, d.A, (d.B / rpi) * d.R, d.A, d.C, a->b_enc_att, 0, 0, a->impl, st));
+  // att1 = enc @ W_e^T + b_e   (hoisted: the reference recomputes it every step, seq2seq_torch.py:186); packed layout: every region
+  // of every image once
+  const int enc_rows = a->reg_off_host ? a->reg_off_host[d.B / rpi] : (d.B / rpi) * d.R;
+  LO_TRY(gemm_nt(a->enc, dt, d.C, a->w_enc_att, dt, d.C, a->att1, dt, d.A, enc_rows, d.A, d.C, a->b_enc_att, 0, 0, a->impl, st));
   const BfViews bv0 = bf_views(a, d);
   // embedding -> gate projection table (replaces embedding lookup + x[:, :E] @ W_ih[:, :E]^T, seq2seq_torch.py:291,:313)
   if (bv0.on && d.E % 64 == 0) {
@@ -1111,7 +1146,10 @@ static int forward_prologue(const lo_decoder_args* a, const Dims& d, cudaStream_
   // init_hidden_state (seq2seq_torch.py:255-265)
   {
     dim3 grid(cdiv(d.C, 256), d.B);
-    LO_DISPATCH_DT(dt, T, (mean_rows_kernel<T><<<grid, 256, 0, st>>>((const T*)a->enc, a->mean, d.R, d.C, rpi)));
+    if (a->reg_off)
+      LO_DISPATCH_DT(dt, T, (mean_segments_kernel<T><<<grid, 256, 0, st>>>((const T*)a->enc, a->mean, a->reg_off, d.C, rpi)));
+    else
+      LO_DISPATCH_DT(dt, T, (mean_rows_kernel<T><<<grid, 256, 0, st>>>((const T*)a->enc, a->mean, d.R, d.C, rpi)));
     LO_LAUNCH_OK();
   }
   const size_t es = dt == LO_F32 ? 4 : 2;
@@ -1150,6 +1188,7 @@ struct Rows {
   int row0, nrows;
   void* work;       // attention workspace of this chain
   int nsplit;       // attention split hint (0 = automatic)
+  const AttRagged* rg = nullptr;     // decode with per-image region counts: the whole batch, row0 = 0
 };
 
 // one decoder step t for the rows of `rs`; tok: token ids consumed at this step (row 0 of the batch)
@@ -1180,7 +1219,14 @@ static int forward_step(const lo_decoder_args* a, const Dims& d, int t, const Ro
   } else {
     LO_TRY(gemm_nt(h_prev, LO_F32, d.D, a->wcat1, dt, d.D, o1, LO_F32, d.O1, nrows, d.O1, d.D, a->bcat1, 0, 0, LO_IMPL_SIMT, st));
   }
-  if (!(g_opt_dbg_skip & 2))
+  if (rs.rg) {
+    if (!(g_opt_dbg_skip & 2)) {
+      AttFwdArgs x{a->att1, a->enc, o1, d.O1, a->w_full, a->alphas + t * d.R, (int64_t)d.T * d.R, a->ctx + (int64_t)t * d.B * d.C, o1 + d.A,
+                   d.O1, a->gctx + (int64_t)t * d.B * d.C, bv.on ? bv.gctx + (int64_t)t * d.B * d.C : nullptr, nrows, d.R, rs.work,
+                   a->rows_per_img, 0, 0, 0, nullptr, 0};
+      LO_TRY(attention_fwd_ragged(x, *rs.rg, dt, d.C, st));
+    }
+  } else if (!(g_opt_dbg_skip & 2))
   LO_TRY(attention_forward_launch(att1, enc, dt, o1, d.O1, a->w_full, a->alphas + (r0 * d.T + t) * d.R, (int64_t)d.T * d.R,
                                   a->ctx + ((int64_t)t * d.B + r0) * d.C, o1 + d.A, d.O1, a->gctx + ((int64_t)t * d.B + r0) * d.C,
                                   bv.on ? bv.gctx + ((int64_t)t * d.B + r0) * d.C : nullptr, nrows, d.R, d.C, rs.work, st,
@@ -1416,6 +1462,7 @@ int lo_attention_step_backward(const void* enc, const void* att1, int dt, const 
 
 int lo_decoder_forward(const lo_decoder_args* a, int with_loss, void* stream) {
   LO_TRY(check_args(a));
+  LO_TRY(refuse_reg_off(a));
   cudaStream_t st = (cudaStream_t)stream;
   const Dims d = dims(a);
   const bool ragged = a->bt_host[d.T - 1] < d.B;
@@ -1569,6 +1616,7 @@ int lo_decoder_pack_bwd_weights(const lo_decoder_args* a, void* stream) {
 
 int lo_decoder_backward(const lo_decoder_args* a, void* stream) {
   LO_TRY(check_args(a));
+  LO_TRY(refuse_reg_off(a));
   LO_CHECK_ARG(!a->dpred_ext || a->dlogits, "dpred_ext needs dlogits");
   LO_CHECK_ARG(!a->dpred_ext || a->dpred_stride >= a->V, "dpred_stride >= V");
   LO_CHECK_ARG(a->phase != 2 || !a->dalpha_ext, "phase 2 reads no d alpha: pass dalpha_ext to the phase-1 call");
@@ -1962,6 +2010,7 @@ int lo_decoder_backward(const lo_decoder_args* a, void* stream) {
 int lo_decoder_greedy_hist(const lo_decoder_args* a, int64_t start_id, int64_t end_id, int max_steps, int64_t* tokens,
                            int32_t* finished, int32_t* fin_hist, void* stream) {
   LO_TRY(check_args(a));
+  LO_TRY(check_reg_off(a));
   LO_CHECK_ARG(!a->ss_prob, "scheduled sampling (ss_prob) is a training mode: greedy decode feeds its own argmax already");
   LO_CHECK_ARG(tokens && finished && max_steps > 0 && max_steps <= a->T, "tokens/finished/max_steps (<= T capacity)");
   cudaStream_t st = (cudaStream_t)stream;
@@ -1971,9 +2020,11 @@ int lo_decoder_greedy_hist(const lo_decoder_args* a, int64_t start_id, int64_t e
   LO_LAUNCH_OK();
   LO_CUDA(cudaMemsetAsync(finished, 0, (size_t)d.B * 4, st));
   LO_TRY(forward_prologue(a, d, st));
+  AttRagged rg = ragged_of(a);
+  if (a->reg_off) LO_TRY(attention_ragged_prepare(rg, d.B, a->rows_per_img > 1 ? a->rows_per_img : 1, st));
   const BfViews bvg = bf_views(a, d);
   for (int t = 0; t < max_steps; t++) {
-    LO_TRY(forward_step(a, d, t, Rows{0, d.B, a->work, 0}, next_tok, 1, nullptr, 0, nullptr, st));
+    LO_TRY(forward_step(a, d, t, Rows{0, d.B, a->work, 0, a->reg_off ? &rg : nullptr}, next_tok, 1, nullptr, 0, nullptr, st));
     // logits_t = fc(h_t)   (no dropout at decode time)
     if (bvg.on)      // bf16 mirror of h_t: mma.sync kernel for <= 64 rows (the dispatcher falls back to CUDA cores otherwise)
       LO_TRY(gemm_nt(bvg.hall + (int64_t)(t + 1) * d.B * d.D, LO_BF16, d.D, a->w_fc, LO_BF16, d.D, a->logits, LO_F32, d.V, d.B, d.V, d.D,
@@ -2005,6 +2056,7 @@ int lo_decoder_beam_div(const lo_decoder_args* a, int64_t start_id, int64_t end_
                         int32_t* fin_hist, float* logp, float div_gamma, float div_prob, const float* div_u,
                         const uint64_t* div_state, void* stream) {
   LO_TRY(check_args(a));
+  LO_TRY(check_reg_off(a));
   LO_CHECK_ARG(!a->ss_prob, "scheduled sampling (ss_prob) is a training mode: not available in beam search");
   const bool div_on = !(div_gamma == 1.f || div_prob == 0.f);               // beam_search_decoder_cell.py:270-273
   LO_CHECK_ARG(!div_on || (div_gamma > 0.f && (div_u || div_state)), "diversity penalty needs gamma > 0 and div_u or div_state");
@@ -2025,6 +2077,8 @@ int lo_decoder_beam_div(const lo_decoder_args* a, int64_t start_id, int64_t end_
   LO_CUDA(cudaMemsetAsync(finished, 0, (size_t)d.B * 4, st));
   LO_CUDA(cudaMemsetAsync(logp, 0, (size_t)d.B * 4, st));          // initial log-probs are zeros (:106-107)
   LO_TRY(forward_prologue(a, d, st));
+  AttRagged rg = ragged_of(a);
+  if (a->reg_off) LO_TRY(attention_ragged_prepare(rg, d.B, beam, st));
   const BfViews bv = bf_views(a, d);
   const size_t smem = (size_t)beam * d.V * 4 * (div_on ? 2 : 1);
   static bool attr = false;
@@ -2033,7 +2087,7 @@ int lo_decoder_beam_div(const lo_decoder_args* a, int64_t start_id, int64_t end_
     attr = true;
   }
   for (int t = 0; t < max_steps; t++) {
-    LO_TRY(forward_step(a, d, t, Rows{0, d.B, a->work, 0}, next_tok, 1, nullptr, 0, nullptr, st));
+    LO_TRY(forward_step(a, d, t, Rows{0, d.B, a->work, 0, a->reg_off ? &rg : nullptr}, next_tok, 1, nullptr, 0, nullptr, st));
     float* h_new = a->hall + (int64_t)(t + 1) * d.B * d.D;
     float* c_new = a->call + (int64_t)(t + 1) * d.B * d.D;
     if (bv.on)       // bf16 mirror of h_t -> mma.sync kernel (row blocks of 64), CUDA cores otherwise

@@ -224,8 +224,9 @@ class DecoderWithAttention(nn.Module):
             p.requires_grad = fine_tune
 
     # ---------------------------------------------------------------------------------------------
-    def workspace(self, B, T, R, need_grad):
-        key = (B, T, R)
+    def workspace(self, B, T, R, need_grad, key=None, att1_rows=None):
+        """``att1_rows``: att1 as [att1_rows, A] (the packed layout of ragged_workspace) instead of [B, R, A]."""
+        key = (B, T, R) if key is None else key
         ws = self._ws.get(key)
         dev = self.store.device
         A, E, D, V, C = self.attention_dim, self.embed_dim, self.decoder_dim, self.vocab_size, self.encoder_dim
@@ -239,7 +240,7 @@ class DecoderWithAttention(nn.Module):
             ws = {"need_grad": False}
             t = ws["t"] = {}
             t["caps"] = z(B, T + 1, dtype=torch.int64)
-            t["att1"] = z(B, R, A, dtype=self.tdtype)
+            t["att1"] = z(B, R, A, dtype=self.tdtype) if att1_rows is None else z(att1_rows, A, dtype=self.tdtype)
             t["ptab"] = z(V, G)
             t["mean"] = z(B, C)
             t["hall"] = z(T + 1, B, D)
@@ -281,6 +282,27 @@ class DecoderWithAttention(nn.Module):
             # ReLU mask bits of every step (forward attention kernel -> backward attention kernel), 1 bit per att1 element
             t["att_mask"] = torch.empty(T, B, (R + 1) // 2 * 2, A // 8, dtype=torch.uint8, device=dev)      # rows padded to an even count
             ws["need_grad"] = True
+        return ws
+
+    def ragged_workspace(self, B, T, R, n_regions):
+        """Decode workspace for images of different sizes (lo_decoder_args.reg_off): the packed encoder output ``t["enc"]``
+        [regions, C], att1 [regions, A] and every per-row buffer, sized by capacity (rows B, steps T, largest region count R,
+        total regions).  One cache entry: a later call whose composition fits reuses it, a larger one replaces it by the element-wise
+        maximum of both capacities (serving traffic gives a new composition on nearly every call)."""
+        ws = self._ws.get("ragged")
+        if ws is not None:
+            cap = ws["cap"]
+            if B <= cap[0] and T <= cap[1] and R <= cap[2] and n_regions <= cap[3]:
+                return stamp(ws)
+            B, T, R, n_regions = max(B, cap[0]), max(T, cap[1]), max(R, cap[2]), max(n_regions, cap[3])
+            del self._ws["ragged"]
+        ws = self.workspace(B, T, R, False, key="ragged", att1_rows=n_regions)
+        ws["cap"] = (B, T, R, n_regions)
+        dev = self.store.device
+        ws["t"]["enc"] = torch.zeros(n_regions, self.encoder_dim, dtype=self.tdtype, device=dev)
+        ws["t"]["reg_off"] = torch.zeros(B + 1, dtype=torch.int32, device=dev)
+        ws["reg_off_host"] = (ctypes.c_int32 * (B + 1))()
+        self.fill_args(ws, ws["t"]["enc"], B, T, R, has_dropout=False)        # sizes bfwork (wgmma staging) by capacity
         return ws
 
     def _fed_buffer(self, ws):

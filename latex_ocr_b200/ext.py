@@ -297,6 +297,8 @@ class Img2SeqRowModel(Img2SeqModel):
     def predict_batch(self, *a, **k):
         raise NotImplementedError("the row-encoder / two-layer extension offers the training path only")
 
+    predict_images = predict_batch
+
     def set_sampling_prob(self, p):
         _refuse_sampling(float(p))
 

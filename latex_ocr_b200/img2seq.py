@@ -316,11 +316,21 @@ class Img2SeqModel:
         """img2seq.py:256-277.  images: tensor [N,1,H,W] (float or uint8) or a list of HxWx1 arrays (padded like
         ``pad_batch_images``).  Returns list[n_hyp][N]: each prediction truncated at END and, when the vocabulary has an
         ``id_to_tok`` table, joined into the formula string like the reference (token-id lists otherwise)."""
-        from . import decode
         if not torch.is_tensor(images):
             from .data import pad_batch_images
             images = torch.from_numpy(pad_batch_images(list(images))).permute(0, 3, 1, 2).contiguous()
-        hyps, end_id = self._decode_ids(images, start_id, decoding, beam_size)
+        return self._format(*self._decode_ids(images, start_id, decoding, beam_size))
+
+    def predict_images(self, images, start_id=None, decoding=None, beam_size=None):
+        """``predict_batch`` for a list of images of different sizes ([1,H,W] tensors or HxWx1 arrays), each decoded at its own
+        size in one time loop: no padding to the largest image, so an image's prediction does not depend on the other images of
+        the call (``predict_batch`` keeps the reference's padding).  Same return value as ``predict_batch``."""
+        return self._format(*self._decode_ids(list(images), start_id, decoding, beam_size))
+
+    def _format(self, hyps, end_id):
+        """list[n_hyp][N] of id lists -> each prediction truncated at END, joined into the formula string when the vocabulary has
+        an ``id_to_tok`` table."""
+        from . import decode
         rev = getattr(self._vocab, "id_to_tok", None)
         out = []
         for hyp in hyps:

@@ -49,15 +49,16 @@ int64_t lo_launch_count(void);
 /* Run-time options.  lo_set_option sets one by name and accepts any int value (an unknown name is refused with LO_EINVAL);
  * lo_get_option reads it back (-1: unknown name); lo_option_name(i) is the i-th name, NULL past the last.  From Python,
  * LO_OPTS=name=value,... in the environment sets them when the library is loaded.  [p]: parity-tested, tests/test_gpu_tc.py,
- * tests/test_gpu_parity.py or tests/test_gpu_attention_grid.py runs the other value against the default and requires the same
+ * tests/test_gpu_parity.py, tests/test_gpu_attention_grid.py or tests/test_gpu_l2_keep.py runs the other value against the default and requires the same
  * results (measured A/B: DESIGN.md §8).
  *
  *   name             default  meaning
  *   att_pipe         1 [p]    attention step kernels: 1 TMA bulk-copy -> shared-memory ring, 0 register-streaming
  *   pdl              1        programmatic dependent launch (above); 0 turns it off everywhere
  *   att_abi_pdl      0        1: the stand-alone attention entry points use it too (the caller vouches for their inputs, above)
- *   att_policy_enc   1        L2 policy of the attention kernels' enc stream: 0 normal, 1 evict_last, 2 evict_first, 3 no hint
- *   att_policy_att1  2        the same for their att1 stream
+ *   att_l2_keep_mb   24 [p]   MiB of the loop-invariant att1 / enc rows that each forward pipe / tensor-core backward attention launch
+ *                             keeps in L2 (evict_normal) from one time step to the next; every other row streams evict_first.  Clamped
+ *                             to the device's L2 size; 0 keeps nothing.  Same results for every value
  *   att_nsplit       0        splits of one batch row in the attention kernels; 0: automatic
  *   att_cluster      1 [p]    how the splits of a batch row meet.  Forward kernel and 512-wide tensor-core backward: 1 launches them
  *                             without a cluster (the last CTA of a row combines the partials in split order) when that grid is one
@@ -86,8 +87,8 @@ int lo_set_option(const char* name, int value);
 int lo_get_option(const char* name);
 const char* lo_option_name(int i);
 /* L2 persistence: access-policy window of `stream` over [base, base+bytes) (hits persist, misses stream) with the
- * persisting carve-out sized to fit; bytes = 0 resets.  The attention kernels honour it with att_policy_enc/att1 = 3
- * (bulk copies without an explicit cache hint). */
+ * persisting carve-out sized to fit; bytes = 0 resets.  It applies to loads without an explicit cache hint; the attention
+ * kernels' bulk copies carry one (att_l2_keep_mb). */
 int lo_set_l2_window(const void* base, int64_t bytes, float hit_ratio, void* stream);
 /* development aid: device buffer (>= 16 int64) that CTA (0,0,0) of the wgmma NT GEMM stamps with clock64 at its
  * pipeline milestones; NULL disables */

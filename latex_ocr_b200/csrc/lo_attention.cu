@@ -4,9 +4,9 @@
 // versions in lo_decoder.cu (attention_fwd_kernel / attention_bwd_kernel), which remain the fallback.
 //   forward : e_r = w . relu(att1_r + att2) ; online softmax ; ctx = sum_r alpha_r enc_r      (seq2seq_torch.py:186-190)
 //   backward: dalpha_r = <dctx, enc_r> + dreg_r ; de_r = alpha_r (dalpha_r - s) ; datt2 = w * sum_r de_r [att1_r + att2 > 0]
-// L2 policy: enc is read again by the next step (and by the backward) -> evict_last; att1 likewise is re-read every
-// step; which of the two to pin is a run-time option (lo_set_option) because together they are larger than the L2.  The
-// tensor-core backward streams enc evict_first (attention_bwd_mma_kernel launch).
+// L2 policy: att1 and enc do not change inside a time loop, so every step reads the same bytes in the same order, but a step
+// streams twice the L2.  The forward pipe kernels and the tensor-core backward keep a fixed share of their ring stages in L2
+// (att_keep_stage, att_keep_q: option att_l2_keep_mb) and stream the rest evict_first; the other backwards use fixed hints.
 #include <cooperative_groups.h>
 
 #include <mutex>
@@ -46,8 +46,14 @@ __device__ __forceinline__ void att_ts(int k) {
 #define ATT_TS(k, cond) do { } while (0)
 #endif
 
-__device__ __forceinline__ uint64_t make_policy(int kind) {
-  return kind == 1 ? l2_policy_evict_last() : (kind == 2 ? l2_policy_evict_first() : l2_policy_evict_normal());
+// L2 residency of ring stage i of a CTA.  The first `depth` stages are issued before griddepcontrol.wait, while the preceding
+// small launches leave HBM idle, so an L2 hit gains nothing there: they always stream.  Of the later stages j = i - depth, a share
+// keep_q / 1024 is kept, spread evenly (stage j is kept when floor((j + 1) q / 1024) > floor(j q / 1024)), so HBM stays busy
+// while the hits are served.  The same stages are kept at every step of a time loop: the rule depends on nothing else.
+// tests/test_l2_keep_rule.py mirrors it.
+__host__ __device__ __forceinline__ bool att_keep_stage(int i, int depth, int keep_q) {
+  const int j = i - depth;
+  return j >= 0 && (((j + 1) * keep_q) >> 10) != ((j * keep_q) >> 10);
 }
 
 // score non-linearity: ACT 0 = ReLU (torch flavour, seq2seq_torch.py:188), 1 = tanh (Genthial cell, attention_mechanism.py:82)
@@ -94,8 +100,8 @@ __device__ __forceinline__ void attention_fwd_pipe_cta(
     const T* __restrict__ att1, const T* __restrict__ enc, const float* __restrict__ att2, int64_t att2_stride,
     const float* __restrict__ wf, float* __restrict__ alpha, int64_t alpha_stride, float* __restrict__ ctx,
     float* __restrict__ gate_pre, int64_t gate_stride, float* __restrict__ gctx, bf16* __restrict__ gctx_bf, int R, int nsplit,
-    int* __restrict__ counters, float* __restrict__ partials, int pol_enc, int pol_att1, uint8_t* __restrict__ mask_out, int b, int sp,
-    int64_t g0, int64_t pbase) {
+    int* __restrict__ counters, float* __restrict__ partials, int keep_q, uint8_t* __restrict__ mask_out, int b, int sp, int64_t g0,
+    int64_t pbase) {
   using C = ApCfg<T, NVA, NVC>;
   constexpr int CHA = C::CHA, CHC = C::CHC;
   extern __shared__ __align__(128) uint8_t ap_smem[];
@@ -135,7 +141,7 @@ __device__ __forceinline__ void attention_fwd_pipe_cta(
   if (wid == AP_CWARPS) {
     // ===== producer warp: one lane issues the bulk copies =====
     if (lane == 0) {
-      const uint64_t pe = make_policy(pol_enc), pa = make_policy(pol_att1);
+      const uint64_t pk = l2_policy_evict_normal(), ps = l2_policy_evict_first();
       for (int i = 0; i < nst; i++) {
         const int s = i % AP_STAGES;
         const uint32_t ph = (i / AP_STAGES) & 1;
@@ -144,13 +150,12 @@ __device__ __forceinline__ void attention_fwd_pipe_cta(
         const int rows = min(C::ROWS, r1 - row);
         const uint32_t bytes_a = (uint32_t)rows * CHA * (uint32_t)sizeof(T), bytes_c = (uint32_t)rows * CHC * (uint32_t)sizeof(T);
         T* sa = ring + (size_t)s * C::STAGE_ELEMS;
+        const uint64_t pol = att_keep_stage(i, AP_STAGES, keep_q) ? pk : ps;      // att1 and enc rows of a stage stay together
         mbar_expect_tx(full_bar + s, bytes_a + bytes_c);
         ATT_TS(6, i == 0);
         ATT_TS(7, i == nst - 1);
-        if (pol_att1 == 3) bulk_g2s_nohint(sa, a1b + (int64_t)row * CHA, bytes_a, full_bar + s);
-        else bulk_g2s(sa, a1b + (int64_t)row * CHA, bytes_a, full_bar + s, pa);
-        if (pol_enc == 3) bulk_g2s_nohint(sa + C::HALF_A, eb + (int64_t)row * CHC, bytes_c, full_bar + s);
-        else bulk_g2s(sa + C::HALF_A, eb + (int64_t)row * CHC, bytes_c, full_bar + s, pe);
+        bulk_g2s(sa, a1b + (int64_t)row * CHA, bytes_a, full_bar + s, pol);
+        bulk_g2s(sa + C::HALF_A, eb + (int64_t)row * CHC, bytes_c, full_bar + s, pol);
       }
     }
     __syncwarp();
@@ -426,11 +431,11 @@ __global__ void __launch_bounds__(AP_THREADS, LO_ATT_MINB) attention_fwd_pipe_ke
     const T* __restrict__ att1, const T* __restrict__ enc, const float* __restrict__ att2, int64_t att2_stride,
     const float* __restrict__ wf, float* __restrict__ alpha, int64_t alpha_stride, float* __restrict__ ctx,
     float* __restrict__ gate_pre, int64_t gate_stride, float* __restrict__ gctx, bf16* __restrict__ gctx_bf, int R, int nsplit,
-    int* __restrict__ counters, float* __restrict__ partials, int pol_enc, int pol_att1, int rpi, uint8_t* __restrict__ mask_out) {
+    int* __restrict__ counters, float* __restrict__ partials, int keep_q, int rpi, uint8_t* __restrict__ mask_out) {
   const int b = blockIdx.y, sp = blockIdx.x;
   // beam search: rpi consecutive rows attend over one image
   attention_fwd_pipe_cta<T, NVA, NVC, CL, ACT, MK>(att1, enc, att2, att2_stride, wf, alpha, alpha_stride, ctx, gate_pre, gate_stride, gctx,
-                                                  gctx_bf, R, nsplit, counters, partials, pol_enc, pol_att1, mask_out, b, sp,
+                                                  gctx_bf, R, nsplit, counters, partials, keep_q, mask_out, b, sp,
                                                   (int64_t)(b / rpi) * R, (int64_t)b * nsplit);
 }
 
@@ -443,14 +448,14 @@ __global__ void __launch_bounds__(AP_THREADS, LO_ATT_MINB) attention_fwd_ragged_
     const float* __restrict__ wf, float* __restrict__ alpha, int64_t alpha_stride, float* __restrict__ ctx,
     float* __restrict__ gate_pre, int64_t gate_stride, float* __restrict__ gctx, bf16* __restrict__ gctx_bf,
     const int4* __restrict__ cta_map, const int32_t* __restrict__ reg_off, int rpi, int* __restrict__ counters,
-    float* __restrict__ partials, int pol_enc, int pol_att1) {
+    float* __restrict__ partials, int keep_q) {
   // the map and the offsets were written by the decode call's prologue, long before the preceding launch: read before its wait
   const int4 e = cta_map[blockIdx.x];
   const int img = e.x / rpi;
   const int g0 = reg_off[img];
   attention_fwd_pipe_cta<T, NVA, NVC, false, 0, false>(att1, enc, att2, att2_stride, wf, alpha, alpha_stride, ctx, gate_pre, gate_stride,
-                                                      gctx, gctx_bf, reg_off[img + 1] - g0, e.z, counters, partials, pol_enc, pol_att1,
-                                                      nullptr, e.x, e.y, (int64_t)g0, (int64_t)e.w);
+                                                      gctx, gctx_bf, reg_off[img + 1] - g0, e.z, counters, partials, keep_q, nullptr,
+                                                      e.x, e.y, (int64_t)g0, (int64_t)e.w);
 }
 
 // Splits of one row of the ragged launch: its share of ns * B splits in proportion to its region count, at least 1 and at most
@@ -493,8 +498,8 @@ __global__ void __launch_bounds__(AP_THREADS) attention_bwd_pipe_kernel(
     const float* __restrict__ ctx, const float* __restrict__ dgctx, int64_t dg_stride, const float* __restrict__ dreg,
     int64_t dreg_stride, const float* __restrict__ sreg, int64_t sreg_stride, float* __restrict__ de, float* __restrict__ datt2,
     float* __restrict__ dgp, int64_t dcat_stride, bf16* __restrict__ datt2_bf, bf16* __restrict__ dgp_bf,
-    float* __restrict__ dctx_out, int R, int nsplit, int* __restrict__ counters, float* __restrict__ partials, int pol_enc,
-    int pol_att1, float* __restrict__ dwf_part, T* __restrict__ datt1) {
+    float* __restrict__ dctx_out, int R, int nsplit, int* __restrict__ counters, float* __restrict__ partials,
+    float* __restrict__ dwf_part, T* __restrict__ datt1) {
   using C = ApCfg<T, NVA, NVC>;
   constexpr int CHA = C::CHA, CHC = C::CHC;
   extern __shared__ __align__(128) uint8_t ap_smem[];
@@ -531,7 +536,7 @@ __global__ void __launch_bounds__(AP_THREADS) attention_bwd_pipe_kernel(
 
   if (wid == AP_CWARPS) {
     if (lane == 0) {
-      const uint64_t pe = make_policy(pol_enc), pa = make_policy(pol_att1);
+      const uint64_t pe = l2_policy_evict_last(), pa = l2_policy_evict_first();
       for (int i = 0; i < nst; i++) {
         const int s = i % AP_STAGES;
         const uint32_t ph = (i / AP_STAGES) & 1;
@@ -541,10 +546,8 @@ __global__ void __launch_bounds__(AP_THREADS) attention_bwd_pipe_kernel(
         const uint32_t bytes_a = (uint32_t)rows * CHA * (uint32_t)sizeof(T), bytes_c = (uint32_t)rows * CHC * (uint32_t)sizeof(T);
         T* sa = ring + (size_t)s * C::STAGE_ELEMS;
         mbar_expect_tx(full_bar + s, bytes_a + bytes_c);
-        if (pol_att1 == 3) bulk_g2s_nohint(sa, a1b + (int64_t)row * CHA, bytes_a, full_bar + s);
-        else bulk_g2s(sa, a1b + (int64_t)row * CHA, bytes_a, full_bar + s, pa);
-        if (pol_enc == 3) bulk_g2s_nohint(sa + C::HALF_A, eb + (int64_t)row * CHC, bytes_c, full_bar + s);
-        else bulk_g2s(sa + C::HALF_A, eb + (int64_t)row * CHC, bytes_c, full_bar + s, pe);
+        bulk_g2s(sa, a1b + (int64_t)row * CHA, bytes_a, full_bar + s, pa);
+        bulk_g2s(sa + C::HALF_A, eb + (int64_t)row * CHC, bytes_c, full_bar + s, pe);
       }
     }
     __syncwarp();
@@ -781,8 +784,7 @@ __global__ void __launch_bounds__(AP_THREADS, LO_ATT_MINB) attention_bwd_mask_ke
     const float* __restrict__ dgctx, int64_t dg_stride, const float* __restrict__ dreg, int64_t dreg_stride,
     const float* __restrict__ sreg, int64_t sreg_stride, float* __restrict__ de, float* __restrict__ datt2, float* __restrict__ dgp,
     int64_t dcat_stride, bf16* __restrict__ datt2_bf, bf16* __restrict__ dgp_bf, float* __restrict__ dctx_out, int R, int nsplit,
-    int* __restrict__ counters, float* __restrict__ partials, int pol_enc, const float* __restrict__ att2,
-    float* __restrict__ dwf_part) {
+    int* __restrict__ counters, float* __restrict__ partials, const float* __restrict__ att2, float* __restrict__ dwf_part) {
   using C = ApmCfg<T, NVA, NVC>;
   constexpr int CHA = C::CHA, CHC = C::CHC, MB = CHA / 8;
   extern __shared__ __align__(128) uint8_t ap_smem[];
@@ -812,7 +814,7 @@ __global__ void __launch_bounds__(AP_THREADS, LO_ATT_MINB) attention_bwd_mask_ke
     // producer: enc is loop-invariant (prefetchable before griddepcontrol.wait); the mask bits of this step were written by the
     // forward pass long ago as well
     if (lane == 0) {
-      const uint64_t pe = make_policy(pol_enc), pm = l2_policy_evict_first();
+      const uint64_t pe = l2_policy_evict_last(), pm = l2_policy_evict_first();
       for (int i = 0; i < nst; i++) {
         const int s = i % APM_STAGES;
         const uint32_t ph = (i / APM_STAGES) & 1;
@@ -1055,7 +1057,7 @@ __global__ void __launch_bounds__(AP_THREADS, LO_ABM_MINB) attention_bwd_mma_ker
     const float* __restrict__ dgctx, int64_t dg_stride, const float* __restrict__ dreg, int64_t dreg_stride,
     const float* __restrict__ sreg, int64_t sreg_stride, float* __restrict__ de, float* __restrict__ datt2, float* __restrict__ dgp,
     int64_t dcat_stride, bf16* __restrict__ datt2_bf, bf16* __restrict__ dgp_bf, float* __restrict__ dctx_out, int R, int nsplit,
-    int* __restrict__ counters, float* __restrict__ partials, int pol_enc, const float* __restrict__ att2,
+    int* __restrict__ counters, float* __restrict__ partials, int keep_q, const float* __restrict__ att2,
     float* __restrict__ dwf_part) {
   constexpr int CH = ABM_CH, MB = CH / 8;
   extern __shared__ __align__(128) uint8_t ap_smem[];
@@ -1098,7 +1100,8 @@ __global__ void __launch_bounds__(AP_THREADS, LO_ABM_MINB) attention_bwd_mma_ker
 
   if (wid == AP_CWARPS) {
     // producer warp: enc and the mask bits of this step were written long before the preceding launch -> no griddepcontrol.wait
-    const uint64_t pe = make_policy(pol_enc), pm = l2_policy_evict_first();
+    // the whole budget goes to enc rows; the mask bits of a step are read once per time loop
+    const uint64_t pk = l2_policy_evict_normal(), pm = l2_policy_evict_first();
     for (int i = 0; i < nst; i++) {
       const int s = i % ABM_STAGES;
       const uint32_t ph = (i / ABM_STAGES) & 1;
@@ -1113,6 +1116,7 @@ __global__ void __launch_bounds__(AP_THREADS, LO_ABM_MINB) attention_bwd_mma_ker
         ATT_TS(7, i == nst - 1);
       }
       __syncwarp();
+      const uint64_t pe = att_keep_stage(i, ABM_STAGES, keep_q) ? pk : pm;
       if (lane < rows) bulk_g2s(st + lane * ABM_PITCH, eb + (int64_t)(row + lane) * CH, CH * 2u, full_bar + s, pe);
       else if (lane == ABM_ROWS) bulk_g2s(st + ABM_ENC_BYTES, mb + (int64_t)(row >> 1) * 2 * MB, bytes_m, full_bar + s, pm);
     }
@@ -1353,6 +1357,25 @@ int att_pipe_splits(int B, int hint = 0) {
   return s;
 }
 
+// Keep share (1/1024 units, att_keep_stage) of a launch whose CTAs stream `bytes` distinct bytes of att1 / enc rows: the
+// att_l2_keep_mb budget, clamped to the device's L2 size, over those bytes.  A CTA keeps at most that share of its stages after the
+// first `depth`, and all but its last stage are full, so the kept bytes of the launch never exceed the budget.
+static int att_keep_q(int64_t bytes) {
+  static const int64_t l2_bytes = [] {
+    int dev = 0, v = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&v, cudaDevAttrL2CacheSize, dev) != cudaSuccess) {
+      cudaGetLastError();
+      return (int64_t)0;         // unknown: keep nothing
+    }
+    return (int64_t)v;
+  }();
+  int64_t budget = (int64_t)g_opt_att_l2_keep_mb << 20;
+  if (budget > l2_bytes) budget = l2_bytes;
+  if (budget <= 0 || bytes <= 0) return 0;
+  const int64_t q = budget * 1024 / bytes;
+  return q > 1024 ? 1024 : (int)q;
+}
+
 // optional L2 access-policy window attached to every attention launch (lo_set_l2_window): as a LAUNCH attribute it is also
 // recorded in CUDA-graph kernel nodes, which a stream attribute is not
 static cudaAccessPolicyWindow g_att_window{};
@@ -1444,16 +1467,16 @@ static int fwd_launch_m(const AttFwdArgs& x, cudaStream_t st) {
   }
   const int ns = att_pipe_splits(x.B, x.nsplit_hint);
   const int rpi = x.rows_per_img > 1 ? x.rows_per_img : 1;
+  const int keep_q = att_keep_q((int64_t)(x.B / rpi) * x.R * (C::CHA + C::CHC) * (int64_t)sizeof(T));     // rows of one image: read once
   if (att_grid_cluster((const void*)attention_fwd_pipe_kernel<T, NVA, NVC, false, ACT, MK>, (size_t)C::SMEM, ns, x.B, x.R)) {
     const size_t smem = C::SMEM + (size_t)((x.R + ns - 1) / ns) * 4;
     LO_CUDA(launch_att(attention_fwd_pipe_kernel<T, NVA, NVC, true, ACT, MK>, dim3(ns, x.B), smem, ns, st, att_pdl_ok(x.abi), (const T*)x.att1, (const T*)x.enc,
                        x.att2, x.att2_stride, x.wf, x.alpha, x.alpha_stride, x.ctx, x.gate_pre, x.gate_stride, x.gctx, x.gctx_bf, x.R, ns,
-                       (int*)x.work, (float*)((char*)x.work + 4096), g_opt_att_policy_enc, g_opt_att_policy_att1, rpi, x.mask_out));
+                       (int*)x.work, (float*)((char*)x.work + 4096), keep_q, rpi, x.mask_out));
   } else {
     LO_CUDA(launch_att(attention_fwd_pipe_kernel<T, NVA, NVC, false, ACT, MK>, dim3(ns, x.B), (size_t)C::SMEM, 1, st, att_pdl_ok(x.abi), (const T*)x.att1,
                        (const T*)x.enc, x.att2, x.att2_stride, x.wf, x.alpha, x.alpha_stride, x.ctx, x.gate_pre, x.gate_stride, x.gctx,
-                       x.gctx_bf, x.R, ns, (int*)x.work, (float*)((char*)x.work + 4096), g_opt_att_policy_enc, g_opt_att_policy_att1, rpi,
-                       x.mask_out));
+                       x.gctx_bf, x.R, ns, (int*)x.work, (float*)((char*)x.work + 4096), keep_q, rpi, x.mask_out));
   }
   LO_LAUNCH_OK();
   return LO_OK;
@@ -1518,10 +1541,11 @@ static int fwd_ragged_launch(const AttFwdArgs& x, const AttRagged& rg, cudaStrea
     attr = true;
   }
   const int4* map = (const int4*)rg.map;
+  const int rpi = x.rows_per_img > 1 ? x.rows_per_img : 1;
+  const int keep_q = att_keep_q((int64_t)rg.reg_off_host[x.B / rpi] * (C::CHA + C::CHC) * (int64_t)sizeof(T));    // all regions, once
   LO_CUDA(launch_att(attention_fwd_ragged_kernel<T, NV, NV>, dim3(rg.ctas), (size_t)C::SMEM, 1, st, true, (const T*)x.att1,
                      (const T*)x.enc, x.att2, x.att2_stride, x.wf, x.alpha, x.alpha_stride, x.ctx, x.gate_pre, x.gate_stride, x.gctx,
-                     x.gctx_bf, map, rg.reg_off, x.rows_per_img > 1 ? x.rows_per_img : 1, (int*)(map + (int64_t)x.B * AP_MAXSPLIT),
-                     (float*)((char*)x.work + 4096), g_opt_att_policy_enc, g_opt_att_policy_att1));
+                     x.gctx_bf, map, rg.reg_off, rpi, (int*)(map + (int64_t)x.B * AP_MAXSPLIT), (float*)((char*)x.work + 4096), keep_q));
   LO_LAUNCH_OK();
   return LO_OK;
 }
@@ -1561,7 +1585,7 @@ static int bwd_launch_a(const AttBwdArgs& x, cudaStream_t st) {
 #define LO_BWDD_ARGS                                                                                                             \
   (const T*)x.att1, (const T*)x.enc, x.att2, x.gate, x.o1_stride, x.wf, x.alpha, x.alpha_stride, x.ctx, x.dgctx, x.dg_stride, x.dreg, \
       x.dreg_stride, x.sreg, x.sreg_stride, x.de, x.datt2, x.dgp, x.dcat_stride, x.datt2_bf, x.dgp_bf, x.dctx_out, x.R, nsd,      \
-      (int*)x.work, (float*)((char*)x.work + 4096), g_opt_att_policy_enc, g_opt_att_policy_att1, x.dwf_part, (T*)x.datt1
+      (int*)x.work, (float*)((char*)x.work + 4096), x.dwf_part, (T*)x.datt1
       if (use_cluster(nsd, x.R)) {
         LO_CUDA(launch_att(attention_bwd_pipe_kernel<T, NVA, NVC, true, ACT, true>, dim3(nsd, x.B), (size_t)C::SMEM, nsd, st, att_pdl_ok(x.abi),
                            LO_BWDD_ARGS));
@@ -1586,9 +1610,10 @@ static int bwd_launch_a(const AttBwdArgs& x, cudaStream_t st) {
 #define LO_BWDT_ARGS                                                                                                                  \
   x.mask_in, (const bf16*)x.enc, x.gate, x.o1_stride, x.wf, x.alpha, x.alpha_stride, x.ctx, x.dgctx, x.dg_stride, x.dreg,            \
       x.dreg_stride, x.sreg, x.sreg_stride, x.de, x.datt2, x.dgp, x.dcat_stride, x.datt2_bf, x.dgp_bf, x.dctx_out, x.R, ns,           \
-      (int*)x.work, (float*)((char*)x.work + 4096), 2, x.att2, x.dwf_part
-    // enc evict_first (policy 2) whatever att_policy_enc says: the 57 MB of enc do not fit the H100's 50 MB L2 and are read once per
-    // launch; measured faster than evict_last in the backward loop (47.0 vs 48.1 us per step; in the forward loop it was slower)
+      (int*)x.work, (float*)((char*)x.work + 4096), keep_q, x.att2, x.dwf_part
+    // a share of the enc rows kept in L2, the rest evict_first: all 57 MB of enc at cfg #2 do not fit the H100's 50 MB L2, and
+    // evict_last on every row was slower than evict_first on every row (47.0 vs 48.1 us per step of the backward loop)
+    const int keep_q = att_keep_q((int64_t)x.B * x.R * ABM_CH * 2);
     const size_t smem_t = (size_t)ABM_SMEM + (size_t)att_rows_per_split(x.R, ns) * 8;      // + alpha / d reg of the CTA's rows
     if (att_grid_cluster((const void*)attention_bwd_mma_kernel<false>, smem_t, ns, x.B, x.R)) {
       LO_CUDA(launch_att(attention_bwd_mma_kernel<true>, dim3(ns, x.B), smem_t, ns, st, att_pdl_ok(x.abi), LO_BWDT_ARGS));
@@ -1610,7 +1635,7 @@ static int bwd_launch_a(const AttBwdArgs& x, cudaStream_t st) {
 #define LO_BWDM_ARGS                                                                                                                  \
   x.mask_in, (const T*)x.enc, x.gate, x.o1_stride, x.wf, x.alpha, x.alpha_stride, x.ctx, x.dgctx, x.dg_stride, x.dreg, x.dreg_stride, \
       x.sreg, x.sreg_stride, x.de, x.datt2, x.dgp, x.dcat_stride, x.datt2_bf, x.dgp_bf, x.dctx_out, x.R, ns, (int*)x.work,           \
-      (float*)((char*)x.work + 4096), g_opt_att_policy_enc, x.att2, x.dwf_part
+      (float*)((char*)x.work + 4096), x.att2, x.dwf_part
     if (use_cluster(ns, x.R)) {
       LO_CUDA(launch_att(attention_bwd_mask_kernel<T, NVA, NVC, true>, dim3(ns, x.B), (size_t)CM::SMEM, ns, st, att_pdl_ok(x.abi), LO_BWDM_ARGS));
     } else {
@@ -1623,7 +1648,7 @@ static int bwd_launch_a(const AttBwdArgs& x, cudaStream_t st) {
 #define LO_BWD_ARGS                                                                                                              \
   (const T*)x.att1, (const T*)x.enc, x.att2, x.gate, x.o1_stride, x.wf, x.alpha, x.alpha_stride, x.ctx, x.dgctx, x.dg_stride, x.dreg, \
       x.dreg_stride, x.sreg, x.sreg_stride, x.de, x.datt2, x.dgp, x.dcat_stride, x.datt2_bf, x.dgp_bf, x.dctx_out, x.R, ns,       \
-      (int*)x.work, (float*)((char*)x.work + 4096), g_opt_att_policy_enc, g_opt_att_policy_att1, x.dwf_part, (T*)nullptr
+      (int*)x.work, (float*)((char*)x.work + 4096), x.dwf_part, (T*)nullptr
   if (use_cluster(ns, x.R)) {
     LO_CUDA(launch_att(attention_bwd_pipe_kernel<T, NVA, NVC, true, ACT>, dim3(ns, x.B), (size_t)C::SMEM, ns, st, att_pdl_ok(x.abi), LO_BWD_ARGS));
   } else {

@@ -60,8 +60,7 @@ constexpr int LO_NUM_SMS = 132;
   X(g_opt_att_pipe, "att_pipe", 1)                /* TMA-pipelined attention kernels; 0: register-streaming */ \
   X(g_opt_pdl, "pdl", 1)                          /* programmatic dependent launch */                         \
   X(g_opt_att_abi_pdl, "att_abi_pdl", 0)          /* ... also for the stand-alone attention entry points */   \
-  X(g_opt_att_policy_enc, "att_policy_enc", 1)    /* L2 policy of the enc stream */                            \
-  X(g_opt_att_policy_att1, "att_policy_att1", 2)  /* L2 policy of the att1 stream */                           \
+  X(g_opt_att_l2_keep_mb, "att_l2_keep_mb", 24)   /* MiB of att1 / enc rows kept in L2 per attention launch */ \
   X(g_opt_att_nsplit, "att_nsplit", 0)            /* attention splits per batch row; 0: automatic */           \
   X(g_opt_att_cluster, "att_cluster", 1)          /* splits of a batch row combine through DSMEM */            \
   X(g_opt_att_maskbits, "att_maskbits", 1)        /* ReLU mask bits instead of att1 in the backward */         \

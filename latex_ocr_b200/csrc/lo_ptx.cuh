@@ -44,12 +44,6 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
       "l"(reinterpret_cast<uint64_t>(src)), "r"(bytes), "r"(smem_u32(bar)), "l"(policy)
       : "memory");
 }
-// without an explicit cache hint: the stream's access-policy window (lo_set_l2_window) decides
-__device__ __forceinline__ void bulk_g2s_nohint(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)),
-               "l"(reinterpret_cast<uint64_t>(src)), "r"(bytes), "r"(smem_u32(bar))
-               : "memory");
-}
 __device__ __forceinline__ uint64_t l2_policy_evict_last() {
   uint64_t p;
   asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));

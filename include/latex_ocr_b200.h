@@ -193,6 +193,9 @@ int lo_relu_mask_cast(const float* g, const void* y, void* out, int dt, int64_t 
  * cancels in the softmax) ; alpha out fp32 [B][alpha_stride>=R] ; ctx out fp32 [B][C].
  * gate_pre (optional) [B][gate_stride]: if given, gate = sigmoid(gate_pre) is written back in place and
  * gctx [B][C] = gate*ctx (seq2seq_torch.py:311-312).  work: lo_attention_workspace_bytes(B, C) bytes.
+ * Layout of one attention workspace of B rows: B int32 ticket counters at offset 0 (zero when given; every launch leaves them
+ * zero), then the split partials [B][16][C + 2] fp32 at offset P = 4096 for B <= 1024, P = 4 * B rounded up to 256 above
+ * (decoding has no row cap).  Size: P + B * 16 * (C + 2) * 4 bytes.
  */
 int64_t lo_attention_workspace_bytes(int B, int C);
 int64_t lo_decoder_workspace_bytes(int B, int C);   /* `work` of lo_decoder_args: two attention regions (two row chains) */

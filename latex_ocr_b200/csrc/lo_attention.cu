@@ -1472,11 +1472,11 @@ static int fwd_launch_m(const AttFwdArgs& x, cudaStream_t st) {
     const size_t smem = C::SMEM + (size_t)((x.R + ns - 1) / ns) * 4;
     LO_CUDA(launch_att(attention_fwd_pipe_kernel<T, NVA, NVC, true, ACT, MK>, dim3(ns, x.B), smem, ns, st, att_pdl_ok(x.abi), (const T*)x.att1, (const T*)x.enc,
                        x.att2, x.att2_stride, x.wf, x.alpha, x.alpha_stride, x.ctx, x.gate_pre, x.gate_stride, x.gctx, x.gctx_bf, x.R, ns,
-                       (int*)x.work, (float*)((char*)x.work + 4096), keep_q, rpi, x.mask_out));
+                       (int*)x.work, (float*)((char*)x.work + att_partials_offset(x.B)), keep_q, rpi, x.mask_out));
   } else {
     LO_CUDA(launch_att(attention_fwd_pipe_kernel<T, NVA, NVC, false, ACT, MK>, dim3(ns, x.B), (size_t)C::SMEM, 1, st, att_pdl_ok(x.abi), (const T*)x.att1,
                        (const T*)x.enc, x.att2, x.att2_stride, x.wf, x.alpha, x.alpha_stride, x.ctx, x.gate_pre, x.gate_stride, x.gctx,
-                       x.gctx_bf, x.R, ns, (int*)x.work, (float*)((char*)x.work + 4096), keep_q, rpi, x.mask_out));
+                       x.gctx_bf, x.R, ns, (int*)x.work, (float*)((char*)x.work + att_partials_offset(x.B)), keep_q, rpi, x.mask_out));
   }
   LO_LAUNCH_OK();
   return LO_OK;
@@ -1545,7 +1545,7 @@ static int fwd_ragged_launch(const AttFwdArgs& x, const AttRagged& rg, cudaStrea
   const int keep_q = att_keep_q((int64_t)rg.reg_off_host[x.B / rpi] * (C::CHA + C::CHC) * (int64_t)sizeof(T));    // all regions, once
   LO_CUDA(launch_att(attention_fwd_ragged_kernel<T, NV, NV>, dim3(rg.ctas), (size_t)C::SMEM, 1, st, true, (const T*)x.att1,
                      (const T*)x.enc, x.att2, x.att2_stride, x.wf, x.alpha, x.alpha_stride, x.ctx, x.gate_pre, x.gate_stride, x.gctx,
-                     x.gctx_bf, map, rg.reg_off, rpi, (int*)(map + (int64_t)x.B * AP_MAXSPLIT), (float*)((char*)x.work + 4096), keep_q));
+                     x.gctx_bf, map, rg.reg_off, rpi, (int*)(map + (int64_t)x.B * AP_MAXSPLIT), (float*)((char*)x.work + att_partials_offset(x.B)), keep_q));
   LO_LAUNCH_OK();
   return LO_OK;
 }
@@ -1585,7 +1585,7 @@ static int bwd_launch_a(const AttBwdArgs& x, cudaStream_t st) {
 #define LO_BWDD_ARGS                                                                                                             \
   (const T*)x.att1, (const T*)x.enc, x.att2, x.gate, x.o1_stride, x.wf, x.alpha, x.alpha_stride, x.ctx, x.dgctx, x.dg_stride, x.dreg, \
       x.dreg_stride, x.sreg, x.sreg_stride, x.de, x.datt2, x.dgp, x.dcat_stride, x.datt2_bf, x.dgp_bf, x.dctx_out, x.R, nsd,      \
-      (int*)x.work, (float*)((char*)x.work + 4096), x.dwf_part, (T*)x.datt1
+      (int*)x.work, (float*)((char*)x.work + att_partials_offset(x.B)), x.dwf_part, (T*)x.datt1
       if (use_cluster(nsd, x.R)) {
         LO_CUDA(launch_att(attention_bwd_pipe_kernel<T, NVA, NVC, true, ACT, true>, dim3(nsd, x.B), (size_t)C::SMEM, nsd, st, att_pdl_ok(x.abi),
                            LO_BWDD_ARGS));
@@ -1610,7 +1610,7 @@ static int bwd_launch_a(const AttBwdArgs& x, cudaStream_t st) {
 #define LO_BWDT_ARGS                                                                                                                  \
   x.mask_in, (const bf16*)x.enc, x.gate, x.o1_stride, x.wf, x.alpha, x.alpha_stride, x.ctx, x.dgctx, x.dg_stride, x.dreg,            \
       x.dreg_stride, x.sreg, x.sreg_stride, x.de, x.datt2, x.dgp, x.dcat_stride, x.datt2_bf, x.dgp_bf, x.dctx_out, x.R, ns,           \
-      (int*)x.work, (float*)((char*)x.work + 4096), keep_q, x.att2, x.dwf_part
+      (int*)x.work, (float*)((char*)x.work + att_partials_offset(x.B)), keep_q, x.att2, x.dwf_part
     // a share of the enc rows kept in L2, the rest evict_first: all 57 MB of enc at cfg #2 do not fit the H100's 50 MB L2, and
     // evict_last on every row was slower than evict_first on every row (47.0 vs 48.1 us per step of the backward loop)
     const int keep_q = att_keep_q((int64_t)x.B * x.R * ABM_CH * 2);
@@ -1635,7 +1635,7 @@ static int bwd_launch_a(const AttBwdArgs& x, cudaStream_t st) {
 #define LO_BWDM_ARGS                                                                                                                  \
   x.mask_in, (const T*)x.enc, x.gate, x.o1_stride, x.wf, x.alpha, x.alpha_stride, x.ctx, x.dgctx, x.dg_stride, x.dreg, x.dreg_stride, \
       x.sreg, x.sreg_stride, x.de, x.datt2, x.dgp, x.dcat_stride, x.datt2_bf, x.dgp_bf, x.dctx_out, x.R, ns, (int*)x.work,           \
-      (float*)((char*)x.work + 4096), x.att2, x.dwf_part
+      (float*)((char*)x.work + att_partials_offset(x.B)), x.att2, x.dwf_part
     if (use_cluster(ns, x.R)) {
       LO_CUDA(launch_att(attention_bwd_mask_kernel<T, NVA, NVC, true>, dim3(ns, x.B), (size_t)CM::SMEM, ns, st, att_pdl_ok(x.abi), LO_BWDM_ARGS));
     } else {
@@ -1648,7 +1648,7 @@ static int bwd_launch_a(const AttBwdArgs& x, cudaStream_t st) {
 #define LO_BWD_ARGS                                                                                                              \
   (const T*)x.att1, (const T*)x.enc, x.att2, x.gate, x.o1_stride, x.wf, x.alpha, x.alpha_stride, x.ctx, x.dgctx, x.dg_stride, x.dreg, \
       x.dreg_stride, x.sreg, x.sreg_stride, x.de, x.datt2, x.dgp, x.dcat_stride, x.datt2_bf, x.dgp_bf, x.dctx_out, x.R, ns,       \
-      (int*)x.work, (float*)((char*)x.work + 4096), x.dwf_part, (T*)nullptr
+      (int*)x.work, (float*)((char*)x.work + att_partials_offset(x.B)), x.dwf_part, (T*)nullptr
   if (use_cluster(ns, x.R)) {
     LO_CUDA(launch_att(attention_bwd_pipe_kernel<T, NVA, NVC, true, ACT>, dim3(ns, x.B), (size_t)C::SMEM, ns, st, att_pdl_ok(x.abi), LO_BWD_ARGS));
   } else {

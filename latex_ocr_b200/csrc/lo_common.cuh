@@ -286,6 +286,14 @@ struct AttBwdArgs {
 };
 int attention_fwd_pipe(const AttFwdArgs& x, int dt, int C, cudaStream_t st);
 int attention_bwd_pipe(const AttBwdArgs& x, int dt, int C, cudaStream_t st);
+// Byte offset of the split partials in the attention workspace of a launch of B rows; the B per-row ticket counters (int) sit in
+// front of them at offset 0.  Up to 1,024 rows it is 4096, the layout the training, stand-alone and TF-decoder entry points use
+// (their dlen scratch at +2048 lies between the counters of <= 512 rows and the partials); decoding has no row cap, and above 1,024
+// rows the counters would run into the partials, so the offset grows with B.  The counters keep their values from one launch to
+// the next (each row's last CTA resets its own), so every launch that shares them must see the same offset: dense decode
+// workspaces are keyed by their exact row count and every row is active at every step, training's shrinking row counts stay
+// <= 512, and the ragged decode keeps its counters next to its CTA map.
+inline int64_t att_partials_offset(int B) { return B <= 1024 ? 4096 : ((int64_t)B * 4 + 255) / 256 * 256; }
 // ragged layout (lo_decoder_args.reg_off): image i owns regions [reg_off[i], reg_off[i+1]) of the packed att1 / enc
 struct AttRagged {
   const int32_t* reg_off;        // device [n_img + 1]

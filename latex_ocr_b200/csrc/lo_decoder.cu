@@ -1056,7 +1056,7 @@ static inline uint8_t* att_mask_at(const lo_decoder_args* a, int t, int64_t r0) 
   if (!a->att_mask || !g_opt_att_maskbits || !g_opt_att_pipe || a->rows_per_img > 1) return nullptr;
   return a->att_mask + ((int64_t)t * a->B + r0) * ((a->R + 1) & ~1) * (a->A / 8);      // rows padded to an even count (pair layout)
 }
-static float* work_partials(const lo_decoder_args* a) { return (float*)((char*)a->work + 4096); }
+static float* work_partials(const lo_decoder_args* a) { return (float*)((char*)a->work + att_partials_offset(a->B)); }
 static int32_t* work_dlen(const lo_decoder_args* a) { return (int32_t*)((char*)a->work + 2048); }
 
 static int attention_forward_launch(const void* att1, const void* enc, int dt, const float* att2, int64_t att2_stride,
@@ -1071,7 +1071,7 @@ static int attention_forward_launch(const void* att1, const void* enc, int dt, c
   }
   const int ns = att_splits(B);
   int* cnt = (int*)work;
-  float* part = (float*)((char*)work + 4096);
+  float* part = (float*)((char*)work + att_partials_offset(B));
   dim3 grid(ns, B);
 #define LO_ATT_FWD(T, NV)                                                                                           \
   attention_fwd_kernel<T, NV><<<grid, LO_ATT_THREADS, 0, st>>>((const T*)att1, (const T*)enc, att2, att2_stride, wf, \
@@ -1334,7 +1334,7 @@ int64_t lo_decoder_bfwork_bytes(const lo_decoder_args* a) {
 int64_t lo_sizeof_decoder_args(void) { return (int64_t)sizeof(lo_decoder_args); }
 
 int64_t lo_attention_workspace_bytes(int B, int C) {
-  return 4096 + (int64_t)B * LO_ATT_MAXSPLIT * (C + 2) * 4;
+  return att_partials_offset(B) + (int64_t)B * LO_ATT_MAXSPLIT * (C + 2) * 4;
 }
 /* the decoder entry points use two such regions (one per row chain) */
 int64_t lo_decoder_workspace_bytes(int B, int C) { return 2 * lo_attention_workspace_bytes(B, C); }
@@ -1821,7 +1821,7 @@ int lo_decoder_backward(const lo_decoder_args* a, void* stream) {
       LO_TRY(attention_bwd_pipe(x, dt, d.C, st));
     } else {
     int* cnt_c = (int*)rs.work;
-    float* part_c = (float*)((char*)rs.work + 4096);
+    float* part_c = (float*)((char*)rs.work + att_partials_offset(nrows));
     dim3 grid(ns, nrows);
 #define LO_ATT_BWD(TY_, NV)                                                                                                       \
   attention_bwd_kernel<TY_, NV><<<grid, LO_ATT_THREADS, 0, st>>>(                                                                 \

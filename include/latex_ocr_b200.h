@@ -443,7 +443,7 @@ typedef struct lo_tfdec_args {
   int32_t ldl;             /* row stride of logits / dlogits (>= V, multiple of 8) */
   int32_t rows_per_img;    /* decode only: beam size (consecutive rows share one image); 0/1 otherwise */
   float inv_n_words;       /* 1 / sum(lengths): the loss is the mean over valid tokens */
-  const void* enc;         /* big [B/rows_per_img][R][C] */
+  const void* enc;         /* big [B/rows_per_img][R][C] (packed [reg_off[n]][C] with reg_off, below) */
   const int64_t* formula;  /* [B][formula_stride] target ids; step t consumes formula[:, t-1], predicts formula[:, t] */
   int64_t formula_stride;
   const int32_t* lengths;  /* device [B]: valid tokens per row incl. END (sequence_mask, img2seq.py:69) */
@@ -471,6 +471,15 @@ typedef struct lo_tfdec_args {
                               instead of enc + att1 (60.5 MB instead of 114 MB per step at cfg #2).  NULL: att1 is re-read. */
   float* loss;             /* [4]: mean CE over valid tokens (x2), 0, n_words — ce_words (img2seq.py:74) = loss[0] * loss[3] */
   float* denc;             /* f32 [B][R][C] gradient w.r.t. the encoder output */
+  /* decode of images of different sizes (lo_tfdec_greedy and lo_tfdec_beam[_div] only), as lo_decoder_args.reg_off: prefix offsets
+   * of the images' regions, [B / rows_per_img + 1] each, the same values on the device and on the host.  Image i owns regions
+   * [reg_off[i], reg_off[i+1]) of a PACKED enc [reg_off[n]][C] (n = B / rows_per_img; beam rows share their image's regions).  R is
+   * then the largest count: the row stride of alphas [B][T][R], whose entries past an image's own count are left untouched.  Every
+   * image attends over its own regions only, so its tokens are those it gets when decoded alone.  Both NULL: every image has R
+   * regions.  Refused (LO_EINVAL) before any GPU work, with the messages of lo_decoder_args: one set without the other, either on
+   * lo_tfdec_forward / lo_tfdec_backward, reg_off_host[0] != 0, a count below 1 or above R, and att_pipe = 0. */
+  const int32_t* reg_off;
+  const int32_t* reg_off_host;
   void* ws;                /* lo_tfdec_workspace_bytes(args) bytes, zero-initialised once by the caller */
   const float* dlogits_ext; /* generic backward (below): d loss / d logits, fp32 rows (b, t) batch-major, dlogits_stride apart */
   int64_t dlogits_stride;  /* elements between consecutive (b, t) rows of dlogits_ext (>= V) */

@@ -441,8 +441,8 @@ __global__ void __launch_bounds__(AP_THREADS, LO_ATT_MINB) attention_fwd_pipe_ke
 
 // Ragged layout (decode of images of different sizes): image i owns regions [reg_off[i], reg_off[i+1]) of the packed att1 / enc.
 // One-dimensional cluster-free grid; CTA x does the work cta_map[x] = {row b, split, splits of row b, first partial slot of row b}
-// says (attention_ragged_map_kernel).  Decode only: ReLU score, no mask bits.
-template <typename T, int NVA, int NVC>
+// says (attention_ragged_map_kernel).  Decode only, no mask bits: ReLU score (ACT = 0, torch flavour) or tanh (ACT = 1, Genthial cell).
+template <typename T, int NVA, int NVC, int ACT>
 __global__ void __launch_bounds__(AP_THREADS, LO_ATT_MINB) attention_fwd_ragged_kernel(
     const T* __restrict__ att1, const T* __restrict__ enc, const float* __restrict__ att2, int64_t att2_stride,
     const float* __restrict__ wf, float* __restrict__ alpha, int64_t alpha_stride, float* __restrict__ ctx,
@@ -453,9 +453,9 @@ __global__ void __launch_bounds__(AP_THREADS, LO_ATT_MINB) attention_fwd_ragged_
   const int4 e = cta_map[blockIdx.x];
   const int img = e.x / rpi;
   const int g0 = reg_off[img];
-  attention_fwd_pipe_cta<T, NVA, NVC, false, 0, false>(att1, enc, att2, att2_stride, wf, alpha, alpha_stride, ctx, gate_pre, gate_stride,
-                                                      gctx, gctx_bf, reg_off[img + 1] - g0, e.z, counters, partials, keep_q, nullptr,
-                                                      e.x, e.y, (int64_t)g0, (int64_t)e.w);
+  attention_fwd_pipe_cta<T, NVA, NVC, false, ACT, false>(att1, enc, att2, att2_stride, wf, alpha, alpha_stride, ctx, gate_pre, gate_stride,
+                                                        gctx, gctx_bf, reg_off[img + 1] - g0, e.z, counters, partials, keep_q, nullptr,
+                                                        e.x, e.y, (int64_t)g0, (int64_t)e.w);
 }
 
 // Splits of one row of the ragged launch: its share of ns * B splits in proportion to its region count, at least 1 and at most
@@ -1532,30 +1532,40 @@ int attention_ragged_prepare(AttRagged& rg, int B, int rpi, cudaStream_t st) {
   return LO_OK;
 }
 
-template <typename T, int NV>
+template <typename T, int NVA, int NVC, int ACT>
 static int fwd_ragged_launch(const AttFwdArgs& x, const AttRagged& rg, cudaStream_t st) {
-  using C = ApCfg<T, NV, NV>;
+  using C = ApCfg<T, NVA, NVC>;
   static bool attr = false;
   if (!attr) {
-    LO_CUDA(cudaFuncSetAttribute(attention_fwd_ragged_kernel<T, NV, NV>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM));
+    LO_CUDA(cudaFuncSetAttribute(attention_fwd_ragged_kernel<T, NVA, NVC, ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM));
     attr = true;
   }
   const int4* map = (const int4*)rg.map;
   const int rpi = x.rows_per_img > 1 ? x.rows_per_img : 1;
   const int keep_q = att_keep_q((int64_t)rg.reg_off_host[x.B / rpi] * (C::CHA + C::CHC) * (int64_t)sizeof(T));    // all regions, once
-  LO_CUDA(launch_att(attention_fwd_ragged_kernel<T, NV, NV>, dim3(rg.ctas), (size_t)C::SMEM, 1, st, true, (const T*)x.att1,
+  LO_CUDA(launch_att(attention_fwd_ragged_kernel<T, NVA, NVC, ACT>, dim3(rg.ctas), (size_t)C::SMEM, 1, st, true, (const T*)x.att1,
                      (const T*)x.enc, x.att2, x.att2_stride, x.wf, x.alpha, x.alpha_stride, x.ctx, x.gate_pre, x.gate_stride, x.gctx,
                      x.gctx_bf, map, rg.reg_off, rpi, (int*)(map + (int64_t)x.B * AP_MAXSPLIT), (float*)((char*)x.work + att_partials_offset(x.B)), keep_q));
   LO_LAUNCH_OK();
   return LO_OK;
 }
 
+template <typename T, int NVA, int NVC>
+static int fwd_ragged_act(const AttFwdArgs& x, const AttRagged& rg, cudaStream_t st) {
+  return x.act == 1 ? fwd_ragged_launch<T, NVA, NVC, 1>(x, rg, st) : fwd_ragged_launch<T, NVA, NVC, 0>(x, rg, st);
+}
+
+// the width pairs of fwd_dispatch: A == C in {256, 512, 1024} with either score, and (A, C) = (256, 512), which only the Genthial
+// cell (tanh) uses
 template <typename T>
 static int fwd_ragged_dispatch(const AttFwdArgs& x, const AttRagged& rg, int C, cudaStream_t st) {
-  if (C == 256) return fwd_ragged_launch<T, 1>(x, rg, st);
-  if (C == 512) return fwd_ragged_launch<T, 2>(x, rg, st);
-  if (C == 1024) return fwd_ragged_launch<T, 4>(x, rg, st);
-  return fail(LO_EINVAL, "%s: attention width %ld not instantiated", __func__, (long)C);
+  const int A = x.a_ch > 0 ? x.a_ch : C;
+  if (A == 256 && C == 512 && x.act == 1) return fwd_ragged_launch<T, 1, 2, 1>(x, rg, st);
+  if (A == C && C == 256) return fwd_ragged_act<T, 1, 1>(x, rg, st);
+  if (A == C && C == 512) return fwd_ragged_act<T, 2, 2>(x, rg, st);
+  if (A == C && C == 1024) return fwd_ragged_act<T, 4, 4>(x, rg, st);
+  return fail(LO_EINVAL, x.act == 1 ? "%s: attention width pair (%ld, %ld), tanh score, not instantiated"
+                                    : "%s: attention width pair (%ld, %ld), ReLU score, not instantiated", __func__, A, C);
 }
 int attention_fwd_ragged(const AttFwdArgs& x, const AttRagged& rg, int dt, int C, cudaStream_t st) {
   return dt == LO_F32 ? fwd_ragged_dispatch<float>(x, rg, C, st) : fwd_ragged_dispatch<bf16>(x, rg, C, st);

@@ -304,7 +304,8 @@ struct AttRagged {
 int64_t attention_ragged_map_bytes(int B);
 // once per decode call: the grid size (host) and the CTA map (device, stream-ordered)
 int attention_ragged_prepare(AttRagged& rg, int B, int rpi, cudaStream_t st);
-// x.B rows (x.R unused, x.alpha_stride >= the largest count), x.work as for attention_fwd_pipe; ReLU score, A == C, no mask bits
+// x.B rows (x.R unused, x.alpha_stride >= the largest count), x.work as for attention_fwd_pipe; no mask bits.  x.act / x.a_ch as
+// for attention_fwd_pipe: A == C in {256, 512, 1024} with either score, (A, C) = (256, 512) with the tanh score
 int attention_fwd_ragged(const AttFwdArgs& x, const AttRagged& rg, int dt, int C, cudaStream_t st);
 
 // wgmma paths (lo_tc.cu)

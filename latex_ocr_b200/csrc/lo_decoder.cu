@@ -1028,22 +1028,23 @@ static int check_args(const lo_decoder_args* a) {
   return LO_OK;
 }
 
-// per-image region counts (reg_off / reg_off_host): decode entry points only
-static int check_reg_off(const lo_decoder_args* a) {
-  if (!a->reg_off && !a->reg_off_host) return LO_OK;
-  LO_CHECK_ARG(a->reg_off && a->reg_off_host, "reg_off and reg_off_host must be set together");
+// per-image region counts (reg_off / reg_off_host of lo_decoder_args and lo_tfdec_args): decode entry points only.  `decode`: the
+// call is a greedy / beam entry point (the offsets are validated), otherwise a training one (the offsets are refused).
+static int check_reg_off(const int32_t* reg_off, const int32_t* reg_off_host, int B, int rows_per_img, int R, bool decode) {
+  if (!reg_off && !reg_off_host) return LO_OK;
+  LO_CHECK_ARG(decode, "reg_off / reg_off_host (per-image region counts) are for the decode entry points only");
+  LO_CHECK_ARG(reg_off && reg_off_host, "reg_off and reg_off_host must be set together");
   LO_CHECK_ARG(g_opt_att_pipe, "per-image region counts (reg_off) need the pipelined attention kernels (att_pipe = 1)");
-  const int rpi = a->rows_per_img > 1 ? a->rows_per_img : 1;
-  LO_CHECK_ARG(a->reg_off_host[0] == 0, "reg_off_host[0] must be 0");
-  for (int i = 0; i < a->B / rpi; i++) {
-    const int n = a->reg_off_host[i + 1] - a->reg_off_host[i];
-    LO_CHECK_ARG(n >= 1 && n <= a->R, "region count of every image in 1..R (reg_off_host)");
+  const int rpi = rows_per_img > 1 ? rows_per_img : 1;
+  LO_CHECK_ARG(reg_off_host[0] == 0, "reg_off_host[0] must be 0");
+  for (int i = 0; i < B / rpi; i++) {
+    const int n = reg_off_host[i + 1] - reg_off_host[i];
+    LO_CHECK_ARG(n >= 1 && n <= R, "region count of every image in 1..R (reg_off_host)");
   }
   return LO_OK;
 }
-static int refuse_reg_off(const lo_decoder_args* a) {
-  LO_CHECK_ARG(!a->reg_off && !a->reg_off_host, "reg_off / reg_off_host (per-image region counts) are for the decode entry points only");
-  return LO_OK;
+static int check_reg_off(const lo_decoder_args* a, bool decode) {
+  return check_reg_off(a->reg_off, a->reg_off_host, a->B, a->rows_per_img, a->R, decode);
 }
 // the ragged attention state of a decode call: map in the second attention region of `work` (the decode loop runs one row chain)
 static AttRagged ragged_of(const lo_decoder_args* a) {
@@ -1462,7 +1463,7 @@ int lo_attention_step_backward(const void* enc, const void* att1, int dt, const 
 
 int lo_decoder_forward(const lo_decoder_args* a, int with_loss, void* stream) {
   LO_TRY(check_args(a));
-  LO_TRY(refuse_reg_off(a));
+  LO_TRY(check_reg_off(a, false));
   cudaStream_t st = (cudaStream_t)stream;
   const Dims d = dims(a);
   const bool ragged = a->bt_host[d.T - 1] < d.B;
@@ -1616,7 +1617,7 @@ int lo_decoder_pack_bwd_weights(const lo_decoder_args* a, void* stream) {
 
 int lo_decoder_backward(const lo_decoder_args* a, void* stream) {
   LO_TRY(check_args(a));
-  LO_TRY(refuse_reg_off(a));
+  LO_TRY(check_reg_off(a, false));
   LO_CHECK_ARG(!a->dpred_ext || a->dlogits, "dpred_ext needs dlogits");
   LO_CHECK_ARG(!a->dpred_ext || a->dpred_stride >= a->V, "dpred_stride >= V");
   LO_CHECK_ARG(a->phase != 2 || !a->dalpha_ext, "phase 2 reads no d alpha: pass dalpha_ext to the phase-1 call");
@@ -2010,7 +2011,7 @@ int lo_decoder_backward(const lo_decoder_args* a, void* stream) {
 int lo_decoder_greedy_hist(const lo_decoder_args* a, int64_t start_id, int64_t end_id, int max_steps, int64_t* tokens,
                            int32_t* finished, int32_t* fin_hist, void* stream) {
   LO_TRY(check_args(a));
-  LO_TRY(check_reg_off(a));
+  LO_TRY(check_reg_off(a, true));
   LO_CHECK_ARG(!a->ss_prob, "scheduled sampling (ss_prob) is a training mode: greedy decode feeds its own argmax already");
   LO_CHECK_ARG(tokens && finished && max_steps > 0 && max_steps <= a->T, "tokens/finished/max_steps (<= T capacity)");
   cudaStream_t st = (cudaStream_t)stream;
@@ -2056,7 +2057,7 @@ int lo_decoder_beam_div(const lo_decoder_args* a, int64_t start_id, int64_t end_
                         int32_t* fin_hist, float* logp, float div_gamma, float div_prob, const float* div_u,
                         const uint64_t* div_state, void* stream) {
   LO_TRY(check_args(a));
-  LO_TRY(check_reg_off(a));
+  LO_TRY(check_reg_off(a, true));
   LO_CHECK_ARG(!a->ss_prob, "scheduled sampling (ss_prob) is a training mode: not available in beam search");
   const bool div_on = !(div_gamma == 1.f || div_prob == 0.f);               // beam_search_decoder_cell.py:270-273
   LO_CHECK_ARG(!div_on || (div_gamma > 0.f && (div_u || div_state)), "diversity penalty needs gamma > 0 and div_u or div_state");

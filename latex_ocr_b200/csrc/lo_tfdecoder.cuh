@@ -241,6 +241,7 @@ struct TfWs {
   bf16 *xh_bf, *ctx_bf, *dout2_bf, *dz_bf, *dlogits_bf, *hd_bf;
   void *wb4, *wb5, *wb6, *wbY, *wimgT;            // dt: transposed weights for the backward GEMMs
   void* attwork;
+  void* ragmap;                                   // ragged decode (reg_off): CTA map and ticket counters of the attention launch
   int64_t* next_tok;
   int32_t *finished, *parent_rows;
   size_t bytes;
@@ -304,11 +305,17 @@ static TfWs tf_carve(const lo_tfdec_args* a) {
   w.finished = (int32_t*)take((size_t)d.B * 4);
   w.parent_rows = (int32_t*)take((size_t)d.B * 4);
   w.sreg = (float*)take(TB * 4);                                      // generic backward: [B][T] sum_r alpha d alpha
+  w.ragmap = take((size_t)attention_ragged_map_bytes(d.B));
   w.bytes = off;
   return w;
 }
 
-static int tf_check(const lo_tfdec_args* a) {
+// `decode`: a greedy / beam entry point (the only ones that take per-image region counts)
+static int check_reg_off(const lo_tfdec_args* a, bool decode) {
+  return check_reg_off(a->reg_off, a->reg_off_host, a->B, a->rows_per_img, a->R, decode);
+}
+
+static int tf_check(const lo_tfdec_args* a, bool decode) {
   LO_CHECK_ARG(a != nullptr, "null args");
   LO_CHECK_ARG(a->B > 0 && a->B <= 512 && a->T > 0 && a->R > 0 && a->V > 1, "B in 1..512, T, R > 0, V > 1");
   LO_CHECK_ARG(a->C == 256 || a->C == 512 || a->C == 1024, "channels in {256,512,1024}");
@@ -321,6 +328,7 @@ static int tf_check(const lo_tfdec_args* a) {
                "null parameter");
   const int rpi = a->rows_per_img > 1 ? a->rows_per_img : 1;
   LO_CHECK_ARG(a->B % rpi == 0, "B must be a multiple of rows_per_img");
+  LO_TRY(check_reg_off(a, decode));
   LO_CHECK_ARG(g_opt_att_pipe, "the Genthial cell runs on the TMA-ring attention kernels only (option att_pipe=1)");
   return LO_OK;
 }
@@ -348,13 +356,17 @@ static int tf_tn(const lo_tfdec_args* a, const float* A32, const bf16* Abf, int6
 
 static int tf_prologue(const lo_tfdec_args* a, const TfDims& d, const TfWs& w, cudaStream_t st) {
   const int dt = a->dt;
-  // att_img = img W_img, no bias, once (attention_mechanism.py:43)
-  LO_TRY(gemm_nt(a->enc, dt, d.C, a->w_img, dt, d.C, w.att_img, dt, d.A, d.nimg * d.R, d.A, d.C, nullptr, 0, 0, a->impl, st));
+  // att_img = img W_img, no bias, once (attention_mechanism.py:43); packed layout (reg_off): every region of every image once
+  const int enc_rows = a->reg_off_host ? a->reg_off_host[d.nimg] : d.nimg * d.R;
+  LO_TRY(gemm_nt(a->enc, dt, d.C, a->w_img, dt, d.C, w.att_img, dt, d.A, enc_rows, d.A, d.C, nullptr, 0, 0, a->impl, st));
   // token -> gate pre-activation table: [embedding_table ; start_token] K[:E] + b   (replaces the lookup + x[:, :E] K[:E])
   LO_TRY(gemm_nt(a->emb, dt, d.E, a->w_lstm, dt, d.LW, w.ptab, LO_F32, d.G, d.V + 1, d.G, d.E, a->b_lstm, 0, 0, LO_IMPL_SIMT, st));
   {
     dim3 grid(cdiv(d.C, 256), d.B);
-    LO_DISPATCH_DT(dt, T, (mean_rows_kernel<T><<<grid, 256, 0, st>>>((const T*)a->enc, w.mean, d.R, d.C, d.rpi)));
+    if (a->reg_off)
+      LO_DISPATCH_DT(dt, T, (mean_segments_kernel<T><<<grid, 256, 0, st>>>((const T*)a->enc, w.mean, a->reg_off, d.C, d.rpi)));
+    else
+      LO_DISPATCH_DT(dt, T, (mean_rows_kernel<T><<<grid, 256, 0, st>>>((const T*)a->enc, w.mean, d.R, d.C, d.rpi)));
     LO_LAUNCH_OK();
   }
   const int IW = 2 * d.D + d.O;
@@ -364,9 +376,10 @@ static int tf_prologue(const lo_tfdec_args* a, const TfDims& d, const TfWs& w, c
   return LO_OK;
 }
 
-// one cell step: consumes xh[t] = [o_{t-1} | h_{t-1}], call[t]; produces xh[t+1], call[t+1], alphas[:, t], ctx[t]
+// one cell step: consumes xh[t] = [o_{t-1} | h_{t-1}], call[t]; produces xh[t+1], call[t+1], alphas[:, t], ctx[t].  rg: decode with
+// per-image region counts (the ragged attention launch), NULL otherwise
 static int tf_step(const lo_tfdec_args* a, const TfDims& d, const TfWs& w, int t, const int64_t* tok, int64_t tok_stride,
-                   cudaStream_t st) {
+                   cudaStream_t st, const AttRagged* rg = nullptr) {
   const size_t es = a->dt == LO_F32 ? 4 : 2;
   const int64_t rowt = (int64_t)t * d.B, rown = (int64_t)(t + 1) * d.B;
   const float* xh_t = w.xh + rowt * d.XH;
@@ -390,7 +403,10 @@ static int tf_step(const lo_tfdec_args* a, const TfDims& d, const TfWs& w, int t
   {
     AttFwdArgs x{w.att_img, a->enc, out2, d.N2, a->beta, a->alphas + (int64_t)t * d.R, (int64_t)d.T * d.R, w.ctx + rowt * d.C, nullptr,
                  0, nullptr, w.ctx_bf ? w.ctx_bf + rowt * d.C : nullptr, d.B, d.R, w.attwork, d.rpi, 0, 1, d.A};
-    LO_TRY(attention_fwd_pipe(x, a->dt, d.C, st));
+    if (rg)
+      LO_TRY(attention_fwd_ragged(x, *rg, a->dt, d.C, st));
+    else
+      LO_TRY(attention_fwd_pipe(x, a->dt, d.C, st));
   }
   // o_t = tanh(h_t o_W_h + ctx o_W_c)
   LO_TRY(tf_nt(a, w.ctx + rowt * d.C, w.ctx_bf ? w.ctx_bf + rowt * d.C : nullptr, d.C, a->w_oc, d.C, w.oc, d.O, d.B, d.O, d.C, nullptr, 0,
@@ -401,6 +417,9 @@ static int tf_step(const lo_tfdec_args* a, const TfDims& d, const TfWs& w, int t
   LO_LAUNCH_OK();
   return LO_OK;
 }
+
+// the ragged attention state of a decode call (lo_tfdec_args.reg_off): its CTA map has a workspace region of its own
+static AttRagged tf_ragged(const lo_tfdec_args* a, const TfWs& w) { return AttRagged{a->reg_off, a->reg_off_host, w.ragmap, 0}; }
 
 // logits of `rows` consecutive state rows starting at xh row `row0` (o part) -> out [rows][ldo]
 static int tf_logits(const lo_tfdec_args* a, const TfDims& d, const TfWs& w, int64_t row0, int rows, float* out, int64_t ldo,
@@ -425,7 +444,7 @@ int64_t lo_tfdec_workspace_bytes(const lo_tfdec_args* a) {
 }
 
 int lo_tfdec_forward(const lo_tfdec_args* a, int with_loss, void* stream) {
-  LO_TRY(tf_check(a));
+  LO_TRY(tf_check(a, false));
   LO_CHECK_ARG(a->formula && a->formula_stride >= a->T, "formula [B][>= T]");
   LO_CHECK_ARG(!with_loss || (a->lengths && a->loss && a->inv_n_words > 0.f), "lengths / loss / inv_n_words");
   cudaStream_t st = (cudaStream_t)stream;
@@ -448,7 +467,7 @@ int lo_tfdec_forward(const lo_tfdec_args* a, int with_loss, void* stream) {
 }
 
 int lo_tfdec_backward(const lo_tfdec_args* a, void* stream) {
-  LO_TRY(tf_check(a));
+  LO_TRY(tf_check(a, false));
   LO_CHECK_ARG(a->dlogits_ext || !a->dalpha_ext, "dalpha_ext needs dlogits_ext (generic mode)");
   LO_CHECK_ARG(!a->dlogits_ext || a->dlogits_stride >= a->V, "dlogits_stride >= V");
   LO_CHECK_ARG(a->formula && a->denc, "formula / denc");
@@ -581,15 +600,17 @@ int lo_tfdec_backward(const lo_tfdec_args* a, void* stream) {
 }
 
 int lo_tfdec_greedy(const lo_tfdec_args* a, int64_t end_id, int max_steps, int64_t* tokens, int32_t* fin_hist, void* stream) {
-  LO_TRY(tf_check(a));
+  LO_TRY(tf_check(a, true));
   LO_CHECK_ARG(tokens && max_steps > 0 && max_steps <= a->T, "tokens / max_steps (<= T capacity)");
   cudaStream_t st = (cudaStream_t)stream;
   const TfDims d = tf_dims(a);
   const TfWs w = tf_carve(a);
   LO_CUDA(cudaMemsetAsync(w.finished, 0, (size_t)d.B * 4, st));
   LO_TRY(tf_prologue(a, d, w, st));
+  AttRagged rg = tf_ragged(a, w);
+  if (a->reg_off) LO_TRY(attention_ragged_prepare(rg, d.B, d.rpi, st));
   for (int t = 0; t < max_steps; t++) {
-    LO_TRY(tf_step(a, d, w, t, t == 0 ? nullptr : w.next_tok, 1, st));
+    LO_TRY(tf_step(a, d, w, t, t == 0 ? nullptr : w.next_tok, 1, st, a->reg_off ? &rg : nullptr));
     LO_TRY(tf_logits(a, d, w, (int64_t)(t + 1) * d.B, d.B, a->logits, d.V, st));
     argmax_kernel<<<cdiv(d.B, 8), 256, 0, st>>>(a->logits, d.V, tokens + t, max_steps, w.next_tok, w.finished, end_id, d.B);
     LO_LAUNCH_OK();
@@ -608,7 +629,7 @@ int lo_tfdec_beam(const lo_tfdec_args* a, int64_t end_id, int max_steps, int64_t
 
 int lo_tfdec_beam_div(const lo_tfdec_args* a, int64_t end_id, int max_steps, int64_t* ids, int64_t* parents, int32_t* fin_hist,
                       float* logp, float div_gamma, float div_prob, const float* div_u, const uint64_t* div_state, void* stream) {
-  LO_TRY(tf_check(a));
+  LO_TRY(tf_check(a, true));
   const bool div_on = !(div_gamma == 1.f || div_prob == 0.f);               // beam_search_decoder_cell.py:270-273
   LO_CHECK_ARG(!div_on || (div_gamma > 0.f && (div_u || div_state)), "diversity penalty needs gamma > 0 and div_u or div_state");
   LO_CHECK_ARG(ids && parents && fin_hist && logp && max_steps > 0 && max_steps <= a->T, "outputs / max_steps (<= T capacity)");
@@ -620,11 +641,13 @@ int lo_tfdec_beam_div(const lo_tfdec_args* a, int64_t end_id, int max_steps, int
   LO_CUDA(cudaMemsetAsync(w.finished, 0, (size_t)d.B * 4, st));
   LO_CUDA(cudaMemsetAsync(logp, 0, (size_t)d.B * 4, st));                    // initial log-probs are zeros (:106-107)
   LO_TRY(tf_prologue(a, d, w, st));
+  AttRagged rg = tf_ragged(a, w);
+  if (a->reg_off) LO_TRY(attention_ragged_prepare(rg, d.B, beam, st));
   const size_t smem = (size_t)beam * d.V * 4 * (div_on ? 2 : 1);
   LO_CHECK_ARG(smem <= 200 * 1024, "beam*V too large for the shared-memory top-k");
   if (smem > 48 * 1024) LO_CUDA(cudaFuncSetAttribute(beam_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
   for (int t = 0; t < max_steps; t++) {
-    LO_TRY(tf_step(a, d, w, t, t == 0 ? nullptr : w.next_tok, 1, st));
+    LO_TRY(tf_step(a, d, w, t, t == 0 ? nullptr : w.next_tok, 1, st, a->reg_off ? &rg : nullptr));
     const int64_t rown = (int64_t)(t + 1) * d.B;
     LO_TRY(tf_logits(a, d, w, rown, d.B, a->logits, d.V, st));
     beam_step_kernel<<<d.nimg, 256, smem, st>>>(a->logits, d.V, beam, t, end_id, logp, w.finished, ids, parents, fin_hist, w.next_tok,

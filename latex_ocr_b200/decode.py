@@ -13,6 +13,7 @@ The torch flavour of the reference has no START symbol; the caller supplies ``st
 uint8 array.  A list is decoded in ONE time loop in which every image attends over its own regions only (lo_decoder_args.reg_off):
 no padding, and an image's tokens are those it gets when decoded alone.
 """
+import collections
 import ctypes
 
 import torch
@@ -54,11 +55,15 @@ def _image(x):
     return t
 
 
-def _prepare_ragged(model, images, rows_per_img, max_steps):
-    """Packed encoder output and the argument block of a decode over images of different sizes.  The images are sorted by shape
-    so that the encoder runs once per distinct shape and each run's output (a workspace buffer the next run overwrites) is one
-    contiguous copy into the packed enc.  Returns (args, workspace, order, region counts) with order[j] = the input index of
-    decode image j."""
+RaggedLayout = collections.namedtuple("RaggedLayout", ("imgs", "order", "groups", "counts", "off"))
+
+
+def ragged_layout(images, out_hw):
+    """Decode order and packed layout of a list of images of different sizes (both flavours).  The images are sorted by shape so
+    that the encoder runs once per distinct shape and each run's output (a workspace buffer the next run overwrites) is one
+    contiguous copy into the packed enc.  ``out_hw(H, W)``: the encoder's feature-map size.  Returns a RaggedLayout: the images as
+    [1,H,W] tensors in input order; order[j] = the input index of decode image j; groups = [first, end) runs of one shape in decode
+    order; counts[j] = the region count of decode image j; off = their prefix offsets (reg_off)."""
     imgs = [_image(x) for x in images]
     if not imgs:
         raise ValueError("no images")
@@ -71,21 +76,35 @@ def _prepare_ragged(model, images, rows_per_img, max_steps):
             groups.append([j, j + 1])
     counts = []
     for j0, j1 in groups:
-        h, w = model.encoder.out_hw(*imgs[order[j0]].shape[1:])
+        h, w = out_hw(*imgs[order[j0]].shape[1:])
         counts += [h * w] * (j1 - j0)
     if min(counts) < 1:
         raise ValueError("an image is too small for the encoder (no feature-map region)")
-    N, R, dev, dec = len(imgs), max(counts), model.device, model.decoder
-    B = N * rows_per_img
     off = [0]
     for n in counts:
         off.append(off[-1] + n)
-    ws = dec.ragged_workspace(B, max_steps, R, off[-1])
-    enc = ws["t"]["enc"]
-    for j0, j1 in groups:
-        batch = torch.stack([imgs[order[j]] for j in range(j0, j1)]).to(dev)
-        e = model.encoder.forward_raw(batch if batch.dtype == torch.uint8 else batch.float(), need_grad=False)
+    return RaggedLayout(imgs, order, groups, counts, off)
+
+
+def encode_packed(encoder, lay, enc, device):
+    """Runs ``encoder`` once per shape group of ``lay`` and writes its output into the packed ``enc`` [regions, C] in decode
+    order."""
+    imgs, order, off = lay.imgs, lay.order, lay.off
+    for j0, j1 in lay.groups:
+        batch = torch.stack([imgs[order[j]] for j in range(j0, j1)]).to(device)
+        e = encoder.forward_raw(batch if batch.dtype == torch.uint8 else batch.float(), need_grad=False)
         enc[off[j0]:off[j1]].copy_(e.reshape(off[j1] - off[j0], e.shape[3]))
+
+
+def _prepare_ragged(model, images, rows_per_img, max_steps):
+    """Packed encoder output and the argument block of a decode over images of different sizes (ragged_layout).  Returns (args,
+    workspace, order, region counts) with order[j] = the input index of decode image j."""
+    lay = ragged_layout(images, model.encoder.out_hw)
+    order, counts, off = lay.order, lay.counts, lay.off
+    N, R, dev, dec = len(order), max(counts), model.device, model.decoder
+    B = N * rows_per_img
+    ws = dec.ragged_workspace(B, max_steps, R, off[-1])
+    encode_packed(model.encoder, lay, ws["t"]["enc"], dev)
     host = ws["reg_off_host"]
     for i, v in enumerate(off):
         host[i] = v
@@ -93,7 +112,7 @@ def _prepare_ragged(model, images, rows_per_img, max_steps):
     dec.store.refresh_shadow()
     for t in range(max_steps):
         ws["bt"][t] = B
-    a = dec.fill_args(ws, enc, B, max_steps, R, has_dropout=False)
+    a = dec.fill_args(ws, ws["t"]["enc"], B, max_steps, R, has_dropout=False)
     a.rows_per_img = rows_per_img
     a.reg_off = ws["t"]["reg_off"].data_ptr()
     a.reg_off_host = ctypes.cast(host, ctypes.c_void_p)

@@ -204,9 +204,39 @@ class Img2SeqModel:
 
     def predict_batch(self, images):
         """img2seq.py:256-275: list over hypotheses (1 for greedy, beam_size for beam search) of N token-id lists, truncated at END."""
-        from . import decode
         enc = self.encoder.forward_raw(self._to_device_images(images))
-        ids = self.decoder.decode(enc).ids
+        return self._format(self.decoder.decode(enc).ids)
+
+    def predict_images(self, images):
+        """``predict_batch`` for a list of images of different sizes (HxWx1 uint8 arrays or [1,H,W] tensors), each decoded at its
+        own size in one time loop: no padding to the largest image, so an image's prediction does not depend on the other images
+        of the call (``predict_batch`` keeps the reference's padding).  The images are sorted by shape and the encoder runs once
+        per shape.  A list of more than ``tf_decoder.MAX_ROWS`` decoder rows (images x beam) is decoded in consecutive chunks of
+        input order, each chunk as its own call.  Same return value as ``predict_batch``."""
+        from .tf_decoder import MAX_ROWS
+        images = list(images)
+        if not images:
+            raise ValueError("no images")
+        per = max(1, MAX_ROWS // self.decoder._tiles)
+        hyps = None
+        for k in range(0, len(images), per):
+            part = self._predict_chunk(images[k:k + per])
+            hyps = part if hyps is None else [h + p for h, p in zip(hyps, part)]
+        return hyps
+
+    def _predict_chunk(self, images):
+        from . import decode
+        dec = self.decoder
+        lay = decode.ragged_layout(images, self.encoder.out_hw)
+        steps = dec.max_length_formula + 2
+        ws = dec.packed_workspace(lay.counts, steps)               # decode order: sorted by shape
+        decode.encode_packed(self.encoder, lay, ws["enc"], self.device)
+        ids = dec.decode_packed(ws, steps).ids
+        return self._format(ids[decode._inverse(lay.order).to(ids.device)])
+
+    def _format(self, ids):
+        """greedy ids [N, time] or beam ids [N, time, beam] -> list over hypotheses of N token-id lists, truncated at END"""
+        from . import decode
         if ids.dim() == 2:
             return [decode.truncate_end(ids.tolist(), self._vocab.id_end)]
         return [decode.truncate_end(ids[:, :, k].tolist(), self._vocab.id_end) for k in range(ids.shape[2])]

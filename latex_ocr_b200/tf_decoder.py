@@ -8,7 +8,8 @@ The reference builds a TF graph; here the same three things the graph offers are
                                                  through ``loss.backward()`` (lo_tfdec_backward in its generic mode)
   * ``loss_and_backward(enc, formula, len)``  -> masked CE of img2seq.py:68-71 + every gradient (+ d enc)
   * ``decode(enc)``                           -> DecoderOutput(logits=None, ids)          (decoder.py:59-70; greedy ids [N,time],
-                                                 beam ids [N,time,beam] like the TF cell before img2seq.py:241 transposes them)
+                                                 beam ids [N,time,beam] like the TF cell before img2seq.py:241 transposes them);
+                                                 ``enc`` may be a list of images' encoder outputs of different sizes
 ``__call__(img, formula, dropout)`` returns ``(train_logits, DecoderOutput)`` like the reference.
 
 Variables keep the TF names and shapes (``embedding_table`` [V,E], ``start_token`` [E], ``att_img.kernel`` [C,A],
@@ -30,6 +31,7 @@ from .params import FlatStore, LRUCache, ParamHolder, bind_grads
 
 DecoderOutput = collections.namedtuple("DecoderOutput", ("logits", "ids"))      # greedy_decoder_cell.py:5-6
 _bind = _lib.lib          # the library with the lo_tfdec_* signatures set (lib() binds them along with the rest)
+MAX_ROWS = 512            # decoder rows (images x beam) of one lo_tfdec_* call: the library refuses more
 
 
 def tf_decoder_specs(V, C, A, D, O, E):
@@ -114,12 +116,13 @@ class Decoder(nn.Module):
                 sd[k].copy_(v.reshape(sd[k].shape))
 
     # ---------------------------------------------------------------------------------------------
-    def _args(self, enc, B, T, R, rows_per_img=1, decode=False):
+    def _args(self, enc, B, T, R, rows_per_img=1, decode=False, ws=None):
         """Args and workspace of one shape.  Decoding has workspaces of its own, so a decode never overwrites the saved state of
-        a teacher-forced pass whose autograd backward is still to run (Decoder.forward runs both)."""
+        a teacher-forced pass whose autograd backward is still to run (Decoder.forward runs both).  ``ws``: a workspace of the
+        caller's (ragged_workspace) instead of the shape's own."""
         L = _lib.lib()
         key = (B, T, R, rows_per_img, "decode") if decode else (B, T, R, rows_per_img)
-        ws = self._ws.get(key)
+        ws = self._ws.get(key) if ws is None else ws
         dev = self.store.device
         if ws is None:
             ws = {"ldl": (self.V + 63) // 64 * 64}
@@ -149,7 +152,7 @@ class Decoder(nn.Module):
         a.g_w_lstm, a.g_b_lstm, a.g_w_oc, a.g_w_y = G("lstm.kernel"), G("lstm.bias"), G("o_W_c"), G("y_W_o")
         a.g_w_init, a.g_b_init, a.g_emb = G("W_c_0"), G("b_c_0"), G("embedding_table")
         for k in ("logits", "alphas", "loss", "denc"):
-            setattr(a, k, ws[k].data_ptr())
+            setattr(a, k, ws[k].data_ptr() if ws[k] is not None else None)
         if "ws" not in ws:
             ws["ws"] = torch.zeros(int(L.lo_tfdec_workspace_bytes(ctypes.byref(a))), dtype=torch.uint8, device=dev)
         a.ws = ws["ws"].data_ptr()
@@ -244,51 +247,149 @@ class Decoder(nn.Module):
             denc = self.run_backward(ws)
             return ws["loss"], denc
 
-    def decode(self, enc, max_steps=None, div_u=None, return_attention=False):
+    def ragged_workspace(self, B, T, R, n_regions):
+        """Decode workspace for images of different sizes (lo_tfdec_args.reg_off): the packed encoder output ``enc`` [regions, C],
+        the region offsets ``reg_off`` / ``reg_off_host`` and every per-row buffer, sized by capacity (rows B, steps T, largest
+        region count R, total regions).  One cache entry: a later call whose composition fits reuses it, a larger one replaces it
+        by the element-wise maximum of both capacities (serving traffic gives a new composition on nearly every call)."""
+        ws = self._ws.get("ragged")
+        if ws is not None:
+            cap = ws["cap"]
+            if B <= cap[0] and T <= cap[1] and R <= cap[2] and n_regions <= cap[3]:
+                return ws
+            B, T, R, n_regions = max(B, cap[0]), max(T, cap[1]), max(R, cap[2]), max(n_regions, cap[3])
+            del self._ws["ragged"]
+        dev = self.store.device
+        ldl = (self.V + 63) // 64 * 64
+        z = lambda *shape, dtype=torch.float32: torch.zeros(*shape, dtype=dtype, device=dev)
+        ws = {"cap": (B, T, R, n_regions), "ldl": ldl,
+              "logits": z(B, ldl),                    # decoding writes one step's logits, [B][V]
+              "alphas": z(B * T * R),                 # [B][T][R] of each call's own B, T and R
+              "loss": z(4), "denc": None, "formula": z(B, T, dtype=torch.int64), "lengths": z(B, dtype=torch.int32),
+              "enc": z(n_regions, self.C, dtype=self.tdtype),
+              "reg_off": z(B + 1, dtype=torch.int32), "reg_off_host": (ctypes.c_int32 * (B + 1))()}
+        self._ws["ragged"] = ws
+        # sizes the kernel workspace: every region of it grows with B, T, R and B / rows_per_img, so any call that fits the
+        # capacity fits in it (the beam size is the decoder's own, fixed at construction)
+        self._args(ws["enc"], B, T, R, rows_per_img=self._tiles, ws=ws)
+        return ws
+
+    def packed_workspace(self, counts, steps):
+        """The ragged workspace of one decode call over images of ``counts`` regions (in the order they are decoded), with their
+        offsets written.  The caller writes image i's encoder output into ``ws["enc"][off[i]:off[i+1]]`` (``ws["off"]``) and then
+        calls decode_packed."""
+        N = len(counts)
+        if N == 0:
+            raise ValueError("no images")
+        if min(counts) < 1:
+            raise ValueError("an image has no encoder region")
+        if N * self._tiles > MAX_ROWS:
+            raise ValueError("%d images x beam %d exceed the %d rows of one decode call" % (N, self._tiles, MAX_ROWS))
+        off = [0]
+        for n in counts:
+            off.append(off[-1] + int(n))
+        ws = self.ragged_workspace(N * self._tiles, steps, max(counts), off[-1])
+        host = ws["reg_off_host"]
+        for i, v in enumerate(off):
+            host[i] = v
+        ws["reg_off"][:N + 1].copy_(torch.tensor(off, dtype=torch.int32))
+        ws["counts"], ws["off"] = [int(n) for n in counts], off
+        return ws
+
+    def decode_packed(self, ws, steps, div_u=None, return_attention=False, return_log_probs=False):
+        """decode() over the images packed in ``ws`` by packed_workspace: every image attends over its own regions only."""
+        counts = ws["counts"]
+        N, beam = len(counts), self._tiles
+        R = max(counts)
+        self.store.refresh_shadow()
+        with torch.no_grad():
+            L, ws, a = self._args(ws["enc"], N * beam, steps, R, rows_per_img=beam, ws=ws)
+            a.reg_off = ws["reg_off"].data_ptr()
+            a.reg_off_host = ctypes.cast(ws["reg_off_host"], ctypes.c_void_p)
+            alphas = ws["alphas"][:N * beam * steps * R].view(N * beam, steps, R) if return_attention else None
+            out = self._run_decode(L, a, N, steps, div_u, alphas, return_log_probs)
+            if alphas is not None and self.decoding == "greedy":
+                out, att = out
+                return out, [att[i, :, :counts[i]].clone() for i in range(N)]
+            return out
+
+    def decode(self, enc, max_steps=None, div_u=None, return_attention=False, return_log_probs=False):
         """dynamic_decode(decoder_cell, max_length_formula + 1) (decoder.py:70): at most max_length_formula + 2 steps, stops when
         every row / beam has emitted END.  Returns DecoderOutput(logits=None, ids).  ``div_u`` (tests): injected uniforms
         [steps, N*beam, V] for the diversity penalty; ``return_attention`` (greedy): also the attention weights [N, steps, R]
-        (the tensor attention_mechanism.py:96-121 hands to visualize_attention.py)."""
+        (the tensor attention_mechanism.py:96-121 hands to visualize_attention.py); ``return_log_probs`` (beam search): also the
+        log-probs of the hypotheses [N, beam].
+
+        ``enc`` [N,R,C] / [N,H,W,C], or a list of the encoder outputs of images of different sizes, each [H_i,W_i,C] or [R_i,C]:
+        the list is decoded in one time loop in which every image attends over its own regions only (lo_tfdec_args.reg_off), so
+        an image's ids do not depend on the other images of the call.  Ids come back in input order, image i draws the rows
+        [i*beam, (i+1)*beam) of ``div_u``, and ``return_attention`` gives a list of [steps, R_i] tensors."""
+        steps = int(max_steps) if max_steps is not None else self.max_length_formula + 2
+        if isinstance(enc, (list, tuple)):
+            encs = [self._enc_regions(e) for e in enc]
+            ws = self.packed_workspace([e.shape[0] for e in encs], steps)
+            off = ws["off"]
+            for i, e in enumerate(encs):
+                ws["enc"][off[i]:off[i + 1]].copy_(e)
+            return self.decode_packed(ws, steps, div_u, return_attention, return_log_probs)
         enc = self._enc(enc)
         N, R, _ = enc.shape
         beam = self._tiles
-        steps = int(max_steps) if max_steps is not None else self.max_length_formula + 2
         B = N * beam
         self.store.refresh_shadow()
         with torch.no_grad():
             L, ws, a = self._args(enc, B, steps, R, rows_per_img=beam, decode=True)
             ws["enc"] = enc
-            dev = self.store.device
-            if self.decoding == "greedy":
-                tokens = torch.zeros(N, steps, dtype=torch.int64, device=dev)
-                fin = torch.zeros(N, steps, dtype=torch.int32, device=dev)
-                check(L.lo_tfdec_greedy(ctypes.byref(a), self._id_end, steps, tokens.data_ptr(), fin.data_ptr(), stream_ptr()))
-                done = fin.bool().all(dim=0)                            # dynamic_decode.py:38-40: loop ends once all rows finished
-                n = int(torch.nonzero(done)[0]) + 1 if bool(done.any()) else steps
-                if return_attention:
-                    return DecoderOutput(None, tokens[:, :n]), ws["alphas"][:, :n].float().clone()
-                return DecoderOutput(None, tokens[:, :n])
-            ids = torch.zeros(N, steps, beam, dtype=torch.int64, device=dev)
-            parents = torch.zeros_like(ids)
-            fin = torch.zeros(N, steps, beam, dtype=torch.int32, device=dev)
-            logp = torch.zeros(N, beam, dtype=torch.float32, device=dev)
-            u_dev = None
-            div_on = not (self.div_gamma == 1 or self.div_prob == 0)
-            if div_on and div_u is not None:
-                u_dev = torch.as_tensor(div_u, dtype=torch.float32).to(dev).contiguous()
-                if tuple(u_dev.shape) != (steps, B, self.V):
-                    raise ValueError("div_u must be [steps, N * beam, V]")
-            elif div_on:
-                if self._div_state is None:
-                    self._div_state = torch.tensor([torch.initial_seed() & 0x7FFFFFFFFFFFFFFF, 0], dtype=torch.int64, device=dev)
-                self._div_state[1] += 1                                  # a new Philox stream per decode call
-            check(L.lo_tfdec_beam_div(ctypes.byref(a), self._id_end, steps, ids.data_ptr(), parents.data_ptr(), fin.data_ptr(),
-                                      logp.data_ptr(), self.div_gamma, self.div_prob, u_dev.data_ptr() if u_dev is not None else None,
-                                      self._div_state.data_ptr() if (div_on and u_dev is None) else None, stream_ptr()))
-            done = fin.bool().all(dim=2).all(dim=0)
+            return self._run_decode(L, a, N, steps, div_u, ws["alphas"] if return_attention else None, return_log_probs)
+
+    def _enc_regions(self, e):
+        """one image's encoder output of a list -> [R_i, C] on the device"""
+        if not e.is_cuda:
+            raise _lib.LatexOcrB200Error("Decoder runs on CUDA tensors only (no CPU fallback)")
+        if e.dim() == 3:
+            e = e.reshape(e.shape[0] * e.shape[1], e.shape[2])
+        if e.dim() != 2 or e.shape[1] != self.C:
+            raise ValueError("each image's encoder output must be [H,W,%d] or [R,%d] (got shape %s)" % (self.C, self.C, tuple(e.shape)))
+        return e
+
+    def _run_decode(self, L, a, N, steps, div_u, alphas, return_log_probs):
+        """The greedy or beam decode of the filled args ``a`` (N images); ``alphas`` [N, steps', R] (greedy attention export) or
+        None."""
+        beam = self._tiles
+        B = N * beam
+        dev = self.store.device
+        if self.decoding == "greedy":
+            tokens = torch.zeros(N, steps, dtype=torch.int64, device=dev)
+            fin = torch.zeros(N, steps, dtype=torch.int32, device=dev)
+            check(L.lo_tfdec_greedy(ctypes.byref(a), self._id_end, steps, tokens.data_ptr(), fin.data_ptr(), stream_ptr()))
+            done = fin.bool().all(dim=0)                            # dynamic_decode.py:38-40: loop ends once all rows finished
             n = int(torch.nonzero(done)[0]) + 1 if bool(done.any()) else steps
-            # finalize (beam_search_decoder_cell.py:189-250) gathers with the unchanged initial parents -> identity (SURVEY §8-A.3)
-            return DecoderOutput(None, ids[:, :n])
+            if alphas is not None:
+                return DecoderOutput(None, tokens[:, :n]), alphas[:, :n].float().clone()
+            return DecoderOutput(None, tokens[:, :n])
+        ids = torch.zeros(N, steps, beam, dtype=torch.int64, device=dev)
+        parents = torch.zeros_like(ids)
+        fin = torch.zeros(N, steps, beam, dtype=torch.int32, device=dev)
+        logp = torch.zeros(N, beam, dtype=torch.float32, device=dev)
+        u_dev = None
+        div_on = not (self.div_gamma == 1 or self.div_prob == 0)
+        if div_on and div_u is not None:
+            u_dev = torch.as_tensor(div_u, dtype=torch.float32).to(dev).contiguous()
+            if tuple(u_dev.shape) != (steps, B, self.V):
+                raise ValueError("div_u must be [steps, N * beam, V]")
+        elif div_on:
+            if self._div_state is None:
+                self._div_state = torch.tensor([torch.initial_seed() & 0x7FFFFFFFFFFFFFFF, 0], dtype=torch.int64, device=dev)
+            self._div_state[1] += 1                                  # a new Philox stream per decode call
+        check(L.lo_tfdec_beam_div(ctypes.byref(a), self._id_end, steps, ids.data_ptr(), parents.data_ptr(), fin.data_ptr(),
+                                  logp.data_ptr(), self.div_gamma, self.div_prob, u_dev.data_ptr() if u_dev is not None else None,
+                                  self._div_state.data_ptr() if (div_on and u_dev is None) else None, stream_ptr()))
+        done = fin.bool().all(dim=2).all(dim=0)
+        n = int(torch.nonzero(done)[0]) + 1 if bool(done.any()) else steps
+        # finalize (beam_search_decoder_cell.py:189-250) gathers with the unchanged initial parents -> identity (SURVEY §8-A.3)
+        if return_log_probs:
+            return DecoderOutput(None, ids[:, :n]), logp
+        return DecoderOutput(None, ids[:, :n])
 
     def forward(self, img, formula=None, dropout=1.0):
         """Decoder.__call__(img, formula, dropout) (decoder.py:24): (pred_train, pred_test).  dropout is the TF keep_prob; the

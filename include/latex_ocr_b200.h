@@ -301,6 +301,14 @@ typedef struct lo_decoder_args {
                               of Philox4x32-10(counter = (0xFFFFFFFF, t, b, call), key = seed) of dropout_state {seed, call} — a
                               counter the dropout stream (j >> 2, t, b, call) never uses.  lo_decoder_backward advances the
                               call counter in this mode as it does for has_dropout = 2 */
+  const float* ss_temp;    /* optional DEVICE scalar tau > 0 (self-critical training, lo_scst_*): a step that samples (u < p) feeds a
+                              draw from softmax(logits[b][t-1] / tau) instead of the argmax,
+                                  fed[b][t] = argmax_v (logits[b][t-1][v] / tau + g_v),  g_v = -log(-log u_v)   (Gumbel-max),
+                              lowest index on ties.  NULL: the argmax above.  A separate pointwise kernel runs the draw */
+  const float* ss_gu;      /* optional injected uniforms [B][T][V] in (0, 1) (parity tests); NULL: u_v = ((x >> 8) + 0.5) * 2^-24 with
+                              x word (v & 3) of Philox4x32-10(counter = (0x80000000 | v >> 2, t, b, call), key = seed) of
+                              dropout_state — a first counter word neither the dropout stream nor the coin uses.  ss_temp or
+                              ss_gu without ss_prob, and ss_gu without ss_temp, are refused (LO_EINVAL) before any GPU work */
   /* inputs */
   const void* enc;         /* big [B][R][C] */
   /* parameters: weight shadows in `dt`, biases fp32.  Wcat1 = [decoder_att; f_beta; weight_hh] rows
@@ -422,6 +430,32 @@ int lo_decoder_beam(const lo_decoder_args* a, int64_t start_id, int64_t end_id, 
 int lo_decoder_beam_div(const lo_decoder_args* a, int64_t start_id, int64_t end_id, int max_steps, int64_t* ids,
                         int64_t* parents, int32_t* fin_hist, float* logp, float div_gamma, float div_prob,
                         const float* div_u, const uint64_t* div_state, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Self-critical sequence training (SCST, Rennie et al. 2017) of the decoder above: a sample pass (lo_decoder_forward with ss_prob
+ * = 1 and ss_temp), a greedy rollout (ss_prob = 1, no ss_temp) as the baseline, the reward of both against the reference
+ * (lo_scst_edit_reward), the policy gradient of the sample (lo_scst_pg_grad) into dpred_ext, and lo_decoder_backward in its
+ * generic mode with ss_prob set (teacher forcing on the sampled fed).
+ */
+/* Edit-distance reward of B rows.  h = a row's tokens truncated at the first end_id (metrics.truncate_end), the reference likewise;
+ * r(h) = 1 - lev(h, ref) / max(|h|, |ref|) (unit-cost Levenshtein), 1 when both are empty.  hyp [B][hyp_stride] (Lh tokens per row),
+ * greedy [B][greedy_stride] (Lg tokens; optional), ref [B][ref_stride] (Lr tokens), all int64.  Writes r_sample [B] and, with greedy,
+ * r_greedy [B] and adv [B] = r_sample - r_greedy (each output but r_sample optional); n_len (optional) int32 [B] = the first t >= 1
+ * with hyp[b][t] == end_id, else Lh - 1 (the steps lo_scst_pg_grad differentiates).  Distances are integers: the result is exact
+ * and deterministic.  Null hyp / ref / r_sample, B < 1 and a length outside 1..512 are refused (LO_EINVAL) before any GPU work. */
+int lo_scst_edit_reward(const int64_t* hyp, int64_t hyp_stride, int Lh, const int64_t* greedy, int64_t greedy_stride, int Lg,
+                        const int64_t* ref, int64_t ref_stride, int Lr, int B, int64_t end_id, float* r_sample, float* r_greedy,
+                        float* adv, int32_t* n_len, void* stream);
+/* Policy gradient of L = -(1/B) sum_b adv[b] sum_{t=1..n_len[b]} log softmax(preds[b][t-1] / tau)[fed[b][t]], tau = *temp (a device
+ * scalar): writes dpred[b][t-1][v] = -adv[b] / (B tau) (1[v = fed[b][t]] - softmax(preds[b][t-1] / tau)_v) for 1 <= t <= n_len[b] and
+ * 0 in every other row (b, s) of [B][T] — V columns, dpred_stride apart: the layout of lo_decoder_args.dpred_ext — and
+ * stats[4] = {L, mean r_sample, mean r_greedy, mean n_len} (r_sample / r_greedy may be NULL: 0).  preds [B][T] rows of V fp32,
+ * pred_stride apart; fed [B][fed_stride] int64 (fed_stride >= T); n_len int32 [B] in 0..T-1; partial [B][T] fp32 scratch.  The
+ * per-row partials are summed in a fixed order without atomics, so the result is bit-reproducible.  Null inputs, B, T < 1, V < 2
+ * and strides below V are refused (LO_EINVAL) before any GPU work. */
+int lo_scst_pg_grad(const float* preds, int64_t pred_stride, const int64_t* fed, int64_t fed_stride, const float* adv,
+                    const int32_t* n_len, const float* temp, const float* r_sample, const float* r_greedy, int B, int T, int V,
+                    float* dpred, int64_t dpred_stride, float* partial, float* stats, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * TensorFlow-flavour decoder (SURVEY.md §8-a row a7): the Genthial attention cell of

@@ -8,7 +8,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, os.environ.get("LO_LIB_DIR", "_C"))      # LO_LIB_DIR: build a tuning variant next to the product library
 LIB = os.path.join(OUT, "liblatex_ocr_b200.so")
-SOURCES = ["lo_gemm.cu", "lo_conv.cu", "lo_decoder.cu", "lo_attention.cu", "lo_skinny.cu", "lo_cluster.cu", "lo_optim.cu", "lo_tc.cu"]
+SOURCES = ["lo_gemm.cu", "lo_conv.cu", "lo_decoder.cu", "lo_attention.cu", "lo_skinny.cu", "lo_cluster.cu", "lo_optim.cu", "lo_tc.cu", "lo_scst.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xptxas", "-v"] + os.environ.get("LO_NVCC_EXTRA", "").split()
 

@@ -442,15 +442,33 @@ struct SsStep {
   bf16* hd_bf;                // bf16 mirror of hd (A operand of the per-step fc GEMM in bf16), NULL otherwise
 };
 
+// the categorical draw of lstm_pw_fwd_gumbel_kernel (lo_decoder_args.ss_temp)
+struct GumbelStep {
+  const float* temp;          // device scalar tau
+  const float* gu;            // injected uniforms of step t, rows gustride apart ([V] each), or NULL: Philox keyed by ss.coin_state
+  int64_t gustride;
+};
+
+// -log(u) of the Gumbel uniform u = ((x >> 8) + 0.5) * 2^-24 in (0, 1).  fp32 holds u exactly only below 1/2 (a 24-bit
+// significand); above, 1 - u is exact and goes through log1p, so u never rounds to 1 (where the Gumbel noise would be infinite).
+__device__ __forceinline__ float neg_log_u24(uint32_t x) {
+  const uint32_t m = x >> 8;
+  if (m < (1u << 23)) return -logf(((float)m + 0.5f) * (1.0f / 16777216.0f));
+  return -log1pf(-(((float)((1u << 24) - 1u - m) + 0.5f) * (1.0f / 16777216.0f)));
+}
+
 // LSTM cell pointwise (nn.LSTMCell, gate order i,f,g,o).  pre = gtmp + ptab[tok] + hh_pre.
-// SS (scheduled sampling): tok is the teacher token; the token fed is chosen here (lo_decoder_args.ss_prob) and recorded.
-template <bool SS>
-__global__ void lstm_pw_fwd_kernel(const float* __restrict__ gtmp, const float* __restrict__ ptab,
-                                   const int64_t* __restrict__ tok, int64_t tok_stride, const float* __restrict__ hh,
-                                   int64_t hh_stride, const float* __restrict__ c_prev, float* __restrict__ gates,
-                                   float* __restrict__ c_out, float* __restrict__ h_out, bf16* __restrict__ h_bf,
-                                   float* __restrict__ hd, int64_t hd_stride, const float* __restrict__ dmask, int nrows, int D,
-                                   int V, const unsigned long long* __restrict__ dstate, float dp, int row0, int t_idx, SsStep ss) {
+// MODE 0: the token is tok.  MODE 1 / 2 (scheduled sampling): tok is the teacher token; the token fed is chosen here
+// (lo_decoder_args.ss_prob) and recorded: the argmax of the previous logits (1) or a Gumbel-max draw from softmax(logits / tau) (2).
+template <int MODE>
+__device__ __forceinline__ void lstm_pw_fwd_body(const float* __restrict__ gtmp, const float* __restrict__ ptab,
+                                                 const int64_t* __restrict__ tok, int64_t tok_stride, const float* __restrict__ hh,
+                                                 int64_t hh_stride, const float* __restrict__ c_prev, float* __restrict__ gates,
+                                                 float* __restrict__ c_out, float* __restrict__ h_out, bf16* __restrict__ h_bf,
+                                                 float* __restrict__ hd, int64_t hd_stride, const float* __restrict__ dmask, int nrows,
+                                                 int D, int V, const unsigned long long* __restrict__ dstate, float dp, int row0,
+                                                 int t_idx, const SsStep& ss, const GumbelStep& gs) {
+  constexpr bool SS = MODE != 0;
   // Everything but the gates GEMM result is at least two launches old (token -> table row, the recurrent projection of this step,
   // c_t; the dropout draw depends on nothing): fetched / computed BEFORE griddepcontrol.wait, so only one L2 round trip (gtmp) is left
   // on the critical path of the time loop instead of two dependent ones.
@@ -482,9 +500,39 @@ __global__ void lstm_pw_fwd_kernel(const float* __restrict__ gtmp, const float* 
           const float* lg = ss.prev_logits + (int64_t)r * ss.lstride;
           float best = -INFINITY;
           int bi = 0;
+          if constexpr (MODE == 2) {
+            // Gumbel-max: argmax_v (lg[v] / tau + g_v), g_v = -log(-log u_v), one exact draw from softmax(lg / tau).  Each lane
+            // visits its v in increasing order and keeps the first maximum, so the reduction below keeps the lowest index.
+            const float tau = *gs.temp;
+            if (gs.gu) {
+              const float* gu = gs.gu + (int64_t)r * gs.gustride;
+              for (int v = lane; v < V; v += 32) {
+                const float x = lg[v] / tau - logf(-logf(gu[v]));
+                if (x > best) { best = x; bi = v; }
+              }
+            } else {
+              // u_v from word v & 3 of Philox4x32-10(counter = (0x80000000 | v >> 2, t, b, call)): a first counter word neither
+              // the dropout stream (j >> 2 < 2^31) nor the coin (0xFFFFFFFF) uses
+              const unsigned long long seed = ss.coin_state[0], call = ss.coin_state[1];
+              for (int v4 = lane; v4 * 4 < V; v4 += 32) {
+                const uint4 w = philox4x32_10(make_uint4(0x80000000u | (uint32_t)v4, (uint32_t)t_idx, (uint32_t)(row0 + r), (uint32_t)call),
+                                              make_uint2((uint32_t)seed, (uint32_t)(seed >> 32)));
+                const uint32_t ws[4] = {w.x, w.y, w.z, w.w};
+#pragma unroll
+                for (int q = 0; q < 4; q++) {
+                  const int v = v4 * 4 + q;
+                  if (v < V) {
+                    const float x = lg[v] / tau - logf(neg_log_u24(ws[q]));
+                    if (x > best) { best = x; bi = v; }
+                  }
+                }
+              }
+            }
+          } else {
           for (int v = lane; v < V; v += 32) {
             const float x = lg[v];
             if (x > best) { best = x; bi = v; }
+          }
           }
 #pragma unroll
           for (int o = 16; o > 0; o >>= 1) {
@@ -537,6 +585,28 @@ __global__ void lstm_pw_fwd_kernel(const float* __restrict__ gtmp, const float* 
   if constexpr (SS) {
     if (ss.hd_bf) ss.hd_bf[(int64_t)b * hd_stride + j] = __float2bfloat16_rn(h * mult);
   }
+}
+
+template <bool SS>
+__global__ void lstm_pw_fwd_kernel(const float* __restrict__ gtmp, const float* __restrict__ ptab,
+                                   const int64_t* __restrict__ tok, int64_t tok_stride, const float* __restrict__ hh,
+                                   int64_t hh_stride, const float* __restrict__ c_prev, float* __restrict__ gates,
+                                   float* __restrict__ c_out, float* __restrict__ h_out, bf16* __restrict__ h_bf,
+                                   float* __restrict__ hd, int64_t hd_stride, const float* __restrict__ dmask, int nrows, int D,
+                                   int V, const unsigned long long* __restrict__ dstate, float dp, int row0, int t_idx, SsStep ss) {
+  lstm_pw_fwd_body<SS ? 1 : 0>(gtmp, ptab, tok, tok_stride, hh, hh_stride, c_prev, gates, c_out, h_out, h_bf, hd, hd_stride, dmask,
+                               nrows, D, V, dstate, dp, row0, t_idx, ss, GumbelStep{});
+}
+// scheduled sampling with a temperature (lo_decoder_args.ss_temp): the token fed is drawn, not the argmax
+__global__ void lstm_pw_fwd_gumbel_kernel(const float* __restrict__ gtmp, const float* __restrict__ ptab,
+                                          const int64_t* __restrict__ tok, int64_t tok_stride, const float* __restrict__ hh,
+                                          int64_t hh_stride, const float* __restrict__ c_prev, float* __restrict__ gates,
+                                          float* __restrict__ c_out, float* __restrict__ h_out, bf16* __restrict__ h_bf,
+                                          float* __restrict__ hd, int64_t hd_stride, const float* __restrict__ dmask, int nrows, int D,
+                                          int V, const unsigned long long* __restrict__ dstate, float dp, int row0, int t_idx, SsStep ss,
+                                          GumbelStep gs) {
+  lstm_pw_fwd_body<2>(gtmp, ptab, tok, tok_stride, hh, hh_stride, c_prev, gates, c_out, h_out, h_bf, hd, hd_stride, dmask, nrows, D, V,
+                      dstate, dp, row0, t_idx, ss, gs);
 }
 
 // backward of the cell pointwise part: dh = dhd[b,t] + dh_next ; writes d(pre-activations), dc_prev in place
@@ -1020,6 +1090,9 @@ static int check_args(const lo_decoder_args* a) {
     LO_CHECK_ARG(a->ss_u || a->dropout_state, "scheduled sampling (ss_prob) needs ss_u or dropout_state for its coin");
     LO_CHECK_ARG(a->phase == 0, "scheduled sampling (ss_prob) needs phase 0: no per-step head when a layer sits between h and fc");
     LO_CHECK_ARG(a->rows_per_img <= 1, "scheduled sampling (ss_prob) needs rows_per_img <= 1");
+    LO_CHECK_ARG(!a->ss_gu || a->ss_temp, "ss_gu (injected Gumbel uniforms) needs ss_temp");
+  } else {
+    LO_CHECK_ARG(!a->ss_temp && !a->ss_gu, "ss_temp / ss_gu (sampling with a temperature) need ss_prob");
   }
   for (int t = 0; t < a->T; t++) {
     LO_CHECK_ARG(a->bt_host[t] >= 1 && a->bt_host[t] <= a->B, "bt_host out of range");
@@ -1266,16 +1339,24 @@ static int forward_step(const lo_decoder_args* a, const Dims& d, int t, const Ro
     ss.fed = a->fed + r0 * d.T + t;
     ss.hd_bf = bv.on ? bv.hd + r0 * hd_stride + t * d.D : nullptr;
   }
-  LO_CUDA(launch_pdl(sampling ? lstm_pw_fwd_kernel<true> : lstm_pw_fwd_kernel<false>, dim3(cdiv((long)nrows * d.D, 256)), dim3(256),
-                     (size_t)0, st, (const float*)gtmp,
-                     (const float*)a->ptab, tok + r0 * tok_stride, tok_stride, (const float*)(o1 + d.A + d.C), (int64_t)d.O1,
-                     (const float*)c_prev, a->gates + ((int64_t)t * d.B + r0) * d.G, a->call + ((int64_t)(t + 1) * d.B + r0) * d.D,
-                     a->hall + ((int64_t)(t + 1) * d.B + r0) * d.D,
-                     bv.on ? bv.hall + ((int64_t)(t + 1) * d.B + r0) * d.D : (bf16*)nullptr,
-                     hd_t ? hd_t + r0 * hd_stride : (float*)nullptr, hd_stride,
-                     dmask_t ? dmask_t + r0 * hd_stride : (const float*)nullptr, nrows, d.D, d.V,
-                     (const unsigned long long*)((hd_t && a->has_dropout == 2) ? a->dropout_state : nullptr), a->dropout_p, (int)r0, t,
-                     ss));
+  // the pointwise launch; `extra` is the GumbelStep of the sampling kernel with a temperature
+  auto launch_pw = [&](auto kernel, auto... extra) {
+    return launch_pdl(kernel, dim3(cdiv((long)nrows * d.D, 256)), dim3(256), (size_t)0, st, (const float*)gtmp,
+                      (const float*)a->ptab, tok + r0 * tok_stride, tok_stride, (const float*)(o1 + d.A + d.C), (int64_t)d.O1,
+                      (const float*)c_prev, a->gates + ((int64_t)t * d.B + r0) * d.G, a->call + ((int64_t)(t + 1) * d.B + r0) * d.D,
+                      a->hall + ((int64_t)(t + 1) * d.B + r0) * d.D,
+                      bv.on ? bv.hall + ((int64_t)(t + 1) * d.B + r0) * d.D : (bf16*)nullptr,
+                      hd_t ? hd_t + r0 * hd_stride : (float*)nullptr, hd_stride,
+                      dmask_t ? dmask_t + r0 * hd_stride : (const float*)nullptr, nrows, d.D, d.V,
+                      (const unsigned long long*)((hd_t && a->has_dropout == 2) ? a->dropout_state : nullptr), a->dropout_p, (int)r0,
+                      t, ss, extra...);
+  };
+  if (sampling && a->ss_temp) {
+    const GumbelStep gs{a->ss_temp, a->ss_gu ? a->ss_gu + (r0 * d.T + t) * d.V : nullptr, (int64_t)d.T * d.V};
+    LO_CUDA(launch_pw(lstm_pw_fwd_gumbel_kernel, gs));
+  } else {
+    LO_CUDA(launch_pw(sampling ? lstm_pw_fwd_kernel<true> : lstm_pw_fwd_kernel<false>));
+  }
   LO_LAUNCH_OK();
   if (sampling) {
     // the head of step t, right after the cell (the next step's cell reads these logits, see lstm_pw_fwd_kernel): the returned

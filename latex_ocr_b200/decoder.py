@@ -182,6 +182,10 @@ class DecoderWithAttention(nn.Module):
         self._ss_prob = None
         self.last_fed_tokens = None
         self._ss_u = None
+        # sampling with a temperature (forward(..., sampling_temperature=tau)): the device scalar tau, created on first use;
+        # injected Gumbel uniforms [B, T, V] for parity tests (None: Philox)
+        self._ss_temp = None
+        self._ss_gu = None
 
     def seed_dropout(self, seed, call=0):
         self.dropout_state.copy_(torch.tensor([int(seed) & 0x7FFFFFFFFFFFFFFF, int(call)], dtype=torch.int64))
@@ -316,7 +320,7 @@ class DecoderWithAttention(nn.Module):
         """The cached workspace of an exact shape (tests / bench probes)."""
         return self._ws[(B, T, R)]
 
-    def fill_args(self, ws, enc, B, T, R, has_dropout, dalpha_ext=None, ss_prob=None):
+    def fill_args(self, ws, enc, B, T, R, has_dropout, dalpha_ext=None, ss_prob=None, ss_temp=None):
         S, t = self.store, ws["t"]
         a = _lib.DecoderArgs()
         a.B, a.T, a.R = B, T, R
@@ -372,6 +376,10 @@ class DecoderWithAttention(nn.Module):
             a.fed = self._fed_buffer(ws).data_ptr()
             if self._ss_u is not None:
                 a.ss_u = self._ss_u.data_ptr()
+            if ss_temp is not None:                # a draw from softmax(logits / tau) instead of the argmax
+                a.ss_temp = ss_temp.data_ptr()
+                if self._ss_gu is not None:
+                    a.ss_gu = self._ss_gu.data_ptr()
         if a.impl == _lib.LO_IMPL_TC:
             if "bfwork" not in t:
                 t["bfwork"] = torch.zeros(int(_lib.lib().lo_decoder_bfwork_bytes(ctypes.byref(a))), dtype=torch.uint8, device=S.device)
@@ -413,15 +421,18 @@ class DecoderWithAttention(nn.Module):
         finally:
             a.phase = 0
 
-    def run_forward(self, enc_flat, caps_sorted, decode_lengths, with_loss, need_grad, dropout_mask=None, phase=0, ss_prob=None):
+    def run_forward(self, enc_flat, caps_sorted, decode_lengths, with_loss, need_grad, dropout_mask=None, phase=0, ss_prob=None,
+                    ss_temp=None, key=None):
         """enc_flat: storage-dtype CUDA [B,R,C] (sorted rows); caps_sorted: CUDA int64 [B,T+1].
         dropout_mask: None (no dropout), a [B,T,D] tensor of multipliers (injected, parity tests) or the string "philox"
         (mask drawn inside the kernels).  ss_prob: None (teacher forcing) or a CUDA float32 scalar p: scheduled sampling, the
-        tokens fed land in ``ws["t"]["fed"]`` (the same argument block serves the backward, run_backward)."""
+        tokens fed land in ``ws["t"]["fed"]`` (the same argument block serves the backward, run_backward).  ss_temp: None or a CUDA
+        float32 scalar tau: a step that samples feeds a draw from softmax(logits / tau).  key: the workspace cache key (default
+        (B, T, R)), so that two forwards of one shape keep separate state."""
         L = _lib.lib()
         B, R, _ = enc_flat.shape
         T = max(decode_lengths)
-        ws = self.workspace(B, T, R, need_grad)
+        ws = self.workspace(B, T, R, need_grad, key=key)
         self.store.refresh_shadow()
         ws["t"]["caps"].copy_(caps_sorted[:, :T + 1])
         self.set_lengths(ws, decode_lengths, B, T)
@@ -431,7 +442,7 @@ class DecoderWithAttention(nn.Module):
                 ws["t"]["dropout_mask"] = torch.zeros(B, T, self.decoder_dim, dtype=torch.float32, device=self.store.device)
                 ws.pop("args", None)
             ws["t"]["dropout_mask"].copy_(dropout_mask)
-        a = self.fill_args(ws, enc_flat, B, T, R, has_do, ss_prob=ss_prob)
+        a = self.fill_args(ws, enc_flat, B, T, R, has_do, ss_prob=ss_prob, ss_temp=ss_temp)
         a.phase = int(phase)
         try:
             check(L.lo_decoder_forward(ctypes.byref(a), 1 if with_loss else 0, stream_ptr()))
@@ -455,7 +466,7 @@ class DecoderWithAttention(nn.Module):
         keep = torch.rand(B, T, self.decoder_dim, device=self.store.device) >= p
         return keep.float() / (1.0 - p)
 
-    def forward(self, encoder_out, encoded_captions, caption_lengths, sampling_prob=0.0):
+    def forward(self, encoder_out, encoded_captions, caption_lengths, sampling_prob=0.0, sampling_temperature=0.0):
         """Reference signature and return tuple (seq2seq_torch.py:267-320): (predictions[B,maxT,V],
         sorted captions, decode_lengths(list), alphas[B,maxT,R], sort_ind).  With grad mode on and ``encoder_out`` or a
         parameter requiring grad, an autograd graph is recorded: ``predictions`` and ``alphas`` are differentiable (any loss of
@@ -467,15 +478,27 @@ class DecoderWithAttention(nn.Module):
         dropout seed (one call counter per forward, also in eval mode; ``seed_dropout`` reproduces them).  Targets of a loss stay
         ``captions[:, 1:]``; the choice is not differentiated: the backward is teacher forcing on the tokens fed, which
         ``last_fed_tokens`` holds ([B, T] in sorted-row order, the teacher token past a row's length).  p = 0 runs the teacher-forced
-        path unchanged (``last_fed_tokens`` is then ``captions[:, :T]``)."""
+        path unchanged (``last_fed_tokens`` is then ``captions[:, :T]``).
+
+        ``sampling_temperature`` = tau > 0 (with p > 0): a step that samples feeds a draw from softmax(prediction / tau) (Gumbel-max,
+        the uniforms from the same Philox call: ``philox.gumbel_uniforms``) instead of the argmax.  With p = 1 the call samples a
+        whole sequence, and the outputs stay differentiable: log pi(sample) is a function of ``predictions`` and the tokens in
+        ``last_fed_tokens``, so a policy-gradient loss (self-critical training, ``scst``) works through ``loss.backward()``.  0 (the
+        default) is the argmax path, bit for bit."""
         (preds, alphas), (caps, decode_lengths, sort_ind) = kernel_forward(
-            self, (encoder_out, encoded_captions, caption_lengths, float(sampling_prob)), (encoder_out,))
+            self, (encoder_out, encoded_captions, caption_lengths, float(sampling_prob), float(sampling_temperature or 0.0)),
+            (encoder_out,))
         return preds, caps, decode_lengths, alphas, sort_ind
 
-    def _forward_impl(self, encoder_out, encoded_captions, caption_lengths, sampling_prob=0.0, need_grad=False):
+    def _forward_impl(self, encoder_out, encoded_captions, caption_lengths, sampling_prob=0.0, sampling_temperature=0.0,
+                      need_grad=False):
         """((predictions, alphas), (captions, decode_lengths, sort_ind), what the backward of this call needs or None)."""
         if not 0.0 <= sampling_prob <= 1.0:
             raise ValueError("sampling_prob must lie in [0, 1] (got %r)" % (sampling_prob,))
+        if not (sampling_temperature >= 0.0 and math.isfinite(sampling_temperature)):
+            raise ValueError("sampling_temperature must be a finite tau >= 0 (got %r)" % (sampling_temperature,))
+        if sampling_temperature > 0.0 and sampling_prob == 0.0:
+            raise ValueError("sampling_temperature needs sampling_prob > 0: it sets how the fed tokens are drawn")
         enc, caps, decode_lengths, sort_ind = self._sorted_inputs(encoder_out, encoded_captions, caption_lengths)
         T = max(decode_lengths)
         mask = self.make_dropout_mask(enc.shape[0], T)
@@ -485,7 +508,14 @@ class DecoderWithAttention(nn.Module):
                 self._ss_prob = torch.zeros((), dtype=torch.float32, device=self.store.device)
             ss = self._ss_prob
             ss.fill_(sampling_prob)
-        ws = self.run_forward(enc, caps, decode_lengths, with_loss=False, need_grad=need_grad, dropout_mask=mask, ss_prob=ss)
+        tau = None
+        if sampling_temperature > 0.0:
+            if self._ss_temp is None:
+                self._ss_temp = torch.zeros((), dtype=torch.float32, device=self.store.device)
+            tau = self._ss_temp
+            tau.fill_(sampling_temperature)
+        ws = self.run_forward(enc, caps, decode_lengths, with_loss=False, need_grad=need_grad, dropout_mask=mask, ss_prob=ss,
+                              ss_temp=tau)
         self.last_fed_tokens = ws["t"]["fed"].clone() if ss is not None else caps[:, :T]
         return self._outputs(ws, encoder_out, enc, caps, decode_lengths, sort_ind, mask, need_grad, sampling=ss is not None)
 

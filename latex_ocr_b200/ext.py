@@ -302,6 +302,11 @@ class Img2SeqRowModel(Img2SeqModel):
     def set_sampling_prob(self, p):
         _refuse_sampling(float(p))
 
+    def set_self_critical(self, temperature):
+        if temperature:
+            raise _lib.LatexOcrB200Error("self-critical training is not available with the second decoder layer: it samples inside "
+                                         "layer 1's time loop, which has no per-step prediction (see scheduled sampling)")
+
     def _keepalive(self):
         keep = super()._keepalive()
         keep += [list(self.row_encoder._out.values()), list(self.layer2._x.values()), list(self.layer2.dir._ws.values())]

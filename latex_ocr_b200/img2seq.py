@@ -8,6 +8,7 @@ decoder then the encoder (:162-170), returns ``-loss`` (:172).  The ``lr`` and `
 are ignored exactly like the reference ignores them (SURVEY.md quirk Q3).
 """
 import ctypes
+import math
 import os
 import time
 
@@ -44,6 +45,10 @@ class Img2SeqModel:
         self.sampling_prob = 0.0
         self._ss_prob_dev = None
         self.set_sampling_prob(getattr(config, "sampling_prob", 0.0) or 0.0)
+        # self-critical training in the fused step: tau (host copy; 0 = cross-entropy) and the device scalars the kernels read
+        self.scst_temperature = 0.0
+        self._scst_temp_dev = None
+        self._scst_one = None
 
     # --- model/base_torch.py:45-71 -------------------------------------------------------------
     def build_train(self, config=None):
@@ -88,11 +93,38 @@ class Img2SeqModel:
         p = float(p)
         if not 0.0 <= p <= 1.0:
             raise ValueError("sampling_prob must lie in [0, 1] (got %r)" % (p,))
+        if p > 0.0 and getattr(self, "scst_temperature", 0.0) > 0.0:
+            raise _lib.LatexOcrB200Error("scheduled sampling and self-critical training exclude each other: call "
+                                         "set_self_critical(None) first")
         self.sampling_prob = p
         if p > 0.0:
             if self._ss_prob_dev is None:
                 self._ss_prob_dev = torch.zeros((), dtype=torch.float32, device=self.device)
             self._ss_prob_dev.fill_(p)
+
+    def set_self_critical(self, temperature):
+        """Self-critical sequence training (SCST; Rennie et al. 2017) in the fused train step.  ``temperature`` = tau > 0: from the
+        next step on, ``train_step`` / ``getLoss`` / ``_run_train_epoch`` / ``train`` sample one formula per image from
+        softmax(logits / tau) inside the CUDA time loop, score it and a greedy rollout (the baseline) with the edit-distance reward of
+        ``scst.edit_reward`` against the reference, and minimise L = -(1/B) sum_b (r_sample - r_greedy)_b log pi(sample_b).  The
+        attention regulariser is not part of this objective.  ``train_step`` then returns the device vector [L, mean r_sample,
+        mean r_greedy, mean sampled length] and ``getLoss`` -L; ``decoder.last_fed_tokens`` holds the samples ([B, L-1], the first
+        token is the caption's).  tau is a device scalar, so a captured step graph picks up a new tau without re-capture.  ``None``
+        or 0: back to cross-entropy.  Refused together with scheduled sampling and with data parallelism (``dist``)."""
+        tau = 0.0 if temperature is None else float(temperature)
+        if not (tau >= 0.0 and math.isfinite(tau)):
+            raise ValueError("temperature must be a finite tau > 0, or None / 0 for cross-entropy (got %r)" % (temperature,))
+        if tau > 0.0:
+            if self.sampling_prob > 0.0:
+                raise _lib.LatexOcrB200Error("self-critical training and scheduled sampling exclude each other: call "
+                                             "set_sampling_prob(0) first")
+            if self.dist is not None:
+                raise _lib.LatexOcrB200Error("self-critical training is not available with data parallelism (dist)")
+            if self._scst_temp_dev is None:
+                self._scst_temp_dev = torch.zeros((), dtype=torch.float32, device=self.device)
+                self._scst_one = torch.ones((), dtype=torch.float32, device=self.device)
+            self._scst_temp_dev.fill_(tau)
+        self.scst_temperature = tau
 
     def train_mode(self, flag=True):
         self.encoder.train(flag)
@@ -134,6 +166,8 @@ class Img2SeqModel:
     def _step_body(self, img, caps, decode_lengths, dropout_mask):
         """encoder fwd -> decoder fwd + loss -> decoder bwd -> encoder bwd -> (grad all-reduce) -> Adam x2.
         img: CUDA fp32 [N,1,H,W]; caps: CUDA int64 [N,L] sorted rows.  Returns the device loss vector."""
+        if self.scst_temperature > 0.0:
+            return self._scst_step_body(img, caps, decode_lengths, dropout_mask)
         N = img.shape[0]
         enc_out = self.encoder.forward_raw(img, need_grad=True)
         R = enc_out.shape[1] * enc_out.shape[2]
@@ -159,6 +193,49 @@ class Img2SeqModel:
         self._adam(self.encoder.store, scale, self.encoder)
         return ws["t"]["loss"]
 
+    def _scst_step_body(self, img, caps, decode_lengths, dropout_mask):
+        """The self-critical step (set_self_critical): encoder fwd -> sample pass (p = 1, tau, train-mode dropout) -> greedy rollout
+        (p = 1, no dropout, its own workspace) -> rewards -> policy gradient -> generic decoder bwd (teacher forcing on the sample)
+        -> encoder bwd -> Adam x2.  Returns the device vector [L, mean r_sample, mean r_greedy, mean n_b]."""
+        from . import scst
+        dec = self.decoder
+        N, V = img.shape[0], dec.vocab_size
+        enc_out = self.encoder.forward_raw(img, need_grad=True)
+        R = enc_out.shape[1] * enc_out.shape[2]
+        enc_flat = enc_out.view(N, R, enc_out.shape[3])
+        T = max(decode_lengths)
+        ws = dec.run_forward(enc_flat, caps, decode_lengths, with_loss=False, need_grad=True, dropout_mask=dropout_mask,
+                             ss_prob=self._scst_one, ss_temp=self._scst_temp_dev)
+        gw = dec.run_forward(enc_flat, caps, decode_lengths, with_loss=False, need_grad=False, ss_prob=self._scst_one,
+                             key=("scst_rollout", N, T, R))
+        t = ws["t"]
+        if t.get("scst_dpred") is None:
+            f32 = dict(dtype=torch.float32, device=self.device)
+            t["scst_dpred"] = torch.zeros(N, T, V, **f32)
+            t["scst_partial"] = torch.zeros(N, T, **f32)
+            t["scst_stats"] = torch.zeros(4, **f32)
+            t["scst_r"] = (torch.zeros(N, **f32), torch.zeros(N, **f32), torch.zeros(N, **f32),
+                           torch.zeros(N, dtype=torch.int32, device=self.device))
+        fed = t["fed"]
+        dec.last_fed_tokens = fed
+        r_s, r_g, adv, n_len = scst.rewards(fed, caps, self._end_id(), greedy=gw["t"]["fed"], out=t["scst_r"])
+        scst.pg_grad(t["logits"], ws["ldl"], fed, adv, n_len, self._scst_temp_dev, N, T, V, t["scst_dpred"], t["scst_partial"],
+                     t["scst_stats"], r_sample=r_s, r_greedy=r_g)
+        has_do = 0 if dropout_mask is None else (2 if isinstance(dropout_mask, str) else 1)
+        a = dec.fill_args(ws, enc_flat, N, T, R, has_do, ss_prob=self._scst_one)
+        a.dpred_ext = t["scst_dpred"].data_ptr()       # generic mode: teacher forcing on the sampled tokens
+        a.dpred_stride = V
+        dec.run_backward(ws)
+        denc = t["denc"].view(N, enc_out.shape[1], enc_out.shape[2], enc_out.shape[3])
+        self.encoder.backward_raw(tuple(img.shape), denc)
+        self._adam(self.decoder.store, 1.0, self.decoder)
+        self._adam(self.encoder.store, 1.0, self.encoder)
+        return t["scst_stats"]
+
+    def _end_id(self):
+        """The END id: the vocabulary's, else the last id (the default of the decode entry points)."""
+        return self._vocab.id_end if self._vocab is not None else self._n_tok - 1
+
     def _keepalive(self):
         """Everything a captured graph replays on (the bounded workspace caches may evict their entries later)."""
         return [list(self.decoder._ws.values()), list(self.encoder._ws.values())]
@@ -173,8 +250,11 @@ class Img2SeqModel:
 
     def train_step(self, img, formula, sync=False):
         """img: float tensor [N,1,H,W] (CPU pinned or CUDA); formula: int64 [N,L] (CPU or CUDA).
-        Returns the device loss vector [total, ce, reg, n_valid] (no host sync unless sync=True)."""
+        Returns the device loss vector [total, ce, reg, n_valid], or [L, mean r_sample, mean r_greedy, mean n_b] in self-critical
+        mode (set_self_critical); no host sync unless sync=True."""
         N, L = formula.shape
+        if self.scst_temperature > 0.0 and self.dist is not None:
+            raise _lib.LatexOcrB200Error("self-critical training is not available with data parallelism (dist)")
         # the step writes the flat gradient buffers; autograd use or zero_grad(set_to_none=True) may have re-pointed p.grad
         for m_ in self._param_modules():
             bind_grads(m_, m_.store)
@@ -198,7 +278,8 @@ class Img2SeqModel:
 
     def _graph_step(self, img_d, caps_d, decode_lengths):
         frozen = tuple(p_._lo_store_name for m_ in (self.encoder, self.decoder) for p_ in m_.parameters() if not p_.requires_grad)
-        key = (tuple(img_d.shape), img_d.dtype, tuple(caps_d.shape), self.decoder.training, frozen, self.sampling_prob > 0.0)
+        key = (tuple(img_d.shape), img_d.dtype, tuple(caps_d.shape), self.decoder.training, frozen, self.sampling_prob > 0.0,
+               self.scst_temperature > 0.0)
         g = self._graphs.get(key)
         if g is None:
             N, T = caps_d.shape[0], caps_d.shape[1] - 1
@@ -298,7 +379,7 @@ class Img2SeqModel:
         reshapes of img2seq.py:236-241 / :265-268."""
         from . import decode
         decoding = decoding or getattr(self._config, "decoding", "greedy")
-        end_id = self._vocab.id_end if self._vocab is not None else self._n_tok - 1
+        end_id = self._end_id()
         start_id = end_id - 1 if start_id is None else start_id          # default: the PAD id (no START in the torch flavour)
         L = int(getattr(self._config, "max_length_formula", 150))
         self.train_mode(False)

@@ -8,6 +8,12 @@ dropout masks and beam-search diversity draws, and documenting the stream layout
   scheduled-sampling coin of (row b, step t) under the same {seed s, call n} (lo_decoder_args.ss_prob without ss_u):
       u = (philox4x32_10(counter = (0xFFFFFFFF, t, b, n), key = (s & 0xffffffff, s >> 32))[0] >> 8) * 2**-24
   a first counter word the dropout stream (j >> 2 < D / 4) never reaches; the model's own argmax is fed where u < p
+
+  Gumbel uniform of (row b, step t, token v) under the same {seed s, call n} (lo_decoder_args.ss_temp without ss_gu):
+      words = philox4x32_10(counter = (0x80000000 | (v >> 2), t, b, n), key = (s & 0xffffffff, s >> 32));
+      u = ((words[v & 3] >> 8) + 0.5) * 2**-24                     in (0, 1), never 0 or 1
+  the first counter word is >= 2**31, which neither the dropout stream (j >> 2 < 2**31) nor the coin (0xFFFFFFFF) uses; a step that
+  samples feeds argmax_v (logits[v] / tau - log(-log u_v)), one draw from softmax(logits / tau)
 """
 import numpy as np
 
@@ -51,3 +57,15 @@ def sampling_uniforms(seed, call, B, T):
     w = philox4x32_10(np.uint64(0xFFFFFFFF) + 0 * b + 0 * t, t + 0 * b, b + 0 * t, np.uint64(call), seed & 0xFFFFFFFF,
                       (seed >> 32) & 0xFFFFFFFF)
     return u01(w[0]).reshape(B, T)
+
+
+def gumbel_uniforms(seed, call, B, T, V):
+    """[B, T, V] float64 uniforms exactly as lstm_pw_fwd_gumbel_kernel draws them (row b, step t, token v); float64 holds every
+    value exactly (25 significant bits)."""
+    b = np.arange(B, dtype=np.uint64)[:, None, None]
+    t = np.arange(T, dtype=np.uint64)[None, :, None]
+    v4 = np.arange((V + 3) // 4, dtype=np.uint64)[None, None, :]
+    w = philox4x32_10(np.uint64(0x80000000) | (v4 + 0 * b + 0 * t), t + 0 * b + 0 * v4, b + 0 * t + 0 * v4, np.uint64(call),
+                      seed & 0xFFFFFFFF, (seed >> 32) & 0xFFFFFFFF)
+    x = np.stack(w, axis=-1).reshape(B, T, -1)[:, :, :V]
+    return ((x >> np.uint64(8)).astype(np.float64) + 0.5) * 2.0 ** -24

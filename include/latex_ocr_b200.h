@@ -456,6 +456,21 @@ int lo_scst_edit_reward(const int64_t* hyp, int64_t hyp_stride, int Lh, const in
 int lo_scst_pg_grad(const float* preds, int64_t pred_stride, const int64_t* fed, int64_t fed_stride, const float* adv,
                     const int32_t* n_len, const float* temp, const float* r_sample, const float* r_greedy, int B, int T, int V,
                     float* dpred, int64_t dpred_stride, float* partial, float* stats, void* stream);
+/* The two calls above in the layout of the TensorFlow-flavour decoder (lo_tfdec_args.ss_prob, below), where every step predicts
+ * and nothing is given: the sample is hyp[b][0..Lh) = fed[b][0..T) and every token of it was drawn.
+ * lo_scst_edit_reward_tf: lo_scst_edit_reward with n_len[b] = min(e + 1, Lh), e the first t >= 0 with hyp[b][t] == end_id, else
+ * Lh (so n_len = 1 when the sample starts with END, Lh when it has none).  Same arguments, refusals and exactness.
+ * lo_scst_pg_grad_tf: lo_scst_pg_grad for L = -(1/B) sum_b adv[b] sum_{t=0..n_len[b]-1} log softmax(logits[t][b] / tau)[fed[b][t]]
+ * over the time-major logits [T][B] of lo_tfdec_args.logits (rows of V fp32, ldl apart: row (t, b) at (t B + b) ldl).  dpred is
+ * batch-major, the layout of lo_tfdec_args.dlogits_ext: dpred[b][t][v] = -adv[b] / (B tau) (1[v = fed[b][t]] - softmax(logits[t][b]
+ * / tau)_v) for t < n_len[b], 0 in every other row (b, t); n_len in 0..T.  stats, partial and the refusals as lo_scst_pg_grad,
+ * with ldl in place of pred_stride. */
+int lo_scst_edit_reward_tf(const int64_t* hyp, int64_t hyp_stride, int Lh, const int64_t* greedy, int64_t greedy_stride, int Lg,
+                           const int64_t* ref, int64_t ref_stride, int Lr, int B, int64_t end_id, float* r_sample, float* r_greedy,
+                           float* adv, int32_t* n_len, void* stream);
+int lo_scst_pg_grad_tf(const float* logits, int64_t ldl, const int64_t* fed, int64_t fed_stride, const float* adv,
+                       const int32_t* n_len, const float* temp, const float* r_sample, const float* r_greedy, int B, int T, int V,
+                       float* dpred, int64_t dpred_stride, float* partial, float* stats, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * TensorFlow-flavour decoder (SURVEY.md §8-a row a7): the Genthial attention cell of
@@ -505,6 +520,30 @@ typedef struct lo_tfdec_args {
                               instead of enc + att1 (60.5 MB instead of 114 MB per step at cfg #2).  NULL: att1 is re-read. */
   float* loss;             /* [4]: mean CE over valid tokens (x2), 0, n_words — ce_words (img2seq.py:74) = loss[0] * loss[3] */
   float* denc;             /* f32 [B][R][C] gradient w.r.t. the encoder output */
+  /* scheduled sampling (Bengio et al. 2015) and self-critical training (lo_scst_*_tf), as lo_decoder_args.ss_prob in the TF layout:
+   * every step predicts and step t consumes token t-1 (the start token at t = 0).  ss_prob != NULL selects the mode; it must then
+   * be set in BOTH the forward and the backward call.  The forward writes, for t = 0 .. T-1,
+   *     fed[b][t] = choice(logits[t][b])   if u[b][t] < p
+   *               = formula[b][t]          otherwise ;       step t+1 consumes fed[b][t]
+   * where logits[t][b] is the returned row (o_t y_W_o with this call's keep_o), p = *ss_prob and choice the lowest-index argmax
+   * (argmax_kernel's rule) or, with ss_temp, the Gumbel-max draw below.  fed[b][T-1] is recorded but consumed by no step.  The
+   * choice is not differentiated: given fed, forward and backward are teacher forcing on fed (the backward scatters the gradient of
+   * the embedding rows and of lstm.kernel's embedding part by fed, not formula); the CE targets stay formula[b][t].  In this mode
+   * the head runs inside the time loop (one GEMM of B rows per step) instead of once after it.  Refused (LO_EINVAL) before any GPU
+   * work: ss_prob without fed, without ss_u and ss_state, with rows_per_img > 1; ss_temp or ss_gu without ss_prob; ss_gu without
+   * ss_temp; any of these six fields on lo_tfdec_greedy / lo_tfdec_beam[_div]. */
+  int64_t* fed;            /* [B][T] tokens chosen at each step (layout of formula, stride T): written by the forward, read by the
+                              backward */
+  const float* ss_prob;    /* DEVICE scalar p, read inside the kernels; NULL: teacher forcing */
+  const float* ss_u;       /* optional injected coins [B][T] (parity tests); NULL: u = (x >> 8) * 2^-24 with x the first word of
+                              Philox4x32-10(counter = (0xFFFFFFFF, t, b, call), key = seed) of ss_state {seed, call} — the coin
+                              stream of lo_decoder_args.ss_u */
+  const float* ss_temp;    /* optional DEVICE scalar tau > 0: a step that samples feeds argmax_v (logits[t][b][v] / tau + g_v),
+                              g_v = -log(-log u_v) (Gumbel-max: one draw from softmax(logits / tau)), lowest index on ties */
+  const float* ss_gu;      /* optional injected uniforms [B][T][V] in (0, 1) (parity tests); NULL: u_v = ((x >> 8) + 0.5) * 2^-24 with
+                              x word (v & 3) of Philox4x32-10(counter = (0x80000000 | v >> 2, t, b, call), key = seed) of ss_state */
+  const uint64_t* ss_state; /* DEVICE {seed, call} keying the Philox coins and Gumbel uniforms (the TF flavour has no in-kernel
+                              dropout state to borrow).  Read only: the caller advances call between sampling forwards */
   /* decode of images of different sizes (lo_tfdec_greedy and lo_tfdec_beam[_div] only), as lo_decoder_args.reg_off: prefix offsets
    * of the images' regions, [B / rows_per_img + 1] each, the same values on the device and on the host.  Image i owns regions
    * [reg_off[i], reg_off[i+1]) of a PACKED enc [reg_off[n]][C] (n = B / rows_per_img; beam rows share their image's regions).  R is
@@ -522,7 +561,8 @@ typedef struct lo_tfdec_args {
 
 int64_t lo_sizeof_tfdec_args(void);
 int64_t lo_tfdec_workspace_bytes(const lo_tfdec_args* a);
-/* all T steps + logits; with_loss: masked CE into loss[] (and d logits kept for the backward) */
+/* all T steps + logits; with_loss: masked CE into loss[] (and d logits kept for the backward).  With ss_prob: the tokens consumed
+ * are chosen in the loop and recorded in fed (lo_tfdec_args, above) */
 int lo_tfdec_forward(const lo_tfdec_args* a, int with_loss, void* stream);
 /* backward of loss[0]: fills every g_* and denc (requires lo_tfdec_forward(with_loss=1) state in ws).
  * Generic mode (dlogits_ext != NULL): the backward of an arbitrary loss of the train logits and the alphas (the autograd path of
@@ -535,6 +575,7 @@ int lo_tfdec_forward(const lo_tfdec_args* a, int with_loss, void* stream);
  *     the preceding launch (programmatic dependent launch): dalpha_ext must be complete before the call, which stream order gives
  *     for anything enqueued before it;
  *   - loss is not touched.
+ * With ss_prob set (both modes) the backward is teacher forcing on fed: the token-table gradient is scattered by fed, not formula.
  * dalpha_ext without dlogits_ext and dlogits_stride < V are refused (LO_EINVAL) before any GPU work. */
 int lo_tfdec_backward(const lo_tfdec_args* a, void* stream);
 /* greedy decode (greedy_decoder_cell.py:38-66 + dynamic_decode.py:38-61): tokens [B][max_steps], fin_hist (optional)

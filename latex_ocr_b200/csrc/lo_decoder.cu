@@ -457,9 +457,90 @@ __device__ __forceinline__ float neg_log_u24(uint32_t x) {
   return -log1pf(-(((float)((1u << 24) - 1u - m) + 0.5f) * (1.0f / 16777216.0f)));
 }
 
+// Scheduled sampling (lo_decoder_args.ss_prob, lo_tfdec_args.ss_prob), shared by the pointwise LSTM kernels of both decoder
+// flavours: the token each row of a 256-thread block of a [nrows][D] launch feeds at this step, chosen and recorded once per row by
+// one warp and handed to the row's threads through shared memory.  tok: the teacher tokens (rows tok_stride apart).  Where the coin
+// (injected ss.u, else Philox counter (0xFFFFFFFF, t_idx, row0 + r, call)) is below p, the row feeds the lowest-index argmax of
+// its ss.prev_logits row (MODE 1) or a Gumbel-max draw from softmax(logits / tau) (MODE 2); ss.prev_logits NULL: the teacher
+// token.  Every thread of the block must call it (it synchronises the block); tk_ss receives the token of the thread's row b when
+// `live`.
+template <int MODE>
+__device__ __forceinline__ void ss_block_tokens(const int64_t* __restrict__ tok, int64_t tok_stride, int nrows, int D, int V, int row0,
+                                                int t_idx, const SsStep& ss, const GumbelStep& gs, bool live, int b, int64_t& tk_ss) {
+  __shared__ int64_t s_tok[256 / 8 + 2];            // rows a 256-thread block touches: <= 256 / D + 1, D % 8 == 0
+  const int first = (int)(blockIdx.x * blockDim.x) / D;
+  const int last = min(nrows - 1, (int)(blockIdx.x * blockDim.x + blockDim.x - 1) / D);
+  const int lane = threadIdx.x & 31;
+  for (int r = first + (int)(threadIdx.x >> 5); r <= last; r += (int)(blockDim.x >> 5)) {
+    int64_t pick = tok[(int64_t)r * tok_stride];
+    if (ss.prev_logits) {
+      float u;
+      if (ss.u) u = ss.u[(int64_t)r * ss.ustride];
+      else {
+        const unsigned long long seed = ss.coin_state[0], call = ss.coin_state[1];
+        u = u01(philox4x32_10(make_uint4(0xFFFFFFFFu, (uint32_t)t_idx, (uint32_t)(row0 + r), (uint32_t)call),
+                              make_uint2((uint32_t)seed, (uint32_t)(seed >> 32))).x);
+      }
+      if (u < *ss.prob) {                           // warp-uniform
+        const float* lg = ss.prev_logits + (int64_t)r * ss.lstride;
+        float best = -INFINITY;
+        int bi = 0;
+        if constexpr (MODE == 2) {
+          // Gumbel-max: argmax_v (lg[v] / tau + g_v), g_v = -log(-log u_v), one exact draw from softmax(lg / tau).  Each lane
+          // visits its v in increasing order and keeps the first maximum, so the reduction below keeps the lowest index.
+          const float tau = *gs.temp;
+          if (gs.gu) {
+            const float* gu = gs.gu + (int64_t)r * gs.gustride;
+            for (int v = lane; v < V; v += 32) {
+              const float x = lg[v] / tau - logf(-logf(gu[v]));
+              if (x > best) { best = x; bi = v; }
+            }
+          } else {
+            // u_v from word v & 3 of Philox4x32-10(counter = (0x80000000 | v >> 2, t, b, call)): a first counter word neither
+            // the dropout stream (j >> 2 < 2^31) nor the coin (0xFFFFFFFF) uses
+            const unsigned long long seed = ss.coin_state[0], call = ss.coin_state[1];
+            for (int v4 = lane; v4 * 4 < V; v4 += 32) {
+              const uint4 w = philox4x32_10(make_uint4(0x80000000u | (uint32_t)v4, (uint32_t)t_idx, (uint32_t)(row0 + r), (uint32_t)call),
+                                            make_uint2((uint32_t)seed, (uint32_t)(seed >> 32)));
+              const uint32_t ws[4] = {w.x, w.y, w.z, w.w};
+#pragma unroll
+              for (int q = 0; q < 4; q++) {
+                const int v = v4 * 4 + q;
+                if (v < V) {
+                  const float x = lg[v] / tau - logf(neg_log_u24(ws[q]));
+                  if (x > best) { best = x; bi = v; }
+                }
+              }
+            }
+          }
+        } else {
+        for (int v = lane; v < V; v += 32) {
+          const float x = lg[v];
+          if (x > best) { best = x; bi = v; }
+        }
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+          const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+          const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+          if (ob > best || (ob == best && oi < bi)) { best = ob; bi = oi; }   // the rule of argmax_kernel (greedy decode)
+        }
+        pick = bi;
+      }
+    }
+    if (lane == 0) {
+      s_tok[r - first] = pick;
+      if ((int64_t)r * D >= (int64_t)blockIdx.x * blockDim.x) ss.fed[(int64_t)r * ss.ustride] = pick;   // the block holding j = 0
+    }
+  }
+  __syncthreads();
+  if (live) tk_ss = s_tok[b - first];
+}
+
 // LSTM cell pointwise (nn.LSTMCell, gate order i,f,g,o).  pre = gtmp + ptab[tok] + hh_pre.
 // MODE 0: the token is tok.  MODE 1 / 2 (scheduled sampling): tok is the teacher token; the token fed is chosen here
-// (lo_decoder_args.ss_prob) and recorded: the argmax of the previous logits (1) or a Gumbel-max draw from softmax(logits / tau) (2).
+// (lo_decoder_args.ss_prob, ss_block_tokens) and recorded: the argmax of the previous logits (1) or a Gumbel-max draw from
+// softmax(logits / tau) (2).
 template <int MODE>
 __device__ __forceinline__ void lstm_pw_fwd_body(const float* __restrict__ gtmp, const float* __restrict__ ptab,
                                                  const int64_t* __restrict__ tok, int64_t tok_stride, const float* __restrict__ hh,
@@ -477,80 +558,10 @@ __device__ __forceinline__ void lstm_pw_fwd_body(const float* __restrict__ gtmp,
   const int b = live ? idx / D : 0, j = live ? idx % D : 0;
   float a4[4] = {0.f, 0.f, 0.f, 0.f}, cp = 0.f, mult = 1.f;
   int64_t tk_ss = 0;
-  if constexpr (SS) {
-    // The logits of step t-1 come from the fc GEMM launched right after lstm_pw_fwd_kernel(t-1); the o1 GEMM, the attention and
-    // the gates GEMM of step t come in between, so they are three launches old and safe to read before griddepcontrol.wait (as
-    // the teacher token is).  The forward keeps that launch order.  One warp per row of the block: coin, then (only when it
-    // says "sample") the lowest-index argmax of the row's V logits.
-    __shared__ int64_t s_tok[256 / 8 + 2];            // rows a 256-thread block touches: <= 256 / D + 1, D % 8 == 0
-    const int first = (int)(blockIdx.x * blockDim.x) / D;
-    const int last = min(nrows - 1, (int)(blockIdx.x * blockDim.x + blockDim.x - 1) / D);
-    const int lane = threadIdx.x & 31;
-    for (int r = first + (int)(threadIdx.x >> 5); r <= last; r += (int)(blockDim.x >> 5)) {
-      int64_t pick = tok[(int64_t)r * tok_stride];
-      if (ss.prev_logits) {
-        float u;
-        if (ss.u) u = ss.u[(int64_t)r * ss.ustride];
-        else {
-          const unsigned long long seed = ss.coin_state[0], call = ss.coin_state[1];
-          u = u01(philox4x32_10(make_uint4(0xFFFFFFFFu, (uint32_t)t_idx, (uint32_t)(row0 + r), (uint32_t)call),
-                                make_uint2((uint32_t)seed, (uint32_t)(seed >> 32))).x);
-        }
-        if (u < *ss.prob) {                           // warp-uniform
-          const float* lg = ss.prev_logits + (int64_t)r * ss.lstride;
-          float best = -INFINITY;
-          int bi = 0;
-          if constexpr (MODE == 2) {
-            // Gumbel-max: argmax_v (lg[v] / tau + g_v), g_v = -log(-log u_v), one exact draw from softmax(lg / tau).  Each lane
-            // visits its v in increasing order and keeps the first maximum, so the reduction below keeps the lowest index.
-            const float tau = *gs.temp;
-            if (gs.gu) {
-              const float* gu = gs.gu + (int64_t)r * gs.gustride;
-              for (int v = lane; v < V; v += 32) {
-                const float x = lg[v] / tau - logf(-logf(gu[v]));
-                if (x > best) { best = x; bi = v; }
-              }
-            } else {
-              // u_v from word v & 3 of Philox4x32-10(counter = (0x80000000 | v >> 2, t, b, call)): a first counter word neither
-              // the dropout stream (j >> 2 < 2^31) nor the coin (0xFFFFFFFF) uses
-              const unsigned long long seed = ss.coin_state[0], call = ss.coin_state[1];
-              for (int v4 = lane; v4 * 4 < V; v4 += 32) {
-                const uint4 w = philox4x32_10(make_uint4(0x80000000u | (uint32_t)v4, (uint32_t)t_idx, (uint32_t)(row0 + r), (uint32_t)call),
-                                              make_uint2((uint32_t)seed, (uint32_t)(seed >> 32)));
-                const uint32_t ws[4] = {w.x, w.y, w.z, w.w};
-#pragma unroll
-                for (int q = 0; q < 4; q++) {
-                  const int v = v4 * 4 + q;
-                  if (v < V) {
-                    const float x = lg[v] / tau - logf(neg_log_u24(ws[q]));
-                    if (x > best) { best = x; bi = v; }
-                  }
-                }
-              }
-            }
-          } else {
-          for (int v = lane; v < V; v += 32) {
-            const float x = lg[v];
-            if (x > best) { best = x; bi = v; }
-          }
-          }
-#pragma unroll
-          for (int o = 16; o > 0; o >>= 1) {
-            const float ob = __shfl_xor_sync(0xffffffffu, best, o);
-            const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-            if (ob > best || (ob == best && oi < bi)) { best = ob; bi = oi; }   // the rule of argmax_kernel (greedy decode)
-          }
-          pick = bi;
-        }
-      }
-      if (lane == 0) {
-        s_tok[r - first] = pick;
-        if ((int64_t)r * D >= (int64_t)blockIdx.x * blockDim.x) ss.fed[(int64_t)r * ss.ustride] = pick;   // the block holding j = 0
-      }
-    }
-    __syncthreads();
-    if (live) tk_ss = s_tok[b - first];
-  }
+  // The logits of step t-1 come from the fc GEMM launched right after lstm_pw_fwd_kernel(t-1); the o1 GEMM, the attention and
+  // the gates GEMM of step t come in between, so they are three launches old and safe to read before griddepcontrol.wait (as
+  // the teacher token is).  The forward keeps that launch order.
+  if constexpr (SS) ss_block_tokens<MODE>(tok, tok_stride, nrows, D, V, row0, t_idx, ss, gs, live, b, tk_ss);
   if (live) {
     int64_t tk = SS ? tk_ss : tok[(int64_t)b * tok_stride];
     if (tk < 0) tk = 0;

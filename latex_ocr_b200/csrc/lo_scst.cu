@@ -1,6 +1,6 @@
-// Self-critical sequence training (Rennie et al. 2017) of the torch-flavour decoder: the edit-distance reward of a sample and of
-// the greedy rollout, and the policy gradient of the sample's log-probability (include/latex_ocr_b200.h, lo_scst_*).  The sample
-// itself is drawn inside the decoder's time loop (lstm_pw_fwd_gumbel_kernel, lo_decoder.cu).
+// Self-critical sequence training (Rennie et al. 2017) of both decoder flavours: the edit-distance reward of a sample and of
+// the greedy rollout, and the policy gradient of the sample's log-probability (include/latex_ocr_b200.h, lo_scst_*; the _tf entry
+// points take the TF layout).  The sample itself is drawn inside the decoder's time loop (ss_block_tokens, lo_decoder.cu).
 #include "lo_common.cuh"
 
 namespace lo {
@@ -39,11 +39,12 @@ __device__ int warp_levenshtein(const int64_t* h, int n, const int64_t* r, int m
 }
 
 // One block per row: warp 0 scores the sample, warp 1 the greedy rollout.  Dynamic shared memory: ref [Lr] | hyp [Lh] | greedy [Lg]
-// int64, then three diagonals of Lmax = max(Lh, Lg) + 1 ints per warp.
+// int64, then three diagonals of Lmax = max(Lh, Lg) + 1 ints per warp.  s0: the first position of hyp that was drawn (1 in the
+// torch layout, where hyp[0] is the given start token; 0 in the TF layout).
 __global__ void __launch_bounds__(64) scst_reward_kernel(const int64_t* __restrict__ hyp, int64_t hs, int Lh,
                                                          const int64_t* __restrict__ greedy, int64_t gs, int Lg,
                                                          const int64_t* __restrict__ ref, int64_t rs, int Lr, int64_t end_id,
-                                                         float* __restrict__ r_sample, float* __restrict__ r_greedy,
+                                                         int s0, float* __restrict__ r_sample, float* __restrict__ r_greedy,
                                                          float* __restrict__ adv, int32_t* __restrict__ n_len) {
   extern __shared__ int64_t sm[];
   __shared__ float s_r[2];
@@ -66,8 +67,9 @@ __global__ void __launch_bounds__(64) scst_reward_kernel(const int64_t* __restri
     // metrics.edit_distance's per-row value, rounded once from double
     if (lane == 0) s_r[w] = mx == 0 ? 1.f : (float)(1.0 - (double)dist / (double)mx);
   }
-  // n_b = the first t >= 1 with hyp[t] == end_id, else Lh - 1
-  const int nb = w == 0 ? min(1 + trunc_len(s_h + 1, Lh - 1, end_id), Lh - 1) : 0;
+  // n_b = the number of draws up to and including the first END: torch (s0 = 1) the first t >= 1 with hyp[t] == end_id, else
+  // Lh - 1; TF (s0 = 0) that t + 1 for t >= 0, else Lh
+  const int nb = w == 0 ? min(1 + trunc_len(s_h + s0, Lh - s0, end_id), Lh - s0) : 0;
   __syncthreads();
   if (threadIdx.x == 0) {
     r_sample[b] = s_r[0];
@@ -91,12 +93,13 @@ __device__ __forceinline__ float block_reduce128(float x, float* sh) {
   return MAX ? fmaxf(fmaxf(sh[0], sh[1]), fmaxf(sh[2], sh[3])) : (sh[0] + sh[1]) + (sh[2] + sh[3]);
 }
 
-// One block per prediction row (s, b), s = t - 1: the softmax of preds / tau, d L / d preds into dpred, and the row's
-// log pi(fed[b][s+1]) into partial (0 past the row's n_b).
-__global__ void __launch_bounds__(128) scst_pg_kernel(const float* __restrict__ preds, int64_t ps, const int64_t* __restrict__ fed,
-                                                      int64_t fs, const float* __restrict__ adv, const int32_t* __restrict__ n_len,
-                                                      const float* __restrict__ temp, int T, int V, float inv_B,
-                                                      float* __restrict__ dpred, int64_t ds, float* __restrict__ partial) {
+// One block per prediction row (s, b): the softmax of preds / tau, d L / d preds into dpred (batch-major rows ds apart), and the
+// row's log pi(fed[b][s + foff]) into partial (0 past the row's n_b).  Row (s, b) of preds is at b * pb + s * pt: torch
+// (batch-major, s = t - 1, foff = 1) or TF (time-major, s = t, foff = 0).
+__global__ void __launch_bounds__(128) scst_pg_kernel(const float* __restrict__ preds, int64_t pb, int64_t pt,
+                                                      const int64_t* __restrict__ fed, int64_t fs, int foff, const float* __restrict__ adv,
+                                                      const int32_t* __restrict__ n_len, const float* __restrict__ temp, int T, int V,
+                                                      float inv_B, float* __restrict__ dpred, int64_t ds, float* __restrict__ partial) {
   __shared__ float sh[4];
   const int s = blockIdx.x, b = blockIdx.y;
   float* out = dpred + ((int64_t)b * T + s) * ds;
@@ -105,7 +108,7 @@ __global__ void __launch_bounds__(128) scst_pg_kernel(const float* __restrict__ 
     if (threadIdx.x == 0) partial[(int64_t)b * T + s] = 0.f;
     return;
   }
-  const float* x = preds + ((int64_t)b * T + s) * ps;
+  const float* x = preds + (int64_t)b * pb + (int64_t)s * pt;
   const float tau = *temp;
   float mx = -INFINITY;
   for (int v = threadIdx.x; v < V; v += blockDim.x) mx = fmaxf(mx, x[v] / tau);
@@ -113,7 +116,7 @@ __global__ void __launch_bounds__(128) scst_pg_kernel(const float* __restrict__ 
   float sum = 0.f;
   for (int v = threadIdx.x; v < V; v += blockDim.x) sum += expf(x[v] / tau - mx);
   const float lse = mx + logf(block_reduce128<false>(sum, sh));
-  int64_t f = fed[(int64_t)b * fs + s + 1];
+  int64_t f = fed[(int64_t)b * fs + s + foff];
   f = f < 0 ? 0 : (f >= V ? V - 1 : f);        // the token the cell embedded (lstm_pw_fwd_body clamps it the same way)
   const float g = -adv[b] * inv_B / tau;
   for (int v = threadIdx.x; v < V; v += blockDim.x) out[v] = g * ((v == f ? 1.f : 0.f) - expf(x[v] / tau - lse));
@@ -155,9 +158,10 @@ __global__ void __launch_bounds__(256) scst_loss_kernel(const float* __restrict_
 
 using namespace lo;
 
-extern "C" int lo_scst_edit_reward(const int64_t* hyp, int64_t hyp_stride, int Lh, const int64_t* greedy, int64_t greedy_stride,
-                                   int Lg, const int64_t* ref, int64_t ref_stride, int Lr, int B, int64_t end_id, float* r_sample,
-                                   float* r_greedy, float* adv, int32_t* n_len, void* stream) {
+// the entry points: torch layout (s0 = 1, foff = 1, batch-major preds) and TF layout (s0 = 0, foff = 0, time-major logits)
+static int edit_reward(const int64_t* hyp, int64_t hyp_stride, int Lh, const int64_t* greedy, int64_t greedy_stride, int Lg,
+                       const int64_t* ref, int64_t ref_stride, int Lr, int B, int64_t end_id, int s0, float* r_sample, float* r_greedy,
+                       float* adv, int32_t* n_len, void* stream) {
   LO_CHECK_ARG(hyp && ref && r_sample, "null pointer");
   LO_CHECK_ARG(B >= 1, "B >= 1");
   LO_CHECK_ARG(Lh >= 1 && Lh <= SCST_MAX_LEN && Lr >= 1 && Lr <= SCST_MAX_LEN, "hypothesis / reference lengths in 1..512");
@@ -166,22 +170,50 @@ extern "C" int lo_scst_edit_reward(const int64_t* hyp, int64_t hyp_stride, int L
   if (!greedy) Lg = 0;
   const size_t smem = (size_t)(Lr + Lh + Lg) * 8 + (size_t)2 * 3 * (max(Lh, Lg) + 1) * 4;
   scst_reward_kernel<<<B, 64, smem, (cudaStream_t)stream>>>(hyp, hyp_stride, Lh, greedy, greedy_stride, Lg, ref, ref_stride, Lr, end_id,
-                                                            r_sample, r_greedy, adv, n_len);
+                                                            s0, r_sample, r_greedy, adv, n_len);
   LO_LAUNCH_OK();
   return LO_OK;
 }
 
-extern "C" int lo_scst_pg_grad(const float* preds, int64_t pred_stride, const int64_t* fed, int64_t fed_stride, const float* adv,
-                               const int32_t* n_len, const float* temp, const float* r_sample, const float* r_greedy, int B, int T,
-                               int V, float* dpred, int64_t dpred_stride, float* partial, float* stats, void* stream) {
+static int pg_grad(const float* preds, int64_t pb, int64_t pt, int64_t pred_stride, const int64_t* fed, int64_t fed_stride, int foff,
+                   const float* adv, const int32_t* n_len, const float* temp, const float* r_sample, const float* r_greedy, int B, int T,
+                   int V, float* dpred, int64_t dpred_stride, float* partial, float* stats, void* stream) {
   LO_CHECK_ARG(preds && fed && adv && n_len && temp && dpred && partial && stats, "null pointer");
   LO_CHECK_ARG(B >= 1 && T >= 1 && V >= 2 && T <= 65535, "B, T >= 1, T <= 65535, V >= 2");
   LO_CHECK_ARG(pred_stride >= V && dpred_stride >= V && fed_stride >= T, "pred_stride, dpred_stride >= V; fed_stride >= T");
   cudaStream_t st = (cudaStream_t)stream;
-  scst_pg_kernel<<<dim3(T, B), 128, 0, st>>>(preds, pred_stride, fed, fed_stride, adv, n_len, temp, T, V, 1.0f / (float)B, dpred,
+  scst_pg_kernel<<<dim3(T, B), 128, 0, st>>>(preds, pb, pt, fed, fed_stride, foff, adv, n_len, temp, T, V, 1.0f / (float)B, dpred,
                                              dpred_stride, partial);
   LO_LAUNCH_OK();
   scst_loss_kernel<<<1, 256, 0, st>>>(partial, adv, n_len, r_sample, r_greedy, B, T, stats);
   LO_LAUNCH_OK();
   return LO_OK;
+}
+
+extern "C" int lo_scst_edit_reward(const int64_t* hyp, int64_t hyp_stride, int Lh, const int64_t* greedy, int64_t greedy_stride,
+                                   int Lg, const int64_t* ref, int64_t ref_stride, int Lr, int B, int64_t end_id, float* r_sample,
+                                   float* r_greedy, float* adv, int32_t* n_len, void* stream) {
+  return edit_reward(hyp, hyp_stride, Lh, greedy, greedy_stride, Lg, ref, ref_stride, Lr, B, end_id, 1, r_sample, r_greedy, adv, n_len,
+                     stream);
+}
+
+extern "C" int lo_scst_edit_reward_tf(const int64_t* hyp, int64_t hyp_stride, int Lh, const int64_t* greedy, int64_t greedy_stride,
+                                      int Lg, const int64_t* ref, int64_t ref_stride, int Lr, int B, int64_t end_id, float* r_sample,
+                                      float* r_greedy, float* adv, int32_t* n_len, void* stream) {
+  return edit_reward(hyp, hyp_stride, Lh, greedy, greedy_stride, Lg, ref, ref_stride, Lr, B, end_id, 0, r_sample, r_greedy, adv, n_len,
+                     stream);
+}
+
+extern "C" int lo_scst_pg_grad(const float* preds, int64_t pred_stride, const int64_t* fed, int64_t fed_stride, const float* adv,
+                               const int32_t* n_len, const float* temp, const float* r_sample, const float* r_greedy, int B, int T,
+                               int V, float* dpred, int64_t dpred_stride, float* partial, float* stats, void* stream) {
+  return pg_grad(preds, (int64_t)T * pred_stride, pred_stride, pred_stride, fed, fed_stride, 1, adv, n_len, temp, r_sample, r_greedy, B,
+                 T, V, dpred, dpred_stride, partial, stats, stream);
+}
+
+extern "C" int lo_scst_pg_grad_tf(const float* logits, int64_t ldl, const int64_t* fed, int64_t fed_stride, const float* adv,
+                                  const int32_t* n_len, const float* temp, const float* r_sample, const float* r_greedy, int B, int T,
+                                  int V, float* dpred, int64_t dpred_stride, float* partial, float* stats, void* stream) {
+  return pg_grad(logits, ldl, (int64_t)B * ldl, ldl, fed, fed_stride, 0, adv, n_len, temp, r_sample, r_greedy, B, T, V, dpred,
+                 dpred_stride, partial, stats, stream);
 }

@@ -14,24 +14,41 @@
 //
 // Schedule (same ideas as the torch flavour, DESIGN.md §4): att_img hoisted; the embedding half of the LSTM kernel folded into a
 // [V+1][4D] table (row V = start token); logits and every weight gradient hoisted out of the time loop into stacked GEMMs;
-// d att_img by one post-loop sweep; d enc by a batched alpha^T dctx GEMM.  The TMA-ring attention kernels serve both flavours:
+// d att_img by one post-loop sweep; d enc by a batched alpha^T dctx GEMM.  Sampling (lo_tfdec_args.ss_prob: scheduled sampling,
+// self-critical training): the logits GEMM moves into the loop and the cell kernel chooses the token consumed (ss_block_tokens).  The TMA-ring attention kernels serve both flavours:
 // the (NVA, NVC) = (1, 2) instantiation streams dim_e = 256 att_img columns next to C = 512 image channels, ACT = tanh.
 
 namespace lo {
 
 // ------------------------------------------------------------------------------------------------ pointwise kernels
-__global__ void tf_lstm_pw_fwd_kernel(const float* __restrict__ z, const float* __restrict__ ptab, const int64_t* __restrict__ tok,
-                                      int64_t tok_stride, int V, const float* __restrict__ c_prev, float* __restrict__ gates,
-                                      float* __restrict__ c_out, float* __restrict__ h_out, bf16* __restrict__ h_bf, int64_t xh_stride,
-                                      const float* __restrict__ keep, float* __restrict__ hd_out, bf16* __restrict__ hd_bf, int nrows,
-                                      int D) {
+// MODE 0: the token is tok (NULL: the start token).  MODE 1 / 2 (sampling, lo_tfdec_args.ss_prob): tok is the teacher token
+// formula[b][t_idx] and the token fed is chosen from the logits of step t_idx and recorded (ss_block_tokens: argmax, or a
+// Gumbel-max draw).  Those logits come from the head GEMM two launches back (head GEMM(t_idx), z GEMM(t_idx + 1), this kernel), so
+// they are read after griddepcontrol.wait: the wait returns once the z GEMM has completed, and the z GEMM's own wait (it reads
+// xh[t_idx + 1], written before the head GEMM) returned only once the head GEMM had.
+template <int MODE>
+__device__ __forceinline__ void tf_lstm_pw_fwd_body(const float* __restrict__ z, const float* __restrict__ ptab,
+                                                    const int64_t* __restrict__ tok, int64_t tok_stride, int V,
+                                                    const float* __restrict__ c_prev, float* __restrict__ gates, float* __restrict__ c_out,
+                                                    float* __restrict__ h_out, bf16* __restrict__ h_bf, int64_t xh_stride,
+                                                    const float* __restrict__ keep, float* __restrict__ hd_out, bf16* __restrict__ hd_bf,
+                                                    int nrows, int D, int t_idx, const SsStep& ss, const GumbelStep& gs) {
   pdl_wait();
   pdl_trigger();
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  int64_t tk_ss = 0;
+  if constexpr (MODE != 0) {
+    const bool live = idx < nrows * D;
+    ss_block_tokens<MODE>(tok, tok_stride, nrows, D, V, 0, t_idx, ss, gs, live, live ? idx / D : 0, tk_ss);
+  }
   if (idx >= nrows * D) return;
   const int b = idx / D, j = idx % D;
   int64_t tk = V;                                       // row V of the table = start token (decoder.py:45-46, :90-93)
-  if (tok) {
+  if constexpr (MODE != 0) {
+    tk = tk_ss;
+    if (tk < 0) tk = 0;
+    if (tk >= V) tk = V - 1;
+  } else if (tok) {
     tk = tok[(int64_t)b * tok_stride];
     if (tk < 0) tk = 0;
     if (tk >= V) tk = V - 1;
@@ -56,6 +73,36 @@ __global__ void tf_lstm_pw_fwd_kernel(const float* __restrict__ z, const float* 
     hd_out[(int64_t)b * D + j] = hdv;
     if (hd_bf) hd_bf[(int64_t)b * D + j] = __float2bfloat16_rn(hdv);
   }
+}
+
+__global__ void tf_lstm_pw_fwd_kernel(const float* __restrict__ z, const float* __restrict__ ptab, const int64_t* __restrict__ tok,
+                                      int64_t tok_stride, int V, const float* __restrict__ c_prev, float* __restrict__ gates,
+                                      float* __restrict__ c_out, float* __restrict__ h_out, bf16* __restrict__ h_bf, int64_t xh_stride,
+                                      const float* __restrict__ keep, float* __restrict__ hd_out, bf16* __restrict__ hd_bf, int nrows,
+                                      int D) {
+  tf_lstm_pw_fwd_body<0>(z, ptab, tok, tok_stride, V, c_prev, gates, c_out, h_out, h_bf, xh_stride, keep, hd_out, hd_bf, nrows, D, 0,
+                         SsStep{}, GumbelStep{});
+}
+// sampling (lo_tfdec_args.ss_prob): MODE 1 feeds the argmax, MODE 2 (ss_temp) a draw from softmax(logits / tau)
+template <int MODE>
+__global__ void tf_lstm_pw_fwd_ss_kernel(const float* __restrict__ z, const float* __restrict__ ptab, const int64_t* __restrict__ tok,
+                                         int64_t tok_stride, int V, const float* __restrict__ c_prev, float* __restrict__ gates,
+                                         float* __restrict__ c_out, float* __restrict__ h_out, bf16* __restrict__ h_bf,
+                                         int64_t xh_stride, const float* __restrict__ keep, float* __restrict__ hd_out,
+                                         bf16* __restrict__ hd_bf, int nrows, int D, int t_idx, SsStep ss, GumbelStep gs) {
+  tf_lstm_pw_fwd_body<MODE>(z, ptab, tok, tok_stride, V, c_prev, gates, c_out, h_out, h_bf, xh_stride, keep, hd_out, hd_bf, nrows, D,
+                            t_idx, ss, gs);
+}
+
+// sampling: the choice of the last step, fed[b][T-1] from the logits of step T-1 (recorded, never consumed: the last token of a
+// self-critical sample).  The same block geometry as the pointwise kernels, no cell.
+template <int MODE>
+__global__ void tf_ss_last_token_kernel(const int64_t* __restrict__ tok, int64_t tok_stride, int V, int nrows, int D, int t_idx,
+                                        SsStep ss, GumbelStep gs) {
+  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  const bool live = idx < nrows * D;
+  int64_t tk = 0;
+  ss_block_tokens<MODE>(tok, tok_stride, nrows, D, V, 0, t_idx, ss, gs, live, live ? idx / D : 0, tk);
 }
 
 __global__ void tf_o_pw_fwd_kernel(const float* __restrict__ oc, const float* __restrict__ oh, int64_t oh_stride,
@@ -329,6 +376,18 @@ static int tf_check(const lo_tfdec_args* a, bool decode) {
   const int rpi = a->rows_per_img > 1 ? a->rows_per_img : 1;
   LO_CHECK_ARG(a->B % rpi == 0, "B must be a multiple of rows_per_img");
   LO_TRY(check_reg_off(a, decode));
+  if (decode) {
+    LO_CHECK_ARG(!a->ss_prob && !a->fed && !a->ss_u && !a->ss_temp && !a->ss_gu && !a->ss_state,
+                 "scheduled sampling (ss_prob, fed, ss_u, ss_temp, ss_gu, ss_state) is a training mode: greedy decode feeds its own "
+                 "argmax already and beam search has no such mode");
+  } else if (a->ss_prob) {
+    LO_CHECK_ARG(a->fed, "scheduled sampling (ss_prob) needs fed");
+    LO_CHECK_ARG(a->ss_u || a->ss_state, "scheduled sampling (ss_prob) needs ss_u or ss_state for its coin");
+    LO_CHECK_ARG(rpi == 1, "scheduled sampling (ss_prob) needs rows_per_img <= 1");
+    LO_CHECK_ARG(!a->ss_gu || a->ss_temp, "ss_gu (injected Gumbel uniforms) needs ss_temp");
+  } else {
+    LO_CHECK_ARG(!a->ss_temp && !a->ss_gu, "ss_temp / ss_gu (sampling with a temperature) need ss_prob");
+  }
   LO_CHECK_ARG(g_opt_att_pipe, "the Genthial cell runs on the TMA-ring attention kernels only (option att_pipe=1)");
   return LO_OK;
 }
@@ -378,6 +437,22 @@ static int tf_prologue(const lo_tfdec_args* a, const TfDims& d, const TfWs& w, c
 
 // one cell step: consumes xh[t] = [o_{t-1} | h_{t-1}], call[t]; produces xh[t+1], call[t+1], alphas[:, t], ctx[t].  rg: decode with
 // per-image region counts (the ragged attention launch), NULL otherwise
+// the sampling operands of the pointwise kernel that chooses fed[:, ti] from the logits of step ti (lo_tfdec_args.ss_prob)
+static SsStep tf_ss_step(const lo_tfdec_args* a, const TfDims& d, int ti) {
+  SsStep ss{};
+  ss.prev_logits = a->logits + (int64_t)ti * d.B * d.Vl;      // time-major: row b of step ti
+  ss.lstride = d.Vl;
+  ss.prob = a->ss_prob;
+  ss.u = a->ss_u ? a->ss_u + ti : nullptr;
+  ss.coin_state = (const unsigned long long*)a->ss_state;
+  ss.ustride = d.T;
+  ss.fed = a->fed + ti;
+  return ss;
+}
+static GumbelStep tf_gumbel_step(const lo_tfdec_args* a, const TfDims& d, int ti) {
+  return GumbelStep{a->ss_temp, a->ss_gu ? a->ss_gu + (int64_t)ti * d.V : nullptr, (int64_t)d.T * d.V};
+}
+
 static int tf_step(const lo_tfdec_args* a, const TfDims& d, const TfWs& w, int t, const int64_t* tok, int64_t tok_stride,
                    cudaStream_t st, const AttRagged* rg = nullptr) {
   const size_t es = a->dt == LO_F32 ? 4 : 2;
@@ -389,11 +464,18 @@ static int tf_step(const lo_tfdec_args* a, const TfDims& d, const TfWs& w, int t
   float* out2 = w.out2 + rowt * d.N2;
   // z = [o_{t-1} ; h_{t-1}] K[E:]   (attention_cell.py:70-71; the embedding rows of K come from the table)
   LO_TRY(tf_nt(a, xh_t, xhb_t, d.XH, (const char*)a->w_lstm + (size_t)d.E * es, d.LW, w.ztmp, d.G, d.B, d.G, d.XH, nullptr, 0, st));
-  LO_CUDA(launch_pdl(tf_lstm_pw_fwd_kernel, dim3(cdiv((long)d.B * d.D, 256)), dim3(256), (size_t)0, st, (const float*)w.ztmp,
-                     (const float*)w.ptab, tok, tok_stride, d.V, (const float*)(w.call + rowt * d.D), w.gates + rowt * d.G,
-                     w.call + rown * d.D, xh_n + d.O, xhb_n ? xhb_n + d.O : (bf16*)nullptr, (int64_t)d.XH,
-                     a->keep_h ? a->keep_h + rowt * d.D : (const float*)nullptr, w.hd + rowt * d.D,
-                     w.hd_bf ? w.hd_bf + rowt * d.D : (bf16*)nullptr, d.B, d.D));
+  // the pointwise launch; `extra`: the step index and sampling operands of tf_lstm_pw_fwd_ss_kernel
+  auto launch_pw = [&](auto kernel, auto... extra) {
+    return launch_pdl(kernel, dim3(cdiv((long)d.B * d.D, 256)), dim3(256), (size_t)0, st, (const float*)w.ztmp, (const float*)w.ptab, tok,
+                      tok_stride, d.V, (const float*)(w.call + rowt * d.D), w.gates + rowt * d.G, w.call + rown * d.D, xh_n + d.O,
+                      xhb_n ? xhb_n + d.O : (bf16*)nullptr, (int64_t)d.XH, a->keep_h ? a->keep_h + rowt * d.D : (const float*)nullptr,
+                      w.hd + rowt * d.D, w.hd_bf ? w.hd_bf + rowt * d.D : (bf16*)nullptr, d.B, d.D, extra...);
+  };
+  if (a->ss_prob && t > 0)          // sampling: the token consumed now is chosen from the logits of step t-1
+    LO_CUDA(launch_pw(a->ss_temp ? tf_lstm_pw_fwd_ss_kernel<2> : tf_lstm_pw_fwd_ss_kernel<1>, t - 1, tf_ss_step(a, d, t - 1),
+                      tf_gumbel_step(a, d, t - 1)));
+  else
+    LO_CUDA(launch_pw(tf_lstm_pw_fwd_kernel));
   LO_LAUNCH_OK();
   // [hd_t W_h | hd_t o_W_h] with hd_t = dropout(h_t)   (attention_cell.py:72, attention_mechanism.py:79, attention_cell.py:82)
   if (a->keep_h)
@@ -452,10 +534,27 @@ int lo_tfdec_forward(const lo_tfdec_args* a, int with_loss, void* stream) {
   LO_CHECK_ARG(d.rpi == 1, "training runs with rows_per_img = 1");
   const TfWs w = tf_carve(a);
   LO_TRY(tf_prologue(a, d, w, st));
-  for (int t = 0; t < d.T; t++)
+  const bool sampling = a->ss_prob != nullptr;
+  for (int t = 0; t < d.T; t++) {
     LO_TRY(tf_step(a, d, w, t, t == 0 ? nullptr : a->formula + (t - 1), a->formula_stride, st));
-  // logits for all (t, b) in one GEMM: rows 1..T of xh hold o_t   (attention_cell.py:84)
-  LO_TRY(tf_logits(a, d, w, d.B, d.T * d.B, a->logits, d.Vl, st));
+    // sampling: the head of step t inside the loop (the next step's cell chooses its token from these logits)
+    if (sampling) LO_TRY(tf_logits(a, d, w, (int64_t)(t + 1) * d.B, d.B, a->logits + (int64_t)t * d.B * d.Vl, d.Vl, st));
+  }
+  if (sampling) {
+    // fed[:, T-1]: chosen like the others, consumed by no step.  One warp per row (the block geometry of a row width of 32)
+    const SsStep ss = tf_ss_step(a, d, d.T - 1);
+    const GumbelStep gs = tf_gumbel_step(a, d, d.T - 1);
+    const int64_t* tok = a->formula + (d.T - 1);
+    const dim3 grid(cdiv((long)d.B * 32, 256));
+    if (a->ss_temp)
+      tf_ss_last_token_kernel<2><<<grid, 256, 0, st>>>(tok, a->formula_stride, d.V, d.B, 32, d.T - 1, ss, gs);
+    else
+      tf_ss_last_token_kernel<1><<<grid, 256, 0, st>>>(tok, a->formula_stride, d.V, d.B, 32, d.T - 1, ss, gs);
+    LO_LAUNCH_OK();
+  } else {
+    // logits for all (t, b) in one GEMM: rows 1..T of xh hold o_t   (attention_cell.py:84)
+    LO_TRY(tf_logits(a, d, w, d.B, d.T * d.B, a->logits, d.Vl, st));
+  }
   if (!with_loss) return LO_OK;
   const int rows = d.T * d.B;
   tf_ce_kernel<<<cdiv(rows, 8), 256, 0, st>>>(a->logits, a->formula, a->formula_stride, a->lengths, w.row_loss, w.dlogits, w.dlogits_bf,
@@ -549,7 +648,9 @@ int lo_tfdec_backward(const lo_tfdec_args* a, void* stream) {
   // LSTM kernel, [o ; h] rows: dz^T xh[0..T-1]
   LO_TRY(tf_tn(a, w.dz, w.dz_bf, d.G, w.xh, w.xh_bf, d.XH, a->g_w_lstm + d.E, d.LW, d.G, d.XH, TB, st));
   // embedding rows through the table: d ptab (scatter), then d emb = d ptab K[:E]^T..., d K[:E] = d ptab^T emb, d b = colsum
-  tf_dptab_scatter_kernel<<<LO_NUM_SMS * 8, 256, 0, st>>>(w.dz, a->formula, a->formula_stride, w.dptab, d.B, d.T, d.G, d.V);
+  // (sampling: the tokens the forward fed, not the targets)
+  tf_dptab_scatter_kernel<<<LO_NUM_SMS * 8, 256, 0, st>>>(w.dz, a->ss_prob ? a->fed : a->formula,
+                                                          a->ss_prob ? (int64_t)d.T : a->formula_stride, w.dptab, d.B, d.T, d.G, d.V);
   LO_LAUNCH_OK();
   LO_TRY(gemm_nn(w.dptab, LO_F32, d.G, a->w_lstm, dt, d.LW, a->g_emb, LO_F32, d.E, d.V + 1, d.E, d.G, 0, LO_IMPL_SIMT, st));
   LO_TRY(gemm_tn(w.dptab, LO_F32, d.G, a->emb, dt, d.E, a->g_w_lstm, LO_F32, d.LW, d.G, d.E, d.V + 1, 0, LO_IMPL_SIMT, st));

@@ -5,7 +5,9 @@ the sm_90a kernels (csrc/lo_tfdecoder.cuh) through the C ABI (``lo_tfdec_*``).
 The reference builds a TF graph; here the same three things the graph offers are methods:
   * ``train_logits(enc, formula)``            -> pred_train  [N,T,V]                      (decoder.py:48-57)
   * ``train_outputs(enc, formula)``           -> (pred_train, alphas [N,T,R]), differentiable: any loss of them trains
-                                                 through ``loss.backward()`` (lo_tfdec_backward in its generic mode)
+                                                 through ``loss.backward()`` (lo_tfdec_backward in its generic mode); with
+                                                 ``sampling_prob`` / ``sampling_temperature`` the fed tokens are the model's own
+                                                 (scheduled sampling, self-critical training: ``scst``)
   * ``loss_and_backward(enc, formula, len)``  -> masked CE of img2seq.py:68-71 + every gradient (+ d enc)
   * ``decode(enc)``                           -> DecoderOutput(logits=None, ids)          (decoder.py:59-70; greedy ids [N,time],
                                                  beam ids [N,time,beam] like the TF cell before img2seq.py:241 transposes them);
@@ -89,6 +91,43 @@ class Decoder(nn.Module):
             bind(self, n, S, n)
         self.reset_parameters()
         self._ws = LRUCache()     # bounded: see params.LRUCache
+        # sampling (train_outputs(..., sampling_prob=p)): the device scalars p and tau the kernels read (created on first use), the
+        # Philox {seed, call} of the coins and Gumbel uniforms (one call per sampling forward), the tokens fed by the last forward
+        # [N, T], and injected coins [N, T] / Gumbel uniforms [N, T, V] for parity tests (None: Philox)
+        self._ss_prob = self._ss_temp = None
+        self.ss_state = torch.tensor([int(torch.initial_seed()) & 0x7FFFFFFFFFFFFFFF, 0], dtype=torch.int64, device=device)
+        self.last_fed_tokens = None
+        self._ss_u = self._ss_gu = None
+
+    def seed_sampling(self, seed, call=0):
+        """Seeds the Philox stream of the sampling coins and Gumbel uniforms; every sampling forward uses up one ``call``."""
+        self.ss_state.copy_(torch.tensor([int(seed) & 0x7FFFFFFFFFFFFFFF, int(call)], dtype=torch.int64))
+
+    @staticmethod
+    def check_sampling(sampling_prob, sampling_temperature):
+        """The argument checks of DecoderWithAttention.forward."""
+        if not 0.0 <= sampling_prob <= 1.0:
+            raise ValueError("sampling_prob must lie in [0, 1] (got %r)" % (sampling_prob,))
+        if not (sampling_temperature >= 0.0 and math.isfinite(sampling_temperature)):
+            raise ValueError("sampling_temperature must be a finite tau >= 0 (got %r)" % (sampling_temperature,))
+        if sampling_temperature > 0.0 and sampling_prob == 0.0:
+            raise ValueError("sampling_temperature needs sampling_prob > 0: it sets how the fed tokens are drawn")
+
+    def sampling_scalars(self, sampling_prob, sampling_temperature=0.0):
+        """(p, tau) as the device scalars run_forward takes, None for off (p = 0: teacher forcing; tau = 0: the argmax)."""
+        self.check_sampling(sampling_prob, sampling_temperature)
+        ss = tau = None
+        if sampling_prob > 0.0:
+            if self._ss_prob is None:
+                self._ss_prob = torch.zeros((), dtype=torch.float32, device=self.store.device)
+            ss = self._ss_prob
+            ss.fill_(sampling_prob)
+        if sampling_temperature > 0.0:
+            if self._ss_temp is None:
+                self._ss_temp = torch.zeros((), dtype=torch.float32, device=self.store.device)
+            tau = self._ss_temp
+            tau.fill_(sampling_temperature)
+        return ss, tau
 
     # tf.get_variable / tf.layers.dense default: glorot_uniform; LSTMCell bias zeros; embeddings decoder.py:98-105
     def reset_parameters(self):
@@ -175,9 +214,11 @@ class Decoder(nn.Module):
             assert ws[name].shape == (T, B, width)
             setattr(a, name, ws[name].data_ptr())
 
-    def run_forward(self, enc, formula, lengths=None, keep_h=None, keep_o=None, n_words=None):
+    def run_forward(self, enc, formula, lengths=None, keep_h=None, keep_o=None, n_words=None, ss_prob=None, ss_temp=None):
         """enc [N,R,C] or [N,H,W,C]; formula int64 [N,T]; lengths [N] (incl. END) enables the loss.  Returns the workspace dict
-        (``logits`` [T,N,ldl] time-major, ``alphas`` [N,T,R], ``loss``)."""
+        (``logits`` [T,N,ldl] time-major, ``alphas`` [N,T,R], ``loss``).  ss_prob / ss_temp: None, or the device scalars of
+        sampling_scalars: the tokens fed land in ``ws["fed"]`` [N,T] (lo_tfdec_args.ss_prob), and the call uses up one Philox call
+        of ``ss_state``."""
         enc = self._enc(enc)
         B, R, _ = enc.shape
         T = formula.shape[1]
@@ -192,7 +233,20 @@ class Decoder(nn.Module):
             # data parallel: n_words = token count of the GLOBAL batch, so that summing rank gradients gives the global mean
             a.inv_n_words = 1.0 / float(n_words if n_words is not None else int(lens.sum()))
         self._keep(a, ws, keep_h, keep_o, T, B)
+        if ss_prob is not None:
+            if ws.get("fed") is None:
+                ws["fed"] = torch.zeros(B, T, dtype=torch.int64, device=self.store.device)
+            a.ss_prob, a.fed, a.ss_state = ss_prob.data_ptr(), ws["fed"].data_ptr(), self.ss_state.data_ptr()
+            for name, inj, shape, on in (("ss_u", self._ss_u, (B, T), True), ("ss_gu", self._ss_gu, (B, T, self.V), ss_temp is not None)):
+                if inj is not None and on:
+                    ws[name] = inj.to(self.store.device, torch.float32).contiguous()
+                    assert ws[name].shape == shape
+                    setattr(a, name, ws[name].data_ptr())
+            if ss_temp is not None:
+                a.ss_temp = ss_temp.data_ptr()
         check(L.lo_tfdec_forward(ctypes.byref(a), 1 if with_loss else 0, stream_ptr()))
+        if ss_prob is not None:
+            self.ss_state[1] += 1            # the next sampling forward draws from a new Philox call
         return ws
 
     def run_backward(self, ws):
@@ -204,16 +258,28 @@ class Decoder(nn.Module):
             ws = self.run_forward(enc, formula, None, keep_h, keep_o)
             return ws["logits"][:, :, :self.V].permute(1, 0, 2).contiguous()
 
-    def train_outputs(self, enc, formula, keep_h=None, keep_o=None):
+    def train_outputs(self, enc, formula, keep_h=None, keep_o=None, sampling_prob=0.0, sampling_temperature=0.0):
         """Teacher-forced pass: (logits [N,T,V], alphas [N,T,R]).  With grad mode on and ``enc`` or a parameter requiring grad, an
         autograd graph is recorded: both outputs are differentiable (any loss of them), d enc comes back in ``enc``'s shape and
         dtype, and the backward runs lo_tfdec_backward in its generic mode with the same keep masks.  The outputs are the same
-        either way."""
-        return kernel_forward(self, (enc, formula, keep_h, keep_o), (enc,))[0]
+        either way.
 
-    def _forward_impl(self, enc, formula, keep_h, keep_o, need_grad):
+        ``sampling_prob`` = p > 0: scheduled sampling (Bengio et al. 2015) inside the CUDA time loop.  Every step predicts: step t
+        predicts ``formula[:, t]`` and step t+1 consumes ``fed[b][t]``, which is the lowest-index argmax of the returned logits
+        ``[b, t]`` where a coin u ~ U[0,1) is below p, ``formula[b][t]`` otherwise (step 0 consumes the start token).  The coins come
+        from Philox keyed by ``ss_state`` (``philox.sampling_uniforms``; one call per sampling forward, also without grad;
+        ``seed_sampling`` reproduces them).  ``last_fed_tokens`` holds fed [N,T]; its last column is consumed by no step.  The
+        choice is not differentiated: the backward is teacher forcing on fed, and a loss's targets stay ``formula``.
+        ``sampling_temperature`` = tau > 0 (with p > 0): a step that samples feeds a draw from softmax(logits / tau) (Gumbel-max,
+        ``philox.gumbel_uniforms``) instead of the argmax; with p = 1 the call samples whole formulas and a policy-gradient loss
+        of the outputs trains through ``loss.backward()`` (``scst``).  p = 0 (the default) is the teacher-forced path unchanged."""
+        return kernel_forward(self, (enc, formula, keep_h, keep_o, float(sampling_prob), float(sampling_temperature or 0.0)), (enc,))[0]
+
+    def _forward_impl(self, enc, formula, keep_h, keep_o, sampling_prob=0.0, sampling_temperature=0.0, need_grad=False):
         """((logits, alphas), None, what the backward of this call needs or None)."""
-        ws = self.run_forward(enc, formula, None, keep_h, keep_o)
+        ss, tau = self.sampling_scalars(sampling_prob, sampling_temperature)
+        ws = self.run_forward(enc, formula, None, keep_h, keep_o, ss_prob=ss, ss_temp=tau)
+        self.last_fed_tokens = (ws["fed"] if ss is not None else ws["formula"]).clone()
         logits = ws["logits"][:, :, :self.V].permute(1, 0, 2).contiguous()
         alphas = ws["alphas"].clone()
         saved = None
@@ -238,12 +304,15 @@ class Decoder(nn.Module):
         check(_lib.lib().lo_tfdec_backward(ctypes.byref(a), stream_ptr()))
         return (ws["denc"].reshape(saved["shape"]).to(saved["dtype"], copy=True),)
 
-    def loss_and_backward(self, enc, formula, lengths, keep_h=None, keep_o=None, n_words=None):
+    def loss_and_backward(self, enc, formula, lengths, keep_h=None, keep_o=None, n_words=None, sampling_prob=0.0):
         """Returns (loss tensor [4] on the device: mean CE, mean CE, 0, n_words; d loss / d enc [N,R,C] fp32).  Parameter
-        gradients land in ``self.store.grad`` (the ``.grad`` of every parameter)."""
+        gradients land in ``self.store.grad`` (the ``.grad`` of every parameter).  ``sampling_prob`` = p > 0: scheduled sampling
+        as in train_outputs (the CE targets stay ``formula``); ``last_fed_tokens`` is then the step's fed buffer [N,T]."""
         bind_grads(self, self.store)             # autograd use or zero_grad(set_to_none=True) may have re-pointed p.grad
         with torch.no_grad():
-            ws = self.run_forward(enc, formula, lengths, keep_h, keep_o, n_words)
+            ss, _ = self.sampling_scalars(float(sampling_prob))
+            ws = self.run_forward(enc, formula, lengths, keep_h, keep_o, n_words, ss_prob=ss)
+            self.last_fed_tokens = ws["fed"] if ss is not None else None
             denc = self.run_backward(ws)
             return ws["loss"], denc
 

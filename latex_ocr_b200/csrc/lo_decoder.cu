@@ -1276,6 +1276,35 @@ struct Rows {
   const AttRagged* rg = nullptr;     // decode with per-image region counts: the whole batch, row0 = 0
 };
 
+// C (+)= A W^T for the per-step GEMMs of the time loops (M <= B rows): the mma.sync kernel for <= 64 rows of the bf16 mirror Abf,
+// wgmma above, CUDA cores on the fp32 operand A32 when there are no mirrors (tc false).  The tensor-core paths run `splits` K slices
+// (atomic_acc: added onto C with fp32 atomics); the CUDA-core path writes C or, with `acc`, adds to it.
+static int step_gemm_nt(bool tc, const float* A32, const bf16* Abf, int64_t lda, const void* W, int dtW, int64_t ldw, float* C,
+                        int64_t ldc, int M, int N, int K, const float* bias, int acc, int splits, int atomic_acc, cudaStream_t st) {
+  if (tc && g_opt_skinny_mma && M <= 64) return skinny_gemm_nt(Abf, lda, (const bf16*)W, ldw, C, ldc, M, N, K, bias, splits, atomic_acc, st);
+  if (tc) return tc_gemm_nt_ex(Abf, lda, (const bf16*)W, ldw, C, LO_F32, ldc, M, N, K, bias, 0, 0, splits, atomic_acc, 1, st);
+  return gemm_nt(A32, LO_F32, lda, W, dtW, ldw, C, LO_F32, ldc, M, N, K, bias, acc, 0, LO_IMPL_SIMT, st);
+}
+
+// logits = fc(h) for M rows inside a time loop (sampling head, greedy and beam decode): the dispatcher's mma.sync kernel for <= 64
+// rows of the bf16 mirror hbf, CUDA cores on h32 otherwise
+static int head_nt(const lo_decoder_args* a, bool tc, const float* h32, const bf16* hbf, int64_t ldh, float* logits, int64_t ldl, int M,
+                   cudaStream_t st) {
+  if (tc) return gemm_nt(hbf, LO_BF16, ldh, a->w_fc, LO_BF16, a->D, logits, LO_F32, ldl, M, a->V, a->D, a->b_fc, 0, 0, LO_IMPL_TC, st);
+  return gemm_nt(h32, LO_F32, ldh, a->w_fc, a->dt, a->D, logits, LO_F32, ldl, M, a->V, a->D, a->b_fc, 0, 0, LO_IMPL_SIMT, st);
+}
+
+// the LSTM cell of step t for the rows from r0 on, run in the epilogue of the gates GEMM: tok, hd_t, dmask_t point at row 0
+static TcLstmEpi lstm_epi(const lo_decoder_args* a, const Dims& d, const BfViews& bv, int t, int64_t r0, const int64_t* tok,
+                          int64_t tok_stride, float* hd_t, int64_t hd_stride, const float* dmask_t) {
+  const int64_t cur = (int64_t)t * d.B + r0, nxt = (int64_t)(t + 1) * d.B + r0;
+  return TcLstmEpi{a->ptab, tok + r0 * tok_stride, tok_stride, a->out1 + cur * d.O1 + d.A + d.C, d.O1, a->call + cur * d.D,
+                   a->gates + cur * d.G, a->call + nxt * d.D, a->hall + nxt * d.D, bv.hall + nxt * d.D,
+                   hd_t ? hd_t + r0 * hd_stride : (float*)nullptr, hd_stride, dmask_t ? dmask_t + r0 * hd_stride : (const float*)nullptr,
+                   d.D, d.V, (const unsigned long long*)((hd_t && a->has_dropout == 2) ? a->dropout_state : nullptr), a->dropout_p,
+                   (int)r0, t};
+}
+
 // one decoder step t for the rows of `rs`; tok: token ids consumed at this step (row 0 of the batch)
 static int forward_step(const lo_decoder_args* a, const Dims& d, int t, const Rows& rs, const int64_t* tok, int64_t tok_stride,
                         float* hd_t, int64_t hd_stride, const float* dmask_t, cudaStream_t st) {
@@ -1294,16 +1323,9 @@ static int forward_step(const lo_decoder_args* a, const Dims& d, int t, const Ro
   const char* enc = (const char*)a->enc + (size_t)(r0 / rpi) * d.R * d.C * es;
   // [att2 | gate_pre | hh_pre] = h_prev @ [W_d; W_beta; W_hh]^T + b   (seq2seq_torch.py:187, :311, LSTMCell hh part)
   const BfViews bv = bf_views(a, d);
-  if (g_opt_dbg_skip & 4) {
-  } else if (bv.on && g_opt_skinny_mma && nrows <= 64) {
-    LO_TRY(skinny_gemm_nt(bv.hall + ((int64_t)t * d.B + r0) * d.D, d.D, (const bf16*)a->wcat1, d.D, o1, d.O1, nrows, d.O1, d.D, a->bcat1, 1,
-                          0, st));
-  } else if (bv.on) {
-    LO_TRY(tc_gemm_nt_ex(bv.hall + ((int64_t)t * d.B + r0) * d.D, d.D, (const bf16*)a->wcat1, d.D, o1, LO_F32, d.O1, nrows, d.O1, d.D,
-                         a->bcat1, 0, 0, 1, 0, 1, st));
-  } else {
-    LO_TRY(gemm_nt(h_prev, LO_F32, d.D, a->wcat1, dt, d.D, o1, LO_F32, d.O1, nrows, d.O1, d.D, a->bcat1, 0, 0, LO_IMPL_SIMT, st));
-  }
+  if (!(g_opt_dbg_skip & 4))
+    LO_TRY(step_gemm_nt(bv.on, h_prev, bv.on ? bv.hall + ((int64_t)t * d.B + r0) * d.D : nullptr, d.D, a->wcat1, dt, d.D, o1, d.O1, nrows,
+                        d.O1, d.D, a->bcat1, 0, 1, 0, st));
   if (rs.rg) {
     if (!(g_opt_dbg_skip & 2)) {
       AttFwdArgs x{a->att1, a->enc, o1, d.O1, a->w_full, a->alphas + t * d.R, (int64_t)d.T * d.R, a->ctx + (int64_t)t * d.B * d.C, o1 + d.A,
@@ -1320,25 +1342,13 @@ static int forward_step(const lo_decoder_args* a, const Dims& d, int t, const Ro
   // gates_x = (gate*ctx) @ W_ih[:, E:]^T
   if (bv.on && g_opt_fuse_lstm && !sampling) {
     // ... with the LSTM cell fused into the GEMM epilogue (no gates_x round trip, one launch less per step)
-    TcLstmEpi e{a->ptab, tok + r0 * tok_stride, tok_stride, o1 + d.A + d.C, d.O1, c_prev, a->gates + ((int64_t)t * d.B + r0) * d.G,
-                a->call + ((int64_t)(t + 1) * d.B + r0) * d.D, a->hall + ((int64_t)(t + 1) * d.B + r0) * d.D,
-                bv.hall + ((int64_t)(t + 1) * d.B + r0) * d.D, hd_t ? hd_t + r0 * hd_stride : (float*)nullptr, hd_stride,
-                dmask_t ? dmask_t + r0 * hd_stride : (const float*)nullptr, d.D, d.V,
-                (const unsigned long long*)((hd_t && a->has_dropout == 2) ? a->dropout_state : nullptr), a->dropout_p, (int)r0, t};
+    const TcLstmEpi e = lstm_epi(a, d, bv, t, r0, tok, tok_stride, hd_t, hd_stride, dmask_t);
     if (g_opt_skinny_mma && nrows <= 64 && d.C <= 512)
       return skinny_gemm_nt_lstm(bv.gctx + ((int64_t)t * d.B + r0) * d.C, d.C, bv.wil, d.C, nrows, d.D, d.C, e, st);
     return tc_gemm_nt_lstm(bv.gctx + ((int64_t)t * d.B + r0) * d.C, d.C, bv.wil, d.C, nrows, d.D, d.C, e, st);
   }
-  if (bv.on && g_opt_skinny_mma && nrows <= 64) {
-    LO_TRY(skinny_gemm_nt(bv.gctx + ((int64_t)t * d.B + r0) * d.C, d.C, (const bf16*)a->w_ih + d.E, d.E + d.C, gtmp, d.G, nrows, d.G, d.C,
-                          nullptr, 1, 0, st));
-  } else if (bv.on) {
-    LO_TRY(tc_gemm_nt_ex(bv.gctx + ((int64_t)t * d.B + r0) * d.C, d.C, (const bf16*)a->w_ih + d.E, d.E + d.C, gtmp, LO_F32, d.G, nrows,
-                         d.G, d.C, nullptr, 0, 0, 1, 0, 1, st));
-  } else {
-    LO_TRY(gemm_nt(a->gctx + ((int64_t)t * d.B + r0) * d.C, LO_F32, d.C, (const char*)a->w_ih + (size_t)d.E * es, dt, d.E + d.C, gtmp,
-                   LO_F32, d.G, nrows, d.G, d.C, nullptr, 0, 0, LO_IMPL_SIMT, st));
-  }
+  LO_TRY(step_gemm_nt(bv.on, a->gctx + ((int64_t)t * d.B + r0) * d.C, bv.on ? bv.gctx + ((int64_t)t * d.B + r0) * d.C : nullptr, d.C,
+                      (const char*)a->w_ih + (size_t)d.E * es, dt, d.E + d.C, gtmp, d.G, nrows, d.G, d.C, nullptr, 0, 1, 0, st));
   SsStep ss{};
   if (sampling) {
     ss.prev_logits = t > 0 ? a->logits + (r0 * d.T + t - 1) * d.Vl : nullptr;
@@ -1371,15 +1381,76 @@ static int forward_step(const lo_decoder_args* a, const Dims& d, int t, const Ro
   LO_LAUNCH_OK();
   if (sampling) {
     // the head of step t, right after the cell (the next step's cell reads these logits, see lstm_pw_fwd_kernel): the returned
-    // predictions of this mode.  The dispatcher of greedy decode: mma.sync for <= 64 bf16 rows, CUDA cores in fp32
-    float* lg = a->logits + (r0 * d.T + t) * d.Vl;
-    if (bv.on)
-      LO_TRY(gemm_nt(ss.hd_bf, LO_BF16, hd_stride, a->w_fc, LO_BF16, d.D, lg, LO_F32, (int64_t)d.T * d.Vl, nrows, d.V, d.D, a->b_fc, 0, 0,
-                     LO_IMPL_TC, st));
-    else
-      LO_TRY(gemm_nt(hd_t + r0 * hd_stride, LO_F32, hd_stride, a->w_fc, dt, d.D, lg, LO_F32, (int64_t)d.T * d.Vl, nrows, d.V, d.D, a->b_fc,
-                     0, 0, LO_IMPL_SIMT, st));
+    // predictions of this mode
+    LO_TRY(head_nt(a, bv.on, hd_t + r0 * hd_stride, ss.hd_bf, hd_stride, a->logits + (r0 * d.T + t) * d.Vl, (int64_t)d.T * d.Vl, nrows, st));
   }
+  return LO_OK;
+}
+
+// one backward step t for the rows of `rs`, the launches of forward_step in reverse; dal, dal_b, dal_t: the d alpha rows of
+// lo_decoder_backward
+static int backward_step(const lo_decoder_args* a, const Dims& d, int t, const Rows& rs, const float* dal, int64_t dal_b, int64_t dal_t,
+                         cudaStream_t st) {
+  const int dt = a->dt;
+  const int nrows = rs.nrows;
+  const int64_t r0 = rs.row0;
+  if (nrows <= 0) return LO_OK;
+  const size_t es = dt == LO_F32 ? 4 : 2;
+  const BfViews bv = bf_views(a, d);
+  float* dcat_t = a->dcat + ((int64_t)t * d.B + r0) * d.O1;
+  bf16* dcat_bf_t = bv.on ? bv.dcat + ((int64_t)t * d.B + r0) * d.O1 : nullptr;
+  const float* o1 = a->out1 + ((int64_t)t * d.B + r0) * d.O1;
+  float* dxh = a->dxh + r0 * (d.C + d.D);
+  const float* dmul = (a->has_dropout == 1 && a->dropout_mask) ? a->dropout_mask + (int64_t)t * d.D + r0 * d.T * d.D : nullptr;
+  if (!(g_opt_dbg_skip & 4))
+    LO_CUDA(launch_pdl(lstm_pw_bwd_kernel, dim3(cdiv((long)nrows * d.D, 256)), dim3(256), (size_t)0, st,
+                       (const float*)(a->dhd + (int64_t)t * d.D + r0 * d.T * d.D), (int64_t)d.T * d.D, dmul, (const float*)(dxh + d.C),
+                       (int64_t)(d.C + d.D), a->dc + r0 * d.D, (const float*)(a->gates + ((int64_t)t * d.B + r0) * d.G),
+                       (const float*)(a->call + ((int64_t)t * d.B + r0) * d.D),
+                       (const float*)(a->call + ((int64_t)(t + 1) * d.B + r0) * d.D), dcat_t + d.A + d.C, (int64_t)d.O1,
+                       bv.on ? dcat_bf_t + d.A + d.C : (bf16*)nullptr, bv.on ? dxh : (float*)nullptr, d.C, nrows, d.D,
+                       (const unsigned long long*)(a->has_dropout == 2 ? a->dropout_state : nullptr), a->dropout_p, (int)r0, t));
+  LO_LAUNCH_OK();
+  // [dgctx | dh_prev] = dG @ [W_ih[:, E:] | W_hh]
+  if (!(g_opt_dbg_skip & 4))
+    LO_TRY(step_gemm_nt(bv.on, dcat_t + d.A + d.C, bv.on ? dcat_bf_t + d.A + d.C : nullptr, d.O1, a->wbwd1, dt, d.G, dxh, d.C + d.D,
+                        nrows, d.C + d.D, d.G, nullptr, 0, 4, 1, st));
+  const char* att1 = (const char*)a->att1 + (size_t)r0 * d.R * d.A * es;
+  const char* enc = (const char*)a->enc + (size_t)r0 * d.R * d.C * es;
+  const float* alpha_t = a->alphas + (r0 * d.T + t) * d.R;
+  const float* ctx_t = a->ctx + ((int64_t)t * d.B + r0) * d.C;
+  const float* dal_t_ptr = dal + (int64_t)t * dal_t + r0 * dal_b;
+  const float* sreg_t = a->sreg + r0 * d.T + t;
+  float* de_t = a->de + (r0 * d.T + t) * d.R;
+  float* dctx_t = a->dctx + ((int64_t)t * d.B + r0) * d.C;
+  if (g_opt_dbg_skip & 2) {
+  } else if (g_opt_att_pipe) {
+    AttBwdArgs x{att1, enc, o1, o1 + d.A, d.O1, a->w_full, alpha_t, (int64_t)d.T * d.R, ctx_t, dxh, d.C + d.D, dal_t_ptr, dal_b, sreg_t,
+                 d.T, de_t, dcat_t, dcat_t + d.A, d.O1, dcat_bf_t, dcat_bf_t ? dcat_bf_t + d.A : nullptr, dctx_t, nrows, d.R, rs.work,
+                 a->dmean + r0 * d.A, rs.nsplit, 0, 0, att_mask_at(a, t, r0)};
+    LO_TRY(attention_bwd_pipe(x, dt, d.C, st));
+  } else {
+    const int ns = att_splits(d.B);
+    int* cnt_c = (int*)rs.work;
+    float* part_c = (float*)((char*)rs.work + att_partials_offset(nrows));
+    dim3 grid(ns, nrows);
+#define LO_ATT_BWD(TY_, NV)                                                                                                       \
+  attention_bwd_kernel<TY_, NV><<<grid, LO_ATT_THREADS, 0, st>>>(                                                                 \
+      (const TY_*)att1, (const TY_*)enc, o1, o1 + d.A, d.O1, a->w_full, alpha_t, (int64_t)d.T * d.R, ctx_t, dxh, d.C + d.D, dal_t_ptr, \
+      dal_b, sreg_t, d.T, de_t, dcat_t, dcat_t + d.A, d.O1, dcat_bf_t, dcat_bf_t ? dcat_bf_t + d.A : nullptr, dctx_t, d.R, ns, cnt_c,  \
+      part_c)
+    if (dt == LO_F32) {
+      if (d.C == 256) LO_ATT_BWD(float, 1); else if (d.C == 512) LO_ATT_BWD(float, 2); else LO_ATT_BWD(float, 4);
+    } else {
+      if (d.C == 256) LO_ATT_BWD(bf16, 1); else if (d.C == 512) LO_ATT_BWD(bf16, 2); else LO_ATT_BWD(bf16, 4);
+    }
+#undef LO_ATT_BWD
+    LO_LAUNCH_OK();
+  }
+  // dh_prev += [datt2 | dgate_pre] @ [W_d ; W_beta]
+  if (!(g_opt_dbg_skip & 4))
+    LO_TRY(step_gemm_nt(bv.on, dcat_t, dcat_bf_t, d.O1, a->wbwd2, dt, d.A + d.C, dxh + d.C, d.C + d.D, nrows, d.D, d.A + d.C, nullptr, 1,
+                        4, 1, st));
   return LO_OK;
 }
 
@@ -1407,6 +1478,151 @@ static inline Rows chain_rows(const lo_decoder_args* a, const Dims& d, int chain
   r.work = (char*)a->work + (size_t)chain * lo_attention_workspace_bytes(d.B, d.C);
   r.nsplit = nchains == 2 ? (LO_NUM_SMS / (half > 0 ? half : 1) > 0 ? LO_NUM_SMS / half : 1) : 0;   // each chain fills one CTA slot per SM
   return r;
+}
+
+// the time loop of a training forward or backward (DESIGN.md §4): per-step launches on one or two row chains, or one fused step
+// kernel per step with a grid barrier (dec_fuse*) or per 16-row cluster (dec_cl*)
+enum class FwdSched { Chains, Fused, Cluster };
+enum class BwdSched { Chains, Fused, Cluster };
+
+static FwdSched pick_fwd(const lo_decoder_args* a, const Dims& d, bool sampling) {
+  const bool bf = bf_views(a, d).on;
+  // dec_step_fwd: every CTA of one grid resident for its barrier (<= 64 rows), the cell on its own mma.sync epilogue, D = C <= 512
+  if (bf && !sampling && g_opt_dec_fuse && g_opt_skinny_mma && !g_opt_fuse_lstm && g_opt_att_pipe && !two_chains(a, d) && d.B <= 64 &&
+      d.C == d.D && d.D <= 512 && d.D % 16 == 0 && d.O1 % 16 == 0 && d.E % 8 == 0 && a->rows_per_img <= 1)
+    return FwdSched::Fused;
+  // dec_cl_fwd: a 16-CTA cluster fits on the device with D = C = 512 and O1 = 3072 (dec_cl_fwd_ok, which also reads dec_cl)
+  if (bf && !sampling && !(g_opt_dbg_skip & 4) && g_opt_skinny_mma && !g_opt_fuse_lstm && g_opt_att_pipe && !two_chains(a, d) &&
+      d.E % 8 == 0 && a->rows_per_img <= 1 && dec_cl_fwd_ok(d.D, d.C, d.O1))
+    return FwdSched::Cluster;
+  return FwdSched::Chains;
+}
+
+static BwdSched pick_bwd(const lo_decoder_args* a, const Dims& d) {
+  const bool bf = bf_views(a, d).on;
+  // dec_step_bwd: K slices of 512 in both GEMMs, C == D, and its whole grid (<= 296 CTAs) resident for the barriers
+  if (bf && g_opt_dec_fuse_bwd && g_opt_skinny_mma && g_opt_att_pipe && !two_chains(a, d) && d.B <= 64 && d.C == d.D &&
+      (d.A + d.C) % 512 == 0 && d.G % 512 == 0 && ((d.C + d.D) / 16) * (d.G / 512) <= 296 && a->rows_per_img <= 1)
+    return BwdSched::Fused;
+  // dec_cl_bwd: a 16-CTA cluster fits on the device with D = C = A = 512 (dec_cl_bwd_ok, which also reads dec_cl_bwd)
+  if (bf && !(g_opt_dbg_skip & 4) && g_opt_skinny_mma && g_opt_att_pipe && !two_chains(a, d) && a->rows_per_img <= 1 &&
+      dec_cl_bwd_ok(d.D, d.C, d.A))
+    return BwdSched::Cluster;
+  return BwdSched::Chains;
+}
+
+// the forward time loop on a fused step kernel, two launches per step: attention(t) -> [gates GEMM + LSTM cell | exchange of h_{t+1} |
+// projection of h_{t+1}], the exchange through a grid barrier (dec_step_fwd, lo_skinny.cu) or within one 16-CTA cluster per block
+// of 16 batch rows (dec_cl_fwd, lo_cluster.cu)
+static int fused_forward(const lo_decoder_args* a, const Dims& d, FwdSched sched, cudaStream_t st) {
+  const BfViews bv = bf_views(a, d);
+  const bool cl = sched == FwdSched::Cluster;
+  unsigned int* bar = (unsigned int*)((char*)a->work + lo_attention_workspace_bytes(d.B, d.C));      // chain-1 region is unused here
+  const int grid = cdiv(d.O1, 16) > cdiv(d.G, 16) ? cdiv(d.O1, 16) : cdiv(d.G, 16);
+  if (!cl) LO_CUDA(cudaMemsetAsync(bar, 0, 16 * 128, st));                                          // 16 arrival counters, one cache line each
+  LO_TRY(skinny_gemm_nt(bv.hall, d.D, (const bf16*)a->wcat1, d.D, a->out1, d.O1, a->bt_host[0], d.O1, d.D, a->bcat1, 1, 0, st));
+  unsigned int epoch = 0;
+  for (int t = 0; t < d.T; t++) {
+    const int nrows = a->bt_host[t];
+    float* o1 = a->out1 + (int64_t)t * d.B * d.O1;
+    if (!(g_opt_dbg_skip & 2))
+      LO_TRY(attention_forward_launch(a->att1, a->enc, a->dt, o1, d.O1, a->w_full, a->alphas + (int64_t)t * d.R, (int64_t)d.T * d.R,
+                                      a->ctx + (int64_t)t * d.B * d.C, o1 + d.A, d.O1, a->gctx + (int64_t)t * d.B * d.C,
+                                      bv.gctx + (int64_t)t * d.B * d.C, nrows, d.R, d.C, a->work, st, 1, 0, att_mask_at(a, t, 0)));
+    DecStepFwd p{};
+    p.gctx = bv.gctx + (int64_t)t * d.B * d.C; p.ld_gctx = d.C;
+    p.wil = bv.wil; p.ld_wil = d.C;
+    const float* dm = (a->has_dropout == 1 && a->dropout_mask) ? a->dropout_mask + (int64_t)t * d.D : nullptr;
+    p.e = lstm_epi(a, d, bv, t, 0, a->caps + t, a->caps_stride, a->hd + (int64_t)t * d.D, (int64_t)d.T * d.D, dm);
+    p.wcat = (const bf16*)a->wcat1; p.ld_wcat = d.D; p.bcat = a->bcat1;
+    const bool more = t + 1 < d.T;
+    p.o1_next = more ? a->out1 + (int64_t)(t + 1) * d.B * d.O1 : nullptr;
+    p.ld_o1 = d.O1; p.N2 = d.O1;
+    p.M = nrows; p.K = d.C;
+    if (cl) {
+      LO_TRY(dec_cl_fwd(p, st));
+    } else {
+      p.bar = bar; p.bar_target = more ? (++epoch) * (unsigned int)grid : 0u;
+      LO_TRY(dec_step_fwd(p, st));
+    }
+  }
+  return LO_OK;
+}
+
+// the backward time loop on a fused step kernel, two launches per step: attention_bwd(t) -> [dh_t += (datt2 | dgate)_t W | LSTM
+// backward of step t-1 | dG_{t-1} W], the phases joined by grid barriers (dec_step_bwd, lo_skinny.cu) or within one 16-CTA cluster per
+// block of 16 batch rows (dec_cl_bwd, lo_cluster.cu).  dal, dal_b, dal_t: the d alpha rows of lo_decoder_backward
+static int fused_backward(const lo_decoder_args* a, const Dims& d, BwdSched sched, const float* dal, int64_t dal_b, int64_t dal_t,
+                          cudaStream_t st) {
+  const BfViews bv = bf_views(a, d);
+  const bool cl = sched == BwdSched::Cluster;
+  unsigned int* bar = (unsigned int*)((char*)a->work + lo_attention_workspace_bytes(d.B, d.C)) + 1024;   // chain-1 region, unused here
+  const unsigned int grid = (unsigned int)(((d.C + d.D) / 16) * (d.G / 512));
+  if (!cl) LO_CUDA(cudaMemsetAsync(bar, 0, 16 * 128, st));
+  unsigned int nb = 0;        // barriers passed so far: one in the first launch, two in every launch that runs the LSTM backward
+  auto fill_common = [&](DecStepBwd& p) {
+    p.wbwd1 = (const bf16*)a->wbwd1; p.ld_w1 = d.G; p.K1 = d.G;      // K1 also sizes dec_step_bwd's grid when phases B/C are skipped
+    p.wbwd2 = (const bf16*)a->wbwd2; p.ld_w2 = d.A + d.C; p.K2 = d.A + d.C;
+    p.dxh = a->dxh; p.C = d.C; p.D = d.D; p.ld_dcat = d.O1;
+    if (!cl) p.bar = bar;
+  };
+  auto fill_bc = [&](DecStepBwd& p, int t) {       // LSTM backward + dG projection of step t
+    p.dhd = a->dhd + (int64_t)t * d.D; p.dhd_stride = (int64_t)d.T * d.D;
+    p.dmask = (a->has_dropout == 1 && a->dropout_mask) ? a->dropout_mask + (int64_t)t * d.D : nullptr;
+    p.dstate = (const unsigned long long*)(a->has_dropout == 2 ? a->dropout_state : nullptr);
+    p.dp = a->dropout_p; p.t_idx = t;
+    p.dc = a->dc; p.gates = a->gates + (int64_t)t * d.B * d.G;
+    p.c_prev = a->call + (int64_t)t * d.B * d.D; p.c_cur = a->call + (int64_t)(t + 1) * d.B * d.D;
+    p.dG = a->dcat + (int64_t)t * d.B * d.O1 + d.A + d.C; p.dG_bf = bv.dcat + (int64_t)t * d.B * d.O1 + d.A + d.C; p.dG_stride = d.O1;
+    p.Mb = a->bt_host[t];
+  };
+  auto launch = [&](DecStepBwd& p, unsigned int barriers) {
+    if (cl) return dec_cl_bwd(p, st);
+    if (barriers) p.bar_target = (nb + 1) * grid;
+    nb += barriers;
+    return dec_step_bwd(p, st);
+  };
+  {
+    DecStepBwd p{};
+    fill_common(p);
+    fill_bc(p, d.T - 1);
+    LO_TRY(launch(p, 1));
+  }
+  for (int t = d.T - 1; t >= 0; t--) {
+    const int nrows = a->bt_host[t];
+    float* dcat_t = a->dcat + (int64_t)t * d.B * d.O1;
+    bf16* dcat_bf_t = bv.dcat + (int64_t)t * d.B * d.O1;
+    const float* o1 = a->out1 + (int64_t)t * d.B * d.O1;
+    AttBwdArgs x{a->att1, a->enc, o1, o1 + d.A, d.O1, a->w_full, a->alphas + (int64_t)t * d.R, (int64_t)d.T * d.R,
+                 a->ctx + (int64_t)t * d.B * d.C, a->dxh, d.C + d.D, dal + (int64_t)t * dal_t, dal_b, a->sreg + t, d.T,
+                 a->de + (int64_t)t * d.R, dcat_t, dcat_t + d.A, d.O1, dcat_bf_t, dcat_bf_t + d.A, a->dctx + (int64_t)t * d.B * d.C,
+                 nrows, d.R, a->work, a->dmean, 0, 0, 0, att_mask_at(a, t, 0)};
+    if (!(cl && (g_opt_dbg_skip & 2))) LO_TRY(attention_bwd_pipe(x, a->dt, d.C, st));     // the cluster loop honours dbg_skip & 2
+    DecStepBwd p{};
+    fill_common(p);
+    p.dcat_a = dcat_bf_t; p.Ma = nrows;
+    if (t > 0) fill_bc(p, t - 1);
+    LO_TRY(launch(p, t > 0 ? 2 : 0));
+  }
+  return LO_OK;
+}
+
+// one beam-search step of either decoder flavour (beam_step_kernel, one CTA per image): the top-k over beam x V log-probs in shared
+// memory, twice that with the diversity penalty (div_on)
+static int beam_select(const float* logits, int V, int beam, int n_img, int t, int max_steps, int64_t end_id, float* logp,
+                       int32_t* finished, int64_t* ids, int64_t* parents, int32_t* fin_hist, int64_t* next_tok, int32_t* parent_rows,
+                       bool div_on, float div_gamma, float div_prob, const float* div_u_t, const uint64_t* div_state, cudaStream_t st) {
+  static bool smem_attr = false;      // the 200 kB opt-in, once per process
+  const size_t smem = (size_t)beam * V * 4 * (div_on ? 2 : 1);
+  if (!smem_attr && smem > 48 * 1024) {
+    LO_CUDA(cudaFuncSetAttribute(beam_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    smem_attr = true;
+  }
+  beam_step_kernel<<<n_img, 256, smem, st>>>(logits, V, beam, t, end_id, logp, finished, ids, parents, fin_hist, next_tok, parent_rows,
+                                             max_steps, div_on ? logf(div_gamma) : 0.f, div_on ? div_prob : 0.f, div_u_t,
+                                             (const unsigned long long*)div_state);
+  LO_LAUNCH_OK();
+  return LO_OK;
 }
 
 }  // namespace lo
@@ -1578,74 +1794,22 @@ int lo_decoder_forward(const lo_decoder_args* a, int with_loss, void* stream) {
     LO_CUDA(cudaEventRecord(g_ev_fork, st));
     LO_CUDA(cudaStreamWaitEvent(g_side, g_ev_fork, 0));
   }
-  const BfViews bvs = bf_views(a, d);
-  const bool fused = bvs.on && !sampling && g_opt_dec_fuse && g_opt_skinny_mma && !g_opt_fuse_lstm && g_opt_att_pipe && nchains == 1 && d.B <= 64 &&
-                     d.C == d.D && d.D <= 512 && d.D % 16 == 0 && d.O1 % 16 == 0 && d.E % 8 == 0 && a->rows_per_img <= 1;
-  const bool clf = bvs.on && !sampling && !fused && !(g_opt_dbg_skip & 4) && g_opt_skinny_mma && !g_opt_fuse_lstm && g_opt_att_pipe && nchains == 1 && d.E % 8 == 0 &&
-                   a->rows_per_img <= 1 && dec_cl_fwd_ok(d.D, d.C, d.O1);
-  if (clf) {
-    // two launches per step: attention(t) -> dec_cl_fwd(t) = [gates GEMM + LSTM cell | cluster all-gather | projection of h_{t+1}],
-    // one 16-CTA cluster per block of 16 batch rows (lo_cluster.cu)
-    LO_TRY(skinny_gemm_nt(bvs.hall, d.D, (const bf16*)a->wcat1, d.D, a->out1, d.O1, a->bt_host[0], d.O1, d.D, a->bcat1, 1, 0, st));
-    for (int t = 0; t < d.T; t++) {
-      const int nrows = a->bt_host[t];
-      float* o1 = a->out1 + (int64_t)t * d.B * d.O1;
-      if (!(g_opt_dbg_skip & 2))
-      LO_TRY(attention_forward_launch(a->att1, a->enc, a->dt, o1, d.O1, a->w_full, a->alphas + (int64_t)t * d.R, (int64_t)d.T * d.R,
-                                      a->ctx + (int64_t)t * d.B * d.C, o1 + d.A, d.O1, a->gctx + (int64_t)t * d.B * d.C,
-                                      bvs.gctx + (int64_t)t * d.B * d.C, nrows, d.R, d.C, a->work, st, 1, 0, att_mask_at(a, t, 0)));
-      DecStepFwd p{};
-      p.gctx = bvs.gctx + (int64_t)t * d.B * d.C; p.ld_gctx = d.C;
-      p.wil = bvs.wil; p.ld_wil = d.C;
-      const float* dm = (a->has_dropout == 1 && a->dropout_mask) ? a->dropout_mask + (int64_t)t * d.D : nullptr;
-      p.e = TcLstmEpi{a->ptab, a->caps + t, a->caps_stride, o1 + d.A + d.C, d.O1, a->call + (int64_t)t * d.B * d.D,
-                      a->gates + (int64_t)t * d.B * d.G, a->call + (int64_t)(t + 1) * d.B * d.D, a->hall + (int64_t)(t + 1) * d.B * d.D,
-                      bvs.hall + (int64_t)(t + 1) * d.B * d.D, a->hd + (int64_t)t * d.D, (int64_t)d.T * d.D, dm, d.D, d.V,
-                      (const unsigned long long*)(a->has_dropout == 2 ? a->dropout_state : nullptr), a->dropout_p, 0, t};
-      p.wcat = (const bf16*)a->wcat1; p.ld_wcat = d.D; p.bcat = a->bcat1;
-      p.o1_next = t + 1 < d.T ? a->out1 + (int64_t)(t + 1) * d.B * d.O1 : nullptr;
-      p.ld_o1 = d.O1; p.N2 = d.O1;
-      p.M = nrows; p.K = d.C;
-      LO_TRY(dec_cl_fwd(p, st));
+  const FwdSched sched = pick_fwd(a, d, sampling);
+  switch (sched) {
+  case FwdSched::Fused:
+  case FwdSched::Cluster:
+    LO_TRY(fused_forward(a, d, sched, st));
+    break;
+  case FwdSched::Chains:
+    for (int chain = 0; chain < nchains; chain++) {
+      cudaStream_t cs = chain == 0 ? st : g_side;
+      for (int t = 0; t < d.T; t++) {
+        const float* dm = (a->has_dropout == 1 && a->dropout_mask) ? a->dropout_mask + (int64_t)t * d.D : nullptr;
+        const Rows rs = chain_rows(a, d, chain, nchains, a->bt_host[t]);
+        LO_TRY(forward_step(a, d, t, rs, a->caps + t, a->caps_stride, a->hd + (int64_t)t * d.D, (int64_t)d.T * d.D, dm, cs));
+      }
     }
-  } else if (fused) {
-    // two launches per step: attention(t) -> dec_step_fwd(t) = [gates GEMM + LSTM cell | grid barrier | projection of h_{t+1}]
-    unsigned int* bar = (unsigned int*)((char*)a->work + lo_attention_workspace_bytes(d.B, d.C));      // chain-1 region is unused here
-    LO_CUDA(cudaMemsetAsync(bar, 0, 16 * 128, st));                                                    // 16 arrival counters, one cache line each
-    const int grid = cdiv(d.O1, 16) > cdiv(d.G, 16) ? cdiv(d.O1, 16) : cdiv(d.G, 16);
-    LO_TRY(skinny_gemm_nt(bvs.hall, d.D, (const bf16*)a->wcat1, d.D, a->out1, d.O1, a->bt_host[0], d.O1, d.D, a->bcat1, 1, 0, st));
-    unsigned int epoch = 0;
-    for (int t = 0; t < d.T; t++) {
-      const int nrows = a->bt_host[t];
-      float* o1 = a->out1 + (int64_t)t * d.B * d.O1;
-      if (!(g_opt_dbg_skip & 2))
-      LO_TRY(attention_forward_launch(a->att1, a->enc, a->dt, o1, d.O1, a->w_full, a->alphas + (int64_t)t * d.R, (int64_t)d.T * d.R,
-                                      a->ctx + (int64_t)t * d.B * d.C, o1 + d.A, d.O1, a->gctx + (int64_t)t * d.B * d.C,
-                                      bvs.gctx + (int64_t)t * d.B * d.C, nrows, d.R, d.C, a->work, st, 1, 0, att_mask_at(a, t, 0)));
-      DecStepFwd p{};
-      p.gctx = bvs.gctx + (int64_t)t * d.B * d.C; p.ld_gctx = d.C;
-      p.wil = bvs.wil; p.ld_wil = d.C;
-      const float* dm = (a->has_dropout == 1 && a->dropout_mask) ? a->dropout_mask + (int64_t)t * d.D : nullptr;
-      p.e = TcLstmEpi{a->ptab, a->caps + t, a->caps_stride, o1 + d.A + d.C, d.O1, a->call + (int64_t)t * d.B * d.D,
-                      a->gates + (int64_t)t * d.B * d.G, a->call + (int64_t)(t + 1) * d.B * d.D, a->hall + (int64_t)(t + 1) * d.B * d.D,
-                      bvs.hall + (int64_t)(t + 1) * d.B * d.D, a->hd + (int64_t)t * d.D, (int64_t)d.T * d.D, dm, d.D, d.V,
-                      (const unsigned long long*)(a->has_dropout == 2 ? a->dropout_state : nullptr), a->dropout_p, 0, t};
-      p.wcat = (const bf16*)a->wcat1; p.ld_wcat = d.D; p.bcat = a->bcat1;
-      const bool more = t + 1 < d.T;
-      p.o1_next = more ? a->out1 + (int64_t)(t + 1) * d.B * d.O1 : nullptr;
-      p.ld_o1 = d.O1; p.N2 = d.O1;
-      p.bar = bar; p.bar_target = more ? (++epoch) * (unsigned int)grid : 0u;
-      p.M = nrows; p.K = d.C;
-      LO_TRY(dec_step_fwd(p, st));
-    }
-  } else
-  for (int chain = 0; chain < nchains; chain++) {
-    cudaStream_t cs = chain == 0 ? st : g_side;
-    for (int t = 0; t < d.T; t++) {
-      const float* dm = (a->has_dropout == 1 && a->dropout_mask) ? a->dropout_mask + (int64_t)t * d.D : nullptr;
-      const Rows rs = chain_rows(a, d, chain, nchains, a->bt_host[t]);
-      LO_TRY(forward_step(a, d, t, rs, a->caps + t, a->caps_stride, a->hd + (int64_t)t * d.D, (int64_t)d.T * d.D, dm, cs));
-    }
+    break;
   }
   if (nchains == 2) {
     LO_CUDA(cudaEventRecord(g_ev_join, g_side));
@@ -1665,10 +1829,8 @@ int lo_decoder_forward(const lo_decoder_args* a, int with_loss, void* stream) {
   } else {
     LO_TRY(gemm_nt(a->hd, LO_F32, d.D, a->w_fc, a->dt, d.D, a->logits, LO_F32, d.Vl, d.B * d.T, d.V, d.D, a->b_fc, 0, 0, LO_IMPL_SIMT, st));
   }
-  if (ragged) {
-    // rows that stopped decoding keep zeros in `predictions` (seq2seq_torch.py:301): re-zero what the GEMM wrote (bias)
-    // handled by the CE kernel (ignores them) and by the Python side for the returned tensor.
-  }
+  // rows that stopped decoding keep zeros in `predictions` (seq2seq_torch.py:301): what the GEMM wrote there (bias) is ignored by
+  // the CE kernel and handled by the Python side for the returned tensor
   if (with_loss) {
     long nvalid = 0;
     for (int t = 0; t < d.T; t++) nvalid += a->bt_host[t];
@@ -1717,7 +1879,6 @@ int lo_decoder_backward(const lo_decoder_args* a, void* stream) {
   const Dims d = dims(a);
   const int dt = a->dt;
   const bool ragged = a->bt_host[d.T - 1] < d.B;
-  const int ns = att_splits(d.B);
   const int64_t BT = (int64_t)d.B * d.T;
   // d alpha rows: the regulariser's (one row per b), the caller's (one per (b, t)), or none (generic mode without dalpha_ext)
   const bool generic = a->dpred_ext != nullptr;
@@ -1774,176 +1935,20 @@ int lo_decoder_backward(const lo_decoder_args* a, void* stream) {
     LO_CUDA(cudaEventRecord(g_ev_fork, st));
     LO_CUDA(cudaStreamWaitEvent(g_side, g_ev_fork, 0));
   }
-  const cudaStream_t st_main = st;
-  const bool fusedb = bv.on && g_opt_dec_fuse_bwd && g_opt_skinny_mma && g_opt_att_pipe && nchains == 1 && d.B <= 64 && d.C == d.D &&
-                      (d.A + d.C) % 512 == 0 && d.G % 512 == 0 && ((d.C + d.D) / 16) * (d.G / 512) <= 296 && a->rows_per_img <= 1;
-  const bool clb = bv.on && !fusedb && !(g_opt_dbg_skip & 4) && g_opt_skinny_mma && g_opt_att_pipe && nchains == 1 && a->rows_per_img <= 1 &&
-                   dec_cl_bwd_ok(d.D, d.C, d.A);
-  if (clb) {
-    // two launches per step: attention_bwd(t) -> dec_cl_bwd = [dh_t += (datt2|dgate)_t W | LSTM bwd (t-1) | cluster all-gather | dG_{t-1} W]
-    auto fill_bc = [&](DecStepBwd& p, int t) {       // LSTM backward + dG projection of step t
-      p.dhd = a->dhd + (int64_t)t * d.D; p.dhd_stride = (int64_t)d.T * d.D;
-      p.dmask = (a->has_dropout == 1 && a->dropout_mask) ? a->dropout_mask + (int64_t)t * d.D : nullptr;
-      p.dstate = (const unsigned long long*)(a->has_dropout == 2 ? a->dropout_state : nullptr);
-      p.dp = a->dropout_p; p.t_idx = t;
-      p.dc = a->dc; p.gates = a->gates + (int64_t)t * d.B * d.G;
-      p.c_prev = a->call + (int64_t)t * d.B * d.D; p.c_cur = a->call + (int64_t)(t + 1) * d.B * d.D;
-      p.dG = a->dcat + (int64_t)t * d.B * d.O1 + d.A + d.C; p.dG_bf = bv.dcat + (int64_t)t * d.B * d.O1 + d.A + d.C; p.dG_stride = d.O1;
-      p.Mb = a->bt_host[t];
-    };
-    auto fill_common = [&](DecStepBwd& p) {
-      p.wbwd1 = (const bf16*)a->wbwd1; p.ld_w1 = d.G; p.K1 = d.G;
-      p.wbwd2 = (const bf16*)a->wbwd2; p.ld_w2 = d.A + d.C; p.K2 = d.A + d.C;
-      p.dxh = a->dxh; p.C = d.C; p.D = d.D; p.ld_dcat = d.O1;
-    };
-    {
-      DecStepBwd p{};
-      fill_common(p);
-      fill_bc(p, d.T - 1);
-      LO_TRY(dec_cl_bwd(p, st));
+  const BwdSched sched = pick_bwd(a, d);
+  switch (sched) {
+  case BwdSched::Fused:
+  case BwdSched::Cluster:
+    LO_TRY(fused_backward(a, d, sched, dal, dal_b, dal_t, st));
+    break;
+  case BwdSched::Chains:
+    for (int chain = 0; chain < nchains; chain++) {
+      cudaStream_t cs = chain == 0 ? st : g_side;
+      for (int t = d.T - 1; t >= 0; t--)
+        LO_TRY(backward_step(a, d, t, chain_rows(a, d, chain, nchains, a->bt_host[t]), dal, dal_b, dal_t, cs));
     }
-    for (int t = d.T - 1; t >= 0; t--) {
-      const int nrows = a->bt_host[t];
-      float* dcat_t = a->dcat + (int64_t)t * d.B * d.O1;
-      bf16* dcat_bf_t = bv.dcat + (int64_t)t * d.B * d.O1;
-      const float* o1 = a->out1 + (int64_t)t * d.B * d.O1;
-      AttBwdArgs x{a->att1, a->enc, o1, o1 + d.A, d.O1, a->w_full, a->alphas + (int64_t)t * d.R, (int64_t)d.T * d.R,
-                   a->ctx + (int64_t)t * d.B * d.C, a->dxh, d.C + d.D, dal + (int64_t)t * dal_t, dal_b, a->sreg + t, d.T,
-                   a->de + (int64_t)t * d.R, dcat_t, dcat_t + d.A, d.O1, dcat_bf_t, dcat_bf_t + d.A, a->dctx + (int64_t)t * d.B * d.C,
-                   nrows, d.R, a->work, a->dmean, 0, 0, 0, att_mask_at(a, t, 0)};
-      if (!(g_opt_dbg_skip & 2)) LO_TRY(attention_bwd_pipe(x, dt, d.C, st));
-      DecStepBwd p{};
-      fill_common(p);
-      p.dcat_a = dcat_bf_t; p.Ma = nrows;
-      if (t > 0) fill_bc(p, t - 1);
-      LO_TRY(dec_cl_bwd(p, st));
-    }
-  } else if (fusedb) {
-    // two launches per step: attention_bwd(t) -> dec_step_bwd = [dh += (datt2|dgate) W | barrier | LSTM bwd (t-1) | barrier | dG W]
-    unsigned int* bar = (unsigned int*)((char*)a->work + lo_attention_workspace_bytes(d.B, d.C)) + 1024;   // chain-1 region, unused here
-    LO_CUDA(cudaMemsetAsync(bar, 0, 16 * 128, st));
-    const unsigned int grid = (unsigned int)(((d.C + d.D) / 16) * (d.G / 512));
-    unsigned int nb = 0;
-    auto fill_bc = [&](DecStepBwd& p, int t) {       // phases B/C for step t
-      p.dhd = a->dhd + (int64_t)t * d.D; p.dhd_stride = (int64_t)d.T * d.D;
-      p.dmask = (a->has_dropout == 1 && a->dropout_mask) ? a->dropout_mask + (int64_t)t * d.D : nullptr;
-      p.dstate = (const unsigned long long*)(a->has_dropout == 2 ? a->dropout_state : nullptr);
-      p.dp = a->dropout_p; p.t_idx = t;
-      p.dc = a->dc; p.gates = a->gates + (int64_t)t * d.B * d.G;
-      p.c_prev = a->call + (int64_t)t * d.B * d.D; p.c_cur = a->call + (int64_t)(t + 1) * d.B * d.D;
-      p.dG = a->dcat + (int64_t)t * d.B * d.O1 + d.A + d.C; p.dG_bf = bv.dcat + (int64_t)t * d.B * d.O1 + d.A + d.C; p.dG_stride = d.O1;
-      p.wbwd1 = (const bf16*)a->wbwd1; p.ld_w1 = d.G; p.K1 = d.G; p.Mb = a->bt_host[t];
-    };
-    {
-      DecStepBwd p{};
-      fill_bc(p, d.T - 1);
-      p.wbwd2 = (const bf16*)a->wbwd2; p.ld_w2 = d.A + d.C; p.K2 = d.A + d.C;
-      p.dxh = a->dxh; p.C = d.C; p.D = d.D; p.bar = bar; p.bar_target = (nb + 1) * grid;
-      nb += 1;
-      LO_TRY(dec_step_bwd(p, st));
-    }
-    for (int t = d.T - 1; t >= 0; t--) {
-      const int nrows = a->bt_host[t];
-      float* dcat_t = a->dcat + (int64_t)t * d.B * d.O1;
-      bf16* dcat_bf_t = bv.dcat + (int64_t)t * d.B * d.O1;
-      const float* o1 = a->out1 + (int64_t)t * d.B * d.O1;
-      AttBwdArgs x{a->att1, a->enc, o1, o1 + d.A, d.O1, a->w_full, a->alphas + (int64_t)t * d.R, (int64_t)d.T * d.R,
-                   a->ctx + (int64_t)t * d.B * d.C, a->dxh, d.C + d.D, dal + (int64_t)t * dal_t, dal_b, a->sreg + t, d.T,
-                   a->de + (int64_t)t * d.R, dcat_t, dcat_t + d.A, d.O1, dcat_bf_t, dcat_bf_t + d.A, a->dctx + (int64_t)t * d.B * d.C,
-                   nrows, d.R, a->work, a->dmean, 0, 0, 0, att_mask_at(a, t, 0)};
-      LO_TRY(attention_bwd_pipe(x, dt, d.C, st));
-      DecStepBwd p{};
-      p.dcat_a = dcat_bf_t; p.ld_dcat = d.O1; p.wbwd2 = (const bf16*)a->wbwd2; p.ld_w2 = d.A + d.C; p.K2 = d.A + d.C; p.Ma = nrows;
-      p.dxh = a->dxh; p.C = d.C; p.D = d.D; p.bar = bar;
-      p.K1 = d.G;                                  // grid size (phase C tiling) even when phases B/C are skipped
-      if (t > 0) {
-        fill_bc(p, t - 1);
-        p.bar_target = (nb + 1) * grid;
-        nb += 2;
-      }
-      LO_TRY(dec_step_bwd(p, st));
-    }
-  } else
-  for (int chain = 0; chain < nchains; chain++) {
-   st = chain == 0 ? st_main : g_side;
-   for (int t = d.T - 1; t >= 0; t--) {
-    const Rows rs = chain_rows(a, d, chain, nchains, a->bt_host[t]);
-    const int nrows = rs.nrows;
-    const int64_t r0 = rs.row0;
-    if (nrows <= 0) continue;
-    const size_t es = dt == LO_F32 ? 4 : 2;
-    float* dcat_t = a->dcat + ((int64_t)t * d.B + r0) * d.O1;
-    bf16* dcat_bf_t = bv.on ? bv.dcat + ((int64_t)t * d.B + r0) * d.O1 : nullptr;
-    const float* o1 = a->out1 + ((int64_t)t * d.B + r0) * d.O1;
-    float* dxh = a->dxh + r0 * (d.C + d.D);
-    const float* dmul = (a->has_dropout == 1 && a->dropout_mask) ? a->dropout_mask + (int64_t)t * d.D + r0 * d.T * d.D : nullptr;
-    if (!(g_opt_dbg_skip & 4))
-    LO_CUDA(launch_pdl(lstm_pw_bwd_kernel, dim3(cdiv((long)nrows * d.D, 256)), dim3(256), (size_t)0, st,
-                       (const float*)(a->dhd + (int64_t)t * d.D + r0 * d.T * d.D), (int64_t)d.T * d.D, dmul, (const float*)(dxh + d.C),
-                       (int64_t)(d.C + d.D), a->dc + r0 * d.D, (const float*)(a->gates + ((int64_t)t * d.B + r0) * d.G),
-                       (const float*)(a->call + ((int64_t)t * d.B + r0) * d.D),
-                       (const float*)(a->call + ((int64_t)(t + 1) * d.B + r0) * d.D), dcat_t + d.A + d.C, (int64_t)d.O1,
-                       bv.on ? dcat_bf_t + d.A + d.C : (bf16*)nullptr, bv.on ? dxh : (float*)nullptr, d.C, nrows, d.D,
-                       (const unsigned long long*)(a->has_dropout == 2 ? a->dropout_state : nullptr), a->dropout_p, (int)r0, t));
-    LO_LAUNCH_OK();
-    // [dgctx | dh_prev] = dG @ [W_ih[:, E:] | W_hh]
-    if (g_opt_dbg_skip & 4) {
-    } else if (bv.on && g_opt_skinny_mma && nrows <= 64) {
-      LO_TRY(skinny_gemm_nt(dcat_bf_t + d.A + d.C, d.O1, (const bf16*)a->wbwd1, d.G, dxh, d.C + d.D, nrows, d.C + d.D, d.G, nullptr, 4, 1,
-                            st));
-    } else if (bv.on) {
-      LO_TRY(tc_gemm_nt_ex(dcat_bf_t + d.A + d.C, d.O1, (const bf16*)a->wbwd1, d.G, dxh, LO_F32, d.C + d.D, nrows, d.C + d.D, d.G,
-                           nullptr, 0, 0, 4, 1, 1, st));
-    } else {
-      LO_TRY(gemm_nt(dcat_t + d.A + d.C, LO_F32, d.O1, a->wbwd1, dt, d.G, dxh, LO_F32, d.C + d.D, nrows, d.C + d.D, d.G, nullptr, 0,
-                     0, LO_IMPL_SIMT, st));
-    }
-    const char* att1 = (const char*)a->att1 + (size_t)r0 * d.R * d.A * es;
-    const char* enc = (const char*)a->enc + (size_t)r0 * d.R * d.C * es;
-    const float* alpha_t = a->alphas + (r0 * d.T + t) * d.R;
-    const float* ctx_t = a->ctx + ((int64_t)t * d.B + r0) * d.C;
-    const float* dal_t_ptr = dal + (int64_t)t * dal_t + r0 * dal_b;
-    const float* sreg_t = a->sreg + r0 * d.T + t;
-    float* de_t = a->de + (r0 * d.T + t) * d.R;
-    float* dctx_t = a->dctx + ((int64_t)t * d.B + r0) * d.C;
-    if (g_opt_dbg_skip & 2) {
-    } else if (g_opt_att_pipe) {
-      AttBwdArgs x{att1, enc, o1, o1 + d.A, d.O1, a->w_full, alpha_t, (int64_t)d.T * d.R, ctx_t, dxh, d.C + d.D, dal_t_ptr, dal_b, sreg_t,
-                   d.T, de_t, dcat_t, dcat_t + d.A, d.O1, dcat_bf_t, dcat_bf_t ? dcat_bf_t + d.A : nullptr, dctx_t, nrows, d.R, rs.work,
-                   a->dmean + r0 * d.A, rs.nsplit, 0, 0, att_mask_at(a, t, r0)};
-      LO_TRY(attention_bwd_pipe(x, dt, d.C, st));
-    } else {
-    int* cnt_c = (int*)rs.work;
-    float* part_c = (float*)((char*)rs.work + att_partials_offset(nrows));
-    dim3 grid(ns, nrows);
-#define LO_ATT_BWD(TY_, NV)                                                                                                       \
-  attention_bwd_kernel<TY_, NV><<<grid, LO_ATT_THREADS, 0, st>>>(                                                                 \
-      (const TY_*)att1, (const TY_*)enc, o1, o1 + d.A, d.O1, a->w_full, alpha_t, (int64_t)d.T * d.R, ctx_t, dxh, d.C + d.D, dal_t_ptr, \
-      dal_b, sreg_t, d.T, de_t, dcat_t, dcat_t + d.A, d.O1, dcat_bf_t, dcat_bf_t ? dcat_bf_t + d.A : nullptr, dctx_t, d.R, ns, cnt_c,  \
-      part_c)
-    if (dt == LO_F32) {
-      if (d.C == 256) LO_ATT_BWD(float, 1); else if (d.C == 512) LO_ATT_BWD(float, 2); else LO_ATT_BWD(float, 4);
-    } else {
-      if (d.C == 256) LO_ATT_BWD(bf16, 1); else if (d.C == 512) LO_ATT_BWD(bf16, 2); else LO_ATT_BWD(bf16, 4);
-    }
-#undef LO_ATT_BWD
-    LO_LAUNCH_OK();
-    }
-    // dh_prev += [datt2 | dgate_pre] @ [W_d ; W_beta]
-    if (g_opt_dbg_skip & 4) {
-    } else if (bv.on && g_opt_skinny_mma && nrows <= 64) {
-      LO_TRY(skinny_gemm_nt(dcat_bf_t, d.O1, (const bf16*)a->wbwd2, d.A + d.C, dxh + d.C, d.C + d.D, nrows, d.D, d.A + d.C, nullptr, 4, 1,
-                            st));
-    } else if (bv.on) {
-      LO_TRY(tc_gemm_nt_ex(dcat_bf_t, d.O1, (const bf16*)a->wbwd2, d.A + d.C, dxh + d.C, LO_F32, d.C + d.D, nrows, d.D, d.A + d.C,
-                           nullptr, 0, 0, 4, 1, 1, st));
-    } else {
-      LO_TRY(gemm_nt(dcat_t, LO_F32, d.O1, a->wbwd2, dt, d.A + d.C, dxh + d.C, LO_F32, d.C + d.D, nrows, d.D, d.A + d.C, nullptr, 1,
-                     0, LO_IMPL_SIMT, st));
-    }
-   }
+    break;
   }
-  st = st_main;
   if (nchains == 2) {
     LO_CUDA(cudaEventRecord(g_ev_join, g_side));
     LO_CUDA(cudaStreamWaitEvent(st, g_ev_join, 0));
@@ -2119,12 +2124,8 @@ int lo_decoder_greedy_hist(const lo_decoder_args* a, int64_t start_id, int64_t e
   for (int t = 0; t < max_steps; t++) {
     LO_TRY(forward_step(a, d, t, Rows{0, d.B, a->work, 0, a->reg_off ? &rg : nullptr}, next_tok, 1, nullptr, 0, nullptr, st));
     // logits_t = fc(h_t)   (no dropout at decode time)
-    if (bvg.on)      // bf16 mirror of h_t: mma.sync kernel for <= 64 rows (the dispatcher falls back to CUDA cores otherwise)
-      LO_TRY(gemm_nt(bvg.hall + (int64_t)(t + 1) * d.B * d.D, LO_BF16, d.D, a->w_fc, LO_BF16, d.D, a->logits, LO_F32, d.V, d.B, d.V, d.D,
-                     a->b_fc, 0, 0, LO_IMPL_TC, st));
-    else
-      LO_TRY(gemm_nt(a->hall + (int64_t)(t + 1) * d.B * d.D, LO_F32, d.D, a->w_fc, a->dt, d.D, a->logits, LO_F32, d.V, d.B, d.V, d.D,
-                     a->b_fc, 0, 0, LO_IMPL_SIMT, st));
+    const int64_t h_t = (int64_t)(t + 1) * d.B * d.D;
+    LO_TRY(head_nt(a, bvg.on, a->hall + h_t, bvg.on ? bvg.hall + h_t : nullptr, d.D, a->logits, d.V, d.B, st));
     argmax_kernel<<<cdiv(d.B, 8), 256, 0, st>>>(a->logits, d.V, tokens + t, max_steps, next_tok, finished, end_id, d.B);
     LO_LAUNCH_OK();
     if (fin_hist) {
@@ -2173,26 +2174,13 @@ int lo_decoder_beam_div(const lo_decoder_args* a, int64_t start_id, int64_t end_
   AttRagged rg = ragged_of(a);
   if (a->reg_off) LO_TRY(attention_ragged_prepare(rg, d.B, beam, st));
   const BfViews bv = bf_views(a, d);
-  const size_t smem = (size_t)beam * d.V * 4 * (div_on ? 2 : 1);
-  static bool attr = false;
-  if (!attr && smem > 48 * 1024) {
-    LO_CUDA(cudaFuncSetAttribute(beam_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    attr = true;
-  }
   for (int t = 0; t < max_steps; t++) {
     LO_TRY(forward_step(a, d, t, Rows{0, d.B, a->work, 0, a->reg_off ? &rg : nullptr}, next_tok, 1, nullptr, 0, nullptr, st));
     float* h_new = a->hall + (int64_t)(t + 1) * d.B * d.D;
     float* c_new = a->call + (int64_t)(t + 1) * d.B * d.D;
-    if (bv.on)       // bf16 mirror of h_t -> mma.sync kernel (row blocks of 64), CUDA cores otherwise
-      LO_TRY(gemm_nt(bv.hall + (int64_t)(t + 1) * d.B * d.D, LO_BF16, d.D, a->w_fc, LO_BF16, d.D, a->logits, LO_F32, d.V, d.B, d.V, d.D,
-                     a->b_fc, 0, 0, LO_IMPL_TC, st));
-    else
-      LO_TRY(gemm_nt(h_new, LO_F32, d.D, a->w_fc, a->dt, d.D, a->logits, LO_F32, d.V, d.B, d.V, d.D, a->b_fc, 0, 0, LO_IMPL_SIMT, st));
-    beam_step_kernel<<<n_img, 256, smem, st>>>(a->logits, d.V, beam, t, end_id, logp, finished, ids, parents, fin_hist, next_tok,
-                                               parent_rows, max_steps, div_on ? logf(div_gamma) : 0.f, div_on ? div_prob : 0.f,
-                                               div_u ? div_u + (int64_t)t * d.B * d.V : (const float*)nullptr,
-                                               (const unsigned long long*)div_state);
-    LO_LAUNCH_OK();
+    LO_TRY(head_nt(a, bv.on, h_new, bv.on ? bv.hall + (int64_t)(t + 1) * d.B * d.D : nullptr, d.D, a->logits, d.V, d.B, st));
+    LO_TRY(beam_select(a->logits, d.V, beam, n_img, t, max_steps, end_id, logp, finished, ids, parents, fin_hist, next_tok, parent_rows,
+                       div_on, div_gamma, div_prob, div_u ? div_u + (int64_t)t * d.B * d.V : nullptr, div_state, st));
     // reorder the recurrent state by parents (through gtmp as a temporary)
     gather_rows_kernel<<<cdiv((long)d.B * d.D, 256), 256, 0, st>>>(h_new, parent_rows, a->gtmp, d.B, d.D);
     LO_LAUNCH_OK();

@@ -576,7 +576,6 @@ int lo_tfdec_backward(const lo_tfdec_args* a, void* stream) {
   const TfDims d = tf_dims(a);
   const TfWs w = tf_carve(a);
   const int dt = a->dt;
-  const size_t es = dt == LO_F32 ? 4 : 2;
   const int TB = d.T * d.B;
   const dim3 tb(32, 8);
   // generic mode: d logits from the caller (batch-major -> the time-major workspace rows; every position carries gradient), and
@@ -696,7 +695,6 @@ int lo_tfdec_backward(const lo_tfdec_args* a, void* stream) {
     add_rowbcast_kernel<<<LO_NUM_SMS * 8, 256, 0, st>>>(a->denc, w.dmean, d.R, d.C, 1.0f / (float)d.R, total);
     LO_LAUNCH_OK();
   }
-  (void)es;
   return LO_OK;
 }
 
@@ -746,16 +744,12 @@ int lo_tfdec_beam_div(const lo_tfdec_args* a, int64_t end_id, int max_steps, int
   if (a->reg_off) LO_TRY(attention_ragged_prepare(rg, d.B, beam, st));
   const size_t smem = (size_t)beam * d.V * 4 * (div_on ? 2 : 1);
   LO_CHECK_ARG(smem <= 200 * 1024, "beam*V too large for the shared-memory top-k");
-  if (smem > 48 * 1024) LO_CUDA(cudaFuncSetAttribute(beam_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
   for (int t = 0; t < max_steps; t++) {
     LO_TRY(tf_step(a, d, w, t, t == 0 ? nullptr : w.next_tok, 1, st, a->reg_off ? &rg : nullptr));
     const int64_t rown = (int64_t)(t + 1) * d.B;
     LO_TRY(tf_logits(a, d, w, rown, d.B, a->logits, d.V, st));
-    beam_step_kernel<<<d.nimg, 256, smem, st>>>(a->logits, d.V, beam, t, end_id, logp, w.finished, ids, parents, fin_hist, w.next_tok,
-                                                w.parent_rows, max_steps, div_on ? logf(div_gamma) : 0.f, div_on ? div_prob : 0.f,
-                                                div_u ? div_u + (int64_t)t * d.B * d.V : (const float*)nullptr,
-                                                (const unsigned long long*)div_state);
-    LO_LAUNCH_OK();
+    LO_TRY(beam_select(a->logits, d.V, beam, d.nimg, t, max_steps, end_id, logp, w.finished, ids, parents, fin_hist, w.next_tok,
+                       w.parent_rows, div_on, div_gamma, div_prob, div_u ? div_u + (int64_t)t * d.B * d.V : nullptr, div_state, st));
     // reorder the cell state (c, h, o) by parents (gather_helper, beam_search_decoder_cell.py:370-391)
     tf_gather_rows_kernel<<<cdiv((long)d.B * d.XH, 256), 256, 0, st>>>(w.xh + rown * d.XH, w.parent_rows, w.gtmp,
                                                                        w.xh_bf ? w.xh_bf + rown * d.XH : nullptr, d.B, d.XH);

@@ -1018,13 +1018,15 @@ __global__ void __launch_bounds__(256) beam_step_kernel(const float* __restrict_
   }
 }
 
-// dst[r][:] = src[rows[r]][:]  (state gather by parents, gather_helper beam_search_decoder_cell.py:370-391)
-__global__ void gather_rows_kernel(const float* __restrict__ src, const int32_t* __restrict__ rows, float* __restrict__ dst, int n,
-                                   int D) {
+// dst[r][:] = src[rows[r]][:] (+ bf16 mirror of dst)  (state gather by parents, gather_helper beam_search_decoder_cell.py:370-391)
+__global__ void gather_rows_kernel(const float* __restrict__ src, const int32_t* __restrict__ rows, float* __restrict__ dst,
+                                   bf16* __restrict__ dst_bf, int n, int W) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= n * D) return;
-  const int r = idx / D, j = idx % D;
-  dst[idx] = src[(int64_t)rows[r] * D + j];
+  if (idx >= n * W) return;
+  const int r = idx / W, j = idx % W;
+  const float v = src[(int64_t)rows[r] * W + j];
+  dst[idx] = v;
+  if (dst_bf) dst_bf[idx] = __float2bfloat16_rn(v);
 }
 
 __global__ void fin_hist_kernel(const int32_t* __restrict__ finished, int32_t* __restrict__ hist, int64_t stride, int B) {
@@ -1127,7 +1129,8 @@ static int check_reg_off(const int32_t* reg_off, const int32_t* reg_off_host, in
   }
   return LO_OK;
 }
-static int check_reg_off(const lo_decoder_args* a, bool decode) {
+template <class Args>            // lo_decoder_args or lo_tfdec_args
+static int check_reg_off(const Args* a, bool decode) {
   return check_reg_off(a->reg_off, a->reg_off_host, a->B, a->rows_per_img, a->R, decode);
 }
 // the ragged attention state of a decode call: map in the second attention region of `work` (the decode loop runs one row chain)
@@ -1625,6 +1628,117 @@ static int beam_select(const float* logits, int V, int beam, int n_img, int t, i
   return LO_OK;
 }
 
+// ------------------------------------------------------------------------------------------------ decode loops of both flavours
+// A flavour F hands the loops F::c: the step's logits [B][V], device scratch of B rows each and the ragged attention state
+// (rg.reg_off NULL: every image has R regions) of rpi rows per image; F::prologue(st); F::step(t, st): the cell step fed next_tok
+// (or the start token), then the head into logits; and for beam search F::reorder(t, st): the state of step t gathered by parent_rows.
+struct DecodeCtx {
+  int B, T, V, rpi;
+  const float* logits;
+  int64_t* next_tok;
+  int32_t *finished, *parent_rows;
+  AttRagged rg;
+  const AttRagged* ragged() const { return rg.reg_off ? &rg : nullptr; }
+};
+
+struct BeamArgs {
+  int beam;
+  float div_gamma, div_prob;
+  const float* div_u;            // [max_steps][B][V] injected uniforms, or NULL (Philox from div_state)
+  const uint64_t* div_state;
+  bool div_on() const { return !(div_gamma == 1.f || div_prob == 0.f); }        // beam_search_decoder_cell.py:270-273
+};
+
+// the decode arguments both flavours check alike (bm NULL: greedy decode), before anything is enqueued; then everything before
+// step 0: finished = 0, log-probs = 0 (beam search, :106-107), the prologue, the ragged CTA map
+template <class F>
+static int decode_begin(F& f, int max_steps, bool outputs, const BeamArgs* bm, float* logp, cudaStream_t st) {
+  DecodeCtx& c = f.c;
+  LO_CHECK_ARG(outputs && max_steps > 0 && max_steps <= c.T, "outputs / max_steps (<= T capacity)");
+  if (bm) {
+    LO_CHECK_ARG(!bm->div_on() || (bm->div_gamma > 0.f && (bm->div_u || bm->div_state)),
+                 "diversity penalty needs gamma > 0 and div_u or div_state");
+    LO_CHECK_ARG(bm->beam >= 1 && bm->beam <= LO_BEAM_MAX && c.B % bm->beam == 0, "1 <= beam (rows_per_img) <= 16, B % beam == 0");
+    LO_CHECK_ARG((size_t)bm->beam * c.V * 4 * (bm->div_on() ? 2 : 1) <= 200 * 1024, "beam*V too large for the shared-memory top-k");
+  }
+  LO_CUDA(cudaMemsetAsync(c.finished, 0, (size_t)c.B * 4, st));
+  if (logp) LO_CUDA(cudaMemsetAsync(logp, 0, (size_t)c.B * 4, st));
+  LO_TRY(f.prologue(st));
+  if (c.rg.reg_off) LO_TRY(attention_ragged_prepare(c.rg, c.B, c.rpi, st));
+  return LO_OK;
+}
+
+template <class F>
+static int greedy_loop(F& f, int64_t end_id, int max_steps, int64_t* tokens, int32_t* fin_hist, cudaStream_t st) {
+  const DecodeCtx& c = f.c;
+  LO_TRY(decode_begin(f, max_steps, tokens && c.finished, nullptr, nullptr, st));
+  for (int t = 0; t < max_steps; t++) {
+    LO_TRY(f.step(t, st));
+    argmax_kernel<<<cdiv(c.B, 8), 256, 0, st>>>(c.logits, c.V, tokens + t, max_steps, c.next_tok, c.finished, end_id, c.B);
+    LO_LAUNCH_OK();
+    if (fin_hist) {
+      fin_hist_kernel<<<cdiv(c.B, 128), 128, 0, st>>>(c.finished, fin_hist + t, max_steps, c.B);
+      LO_LAUNCH_OK();
+    }
+  }
+  return LO_OK;
+}
+
+// bm.beam == c.rpi once decode_begin has checked it
+template <class F>
+static int beam_loop(F& f, const BeamArgs& bm, int64_t end_id, int max_steps, int64_t* ids, int64_t* parents, int32_t* fin_hist,
+                     float* logp, cudaStream_t st) {
+  const DecodeCtx& c = f.c;
+  LO_TRY(decode_begin(f, max_steps, ids && parents && fin_hist && logp, &bm, logp, st));
+  for (int t = 0; t < max_steps; t++) {
+    LO_TRY(f.step(t, st));
+    LO_TRY(beam_select(c.logits, c.V, bm.beam, c.B / bm.beam, t, max_steps, end_id, logp, c.finished, ids, parents, fin_hist,
+                       c.next_tok, c.parent_rows, bm.div_on(), bm.div_gamma, bm.div_prob,
+                       bm.div_u ? bm.div_u + (int64_t)t * c.B * c.V : nullptr, bm.div_state, st));
+    LO_TRY(f.reorder(t, st));
+  }
+  return LO_OK;
+}
+
+// the torch flavour in the decode loops: next tokens (int64 [B], start_id before step 0) in sreg ([B][>= 2] floats); greedy
+// decode's `finished` comes from the caller, beam search keeps finished and the parent rows (int32 [B] each) in row_loss
+struct TorchDecode {
+  const lo_decoder_args* a;
+  int64_t start_id;
+  Dims d;
+  BfViews bv;
+  DecodeCtx c;
+  TorchDecode(const lo_decoder_args* a_, int64_t start, int32_t* finished, int32_t* parent_rows)
+      : a(a_), start_id(start), d(dims(a_)), bv(bf_views(a_, d)),
+        c{d.B, d.T, d.V, a_->rows_per_img > 1 ? a_->rows_per_img : 1, a_->logits, (int64_t*)a_->sreg, finished, parent_rows,
+          ragged_of(a_)} {}
+  int prologue(cudaStream_t st) {
+    fill_i64_kernel<<<cdiv(d.B, 128), 128, 0, st>>>(c.next_tok, start_id, d.B);
+    LO_LAUNCH_OK();
+    return forward_prologue(a, d, st);
+  }
+  // the cell step, then logits_t = fc(h_t)   (no dropout at decode time)
+  int step(int t, cudaStream_t st) {
+    LO_TRY(forward_step(a, d, t, Rows{0, d.B, a->work, 0, c.ragged()}, c.next_tok, 1, nullptr, 0, nullptr, st));
+    const int64_t h_t = (int64_t)(t + 1) * d.B * d.D;
+    return head_nt(a, bv.on, a->hall + h_t, bv.on ? bv.hall + h_t : nullptr, d.D, a->logits, d.V, d.B, st);
+  }
+  // h and c of step t by parents (through gtmp as a temporary), then the bf16 copy of h
+  int reorder(int t, cudaStream_t st) {
+    const int64_t n = (int64_t)d.B * d.D;
+    float* h_new = a->hall + (t + 1) * n;
+    float* c_new = a->call + (t + 1) * n;
+    gather_rows_kernel<<<cdiv((long)n, 256), 256, 0, st>>>(h_new, c.parent_rows, a->gtmp, nullptr, d.B, d.D);
+    LO_LAUNCH_OK();
+    gather_rows_kernel<<<cdiv((long)n, 256), 256, 0, st>>>(c_new, c.parent_rows, a->gtmp + n, nullptr, d.B, d.D);
+    LO_LAUNCH_OK();
+    LO_CUDA(cudaMemcpyAsync(h_new, a->gtmp, (size_t)n * 4, cudaMemcpyDeviceToDevice, st));
+    LO_CUDA(cudaMemcpyAsync(c_new, a->gtmp + n, (size_t)n * 4, cudaMemcpyDeviceToDevice, st));
+    if (bv.on) LO_TRY(lo_cast(h_new, LO_F32, bv.hall + (t + 1) * n, LO_BF16, n, st));
+    return LO_OK;
+  }
+};
+
 }  // namespace lo
 
 using namespace lo;
@@ -2110,30 +2224,8 @@ int lo_decoder_greedy_hist(const lo_decoder_args* a, int64_t start_id, int64_t e
   LO_TRY(check_args(a));
   LO_TRY(check_reg_off(a, true));
   LO_CHECK_ARG(!a->ss_prob, "scheduled sampling (ss_prob) is a training mode: greedy decode feeds its own argmax already");
-  LO_CHECK_ARG(tokens && finished && max_steps > 0 && max_steps <= a->T, "tokens/finished/max_steps (<= T capacity)");
-  cudaStream_t st = (cudaStream_t)stream;
-  const Dims d = dims(a);
-  int64_t* next_tok = (int64_t*)a->sreg;          // scratch: [B] int64 fits in sreg [B][>=2] floats
-  fill_i64_kernel<<<cdiv(d.B, 128), 128, 0, st>>>(next_tok, start_id, d.B);
-  LO_LAUNCH_OK();
-  LO_CUDA(cudaMemsetAsync(finished, 0, (size_t)d.B * 4, st));
-  LO_TRY(forward_prologue(a, d, st));
-  AttRagged rg = ragged_of(a);
-  if (a->reg_off) LO_TRY(attention_ragged_prepare(rg, d.B, a->rows_per_img > 1 ? a->rows_per_img : 1, st));
-  const BfViews bvg = bf_views(a, d);
-  for (int t = 0; t < max_steps; t++) {
-    LO_TRY(forward_step(a, d, t, Rows{0, d.B, a->work, 0, a->reg_off ? &rg : nullptr}, next_tok, 1, nullptr, 0, nullptr, st));
-    // logits_t = fc(h_t)   (no dropout at decode time)
-    const int64_t h_t = (int64_t)(t + 1) * d.B * d.D;
-    LO_TRY(head_nt(a, bvg.on, a->hall + h_t, bvg.on ? bvg.hall + h_t : nullptr, d.D, a->logits, d.V, d.B, st));
-    argmax_kernel<<<cdiv(d.B, 8), 256, 0, st>>>(a->logits, d.V, tokens + t, max_steps, next_tok, finished, end_id, d.B);
-    LO_LAUNCH_OK();
-    if (fin_hist) {
-      fin_hist_kernel<<<cdiv(d.B, 128), 128, 0, st>>>(finished, fin_hist + t, max_steps, d.B);
-      LO_LAUNCH_OK();
-    }
-  }
-  return LO_OK;
+  TorchDecode f(a, start_id, finished, nullptr);
+  return greedy_loop(f, end_id, max_steps, tokens, fin_hist, (cudaStream_t)stream);
 }
 
 int lo_decoder_greedy(const lo_decoder_args* a, int64_t start_id, int64_t end_id, int max_steps, int64_t* tokens,
@@ -2152,45 +2244,11 @@ int lo_decoder_beam_div(const lo_decoder_args* a, int64_t start_id, int64_t end_
   LO_TRY(check_args(a));
   LO_TRY(check_reg_off(a, true));
   LO_CHECK_ARG(!a->ss_prob, "scheduled sampling (ss_prob) is a training mode: not available in beam search");
-  const bool div_on = !(div_gamma == 1.f || div_prob == 0.f);               // beam_search_decoder_cell.py:270-273
-  LO_CHECK_ARG(!div_on || (div_gamma > 0.f && (div_u || div_state)), "diversity penalty needs gamma > 0 and div_u or div_state");
-  const int beam = a->rows_per_img;
-  LO_CHECK_ARG(beam >= 1 && beam <= LO_BEAM_MAX && a->B % beam == 0, "1 <= beam (rows_per_img) <= 16, B % beam == 0");
-  LO_CHECK_ARG(ids && parents && fin_hist && logp && max_steps > 0 && max_steps <= a->T, "outputs / max_steps (<= T capacity)");
-  LO_CHECK_ARG((size_t)beam * a->V * 4 * (div_on ? 2 : 1) <= 200 * 1024, "beam*V too large for the shared-memory top-k");
-  cudaStream_t st = (cudaStream_t)stream;
-  const Dims d = dims(a);
-  const int n_img = d.B / beam;
-  // scratch: next tokens (int64 [B]) in sreg, finished + parent rows (int32 [B] each) in row_loss
-  int64_t* next_tok = (int64_t*)a->sreg;
+  LO_CHECK_ARG((int64_t)a->B * a->T >= 2 * a->B, "row_loss scratch too small");
   int32_t* finished = (int32_t*)a->row_loss;
-  int32_t* parent_rows = finished + d.B;
-  LO_CHECK_ARG((int64_t)d.B * d.T >= 2 * d.B, "row_loss scratch too small");
-  fill_i64_kernel<<<cdiv(d.B, 128), 128, 0, st>>>(next_tok, start_id, d.B);
-  LO_LAUNCH_OK();
-  LO_CUDA(cudaMemsetAsync(finished, 0, (size_t)d.B * 4, st));
-  LO_CUDA(cudaMemsetAsync(logp, 0, (size_t)d.B * 4, st));          // initial log-probs are zeros (:106-107)
-  LO_TRY(forward_prologue(a, d, st));
-  AttRagged rg = ragged_of(a);
-  if (a->reg_off) LO_TRY(attention_ragged_prepare(rg, d.B, beam, st));
-  const BfViews bv = bf_views(a, d);
-  for (int t = 0; t < max_steps; t++) {
-    LO_TRY(forward_step(a, d, t, Rows{0, d.B, a->work, 0, a->reg_off ? &rg : nullptr}, next_tok, 1, nullptr, 0, nullptr, st));
-    float* h_new = a->hall + (int64_t)(t + 1) * d.B * d.D;
-    float* c_new = a->call + (int64_t)(t + 1) * d.B * d.D;
-    LO_TRY(head_nt(a, bv.on, h_new, bv.on ? bv.hall + (int64_t)(t + 1) * d.B * d.D : nullptr, d.D, a->logits, d.V, d.B, st));
-    LO_TRY(beam_select(a->logits, d.V, beam, n_img, t, max_steps, end_id, logp, finished, ids, parents, fin_hist, next_tok, parent_rows,
-                       div_on, div_gamma, div_prob, div_u ? div_u + (int64_t)t * d.B * d.V : nullptr, div_state, st));
-    // reorder the recurrent state by parents (through gtmp as a temporary)
-    gather_rows_kernel<<<cdiv((long)d.B * d.D, 256), 256, 0, st>>>(h_new, parent_rows, a->gtmp, d.B, d.D);
-    LO_LAUNCH_OK();
-    gather_rows_kernel<<<cdiv((long)d.B * d.D, 256), 256, 0, st>>>(c_new, parent_rows, a->gtmp + (int64_t)d.B * d.D, d.B, d.D);
-    LO_LAUNCH_OK();
-    LO_CUDA(cudaMemcpyAsync(h_new, a->gtmp, (size_t)d.B * d.D * 4, cudaMemcpyDeviceToDevice, st));
-    LO_CUDA(cudaMemcpyAsync(c_new, a->gtmp + (int64_t)d.B * d.D, (size_t)d.B * d.D * 4, cudaMemcpyDeviceToDevice, st));
-    if (bv.on) LO_TRY(lo_cast(h_new, LO_F32, bv.hall + (int64_t)(t + 1) * d.B * d.D, LO_BF16, (int64_t)d.B * d.D, stream));
-  }
-  return LO_OK;
+  TorchDecode f(a, start_id, finished, finished + a->B);
+  return beam_loop(f, BeamArgs{a->rows_per_img, div_gamma, div_prob, div_u, div_state}, end_id, max_steps, ids, parents, fin_hist, logp,
+                   (cudaStream_t)stream);
 }
 
 }  // extern "C"

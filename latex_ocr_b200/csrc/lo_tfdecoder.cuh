@@ -1,6 +1,6 @@
 // TensorFlow-flavour decoder (SURVEY.md §8-a row a7): the Genthial attention cell, teacher-forced training pass with a
 // hand-derived backward, masked cross-entropy, greedy and beam decode.  Part of the lo_decoder.cu translation unit (it
-// reuses that file's kernels: attention launchers, datt1 sweep, transposes, beam step, argmax ...).
+// reuses that file's kernels: attention launchers, datt1 sweep, transposes, beam step, argmax ..., and its decode loops).
 //
 // Reference semantics (paths relative to the reference root):
 //   model/components/attention_cell.py:58-89   step:  x = [emb ; o] ; (c,h) = LSTMCell(x,(c,h)) ; hd = dropout(h) ; ctx = attention(hd) ;
@@ -255,17 +255,6 @@ __global__ void tf_dptab_scatter_kernel(const float* __restrict__ dz, const int6
   }
 }
 
-// dst[r][:] = src[rows[r]][:] (+ bf16 mirror of dst)
-__global__ void tf_gather_rows_kernel(const float* __restrict__ src, const int32_t* __restrict__ rows, float* __restrict__ dst,
-                                      bf16* __restrict__ dst_bf, int n, int W) {
-  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= n * W) return;
-  const int r = idx / W, j = idx % W;
-  const float v = src[(int64_t)rows[r] * W + j];
-  dst[idx] = v;
-  if (dst_bf) dst_bf[idx] = __float2bfloat16_rn(v);
-}
-
 // ------------------------------------------------------------------------------------------------ workspace
 struct TfDims {
   int B, T, R, C, A, D, O, E, V, XH, G, LW, N2, DW, Vl, rpi, nimg;
@@ -355,11 +344,6 @@ static TfWs tf_carve(const lo_tfdec_args* a) {
   w.ragmap = take((size_t)attention_ragged_map_bytes(d.B));
   w.bytes = off;
   return w;
-}
-
-// `decode`: a greedy / beam entry point (the only ones that take per-image region counts)
-static int check_reg_off(const lo_tfdec_args* a, bool decode) {
-  return check_reg_off(a->reg_off, a->reg_off_host, a->B, a->rows_per_img, a->R, decode);
 }
 
 static int tf_check(const lo_tfdec_args* a, bool decode) {
@@ -500,15 +484,42 @@ static int tf_step(const lo_tfdec_args* a, const TfDims& d, const TfWs& w, int t
   return LO_OK;
 }
 
-// the ragged attention state of a decode call (lo_tfdec_args.reg_off): its CTA map has a workspace region of its own
-static AttRagged tf_ragged(const lo_tfdec_args* a, const TfWs& w) { return AttRagged{a->reg_off, a->reg_off_host, w.ragmap, 0}; }
-
 // logits of `rows` consecutive state rows starting at xh row `row0` (o part) -> out [rows][ldo]
 static int tf_logits(const lo_tfdec_args* a, const TfDims& d, const TfWs& w, int64_t row0, int rows, float* out, int64_t ldo,
                      cudaStream_t st) {
   return tf_nt(a, w.xh + row0 * d.XH, w.xh_bf ? w.xh_bf + row0 * d.XH : nullptr, d.XH, a->w_y, d.O, out, ldo, rows, d.V, d.O, nullptr, 0,
                st);
 }
+
+// the TF flavour in the decode loops of lo_decoder.cu: its scratch, the ragged CTA map included, is carved from ws
+struct TfDecode {
+  const lo_tfdec_args* a;
+  TfDims d;
+  TfWs w;
+  DecodeCtx c;
+  explicit TfDecode(const lo_tfdec_args* a_)
+      : a(a_), d(tf_dims(a_)), w(tf_carve(a_)),
+        c{d.B, d.T, d.V, d.rpi, a_->logits, w.next_tok, w.finished, w.parent_rows,
+          AttRagged{a_->reg_off, a_->reg_off_host, w.ragmap, 0}} {}
+  int prologue(cudaStream_t st) { return tf_prologue(a, d, w, st); }
+  // step 0 is fed tok = NULL: the start-token row V of the token table
+  int step(int t, cudaStream_t st) {
+    LO_TRY(tf_step(a, d, w, t, t == 0 ? nullptr : w.next_tok, 1, st, c.ragged()));
+    return tf_logits(a, d, w, (int64_t)(t + 1) * d.B, d.B, a->logits, d.V, st);
+  }
+  // the cell state (c, h, o) of step t by parents (gather_helper, beam_search_decoder_cell.py:370-391): xh and its mirror, then c
+  int reorder(int t, cudaStream_t st) {
+    const int64_t rown = (int64_t)(t + 1) * d.B;
+    gather_rows_kernel<<<cdiv((long)d.B * d.XH, 256), 256, 0, st>>>(w.xh + rown * d.XH, c.parent_rows, w.gtmp,
+                                                                    w.xh_bf ? w.xh_bf + rown * d.XH : nullptr, d.B, d.XH);
+    LO_LAUNCH_OK();
+    LO_CUDA(cudaMemcpyAsync(w.xh + rown * d.XH, w.gtmp, (size_t)d.B * d.XH * 4, cudaMemcpyDeviceToDevice, st));
+    gather_rows_kernel<<<cdiv((long)d.B * d.D, 256), 256, 0, st>>>(w.call + rown * d.D, c.parent_rows, w.gtmp, nullptr, d.B, d.D);
+    LO_LAUNCH_OK();
+    LO_CUDA(cudaMemcpyAsync(w.call + rown * d.D, w.gtmp, (size_t)d.B * d.D * 4, cudaMemcpyDeviceToDevice, st));
+    return LO_OK;
+  }
+};
 
 }  // namespace lo
 
@@ -700,25 +711,8 @@ int lo_tfdec_backward(const lo_tfdec_args* a, void* stream) {
 
 int lo_tfdec_greedy(const lo_tfdec_args* a, int64_t end_id, int max_steps, int64_t* tokens, int32_t* fin_hist, void* stream) {
   LO_TRY(tf_check(a, true));
-  LO_CHECK_ARG(tokens && max_steps > 0 && max_steps <= a->T, "tokens / max_steps (<= T capacity)");
-  cudaStream_t st = (cudaStream_t)stream;
-  const TfDims d = tf_dims(a);
-  const TfWs w = tf_carve(a);
-  LO_CUDA(cudaMemsetAsync(w.finished, 0, (size_t)d.B * 4, st));
-  LO_TRY(tf_prologue(a, d, w, st));
-  AttRagged rg = tf_ragged(a, w);
-  if (a->reg_off) LO_TRY(attention_ragged_prepare(rg, d.B, d.rpi, st));
-  for (int t = 0; t < max_steps; t++) {
-    LO_TRY(tf_step(a, d, w, t, t == 0 ? nullptr : w.next_tok, 1, st, a->reg_off ? &rg : nullptr));
-    LO_TRY(tf_logits(a, d, w, (int64_t)(t + 1) * d.B, d.B, a->logits, d.V, st));
-    argmax_kernel<<<cdiv(d.B, 8), 256, 0, st>>>(a->logits, d.V, tokens + t, max_steps, w.next_tok, w.finished, end_id, d.B);
-    LO_LAUNCH_OK();
-    if (fin_hist) {
-      fin_hist_kernel<<<cdiv(d.B, 128), 128, 0, st>>>(w.finished, fin_hist + t, max_steps, d.B);
-      LO_LAUNCH_OK();
-    }
-  }
-  return LO_OK;
+  TfDecode f(a);
+  return greedy_loop(f, end_id, max_steps, tokens, fin_hist, (cudaStream_t)stream);
 }
 
 int lo_tfdec_beam(const lo_tfdec_args* a, int64_t end_id, int max_steps, int64_t* ids, int64_t* parents, int32_t* fin_hist, float* logp,
@@ -729,37 +723,9 @@ int lo_tfdec_beam(const lo_tfdec_args* a, int64_t end_id, int max_steps, int64_t
 int lo_tfdec_beam_div(const lo_tfdec_args* a, int64_t end_id, int max_steps, int64_t* ids, int64_t* parents, int32_t* fin_hist,
                       float* logp, float div_gamma, float div_prob, const float* div_u, const uint64_t* div_state, void* stream) {
   LO_TRY(tf_check(a, true));
-  const bool div_on = !(div_gamma == 1.f || div_prob == 0.f);               // beam_search_decoder_cell.py:270-273
-  LO_CHECK_ARG(!div_on || (div_gamma > 0.f && (div_u || div_state)), "diversity penalty needs gamma > 0 and div_u or div_state");
-  LO_CHECK_ARG(ids && parents && fin_hist && logp && max_steps > 0 && max_steps <= a->T, "outputs / max_steps (<= T capacity)");
-  cudaStream_t st = (cudaStream_t)stream;
-  const TfDims d = tf_dims(a);
-  const int beam = d.rpi;
-  LO_CHECK_ARG(beam >= 1 && beam <= LO_BEAM_MAX, "beam size 1..16");
-  const TfWs w = tf_carve(a);
-  LO_CUDA(cudaMemsetAsync(w.finished, 0, (size_t)d.B * 4, st));
-  LO_CUDA(cudaMemsetAsync(logp, 0, (size_t)d.B * 4, st));                    // initial log-probs are zeros (:106-107)
-  LO_TRY(tf_prologue(a, d, w, st));
-  AttRagged rg = tf_ragged(a, w);
-  if (a->reg_off) LO_TRY(attention_ragged_prepare(rg, d.B, beam, st));
-  const size_t smem = (size_t)beam * d.V * 4 * (div_on ? 2 : 1);
-  LO_CHECK_ARG(smem <= 200 * 1024, "beam*V too large for the shared-memory top-k");
-  for (int t = 0; t < max_steps; t++) {
-    LO_TRY(tf_step(a, d, w, t, t == 0 ? nullptr : w.next_tok, 1, st, a->reg_off ? &rg : nullptr));
-    const int64_t rown = (int64_t)(t + 1) * d.B;
-    LO_TRY(tf_logits(a, d, w, rown, d.B, a->logits, d.V, st));
-    LO_TRY(beam_select(a->logits, d.V, beam, d.nimg, t, max_steps, end_id, logp, w.finished, ids, parents, fin_hist, w.next_tok,
-                       w.parent_rows, div_on, div_gamma, div_prob, div_u ? div_u + (int64_t)t * d.B * d.V : nullptr, div_state, st));
-    // reorder the cell state (c, h, o) by parents (gather_helper, beam_search_decoder_cell.py:370-391)
-    tf_gather_rows_kernel<<<cdiv((long)d.B * d.XH, 256), 256, 0, st>>>(w.xh + rown * d.XH, w.parent_rows, w.gtmp,
-                                                                       w.xh_bf ? w.xh_bf + rown * d.XH : nullptr, d.B, d.XH);
-    LO_LAUNCH_OK();
-    LO_CUDA(cudaMemcpyAsync(w.xh + rown * d.XH, w.gtmp, (size_t)d.B * d.XH * 4, cudaMemcpyDeviceToDevice, st));
-    tf_gather_rows_kernel<<<cdiv((long)d.B * d.D, 256), 256, 0, st>>>(w.call + rown * d.D, w.parent_rows, w.gtmp, nullptr, d.B, d.D);
-    LO_LAUNCH_OK();
-    LO_CUDA(cudaMemcpyAsync(w.call + rown * d.D, w.gtmp, (size_t)d.B * d.D * 4, cudaMemcpyDeviceToDevice, st));
-  }
-  return LO_OK;
+  TfDecode f(a);
+  return beam_loop(f, BeamArgs{f.d.rpi, div_gamma, div_prob, div_u, div_state}, end_id, max_steps, ids, parents, fin_hist, logp,
+                   (cudaStream_t)stream);
 }
 
 }  // extern "C"

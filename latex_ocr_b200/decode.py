@@ -12,14 +12,19 @@ The torch flavour of the reference has no START symbol; the caller supplies ``st
 ``img`` is a tensor [N,1,H,W] (one size for the batch) or a list of images of different sizes, each a [1,H,W] tensor or an HxWx1
 uint8 array.  A list is decoded in ONE time loop in which every image attends over its own regions only (lo_decoder_args.reg_off):
 no padding, and an image's tokens are those it gets when decoded alone.
+
+Also the host side both decoder flavours share (tf_decoder.Decoder): region offsets, the ragged workspace's capacity rule, and
+greedy / beam calls with their outputs trimmed to the steps the reference would have run.
 """
 import collections
 import ctypes
+import itertools
 
 import torch
 
 from . import _lib
 from ._lib import check, stream_ptr
+from .kernel_module import stamp
 
 
 def _n_steps(fin_hist):
@@ -31,20 +36,63 @@ def _n_steps(fin_hist):
     return int(idx[0]) + 1 if idx.numel() else S
 
 
-def _prepare(model, img, rows_per_img, max_steps):
-    enc = model.encoder.forward_raw(img.to(model.device).float(), need_grad=False)
-    N = enc.shape[0]
-    R = enc.shape[1] * enc.shape[2]
-    enc_flat = enc.view(N, R, enc.shape[3])
-    dec = model.decoder
-    B = N * rows_per_img
-    ws = dec.workspace(B, max_steps, R, need_grad=False)
-    dec.store.refresh_shadow()
-    for t in range(max_steps):
-        ws["bt"][t] = B
-    a = dec.fill_args(ws, enc_flat, B, max_steps, R, has_dropout=False)
-    a.rows_per_img = rows_per_img
-    return a, ws, N
+def region_offsets(counts):
+    """[0, n_0, n_0 + n_1, ...]: the offsets (reg_off) of images of ``counts`` regions, in decode order"""
+    return list(itertools.accumulate((int(n) for n in counts), initial=0))
+
+
+def set_region_offsets(a, host, dev, off):
+    """Writes the offsets ``off`` into a ragged workspace's host array ``host`` and device tensor ``dev`` and points the args
+    ``a`` (lo_decoder_args or lo_tfdec_args) at them."""
+    for i, v in enumerate(off):
+        host[i] = v
+    dev[:len(off)].copy_(torch.tensor(off, dtype=torch.int32))
+    a.reg_off = dev.data_ptr()
+    a.reg_off_host = ctypes.cast(host, ctypes.c_void_p)
+
+
+def ragged_cache(cache, cap, build):
+    """The one ragged decode workspace of ``cache`` (key "ragged") for a call of capacity ``cap`` = (rows B, steps T, largest
+    region count R, total regions).  A cached workspace whose capacity covers the call is reused; otherwise ``build(*cap)`` makes
+    one of the element-wise maximum of both capacities (serving traffic gives a new composition on nearly every call)."""
+    ws = cache.get("ragged")
+    if ws is not None:
+        if all(c <= h for c, h in zip(cap, ws["cap"])):
+            return stamp(ws)
+        cap = tuple(max(c, h) for c, h in zip(cap, ws["cap"]))
+        del cache["ragged"]
+    ws = build(*cap)
+    ws["cap"] = cap
+    cache["ragged"] = ws
+    return ws
+
+
+def run_greedy(call, N, steps, device):
+    """Greedy decode of N rows: ``call(tokens, fin_hist)`` runs the flavour's entry point on the device pointers of the outputs
+    [N, steps].  Returns the tokens [N, n] on the device, n the steps the reference would have run."""
+    tokens = torch.zeros(N, steps, dtype=torch.int64, device=device)
+    hist = torch.zeros(N, steps, dtype=torch.int32, device=device)
+    check(call(tokens.data_ptr(), hist.data_ptr()))
+    return tokens[:, :_n_steps(hist)]
+
+
+def run_beam(call, N, beam, steps, V, device, div_u=None, order=None):
+    """Beam search of N images: ``call(ids, parents, fin_hist, logp, div_u)`` runs the flavour's entry point on device pointers.
+    ``div_u``: None or injected uniforms [steps, N * beam, V] in input order (``order``: the input index of each decode image).
+    Returns (ids [N, n, beam], parents [N, n, beam], logp [N, beam]) on the device, n the steps the reference would have run."""
+    ids = torch.zeros(N, steps, beam, dtype=torch.int64, device=device)
+    parents = torch.zeros_like(ids)
+    hist = torch.zeros(N, steps, beam, dtype=torch.int32, device=device)
+    logp = torch.zeros(N, beam, dtype=torch.float32, device=device)
+    if div_u is not None:
+        div_u = torch.as_tensor(div_u, dtype=torch.float32).to(device).contiguous()
+        if tuple(div_u.shape) != (steps, N * beam, V):
+            raise ValueError("div_u must be [steps, N * beam, V] = [%d, %d, %d]" % (steps, N * beam, V))
+        if order is not None:
+            div_u = div_u.view(steps, N, beam, V)[:, torch.tensor(order, device=device)].reshape(steps, N * beam, V)
+    check(call(ids.data_ptr(), parents.data_ptr(), hist.data_ptr(), logp.data_ptr(), div_u.data_ptr() if div_u is not None else None))
+    n = _n_steps(hist)
+    return ids[:, :n], parents[:, :n], logp
 
 
 def _image(x):
@@ -80,10 +128,7 @@ def ragged_layout(images, out_hw):
         counts += [h * w] * (j1 - j0)
     if min(counts) < 1:
         raise ValueError("an image is too small for the encoder (no feature-map region)")
-    off = [0]
-    for n in counts:
-        off.append(off[-1] + n)
-    return RaggedLayout(imgs, order, groups, counts, off)
+    return RaggedLayout(imgs, order, groups, counts, region_offsets(counts))
 
 
 def encode_packed(encoder, lay, enc, device):
@@ -96,27 +141,31 @@ def encode_packed(encoder, lay, enc, device):
         enc[off[j0]:off[j1]].copy_(e.reshape(off[j1] - off[j0], e.shape[3]))
 
 
-def _prepare_ragged(model, images, rows_per_img, max_steps):
-    """Packed encoder output and the argument block of a decode over images of different sizes (ragged_layout).  Returns (args,
-    workspace, order, region counts) with order[j] = the input index of decode image j."""
-    lay = ragged_layout(images, model.encoder.out_hw)
-    order, counts, off = lay.order, lay.counts, lay.off
-    N, R, dev, dec = len(order), max(counts), model.device, model.decoder
+def _prepare(model, img, rows_per_img, max_steps):
+    """Encoder output and the argument block of a decode of ``img``: a batch tensor, or a list of images of different sizes packed
+    by ragged_layout.  Returns (args, workspace, N, the RaggedLayout of a list or None)."""
+    dec = model.decoder
+    lay = None
+    if isinstance(img, (list, tuple)):
+        lay = ragged_layout(img, model.encoder.out_hw)
+        N, R = len(lay.order), max(lay.counts)
+        ws = dec.ragged_workspace(N * rows_per_img, max_steps, R, lay.off[-1])
+        enc = ws["t"]["enc"]
+        encode_packed(model.encoder, lay, enc, model.device)
+    else:
+        enc = model.encoder.forward_raw(img.to(model.device).float(), need_grad=False)
+        N, R = enc.shape[0], enc.shape[1] * enc.shape[2]
+        enc = enc.view(N, R, enc.shape[3])
+        ws = dec.workspace(N * rows_per_img, max_steps, R, need_grad=False)
     B = N * rows_per_img
-    ws = dec.ragged_workspace(B, max_steps, R, off[-1])
-    encode_packed(model.encoder, lay, ws["t"]["enc"], dev)
-    host = ws["reg_off_host"]
-    for i, v in enumerate(off):
-        host[i] = v
-    ws["t"]["reg_off"][:N + 1].copy_(torch.tensor(off, dtype=torch.int32))
     dec.store.refresh_shadow()
     for t in range(max_steps):
         ws["bt"][t] = B
-    a = dec.fill_args(ws, ws["t"]["enc"], B, max_steps, R, has_dropout=False)
+    a = dec.fill_args(ws, enc, B, max_steps, R, has_dropout=False)
     a.rows_per_img = rows_per_img
-    a.reg_off = ws["t"]["reg_off"].data_ptr()
-    a.reg_off_host = ctypes.cast(host, ctypes.c_void_p)
-    return a, ws, order, counts
+    if lay is not None:
+        set_region_offsets(a, ws["reg_off_host"], ws["t"]["reg_off"], lay.off)
+    return a, ws, N, lay
 
 
 def _inverse(order):
@@ -134,28 +183,19 @@ def greedy_decode(model, img, start_id, end_id, max_length_formula=150, return_a
     L = _lib.lib()
     max_steps = max_length_formula + 2
     with torch.no_grad():
-        if isinstance(img, (list, tuple)):
-            a, ws, order, counts = _prepare_ragged(model, img, 1, max_steps)
-            N = len(order)
-        else:
-            a, ws, N = _prepare(model, img, 1, max_steps)
-        dev = model.device
-        tokens = torch.zeros(N, max_steps, dtype=torch.int64, device=dev)
-        finished = torch.zeros(N, dtype=torch.int32, device=dev)
-        hist = torch.zeros(N, max_steps, dtype=torch.int32, device=dev)
-        check(L.lo_decoder_greedy_hist(ctypes.byref(a), int(start_id), int(end_id), max_steps, tokens.data_ptr(), finished.data_ptr(),
-                                       hist.data_ptr(), stream_ptr()))
-        n = _n_steps(hist.cpu())
-        if isinstance(img, (list, tuple)):
-            inv = _inverse(order)
-            ids = tokens[:, :n].cpu()[inv]
-            if return_attention:
-                al = ws["t"]["alphas"].view(-1)[:N * max_steps * a.R].view(N, max_steps, a.R)[:, :n].cpu()
-                return ids, [al[j, :, :counts[j]].clone() for j in inv.tolist()]
-            return ids
+        a, ws, N, lay = _prepare(model, img, 1, max_steps)
+        finished = torch.zeros(N, dtype=torch.int32, device=model.device)
+        ids = run_greedy(lambda tokens, hist: L.lo_decoder_greedy_hist(ctypes.byref(a), int(start_id), int(end_id), max_steps, tokens,
+                                                                      finished.data_ptr(), hist, stream_ptr()),
+                         N, max_steps, model.device).cpu()
+        n = ids.shape[1]
+        if lay is None:
+            return (ids, ws["t"]["alphas"][:, :n].float().cpu()) if return_attention else ids
+        inv = _inverse(lay.order)
         if return_attention:
-            return tokens[:, :n].cpu(), ws["t"]["alphas"][:, :n].float().cpu()
-        return tokens[:, :n].cpu()
+            al = ws["t"]["alphas"].view(-1)[:N * max_steps * a.R].view(N, max_steps, a.R)[:, :n].cpu()
+            return ids[inv], [al[j, :, :lay.counts[j]].clone() for j in inv.tolist()]
+        return ids[inv]
 
 
 def attention_maps(alphas, att_h, att_w):
@@ -178,37 +218,25 @@ def beam_decode(model, img, start_id, end_id, beam_size=5, max_length_formula=15
         raise NotImplementedError("finalize must be 'reference' or 'backtrack'")
     L = _lib.lib()
     max_steps = max_length_formula + 2
-    ragged = isinstance(img, (list, tuple))
     with torch.no_grad():
-        if ragged:
-            a, ws, order, _ = _prepare_ragged(model, img, beam_size, max_steps)
-            N = len(order)
-        else:
-            a, ws, N = _prepare(model, img, beam_size, max_steps)
+        a, ws, N, lay = _prepare(model, img, beam_size, max_steps)
         dev = model.device
-        ids = torch.zeros(N, max_steps, beam_size, dtype=torch.int64, device=dev)
-        parents = torch.zeros_like(ids)
-        hist = torch.zeros(N, max_steps, beam_size, dtype=torch.int32, device=dev)
-        logp = torch.zeros(N, beam_size, dtype=torch.float32, device=dev)
         div_on = not (div_gamma == 1 or div_prob == 0)
-        u_dev = state = None
-        if div_on and div_u is not None:
-            u_dev = torch.as_tensor(div_u, dtype=torch.float32).to(dev).contiguous()
-            if tuple(u_dev.shape) != (max_steps, N * beam_size, a.V):
-                raise ValueError("div_u must be [max_length_formula + 2, N * beam, V]")
-            if ragged:          # decode order
-                u_dev = u_dev.view(max_steps, N, beam_size, a.V)[:, torch.tensor(order, device=dev)].reshape(max_steps, N * beam_size, a.V)
-        elif div_on:
+        state = None
+        if div_on and div_u is None:
             seed = torch.initial_seed() if div_seed is None else int(div_seed)
             state = torch.tensor([seed & 0x7FFFFFFFFFFFFFFF, 0], dtype=torch.int64, device=dev)
-        check(L.lo_decoder_beam_div(ctypes.byref(a), int(start_id), int(end_id), max_steps, ids.data_ptr(), parents.data_ptr(),
-                                    hist.data_ptr(), logp.data_ptr(), float(div_gamma), float(div_prob),
-                                    u_dev.data_ptr() if u_dev is not None else None,
-                                    state.data_ptr() if state is not None else None, stream_ptr()))
-        n = _n_steps(hist.cpu())
-        ids, parents, logp = ids[:, :n].cpu(), parents[:, :n].cpu(), logp.cpu()
-        if ragged:
-            inv = _inverse(order)
+
+        def call(ids, parents, hist, logp, u):
+            return L.lo_decoder_beam_div(ctypes.byref(a), int(start_id), int(end_id), max_steps, ids, parents, hist, logp,
+                                         float(div_gamma), float(div_prob), u, state.data_ptr() if state is not None else None,
+                                         stream_ptr())
+        ids, parents, logp = run_beam(call, N, beam_size, max_steps, a.V, dev, div_u if div_on else None,
+                                      lay.order if lay else None)
+        n = ids.shape[1]
+        ids, parents, logp = ids.cpu(), parents.cpu(), logp.cpu()
+        if lay is not None:
+            inv = _inverse(lay.order)
             ids, parents, logp = ids[inv], parents[inv], logp[inv]
         if finalize == "backtrack":
             out = torch.zeros_like(ids)

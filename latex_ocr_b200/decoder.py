@@ -10,7 +10,7 @@ import math
 import torch
 import torch.nn as nn
 
-from . import _lib
+from . import _lib, decode
 from ._lib import check, dtype_code, impl_code, ptr, stream_ptr
 from .kernel_module import kernel_forward, stamp
 from .params import FlatStore, LRUCache, ParamHolder, grad_view
@@ -291,23 +291,16 @@ class DecoderWithAttention(nn.Module):
     def ragged_workspace(self, B, T, R, n_regions):
         """Decode workspace for images of different sizes (lo_decoder_args.reg_off): the packed encoder output ``t["enc"]``
         [regions, C], att1 [regions, A] and every per-row buffer, sized by capacity (rows B, steps T, largest region count R,
-        total regions).  One cache entry: a later call whose composition fits reuses it, a larger one replaces it by the element-wise
-        maximum of both capacities (serving traffic gives a new composition on nearly every call)."""
-        ws = self._ws.get("ragged")
-        if ws is not None:
-            cap = ws["cap"]
-            if B <= cap[0] and T <= cap[1] and R <= cap[2] and n_regions <= cap[3]:
-                return stamp(ws)
-            B, T, R, n_regions = max(B, cap[0]), max(T, cap[1]), max(R, cap[2]), max(n_regions, cap[3])
-            del self._ws["ragged"]
-        ws = self.workspace(B, T, R, False, key="ragged", att1_rows=n_regions)
-        ws["cap"] = (B, T, R, n_regions)
-        dev = self.store.device
-        ws["t"]["enc"] = torch.zeros(n_regions, self.encoder_dim, dtype=self.tdtype, device=dev)
-        ws["t"]["reg_off"] = torch.zeros(B + 1, dtype=torch.int32, device=dev)
-        ws["reg_off_host"] = (ctypes.c_int32 * (B + 1))()
-        self.fill_args(ws, ws["t"]["enc"], B, T, R, has_dropout=False)        # sizes bfwork (wgmma staging) by capacity
-        return ws
+        total regions; decode.ragged_cache)."""
+        def build(B, T, R, n_regions):
+            ws = self.workspace(B, T, R, False, key="ragged", att1_rows=n_regions)
+            dev = self.store.device
+            ws["t"]["enc"] = torch.zeros(n_regions, self.encoder_dim, dtype=self.tdtype, device=dev)
+            ws["t"]["reg_off"] = torch.zeros(B + 1, dtype=torch.int32, device=dev)
+            ws["reg_off_host"] = (ctypes.c_int32 * (B + 1))()
+            self.fill_args(ws, ws["t"]["enc"], B, T, R, has_dropout=False)        # sizes bfwork (wgmma staging) by capacity
+            return ws
+        return decode.ragged_cache(self._ws, (B, T, R, n_regions), build)
 
     def _fed_buffer(self, ws):
         """[B, T] int64 tokens fed by a scheduled-sampling forward (allocated on first use of the mode for this shape)."""

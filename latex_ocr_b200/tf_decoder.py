@@ -26,7 +26,7 @@ import math
 import torch
 import torch.nn as nn
 
-from . import _lib
+from . import _lib, decode
 from ._lib import TfDecArgs, check, dtype_code, impl_code, stream_ptr
 from .kernel_module import kernel_forward, stamp
 from .params import FlatStore, LRUCache, ParamHolder, bind_grads
@@ -319,34 +319,26 @@ class Decoder(nn.Module):
     def ragged_workspace(self, B, T, R, n_regions):
         """Decode workspace for images of different sizes (lo_tfdec_args.reg_off): the packed encoder output ``enc`` [regions, C],
         the region offsets ``reg_off`` / ``reg_off_host`` and every per-row buffer, sized by capacity (rows B, steps T, largest
-        region count R, total regions).  One cache entry: a later call whose composition fits reuses it, a larger one replaces it
-        by the element-wise maximum of both capacities (serving traffic gives a new composition on nearly every call)."""
-        ws = self._ws.get("ragged")
-        if ws is not None:
-            cap = ws["cap"]
-            if B <= cap[0] and T <= cap[1] and R <= cap[2] and n_regions <= cap[3]:
-                return ws
-            B, T, R, n_regions = max(B, cap[0]), max(T, cap[1]), max(R, cap[2]), max(n_regions, cap[3])
-            del self._ws["ragged"]
-        dev = self.store.device
-        ldl = (self.V + 63) // 64 * 64
-        z = lambda *shape, dtype=torch.float32: torch.zeros(*shape, dtype=dtype, device=dev)
-        ws = {"cap": (B, T, R, n_regions), "ldl": ldl,
-              "logits": z(B, ldl),                    # decoding writes one step's logits, [B][V]
-              "alphas": z(B * T * R),                 # [B][T][R] of each call's own B, T and R
-              "loss": z(4), "denc": None, "formula": z(B, T, dtype=torch.int64), "lengths": z(B, dtype=torch.int32),
-              "enc": z(n_regions, self.C, dtype=self.tdtype),
-              "reg_off": z(B + 1, dtype=torch.int32), "reg_off_host": (ctypes.c_int32 * (B + 1))()}
-        self._ws["ragged"] = ws
-        # sizes the kernel workspace: every region of it grows with B, T, R and B / rows_per_img, so any call that fits the
-        # capacity fits in it (the beam size is the decoder's own, fixed at construction)
-        self._args(ws["enc"], B, T, R, rows_per_img=self._tiles, ws=ws)
-        return ws
+        region count R, total regions; decode.ragged_cache)."""
+        def build(B, T, R, n_regions):
+            dev = self.store.device
+            ldl = (self.V + 63) // 64 * 64
+            z = lambda *shape, dtype=torch.float32: torch.zeros(*shape, dtype=dtype, device=dev)
+            ws = {"ldl": ldl,
+                  "logits": z(B, ldl),                    # decoding writes one step's logits, [B][V]
+                  "alphas": z(B * T * R),                 # [B][T][R] of each call's own B, T and R
+                  "loss": z(4), "denc": None, "formula": z(B, T, dtype=torch.int64), "lengths": z(B, dtype=torch.int32),
+                  "enc": z(n_regions, self.C, dtype=self.tdtype),
+                  "reg_off": z(B + 1, dtype=torch.int32), "reg_off_host": (ctypes.c_int32 * (B + 1))()}
+            # sizes the kernel workspace: every region of it grows with B, T, R and B / rows_per_img, so any call that fits the
+            # capacity fits in it (the beam size is the decoder's own, fixed at construction)
+            self._args(ws["enc"], B, T, R, rows_per_img=self._tiles, ws=ws)
+            return ws
+        return decode.ragged_cache(self._ws, (B, T, R, n_regions), build)
 
     def packed_workspace(self, counts, steps):
-        """The ragged workspace of one decode call over images of ``counts`` regions (in the order they are decoded), with their
-        offsets written.  The caller writes image i's encoder output into ``ws["enc"][off[i]:off[i+1]]`` (``ws["off"]``) and then
-        calls decode_packed."""
+        """The ragged workspace of one decode call over images of ``counts`` regions (in the order they are decoded).  The caller
+        writes image i's encoder output into ``ws["enc"][off[i]:off[i+1]]`` (``ws["off"]``) and then calls decode_packed."""
         N = len(counts)
         if N == 0:
             raise ValueError("no images")
@@ -354,14 +346,8 @@ class Decoder(nn.Module):
             raise ValueError("an image has no encoder region")
         if N * self._tiles > MAX_ROWS:
             raise ValueError("%d images x beam %d exceed the %d rows of one decode call" % (N, self._tiles, MAX_ROWS))
-        off = [0]
-        for n in counts:
-            off.append(off[-1] + int(n))
+        off = decode.region_offsets(counts)
         ws = self.ragged_workspace(N * self._tiles, steps, max(counts), off[-1])
-        host = ws["reg_off_host"]
-        for i, v in enumerate(off):
-            host[i] = v
-        ws["reg_off"][:N + 1].copy_(torch.tensor(off, dtype=torch.int32))
         ws["counts"], ws["off"] = [int(n) for n in counts], off
         return ws
 
@@ -373,8 +359,7 @@ class Decoder(nn.Module):
         self.store.refresh_shadow()
         with torch.no_grad():
             L, ws, a = self._args(ws["enc"], N * beam, steps, R, rows_per_img=beam, ws=ws)
-            a.reg_off = ws["reg_off"].data_ptr()
-            a.reg_off_host = ctypes.cast(ws["reg_off_host"], ctypes.c_void_p)
+            decode.set_region_offsets(a, ws["reg_off_host"], ws["reg_off"], ws["off"])
             alphas = ws["alphas"][:N * beam * steps * R].view(N * beam, steps, R) if return_attention else None
             out = self._run_decode(L, a, N, steps, div_u, alphas, return_log_probs)
             if alphas is not None and self.decoding == "greedy":
@@ -403,11 +388,9 @@ class Decoder(nn.Module):
             return self.decode_packed(ws, steps, div_u, return_attention, return_log_probs)
         enc = self._enc(enc)
         N, R, _ = enc.shape
-        beam = self._tiles
-        B = N * beam
         self.store.refresh_shadow()
         with torch.no_grad():
-            L, ws, a = self._args(enc, B, steps, R, rows_per_img=beam, decode=True)
+            L, ws, a = self._args(enc, N * self._tiles, steps, R, rows_per_img=self._tiles, decode=True)
             ws["enc"] = enc
             return self._run_decode(L, a, N, steps, div_u, ws["alphas"] if return_attention else None, return_log_probs)
 
@@ -424,41 +407,29 @@ class Decoder(nn.Module):
     def _run_decode(self, L, a, N, steps, div_u, alphas, return_log_probs):
         """The greedy or beam decode of the filled args ``a`` (N images); ``alphas`` [N, steps', R] (greedy attention export) or
         None."""
-        beam = self._tiles
-        B = N * beam
         dev = self.store.device
         if self.decoding == "greedy":
-            tokens = torch.zeros(N, steps, dtype=torch.int64, device=dev)
-            fin = torch.zeros(N, steps, dtype=torch.int32, device=dev)
-            check(L.lo_tfdec_greedy(ctypes.byref(a), self._id_end, steps, tokens.data_ptr(), fin.data_ptr(), stream_ptr()))
-            done = fin.bool().all(dim=0)                            # dynamic_decode.py:38-40: loop ends once all rows finished
-            n = int(torch.nonzero(done)[0]) + 1 if bool(done.any()) else steps
+            ids = decode.run_greedy(lambda tokens, fin: L.lo_tfdec_greedy(ctypes.byref(a), self._id_end, steps, tokens, fin,
+                                                                          stream_ptr()), N, steps, dev)
             if alphas is not None:
-                return DecoderOutput(None, tokens[:, :n]), alphas[:, :n].float().clone()
-            return DecoderOutput(None, tokens[:, :n])
-        ids = torch.zeros(N, steps, beam, dtype=torch.int64, device=dev)
-        parents = torch.zeros_like(ids)
-        fin = torch.zeros(N, steps, beam, dtype=torch.int32, device=dev)
-        logp = torch.zeros(N, beam, dtype=torch.float32, device=dev)
-        u_dev = None
+                return DecoderOutput(None, ids), alphas[:, :ids.shape[1]].float().clone()
+            return DecoderOutput(None, ids)
         div_on = not (self.div_gamma == 1 or self.div_prob == 0)
-        if div_on and div_u is not None:
-            u_dev = torch.as_tensor(div_u, dtype=torch.float32).to(dev).contiguous()
-            if tuple(u_dev.shape) != (steps, B, self.V):
-                raise ValueError("div_u must be [steps, N * beam, V]")
-        elif div_on:
+        state = None
+        if div_on and div_u is None:
             if self._div_state is None:
                 self._div_state = torch.tensor([torch.initial_seed() & 0x7FFFFFFFFFFFFFFF, 0], dtype=torch.int64, device=dev)
             self._div_state[1] += 1                                  # a new Philox stream per decode call
-        check(L.lo_tfdec_beam_div(ctypes.byref(a), self._id_end, steps, ids.data_ptr(), parents.data_ptr(), fin.data_ptr(),
-                                  logp.data_ptr(), self.div_gamma, self.div_prob, u_dev.data_ptr() if u_dev is not None else None,
-                                  self._div_state.data_ptr() if (div_on and u_dev is None) else None, stream_ptr()))
-        done = fin.bool().all(dim=2).all(dim=0)
-        n = int(torch.nonzero(done)[0]) + 1 if bool(done.any()) else steps
+            state = self._div_state.data_ptr()
+
+        def call(ids, parents, fin, logp, u):
+            return L.lo_tfdec_beam_div(ctypes.byref(a), self._id_end, steps, ids, parents, fin, logp, self.div_gamma, self.div_prob, u,
+                                       state, stream_ptr())
+        ids, _, logp = decode.run_beam(call, N, self._tiles, steps, self.V, dev, div_u if div_on else None)
         # finalize (beam_search_decoder_cell.py:189-250) gathers with the unchanged initial parents -> identity (SURVEY §8-A.3)
         if return_log_probs:
-            return DecoderOutput(None, ids[:, :n]), logp
-        return DecoderOutput(None, ids[:, :n])
+            return DecoderOutput(None, ids), logp
+        return DecoderOutput(None, ids)
 
     def forward(self, img, formula=None, dropout=1.0):
         """Decoder.__call__(img, formula, dropout) (decoder.py:24): (pred_train, pred_test).  dropout is the TF keep_prob; the

@@ -11,8 +11,10 @@ runs once.  Every case starts from the same seeded weights and inputs.  Cases:
     dec_fuse_bwd, dec_cl, dec_cl_bwd, fuse_lstm, skinny_mma=0, att_pipe=0, scheduled sampling (p = 0.25) and self-critical
     training (tau = 1);
   TensorFlow flavour, one train step: teacher forcing, scheduled sampling, self-critical training;
-  both flavours: greedy decode of images of different sizes in one batch (ragged), and beam search with the diversity penalty.
-Compared per case: lo_launch_count() over the case, and the loss, the gradients, the fed tokens and the decoded ids / log-probs.
+  both flavours: greedy decode of images of different sizes in one batch (ragged), beam search with the diversity penalty, greedy
+    decode of one batch with its attention weights, and beam search of a ragged batch (the TF flavour's with its log-probs).
+Compared per case: lo_launch_count() over the case, and the loss, the gradients, the fed tokens and the decoded ids / attention
+weights / log-probs.
 Launch counts must be equal, and every output bit-identical across the three runs, except on the paths that still add with fp32
 atomics under "deterministic".  Those are two torch-flavour paths that DESIGN.md §4 lists: the fused backward step kernels
 (dec_fuse_bwd), and the wgmma split-K of the per-step backward GEMMs (skinny_mma=0 puts it on every step).  The third is the
@@ -116,6 +118,18 @@ def run_cases():
         ids, logp = decode.beam_decode(m, dense, end_id - 1, end_id, BEAM, T, div_gamma=DIV_GAMMA, div_prob=DIV_PROB, div_seed=7)
         return {"ids": ids, "logp": logp}
     record("beam_div", beam)
+    m = torch_model()
+
+    def greedy_att():
+        ids, alphas = decode.greedy_decode(m, dense, end_id - 1, end_id, T, return_attention=True)
+        return {"ids": ids, "alphas": alphas}
+    record("greedy_att", greedy_att)
+    m = torch_model()
+
+    def beam_ragged():
+        ids, logp = decode.beam_decode(m, ragged, end_id - 1, end_id, BEAM, T)
+        return {"ids": ids, "logp": logp}
+    record("beam_ragged", beam_ragged)
 
     tf_step = lambda m: (lambda: m.train_step(tf_img, (tf_formula.cpu(), tf_lengths.cpu())))
     m = tf_model()
@@ -130,6 +144,19 @@ def run_cases():
     record("tf_greedy_ragged", lambda: {"ids": torch.tensor([t for s in m.predict_images(ragged)[0] for t in s + [-1]])})
     m = tf_model("beam_search")
     record("tf_beam_div", lambda: {"ids": torch.tensor([t for h in m.predict_batch(dense) for s in h for t in s + [-1]])})
+    m = tf_model()
+
+    def tf_greedy_att():
+        out, alphas = m.decoder.decode(m.encoder.forward_raw(dense), return_attention=True)
+        return {"ids": out.ids, "alphas": alphas}
+    record("tf_greedy_att", tf_greedy_att)
+    m = tf_model("beam_search")
+
+    def tf_beam_ragged():
+        encs = [m.encoder.forward_raw(x[None].cuda())[0].clone() for x in ragged]     # each run overwrites the encoder's output
+        out, logp = m.decoder.decode(encs, return_log_probs=True)
+        return {"ids": out.ids, "logp": logp}
+    record("tf_beam_ragged", tf_beam_ragged)
     return res
 
 

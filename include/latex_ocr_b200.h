@@ -431,6 +431,28 @@ int lo_decoder_beam_div(const lo_decoder_args* a, int64_t start_id, int64_t end_
                         int64_t* parents, int32_t* fin_hist, float* logp, float div_gamma, float div_prob,
                         const float* div_u, const uint64_t* div_state, void* stream);
 
+/* The hypotheses of a finished beam search of either flavour (lo_decoder_beam[_div], lo_tfdec_beam[_div]) and the attention weights
+ * under which their tokens were chosen.  ids / parents: that call's outputs, [n_img][ids_stride_steps][beam] int64 (ids_stride_steps =
+ * its max_steps), of which the first n steps are read.  alphas: the attention rows the decode wrote, row b = i*beam + s (slot s of
+ * image i), step t at alphas + b * alpha_row_stride + t * R (lo_decoder_args.alphas / lo_tfdec_args.alphas: alpha_row_stride = T * R).
+ * For every image i and slot s it writes ids_out [n_img][beam][n] int64 and att_out [n_img][beam][n][R] fp32:
+ *   mode LO_BEAM_SLOTS (the reference's identity finalize): ids_out[i][s][t] = ids[i][t][s], att_out[i][s][t] = alphas row i*beam + s
+ *     at step t — the rows the reference collects in attention_mechanism.ctx_vector;
+ *   mode LO_BEAM_LINEAGE (lineage-consistent hypotheses): cur = s at t = n-1, then for t = n-1 down to 0: ids_out[i][s][t] =
+ *     ids[i][t][cur], p = parents[i][t][cur], att_out[i][s][t] = alphas row i*beam + p at step t, cur = p.  Each att_out row is the
+ *     attention of the step that chose that token, what a teacher-forced pass over the hypothesis computes.
+ * A parent outside [0, beam) is read as 0, so foreign data cannot make the walk read out of bounds.  reg_off / reg_off_host (both or
+ * neither; as in lo_decoder_args): images of different sizes, image i has reg_off[i+1] - reg_off[i] regions; att_out entries past
+ * an image's count are written as 0 and the alphas past it are not read.  alphas and att_out NULL together: the ids only.
+ * Refused (LO_EINVAL) before any GPU work: null ids / parents / ids_out, one of alphas / att_out without the other, n_img < 1, beam
+ * outside 1..16, n < 1 or n > ids_stride_steps, a mode other than the two below, n * (beam + 2) * 4 bytes above 48 kB, and with
+ * att_out: R < 1, alpha_row_stride < n * R, one of reg_off / reg_off_host without the other, a count outside 1..R. */
+#define LO_BEAM_SLOTS 0
+#define LO_BEAM_LINEAGE 1
+int lo_beam_backtrack(const int64_t* ids, const int64_t* parents, int64_t ids_stride_steps, int n_img, int beam, int n,
+                      const float* alphas, int64_t alpha_row_stride, int R, const int32_t* reg_off, const int32_t* reg_off_host,
+                      int mode, int64_t* ids_out, float* att_out, void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Self-critical sequence training (SCST, Rennie et al. 2017) of the decoder above: a sample pass (lo_decoder_forward with ss_prob
  * = 1 and ss_temp), a greedy rollout (ss_prob = 1, no ss_temp) as the baseline, the reward of both against the reference

@@ -1628,6 +1628,69 @@ static int beam_select(const float* logits, int V, int beam, int n_img, int t, i
   return LO_OK;
 }
 
+// the hypotheses of a finished beam search (lo_beam_backtrack): one CTA per (image, slot).  The image's parents [n][beam] go to shared
+// memory with coalesced loads and thread 0 walks them there (a walk over global memory is n dependent loads), leaving per step the slot
+// whose token the hypothesis holds and the row that emitted it; then the CTA writes the ids and copies the n attention rows, 16 bytes at
+// a time when VEC (R % 4 == 0 and every row 16-byte aligned), zeros past the image's region count.  A parent outside [0, beam) reads as
+// slot 0, so foreign data cannot send the walk out of bounds.
+template <bool VEC>
+__global__ void __launch_bounds__(256) beam_backtrack_kernel(const int64_t* __restrict__ ids, const int64_t* __restrict__ parents,
+                                                             int64_t ids_stride_steps, int beam, int n, const float* __restrict__ alphas,
+                                                             int64_t alpha_row_stride, int R, const int32_t* __restrict__ reg_off,
+                                                             int lineage, int64_t* __restrict__ ids_out, float* __restrict__ att_out) {
+  extern __shared__ int32_t s_bt[];           // parents [n][beam], then slot [n] and row [n]
+  int32_t* s_slot = s_bt + n * beam;
+  int32_t* s_row = s_slot + n;
+  const int img = blockIdx.x / beam, s = blockIdx.x % beam, tid = threadIdx.x;
+  const int64_t src0 = (int64_t)img * ids_stride_steps * beam;
+  if (lineage) {
+    for (int j = tid; j < n * beam; j += blockDim.x) {
+      const int64_t p = parents[src0 + j];
+      s_bt[j] = (p >= 0 && p < beam) ? (int32_t)p : 0;
+    }
+    __syncthreads();
+    if (tid == 0) {
+      int cur = s;
+      for (int t = n - 1; t >= 0; t--) {
+        s_slot[t] = cur;
+        cur = s_bt[t * beam + cur];
+        s_row[t] = cur;
+      }
+    }
+  } else {
+    for (int t = tid; t < n; t += blockDim.x) s_slot[t] = s_row[t] = s;
+  }
+  __syncthreads();
+  const int64_t hyp = (int64_t)img * beam + s;
+  for (int t = tid; t < n; t += blockDim.x) ids_out[hyp * n + t] = ids[src0 + (int64_t)t * beam + s_slot[t]];
+  if (!att_out) return;
+  const int Ri = reg_off ? reg_off[img + 1] - reg_off[img] : R;
+  const float* src = alphas + (int64_t)img * beam * alpha_row_stride;
+  float* dst = att_out + hyp * n * R;
+  if (VEC) {
+    const int R4 = R / 4;
+    for (int j = tid; j < n * R4; j += blockDim.x) {
+      const int t = j / R4, q = j - t * R4;
+      const float* a = src + s_row[t] * alpha_row_stride + (int64_t)t * R + 4 * q;
+      float4 v;
+      if (4 * q + 3 < Ri) {
+        v = *(const float4*)a;
+      } else {
+        v.x = 4 * q < Ri ? a[0] : 0.f;
+        v.y = 4 * q + 1 < Ri ? a[1] : 0.f;
+        v.z = 4 * q + 2 < Ri ? a[2] : 0.f;
+        v.w = 0.f;
+      }
+      *(float4*)(dst + (int64_t)t * R + 4 * q) = v;
+    }
+  } else {
+    for (int j = tid; j < n * R; j += blockDim.x) {
+      const int t = j / R, r = j - t * R;
+      dst[j] = r < Ri ? src[s_row[t] * alpha_row_stride + (int64_t)t * R + r] : 0.f;
+    }
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ decode loops of both flavours
 // A flavour F hands the loops F::c: the step's logits [B][V], device scratch of B rows each and the ragged attention state
 // (rg.reg_off NULL: every image has R regions) of rpi rows per image; F::prologue(st); F::step(t, st): the cell step fed next_tok
@@ -2249,6 +2312,40 @@ int lo_decoder_beam_div(const lo_decoder_args* a, int64_t start_id, int64_t end_
   TorchDecode f(a, start_id, finished, finished + a->B);
   return beam_loop(f, BeamArgs{a->rows_per_img, div_gamma, div_prob, div_u, div_state}, end_id, max_steps, ids, parents, fin_hist, logp,
                    (cudaStream_t)stream);
+}
+
+int lo_beam_backtrack(const int64_t* ids, const int64_t* parents, int64_t ids_stride_steps, int n_img, int beam, int n,
+                      const float* alphas, int64_t alpha_row_stride, int R, const int32_t* reg_off, const int32_t* reg_off_host,
+                      int mode, int64_t* ids_out, float* att_out, void* stream) {
+  LO_CHECK_ARG(ids && parents && ids_out, "null ids / parents / ids_out");
+  LO_CHECK_ARG(!alphas == !att_out, "alphas and att_out must be set together");
+  LO_CHECK_ARG(n_img >= 1 && beam >= 1 && beam <= LO_BEAM_MAX, "n_img >= 1 and 1 <= beam <= 16");
+  LO_CHECK_ARG(n >= 1 && n <= ids_stride_steps, "1 <= n <= ids_stride_steps");
+  LO_CHECK_ARG(mode == LO_BEAM_SLOTS || mode == LO_BEAM_LINEAGE, "mode must be LO_BEAM_SLOTS or LO_BEAM_LINEAGE");
+  const size_t smem = (size_t)n * (beam + 2) * 4;
+  LO_CHECK_ARG(smem <= 48 * 1024, "n * (beam + 2) * 4 bytes of parents and walk exceed 48 kB of shared memory");
+  bool vec = false;
+  if (att_out) {
+    LO_CHECK_ARG(R >= 1 && (int64_t)n * R <= INT32_MAX, "1 <= R and n * R < 2^31");
+    LO_CHECK_ARG(alpha_row_stride >= (int64_t)n * R, "alpha_row_stride >= n * R");
+    LO_CHECK_ARG(!reg_off == !reg_off_host, "reg_off and reg_off_host must be set together");
+    if (reg_off_host)
+      for (int i = 0; i < n_img; i++) {
+        const int c = reg_off_host[i + 1] - reg_off_host[i];
+        LO_CHECK_ARG(c >= 1 && c <= R, "region count of every image in 1..R (reg_off_host)");
+      }
+    vec = R % 4 == 0 && alpha_row_stride % 4 == 0 && (uintptr_t)alphas % 16 == 0 && (uintptr_t)att_out % 16 == 0;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  const int lineage = mode == LO_BEAM_LINEAGE;
+  if (vec)
+    beam_backtrack_kernel<true><<<n_img * beam, 256, smem, st>>>(ids, parents, ids_stride_steps, beam, n, alphas, alpha_row_stride, R,
+                                                                 reg_off, lineage, ids_out, att_out);
+  else
+    beam_backtrack_kernel<false><<<n_img * beam, 256, smem, st>>>(ids, parents, ids_stride_steps, beam, n, alphas, alpha_row_stride, R,
+                                                                  reg_off, lineage, ids_out, att_out);
+  LO_LAUNCH_OK();
+  return LO_OK;
 }
 
 }  // extern "C"

@@ -95,6 +95,26 @@ def run_beam(call, N, beam, steps, V, device, div_u=None, order=None):
     return ids[:, :n], parents[:, :n], logp
 
 
+def beam_hypotheses(ids, parents, finalize, a=None, alphas=None):
+    """The hypotheses of run_beam's ``ids`` / ``parents`` [N, n, beam] (device) as ids [N, beam, n] and, with ``alphas``, their
+    attention weights [N, beam, n, R] (lo_beam_backtrack), both on the device.  ``finalize``: 'reference' (slot s of every step, the
+    reference's identity finalize) or 'backtrack' (the lineage of the final slot s).  ``alphas``: the decode's attention rows [B, T, R]
+    (row b = image b // beam, slot b % beam); ``a``: the decode's args, whose region offsets (reg_off) give each image's own count
+    (entries past it are 0).  Returns (ids, attention or None)."""
+    N, n, beam = ids.shape
+    out = torch.empty(N, beam, n, dtype=torch.int64, device=ids.device)
+    att = None
+    if alphas is not None:
+        att = torch.empty(N, beam, n, alphas.shape[2], dtype=torch.float32, device=ids.device)
+    mode = _lib.LO_BEAM_LINEAGE if finalize == "backtrack" else _lib.LO_BEAM_SLOTS
+    check(_lib.lib().lo_beam_backtrack(ids.data_ptr(), parents.data_ptr(), ids.stride(0) // beam, N, beam, n,
+                                       alphas.data_ptr() if att is not None else None, alphas.stride(0) if att is not None else 0,
+                                       alphas.shape[2] if att is not None else 0, a.reg_off if a is not None else None,
+                                       a.reg_off_host if a is not None else None, mode, out.data_ptr(),
+                                       att.data_ptr() if att is not None else None, stream_ptr()))
+    return out, att
+
+
 def _image(x):
     """one image of a list: [1,H,W] tensor (uint8 or float) on the CPU or the GPU"""
     t = x if torch.is_tensor(x) else torch.from_numpy(x).permute(2, 0, 1)      # HxWx1 array -> [1,H,W]
@@ -208,12 +228,17 @@ def attention_maps(alphas, att_h, att_w):
 
 
 def beam_decode(model, img, start_id, end_id, beam_size=5, max_length_formula=150, finalize="reference",
-                div_gamma=1, div_prob=0, div_u=None, div_seed=None):
+                div_gamma=1, div_prob=0, div_u=None, div_seed=None, return_attention=False):
     """Returns (ids [N, beam, steps], log_probs [N, beam]) on the CPU; hypothesis 0 is the one the reference scores
     (img2seq.py:210).  ``div_gamma`` / ``div_prob``: the diversity penalty of beam_search_decoder_cell.py:258-287 (off when
     gamma == 1 or prob == 0, as in configs/model.json:15-16); its Bernoulli draws come from the in-kernel Philox stream seeded
     by ``div_seed`` (default: torch's initial seed), or from ``div_u`` — uniforms [steps, N*beam, V] — when given (tests).  For a
-    list of images, results are in input order and image i draws the rows [i*beam, (i+1)*beam) of ``div_u``."""
+    list of images, results are in input order and image i draws the rows [i*beam, (i+1)*beam) of ``div_u``.
+
+    ``return_attention=True`` also returns the attention weights of every hypothesis, [N, beam, steps, R] fp32 on the CPU (a list
+    of [beam, steps, R_i] for a list of images): under ``finalize='reference'`` the rows slot s computed at each step, what the
+    reference's attention_mechanism.ctx_vector holds and visualize_attention.py draws for s = 0; under ``'backtrack'`` the
+    attention under which each token of the hypothesis was chosen (the rows of a teacher-forced pass over its tokens)."""
     if finalize not in ("reference", "backtrack"):
         raise NotImplementedError("finalize must be 'reference' or 'backtrack'")
     L = _lib.lib()
@@ -233,19 +258,20 @@ def beam_decode(model, img, start_id, end_id, beam_size=5, max_length_formula=15
                                          stream_ptr())
         ids, parents, logp = run_beam(call, N, beam_size, max_steps, a.V, dev, div_u if div_on else None,
                                       lay.order if lay else None)
-        n = ids.shape[1]
-        ids, parents, logp = ids.cpu(), parents.cpu(), logp.cpu()
+        att = None
+        if return_attention or finalize == "backtrack":
+            alphas = ws["t"]["alphas"].view(-1)[:a.B * a.T * a.R].view(a.B, a.T, a.R) if return_attention else None
+            ids, att = beam_hypotheses(ids, parents, finalize, a, alphas)
+            ids, att = ids.cpu(), att.cpu() if att is not None else None
+        else:
+            ids = ids.cpu().permute(0, 2, 1).contiguous()     # [N, beam, time] like img2seq.py:239-241
+        logp = logp.cpu()
         if lay is not None:
             inv = _inverse(lay.order)
-            ids, parents, logp = ids[inv], parents[inv], logp[inv]
-        if finalize == "backtrack":
-            out = torch.zeros_like(ids)
-            cur = torch.arange(beam_size).unsqueeze(0).repeat(N, 1)
-            for t in range(n - 1, -1, -1):
-                out[:, t] = torch.gather(ids[:, t], 1, cur)
-                cur = torch.gather(parents[:, t], 1, cur)
-            ids = out
-        return ids.permute(0, 2, 1).contiguous(), logp      # [N, beam, time] like img2seq.py:239-241
+            ids, logp = ids[inv], logp[inv]
+            if att is not None:
+                att = [att[j, :, :, :lay.counts[j]].clone() for j in inv.tolist()]
+        return (ids, logp, att) if return_attention else (ids, logp)
 
 
 def truncate_end(list_of_ids, id_end):

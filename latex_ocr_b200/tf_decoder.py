@@ -351,8 +351,10 @@ class Decoder(nn.Module):
         ws["counts"], ws["off"] = [int(n) for n in counts], off
         return ws
 
-    def decode_packed(self, ws, steps, div_u=None, return_attention=False, return_log_probs=False):
+    def decode_packed(self, ws, steps, div_u=None, return_attention=False, return_log_probs=False, finalize="reference"):
         """decode() over the images packed in ``ws`` by packed_workspace: every image attends over its own regions only."""
+        if finalize not in ("reference", "backtrack"):
+            raise NotImplementedError("finalize must be 'reference' or 'backtrack'")
         counts = ws["counts"]
         N, beam = len(counts), self._tiles
         R = max(counts)
@@ -361,23 +363,32 @@ class Decoder(nn.Module):
             L, ws, a = self._args(ws["enc"], N * beam, steps, R, rows_per_img=beam, ws=ws)
             decode.set_region_offsets(a, ws["reg_off_host"], ws["reg_off"], ws["off"])
             alphas = ws["alphas"][:N * beam * steps * R].view(N * beam, steps, R) if return_attention else None
-            out = self._run_decode(L, a, N, steps, div_u, alphas, return_log_probs)
-            if alphas is not None and self.decoding == "greedy":
-                out, att = out
-                return out, [att[i, :, :counts[i]].clone() for i in range(N)]
-            return out
+            out = self._run_decode(L, a, N, steps, div_u, alphas, return_log_probs, finalize)
+            if alphas is None:
+                return out
+            att = out[-1]
+            if self.decoding == "greedy":
+                return out[:-1] + ([att[i, :, :counts[i]].clone() for i in range(N)],)
+            return out[:-1] + ([att[i, :, :, :counts[i]].clone() for i in range(N)],)
 
-    def decode(self, enc, max_steps=None, div_u=None, return_attention=False, return_log_probs=False):
+    def decode(self, enc, max_steps=None, div_u=None, return_attention=False, return_log_probs=False, finalize="reference"):
         """dynamic_decode(decoder_cell, max_length_formula + 1) (decoder.py:70): at most max_length_formula + 2 steps, stops when
         every row / beam has emitted END.  Returns DecoderOutput(logits=None, ids).  ``div_u`` (tests): injected uniforms
-        [steps, N*beam, V] for the diversity penalty; ``return_attention`` (greedy): also the attention weights [N, steps, R]
-        (the tensor attention_mechanism.py:96-121 hands to visualize_attention.py); ``return_log_probs`` (beam search): also the
-        log-probs of the hypotheses [N, beam].
+        [steps, N*beam, V] for the diversity penalty; ``return_log_probs`` (beam search): also the log-probs of the hypotheses
+        [N, beam]; ``return_attention``: also the attention weights (the tensor attention_mechanism.py:96-121 hands to
+        visualize_attention.py), after the log-probs: greedy [N, steps, R], beam search [N, beam, steps, R].
+        ``finalize`` (beam search): 'reference' returns the reference's identity finalize (ids[:, t, s] is what slot s chose at step
+        t) and the rows slot s computed, what visualize_attention.py draws for s = 0; 'backtrack' returns lineage-consistent
+        hypotheses, ids [N, steps, beam] followed back from each final slot, and the attention under which each of their tokens
+        was chosen (the rows of a teacher-forced pass over the hypothesis).
 
         ``enc`` [N,R,C] / [N,H,W,C], or a list of the encoder outputs of images of different sizes, each [H_i,W_i,C] or [R_i,C]:
         the list is decoded in one time loop in which every image attends over its own regions only (lo_tfdec_args.reg_off), so
         an image's ids do not depend on the other images of the call.  Ids come back in input order, image i draws the rows
-        [i*beam, (i+1)*beam) of ``div_u``, and ``return_attention`` gives a list of [steps, R_i] tensors."""
+        [i*beam, (i+1)*beam) of ``div_u``, and ``return_attention`` gives a list of [steps, R_i] (greedy) or [beam, steps, R_i]
+        tensors."""
+        if finalize not in ("reference", "backtrack"):
+            raise NotImplementedError("finalize must be 'reference' or 'backtrack'")
         steps = int(max_steps) if max_steps is not None else self.max_length_formula + 2
         if isinstance(enc, (list, tuple)):
             encs = [self._enc_regions(e) for e in enc]
@@ -385,14 +396,14 @@ class Decoder(nn.Module):
             off = ws["off"]
             for i, e in enumerate(encs):
                 ws["enc"][off[i]:off[i + 1]].copy_(e)
-            return self.decode_packed(ws, steps, div_u, return_attention, return_log_probs)
+            return self.decode_packed(ws, steps, div_u, return_attention, return_log_probs, finalize)
         enc = self._enc(enc)
         N, R, _ = enc.shape
         self.store.refresh_shadow()
         with torch.no_grad():
             L, ws, a = self._args(enc, N * self._tiles, steps, R, rows_per_img=self._tiles, decode=True)
             ws["enc"] = enc
-            return self._run_decode(L, a, N, steps, div_u, ws["alphas"] if return_attention else None, return_log_probs)
+            return self._run_decode(L, a, N, steps, div_u, ws["alphas"] if return_attention else None, return_log_probs, finalize)
 
     def _enc_regions(self, e):
         """one image's encoder output of a list -> [R_i, C] on the device"""
@@ -404,9 +415,9 @@ class Decoder(nn.Module):
             raise ValueError("each image's encoder output must be [H,W,%d] or [R,%d] (got shape %s)" % (self.C, self.C, tuple(e.shape)))
         return e
 
-    def _run_decode(self, L, a, N, steps, div_u, alphas, return_log_probs):
-        """The greedy or beam decode of the filled args ``a`` (N images); ``alphas`` [N, steps', R] (greedy attention export) or
-        None."""
+    def _run_decode(self, L, a, N, steps, div_u, alphas, return_log_probs, finalize="reference"):
+        """The greedy or beam decode of the filled args ``a`` (N images); ``alphas``: the attention rows [B, steps, R] of the call
+        (attention export) or None."""
         dev = self.store.device
         if self.decoding == "greedy":
             ids = decode.run_greedy(lambda tokens, fin: L.lo_tfdec_greedy(ctypes.byref(a), self._id_end, steps, tokens, fin,
@@ -425,11 +436,15 @@ class Decoder(nn.Module):
         def call(ids, parents, fin, logp, u):
             return L.lo_tfdec_beam_div(ctypes.byref(a), self._id_end, steps, ids, parents, fin, logp, self.div_gamma, self.div_prob, u,
                                        state, stream_ptr())
-        ids, _, logp = decode.run_beam(call, N, self._tiles, steps, self.V, dev, div_u if div_on else None)
+        ids, parents, logp = decode.run_beam(call, N, self._tiles, steps, self.V, dev, div_u if div_on else None)
         # finalize (beam_search_decoder_cell.py:189-250) gathers with the unchanged initial parents -> identity (SURVEY §8-A.3)
-        if return_log_probs:
-            return DecoderOutput(None, ids), logp
-        return DecoderOutput(None, ids)
+        att = None
+        if alphas is not None or finalize == "backtrack":
+            hyp, att = decode.beam_hypotheses(ids, parents, finalize, a, alphas)
+            if finalize == "backtrack":
+                ids = hyp.permute(0, 2, 1).contiguous()
+        out = (DecoderOutput(None, ids),) + ((logp,) if return_log_probs else ()) + ((att,) if alphas is not None else ())
+        return out if len(out) > 1 else out[0]
 
     def forward(self, img, formula=None, dropout=1.0):
         """Decoder.__call__(img, formula, dropout) (decoder.py:24): (pred_train, pred_test).  dropout is the TF keep_prob; the

@@ -78,7 +78,8 @@ int64_t lo_launch_count(void);
  *   conv_persist     1 [p]    1: persistent double-accumulator convolution kernel; 0: one tile per CTA
  *   conv_mt2         1 [p]    1: layers with <= 128 output channels: two 128-position sub-tiles per CTA share each weight stage
  *   conv_mc          1        1: cluster-of-2 multicast of the A tile in the wgmma GEMM
- *   wgrad256         0 [p]    1: conv weight gradient with 128 x 256 tiles when Cin % 256 == 0; off: two 96 KB stages cannot hide the loads
+ *   wgrad256         0 [p]    1: the TN weight-gradient GEMMs also run 128 x 256 tiles when N % 256 == 0 (the conv weight gradient
+ *                             always does when Cin % 256 == 0); off: slower on two of the decoder backward's four such GEMMs
  *   deterministic    0        1: cross-CTA sums of the train step add in a fixed order, bit-reproducible but slower; 0: fp32 atomics
  *   dbg_skip         0        timing aid, results garbage: skips bwd hoisted part (1), loop attention (2), loop GEMM/LSTM (4), fwd hoisted (8)
  *   l2_persist_mb    0        an action: sets the persisting-L2 set-aside to value MiB (0: driver default); reads back the last value set

@@ -1423,9 +1423,10 @@ static inline bool use_cluster(int ns, int R) {
   return g_opt_att_cluster && ns >= 2 && ns <= 8 && ((R + ns - 1) / ns) * 4 <= 16 * 1024;
 }
 
-// Resident CTAs of `kernel` at `smem` bytes of dynamic shared memory on the whole device.  Queried once per (device, kernel,
-// shared memory) and cached: the launch paths call this on every step, also while a CUDA graph is being captured.
-static int att_resident_ctas(const void* kernel, size_t smem) {
+// Resident CTAs of `kernel` (blocks of `threads`) at `smem` bytes of dynamic shared memory on the whole device; 0 if the query
+// fails.  Queried once per (device, kernel, shared memory) and cached: the launch paths call this on every step, also while a
+// CUDA graph is being captured.
+int resident_ctas(const void* kernel, int threads, size_t smem) {
   struct Entry { int dev; const void* k; size_t smem; int ctas; };
   static std::mutex mu;
   static std::vector<Entry> cache;
@@ -1435,10 +1436,10 @@ static int att_resident_ctas(const void* kernel, size_t smem) {
   for (const Entry& e : cache)
     if (e.dev == dev && e.k == kernel && e.smem == smem) return e.ctas;
   int per_sm = 0, sms = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, AP_THREADS, smem) != cudaSuccess ||
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem) != cudaSuccess ||
       cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) {
     cudaGetLastError();
-    return 0;                    // unknown: the caller keeps the cluster launch
+    return 0;
   }
   cache.push_back({dev, kernel, smem, per_sm * sms});
   return per_sm * sms;
@@ -1452,7 +1453,7 @@ static int att_resident_ctas(const void* kernel, size_t smem) {
 static bool att_grid_cluster(const void* free_kernel, size_t free_smem, int ns, int B, int R) {
   if (!use_cluster(ns, R)) return false;
   if (g_opt_att_cluster != 1) return true;
-  return att_resident_ctas(free_kernel, free_smem) < ns * B;
+  return resident_ctas(free_kernel, AP_THREADS, free_smem) < ns * B;       // 0 (unknown): keep the cluster launch
 }
 
 template <typename T, int NVA, int NVC, int ACT, bool MK>

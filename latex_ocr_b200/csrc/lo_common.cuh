@@ -77,7 +77,7 @@ constexpr int LO_NUM_SMS = 132;
   X(g_opt_conv_persist, "conv_persist", 1)        /* persistent double-accumulator conv kernel */              \
   X(g_opt_conv_mt2, "conv_mt2", 1)                /* two position sub-tiles share a weight stage */            \
   X(g_opt_conv_mc, "conv_mc", 1)                  /* cluster-of-2 multicast of the A tile */                   \
-  X(g_opt_wgrad256, "wgrad256", 0)                /* 128 x 256 conv weight-gradient tiles */                   \
+  X(g_opt_wgrad256, "wgrad256", 0)                /* 128 x 256 tiles also for the TN weight-gradient GEMMs */  \
   X(g_opt_det, "deterministic", 0)                /* fixed-order cross-CTA sums */                             \
   X(g_opt_dbg_skip, "dbg_skip", 0)                /* timing dissection: skip launch groups */                  \
   X(g_opt_l2_persist_mb, "l2_persist_mb", 0)      /* last persisting-L2 set-aside set, MiB */
@@ -365,6 +365,7 @@ int tc_gemm_nt_lstm(const bf16* A, int64_t lda, const bf16* Wil, int64_t ldw, in
 int skinny_gemm_nt_lstm(const bf16* A, int64_t lda, const bf16* Wil, int64_t ldw, int M, int D, int K, const TcLstmEpi& e, cudaStream_t st);
 int skinny_gemm_nt(const bf16* A, int64_t lda, const bf16* W, int64_t ldw, float* C, int64_t ldc, int M, int N, int K, const float* bias,
                    int splits, int atomic_acc, cudaStream_t st);
+int resident_ctas(const void* kernel, int threads, size_t smem);
 int tc_gemm_tn(const bf16* A, int64_t lda, const bf16* B, int64_t ldb, float* C, int64_t ldc, int M, int N, int K, cudaStream_t st);
 int tc_gemm_tn_batched(const bf16* A, int64_t sAk, int64_t sAb, const bf16* B, int64_t sBk, int64_t sBb, float* C, int64_t ldc,
                        int64_t sCb, int M, int N, int K, int batch, cudaStream_t st);

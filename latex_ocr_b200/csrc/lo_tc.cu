@@ -516,10 +516,13 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_conv_p_kernel(const __grid_c
 // ------------------------------------------------------------------------------------------------
 // Weight gradient on wgmma:  dW[co][tap][ci] += sum_p dY[p][co] * X[p + tap][ci]
 // GEMM view: M = co (128), N = ci (NT), K = output positions.  Both operands are "MN-major" (the channel index is
-// contiguous in NHWC), which wgmma takes directly (transpose flags): smem tile = [128 positions][64 channels] (one TMA
+// contiguous in NHWC), which wgmma takes directly (transpose flags): smem tile = [KP positions][64 channels] (one TMA
 // box, SWIZZLE_128B), descriptor LBO = distance between 64-channel boxes, SBO = 1024 B (8 positions), 16 positions
-// (2048 B) per MMA.  grid: (co tiles * ci tiles, 9 taps, K splits); the splits add their partial sums onto dW with fp32 atomics,
-// or — option "deterministic" — form one cluster (<= 8) whose rank 0 adds them in split order and alone adds the result.
+// (2048 B) per MMA.  KP = 128 positions per K block, or 64 for the 128 x 256 tiles (16 KB of dY + 32 KB of X per
+// stage, four stages): the host then cuts every 128-position box into two 64-position boxes in the same row-major order and
+// doubles the split length, so each output element sees the same sequence of k16 MMAs.  grid: (co tiles * ci tiles,
+// 9 taps, K splits); the splits add their partial sums onto dW with fp32 atomics, or — option "deterministic" — form one
+// cluster (<= 8) whose rank 0 adds them in split order and alone adds the result.
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint64_t make_mnmajor_sw128_desc(uint32_t saddr, uint32_t lbo_bytes) {
   uint64_t d = 0;
@@ -541,10 +544,10 @@ struct WgParams {
   int ordered;        // 1: the K splits of a tile are one cluster, summed in split order (option "deterministic")
 };
 
-template <int NT, int STAGES>
+template <int NT, int KP, int STAGES>
 __global__ void __launch_bounds__(TC_THREADS, 1) tc_wgrad_kernel(const __grid_constant__ CUtensorMap mapDY,
                                                                   const __grid_constant__ CUtensorMap mapX, WgParams p) {
-  constexpr int BOX = 128 * 64 * 2;                 // one [128 pos][64 ch] box
+  constexpr int BOX = KP * 64 * 2;                  // one [KP pos][64 ch] box
   constexpr int A_BYTES = 2 * BOX, B_BYTES = (NT / 64) * BOX, STAGE_BYTES = A_BYTES + B_BYTES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -578,11 +581,11 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_wgrad_kernel(const __grid_co
         uint8_t* sa = smem + s * STAGE_BYTES;
         mbar_expect_tx(full_bar + s, A_BYTES);
         if (p.plain == 2) {
-          tma_load_3d(sa, &mapDY, full_bar + s, co0, ks * 128, bz);
-          tma_load_3d(sa + BOX, &mapDY, full_bar + s, co0 + 64, ks * 128, bz);
+          tma_load_3d(sa, &mapDY, full_bar + s, co0, ks * KP, bz);
+          tma_load_3d(sa + BOX, &mapDY, full_bar + s, co0 + 64, ks * KP, bz);
         } else if (p.plain) {
-          tma_load_2d(sa, &mapDY, full_bar + s, co0, ks * 128);
-          tma_load_2d(sa + BOX, &mapDY, full_bar + s, co0 + 64, ks * 128);
+          tma_load_2d(sa, &mapDY, full_bar + s, co0, ks * KP);
+          tma_load_2d(sa + BOX, &mapDY, full_bar + s, co0 + 64, ks * KP);
         } else {
           tma_load_4d(sa, &mapDY, full_bar + s, co0, w0, h0, img);
           tma_load_4d(sa + BOX, &mapDY, full_bar + s, co0 + 64, w0, h0, img);
@@ -604,10 +607,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_wgrad_kernel(const __grid_co
         mbar_expect_tx(full_bar + s, B_BYTES);
         if (p.plain == 2) {
 #pragma unroll
-          for (int j = 0; j < NT / 64; j++) tma_load_3d(sb + j * BOX, &mapX, full_bar + s, ci0 + 64 * j, ks * 128, bz);
+          for (int j = 0; j < NT / 64; j++) tma_load_3d(sb + j * BOX, &mapX, full_bar + s, ci0 + 64 * j, ks * KP, bz);
         } else if (p.plain) {
 #pragma unroll
-          for (int j = 0; j < NT / 64; j++) tma_load_2d(sb + j * BOX, &mapX, full_bar + s, ci0 + 64 * j, ks * 128);
+          for (int j = 0; j < NT / 64; j++) tma_load_2d(sb + j * BOX, &mapX, full_bar + s, ci0 + 64 * j, ks * KP);
         } else {
 #pragma unroll
           for (int j = 0; j < NT / 64; j++)
@@ -629,7 +632,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_wgrad_kernel(const __grid_co
       const uint32_t sb = smem_u32(smem + s * STAGE_BYTES) + A_BYTES;
       wgmma_fence();
 #pragma unroll
-      for (int k = 0; k < 8; k++)
+      for (int k = 0; k < KP / 16; k++)
         Wgmma<NT, 1, 1>::mma(acc, make_mnmajor_sw128_desc(sa + k * 2048, BOX), make_mnmajor_sw128_desc(sb + k * 2048, BOX), 1u);
       wgmma_commit();
       wgmma_wait0();
@@ -928,18 +931,59 @@ int tc_conv3x3(const bf16* x, const bf16* w, const float* bias, const bf16* mask
 }
 
 
-template <int NT, int STAGES>
-static int launch_wgrad(const CUtensorMap& mDY, const CUtensorMap& mX, const WgParams& p, dim3 grid, cudaStream_t st) {
-  constexpr int TOTAL = STAGES * (2 + NT / 64) * 16384 + 1024 + 256;
+// K splits of a weight-gradient launch of `tiles` CTA tiles over `kstages` K blocks when `slots` CTAs are resident at once.
+// The kernel holds one CTA per SM, so a short last wave takes about as long as a full one: the fewest CTAs whose last wave
+// is at least 90 % full, every split keeping at least `min_ks` K blocks (a full ring); failing that, the fullest last wave.
+static int whole_wave_splits(int tiles, int kstages, int min_ks, int slots) {
+  int best = 1;
+  double best_fill = -1.0;
+  const int smax = kstages / min_ks > 1 ? kstages / min_ks : 1;
+  for (int s = 1; s <= smax; s++) {
+    const int splits = cdiv(kstages, cdiv(kstages, s));      // the count the rounded-up split length gives
+    const long ctas = (long)tiles * splits;
+    const double fill = (double)ctas / ((double)((ctas + slots - 1) / slots) * slots);
+    if (fill >= 0.9) return splits;
+    if (fill > best_fill) { best_fill = fill; best = splits; }
+  }
+  return best;
+}
+
+// One weight-gradient launch over a grid of (tiles_x, tiles_y) output tiles; p.kstages counts K blocks of KP positions.
+// split_k: the K blocks are cut into splits along grid.z (whole waves, or with option "deterministic" the decomposition its
+// ordered cluster sum was built on: two CTAs per SM targeted, at most 8 splits, counted for 128-channel tiles of 128-position
+// blocks, so the split boundaries fall on the same positions for either tile shape).
+template <int NT, int KP, int STAGES>
+static int launch_wgrad(const CUtensorMap& mDY, const CUtensorMap& mX, WgParams& p, int tiles_x, int tiles_y, bool split_k,
+                        cudaStream_t st) {
+  constexpr int TOTAL = STAGES * (2 + NT / 64) * KP * 128 + 1024 + 256;
   static bool attr_set = false;
   if (!attr_set) {
-    LO_CUDA(cudaFuncSetAttribute(tc_wgrad_kernel<NT, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, TOTAL));
+    LO_CUDA(cudaFuncSetAttribute(tc_wgrad_kernel<NT, KP, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, TOTAL));
     attr_set = true;
   }
+  const int tiles = tiles_x * tiles_y;
+  if (!split_k) {
+    p.per_split = p.kstages;
+  } else if (g_opt_det) {
+    constexpr int PB = 128 / KP;                                // K blocks per 128 positions
+    const int ks128 = cdiv(p.kstages, PB);
+    int s = cdiv(LO_NUM_SMS * 2, NT == 256 ? 2 * tiles : tiles);
+    if (s > 8) s = 8;
+    if (s > ks128) s = ks128;
+    if (s < 1) s = 1;
+    p.per_split = cdiv(ks128, s) * PB;
+  } else {
+    const int slots = resident_ctas((const void*)tc_wgrad_kernel<NT, KP, STAGES>, TC_THREADS, TOTAL);
+    if (slots <= 0) return fail(LO_ECUDA, "%s: occupancy query failed", __func__);
+    p.per_split = cdiv(p.kstages, whole_wave_splits(tiles, p.kstages, STAGES, slots));
+  }
+  const int splits = cdiv(p.kstages, p.per_split);
+  p.ordered = g_opt_det && splits > 1;
+  const dim3 grid(tiles_x, tiles_y, splits);
   if (p.ordered)
-    LO_CUDA(launch_cluster(tc_wgrad_kernel<NT, STAGES>, grid, dim3(TC_THREADS), (size_t)TOTAL, st, dim3(1, 1, grid.z), false, mDY, mX, p));
+    LO_CUDA(launch_cluster(tc_wgrad_kernel<NT, KP, STAGES>, grid, dim3(TC_THREADS), (size_t)TOTAL, st, dim3(1, 1, splits), false, mDY, mX, p));
   else
-    tc_wgrad_kernel<NT, STAGES><<<grid, TC_THREADS, TOTAL, st>>>(mDY, mX, p);
+    tc_wgrad_kernel<NT, KP, STAGES><<<grid, TC_THREADS, TOTAL, st>>>(mDY, mX, p);
   LO_LAUNCH_OK();
   return LO_OK;
 }
@@ -952,39 +996,37 @@ int tc_conv3x3_wgrad(const bf16* x, const bf16* dy, float* dw, int N, int H, int
   int BW = 128;
   while (BW > 8 && BW / 2 >= Wo) BW /= 2;
   const int BH = 128 / BW;
+  // 128 (co) x 256 (ci) tiles when Cin allows it: 87 instead of 64 FLOP per byte pulled from L2, on 64-position K blocks
+  const int NT = Cin % 256 == 0 ? 256 : (Cin >= 128 ? 128 : 64);
+  WgParams p{};
+  p.Cin = Cin; p.Cout = Cout; p.Ho = Ho; p.Wo = Wo; p.pad = pad;
+  p.BW = BW; p.BH = BH; p.tiles_w = cdiv(Wo, BW); p.tiles_h = cdiv(Ho, BH);
+  if (NT == 256) {
+    // each 128-position box BW x BH becomes two 64-position boxes in the same row-major order: its upper and lower half
+    // rows, or (one row of 128) its left and right half
+    if (BH >= 2) { p.BH = BH / 2; p.tiles_h *= 2; }
+    else { p.BW = BW / 2; p.tiles_w *= 2; }
+  }
+  p.kstages = N * p.tiles_w * p.tiles_h;
+  p.dw = dw;
+  p.ci_tiles = Cin / NT;
   CUtensorMap mDY, mX;
   {
     cuuint64_t dims[4] = {(cuuint64_t)Cout, (cuuint64_t)Wo, (cuuint64_t)Ho, (cuuint64_t)N};
     cuuint64_t str[3] = {(cuuint64_t)Cout * 2, (cuuint64_t)Wo * Cout * 2, (cuuint64_t)Ho * Wo * Cout * 2};
-    cuuint32_t box[4] = {64, (cuuint32_t)BW, (cuuint32_t)BH, 1};
+    cuuint32_t box[4] = {64, (cuuint32_t)p.BW, (cuuint32_t)p.BH, 1};
     LO_TRY(make_map(&mDY, dy, 4, dims, str, box));
   }
   {
     cuuint64_t dims[4] = {(cuuint64_t)Cin, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
     cuuint64_t str[3] = {(cuuint64_t)Cin * 2, (cuuint64_t)W * Cin * 2, (cuuint64_t)H * W * Cin * 2};
-    cuuint32_t box[4] = {64, (cuuint32_t)BW, (cuuint32_t)BH, 1};
+    cuuint32_t box[4] = {64, (cuuint32_t)p.BW, (cuuint32_t)p.BH, 1};
     LO_TRY(make_map(&mX, x, 4, dims, str, box));
   }
-  WgParams p{};
-  p.Cin = Cin; p.Cout = Cout; p.Ho = Ho; p.Wo = Wo; p.pad = pad;
-  p.BW = BW; p.BH = BH; p.tiles_w = cdiv(Wo, BW); p.tiles_h = cdiv(Ho, BH);
-  p.kstages = N * p.tiles_w * p.tiles_h;
-  p.dw = dw;
-  // 128 (co) x 256 (ci) tiles when Cin allows it: 87 instead of 64 FLOP per byte pulled from L2 (two 96 KB stages)
-  const int NT = (g_opt_wgrad256 && Cin % 256 == 0) ? 256 : (Cin >= 128 ? 128 : 64);
-  p.ci_tiles = Cin / NT;
-  const int tiles = (Cout / 128) * p.ci_tiles * 9;
-  int splits = cdiv(NT == 256 ? LO_NUM_SMS : LO_NUM_SMS * 2, tiles);
-  if (g_opt_det && splits > 8) splits = 8;      // ordered: the splits of a tile are summed inside one (portable) cluster
-  if (splits > p.kstages) splits = p.kstages;
-  if (splits < 1) splits = 1;
-  p.per_split = cdiv(p.kstages, splits);
-  splits = cdiv(p.kstages, p.per_split);
-  p.ordered = g_opt_det && splits > 1;
-  dim3 grid((Cout / 128) * p.ci_tiles, 9, splits);
-  if (NT == 256) return launch_wgrad<256, 2>(mDY, mX, p, grid, st);
-  if (NT == 128) return launch_wgrad<128, 3>(mDY, mX, p, grid, st);
-  return launch_wgrad<64, 4>(mDY, mX, p, grid, st);
+  const int tiles_x = (Cout / 128) * p.ci_tiles;
+  if (NT == 256) return launch_wgrad<256, 64, 4>(mDY, mX, p, tiles_x, 9, true, st);
+  if (NT == 128) return launch_wgrad<128, 128, 3>(mDY, mX, p, tiles_x, 9, true, st);
+  return launch_wgrad<64, 128, 4>(mDY, mX, p, tiles_x, 9, true, st);
 }
 
 // C[M][N] (fp32, ldc) += A[K][M]^T * B[K][N]; A, B bf16 row-major.  C must hold the values to accumulate onto
@@ -993,37 +1035,32 @@ int tc_gemm_tn(const bf16* A, int64_t lda, const bf16* B, int64_t ldb, float* C,
   if (!tc_available()) return fail(LO_ENOTSUP, "%s: needs an sm_90 device", __func__);
   LO_CHECK_ARG(lda % 8 == 0 && ldb % 8 == 0, "lda%8, ldb%8");
   LO_CHECK_ARG(((uintptr_t)A & 15) == 0 && ((uintptr_t)B & 15) == 0, "16-byte alignment");
+  // 128 x 128 tiles by default also where N % 256 == 0: with the decoder's K = B * T a split runs few K blocks, and the
+  // 128 x 256 grid needs twice the splits (twice the fp32 atomics); measured slower on two of its four such GEMMs (DESIGN.md §8)
+  const int NT = (g_opt_wgrad256 && N % 256 == 0) ? 256 : (N > 64 ? 128 : 64);
+  const int KP = NT == 256 ? 64 : 128;                          // positions per K block
   CUtensorMap mA, mB;
   {
     cuuint64_t dims[2] = {(cuuint64_t)M, (cuuint64_t)K};
     cuuint64_t str[1] = {(cuuint64_t)lda * 2};
-    cuuint32_t box[2] = {64, 128};
+    cuuint32_t box[2] = {64, (cuuint32_t)KP};
     LO_TRY(make_map(&mA, A, 2, dims, str, box));
   }
   {
     cuuint64_t dims[2] = {(cuuint64_t)N, (cuuint64_t)K};
     cuuint64_t str[1] = {(cuuint64_t)ldb * 2};
-    cuuint32_t box[2] = {64, 128};
+    cuuint32_t box[2] = {64, (cuuint32_t)KP};
     LO_TRY(make_map(&mB, B, 2, dims, str, box));
   }
   WgParams p{};
   p.plain = 1; p.Cout = M; p.Cin = N; p.dw = C; p.ldc = ldc;
-  p.tiles_w = p.tiles_h = 1; p.BW = 128; p.BH = 1;
-  p.kstages = cdiv(K, 128);
-  const int NT = N > 64 ? 128 : 64;
+  p.tiles_w = p.tiles_h = 1; p.BW = KP; p.BH = 1;
+  p.kstages = cdiv(K, KP);
   p.ci_tiles = cdiv(N, NT);
-  const int mt = cdiv(M, 128);
-  const int tiles = mt * p.ci_tiles;
-  int splits = cdiv(LO_NUM_SMS * 2, tiles);
-  if (g_opt_det && splits > 8) splits = 8;
-  if (splits > p.kstages) splits = p.kstages;
-  if (splits < 1) splits = 1;
-  p.per_split = cdiv(p.kstages, splits);
-  splits = cdiv(p.kstages, p.per_split);
-  p.ordered = g_opt_det && splits > 1;
-  dim3 grid(mt * p.ci_tiles, 1, splits);
-  if (NT == 128) return launch_wgrad<128, 3>(mA, mB, p, grid, st);
-  return launch_wgrad<64, 4>(mA, mB, p, grid, st);
+  const int tiles_x = cdiv(M, 128) * p.ci_tiles;
+  if (NT == 256) return launch_wgrad<256, 64, 4>(mA, mB, p, tiles_x, 1, true, st);
+  if (NT == 128) return launch_wgrad<128, 128, 3>(mA, mB, p, tiles_x, 1, true, st);
+  return launch_wgrad<64, 128, 4>(mA, mB, p, tiles_x, 1, true, st);
 }
 
 // Batched C[b][M][N] (fp32) += A[b][K][M]^T * B[b][K][N]; A, B bf16 with arbitrary (16-byte multiple) strides:
@@ -1050,13 +1087,11 @@ int tc_gemm_tn_batched(const bf16* A, int64_t sAk, int64_t sAb, const bf16* B, i
   WgParams p{};
   p.plain = 2; p.Cout = M; p.Cin = N; p.dw = C; p.ldc = ldc; p.batch_c = sCb;
   p.tiles_w = p.tiles_h = 1; p.BW = 128; p.BH = 1;
-  p.kstages = cdiv(K, 128);
-  p.per_split = p.kstages;                      // no split-K: the batch dimension supplies the parallelism
+  p.kstages = cdiv(K, 128);                     // no split-K: the batch dimension supplies the parallelism
   const int NT = N > 64 ? 128 : 64;
   p.ci_tiles = cdiv(N, NT);
-  dim3 grid(cdiv(M, 128) * p.ci_tiles, batch, 1);
-  if (NT == 128) return launch_wgrad<128, 3>(mA, mB, p, grid, st);
-  return launch_wgrad<64, 4>(mA, mB, p, grid, st);
+  if (NT == 128) return launch_wgrad<128, 128, 3>(mA, mB, p, cdiv(M, 128) * p.ci_tiles, batch, false, st);
+  return launch_wgrad<64, 128, 4>(mA, mB, p, cdiv(M, 128) * p.ci_tiles, batch, false, st);
 }
 
 }  // namespace lo

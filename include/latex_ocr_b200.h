@@ -67,10 +67,6 @@ int64_t lo_launch_count(void);
  *   att_maskbits     1 [p]    1: the forward attention kernel stores the ReLU mask bits, the backward streams them instead of att1
  *   att_bwd_mma      1 [p]    1: the 512-wide bf16 attention backward runs both contractions on mma.sync
  *   dec_streams      1 [p]    >= 2: the decoder time loop runs as two half-batch chains on two streams; also sets skinny8 = value < 2
- *   dec_fuse         0 [p]    1: grid-barrier fused forward step; off: measured no faster than the separate launches
- *   dec_fuse_bwd     0 [p]    1: grid-barrier fused backward step; off: two grid barriers cost more than two PDL boundaries
- *   dec_cl           0 [p]    1: cluster-fused forward step; off: slower, each CTA pulls its 320 KB weight slice through one SM
- *   dec_cl_bwd       0 [p]    1: cluster-fused backward step; off for the same reason
  *   fuse_lstm        0 [p]    1: LSTM cell in the gates GEMM's epilogue; off: it cannot hide the dependent loads the pointwise kernel hides
  *   skinny_mma       1 [p]    decoder per-step GEMMs (M <= 64) on mma.sync; 0: on wgmma
  *   skinny_tma       1 [p]    1: their operands by cp.async.bulk, one copy per row; 0: 16-byte cp.async
@@ -292,7 +288,7 @@ typedef struct lo_decoder_args {
    * is not differentiated: given fed, forward and backward are teacher forcing on the input sequence fed (the embedding and
    * weight_ih[:, :E] gradients go to the rows of the tokens fed); ce_kernel's targets stay caps[b][t+1].  In this mode the head
    * fc(hd_t) runs inside the time loop (one GEMM per step, writing only the rows active at step t) instead of once after it, and
-   * the forward always runs the default single-chain step loop: dec_fuse, dec_cl, fuse_lstm and dec_streams >= 2 are ignored.
+   * the forward always runs the default single-chain step loop: fuse_lstm and dec_streams >= 2 are ignored.
    * Refused (LO_EINVAL) before any GPU work: ss_prob without fed, without ss_u and dropout_state, with phase != 0, with
    * rows_per_img > 1, and on the greedy / beam entry points. */
   int64_t* fed;            /* [B][T] tokens fed at each step: written by the forward (positions past a row's decode length get

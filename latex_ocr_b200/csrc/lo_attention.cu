@@ -1693,8 +1693,6 @@ int attention_bwd_pipe(const AttBwdArgs& x, int dt, int C, cudaStream_t st) {
 namespace lo { extern long long* g_tc_dbg; }
 extern "C" int lo_debug_buffer(void* p) {
   lo::g_tc_dbg = (long long*)p;
-  LO_TRY(lo::cl_set_ts((long long*)p));
-  LO_TRY(lo::sk_set_ts((long long*)p));
 #ifdef LO_ATT_TIMING
   long long* q = (long long*)p;
   LO_CUDA(cudaMemcpyToSymbol(lo::g_att_ts, &q, sizeof(q)));

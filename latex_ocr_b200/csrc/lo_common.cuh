@@ -66,10 +66,6 @@ constexpr int LO_NUM_SMS = 132;
   X(g_opt_att_maskbits, "att_maskbits", 1)        /* ReLU mask bits instead of att1 in the backward */         \
   X(g_opt_att_bwd_mma, "att_bwd_mma", 1)          /* 512-wide bf16 attention backward on mma.sync */           \
   X(g_opt_dec_streams, "dec_streams", 1)          /* decoder time loop as two half-batch chains when >= 2 */   \
-  X(g_opt_dec_fuse, "dec_fuse", 0)                /* grid-barrier fused forward step */                        \
-  X(g_opt_dec_fuse_bwd, "dec_fuse_bwd", 0)        /* grid-barrier fused backward step */                       \
-  X(g_opt_dec_cl, "dec_cl", 0)                    /* cluster-fused forward step */                             \
-  X(g_opt_dec_cl_bwd, "dec_cl_bwd", 0)            /* cluster-fused backward step */                            \
   X(g_opt_fuse_lstm, "fuse_lstm", 0)              /* LSTM cell in the gates GEMM's epilogue */                 \
   X(g_opt_skinny_mma, "skinny_mma", 1)            /* per-step GEMMs on mma.sync; 0: wgmma */                   \
   X(g_opt_skinny_tma, "skinny_tma", 1)            /* their operands by cp.async.bulk */                        \
@@ -323,44 +319,6 @@ struct TcLstmEpi {
   // in-kernel dropout (has_dropout = 2): Philox state, drop probability, first batch row of this launch, step index
   const unsigned long long* dstate; float dp; int row0, t_idx;
 };
-// fused decoder forward step (lo_skinny.cu): [gates GEMM + LSTM cell] -> grid barrier -> [projection of h_{t+1} for step t+1]
-struct DecStepFwd {
-  const bf16* gctx; int64_t ld_gctx;       // A of phase 1: gate * context of step t, [M][K]
-  const bf16* wil; int64_t ld_wil;         // gate-interleaved context half of weight_ih [4D][K]
-  TcLstmEpi e;                             // LSTM epilogue (writes h_{t+1} fp32 + bf16 mirror, c, gates, hd)
-  const bf16* wcat; int64_t ld_wcat;       // [N2][D] = [decoder_att; f_beta; weight_hh]
-  const float* bcat; float* o1_next; int64_t ld_o1; int N2;   // phase 2 output (NULL: last step, phase 2 skipped)
-  unsigned int* bar; unsigned int bar_target;                 // monotonic arrival counter of the grid barrier
-  int M, K;
-};
-int dec_step_fwd(const DecStepFwd& p, cudaStream_t st);
-// fused decoder backward step (lo_skinny.cu), launched after the attention backward of step t:
-//   phase A: dh_{t-1} += [datt2 | dgate_pre]_t [W_d ; W_beta]          (K = A+C, two K slices, fp32 atomics)
-//   grid barrier ; phase B: LSTM-cell backward of step t-1 (pointwise, spread over the whole grid) ; grid barrier
-//   phase C: [dgctx | dh]_{t-1} = dG_{t-1} [W_ih[:, E:] | W_hh]          (K = 4D, four K slices, fp32 atomics)
-struct DecStepBwd {
-  // phase A (skipped when dcat_a == NULL: first launch of the loop)
-  const bf16* dcat_a; int64_t ld_dcat;      // [Ma][A+C] bf16 mirror of datt2 | dgate_pre of step t
-  const bf16* wbwd2; int64_t ld_w2; int K2; // [D][A+C]
-  int Ma;
-  // phase B/C (skipped when gates == NULL: last launch of the loop)
-  const float* dhd; int64_t dhd_stride; const float* dmask; const unsigned long long* dstate; float dp; int t_idx;
-  float* dc; const float* gates; const float* c_prev; const float* c_cur;
-  float* dG; bf16* dG_bf; int64_t dG_stride;      // d pre-activations of step t-1 (fp32 + bf16 mirror), row stride O1
-  const bf16* wbwd1; int64_t ld_w1; int K1;       // [C+D][4D]
-  int Mb;
-  float* dxh; int C, D;                            // [B][C+D]: dgctx | dh (accumulated with atomics, cleared in phase B)
-  unsigned int* bar; unsigned int bar_target;      // target of the FIRST barrier of this launch (the second is + gridDim.x)
-};
-int dec_step_bwd(const DecStepBwd& p, cudaStream_t st);
-// cluster-fused step kernels (lo_cluster.cu): the same DecStepFwd / DecStepBwd contracts, rows split into blocks of 16 (one 16-CTA cluster
-// each), no grid barrier (bar / bar_target unused), dxh written instead of accumulated
-bool dec_cl_fwd_ok(int D, int C, int N2);
-bool dec_cl_bwd_ok(int D, int C, int A);
-int dec_cl_fwd(const DecStepFwd& p, cudaStream_t st);
-int dec_cl_bwd(const DecStepBwd& p, cudaStream_t st);
-int cl_set_ts(long long* p);      // timing build only
-int sk_set_ts(long long* p);      // timing build only
 int tc_gemm_nt_lstm(const bf16* A, int64_t lda, const bf16* Wil, int64_t ldw, int M, int D, int K, const TcLstmEpi& e, cudaStream_t st);
 int skinny_gemm_nt_lstm(const bf16* A, int64_t lda, const bf16* Wil, int64_t ldw, int M, int D, int K, const TcLstmEpi& e, cudaStream_t st);
 int skinny_gemm_nt(const bf16* A, int64_t lda, const bf16* W, int64_t ldw, float* C, int64_t ldc, int M, int N, int K, const float* bias,

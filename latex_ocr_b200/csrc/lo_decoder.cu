@@ -1261,7 +1261,7 @@ static int forward_prologue(const lo_decoder_args* a, const Dims& d, cudaStream_
   const BfViews bv = bf_views(a, d);
   if (bv.on) {
     LO_TRY(lo_cast(a->hall, LO_F32, bv.hall, LO_BF16, (int64_t)d.B * d.D, (void*)st));
-    if ((g_opt_fuse_lstm || g_opt_dec_fuse || g_opt_dec_cl) && d.E % 8 == 0 && d.C % 8 == 0) {
+    if (g_opt_fuse_lstm && d.E % 8 == 0 && d.C % 8 == 0) {
       interleave_wih_kernel<<<LO_NUM_SMS * 2, 256, 0, st>>>((const bf16*)a->w_ih, bv.wil, d.D, d.E, d.C);
       LO_LAUNCH_OK();
     }
@@ -1481,133 +1481,6 @@ static inline Rows chain_rows(const lo_decoder_args* a, const Dims& d, int chain
   r.work = (char*)a->work + (size_t)chain * lo_attention_workspace_bytes(d.B, d.C);
   r.nsplit = nchains == 2 ? (LO_NUM_SMS / (half > 0 ? half : 1) > 0 ? LO_NUM_SMS / half : 1) : 0;   // each chain fills one CTA slot per SM
   return r;
-}
-
-// the time loop of a training forward or backward (DESIGN.md §4): per-step launches on one or two row chains, or one fused step
-// kernel per step with a grid barrier (dec_fuse*) or per 16-row cluster (dec_cl*)
-enum class FwdSched { Chains, Fused, Cluster };
-enum class BwdSched { Chains, Fused, Cluster };
-
-static FwdSched pick_fwd(const lo_decoder_args* a, const Dims& d, bool sampling) {
-  const bool bf = bf_views(a, d).on;
-  // dec_step_fwd: every CTA of one grid resident for its barrier (<= 64 rows), the cell on its own mma.sync epilogue, D = C <= 512
-  if (bf && !sampling && g_opt_dec_fuse && g_opt_skinny_mma && !g_opt_fuse_lstm && g_opt_att_pipe && !two_chains(a, d) && d.B <= 64 &&
-      d.C == d.D && d.D <= 512 && d.D % 16 == 0 && d.O1 % 16 == 0 && d.E % 8 == 0 && a->rows_per_img <= 1)
-    return FwdSched::Fused;
-  // dec_cl_fwd: a 16-CTA cluster fits on the device with D = C = 512 and O1 = 3072 (dec_cl_fwd_ok, which also reads dec_cl)
-  if (bf && !sampling && !(g_opt_dbg_skip & 4) && g_opt_skinny_mma && !g_opt_fuse_lstm && g_opt_att_pipe && !two_chains(a, d) &&
-      d.E % 8 == 0 && a->rows_per_img <= 1 && dec_cl_fwd_ok(d.D, d.C, d.O1))
-    return FwdSched::Cluster;
-  return FwdSched::Chains;
-}
-
-static BwdSched pick_bwd(const lo_decoder_args* a, const Dims& d) {
-  const bool bf = bf_views(a, d).on;
-  // dec_step_bwd: K slices of 512 in both GEMMs, C == D, and its whole grid (<= 296 CTAs) resident for the barriers
-  if (bf && g_opt_dec_fuse_bwd && g_opt_skinny_mma && g_opt_att_pipe && !two_chains(a, d) && d.B <= 64 && d.C == d.D &&
-      (d.A + d.C) % 512 == 0 && d.G % 512 == 0 && ((d.C + d.D) / 16) * (d.G / 512) <= 296 && a->rows_per_img <= 1)
-    return BwdSched::Fused;
-  // dec_cl_bwd: a 16-CTA cluster fits on the device with D = C = A = 512 (dec_cl_bwd_ok, which also reads dec_cl_bwd)
-  if (bf && !(g_opt_dbg_skip & 4) && g_opt_skinny_mma && g_opt_att_pipe && !two_chains(a, d) && a->rows_per_img <= 1 &&
-      dec_cl_bwd_ok(d.D, d.C, d.A))
-    return BwdSched::Cluster;
-  return BwdSched::Chains;
-}
-
-// the forward time loop on a fused step kernel, two launches per step: attention(t) -> [gates GEMM + LSTM cell | exchange of h_{t+1} |
-// projection of h_{t+1}], the exchange through a grid barrier (dec_step_fwd, lo_skinny.cu) or within one 16-CTA cluster per block
-// of 16 batch rows (dec_cl_fwd, lo_cluster.cu)
-static int fused_forward(const lo_decoder_args* a, const Dims& d, FwdSched sched, cudaStream_t st) {
-  const BfViews bv = bf_views(a, d);
-  const bool cl = sched == FwdSched::Cluster;
-  unsigned int* bar = (unsigned int*)((char*)a->work + lo_attention_workspace_bytes(d.B, d.C));      // chain-1 region is unused here
-  const int grid = cdiv(d.O1, 16) > cdiv(d.G, 16) ? cdiv(d.O1, 16) : cdiv(d.G, 16);
-  if (!cl) LO_CUDA(cudaMemsetAsync(bar, 0, 16 * 128, st));                                          // 16 arrival counters, one cache line each
-  LO_TRY(skinny_gemm_nt(bv.hall, d.D, (const bf16*)a->wcat1, d.D, a->out1, d.O1, a->bt_host[0], d.O1, d.D, a->bcat1, 1, 0, st));
-  unsigned int epoch = 0;
-  for (int t = 0; t < d.T; t++) {
-    const int nrows = a->bt_host[t];
-    float* o1 = a->out1 + (int64_t)t * d.B * d.O1;
-    if (!(g_opt_dbg_skip & 2))
-      LO_TRY(attention_forward_launch(a->att1, a->enc, a->dt, o1, d.O1, a->w_full, a->alphas + (int64_t)t * d.R, (int64_t)d.T * d.R,
-                                      a->ctx + (int64_t)t * d.B * d.C, o1 + d.A, d.O1, a->gctx + (int64_t)t * d.B * d.C,
-                                      bv.gctx + (int64_t)t * d.B * d.C, nrows, d.R, d.C, a->work, st, 1, 0, att_mask_at(a, t, 0)));
-    DecStepFwd p{};
-    p.gctx = bv.gctx + (int64_t)t * d.B * d.C; p.ld_gctx = d.C;
-    p.wil = bv.wil; p.ld_wil = d.C;
-    const float* dm = (a->has_dropout == 1 && a->dropout_mask) ? a->dropout_mask + (int64_t)t * d.D : nullptr;
-    p.e = lstm_epi(a, d, bv, t, 0, a->caps + t, a->caps_stride, a->hd + (int64_t)t * d.D, (int64_t)d.T * d.D, dm);
-    p.wcat = (const bf16*)a->wcat1; p.ld_wcat = d.D; p.bcat = a->bcat1;
-    const bool more = t + 1 < d.T;
-    p.o1_next = more ? a->out1 + (int64_t)(t + 1) * d.B * d.O1 : nullptr;
-    p.ld_o1 = d.O1; p.N2 = d.O1;
-    p.M = nrows; p.K = d.C;
-    if (cl) {
-      LO_TRY(dec_cl_fwd(p, st));
-    } else {
-      p.bar = bar; p.bar_target = more ? (++epoch) * (unsigned int)grid : 0u;
-      LO_TRY(dec_step_fwd(p, st));
-    }
-  }
-  return LO_OK;
-}
-
-// the backward time loop on a fused step kernel, two launches per step: attention_bwd(t) -> [dh_t += (datt2 | dgate)_t W | LSTM
-// backward of step t-1 | dG_{t-1} W], the phases joined by grid barriers (dec_step_bwd, lo_skinny.cu) or within one 16-CTA cluster per
-// block of 16 batch rows (dec_cl_bwd, lo_cluster.cu).  dal, dal_b, dal_t: the d alpha rows of lo_decoder_backward
-static int fused_backward(const lo_decoder_args* a, const Dims& d, BwdSched sched, const float* dal, int64_t dal_b, int64_t dal_t,
-                          cudaStream_t st) {
-  const BfViews bv = bf_views(a, d);
-  const bool cl = sched == BwdSched::Cluster;
-  unsigned int* bar = (unsigned int*)((char*)a->work + lo_attention_workspace_bytes(d.B, d.C)) + 1024;   // chain-1 region, unused here
-  const unsigned int grid = (unsigned int)(((d.C + d.D) / 16) * (d.G / 512));
-  if (!cl) LO_CUDA(cudaMemsetAsync(bar, 0, 16 * 128, st));
-  unsigned int nb = 0;        // barriers passed so far: one in the first launch, two in every launch that runs the LSTM backward
-  auto fill_common = [&](DecStepBwd& p) {
-    p.wbwd1 = (const bf16*)a->wbwd1; p.ld_w1 = d.G; p.K1 = d.G;      // K1 also sizes dec_step_bwd's grid when phases B/C are skipped
-    p.wbwd2 = (const bf16*)a->wbwd2; p.ld_w2 = d.A + d.C; p.K2 = d.A + d.C;
-    p.dxh = a->dxh; p.C = d.C; p.D = d.D; p.ld_dcat = d.O1;
-    if (!cl) p.bar = bar;
-  };
-  auto fill_bc = [&](DecStepBwd& p, int t) {       // LSTM backward + dG projection of step t
-    p.dhd = a->dhd + (int64_t)t * d.D; p.dhd_stride = (int64_t)d.T * d.D;
-    p.dmask = (a->has_dropout == 1 && a->dropout_mask) ? a->dropout_mask + (int64_t)t * d.D : nullptr;
-    p.dstate = (const unsigned long long*)(a->has_dropout == 2 ? a->dropout_state : nullptr);
-    p.dp = a->dropout_p; p.t_idx = t;
-    p.dc = a->dc; p.gates = a->gates + (int64_t)t * d.B * d.G;
-    p.c_prev = a->call + (int64_t)t * d.B * d.D; p.c_cur = a->call + (int64_t)(t + 1) * d.B * d.D;
-    p.dG = a->dcat + (int64_t)t * d.B * d.O1 + d.A + d.C; p.dG_bf = bv.dcat + (int64_t)t * d.B * d.O1 + d.A + d.C; p.dG_stride = d.O1;
-    p.Mb = a->bt_host[t];
-  };
-  auto launch = [&](DecStepBwd& p, unsigned int barriers) {
-    if (cl) return dec_cl_bwd(p, st);
-    if (barriers) p.bar_target = (nb + 1) * grid;
-    nb += barriers;
-    return dec_step_bwd(p, st);
-  };
-  {
-    DecStepBwd p{};
-    fill_common(p);
-    fill_bc(p, d.T - 1);
-    LO_TRY(launch(p, 1));
-  }
-  for (int t = d.T - 1; t >= 0; t--) {
-    const int nrows = a->bt_host[t];
-    float* dcat_t = a->dcat + (int64_t)t * d.B * d.O1;
-    bf16* dcat_bf_t = bv.dcat + (int64_t)t * d.B * d.O1;
-    const float* o1 = a->out1 + (int64_t)t * d.B * d.O1;
-    AttBwdArgs x{a->att1, a->enc, o1, o1 + d.A, d.O1, a->w_full, a->alphas + (int64_t)t * d.R, (int64_t)d.T * d.R,
-                 a->ctx + (int64_t)t * d.B * d.C, a->dxh, d.C + d.D, dal + (int64_t)t * dal_t, dal_b, a->sreg + t, d.T,
-                 a->de + (int64_t)t * d.R, dcat_t, dcat_t + d.A, d.O1, dcat_bf_t, dcat_bf_t + d.A, a->dctx + (int64_t)t * d.B * d.C,
-                 nrows, d.R, a->work, a->dmean, 0, 0, 0, att_mask_at(a, t, 0)};
-    if (!(cl && (g_opt_dbg_skip & 2))) LO_TRY(attention_bwd_pipe(x, a->dt, d.C, st));     // the cluster loop honours dbg_skip & 2
-    DecStepBwd p{};
-    fill_common(p);
-    p.dcat_a = dcat_bf_t; p.Ma = nrows;
-    if (t > 0) fill_bc(p, t - 1);
-    LO_TRY(launch(p, t > 0 ? 2 : 0));
-  }
-  return LO_OK;
 }
 
 // one beam-search step of either decoder flavour (beam_step_kernel, one CTA per image): the top-k over beam x V log-probs in shared
@@ -1971,22 +1844,14 @@ int lo_decoder_forward(const lo_decoder_args* a, int with_loss, void* stream) {
     LO_CUDA(cudaEventRecord(g_ev_fork, st));
     LO_CUDA(cudaStreamWaitEvent(g_side, g_ev_fork, 0));
   }
-  const FwdSched sched = pick_fwd(a, d, sampling);
-  switch (sched) {
-  case FwdSched::Fused:
-  case FwdSched::Cluster:
-    LO_TRY(fused_forward(a, d, sched, st));
-    break;
-  case FwdSched::Chains:
-    for (int chain = 0; chain < nchains; chain++) {
-      cudaStream_t cs = chain == 0 ? st : g_side;
-      for (int t = 0; t < d.T; t++) {
-        const float* dm = (a->has_dropout == 1 && a->dropout_mask) ? a->dropout_mask + (int64_t)t * d.D : nullptr;
-        const Rows rs = chain_rows(a, d, chain, nchains, a->bt_host[t]);
-        LO_TRY(forward_step(a, d, t, rs, a->caps + t, a->caps_stride, a->hd + (int64_t)t * d.D, (int64_t)d.T * d.D, dm, cs));
-      }
+  // the time loop (DESIGN.md §4): per-step launches on one or two row chains
+  for (int chain = 0; chain < nchains; chain++) {
+    cudaStream_t cs = chain == 0 ? st : g_side;
+    for (int t = 0; t < d.T; t++) {
+      const float* dm = (a->has_dropout == 1 && a->dropout_mask) ? a->dropout_mask + (int64_t)t * d.D : nullptr;
+      const Rows rs = chain_rows(a, d, chain, nchains, a->bt_host[t]);
+      LO_TRY(forward_step(a, d, t, rs, a->caps + t, a->caps_stride, a->hd + (int64_t)t * d.D, (int64_t)d.T * d.D, dm, cs));
     }
-    break;
   }
   if (nchains == 2) {
     LO_CUDA(cudaEventRecord(g_ev_join, g_side));
@@ -2112,19 +1977,10 @@ int lo_decoder_backward(const lo_decoder_args* a, void* stream) {
     LO_CUDA(cudaEventRecord(g_ev_fork, st));
     LO_CUDA(cudaStreamWaitEvent(g_side, g_ev_fork, 0));
   }
-  const BwdSched sched = pick_bwd(a, d);
-  switch (sched) {
-  case BwdSched::Fused:
-  case BwdSched::Cluster:
-    LO_TRY(fused_backward(a, d, sched, dal, dal_b, dal_t, st));
-    break;
-  case BwdSched::Chains:
-    for (int chain = 0; chain < nchains; chain++) {
-      cudaStream_t cs = chain == 0 ? st : g_side;
-      for (int t = d.T - 1; t >= 0; t--)
-        LO_TRY(backward_step(a, d, t, chain_rows(a, d, chain, nchains, a->bt_host[t]), dal, dal_b, dal_t, cs));
-    }
-    break;
+  for (int chain = 0; chain < nchains; chain++) {
+    cudaStream_t cs = chain == 0 ? st : g_side;
+    for (int t = d.T - 1; t >= 0; t--)
+      LO_TRY(backward_step(a, d, t, chain_rows(a, d, chain, nchains, a->bt_host[t]), dal, dal_b, dal_t, cs));
   }
   if (nchains == 2) {
     LO_CUDA(cudaEventRecord(g_ev_join, g_side));

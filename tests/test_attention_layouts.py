@@ -84,29 +84,3 @@ def test_hi_lo_split_keeps_fp32_products():
     assert rel <= 2.0 ** -16
     assert ((hi.float() - v).abs() / v.abs().clamp_min(1e-30)).max().item() > 2.0 ** -10      # what a single bf16 would lose
 
-
-def test_cluster_all_gather_maps_cover_every_element_once():
-    """lo_cluster.cu: the 16 CTAs of a cluster each own 32 hidden units (forward: bf16 h slab [16 rows][32]; backward: dG slab
-    [16 rows][4 gates][32]); every CTA copies all 16 slabs into its A operand with 16-byte DSMEM loads.  The (rank, row, segment) ->
-    (source offset, destination offset) maps must tile the [16][512] / [16][4*512] operand exactly once."""
-    APITCH, CL_D = 512 * 2 + 16, 512
-    seen = np.zeros((16, CL_D), np.int32)
-    for i in range(16 * 16 * 4):
-        rank, r, sg = i >> 6, (i >> 2) & 15, i & 3
-        src = r * 64 + sg * 16                                # byte offset inside rank's [16][32] bf16 slab
-        dst = r * APITCH + rank * 64 + sg * 16                # byte offset inside this CTA's [16][1040 B] operand
-        assert src % 16 == 0 and dst % 16 == 0 and src + 16 <= 16 * 64
-        u0 = (dst - r * APITCH) // 2                          # first of 8 units written
-        assert u0 == rank * 32 + (src - r * 64) // 2
-        seen[r, u0:u0 + 8] += 1
-    assert (seen == 1).all()
-    APITCH_C, NA = 4 * CL_D * 2 + 16, 32
-    seen = np.zeros((16, 4 * CL_D), np.int32)
-    for i in range(16 * 16 * 4 * 4):
-        rank, r, q, sg = i >> 8, (i >> 4) & 15, (i >> 2) & 3, i & 3
-        src = (r * 4 + q) * (NA * 2) + sg * 16
-        dst = r * APITCH_C + (q * CL_D + rank * NA) * 2 + sg * 16
-        k0 = (dst - r * APITCH_C) // 2                        # K index of the [dgctx | dh] GEMM: gate * 512 + unit
-        assert k0 == q * CL_D + rank * NA + sg * 8 and src + 16 <= 16 * 4 * NA * 2
-        seen[r, k0:k0 + 8] += 1
-    assert (seen == 1).all()

@@ -203,7 +203,7 @@ def test_custom_loss_vs_cpu_oracle_ragged():
         _close(g, pdd[k].grad, 1e-3, k)
 
 
-@pytest.mark.parametrize("option", ["dec_cl_bwd", "dec_fuse_bwd", "att_bwd_mma", "att_maskbits"])
+@pytest.mark.parametrize("option", ["att_bwd_mma", "att_maskbits"])
 def test_custom_loss_under_backward_schedules(option):
     V = 50
     pe, pd, formula, lengths, enc = _ragged_case(V)

@@ -130,15 +130,15 @@ def test_tc_conv3x3_wgrad(N, H, W, Cin, Cout, pad):
     assert relerr(db, dy.double().sum(dim=(0, 2, 3)).float()) < 1e-5
 
 
-_SCHEDULE_OPTS = {"fuse_lstm": (0, 1), "dec_streams": (1, 2), "skinny_mma": (1, 0), "dec_fuse": (0, 1), "dec_fuse_bwd": (0, 1), "att_maskbits": (1, 0),
-                  "conv_persist": (1, 0), "wgrad256": (0, 1), "conv_mt2": (1, 0), "dec_cl": (0, 1), "dec_cl_bwd": (0, 1), "att_bwd_mma": (1, 0), "skinny_tma": (1, 0)}
+_SCHEDULE_OPTS = {"fuse_lstm": (0, 1), "dec_streams": (1, 2), "skinny_mma": (1, 0), "att_maskbits": (1, 0), "conv_persist": (1, 0),
+                  "wgrad256": (0, 1), "conv_mt2": (1, 0), "att_bwd_mma": (1, 0), "skinny_tma": (1, 0)}
 
 
 @pytest.mark.parametrize("opt", sorted(_SCHEDULE_OPTS))
 def test_optional_decoder_schedules_match_default(opt):
     """Every optional schedule (first value = default) must give the default schedule's numbers: the measured-no-faster variants kept
-    as run-time options (DESIGN.md §8) and, the other way round, the separate-launch time loop and the CUDA-core attention backward
-    that the cluster-fused step kernels / the tensor-core backward replaced."""
+    as run-time options (DESIGN.md §8) and, the other way round, the paths the defaults replaced, such as the CUDA-core attention
+    backward."""
     from util import build_model, load_golden
     from latex_ocr_b200 import _lib
     from oracle import ref_model as rm

@@ -7,20 +7,19 @@ numbers, case by case, at the cfg #2 shapes (bf16 on the wgmma / mma.sync kernel
 the parent commit made in another checkout and copied next to this one.  Each run is a process of its own with the library
 option "deterministic" = 1; the base build runs twice, which measures the spread of the order-dependent paths, then the head build
 runs once.  Every case starts from the same seeded weights and inputs.  Cases:
-  torch flavour, one train step (forward, loss, backward, Adam): the default, each of the schedule options dec_streams=2, dec_fuse,
-    dec_fuse_bwd, dec_cl, dec_cl_bwd, fuse_lstm, skinny_mma=0, att_pipe=0, scheduled sampling (p = 0.25) and self-critical
-    training (tau = 1);
+  torch flavour, one train step (forward, loss, backward, Adam): the default, each of the schedule options dec_streams=2,
+    fuse_lstm, skinny_mma=0, att_pipe=0, scheduled sampling (p = 0.25) and self-critical training (tau = 1);
   TensorFlow flavour, one train step: teacher forcing, scheduled sampling, self-critical training;
   both flavours: greedy decode of images of different sizes in one batch (ragged), beam search with the diversity penalty, greedy
     decode of one batch with its attention weights, and beam search of a ragged batch (the TF flavour's with its log-probs).
 Compared per case: lo_launch_count() over the case, and the loss, the gradients, the fed tokens and the decoded ids / attention
 weights / log-probs.
 Launch counts must be equal, and every output bit-identical across the three runs, except on the paths that still add with fp32
-atomics under "deterministic".  Those are two torch-flavour paths that DESIGN.md §4 lists: the fused backward step kernels
-(dec_fuse_bwd), and the wgmma split-K of the per-step backward GEMMs (skinny_mma=0 puts it on every step).  The third is the
-TensorFlow-flavour train step, whose attention backward adds d beta with atomics.  On those paths a head-against-base difference
-of up to 1e-4 of the largest magnitude passes.  The base build's difference from itself is printed beside it.  Measured on an H100
-80GB HBM3 at a 700 W power limit, that spread was 1e-5 to 3e-5 of max-abs on the two torch paths and below 1e-7 on the TF step.
+atomics under "deterministic".  One is a torch-flavour path that DESIGN.md §4 lists: the wgmma split-K of the per-step backward
+GEMMs (skinny_mma=0 puts it on every step).  The other is the TensorFlow-flavour train step, whose attention backward adds d beta
+with atomics.  On those paths a head-against-base difference of up to 1e-4 of the largest magnitude passes.  The base build's
+difference from itself is printed beside it.  Measured on an H100 80GB HBM3 at a 700 W power limit, that spread was 1e-5 to 3e-5
+of max-abs on the torch paths and below 1e-7 on the TF step.
 Prints one line per case and exits non-zero on a mismatch.
 """
 import argparse
@@ -31,10 +30,9 @@ import tempfile
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 B, H, W, T, V = 64, 128, 512, 150, 500
-OPTION_CASES = {"default": {}, "dec_streams=2": {"dec_streams": 2}, "dec_fuse": {"dec_fuse": 1}, "dec_fuse_bwd": {"dec_fuse_bwd": 1},
-                "dec_cl": {"dec_cl": 1}, "dec_cl_bwd": {"dec_cl_bwd": 1}, "fuse_lstm": {"fuse_lstm": 1}, "skinny_mma=0": {"skinny_mma": 0},
+OPTION_CASES = {"default": {}, "dec_streams=2": {"dec_streams": 2}, "fuse_lstm": {"fuse_lstm": 1}, "skinny_mma=0": {"skinny_mma": 0},
                 "att_pipe=0": {"att_pipe": 0}}
-ORDER_DEPENDENT = {"dec_fuse_bwd", "skinny_mma=0", "tf_default", "tf_sampling", "tf_scst"}
+ORDER_DEPENDENT = {"skinny_mma=0", "tf_default", "tf_sampling", "tf_scst"}
 TOL = 1e-4
 DECODE_WIDTHS = (128, 192, 256, 320, 384, 448, 512, 160, 224, 288, 352, 416, 480, 512, 128, 256)
 BEAM, DIV_GAMMA, DIV_PROB = 5, 0.5, 0.5

@@ -56,37 +56,6 @@ def test_skinny_mma_gemm(M, N, K, acc):
         assert relerr(C, ref) < 1e-5, opt
 
 
-@pytest.mark.parametrize("N,H,W,Cin,Cout,pad", [(2, 8, 128, 64, 128, 1), (2, 16, 64, 128, 256, 1), (3, 16, 64, 512, 512, 0),
-                                                 (2, 14, 62, 512, 512, 2), (1, 6, 30, 256, 64, 1), (2, 9, 13, 64, 72, 1)])
-def test_tc_conv3x3(N, H, W, Cin, Cout, pad):
-    _lib, L = _L()
-    torch.manual_seed(1)
-    x = torch.randn(N, Cin, H, W, device="cuda").bfloat16()
-    w = (torch.randn(Cout, Cin, 3, 3, device="cuda") * (1.0 / (3 * Cin ** 0.5))).bfloat16()
-    b = torch.randn(Cout, device="cuda")
-    ref = F.relu(F.conv2d(x.double(), w.double(), b.double(), padding=pad))
-    xn = x.permute(0, 2, 3, 1).contiguous()
-    wk = w.permute(0, 2, 3, 1).contiguous()
-    Ho, Wo = H + 2 * pad - 2, W + 2 * pad - 2
-    y = torch.full((N, Ho, Wo, Cout), 5.0, device="cuda", dtype=torch.bfloat16)
-    st = _lib.stream_ptr()
-    _lib.check(L.lo_conv3x3(_lib.ptr(xn), _lib.ptr(wk), _lib.ptr(b), None, _lib.ptr(y), 1, N, H, W, Cin, Cout, pad, 1, 1, st))
-    torch.cuda.synchronize()
-    assert relerr(y.float().permute(0, 3, 1, 2), ref.float()) < 1e-2
-    # identical math on the CUDA-core path (same bf16 inputs, fp32 accumulate): differences are summation order only
-    y2 = torch.zeros_like(y)
-    _lib.check(L.lo_conv3x3(_lib.ptr(xn), _lib.ptr(wk), _lib.ptr(b), None, _lib.ptr(y2), 1, N, H, W, Cin, Cout, pad, 1, 0, st))
-    torch.cuda.synchronize()
-    assert relerr(y.float(), y2.float()) < 1e-2
-    # data-gradient use: mask epilogue, no bias, no ReLU
-    mask = (torch.rand(N, Ho, Wo, Cout, device="cuda") > 0.5).bfloat16()
-    y3 = torch.zeros_like(y)
-    _lib.check(L.lo_conv3x3(_lib.ptr(xn), _lib.ptr(wk), None, _lib.ptr(mask), _lib.ptr(y3), 1, N, H, W, Cin, Cout, pad, 0, 1, st))
-    torch.cuda.synchronize()
-    ref3 = F.conv2d(x.double(), w.double(), None, padding=pad) * mask.double().permute(0, 3, 1, 2)
-    assert relerr(y3.float().permute(0, 3, 1, 2), ref3.float()) < 1e-2
-
-
 def test_tc_train_step_matches_simt_bf16():
     from util import build_model, load_golden
     from oracle import ref_model as rm
@@ -131,7 +100,7 @@ def test_tc_conv3x3_wgrad(N, H, W, Cin, Cout, pad):
 
 
 _SCHEDULE_OPTS = {"fuse_lstm": (0, 1), "dec_streams": (1, 2), "skinny_mma": (1, 0), "att_maskbits": (1, 0), "conv_persist": (1, 0),
-                  "wgrad256": (0, 1), "conv_mt2": (1, 0), "att_bwd_mma": (1, 0), "skinny_tma": (1, 0)}
+                  "wgrad256": (0, 1), "conv_mt2": (1, 0), "conv_mc": (1, 0), "att_bwd_mma": (1, 0), "skinny_tma": (1, 0)}
 
 
 @pytest.mark.parametrize("opt", sorted(_SCHEDULE_OPTS))

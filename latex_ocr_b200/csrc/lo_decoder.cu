@@ -1095,9 +1095,8 @@ static int check_args(const lo_decoder_args* a) {
   LO_CHECK_ARG(a->rows_per_img <= 1 || a->B % a->rows_per_img == 0, "B must be a multiple of rows_per_img");
   LO_CHECK_ARG(a->phase >= 0 && a->phase <= 2, "phase in 0..2");
   LO_CHECK_ARG(a->bt_host && a->caps && a->enc && a->work, "null pointer");
-  LO_CHECK_ARG(a->has_dropout != 2 || (a->dropout_state && a->dropout_p >= 0.f && a->dropout_p < 1.f &&
-                                       (!g_opt_fuse_lstm || g_opt_skinny_mma)),
-               "has_dropout=2 needs dropout_state, 0 <= dropout_p < 1 (and the mma.sync kernel when fuse_lstm=1)");
+  LO_CHECK_ARG(a->has_dropout != 2 || (a->dropout_state && a->dropout_p >= 0.f && a->dropout_p < 1.f),
+               "has_dropout=2 needs dropout_state, 0 <= dropout_p < 1");
   if (a->ss_prob) {
     LO_CHECK_ARG(a->fed, "scheduled sampling (ss_prob) needs fed");
     LO_CHECK_ARG(a->ss_u || a->dropout_state, "scheduled sampling (ss_prob) needs ss_u or dropout_state for its coin");
@@ -1281,11 +1280,14 @@ struct Rows {
 
 // C (+)= A W^T for the per-step GEMMs of the time loops (M <= B rows): the mma.sync kernel for <= 64 rows of the bf16 mirror Abf,
 // wgmma above, CUDA cores on the fp32 operand A32 when there are no mirrors (tc false).  The tensor-core paths run `splits` K slices
-// (atomic_acc: added onto C with fp32 atomics); the CUDA-core path writes C or, with `acc`, adds to it.
+// (atomic_acc: added onto C with fp32 atomics); the CUDA-core path writes C or, with `acc`, adds to it.  Option "deterministic" on
+// wgmma: one K slice, so every element of C receives a single atomic add onto its base value and the result does not depend on the
+// order in which CTAs finish (the mma.sync kernel orders its slices itself).
 static int step_gemm_nt(bool tc, const float* A32, const bf16* Abf, int64_t lda, const void* W, int dtW, int64_t ldw, float* C,
                         int64_t ldc, int M, int N, int K, const float* bias, int acc, int splits, int atomic_acc, cudaStream_t st) {
   if (tc && g_opt_skinny_mma && M <= 64) return skinny_gemm_nt(Abf, lda, (const bf16*)W, ldw, C, ldc, M, N, K, bias, splits, atomic_acc, st);
-  if (tc) return tc_gemm_nt_ex(Abf, lda, (const bf16*)W, ldw, C, LO_F32, ldc, M, N, K, bias, 0, 0, splits, atomic_acc, 1, st);
+  if (tc)
+    return tc_gemm_nt_ex(Abf, lda, (const bf16*)W, ldw, C, LO_F32, ldc, M, N, K, bias, 0, 0, g_opt_det ? 1 : splits, atomic_acc, 1, st);
   return gemm_nt(A32, LO_F32, lda, W, dtW, ldw, C, LO_F32, ldc, M, N, K, bias, acc, 0, LO_IMPL_SIMT, st);
 }
 

@@ -118,6 +118,8 @@ struct TcParams {
   const float* l_cprev; float* l_gates; float* l_c; float* l_h; bf16* l_hbf;
   float* l_hd; int64_t l_hd_stride; const float* l_dmask;
   int l_D, l_V;
+  // in-kernel dropout (has_dropout = 2, no l_dmask): Philox {seed, call}, drop probability, first batch row of the launch, step
+  const unsigned long long* l_dstate; float l_dp; int l_row0, l_t;
 };
 
 constexpr int TC_BM = 128, TC_BK = 64;
@@ -320,7 +322,13 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_gemm_conv_kernel(const __gri
           p.l_c[(int64_t)b * D + j] = cn;
           p.l_h[(int64_t)b * D + j] = hn;
           if (p.l_hbf) p.l_hbf[(int64_t)b * D + j] = __float2bfloat16_rn(hn);
-          if (p.l_hd) p.l_hd[(int64_t)b * p.l_hd_stride + j] = p.l_dmask ? hn * p.l_dmask[(int64_t)b * p.l_hd_stride + j] : hn;
+          if (p.l_hd) {
+            // the multiplier lstm_pw_fwd_body and skinny_lstm_kernel apply, and lstm_pw_bwd_kernel redraws
+            float mult = 1.f;
+            if (p.l_dmask) mult = p.l_dmask[(int64_t)b * p.l_hd_stride + j];
+            else if (p.l_dstate) mult = philox_dropout_mult(p.l_dstate, p.l_row0 + b, p.l_t, j, p.l_dp, 1.f / (1.f - p.l_dp));
+            p.l_hd[(int64_t)b * p.l_hd_stride + j] = hn * mult;
+          }
         }
       }
     } else {
@@ -828,6 +836,7 @@ int tc_gemm_nt_ex(const bf16* A, int64_t lda, const bf16* W, int64_t ldw, void* 
     p.l_ptab = e.ptab; p.l_tok = e.tok; p.l_tok_stride = e.tok_stride; p.l_hh = e.hh; p.l_hh_stride = e.hh_stride;
     p.l_cprev = e.c_prev; p.l_gates = e.gates; p.l_c = e.c_out; p.l_h = e.h_out; p.l_hbf = e.h_bf;
     p.l_hd = e.hd; p.l_hd_stride = e.hd_stride; p.l_dmask = e.dmask; p.l_D = e.D; p.l_V = e.V;
+    p.l_dstate = e.dstate; p.l_dp = e.dp; p.l_row0 = e.row0; p.l_t = e.t_idx;
   }
   return launch_tc_any(mA, mB, p, cdiv(M, TC_BM), splits, NT, st, mc);
 }

@@ -66,11 +66,9 @@ int64_t lo_launch_count(void);
  *                             as a cluster; 0 never.  The other attention kernels: cluster unless 0.  Same results for 1 and 2
  *   att_maskbits     1 [p]    1: the forward attention kernel stores the ReLU mask bits, the backward streams them instead of att1
  *   att_bwd_mma      1 [p]    1: the 512-wide bf16 attention backward runs both contractions on mma.sync
- *   dec_streams      1 [p]    >= 2: the decoder time loop runs as two half-batch chains on two streams; also sets skinny8 = value < 2
- *   fuse_lstm        0 [p]    1: LSTM cell in the gates GEMM's epilogue; off: it cannot hide the dependent loads the pointwise kernel hides
  *   skinny_mma       1 [p]    decoder per-step GEMMs (M <= 64) on mma.sync; 0: on wgmma
  *   skinny_tma       1 [p]    1: their operands by cp.async.bulk, one copy per row; 0: 16-byte cp.async
- *   skinny8          1        1: 8-stage (198 KB shared memory) wgmma config for GEMMs with M <= 128; rewritten by dec_streams
+ *   skinny8          1        1: 8-stage (198 KB shared memory) wgmma config for GEMMs with M <= 128
  *   conv_persist     1 [p]    1: persistent double-accumulator convolution kernel; 0: one tile per CTA
  *   conv_mt2         1 [p]    1: layers with <= 128 output channels: two 128-position sub-tiles per CTA share each weight stage
  *   conv_mc          1        1: cluster-of-2 multicast of the A tile in the wgmma GEMM
@@ -195,7 +193,7 @@ int lo_relu_mask_cast(const float* g, const void* y, void* out, int dt, int64_t 
  * (decoding has no row cap).  Size: P + B * 16 * (C + 2) * 4 bytes.
  */
 int64_t lo_attention_workspace_bytes(int B, int C);
-int64_t lo_decoder_workspace_bytes(int B, int C);   /* `work` of lo_decoder_args: two attention regions (two row chains) */
+int64_t lo_decoder_workspace_bytes(int B, int C);   /* `work` of lo_decoder_args: two attention regions (time loop; ragged decode's CTA map) */
 int lo_attention_forward(const void* att1, const void* enc, int dt, const float* att2, int64_t att2_stride,
                          const float* wf, float* alpha, int64_t alpha_stride, float* ctx,
                          float* gate_pre, int64_t gate_stride, float* gctx,
@@ -287,8 +285,7 @@ typedef struct lo_decoder_args {
    * where logits[b][t-1] is the returned prediction row (fc(dropout(h)) with the dropout of this call), p = *ss_prob.  The choice
    * is not differentiated: given fed, forward and backward are teacher forcing on the input sequence fed (the embedding and
    * weight_ih[:, :E] gradients go to the rows of the tokens fed); ce_kernel's targets stay caps[b][t+1].  In this mode the head
-   * fc(hd_t) runs inside the time loop (one GEMM per step, writing only the rows active at step t) instead of once after it, and
-   * the forward always runs the default single-chain step loop: fuse_lstm and dec_streams >= 2 are ignored.
+   * fc(hd_t) runs inside the time loop (one GEMM per step, writing only the rows active at step t) instead of once after it.
    * Refused (LO_EINVAL) before any GPU work: ss_prob without fed, without ss_u and dropout_state, with phase != 0, with
    * rows_per_img > 1, and on the greedy / beam entry points. */
   int64_t* fed;            /* [B][T] tokens fed at each step: written by the forward (positions past a row's decode length get

@@ -1346,9 +1346,8 @@ __global__ void __launch_bounds__(AP_THREADS, LO_ABM_MINB) attention_bwd_mma_ker
   ATT_TS(5, threadIdx.x == 0);
 }
 
-int att_pipe_splits(int B, int hint = 0) {
+int att_pipe_splits(int B) {
   if (g_opt_att_nsplit > 0) return g_opt_att_nsplit > AP_MAXSPLIT ? AP_MAXSPLIT : g_opt_att_nsplit;      // explicit option wins
-  if (hint > 0) return hint > 8 ? 8 : hint;
   // two CTAs per SM are resident (smem): aim for one full wave — per-CTA start-up/combine costs dominate short CTAs
   int s = (LO_NUM_SMS * LO_ATT_MINB) / B;
   if (s < 1) s = 1;
@@ -1466,7 +1465,7 @@ static int fwd_launch_m(const AttFwdArgs& x, cudaStream_t st) {
     LO_CUDA(cudaFuncSetAttribute(attention_fwd_pipe_kernel<T, NVA, NVC, true, ACT, MK>, cudaFuncAttributeMaxDynamicSharedMemorySize, SM_MAX));
     attr = true;
   }
-  const int ns = att_pipe_splits(x.B, x.nsplit_hint);
+  const int ns = att_pipe_splits(x.B);
   const int rpi = x.rows_per_img > 1 ? x.rows_per_img : 1;
   const int keep_q = att_keep_q((int64_t)(x.B / rpi) * x.R * (C::CHA + C::CHC) * (int64_t)sizeof(T));     // rows of one image: read once
   if (att_grid_cluster((const void*)attention_fwd_pipe_kernel<T, NVA, NVC, false, ACT, MK>, (size_t)C::SMEM, ns, x.B, x.R)) {
@@ -1581,7 +1580,7 @@ static int bwd_launch_a(const AttBwdArgs& x, cudaStream_t st) {
     LO_CUDA(cudaFuncSetAttribute(attention_bwd_pipe_kernel<T, NVA, NVC, true, ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM));
     attr = true;
   }
-  const int ns = att_pipe_splits(x.B, x.nsplit_hint);
+  const int ns = att_pipe_splits(x.B);
   if (x.datt1) {
     if constexpr (ACT == 0) {
       LO_CHECK_ARG(!x.mask_in, "d att1 is computed from att1, not from the mask bits");

@@ -65,8 +65,6 @@ constexpr int LO_NUM_SMS = 132;
   X(g_opt_att_cluster, "att_cluster", 1)          /* splits of a batch row combine through DSMEM */            \
   X(g_opt_att_maskbits, "att_maskbits", 1)        /* ReLU mask bits instead of att1 in the backward */         \
   X(g_opt_att_bwd_mma, "att_bwd_mma", 1)          /* 512-wide bf16 attention backward on mma.sync */           \
-  X(g_opt_dec_streams, "dec_streams", 1)          /* decoder time loop as two half-batch chains when >= 2 */   \
-  X(g_opt_fuse_lstm, "fuse_lstm", 0)              /* LSTM cell in the gates GEMM's epilogue */                 \
   X(g_opt_skinny_mma, "skinny_mma", 1)            /* per-step GEMMs on mma.sync; 0: wgmma */                   \
   X(g_opt_skinny_tma, "skinny_tma", 1)            /* their operands by cp.async.bulk */                        \
   X(g_opt_skinny8, "skinny8", 1)                  /* 8-stage wgmma config for M <= 128 */                      \
@@ -255,7 +253,6 @@ struct AttFwdArgs {
   int B, R;
   void* work;
   int rows_per_img;
-  int nsplit_hint;
   int act;             // 0 ReLU score (torch flavour), 1 tanh (Genthial cell)
   int a_ch;            // channels of att1 / att2 / wf (0 = same as enc)
   uint8_t* mask_out;   // optional (ReLU score only): [B][R][A/8] bits (att1 + att2 > 0) of this step, for the backward
@@ -271,7 +268,6 @@ struct AttBwdArgs {
   int B, R;
   void* work;
   float* dwf_part;     // [B][A] running sum over the time loop of the full_att.weight gradient contributions (optional)
-  int nsplit_hint;
   int act;
   int a_ch;
   const uint8_t* mask_in;   // optional (ReLU score only): the forward's mask bits; the kernel then streams enc + 1 bit per att1
@@ -310,17 +306,6 @@ int tc_gemm_nt(const bf16* A, int64_t lda, const bf16* W, int64_t ldw, void* C, 
                int M, int N, int K, const float* bias, int accumulate, int relu, cudaStream_t st);
 int tc_gemm_nt_ex(const bf16* A, int64_t lda, const bf16* W, int64_t ldw, void* C, int dtC, int64_t ldc, int M, int N, int K,
                   const float* bias, int accumulate, int relu, int splits, int atomic_acc, int small_n_tile, cudaStream_t st);
-struct TcLstmEpi {
-  const float* ptab; const int64_t* tok; int64_t tok_stride;
-  const float* hh; int64_t hh_stride;
-  const float* c_prev; float* gates; float* c_out; float* h_out; bf16* h_bf;
-  float* hd; int64_t hd_stride; const float* dmask;
-  int D, V;
-  // in-kernel dropout (has_dropout = 2): Philox state, drop probability, first batch row of this launch, step index
-  const unsigned long long* dstate; float dp; int row0, t_idx;
-};
-int tc_gemm_nt_lstm(const bf16* A, int64_t lda, const bf16* Wil, int64_t ldw, int M, int D, int K, const TcLstmEpi& e, cudaStream_t st);
-int skinny_gemm_nt_lstm(const bf16* A, int64_t lda, const bf16* Wil, int64_t ldw, int M, int D, int K, const TcLstmEpi& e, cudaStream_t st);
 int skinny_gemm_nt(const bf16* A, int64_t lda, const bf16* W, int64_t ldw, float* C, int64_t ldc, int M, int N, int K, const float* bias,
                    int splits, int atomic_acc, cudaStream_t st);
 int resident_ctas(const void* kernel, int threads, size_t smem);

@@ -1060,11 +1060,11 @@ static inline Dims dims(const lo_decoder_args* a) {
 // bf16 staging used when impl == TC: mirrors written by the step kernels feed the wgmma GEMMs directly
 struct BfViews {
   bool on;
-  bf16 *dcat, *hall, *gctx, *wet, *onehot, *hd, *dlogits, *wfct, *wil, *alphas, *dctx, *dptab, *wihT;
+  bf16 *dcat, *hall, *gctx, *wet, *onehot, *hd, *dlogits, *wfct, *alphas, *dctx, *dptab, *wihT;
 };
 static inline int64_t rpad8(int64_t r) { return (r + 7) / 8 * 8; }
 static BfViews bf_views(const lo_decoder_args* a, const Dims& d) {
-  BfViews v{false, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+  BfViews v{false, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
   if (a->impl == LO_IMPL_TC && a->dt == LO_BF16 && a->bfwork && tc_available()) {
     const int64_t TB = (int64_t)d.T * d.B;
     v.on = true;
@@ -1076,8 +1076,7 @@ static BfViews bf_views(const lo_decoder_args* a, const Dims& d) {
     v.hd = v.onehot + TB * ((d.V + 7) / 8 * 8);
     v.dlogits = v.hd + TB * d.D;
     v.wfct = v.dlogits + TB * d.Vl;
-    v.wil = v.wfct + (int64_t)d.D * d.Vl;
-    v.alphas = v.wil + (int64_t)4 * d.D * d.C;            // [B][T][roundup8(R)] (zero padded): A operand of the batched alpha^T dctx GEMM
+    v.alphas = v.wfct + (int64_t)d.D * d.Vl;               // [B][T][roundup8(R)] (zero padded): A operand of the batched alpha^T dctx GEMM
     v.dctx = v.alphas + TB * rpad8(d.R);                   // [B][T][C]
     v.dptab = v.dctx + TB * d.C;                           // [V][4D] bf16 copy of the embedding-table gradient
     v.wihT = v.dptab + (int64_t)d.V * d.G;                 // [E][4D] = (weight_ih[:, :E])^T
@@ -1132,16 +1131,16 @@ template <class Args>            // lo_decoder_args or lo_tfdec_args
 static int check_reg_off(const Args* a, bool decode) {
   return check_reg_off(a->reg_off, a->reg_off_host, a->B, a->rows_per_img, a->R, decode);
 }
-// the ragged attention state of a decode call: map in the second attention region of `work` (the decode loop runs one row chain)
+// the ragged attention state of a decode call: map in the second attention region of `work` (the time loop's launches use the first)
 static AttRagged ragged_of(const lo_decoder_args* a) {
   return AttRagged{a->reg_off, a->reg_off_host, (char*)a->work + lo_attention_workspace_bytes(a->B, a->C), 0};
 }
 
 static int* work_counters(const lo_decoder_args* a) { return (int*)a->work; }
-// ReLU mask bits of step t, first row r0 (NULL when the scheme is off)
-static inline uint8_t* att_mask_at(const lo_decoder_args* a, int t, int64_t r0) {
+// ReLU mask bits of step t (NULL when the scheme is off)
+static inline uint8_t* att_mask_at(const lo_decoder_args* a, int t) {
   if (!a->att_mask || !g_opt_att_maskbits || !g_opt_att_pipe || a->rows_per_img > 1) return nullptr;
-  return a->att_mask + ((int64_t)t * a->B + r0) * ((a->R + 1) & ~1) * (a->A / 8);      // rows padded to an even count (pair layout)
+  return a->att_mask + (int64_t)t * a->B * ((a->R + 1) & ~1) * (a->A / 8);      // rows padded to an even count (pair layout)
 }
 static float* work_partials(const lo_decoder_args* a) { return (float*)((char*)a->work + att_partials_offset(a->B)); }
 static int32_t* work_dlen(const lo_decoder_args* a) { return (int32_t*)((char*)a->work + 2048); }
@@ -1149,11 +1148,11 @@ static int32_t* work_dlen(const lo_decoder_args* a) { return (int32_t*)((char*)a
 static int attention_forward_launch(const void* att1, const void* enc, int dt, const float* att2, int64_t att2_stride,
                                     const float* wf, float* alpha, int64_t alpha_stride, float* ctx, float* gate_pre,
                                     int64_t gate_stride, float* gctx, bf16* gctx_bf, int B, int R, int C, void* work, cudaStream_t st,
-                                    int rpi = 1, int nsplit_hint = 0, uint8_t* mask_out = nullptr, int abi = 0) {
+                                    int rpi = 1, uint8_t* mask_out = nullptr, int abi = 0) {
   if (rpi < 1) rpi = 1;
   if (g_opt_att_pipe) {
     AttFwdArgs x{att1, enc, att2, att2_stride, wf, alpha, alpha_stride, ctx, gate_pre, gate_stride, gctx, gctx_bf, B, R, work, rpi,
-                 nsplit_hint, 0, 0, mask_out, abi};
+                 0, 0, mask_out, abi};
     return attention_fwd_pipe(x, dt, C, st);
   }
   const int ns = att_splits(B);
@@ -1202,19 +1201,6 @@ __global__ void split_bf16_kernel(const float* __restrict__ x, bf16* __restrict_
   }
 }
 
-// wil[4*j + g][c] = w_ih[g*D + j][E + c]: gate-interleaved copy of the context half of weight_ih, so that one 32-column
-// accumulator chunk of the wgmma GEMM holds whole hidden units and the LSTM cell can run in its epilogue
-__global__ void interleave_wih_kernel(const bf16* __restrict__ w_ih, bf16* __restrict__ wil, int D, int E, int C) {
-  const int64_t total = (int64_t)4 * D * (C / 8);
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-    const int c8 = (int)(i % (C / 8));
-    const int n = (int)(i / (C / 8));        // interleaved row 4*j + g
-    const int j = n >> 2, g = n & 3;
-    *reinterpret_cast<uint4*>(wil + (int64_t)n * C + c8 * 8) =
-        *reinterpret_cast<const uint4*>(w_ih + ((int64_t)g * D + j) * (E + C) + E + c8 * 8);
-  }
-}
-
 static int forward_prologue(const lo_decoder_args* a, const Dims& d, cudaStream_t st) {
   const int dt = a->dt;
   const int rpi = a->rows_per_img > 1 ? a->rows_per_img : 1;
@@ -1258,25 +1244,9 @@ static int forward_prologue(const lo_decoder_args* a, const Dims& d, cudaStream_
                    d.D, d.C, a->b_init + d.D, 0, 0, LO_IMPL_SIMT, st));
   }
   const BfViews bv = bf_views(a, d);
-  if (bv.on) {
-    LO_TRY(lo_cast(a->hall, LO_F32, bv.hall, LO_BF16, (int64_t)d.B * d.D, (void*)st));
-    if (g_opt_fuse_lstm && d.E % 8 == 0 && d.C % 8 == 0) {
-      interleave_wih_kernel<<<LO_NUM_SMS * 2, 256, 0, st>>>((const bf16*)a->w_ih, bv.wil, d.D, d.E, d.C);
-      LO_LAUNCH_OK();
-    }
-  }
+  if (bv.on) LO_TRY(lo_cast(a->hall, LO_F32, bv.hall, LO_BF16, (int64_t)d.B * d.D, (void*)st));
   return LO_OK;
 }
-
-// a contiguous slice of batch rows processed on one stream.  The rows of a batch never interact inside the time loop
-// (only the hoisted weight-gradient GEMMs mix them), so the loop can run as independent half-batch chains on two
-// streams: while one chain streams att1/enc (HBM bound, all SMs) the other runs its latency-bound GEMM / LSTM kernels.
-struct Rows {
-  int row0, nrows;
-  void* work;       // attention workspace of this chain
-  int nsplit;       // attention split hint (0 = automatic)
-  const AttRagged* rg = nullptr;     // decode with per-image region counts: the whole batch, row0 = 0
-};
 
 // C (+)= A W^T for the per-step GEMMs of the time loops (M <= B rows): the mma.sync kernel for <= 64 rows of the bf16 mirror Abf,
 // wgmma above, CUDA cores on the fp32 operand A32 when there are no mirrors (tc false).  The tensor-core paths run `splits` K slices
@@ -1299,86 +1269,57 @@ static int head_nt(const lo_decoder_args* a, bool tc, const float* h32, const bf
   return gemm_nt(h32, LO_F32, ldh, a->w_fc, a->dt, a->D, logits, LO_F32, ldl, M, a->V, a->D, a->b_fc, 0, 0, LO_IMPL_SIMT, st);
 }
 
-// the LSTM cell of step t for the rows from r0 on, run in the epilogue of the gates GEMM: tok, hd_t, dmask_t point at row 0
-static TcLstmEpi lstm_epi(const lo_decoder_args* a, const Dims& d, const BfViews& bv, int t, int64_t r0, const int64_t* tok,
-                          int64_t tok_stride, float* hd_t, int64_t hd_stride, const float* dmask_t) {
-  const int64_t cur = (int64_t)t * d.B + r0, nxt = (int64_t)(t + 1) * d.B + r0;
-  return TcLstmEpi{a->ptab, tok + r0 * tok_stride, tok_stride, a->out1 + cur * d.O1 + d.A + d.C, d.O1, a->call + cur * d.D,
-                   a->gates + cur * d.G, a->call + nxt * d.D, a->hall + nxt * d.D, bv.hall + nxt * d.D,
-                   hd_t ? hd_t + r0 * hd_stride : (float*)nullptr, hd_stride, dmask_t ? dmask_t + r0 * hd_stride : (const float*)nullptr,
-                   d.D, d.V, (const unsigned long long*)((hd_t && a->has_dropout == 2) ? a->dropout_state : nullptr), a->dropout_p,
-                   (int)r0, t};
-}
-
-// one decoder step t for the rows of `rs`; tok: token ids consumed at this step (row 0 of the batch)
-static int forward_step(const lo_decoder_args* a, const Dims& d, int t, const Rows& rs, const int64_t* tok, int64_t tok_stride,
-                        float* hd_t, int64_t hd_stride, const float* dmask_t, cudaStream_t st) {
+// one decoder step t for the first nrows rows of the batch (those still decoding); rg: decode with per-image region counts (the
+// whole batch), else null; tok: token ids consumed at this step
+static int forward_step(const lo_decoder_args* a, const Dims& d, int t, int nrows, const AttRagged* rg, const int64_t* tok,
+                        int64_t tok_stride, float* hd_t, int64_t hd_stride, const float* dmask_t, cudaStream_t st) {
   const int dt = a->dt;
-  const int nrows = rs.nrows;
-  const int64_t r0 = rs.row0;
   const bool sampling = a->ss_prob && hd_t;     // scheduled sampling: token chosen in the cell, head inside the loop
-  if (nrows <= 0) return LO_OK;
   const size_t es = dt == LO_F32 ? 4 : 2;
-  float* h_prev = a->hall + ((int64_t)t * d.B + r0) * d.D;
-  float* c_prev = a->call + ((int64_t)t * d.B + r0) * d.D;
-  float* o1 = a->out1 + ((int64_t)t * d.B + r0) * d.O1;
-  float* gtmp = a->gtmp + r0 * d.G;
-  const int rpi = a->rows_per_img > 1 ? a->rows_per_img : 1;
-  const char* att1 = (const char*)a->att1 + (size_t)(r0 / rpi) * d.R * d.A * es;
-  const char* enc = (const char*)a->enc + (size_t)(r0 / rpi) * d.R * d.C * es;
+  const int64_t cur = (int64_t)t * d.B, nxt = (int64_t)(t + 1) * d.B;     // first row of steps t and t + 1 (time-major arrays)
+  float* o1 = a->out1 + cur * d.O1;
   // [att2 | gate_pre | hh_pre] = h_prev @ [W_d; W_beta; W_hh]^T + b   (seq2seq_torch.py:187, :311, LSTMCell hh part)
   const BfViews bv = bf_views(a, d);
   if (!(g_opt_dbg_skip & 4))
-    LO_TRY(step_gemm_nt(bv.on, h_prev, bv.on ? bv.hall + ((int64_t)t * d.B + r0) * d.D : nullptr, d.D, a->wcat1, dt, d.D, o1, d.O1, nrows,
+    LO_TRY(step_gemm_nt(bv.on, a->hall + cur * d.D, bv.on ? bv.hall + cur * d.D : nullptr, d.D, a->wcat1, dt, d.D, o1, d.O1, nrows,
                         d.O1, d.D, a->bcat1, 0, 1, 0, st));
-  if (rs.rg) {
+  if (rg) {
     if (!(g_opt_dbg_skip & 2)) {
-      AttFwdArgs x{a->att1, a->enc, o1, d.O1, a->w_full, a->alphas + t * d.R, (int64_t)d.T * d.R, a->ctx + (int64_t)t * d.B * d.C, o1 + d.A,
-                   d.O1, a->gctx + (int64_t)t * d.B * d.C, bv.on ? bv.gctx + (int64_t)t * d.B * d.C : nullptr, nrows, d.R, rs.work,
-                   a->rows_per_img, 0, 0, 0, nullptr, 0};
-      LO_TRY(attention_fwd_ragged(x, *rs.rg, dt, d.C, st));
+      AttFwdArgs x{a->att1, a->enc, o1, d.O1, a->w_full, a->alphas + t * d.R, (int64_t)d.T * d.R, a->ctx + cur * d.C, o1 + d.A,
+                   d.O1, a->gctx + cur * d.C, bv.on ? bv.gctx + cur * d.C : nullptr, nrows, d.R, a->work, a->rows_per_img, 0, 0, nullptr, 0};
+      LO_TRY(attention_fwd_ragged(x, *rg, dt, d.C, st));
     }
   } else if (!(g_opt_dbg_skip & 2))
-  LO_TRY(attention_forward_launch(att1, enc, dt, o1, d.O1, a->w_full, a->alphas + (r0 * d.T + t) * d.R, (int64_t)d.T * d.R,
-                                  a->ctx + ((int64_t)t * d.B + r0) * d.C, o1 + d.A, d.O1, a->gctx + ((int64_t)t * d.B + r0) * d.C,
-                                  bv.on ? bv.gctx + ((int64_t)t * d.B + r0) * d.C : nullptr, nrows, d.R, d.C, rs.work, st,
-                                  a->rows_per_img, rs.nsplit, hd_t ? att_mask_at(a, t, r0) : nullptr));
+  LO_TRY(attention_forward_launch(a->att1, a->enc, dt, o1, d.O1, a->w_full, a->alphas + t * d.R, (int64_t)d.T * d.R, a->ctx + cur * d.C,
+                                  o1 + d.A, d.O1, a->gctx + cur * d.C, bv.on ? bv.gctx + cur * d.C : nullptr, nrows, d.R, d.C, a->work, st,
+                                  a->rows_per_img, hd_t ? att_mask_at(a, t) : nullptr));
   if (g_opt_dbg_skip & 4) return LO_OK;
   // gates_x = (gate*ctx) @ W_ih[:, E:]^T
-  if (bv.on && g_opt_fuse_lstm && !sampling) {
-    // ... with the LSTM cell fused into the GEMM epilogue (no gates_x round trip, one launch less per step)
-    const TcLstmEpi e = lstm_epi(a, d, bv, t, r0, tok, tok_stride, hd_t, hd_stride, dmask_t);
-    if (g_opt_skinny_mma && nrows <= 64 && d.C <= 512)
-      return skinny_gemm_nt_lstm(bv.gctx + ((int64_t)t * d.B + r0) * d.C, d.C, bv.wil, d.C, nrows, d.D, d.C, e, st);
-    return tc_gemm_nt_lstm(bv.gctx + ((int64_t)t * d.B + r0) * d.C, d.C, bv.wil, d.C, nrows, d.D, d.C, e, st);
-  }
-  LO_TRY(step_gemm_nt(bv.on, a->gctx + ((int64_t)t * d.B + r0) * d.C, bv.on ? bv.gctx + ((int64_t)t * d.B + r0) * d.C : nullptr, d.C,
-                      (const char*)a->w_ih + (size_t)d.E * es, dt, d.E + d.C, gtmp, d.G, nrows, d.G, d.C, nullptr, 0, 1, 0, st));
+  LO_TRY(step_gemm_nt(bv.on, a->gctx + cur * d.C, bv.on ? bv.gctx + cur * d.C : nullptr, d.C, (const char*)a->w_ih + (size_t)d.E * es, dt,
+                      d.E + d.C, a->gtmp, d.G, nrows, d.G, d.C, nullptr, 0, 1, 0, st));
   SsStep ss{};
   if (sampling) {
-    ss.prev_logits = t > 0 ? a->logits + (r0 * d.T + t - 1) * d.Vl : nullptr;
+    ss.prev_logits = t > 0 ? a->logits + (int64_t)(t - 1) * d.Vl : nullptr;
     ss.lstride = (int64_t)d.T * d.Vl;
     ss.prob = a->ss_prob;
-    ss.u = a->ss_u ? a->ss_u + r0 * d.T + t : nullptr;
+    ss.u = a->ss_u ? a->ss_u + t : nullptr;
     ss.coin_state = (const unsigned long long*)a->dropout_state;
     ss.ustride = d.T;
-    ss.fed = a->fed + r0 * d.T + t;
-    ss.hd_bf = bv.on ? bv.hd + r0 * hd_stride + t * d.D : nullptr;
+    ss.fed = a->fed + t;
+    ss.hd_bf = bv.on ? bv.hd + t * d.D : nullptr;
   }
-  // the pointwise launch; `extra` is the GumbelStep of the sampling kernel with a temperature
+  // the pointwise launch; `extra` is the GumbelStep of the sampling kernel with a temperature.  Its row0 argument (the first batch row
+  // of the launch) is 0: every launch starts at row 0.
   auto launch_pw = [&](auto kernel, auto... extra) {
-    return launch_pdl(kernel, dim3(cdiv((long)nrows * d.D, 256)), dim3(256), (size_t)0, st, (const float*)gtmp,
-                      (const float*)a->ptab, tok + r0 * tok_stride, tok_stride, (const float*)(o1 + d.A + d.C), (int64_t)d.O1,
-                      (const float*)c_prev, a->gates + ((int64_t)t * d.B + r0) * d.G, a->call + ((int64_t)(t + 1) * d.B + r0) * d.D,
-                      a->hall + ((int64_t)(t + 1) * d.B + r0) * d.D,
-                      bv.on ? bv.hall + ((int64_t)(t + 1) * d.B + r0) * d.D : (bf16*)nullptr,
-                      hd_t ? hd_t + r0 * hd_stride : (float*)nullptr, hd_stride,
-                      dmask_t ? dmask_t + r0 * hd_stride : (const float*)nullptr, nrows, d.D, d.V,
-                      (const unsigned long long*)((hd_t && a->has_dropout == 2) ? a->dropout_state : nullptr), a->dropout_p, (int)r0,
-                      t, ss, extra...);
+    return launch_pdl(kernel, dim3(cdiv((long)nrows * d.D, 256)), dim3(256), (size_t)0, st, (const float*)a->gtmp,
+                      (const float*)a->ptab, tok, tok_stride, (const float*)(o1 + d.A + d.C), (int64_t)d.O1,
+                      (const float*)(a->call + cur * d.D), a->gates + cur * d.G, a->call + nxt * d.D, a->hall + nxt * d.D,
+                      bv.on ? bv.hall + nxt * d.D : (bf16*)nullptr, hd_t, hd_stride, dmask_t, nrows, d.D, d.V,
+                      (const unsigned long long*)((hd_t && a->has_dropout == 2) ? a->dropout_state : nullptr), a->dropout_p, 0, t, ss,
+                      extra...);
   };
   if (sampling && a->ss_temp) {
-    const GumbelStep gs{a->ss_temp, a->ss_gu ? a->ss_gu + (r0 * d.T + t) * d.V : nullptr, (int64_t)d.T * d.V};
+    const GumbelStep gs{a->ss_temp, a->ss_gu ? a->ss_gu + (int64_t)t * d.V : nullptr, (int64_t)d.T * d.V};
     LO_CUDA(launch_pw(lstm_pw_fwd_gumbel_kernel, gs));
   } else {
     LO_CUDA(launch_pw(sampling ? lstm_pw_fwd_kernel<true> : lstm_pw_fwd_kernel<false>));
@@ -1387,63 +1328,57 @@ static int forward_step(const lo_decoder_args* a, const Dims& d, int t, const Ro
   if (sampling) {
     // the head of step t, right after the cell (the next step's cell reads these logits, see lstm_pw_fwd_kernel): the returned
     // predictions of this mode
-    LO_TRY(head_nt(a, bv.on, hd_t + r0 * hd_stride, ss.hd_bf, hd_stride, a->logits + (r0 * d.T + t) * d.Vl, (int64_t)d.T * d.Vl, nrows, st));
+    LO_TRY(head_nt(a, bv.on, hd_t, ss.hd_bf, hd_stride, a->logits + (int64_t)t * d.Vl, (int64_t)d.T * d.Vl, nrows, st));
   }
   return LO_OK;
 }
 
-// one backward step t for the rows of `rs`, the launches of forward_step in reverse; dal, dal_b, dal_t: the d alpha rows of
+// one backward step t for the first nrows rows, the launches of forward_step in reverse; dal, dal_b, dal_t: the d alpha rows of
 // lo_decoder_backward
-static int backward_step(const lo_decoder_args* a, const Dims& d, int t, const Rows& rs, const float* dal, int64_t dal_b, int64_t dal_t,
+static int backward_step(const lo_decoder_args* a, const Dims& d, int t, int nrows, const float* dal, int64_t dal_b, int64_t dal_t,
                          cudaStream_t st) {
   const int dt = a->dt;
-  const int nrows = rs.nrows;
-  const int64_t r0 = rs.row0;
-  if (nrows <= 0) return LO_OK;
-  const size_t es = dt == LO_F32 ? 4 : 2;
   const BfViews bv = bf_views(a, d);
-  float* dcat_t = a->dcat + ((int64_t)t * d.B + r0) * d.O1;
-  bf16* dcat_bf_t = bv.on ? bv.dcat + ((int64_t)t * d.B + r0) * d.O1 : nullptr;
-  const float* o1 = a->out1 + ((int64_t)t * d.B + r0) * d.O1;
-  float* dxh = a->dxh + r0 * (d.C + d.D);
-  const float* dmul = (a->has_dropout == 1 && a->dropout_mask) ? a->dropout_mask + (int64_t)t * d.D + r0 * d.T * d.D : nullptr;
-  if (!(g_opt_dbg_skip & 4))
+  const int64_t cur = (int64_t)t * d.B, nxt = (int64_t)(t + 1) * d.B;
+  float* dcat_t = a->dcat + cur * d.O1;
+  bf16* dcat_bf_t = bv.on ? bv.dcat + cur * d.O1 : nullptr;
+  const float* o1 = a->out1 + cur * d.O1;
+  float* dxh = a->dxh;
+  const float* dmul = (a->has_dropout == 1 && a->dropout_mask) ? a->dropout_mask + (int64_t)t * d.D : nullptr;
+  if (!(g_opt_dbg_skip & 4))   // row0 = 0 as in forward_step
     LO_CUDA(launch_pdl(lstm_pw_bwd_kernel, dim3(cdiv((long)nrows * d.D, 256)), dim3(256), (size_t)0, st,
-                       (const float*)(a->dhd + (int64_t)t * d.D + r0 * d.T * d.D), (int64_t)d.T * d.D, dmul, (const float*)(dxh + d.C),
-                       (int64_t)(d.C + d.D), a->dc + r0 * d.D, (const float*)(a->gates + ((int64_t)t * d.B + r0) * d.G),
-                       (const float*)(a->call + ((int64_t)t * d.B + r0) * d.D),
-                       (const float*)(a->call + ((int64_t)(t + 1) * d.B + r0) * d.D), dcat_t + d.A + d.C, (int64_t)d.O1,
+                       (const float*)(a->dhd + (int64_t)t * d.D), (int64_t)d.T * d.D, dmul, (const float*)(dxh + d.C),
+                       (int64_t)(d.C + d.D), a->dc, (const float*)(a->gates + cur * d.G), (const float*)(a->call + cur * d.D),
+                       (const float*)(a->call + nxt * d.D), dcat_t + d.A + d.C, (int64_t)d.O1,
                        bv.on ? dcat_bf_t + d.A + d.C : (bf16*)nullptr, bv.on ? dxh : (float*)nullptr, d.C, nrows, d.D,
-                       (const unsigned long long*)(a->has_dropout == 2 ? a->dropout_state : nullptr), a->dropout_p, (int)r0, t));
+                       (const unsigned long long*)(a->has_dropout == 2 ? a->dropout_state : nullptr), a->dropout_p, 0, t));
   LO_LAUNCH_OK();
   // [dgctx | dh_prev] = dG @ [W_ih[:, E:] | W_hh]
   if (!(g_opt_dbg_skip & 4))
     LO_TRY(step_gemm_nt(bv.on, dcat_t + d.A + d.C, bv.on ? dcat_bf_t + d.A + d.C : nullptr, d.O1, a->wbwd1, dt, d.G, dxh, d.C + d.D,
                         nrows, d.C + d.D, d.G, nullptr, 0, 4, 1, st));
-  const char* att1 = (const char*)a->att1 + (size_t)r0 * d.R * d.A * es;
-  const char* enc = (const char*)a->enc + (size_t)r0 * d.R * d.C * es;
-  const float* alpha_t = a->alphas + (r0 * d.T + t) * d.R;
-  const float* ctx_t = a->ctx + ((int64_t)t * d.B + r0) * d.C;
-  const float* dal_t_ptr = dal + (int64_t)t * dal_t + r0 * dal_b;
-  const float* sreg_t = a->sreg + r0 * d.T + t;
-  float* de_t = a->de + (r0 * d.T + t) * d.R;
-  float* dctx_t = a->dctx + ((int64_t)t * d.B + r0) * d.C;
+  const float* alpha_t = a->alphas + t * d.R;
+  const float* ctx_t = a->ctx + cur * d.C;
+  const float* dal_t_ptr = dal + (int64_t)t * dal_t;
+  const float* sreg_t = a->sreg + t;
+  float* de_t = a->de + t * d.R;
+  float* dctx_t = a->dctx + cur * d.C;
   if (g_opt_dbg_skip & 2) {
   } else if (g_opt_att_pipe) {
-    AttBwdArgs x{att1, enc, o1, o1 + d.A, d.O1, a->w_full, alpha_t, (int64_t)d.T * d.R, ctx_t, dxh, d.C + d.D, dal_t_ptr, dal_b, sreg_t,
-                 d.T, de_t, dcat_t, dcat_t + d.A, d.O1, dcat_bf_t, dcat_bf_t ? dcat_bf_t + d.A : nullptr, dctx_t, nrows, d.R, rs.work,
-                 a->dmean + r0 * d.A, rs.nsplit, 0, 0, att_mask_at(a, t, r0)};
+    AttBwdArgs x{a->att1, a->enc, o1, o1 + d.A, d.O1, a->w_full, alpha_t, (int64_t)d.T * d.R, ctx_t, dxh, d.C + d.D, dal_t_ptr, dal_b,
+                 sreg_t, d.T, de_t, dcat_t, dcat_t + d.A, d.O1, dcat_bf_t, dcat_bf_t ? dcat_bf_t + d.A : nullptr, dctx_t, nrows, d.R,
+                 a->work, a->dmean, 0, 0, att_mask_at(a, t)};
     LO_TRY(attention_bwd_pipe(x, dt, d.C, st));
   } else {
     const int ns = att_splits(d.B);
-    int* cnt_c = (int*)rs.work;
-    float* part_c = (float*)((char*)rs.work + att_partials_offset(nrows));
+    int* cnt_c = (int*)a->work;
+    float* part_c = (float*)((char*)a->work + att_partials_offset(nrows));
     dim3 grid(ns, nrows);
 #define LO_ATT_BWD(TY_, NV)                                                                                                       \
   attention_bwd_kernel<TY_, NV><<<grid, LO_ATT_THREADS, 0, st>>>(                                                                 \
-      (const TY_*)att1, (const TY_*)enc, o1, o1 + d.A, d.O1, a->w_full, alpha_t, (int64_t)d.T * d.R, ctx_t, dxh, d.C + d.D, dal_t_ptr, \
-      dal_b, sreg_t, d.T, de_t, dcat_t, dcat_t + d.A, d.O1, dcat_bf_t, dcat_bf_t ? dcat_bf_t + d.A : nullptr, dctx_t, d.R, ns, cnt_c,  \
-      part_c)
+      (const TY_*)a->att1, (const TY_*)a->enc, o1, o1 + d.A, d.O1, a->w_full, alpha_t, (int64_t)d.T * d.R, ctx_t, dxh, d.C + d.D,    \
+      dal_t_ptr, dal_b, sreg_t, d.T, de_t, dcat_t, dcat_t + d.A, d.O1, dcat_bf_t, dcat_bf_t ? dcat_bf_t + d.A : nullptr, dctx_t, d.R, \
+      ns, cnt_c, part_c)
     if (dt == LO_F32) {
       if (d.C == 256) LO_ATT_BWD(float, 1); else if (d.C == 512) LO_ATT_BWD(float, 2); else LO_ATT_BWD(float, 4);
     } else {
@@ -1457,32 +1392,6 @@ static int backward_step(const lo_decoder_args* a, const Dims& d, int t, const R
     LO_TRY(step_gemm_nt(bv.on, dcat_t, dcat_bf_t, d.O1, a->wbwd2, dt, d.A + d.C, dxh + d.C, d.C + d.D, nrows, d.D, d.A + d.C, nullptr, 1,
                         4, 1, st));
   return LO_OK;
-}
-
-// fork/join helpers for the two-chain time loop (legal inside stream capture: the side stream joins back)
-static cudaStream_t g_side = nullptr;
-static cudaEvent_t g_ev_fork = nullptr, g_ev_join = nullptr;
-static int side_stream_init() {
-  if (g_side) return LO_OK;
-  LO_CUDA(cudaStreamCreateWithFlags(&g_side, cudaStreamNonBlocking));
-  LO_CUDA(cudaEventCreateWithFlags(&g_ev_fork, cudaEventDisableTiming));
-  LO_CUDA(cudaEventCreateWithFlags(&g_ev_join, cudaEventDisableTiming));
-  return LO_OK;
-}
-static inline bool two_chains(const lo_decoder_args* a, const Dims& d) {
-  return g_opt_dec_streams >= 2 && d.B >= 32 && a->rows_per_img <= 1;
-}
-static inline Rows chain_rows(const lo_decoder_args* a, const Dims& d, int chain, int nchains, int active) {
-  // rows [0, half) -> chain 0, [half, B) -> chain 1; `active` = rows still decoding at this step (sorted by length)
-  const int half = nchains == 2 ? (d.B + 1) / 2 : d.B;
-  Rows r;
-  r.row0 = chain * half;
-  const int hi = chain == 0 ? (active < half ? active : half) : active;
-  r.nrows = hi - r.row0 > 0 ? hi - r.row0 : 0;
-  if (chain == 0 && nchains == 1) r.nrows = active;
-  r.work = (char*)a->work + (size_t)chain * lo_attention_workspace_bytes(d.B, d.C);
-  r.nsplit = nchains == 2 ? (LO_NUM_SMS / (half > 0 ? half : 1) > 0 ? LO_NUM_SMS / half : 1) : 0;   // each chain fills one CTA slot per SM
-  return r;
 }
 
 // one beam-search step of either decoder flavour (beam_step_kernel, one CTA per image): the top-k over beam x V log-probs in shared
@@ -1657,7 +1566,7 @@ struct TorchDecode {
   }
   // the cell step, then logits_t = fc(h_t)   (no dropout at decode time)
   int step(int t, cudaStream_t st) {
-    LO_TRY(forward_step(a, d, t, Rows{0, d.B, a->work, 0, c.ragged()}, c.next_tok, 1, nullptr, 0, nullptr, st));
+    LO_TRY(forward_step(a, d, t, d.B, c.ragged(), c.next_tok, 1, nullptr, 0, nullptr, st));
     const int64_t h_t = (int64_t)(t + 1) * d.B * d.D;
     return head_nt(a, bv.on, a->hall + h_t, bv.on ? bv.hall + h_t : nullptr, d.D, a->logits, d.V, d.B, st);
   }
@@ -1689,7 +1598,7 @@ int64_t lo_decoder_bfwork_bytes(const lo_decoder_args* a) {
   const int64_t Vp = (a->V + 7) / 8 * 8;
   const int64_t Vl = a->ldl > 0 ? a->ldl : a->V;
   return (TB * (O1 + a->D + a->C + Vp + a->D + Vl) + (int64_t)a->B * a->D + (int64_t)a->A * a->C + (int64_t)a->D * Vl +
-          (int64_t)4 * a->D * a->C + TB * ((a->R + 7) / 8 * 8) + TB * a->C + (int64_t)(a->V + a->E) * 4 * a->D) * 2 + 1024;
+          TB * ((a->R + 7) / 8 * 8) + TB * a->C + (int64_t)(a->V + a->E) * 4 * a->D) * 2 + 1024;
 }
 
 int64_t lo_sizeof_decoder_args(void) { return (int64_t)sizeof(lo_decoder_args); }
@@ -1697,7 +1606,8 @@ int64_t lo_sizeof_decoder_args(void) { return (int64_t)sizeof(lo_decoder_args); 
 int64_t lo_attention_workspace_bytes(int B, int C) {
   return att_partials_offset(B) + (int64_t)B * LO_ATT_MAXSPLIT * (C + 2) * 4;
 }
-/* the decoder entry points use two such regions (one per row chain) */
+/* the decoder entry points use two such regions: the first for the attention launches of the time loop, the second for the CTA map
+   of a decode call with per-image region counts (ragged_of) */
 int64_t lo_decoder_workspace_bytes(int B, int C) { return 2 * lo_attention_workspace_bytes(B, C); }
 
 int lo_attention_forward(const void* att1, const void* enc, int dt, const float* att2, int64_t att2_stride, const float* wf,
@@ -1708,7 +1618,7 @@ int lo_attention_forward(const void* att1, const void* enc, int dt, const float*
   LO_CHECK_ARG(B > 0 && B <= 512 && R > 0, "B in 1..512, R > 0");
   LO_CHECK_ARG(att2_stride % 4 == 0, "att2 rows must be 16-byte aligned");
   return attention_forward_launch(att1, enc, dt, att2, att2_stride, wf, alpha, alpha_stride, ctx, gate_pre, gate_stride, gctx, nullptr,
-                                  B, R, C, work, (cudaStream_t)stream, 1, 0, nullptr, 1);
+                                  B, R, C, work, (cudaStream_t)stream, 1, nullptr, 1);
 }
 
 int lo_attention_forward_mask(const void* att1, const void* enc, int dt, const float* att2, int64_t att2_stride, const float* wf,
@@ -1720,7 +1630,7 @@ int lo_attention_forward_mask(const void* att1, const void* enc, int dt, const f
   LO_CHECK_ARG(att2_stride % 4 == 0, "att2 rows must be 16-byte aligned");
   LO_CHECK_ARG(!relu_mask_out || g_opt_att_pipe, "mask bits are written by the TMA-ring kernel (option att_pipe=1)");
   return attention_forward_launch(att1, enc, dt, att2, att2_stride, wf, alpha, alpha_stride, ctx, gate_pre, gate_stride, gctx, nullptr,
-                                  B, R, C, work, (cudaStream_t)stream, 1, 0, relu_mask_out, 1);
+                                  B, R, C, work, (cudaStream_t)stream, 1, relu_mask_out, 1);
 }
 
 int lo_attention_backward(const void* att1, const void* enc, int dt, const float* att2, const float* gate, int64_t o1_stride,
@@ -1733,7 +1643,7 @@ int lo_attention_backward(const void* att1, const void* enc, int dt, const float
   LO_CHECK_ARG(B > 0 && B <= 512 && R > 0, "B in 1..512, R > 0");
   LO_CHECK_ARG(g_opt_att_pipe, "stand-alone attention backward runs on the TMA-ring kernel (option att_pipe=1)");
   AttBwdArgs x{att1, enc, att2, gate, o1_stride, wf, alpha, alpha_stride, ctx, dgctx, dg_stride, dreg, dreg_stride, sreg, sreg_stride,
-               de, datt2, dgp, dcat_stride, nullptr, nullptr, dctx_out, B, R, work, dwf_part, 0, 0, 0, relu_mask};
+               de, datt2, dgp, dcat_stride, nullptr, nullptr, dctx_out, B, R, work, dwf_part, 0, 0, relu_mask};
   x.abi = 1;
   return attention_bwd_pipe(x, dt, C, (cudaStream_t)stream);
 }
@@ -1785,7 +1695,7 @@ int lo_attention_step_backward(const void* enc, const void* att1, int dt, const 
   }
   if (g_w_full) LO_CUDA(cudaMemsetAsync(ws_dwf, 0, (size_t)B * A * 4, st));
   AttBwdArgs x{att1, enc, att2, nullptr, A, wf, alpha, R, ctx, dctx, C, dalpha, R, dalpha ? ws_sreg : nullptr, 1, de_, datt2_, nullptr, A,
-               nullptr, nullptr, nullptr, B, R, work, g_w_full ? ws_dwf : nullptr, 0, 0, 0, nullptr};
+               nullptr, nullptr, nullptr, B, R, work, g_w_full ? ws_dwf : nullptr, 0, 0, nullptr};
   x.abi = 1;
   x.datt1 = need_d1 ? d1 : nullptr;
   x.ordered_dwf = g_opt_det;
@@ -1840,24 +1750,11 @@ int lo_decoder_forward(const lo_decoder_args* a, int with_loss, void* stream) {
   LO_TRY(upload_dlen(a, st));
   if (a->phase != 2) {
   LO_TRY(forward_prologue(a, d, st));
-  const int nchains = two_chains(a, d) && !sampling ? 2 : 1;
-  if (nchains == 2) {
-    LO_TRY(side_stream_init());
-    LO_CUDA(cudaEventRecord(g_ev_fork, st));
-    LO_CUDA(cudaStreamWaitEvent(g_side, g_ev_fork, 0));
-  }
-  // the time loop (DESIGN.md §4): per-step launches on one or two row chains
-  for (int chain = 0; chain < nchains; chain++) {
-    cudaStream_t cs = chain == 0 ? st : g_side;
-    for (int t = 0; t < d.T; t++) {
-      const float* dm = (a->has_dropout == 1 && a->dropout_mask) ? a->dropout_mask + (int64_t)t * d.D : nullptr;
-      const Rows rs = chain_rows(a, d, chain, nchains, a->bt_host[t]);
-      LO_TRY(forward_step(a, d, t, rs, a->caps + t, a->caps_stride, a->hd + (int64_t)t * d.D, (int64_t)d.T * d.D, dm, cs));
-    }
-  }
-  if (nchains == 2) {
-    LO_CUDA(cudaEventRecord(g_ev_join, g_side));
-    LO_CUDA(cudaStreamWaitEvent(st, g_ev_join, 0));
+  // the time loop (DESIGN.md §4): per-step launches over the rows still decoding
+  for (int t = 0; t < d.T; t++) {
+    const float* dm = (a->has_dropout == 1 && a->dropout_mask) ? a->dropout_mask + (int64_t)t * d.D : nullptr;
+    LO_TRY(forward_step(a, d, t, a->bt_host[t], nullptr, a->caps + t, a->caps_stride, a->hd + (int64_t)t * d.D, (int64_t)d.T * d.D, dm,
+                        st));
   }
   }   // phase != 2
   if (a->phase == 1) return LO_OK;       // extension: the caller runs a second layer over hd before the head
@@ -1973,21 +1870,7 @@ int lo_decoder_backward(const lo_decoder_args* a, void* stream) {
   }
   const BfViews bv = bf_views(a, d);
   if (g_opt_att_pipe) LO_CUDA(cudaMemsetAsync(a->dmean, 0, (size_t)d.B * d.A * 4, st));    // [B][A] scratch for d w_full
-  const int nchains = two_chains(a, d) ? 2 : 1;
-  if (nchains == 2) {
-    LO_TRY(side_stream_init());
-    LO_CUDA(cudaEventRecord(g_ev_fork, st));
-    LO_CUDA(cudaStreamWaitEvent(g_side, g_ev_fork, 0));
-  }
-  for (int chain = 0; chain < nchains; chain++) {
-    cudaStream_t cs = chain == 0 ? st : g_side;
-    for (int t = d.T - 1; t >= 0; t--)
-      LO_TRY(backward_step(a, d, t, chain_rows(a, d, chain, nchains, a->bt_host[t]), dal, dal_b, dal_t, cs));
-  }
-  if (nchains == 2) {
-    LO_CUDA(cudaEventRecord(g_ev_join, g_side));
-    LO_CUDA(cudaStreamWaitEvent(st, g_ev_join, 0));
-  }
+  for (int t = d.T - 1; t >= 0; t--) LO_TRY(backward_step(a, d, t, a->bt_host[t], dal, dal_b, dal_t, st));
   // dinit = [dh0 | dc0]
   LO_CUDA(cudaMemcpy2DAsync(a->dinit, (size_t)2 * d.D * 4, a->dxh + d.C, (size_t)(d.C + d.D) * 4, (size_t)d.D * 4, d.B,
                             cudaMemcpyDeviceToDevice, st));
@@ -2046,7 +1929,7 @@ int lo_decoder_backward(const lo_decoder_args* a, void* stream) {
   }
   // d att1 + d w_full in one sweep over att1
   LO_CUDA(cudaMemsetAsync(a->g_b_full, 0, 4, st));   // sum_r de = 0 exactly (softmax); reference value is rounding noise
-  const bool pipe_dwf = g_opt_att_pipe && !att_mask_at(a, 0, 0);   // d w_full accumulated per batch row by the attention backward
+  const bool pipe_dwf = g_opt_att_pipe && !att_mask_at(a, 0);   // d w_full accumulated per batch row by the attention backward
   if (!g_opt_det) {
     dim3 grid(d.A / 64, cdiv(d.R, 32), d.B);
     if (g_opt_att_pipe) {

@@ -351,9 +351,6 @@ int lo_set_option(const char* name, int value) {
     if (e != cudaSuccess) return lo::fail(LO_ECUDA, "lo_set_option(l2_persist_mb): %s (%ld)", cudaGetErrorString(e), (long)e);
   }
   *v = value;
-  // the 8-stage skinny wgmma config takes 198 KB of shared memory, a whole SM: with two decoder chains (dec_streams >= 2) it
-  // would keep the other chain's kernels off the SMs it runs on
-  if (v == &lo::g_opt_dec_streams) lo::g_opt_skinny8 = value >= 2 ? 0 : 1;
   return LO_OK;
 }
 

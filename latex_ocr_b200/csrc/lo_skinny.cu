@@ -174,126 +174,6 @@ __global__ void __launch_bounds__(128) skinny_mma_kernel(const bf16* __restrict_
   }
 }
 
-// The same GEMM over the gate-interleaved context half of weight_ih (row 4*u + gate, lo_decoder.cu:interleave_wih_kernel) with the
-// LSTM cell (nn.LSTMCell, gates i,f,g,o: seq2seq_torch.py:313) in the epilogue: a CTA's 16 columns are 4 whole hidden units, lane
-// pairs (t, t^1) hold (i,f) and (g,o) of one unit for rows g and g+8 and swap halves with one shuffle, so every thread finalises
-// one (row, unit).  The table row, the recurrent projection and c_{t-1} are fetched BEFORE the MMA loop (they do not depend on
-// it), which a separate GEMM epilogue could not hide.  K <= 512 (one slice).  Replaces gemm + lstm_pw_fwd_kernel.
-__global__ void __launch_bounds__(128) skinny_lstm_kernel(const bf16* __restrict__ A, int64_t lda, const bf16* __restrict__ Wil, int64_t ldw,
-                                                           int M, int K, TcLstmEpi e) {
-  extern __shared__ __align__(16) uint8_t sk_smem[];
-  bf16* sA = reinterpret_cast<bf16*>(sk_smem);
-  bf16* sW = sA + 64 * SK_PITCH;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sk_smem + SK_SMEM);      // [0] weights, [1] activations
-  const int n0 = blockIdx.x * SK_NT;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int cpr = K / 8;
-  const uint32_t row_bytes = (uint32_t)K * 2u;
-  if (tid == 0) {
-    mbar_init(bars, 1);
-    mbar_init(bars + 1, 1);
-    fence_barrier_init();
-  }
-  __syncthreads();
-  if (warp == 0) {                         // weights: a parameter, bulk copies issued before griddepcontrol.wait
-    const uint64_t pol = l2_policy_evict_last();
-    if (lane == 0) mbar_expect_tx(bars, (uint32_t)SK_NT * row_bytes);
-    __syncwarp();
-    if (lane < SK_NT) bulk_g2s(sW + lane * SK_PITCH, Wil + (int64_t)(n0 + lane) * ldw, row_bytes, bars, pol);
-  }
-  for (int i = tid; i < (64 - M) * cpr; i += 128)
-    *reinterpret_cast<uint4*>(sA + (M + i / cpr) * SK_PITCH + (i % cpr) * 8) = make_uint4(0, 0, 0, 0);
-  // epilogue operands of this thread's (row, unit) pairs.  The token's table row, the recurrent projection of THIS step (written by the
-  // projection kernel two launches back: the attention kernel in between has waited for it) and c_t are all older than the preceding
-  // launch: fetched before griddepcontrol.wait, so the two dependent round trips (token, then its table row) leave the critical path
-  const int D = e.D;
-  const int g = lane >> 2, t = lane & 3;
-  const bool even = (t & 1) == 0;
-  const int row = warp * 16 + g + (even ? 0 : 8);
-  const bool live = row < M;
-  float add[2][4], cprev[2];
-#pragma unroll
-  for (int j = 0; j < 2; j++) {
-    cprev[j] = 0.f;
-#pragma unroll
-    for (int q = 0; q < 4; q++) add[j][q] = 0.f;
-  }
-  if (live) {
-    int64_t tk = e.tok[(int64_t)row * e.tok_stride];
-    if (tk < 0) tk = 0;
-    if (tk >= e.V) tk = e.V - 1;
-    const float* pt = e.ptab + tk * 4 * D;
-    const float* hh = e.hh + (int64_t)row * e.hh_stride;
-#pragma unroll
-    for (int j = 0; j < 2; j++) {
-      const int u = n0 / 4 + 2 * j + (t >> 1);
-      cprev[j] = e.c_prev[(int64_t)row * D + u];
-#pragma unroll
-      for (int q = 0; q < 4; q++) add[j][q] = pt[q * D + u] + hh[q * D + u];
-    }
-  }
-  pdl_wait();
-  pdl_trigger();
-  if (warp == 0) {
-    const uint64_t pol = l2_policy_evict_first();
-    if (lane == 0) mbar_expect_tx(bars + 1, (uint32_t)M * row_bytes);
-    __syncwarp();
-    for (int r = lane; r < M; r += 32) bulk_g2s(sA + r * SK_PITCH, A + (int64_t)r * lda, row_bytes, bars + 1, pol);
-  }
-  mbar_wait(bars, 0);
-  mbar_wait(bars + 1, 0);
-  __syncthreads();                         // the zero-filled rows
-  float acc[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
-  const bf16* a_ptr = sA + (warp * 16 + (lane & 7) + ((lane >> 3) & 1) * 8) * SK_PITCH + (lane >> 4) * 8;
-  const bf16* b_ptr = sW + ((lane & 7) + (lane >> 4) * 8) * SK_PITCH + ((lane >> 3) & 1) * 8;
-#pragma unroll 4
-  for (int k = 0; k < K; k += 16) {
-    uint32_t a0, a1, a2, a3, b0, b1, b2, b3;
-    ldmatrix_x4(a0, a1, a2, a3, a_ptr + k);
-    ldmatrix_x4(b0, b1, b2, b3, b_ptr + k);
-    mma_bf16_16816(acc[0], a0, a1, a2, a3, b0, b1);
-    mma_bf16_16816(acc[1], a0, a1, a2, a3, b2, b3);
-  }
-#pragma unroll
-  for (int j = 0; j < 2; j++) {
-    // even lanes hold (i,f), odd lanes (g,o) of unit u for rows g (acc[.][0..1]) and g+8 (acc[.][2..3])
-    const float sx = even ? acc[j][2] : acc[j][0], sy = even ? acc[j][3] : acc[j][1];
-    const float rx = __shfl_xor_sync(0xffffffffu, sx, 1), ry = __shfl_xor_sync(0xffffffffu, sy, 1);
-    if (!live) continue;
-    const float pi = (even ? acc[j][0] : rx) + add[j][0];
-    const float pf = (even ? acc[j][1] : ry) + add[j][1];
-    const float pg = (even ? rx : acc[j][2]) + add[j][2];
-    const float po = (even ? ry : acc[j][3]) + add[j][3];
-    const int u = n0 / 4 + 2 * j + (t >> 1);
-    const float ig = sigmoidf_(pi), fg = sigmoidf_(pf), gg = tanhf(pg), og = sigmoidf_(po);
-    const float c = fg * cprev[j] + ig * gg;
-    const float h = og * tanhf(c);
-    float* gt = e.gates + (int64_t)row * 4 * D;
-    gt[u] = ig; gt[D + u] = fg; gt[2 * D + u] = gg; gt[3 * D + u] = og;
-    e.c_out[(int64_t)row * D + u] = c;
-    e.h_out[(int64_t)row * D + u] = h;
-    if (e.h_bf) e.h_bf[(int64_t)row * D + u] = __float2bfloat16_rn(h);
-    if (e.hd) {
-      float mult = 1.f;
-      if (e.dmask) mult = e.dmask[(int64_t)row * e.hd_stride + u];
-      else if (e.dstate) mult = philox_dropout_mult(e.dstate, e.row0 + row, e.t_idx, u, e.dp, 1.f / (1.f - e.dp));
-      e.hd[(int64_t)row * e.hd_stride + u] = h * mult;
-    }
-  }
-}
-
-int skinny_gemm_nt_lstm(const bf16* A, int64_t lda, const bf16* Wil, int64_t ldw, int M, int D, int K, const TcLstmEpi& e, cudaStream_t st) {
-  LO_CHECK_ARG(M >= 1 && M <= 64 && K % 16 == 0 && K <= SK_KC && lda % 8 == 0 && ldw % 8 == 0 && D % 4 == 0, "M<=64, K%16, K<=512");
-  static bool attr = false;
-  if (!attr) {
-    LO_CUDA(cudaFuncSetAttribute(skinny_lstm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SK_SMEM + 16));
-    attr = true;
-  }
-  LO_CUDA(launch_pdl(skinny_lstm_kernel, dim3(4 * D / SK_NT), dim3(128), (size_t)SK_SMEM + 16, st, A, lda, Wil, ldw, M, K, e));
-  LO_LAUNCH_OK();
-  return LO_OK;
-}
-
 // atomic_acc: the product is added onto C (C holds the base values).  splits > 1: the K slices add their partial sums onto C with
 // fp32 atomics, or — option "deterministic" — groups of up to 8 slices run as one thread-block cluster each, summed in slice order
 // and added onto C group after group in stream order (run-to-run identical results)

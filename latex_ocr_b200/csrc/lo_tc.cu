@@ -110,16 +110,6 @@ struct TcParams {
   int w_evict_last;           // keep the B (weight) tiles in L2: the per-step decoder GEMMs re-read them every step
   int half_w, half_h;         // MC=1 conv: box offset of the second half of the A tile (one of them is 0)
   long long* dbg;             // optional: clock64 stamps of CTA (0,0,0) at the pipeline milestones (lo_debug_buffer)
-  // fused LSTM-cell epilogue (decoder forward): the GEMM's N dimension is gate-interleaved (column 4*j + gate), the
-  // epilogue adds the embedding-table row and the recurrent projection, applies the cell and writes h, c, gates
-  int lstm;
-  const float* l_ptab; const int64_t* l_tok; int64_t l_tok_stride;
-  const float* l_hh; int64_t l_hh_stride;
-  const float* l_cprev; float* l_gates; float* l_c; float* l_h; bf16* l_hbf;
-  float* l_hd; int64_t l_hd_stride; const float* l_dmask;
-  int l_D, l_V;
-  // in-kernel dropout (has_dropout = 2, no l_dmask): Philox {seed, call}, drop probability, first batch row of the launch, step
-  const unsigned long long* l_dstate; float l_dp; int l_row0, l_t;
 };
 
 constexpr int TC_BM = 128, TC_BK = 64;
@@ -293,66 +283,26 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_gemm_conv_kernel(const __gri
     // ===== epilogue from the accumulators (layout: lo_wgmma.cuh) =====
     const int rbase = wg * 64 + (warp & 3) * 16 + (lane >> 2);
     const int cq = 2 * (lane & 3);
-    if (p.lstm) {
-      // ---- fused LSTM cell (nn.LSTMCell, gate order i,f,g,o).  Columns 4u..4u+3 hold the gates of hidden unit u: the even
-      // lane of a pair holds (i, f), the odd one (g, o)
-      const int D = p.l_D;
+    const bool use_mask = p.mask && !p.out_f32 && !p.atomic;
 #pragma unroll
-      for (int h = 0; h < 2; h++) {
-        const int b = m0 + rbase + 8 * h;
-#pragma unroll
-        for (int i = 0; i < NT / 8; i++) {
-          const float a0 = acc[4 * i + 2 * h], a1 = acc[4 * i + 2 * h + 1];
-          const float o0 = __shfl_xor_sync(0xffffffffu, a0, 1), o1 = __shfl_xor_sync(0xffffffffu, a1, 1);
-          const int j = (n0 + 8 * i + cq) / 4;
-          if ((lane & 1) || b >= p.M || j >= D) continue;
-          int64_t tk = p.l_tok[(int64_t)b * p.l_tok_stride];
-          tk = tk < 0 ? 0 : (tk >= p.l_V ? p.l_V - 1 : tk);
-          const float* pt = p.l_ptab + tk * 4 * D;
-          const float* hh = p.l_hh + (int64_t)b * p.l_hh_stride;
-          const float pi = a0 + pt[j] + hh[j];
-          const float pf = a1 + pt[D + j] + hh[D + j];
-          const float pg = o0 + pt[2 * D + j] + hh[2 * D + j];
-          const float po = o1 + pt[3 * D + j] + hh[3 * D + j];
-          const float ig = sigmoidf_(pi), fg = sigmoidf_(pf), gg = tanhf(pg), og = sigmoidf_(po);
-          const float cn = fg * p.l_cprev[(int64_t)b * D + j] + ig * gg;
-          const float hn = og * tanhf(cn);
-          float* gt = p.l_gates + (int64_t)b * 4 * D;
-          gt[j] = ig; gt[D + j] = fg; gt[2 * D + j] = gg; gt[3 * D + j] = og;
-          p.l_c[(int64_t)b * D + j] = cn;
-          p.l_h[(int64_t)b * D + j] = hn;
-          if (p.l_hbf) p.l_hbf[(int64_t)b * D + j] = __float2bfloat16_rn(hn);
-          if (p.l_hd) {
-            // the multiplier lstm_pw_fwd_body and skinny_lstm_kernel apply, and lstm_pw_bwd_kernel redraws
-            float mult = 1.f;
-            if (p.l_dmask) mult = p.l_dmask[(int64_t)b * p.l_hd_stride + j];
-            else if (p.l_dstate) mult = philox_dropout_mult(p.l_dstate, p.l_row0 + b, p.l_t, j, p.l_dp, 1.f / (1.f - p.l_dp));
-            p.l_hd[(int64_t)b * p.l_hd_stride + j] = hn * mult;
-          }
-        }
+    for (int h = 0; h < 2; h++) {
+      const int row = rbase + 8 * h;
+      bool row_ok;
+      int64_t row_off;
+      if (p.conv) {
+        const int hh = h0 + row / p.BW, ww = w0 + row % p.BW;
+        row_ok = (hh < p.Ho) && (ww < p.Wo);
+        row_off = (((int64_t)img * p.Ho + hh) * p.Wo + ww) * p.ldc;
+      } else {
+        row_ok = (m0 + row) < p.M;
+        row_off = (int64_t)(m0 + row) * p.ldc;
       }
-    } else {
-      const bool use_mask = p.mask && !p.out_f32 && !p.atomic;
+      if (!row_ok) continue;
 #pragma unroll
-      for (int h = 0; h < 2; h++) {
-        const int row = rbase + 8 * h;
-        bool row_ok;
-        int64_t row_off;
-        if (p.conv) {
-          const int hh = h0 + row / p.BW, ww = w0 + row % p.BW;
-          row_ok = (hh < p.Ho) && (ww < p.Wo);
-          row_off = (((int64_t)img * p.Ho + hh) * p.Wo + ww) * p.ldc;
-        } else {
-          row_ok = (m0 + row) < p.M;
-          row_off = (int64_t)(m0 + row) * p.ldc;
-        }
-        if (!row_ok) continue;
-#pragma unroll
-        for (int i = 0; i < NT / 8; i++) {
-          if (n0 + 8 * i >= p.N) continue;       // 8-column groups: columns up to roundup8(N) are written (ldc allows it)
-          const int c = 8 * i + cq;
-          tc_store_pair(p, row_off + n0 + c, acc[4 * i + 2 * h] + s_bias[c], acc[4 * i + 2 * h + 1] + s_bias[c + 1], use_mask);
-        }
+      for (int i = 0; i < NT / 8; i++) {
+        if (n0 + 8 * i >= p.N) continue;       // 8-column groups: columns up to roundup8(N) are written (ldc allows it)
+        const int c = 8 * i + cq;
+        tc_store_pair(p, row_off + n0 + c, acc[4 * i + 2 * h] + s_bias[c], acc[4 * i + 2 * h + 1] + s_bias[c + 1], use_mask);
       }
     }
     if (dbg && threadIdx.x == 0) p.dbg[6] = clock64();
@@ -799,9 +749,6 @@ static int launch_tc_any(const CUtensorMap& mA, const CUtensorMap& mB, TcParams&
   return launch_tc<128, 3, 0>(mA, mB, p, mtiles, splits, st);
 }
 
-static TcLstmEpi g_lstm_epi;
-static bool g_lstm_epi_on = false;
-
 // splits > 1 (or atomic_acc): fp32 C only, partial sums are ADDED onto C with atomics (C must hold the base values)
 int tc_gemm_nt_ex(const bf16* A, int64_t lda, const bf16* W, int64_t ldw, void* C, int dtC, int64_t ldc, int M, int N, int K,
                   const float* bias, int accumulate, int relu, int splits, int atomic_acc, int small_n_tile, cudaStream_t st) {
@@ -830,24 +777,7 @@ int tc_gemm_nt_ex(const bf16* A, int64_t lda, const bf16* W, int64_t ldw, void* 
   p.out_f32 = (dtC == LO_F32); p.accumulate = accumulate; p.relu = relu; p.atomic = atomic_acc;
   p.w_evict_last = (M <= 128) ? 1 : 0;
   p.dbg = g_tc_dbg;
-  if (g_lstm_epi_on) {
-    const TcLstmEpi& e = g_lstm_epi;
-    p.lstm = 1;
-    p.l_ptab = e.ptab; p.l_tok = e.tok; p.l_tok_stride = e.tok_stride; p.l_hh = e.hh; p.l_hh_stride = e.hh_stride;
-    p.l_cprev = e.c_prev; p.l_gates = e.gates; p.l_c = e.c_out; p.l_h = e.h_out; p.l_hbf = e.h_bf;
-    p.l_hd = e.hd; p.l_hd_stride = e.hd_stride; p.l_dmask = e.dmask; p.l_D = e.D; p.l_V = e.V;
-    p.l_dstate = e.dstate; p.l_dp = e.dp; p.l_row0 = e.row0; p.l_t = e.t_idx;
-  }
   return launch_tc_any(mA, mB, p, cdiv(M, TC_BM), splits, NT, st, mc);
-}
-
-// gates = A @ Wil^T (Wil gate-interleaved [4D][K]) followed by the LSTM cell in the epilogue (see TcParams)
-int tc_gemm_nt_lstm(const bf16* A, int64_t lda, const bf16* Wil, int64_t ldw, int M, int D, int K, const TcLstmEpi& e, cudaStream_t st) {
-  g_lstm_epi = e;
-  g_lstm_epi_on = true;
-  const int r = tc_gemm_nt_ex(A, lda, Wil, ldw, e.gates /*unused as C*/, LO_F32, 4 * D, M, 4 * D, K, nullptr, 0, 0, 1, 0, 1, st);
-  g_lstm_epi_on = false;
-  return r;
 }
 
 int tc_gemm_nt(const bf16* A, int64_t lda, const bf16* W, int64_t ldw, void* C, int dtC, int64_t ldc, int M, int N, int K,

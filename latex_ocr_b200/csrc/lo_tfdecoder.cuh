@@ -468,7 +468,7 @@ static int tf_step(const lo_tfdec_args* a, const TfDims& d, const TfWs& w, int t
     LO_TRY(tf_nt(a, xh_n + d.O, xhb_n ? xhb_n + d.O : nullptr, d.XH, a->w_cat2, d.D, out2, d.N2, d.B, d.N2, d.D, nullptr, 0, st));
   {
     AttFwdArgs x{w.att_img, a->enc, out2, d.N2, a->beta, a->alphas + (int64_t)t * d.R, (int64_t)d.T * d.R, w.ctx + rowt * d.C, nullptr,
-                 0, nullptr, w.ctx_bf ? w.ctx_bf + rowt * d.C : nullptr, d.B, d.R, w.attwork, d.rpi, 0, 1, d.A};
+                 0, nullptr, w.ctx_bf ? w.ctx_bf + rowt * d.C : nullptr, d.B, d.R, w.attwork, d.rpi, 1, d.A};
     if (rg)
       LO_TRY(attention_fwd_ragged(x, *rg, a->dt, d.C, st));
     else
@@ -635,7 +635,7 @@ int lo_tfdec_backward(const lo_tfdec_args* a, void* stream) {
       AttBwdArgs x{w.att_img, a->enc, w.out2 + rowt * d.N2, nullptr, d.N2, a->beta, a->alphas + (int64_t)t * d.R, (int64_t)d.T * d.R,
                    w.ctx + rowt * d.C, w.dhc + d.D, d.D + d.C, dal ? dal + (int64_t)t * d.R : nullptr, dal ? (int64_t)d.T * d.R : 0,
                    dal ? w.sreg + t : nullptr, dal ? d.T : 0, w.de + (int64_t)t * d.R, dout2, nullptr, d.DW,
-                   dout2b, nullptr, w.dctx + rowt * d.C, d.B, d.R, w.attwork, w.dbeta_acc, 0, 1, d.A};
+                   dout2b, nullptr, w.dctx + rowt * d.C, d.B, d.R, w.attwork, w.dbeta_acc, 1, d.A};
       LO_TRY(attention_bwd_pipe(x, dt, d.C, st));
     }
     // d h_t += d att_h W_h^T

@@ -65,8 +65,8 @@ _P = 0.5
 
 # name: (precision, impl, B, R, T, decode lengths, A = C, dropout, D)  dropout: "philox" or "mask" (injected multipliers).
 # b72: steps 0 and 1 run 72 rows (the per-step GEMMs on wgmma, split-K atomics in the backward), steps 2 and 3 60 and 40 (mma.sync).
-# b40: under dec_streams=2, two chains of 20 rows that shrink differently.  c1024: the skinny LSTM kernel takes K <= 512 only, so
-# fuse_lstm runs the wgmma LSTM epilogue.  d640: the h projection has K = 640 > 512, two K slices of the mma.sync kernel with a bias.
+# b40: 40 rows that shrink at every step, to 33, 25 and 12 (ragged).  c1024: A = C = 1024, the widest attention and a 1024-wide K
+# for the gates GEMM.  d640: the h projection has K = 640 > 512, two K slices of the mma.sync kernel with a bias.
 _CASES = {
     "b8": ("bf16", "tc", 8, 44, 7, [7, 7, 6, 5, 5, 3, 2, 1], 512, "philox", 512),
     "b64": ("bf16", "tc", 64, 868, 4, [4] * 64, 512, "philox", 512),
@@ -79,14 +79,12 @@ _CASES = {
     "b8simt": ("bf16", "simt", 8, 44, 7, [7, 7, 6, 5, 5, 3, 2, 1], 512, "philox", 512),
 }
 
-# schedule -> (library options, the cases it runs).  skinny8 is set after dec_streams, which rewrites it.
+# schedule -> (library options, the cases it runs)
 _SCHEDULES = {
     "default": ({}, ["b8", "b64", "b72", "b72mask", "b40", "c1024", "d640", "b8fp32", "b8simt"]),
-    "fuse_lstm": ({"fuse_lstm": 1}, ["b8", "b64", "b72", "b72mask", "c1024"]),
     "skinny_mma0": ({"skinny_mma": 0}, ["b8", "b64", "c1024"]),
     "skinny_tma0": ({"skinny_tma": 0}, ["b8", "b64"]),
-    "skinny8_0": ({"dec_streams": 1, "skinny8": 0}, ["b72", "b8"]),
-    "dec_streams2": ({"dec_streams": 2}, ["b40", "b64"]),
+    "skinny8_0": ({"skinny8": 0}, ["b72", "b8"]),
     "deterministic": ({"deterministic": 1}, ["b8", "b72", "d640"]),
     "wgrad256": ({"wgrad256": 1}, ["b64", "b72"]),
     "att_pipe0": ({"att_pipe": 0}, ["b8", "b72"]),

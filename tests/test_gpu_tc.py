@@ -99,8 +99,8 @@ def test_tc_conv3x3_wgrad(N, H, W, Cin, Cout, pad):
     assert relerr(db, dy.double().sum(dim=(0, 2, 3)).float()) < 1e-5
 
 
-_SCHEDULE_OPTS = {"fuse_lstm": (0, 1), "dec_streams": (1, 2), "skinny_mma": (1, 0), "att_maskbits": (1, 0), "conv_persist": (1, 0),
-                  "wgrad256": (0, 1), "conv_mt2": (1, 0), "conv_mc": (1, 0), "att_bwd_mma": (1, 0), "skinny_tma": (1, 0)}
+_SCHEDULE_OPTS = {"skinny_mma": (1, 0), "att_maskbits": (1, 0), "conv_persist": (1, 0), "wgrad256": (0, 1), "conv_mt2": (1, 0),
+                  "conv_mc": (1, 0), "att_bwd_mma": (1, 0), "skinny_tma": (1, 0)}
 
 
 @pytest.mark.parametrize("opt", sorted(_SCHEDULE_OPTS))
@@ -114,7 +114,7 @@ def test_optional_decoder_schedules_match_default(opt):
     _L()
     V = 60
     pe, pd = rm.init_params(V, seed=41)
-    img, formula = rm.synthetic_batch(40, 32, 64, V, 4, 6, seed=42)     # B >= 32 so that the two-chain loop engages
+    img, formula = rm.synthetic_batch(40, 32, 64, V, 4, 6, seed=42)     # 40 rows: the per-step GEMMs (M <= 64) on mma.sync by default
     B, T = formula.shape[0], formula.shape[1] - 1
     res = {}
     for val in _SCHEDULE_OPTS[opt]:

@@ -1655,14 +1655,16 @@ static int bwd_launch_a(const AttBwdArgs& x, cudaStream_t st) {
     LO_LAUNCH_OK();
     return LO_OK;
   }
+  // the same rule for the d w_full (d att_beta) partials of the plain kernel
+  const int nsw = (x.ordered_dwf && x.dwf_part && !use_cluster(ns, x.R)) ? 1 : ns;
 #define LO_BWD_ARGS                                                                                                              \
   (const T*)x.att1, (const T*)x.enc, x.att2, x.gate, x.o1_stride, x.wf, x.alpha, x.alpha_stride, x.ctx, x.dgctx, x.dg_stride, x.dreg, \
-      x.dreg_stride, x.sreg, x.sreg_stride, x.de, x.datt2, x.dgp, x.dcat_stride, x.datt2_bf, x.dgp_bf, x.dctx_out, x.R, ns,       \
+      x.dreg_stride, x.sreg, x.sreg_stride, x.de, x.datt2, x.dgp, x.dcat_stride, x.datt2_bf, x.dgp_bf, x.dctx_out, x.R, nsw,      \
       (int*)x.work, (float*)((char*)x.work + att_partials_offset(x.B)), x.dwf_part, (T*)nullptr
-  if (use_cluster(ns, x.R)) {
-    LO_CUDA(launch_att(attention_bwd_pipe_kernel<T, NVA, NVC, true, ACT>, dim3(ns, x.B), (size_t)C::SMEM, ns, st, att_pdl_ok(x.abi), LO_BWD_ARGS));
+  if (use_cluster(nsw, x.R)) {
+    LO_CUDA(launch_att(attention_bwd_pipe_kernel<T, NVA, NVC, true, ACT>, dim3(nsw, x.B), (size_t)C::SMEM, nsw, st, att_pdl_ok(x.abi), LO_BWD_ARGS));
   } else {
-    LO_CUDA(launch_att(attention_bwd_pipe_kernel<T, NVA, NVC, false, ACT>, dim3(ns, x.B), (size_t)C::SMEM, 1, st, att_pdl_ok(x.abi), LO_BWD_ARGS));
+    LO_CUDA(launch_att(attention_bwd_pipe_kernel<T, NVA, NVC, false, ACT>, dim3(nsw, x.B), (size_t)C::SMEM, 1, st, att_pdl_ok(x.abi), LO_BWD_ARGS));
   }
 #undef LO_BWD_ARGS
   LO_LAUNCH_OK();

@@ -1368,6 +1368,7 @@ static int backward_step(const lo_decoder_args* a, const Dims& d, int t, int nro
     AttBwdArgs x{a->att1, a->enc, o1, o1 + d.A, d.O1, a->w_full, alpha_t, (int64_t)d.T * d.R, ctx_t, dxh, d.C + d.D, dal_t_ptr, dal_b,
                  sreg_t, d.T, de_t, dcat_t, dcat_t + d.A, d.O1, dcat_bf_t, dcat_bf_t ? dcat_bf_t + d.A : nullptr, dctx_t, nrows, d.R,
                  a->work, a->dmean, 0, 0, att_mask_at(a, t)};
+    x.ordered_dwf = g_opt_det;
     LO_TRY(attention_bwd_pipe(x, dt, d.C, st));
   } else {
     const int ns = att_splits(d.B);

@@ -255,6 +255,60 @@ __global__ void tf_dptab_scatter_kernel(const float* __restrict__ dz, const int6
   }
 }
 
+// The same sum under option deterministic: d ptab[v][:] = sum of dz[t][b][:] over the (t, b) that consumed token v, added in
+// ascending (t, b) order, so the sum does not depend on scheduling.  One block per (table row, TF_DPT_COLS columns): 256 threads
+// scan the tokens of steps 1.. in time-major order with one ballot per 256 of them and add the dz rows of the hits.  It writes every
+// element.  Not the default: at the tools/tf_bench.py shape the train step took 24.2 ms with it against 23.8 ms with the scatter
+// (H100 80GB HBM3, 700 W power limit).
+#define TF_DPT_COLS 1024
+__global__ void __launch_bounds__(256) tf_dptab_kernel(const float* __restrict__ dz, const int64_t* __restrict__ formula,
+                                                       int64_t f_stride, float* __restrict__ dptab, int B, int Tn, int G, int V) {
+  constexpr int NC = TF_DPT_COLS / 256;
+  const int v = blockIdx.y;
+  const int j0 = blockIdx.x * TF_DPT_COLS + threadIdx.x;
+  __shared__ unsigned s_bits[8];
+  float acc[NC];
+#pragma unroll
+  for (int k = 0; k < NC; k++) acc[k] = 0.f;
+  if (v == V) {                                          // the start token: every row of step 0
+    for (int b = 0; b < B; b++)
+#pragma unroll
+      for (int k = 0; k < NC; k++)
+        if (j0 + k * 256 < G) acc[k] += dz[(int64_t)b * G + j0 + k * 256];
+  } else {
+    const int total = B * (Tn - 1);                        // idx = (t - 1) B + b, t >= 1
+    for (int base = 0; base < total; base += 256) {
+      const int idx = base + threadIdx.x;
+      bool hit = false;
+      if (idx < total) {
+        int64_t tk = formula[(int64_t)(idx % B) * f_stride + idx / B];
+        if (tk < 0) tk = 0;
+        if (tk >= V) tk = V - 1;
+        hit = tk == (int64_t)v;
+      }
+      const unsigned bal = __ballot_sync(0xffffffffu, hit);
+      if ((threadIdx.x & 31) == 0) s_bits[threadIdx.x >> 5] = bal;
+      __syncthreads();
+#pragma unroll
+      for (int w = 0; w < 8; w++) {
+        unsigned bits = s_bits[w];
+        while (bits) {                                     // ascending index order -> deterministic sum
+          const int k = __ffs(bits) - 1;
+          bits &= bits - 1;
+          const float* row = dz + ((int64_t)B + base + w * 32 + k) * G;      // row (t, b) of dz = B + idx
+#pragma unroll
+          for (int q = 0; q < NC; q++)
+            if (j0 + q * 256 < G) acc[q] += row[j0 + q * 256];
+        }
+      }
+      __syncthreads();
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < NC; k++)
+    if (j0 + k * 256 < G) dptab[(int64_t)v * G + j0 + k * 256] = acc[k];
+}
+
 // ------------------------------------------------------------------------------------------------ workspace
 struct TfDims {
   int B, T, R, C, A, D, O, E, V, XH, G, LW, N2, DW, Vl, rpi, nimg;
@@ -620,7 +674,6 @@ int lo_tfdec_backward(const lo_tfdec_args* a, void* stream) {
   LO_CUDA(cudaMemsetAsync(w.dxh, 0, (size_t)d.B * d.XH * 4, st));
   LO_CUDA(cudaMemsetAsync(w.dc, 0, (size_t)d.B * d.D * 4, st));
   LO_CUDA(cudaMemsetAsync(w.dbeta_acc, 0, (size_t)d.B * d.A * 4, st));
-  LO_CUDA(cudaMemsetAsync(w.dptab, 0, (size_t)(d.V + 1) * d.G * 4, st));
   for (int t = d.T - 1; t >= 0; t--) {
     const int64_t rowt = (int64_t)t * d.B, rown = (int64_t)(t + 1) * d.B;
     float* dout2 = w.dout2 + rowt * d.DW;
@@ -636,6 +689,7 @@ int lo_tfdec_backward(const lo_tfdec_args* a, void* stream) {
                    w.ctx + rowt * d.C, w.dhc + d.D, d.D + d.C, dal ? dal + (int64_t)t * d.R : nullptr, dal ? (int64_t)d.T * d.R : 0,
                    dal ? w.sreg + t : nullptr, dal ? d.T : 0, w.de + (int64_t)t * d.R, dout2, nullptr, d.DW,
                    dout2b, nullptr, w.dctx + rowt * d.C, d.B, d.R, w.attwork, w.dbeta_acc, 1, d.A};
+      x.ordered_dwf = g_opt_det;
       LO_TRY(attention_bwd_pipe(x, dt, d.C, st));
     }
     // d h_t += d att_h W_h^T
@@ -657,10 +711,18 @@ int lo_tfdec_backward(const lo_tfdec_args* a, void* stream) {
   const bf16* Obf = w.xh_bf ? w.xh_bf + (int64_t)d.B * d.XH : nullptr;
   // LSTM kernel, [o ; h] rows: dz^T xh[0..T-1]
   LO_TRY(tf_tn(a, w.dz, w.dz_bf, d.G, w.xh, w.xh_bf, d.XH, a->g_w_lstm + d.E, d.LW, d.G, d.XH, TB, st));
-  // embedding rows through the table: d ptab (scatter), then d emb = d ptab K[:E]^T..., d K[:E] = d ptab^T emb, d b = colsum
-  // (sampling: the tokens the forward fed, not the targets)
-  tf_dptab_scatter_kernel<<<LO_NUM_SMS * 8, 256, 0, st>>>(w.dz, a->ss_prob ? a->fed : a->formula,
-                                                          a->ss_prob ? (int64_t)d.T : a->formula_stride, w.dptab, d.B, d.T, d.G, d.V);
+  // embedding rows through the table: d ptab (scatter, or the fixed-order gather under option deterministic), then d emb =
+  // d ptab K[:E]^T..., d K[:E] = d ptab^T emb, d b = colsum (sampling: the tokens the forward fed, not the targets)
+  {
+    const int64_t* tok = a->ss_prob ? a->fed : a->formula;
+    const int64_t tok_stride = a->ss_prob ? (int64_t)d.T : a->formula_stride;
+    if (g_opt_det) {
+      tf_dptab_kernel<<<dim3(cdiv(d.G, TF_DPT_COLS), d.V + 1), 256, 0, st>>>(w.dz, tok, tok_stride, w.dptab, d.B, d.T, d.G, d.V);
+    } else {
+      LO_CUDA(cudaMemsetAsync(w.dptab, 0, (size_t)(d.V + 1) * d.G * 4, st));
+      tf_dptab_scatter_kernel<<<LO_NUM_SMS * 8, 256, 0, st>>>(w.dz, tok, tok_stride, w.dptab, d.B, d.T, d.G, d.V);
+    }
+  }
   LO_LAUNCH_OK();
   LO_TRY(gemm_nn(w.dptab, LO_F32, d.G, a->w_lstm, dt, d.LW, a->g_emb, LO_F32, d.E, d.V + 1, d.E, d.G, 0, LO_IMPL_SIMT, st));
   LO_TRY(gemm_tn(w.dptab, LO_F32, d.G, a->emb, dt, d.E, a->g_w_lstm, LO_F32, d.LW, d.G, d.E, d.V + 1, 0, LO_IMPL_SIMT, st));

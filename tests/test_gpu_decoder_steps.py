@@ -86,6 +86,7 @@ _SCHEDULES = {
     "skinny_tma0": ({"skinny_tma": 0}, ["b8", "b64"]),
     "skinny8_0": ({"skinny8": 0}, ["b72", "b8"]),
     "deterministic": ({"deterministic": 1}, ["b8", "b72", "d640"]),
+    "deterministic_maskbits0": ({"deterministic": 1, "att_maskbits": 0}, ["b8"]),
     "wgrad256": ({"wgrad256": 1}, ["b64", "b72"]),
     "att_pipe0": ({"att_pipe": 0}, ["b8", "b72"]),
     "att_maskbits0": ({"att_maskbits": 0}, ["b8", "b64"]),
@@ -445,7 +446,7 @@ def test_decoder_steps_vs_float64(schedule, case):
     dec, enc, caps, lengths, mask = _model(case, seed)
     with _lib.option(**opts):
         ws, mult = _run(dec, enc, caps, lengths, mask, seed)
-        first = _outputs(dec, ws) if schedule == "deterministic" else None
+        first = _outputs(dec, ws) if "deterministic" in opts else None
         ck = _Checker("%s %s" % (schedule, case))
         _check(ck, dec, ws, enc, caps, lengths, mult)
         if first is not None:

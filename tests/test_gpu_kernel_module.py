@@ -85,9 +85,11 @@ def _cases():
     feat_a, feat_b = _enc(2, 12, seed=8).view(2, 2, 6, 512), _enc(3, 5, seed=9).view(3, 1, 5, 512)
     enc_a, enc_b = _enc(4, 12, seed=10), _enc(3, 9, seed=11)
     (f_a, l_a), (f_b, l_b) = _captions(4, 8, seed=12), _captions(3, 5, seed=13)
-    # TF decoder: one row of distinct tokens, because its embedding-table gradient is scattered with fp32 atomics whose order
-    # option deterministic does not fix (two identical backwards differ in the last bits when a token row is hit twice)
-    tf_enc_a, tf_a = _enc(1, 12, seed=19), torch.randperm(V, generator=g)[:7].view(1, 7).cuda()
+    # TF decoder: rows that repeat tokens, so that rows of the embedding-table gradient sum several steps' gradients
+    tf_enc_a, tf_a = _enc(3, 12, seed=19), torch.randint(0, V, (3, 7), generator=g)
+    tf_a[1] = tf_a[0]
+    tf_a[2, 1:4] = tf_a[2, 0]
+    tf_a = tf_a.cuda()
     tf_b = torch.randint(0, V, (3, 5), generator=g).cuda()
 
     def weighted(out, seed):

@@ -610,6 +610,9 @@ int lo_tfdec_beam_div(const lo_tfdec_args* a, int64_t end_id, int max_steps, int
  * two bias vectors), forward over S steps for M independent sequences + hand-derived backward.  Used for the row-encoder biLSTM
  * over the CNN feature rows (two calls, `reverse` = 0 / 1, writing the two halves of the output channels) and for a second decoder
  * layer.  Element (t, m) of x / dx lives at m * row + t * step (+ channel); of hs / hs_st / dhs at m * hs_row + t * hs_step.
+ * x and dx are read and written 16 bytes at a time: x must be 16-byte aligned with x_row, x_step multiples of 8 elements, and a
+ * dx given to the backward 16-byte aligned with dx_row, dx_step multiples of 4; otherwise both calls return LO_EINVAL before any
+ * GPU work.
  */
 typedef struct lo_lstm_seq_args {
   int32_t S, M, I, H;      /* steps, sequences, input width, hidden width (I, H multiples of 8) */

@@ -159,6 +159,10 @@ static int seq_check(const lo_lstm_seq_args* a) {
   LO_CHECK_ARG(a->dt == LO_F32 || a->dt == LO_BF16, "dt");
   LO_CHECK_ARG(a->x && a->w_ih && a->w_hh && a->b_ih && a->b_hh && a->ws, "null pointer");
   LO_CHECK_ARG(a->x_row % 8 == 0 && a->x_step % 8 == 0, "x strides must be multiples of 8 elements");
+  // the gather reads x 8 elements at a time and the scatter writes dx as float4: both need 16-byte aligned rows
+  LO_CHECK_ARG(((uintptr_t)a->x & 15) == 0, "x must be 16-byte aligned");
+  LO_CHECK_ARG(!a->dx || ((uintptr_t)a->dx & 15) == 0, "dx must be 16-byte aligned");
+  LO_CHECK_ARG(!a->dx || (a->dx_row % 4 == 0 && a->dx_step % 4 == 0), "dx strides must be multiples of 4 elements");
   return LO_OK;
 }
 

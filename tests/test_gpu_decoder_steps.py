@@ -8,6 +8,14 @@ RN_bf16(dcat), RN_bf16(dlogits), RN_bf16(dptab), RN_bf16(alphas), RN_bf16(dctx) 
 the kernels see them (bf16 shadows in bf16, the fp32 master otherwise; biases and full_att.weight fp32).  So an error never
 compounds across steps: each check sees one launch's arithmetic.
 
+The two-layer decoder of the extension (cases b8l2, b72maskl2) runs the phases the way TwoLayerDecoder drives them, with
+snapshots between them: the phase-1 forward must leave the logits and row_loss holding the sentinel and write hd = hall x
+multiplier; DecoderLayer2 over hd is checked launch by launch with tests/test_gpu_lstmseq_steps.py's checks on its own
+workspace; the phase-2 forward's logits are fc(RN_bf16(h2)) and its cross entropy is checked as in phase 0; the phase-2 backward
+writes dhd = dlogits W_fc and the fc gradients and leaves every other gradient holding the sentinel; the phase-1 backward's
+time loop takes dh = (layer 2's d x, read from dhd) x multiplier + carried.  Checks and bounds are the ones of phase 0 (helpers
+shared through tests/step_check.py).
+
 Bounds (every check, element-wise; S = the float64 sum of the magnitudes of the terms of the exact value):
   * fp32 GEMM / reduction outputs (out1's att2 and hh blocks, ptab, logits, dhd, the dh and d gctx products, every hoisted
     weight gradient, d encoder_out):  |y - ref| <= 2^-16 S.  bf16 products are exact in fp32 (and fp32 x fp32 products are
@@ -40,7 +48,8 @@ past bt[t] must keep it (or hold the zeros the ragged path writes) and it must n
 zero d logits row is zero, so a NaN sentinel would be a false alarm.
 
 Worst |y - ref| / bound per quantity, over every case and schedule, measured on an H100 80GB HBM3 (700 W power limit); the
-whole file ran in 15 s there:
+whole file ran in 15 s there before the two-layer cases came (with them, this file, tests/test_gpu_lstmseq_steps.py and
+tests/test_gpu_ext.py ran in 20 s together):
     bf16 roundings (a value next to a rounding midpoint nears half an ulp): att1 0.983, d att1 0.996
     pointwise and cross entropy: c 0.467, h 0.351, d gates 0.343, dc0 0.325, dlogits 0.776, dreg 0.161, gates 0.067, gate 0.068,
         row loss 0.020, loss 0.006, n_valid 0.262
@@ -49,17 +58,20 @@ whole file ran in 15 s there:
         dh0 0.040, sreg 0.010, g_wcat1 0.038, g_bcat1 0.018, g_w_ih 0.030 / 0.027, g_b_ih 0.018, dptab 0.006, g_emb 0.041,
         g_w_fc 0.066, g_b_fc 0.023, g_w_full 0.031, g_w_enc_att 0.029, g_b_enc_att 0.004, g_w_init 0.023, g_b_init 0.012,
         d encoder_out 0.015
+    layer 2 of the two-layer cases: c 0.432, h 0.279, gates 0.070, dG 0.332, dc 0.304, dh 0.037, dxt 0.037, g_w_hh 0.015,
+        g_w_ih 0.021, g_b 0.013
 """
+from types import SimpleNamespace
+
 import pytest
 import torch
 
 import decoder_step_ref as ds
+import lstmseq_step_ref as lr
+from step_check import ACC, SENTINEL, ULPS, Checker, cell_backward_bounds, check_cell, check_gates, half_ulp_bf16, rn
 
 pytestmark = pytest.mark.gpu
 
-_SENTINEL = -1536.0                 # exact in bf16 and fp32, never produced by the data here
-_ACC = 2.0 ** -16
-_ULPS = 2.0 ** -21                  # a few fp32 ulps of a value <= 1
 _V, _E = 500, 512
 _P = 0.5
 
@@ -79,82 +91,42 @@ _CASES = {
     "b8simt": ("bf16", "simt", 8, 44, 7, [7, 7, 6, 5, 5, 3, 2, 1], 512, "philox", 512),
 }
 
+# the two-layer decoder of the extension (latex_ocr_b200/ext.py TwoLayerDecoder) on the data of a case above: phase-1 time loop,
+# DecoderLayer2 over hd, phase-2 head and loss; backward phase 2, layer 2, phase 1
+_TWO_LAYER = {"b8l2": "b8", "b72maskl2": "b72mask"}
+
 # schedule -> (library options, the cases it runs)
 _SCHEDULES = {
-    "default": ({}, ["b8", "b64", "b72", "b72mask", "b40", "c1024", "d640", "b8fp32", "b8simt"]),
+    "default": ({}, ["b8", "b64", "b72", "b72mask", "b40", "c1024", "d640", "b8fp32", "b8simt", "b8l2", "b72maskl2"]),
     "skinny_mma0": ({"skinny_mma": 0}, ["b8", "b64", "c1024"]),
     "skinny_tma0": ({"skinny_tma": 0}, ["b8", "b64"]),
     "skinny8_0": ({"skinny8": 0}, ["b72", "b8"]),
-    "deterministic": ({"deterministic": 1}, ["b8", "b72", "d640"]),
+    "deterministic": ({"deterministic": 1}, ["b8", "b72", "d640", "b8l2", "b72maskl2"]),
     "deterministic_maskbits0": ({"deterministic": 1, "att_maskbits": 0}, ["b8"]),
     "wgrad256": ({"wgrad256": 1}, ["b64", "b72"]),
     "att_pipe0": ({"att_pipe": 0}, ["b8", "b72"]),
     "att_maskbits0": ({"att_maskbits": 0}, ["b8", "b64"]),
     "att_bwd_mma0": ({"att_bwd_mma": 0}, ["b8", "b64"]),
-    "pdl0": ({"pdl": 0}, ["b8", "b72"]),
+    "pdl0": ({"pdl": 0}, ["b8", "b72", "b8l2", "b72maskl2"]),
 }
 _PARAMS = [(s, c) for s, (_, cs) in _SCHEDULES.items() for c in cs]
 
 _WORST = {}
 
 
-def _rn(x):
-    return x.bfloat16().double()
-
-
-def _half_ulp_bf16(ref):
-    _, e = torch.frexp(ref)
-    return torch.where(ref != 0, torch.ldexp(torch.full_like(ref, 0.5), e - 8), torch.zeros_like(ref))
-
-
-def _bits(t):
-    t = t.contiguous()
-    return t.view(torch.int16) if t.dtype == torch.bfloat16 else t.view(torch.int32)
-
-
-class _Checker:
-    def __init__(self, tag):
-        self.tag = tag
-        self.worst = {}
-
-    def bound(self, name, y, ref, bound):
-        """|y - ref| <= bound element-wise (NaN fails); records the worst ratio."""
-        d = (y.double() - ref).abs()
-        bound = torch.broadcast_to(torch.as_tensor(bound, dtype=torch.float64, device=d.device), d.shape)
-        ok = d <= bound
-        if not bool(ok.all()):
-            bad = (~ok).nonzero()
-            i = tuple(bad[0].tolist())
-            raise AssertionError("%s %s: %d of %d elements outside the bound; first at %s: got %r, float64 %r, bound %.3g"
-                                 % (self.tag, name, bad.shape[0], y.numel(), i, y[i].item(), ref[i].item(), bound[i].item()))
-        r = torch.where(bound > 0, d / bound.clamp_min(1e-300), torch.zeros_like(d)).max().item() if d.numel() else 0.0
-        self.worst[name] = max(self.worst.get(name, 0.0), r)
-
-    def gemm(self, name, y, ref, S):
-        self.bound(name, y, ref, _ACC * S)
-
-    def attn(self, name, y, ref):
-        """The attention kernels' rule: 1e-5 of max |ref| plus 2e-8."""
-        self.bound(name, y, ref, torch.full_like(ref, 1e-5 * ref.abs().max().item() + 2e-8))
-
-    def exact(self, name, y, ref):
-        assert torch.equal(_bits(y), _bits(ref.to(y.dtype))), "%s %s: not bit for bit" % (self.tag, name)
-
-    def value(self, name, y, v):
-        assert bool((y == v).all()), "%s %s: expected every element to be %r" % (self.tag, name, v)
-
-
 def _lin(x, w, b=None):
     return ds.linear(x, w, b)
 
 
-def _model(case, seed):
+def _model(case, seed, two_layer=False):
     from latex_ocr_b200.decoder import DecoderWithAttention
+    from latex_ocr_b200.ext import DecoderLayer2
     precision, impl, B, R, T, lengths, C, dropout, D = _CASES[case]
     torch.manual_seed(seed)
     dec = DecoderWithAttention(C, _E, D, _V, encoder_dim=C, dropout=_P, device="cuda", precision=precision, impl=impl)
     with torch.no_grad():
         dec.fc.bias.uniform_(-0.1, 0.1)           # init_weights zeroes it: give the bias path something to add
+    layer2 = DecoderLayer2(D, device="cuda", precision=precision, impl=impl) if two_layer else None
     g = torch.Generator(device="cuda").manual_seed(seed + 1)
     enc = torch.randn(B, R, C, device="cuda", generator=g).to(dec.tdtype)
     caps = torch.randint(0, _V, (B, T + 1), device="cuda", generator=g)
@@ -163,15 +135,28 @@ def _model(case, seed):
         mask = (torch.rand(B, T, D, device="cuda", generator=g) >= _P).float() / (1 - _P)
     elif dropout == "philox":
         mask = "philox"
-    return dec, enc, caps, lengths, mask
+    return dec, enc, caps, lengths, mask, layer2
+
+
+def _layer2_dir(layer2, B, T):
+    """Layer 2's direction as tests/test_gpu_lstmseq_steps.py's checks take it: its workspace views, weights and gradients."""
+    st, n, D = layer2.store, layer2.dir.names, layer2.D
+    bf = layer2.precision == "bf16"
+    ent = layer2.dir.entry(T, B)
+    return SimpleNamespace(v=lr.views(ent["ws"], T, B, D, D, bf), ws=ent["ws"], S=T, M=B, I=D, H=D, reverse=False, bf=bf,
+                           dt=torch.bfloat16 if bf else torch.float32, w_ih=st.w(n["weight_ih"]), w_hh=st.w(n["weight_hh"]),
+                           b_ih=st.f32(n["bias_ih"]), b_hh=st.f32(n["bias_hh"]), h0=None, c0=None, dh0=None, dc0=None,
+                           grads={k: st.g(n[w]) for k, w in (("g_w_ih", "weight_ih"), ("g_w_hh", "weight_hh"),
+                                                             ("g_b_ih", "bias_ih"), ("g_b_hh", "bias_hh"))})
 
 
 _FILLED = ("out1", "hall", "call", "gates", "ctx", "gctx", "gtmp", "alphas", "hd", "row_loss", "loss", "sreg", "dlogits", "dhd",
            "dreg", "dcat", "dxh", "dc", "dctx", "de", "dptab", "datt1", "denc", "dinit", "dmean", "ptab", "mean", "att1", "bfwork")
 
 
-def _run(dec, enc, caps, lengths, mask, seed):
-    """One forward + backward from sentinel-filled buffers; returns (ws, multipliers [B][T][D] fp32)."""
+def _run(dec, enc, caps, lengths, mask, seed, layer2=None):
+    """One forward + backward from sentinel-filled buffers; returns (ws, multipliers [B][T][D] fp32, snapshots).  With
+    ``layer2`` the phases run the way TwoLayerDecoder drives them, and the snapshots hold what the buffers held between them."""
     from latex_ocr_b200 import philox
     B, R, _ = enc.shape
     T = max(lengths)
@@ -185,13 +170,29 @@ def _run(dec, enc, caps, lengths, mask, seed):
     t = ws["t"]
     for k in _FILLED:
         if k in t:
-            t[k].view(torch.bfloat16 if k == "bfwork" else t[k].dtype).fill_(_SENTINEL)
-    t["logits"][:, :, :_V].fill_(_SENTINEL)          # the padding columns keep the zeros they were allocated with
-    dec.store.grad.fill_(_SENTINEL)
+            t[k].view(torch.bfloat16 if k == "bfwork" else t[k].dtype).fill_(SENTINEL)
+    t["logits"][:, :, :_V].fill_(SENTINEL)          # the padding columns keep the zeros they were allocated with
+    dec.store.grad.fill_(SENTINEL)
+    if layer2 is not None:
+        l2 = _layer2_dir(layer2, B, T)
+        for v in l2.v.values():
+            v.fill_(SENTINEL)
+        layer2.store.grad.fill_(SENTINEL)
     dec.seed_dropout(1000 + seed, 7)
     state = dec.dropout_state.cpu().tolist()
-    ws = dec.run_forward(enc, caps, lengths, with_loss=True, need_grad=True, dropout_mask=mask)
-    dec.run_backward(ws)
+    snap = {}
+    if layer2 is None:
+        ws = dec.run_forward(enc, caps, lengths, with_loss=True, need_grad=True, dropout_mask=mask)
+        dec.run_backward(ws)
+    else:
+        ws = dec.run_forward(enc, caps, lengths, with_loss=True, need_grad=True, dropout_mask=mask, phase=1)
+        snap.update(hd1=t["hd"].clone(), logits1=t["logits"].clone(), row_loss1=t["row_loss"].clone())
+        snap["l2"] = layer2.forward_inplace(t["hd"])                # hd: dropout(h1) -> h2
+        dec.run_phase(ws, 2, backward=False)
+        dec.run_phase(ws, 2, backward=True)                          # dhd = d h2
+        snap.update(dhd2=t["dhd"].clone(), grad2=dec.store.grad.clone())
+        layer2.backward_inplace(t["dhd"], snap["l2"])                # dhd: d h2 -> d dropout(h1)
+        dec.run_phase(ws, 1, backward=True)
     torch.cuda.synchronize()
     if has_do == 2:
         mult = torch.from_numpy(philox.dropout_multipliers(state[0], state[1], B, T, D, _P)).cuda()
@@ -199,21 +200,22 @@ def _run(dec, enc, caps, lengths, mask, seed):
         mult = mask.float()
     else:
         mult = torch.ones(B, T, D, device="cuda")
-    return ws, mult
+    return ws, mult, snap
 
 
-def _check(ck, dec, ws, enc, caps, lengths, mult):
+def _check(ck, dec, ws, enc, caps, lengths, mult, snap=None, layer2=None):
     S = dec.store
     t_ = ws["t"]
+    hd1 = snap["hd1"] if layer2 is not None else t_["hd"]               # what the time loop wrote into hd
     B, R, C = enc.shape
     T = max(lengths)
     A, D, V, E = C, dec.decoder_dim, _V, _E
     O1, G = A + C + 4 * D, 4 * D
     ldl = ws["ldl"]
     tc = dec.impl == "tc" and dec.precision == "bf16"
-    act = _rn if tc else (lambda x: x.double())
-    fc_act = _rn if (tc and ldl % 64 == 0 and D % 64 == 0) else (lambda x: x.double())
-    pt_act = _rn if (tc and E % 64 == 0 and G % 64 == 0 and V >= 64) else (lambda x: x.double())
+    act = rn if tc else (lambda x: x.double())
+    fc_act = rn if (tc and ldl % 64 == 0 and D % 64 == 0) else (lambda x: x.double())
+    pt_act = rn if (tc and E % 64 == 0 and G % 64 == 0 and V >= 64) else (lambda x: x.double())
     names_w = ("attention.encoder_att.weight", "attention.decoder_att.weight", "f_beta.weight", "decode_step.weight_hh",
                "embedding.weight", "decode_step.weight_ih", "init_h.weight", "init_c.weight", "fc.weight")
     p = {n: S.w(n).double() for n in names_w}
@@ -231,7 +233,7 @@ def _check(ck, dec, ws, enc, caps, lengths, mult):
 
     # ---- hoisted forward: att1, ptab, the row means, h0, c0
     ref, Sa = _lin(encd, p["attention.encoder_att.weight"], p["attention.encoder_att.bias"])
-    ck.bound("att1", att1, ref, _ACC * Sa + (_half_ulp_bf16(ref) if att1.dtype == torch.bfloat16 else 0))
+    ck.bound("att1", att1, ref, ACC * Sa + (half_ulp_bf16(ref) if att1.dtype == torch.bfloat16 else 0))
     ref, Sp = _lin(p["embedding.weight"], p["decode_step.weight_ih"][:, :E], p["decode_step.bias_ih"])
     ck.gemm("ptab", t_["ptab"], ref, Sp)
     ck.bound("mean", t_["mean"], encd.mean(1), (R + 1) * 2.0 ** -24 * encd.abs().mean(1))
@@ -239,7 +241,7 @@ def _check(ck, dec, ws, enc, caps, lengths, mult):
     split = 2.0 ** -18 if (tc and C % 64 == 0 and T >= 2) else 0.0
     for k, n in ((t_["hall"][0], "init_h"), (t_["call"][0], "init_c")):
         ref, Si = _lin(mean, p[n + ".weight"], p[n + ".bias"])
-        ck.bound("h0 c0", k, ref, (_ACC + split) * Si)
+        ck.bound("h0 c0", k, ref, (ACC + split) * Si)
 
     # ---- the forward time loop, step by step from the kernel's own inputs
     ptab = t_["ptab"].double()
@@ -249,7 +251,7 @@ def _check(ck, dec, ws, enc, caps, lengths, mult):
         ref, S1 = _lin(act(t_["hall"][t][:n]), wc, bc)
         ck.gemm("out1 att2", out1[:n, :A], ref[:, :A], S1[:, :A])
         ck.gemm("out1 hh", out1[:n, A + C:], ref[:, A + C:], S1[:, A + C:])
-        ck.bound("out1 gate", out1[:n, A:A + C], torch.sigmoid(ref[:, A:A + C]), 0.25 * _ACC * S1[:, A:A + C] + _ULPS)
+        ck.bound("out1 gate", out1[:n, A:A + C], torch.sigmoid(ref[:, A:A + C]), 0.25 * ACC * S1[:, A:A + C] + ULPS)
         att2, gate, hh = out1[:n, :A].double(), out1[:n, A:A + C].double(), out1[:n, A + C:].double()
         _, alpha, ctx, _ = ds.attention(att1d[:n], encd[:n], att2, wf, gate)
         ck.attn("alphas", t_["alphas"][:n, t], alpha)
@@ -258,26 +260,37 @@ def _check(ck, dec, ws, enc, caps, lengths, mult):
         tok = caps[:n, t]
         pre_g, Sg = _lin(act(t_["gctx"][t][:n]), w_ctx)
         pre = pre_g + ptab[tok] + hh
-        e_pre = _ACC * (Sg + ptab[tok].abs() + hh.abs())
+        e_pre = ACC * (Sg + ptab[tok].abs() + hh.abs())
         gts = t_["gates"][t][:n]
-        for q, (fn, lip) in enumerate(((torch.sigmoid, 0.25), (torch.sigmoid, 0.25), (torch.tanh, 1.0), (torch.sigmoid, 0.25))):
-            sl = slice(q * D, (q + 1) * D)
-            ck.bound("gates", gts[:, sl], fn(pre[:, sl]), lip * e_pre[:, sl] + _ULPS)
+        check_gates(ck, gts, pre, e_pre)
         i, f, g, o = gts.double().chunk(4, 1)
-        cp = t_["call"][t][:n].double()
-        ck.bound("c", t_["call"][t + 1][:n], f * cp + i * g, 2.0 ** -22 * ((f * cp).abs() + (i * g).abs()) + 1e-38)
-        cn = t_["call"][t + 1][:n].double()
-        href = o * torch.tanh(cn)
-        ck.bound("h", t_["hall"][t + 1][:n], href, 2.0 ** -21 * href.abs() + 1e-38)
-        ck.exact("hd", t_["hd"][:n, t], t_["hall"][t + 1][:n] * mult[:n, t])
+        check_cell(ck, t_["call"][t + 1][:n], t_["hall"][t + 1][:n], i, f, g, o, t_["call"][t][:n].double())
+        ck.exact("hd", hd1[:n, t], t_["hall"][t + 1][:n] * mult[:n, t])
         # rows that stopped decoding: untouched, or the zeros of the ragged path
         for k, v in (("out1", t_["out1"][t][n:]), ("gates", t_["gates"][t][n:]), ("call", t_["call"][t + 1][n:]),
                      ("hall", t_["hall"][t + 1][n:]), ("ctx", t_["ctx"][t][n:]), ("gctx", t_["gctx"][t][n:])):
-            ck.value("inactive rows of %s[%d]" % (k, t), v, _SENTINEL)
+            ck.value("inactive rows of %s[%d]" % (k, t), v, SENTINEL)
         ck.value("alphas of inactive rows", t_["alphas"][n:, t], 0.0)
-        ck.value("hd of inactive rows", t_["hd"][n:, t], 0.0)
+        ck.value("hd of inactive rows", hd1[n:, t], 0.0)
 
-    # ---- head, loss
+    if layer2 is not None:
+        # phase 1 stops before the head; layer 2 over hd1 (its input in storage dtype) into hd, checked launch by launch
+        ck.value("logits after phase 1", snap["logits1"][:, :, :V], SENTINEL)
+        ck.value("row_loss after phase 1", snap["row_loss1"], SENTINEL)
+        from test_gpu_lstmseq_steps import check_backward, check_forward
+        ck2 = Checker(ck.tag + " layer 2")
+        l2 = _layer2_dir(layer2, B, T)
+        x2 = snap["l2"][0]["x"]
+        ck2.exact("x", x2, hd1)
+        check_forward(ck2, l2, x2, hs=t_["hd"], before_backward=False)
+        check_backward(ck2, l2, snap["dhd2"], t_["dhd"])                  # d x written over d h2, after the loop read it
+        ck.worst.update({"layer2 " + k: v for k, v in ck2.worst.items()})
+        # phase-2 backward: the fc gradients only
+        for n in S.offsets:
+            if not n.startswith("fc."):
+                ck.value("%s gradient after phase 2" % n, S.view(snap["grad2"], n), SENTINEL)
+
+    # ---- head, loss (phase 2 of the two-layer decoder: over h2)
     hd = t_["hd"]
     ref, Sl = _lin(fc_act(hd), p["fc.weight"], p["fc.bias"])
     ck.gemm("logits", t_["logits"][:, :, :V], ref, Sl)
@@ -305,9 +318,9 @@ def _check(ck, dec, ws, enc, caps, lengths, mult):
     e_S = (T + 1) * 2.0 ** -24 * (1 + Ssum)
     ck.bound("dreg", t_["dreg"], dreg, 2 * dec.alpha_c * e_S / (B * R) + 2.0 ** -22 * dreg.abs())
     ck.bound("loss", t_["loss"][1:2], (row.sum() * inv_n).reshape(1),
-             (inv_n * row_b.sum() + _ACC * inv_n * row.abs().sum()).reshape(1))
+             (inv_n * row_b.sum() + ACC * inv_n * row.abs().sum()).reshape(1))
     ck.bound("loss", t_["loss"][2:3], (sq / (B * R)).reshape(1),
-             ((2 * (1 - Ssum).abs() * e_S).sum() / (B * R) + _ACC * sq / (B * R)).reshape(1))
+             ((2 * (1 - Ssum).abs() * e_S).sum() / (B * R) + ACC * sq / (B * R)).reshape(1))
     ck.bound("loss n_valid", t_["loss"][3:4], torch.full((1,), float(nvalid), dtype=torch.float64, device="cuda"),
              2.0 ** -22 * nvalid)                          # 1 / (1 / n) in fp32: two roundings
     dregk = t_["dreg"].double()
@@ -317,8 +330,8 @@ def _check(ck, dec, ws, enc, caps, lengths, mult):
     # ---- backward: d hd, then the time loop in reverse from the kernel's own stored values
     dlk = t_["dlogits"][:, :, :V]
     ref, Sd = fc_act(dlk) @ p["fc.weight"], fc_act(dlk).abs() @ p["fc.weight"].abs()
-    ck.gemm("dhd", t_["dhd"], ref, Sd)
-    dhd = t_["dhd"].double()
+    ck.gemm("dhd", snap["dhd2"] if layer2 is not None else t_["dhd"], ref, Sd)
+    dhd = t_["dhd"].double()                         # the two-layer decoder: layer 2's d x, read by the phase-1 backward
     multd = mult.double()
     dc = torch.zeros(B, D, dtype=torch.float64, device="cuda")
     e_dc = torch.zeros_like(dc)
@@ -328,7 +341,7 @@ def _check(ck, dec, ws, enc, caps, lengths, mult):
         dcat = t_["dcat"][t][:n]
         if t + 1 < T:
             x = act(t_["dcat"][t + 1][:n])
-            dhn, e_dhn = x @ wc, _ACC * (x.abs() @ wc.abs())
+            dhn, e_dhn = x @ wc, ACC * (x.abs() @ wc.abs())
         else:
             dhn, e_dhn = torch.zeros(n, D, dtype=torch.float64, device="cuda"), 0.0
         dh = dhd[:n, t] * multd[:n, t] + dhn
@@ -337,21 +350,17 @@ def _check(ck, dec, ws, enc, caps, lengths, mult):
         th = torch.tanh(t_["call"][t + 1][:n].double())
         cp = t_["call"][t][:n].double()
         dG, dct, dcp = ds.cell_backward(dh, dc[:n], i, f, g, o, t_["call"][t + 1][:n].double(), cp)
-        e_dct = (e_dc[:n] + e_dh * (o * (1 - th * th)).abs() + (dh * o).abs() * (2 * th.abs() * 2.0 ** -22 * th.abs() + 2.0 ** -23)
-                 + 2.0 ** -22 * (dc[:n].abs() + (dh * o * (1 - th * th)).abs()))
-        bnd = torch.cat([e_dct * (g * i * (1 - i)).abs(), e_dct * (cp * f * (1 - f)).abs(),
-                         e_dct * (i * (1 - g * g)).abs() + (dct * i).abs() * 2.0 ** -23,
-                         e_dh * (th * o * (1 - o)).abs() + (dh * o * (1 - o)).abs() * 2.0 ** -22 * th.abs()], 1) + _ULPS * dG.abs()
-        ck.bound("dcat gates", dcat[:, A + C:], dG, bnd + 1e-38)
+        bnd, e_dct = cell_backward_bounds(e_dc[:n], e_dh, dc[:n], dh, dct, i, f, g, o, th, cp, dG)
+        ck.bound("dcat gates", dcat[:, A + C:], dG, bnd)
         dc[:n], e_dc[:n] = dcp, e_dct * f.abs() + 2.0 ** -24 * dcp.abs()
         # the attention backward: d gctx = (RN dG) @ W_ih[:, E:] from the stored d gates
         x = act(dcat[:, A + C:])
-        dgctx, e_dg = x @ w_ctx, _ACC * (x.abs() @ w_ctx.abs())
+        dgctx, e_dg = x @ w_ctx, ACC * (x.abs() @ w_ctx.abs())
         gate = t_["out1"][t][:n, A:A + C].double()
         ctxk = t_["ctx"][t][:n].double()
         ck.bound("dctx", t_["dctx"][t][:n], dgctx * gate, e_dg * gate + 2.0 ** -24 * (dgctx * gate).abs() + 1e-38)
         dgp = dgctx * ctxk * gate * (1 - gate)
-        ck.bound("dcat gate_pre", dcat[:, A:A + C], dgp, e_dg * (ctxk * gate * (1 - gate)).abs() + _ULPS * dgp.abs() + 1e-38)
+        ck.bound("dcat gate_pre", dcat[:, A:A + C], dgp, e_dg * (ctxk * gate * (1 - gate)).abs() + ULPS * dgp.abs() + 1e-38)
         de, datt2 = ds.attention_backward_from_dctx(att1d[:n], encd[:n], t_["out1"][t][:n, :A].double(), wf, alphas[:n, t], ctxk,
                                                     t_["dctx"][t][:n].double(), dregk[:n], sregk[:n, t])
         ck.attn("de", t_["de"][:n, t], de)
@@ -415,7 +424,7 @@ def _check(ck, dec, ws, enc, caps, lengths, mult):
     ck.value("g_b_full", S.g("attention.full_att.bias"), 0.0)
     da1, Sda1 = da1 * wf, Sda1 * wf.abs()
     datt1 = t_["datt1"]
-    ck.bound("datt1", datt1, da1, _ACC * Sda1 + (_half_ulp_bf16(da1) if datt1.dtype == torch.bfloat16 else 0))
+    ck.bound("datt1", datt1, da1, ACC * Sda1 + (half_ulp_bf16(da1) if datt1.dtype == torch.bfloat16 else 0))
     d1 = datt1.double().reshape(B * R, A)
     tn("g_w_enc_att", S.g("attention.encoder_att.weight"), d1, encd.reshape(B * R, C))
     colsum("g_b_enc_att", S.g("attention.encoder_att.bias"), d1)
@@ -431,8 +440,12 @@ def _check(ck, dec, ws, enc, caps, lengths, mult):
     ck.gemm("d encoder_out", t_["denc"], ref, Sref)
 
 
-def _outputs(dec, ws):
-    return [ws["t"][k].clone() for k in _FILLED if k in ws["t"]] + [ws["t"]["logits"].clone(), dec.store.grad.clone()]
+def _outputs(dec, ws, layer2=None):
+    out = [ws["t"][k].clone() for k in _FILLED if k in ws["t"]] + [ws["t"]["logits"].clone(), dec.store.grad.clone()]
+    if layer2 is not None:
+        B, T = ws["t"]["hd"].shape[:2]
+        out += [_layer2_dir(layer2, B, T).ws.clone(), layer2.store.grad.clone()]
+    return out
 
 
 @pytest.mark.parametrize("schedule,case", _PARAMS, ids=["%s-%s" % sc for sc in _PARAMS])
@@ -442,16 +455,17 @@ def test_decoder_steps_vs_float64(schedule, case):
     "deterministic" two runs from the same state must agree bit for bit."""
     from latex_ocr_b200 import _lib
     opts, _ = _SCHEDULES[schedule]
-    seed = sorted(_CASES).index(case)
-    dec, enc, caps, lengths, mask = _model(case, seed)
+    base = _TWO_LAYER.get(case, case)
+    seed = sorted(_CASES).index(base)
+    dec, enc, caps, lengths, mask, layer2 = _model(base, seed, case in _TWO_LAYER)
     with _lib.option(**opts):
-        ws, mult = _run(dec, enc, caps, lengths, mask, seed)
-        first = _outputs(dec, ws) if "deterministic" in opts else None
-        ck = _Checker("%s %s" % (schedule, case))
-        _check(ck, dec, ws, enc, caps, lengths, mult)
+        ws, mult, snap = _run(dec, enc, caps, lengths, mask, seed, layer2)
+        first = _outputs(dec, ws, layer2) if "deterministic" in opts else None
+        ck = Checker("%s %s" % (schedule, case))
+        _check(ck, dec, ws, enc, caps, lengths, mult, snap, layer2)
         if first is not None:
-            ws, _ = _run(dec, enc, caps, lengths, mask, seed)
-            for a, b in zip(first, _outputs(dec, ws)):
+            ws, _, _ = _run(dec, enc, caps, lengths, mask, seed, layer2)
+            for a, b in zip(first, _outputs(dec, ws, layer2)):
                 assert torch.equal(a.view(torch.uint8), b.view(torch.uint8)), "deterministic: two runs differ"
     for k, v in ck.worst.items():
         _WORST[k] = max(_WORST.get(k, 0.0), v)

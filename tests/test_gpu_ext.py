@@ -144,3 +144,33 @@ def test_ext_bf16_close_to_oracle_and_trains():
     assert last < first, (first, last)
     with pytest.raises(NotImplementedError):
         m.predict_batch(img)
+
+
+def test_ext_train_step_deterministic_option_gives_bit_identical_steps():
+    """Option "deterministic" on the extension's train step (CNN -> row biLSTM -> two-layer decoder -> loss -> backward -> Adam):
+    two steps from the same parameters and batch give bitwise the same gradients and updated master weights in all four
+    stores (encoder, row encoder, decoder, layer 2).  The default mode's gradients (fp32 atomics) agree with them to rounding,
+    parameter by parameter, as in tests/test_gpu_tc.py."""
+    from latex_ocr_b200 import _lib
+    from oracle import ref_ext as rx
+    from oracle import ref_model as rm
+    V = 50
+    pe, pd = rm.init_params(V, seed=7)
+    prow, p2 = rx.init_params_ext(seed=8)
+    img, formula = rm.synthetic_batch(4, 32, 64, V, 4, 6, seed=10)
+    B, T = formula.shape[0], formula.shape[1] - 1
+    runs = {}
+    for det in (1, 1, 0):
+        with _lib.option(deterministic=det):
+            m = _ext_model(V, pe, prow, pd, p2, "bf16")
+            m._step_body(img.cuda(), formula.cuda(), [T] * B, None)
+            torch.cuda.synchronize()
+        stores = (m.encoder.store, m.row_encoder.store, m.decoder.store, m.layer2.store)
+        runs.setdefault(det, []).append([t.clone() for s_ in stores for t in (s_.grad, s_.master)])
+    first, second = runs[1]
+    for k, (a, b) in enumerate(zip(first, second)):
+        assert torch.equal(a, b), ("store %d %s differs between two deterministic steps" % (k // 2, ("grad", "master")[k % 2]))
+    for i, s_ in enumerate(stores):
+        for name, (off, n, _) in s_.offsets.items():
+            a, b = first[2 * i][off:off + n], runs[0][0][2 * i][off:off + n]
+            assert (a - b).norm().item() <= 5e-3 * b.norm().item() + 1e-9, name

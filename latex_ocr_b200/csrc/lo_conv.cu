@@ -357,8 +357,8 @@ __global__ void __launch_bounds__(256) conv3x3_igemm_kernel(const T* __restrict_
   const int K = 9 * Cin;
   const int tid = threadIdx.x;
   const int tx = tid % 16, ty = tid / 16;
-  const int64_t m0 = (int64_t)blockIdx.y * BM;
-  const int n0 = blockIdx.x * BN;
+  const int64_t m0 = (int64_t)blockIdx.x * BM;     // M tiles on grid.x (up to 2^31 - 1 of them; grid.y stops at 65535)
+  const int n0 = blockIdx.y * BN;
   // this thread loads A rows (tid/16 + 16*j), k = tid%16
   const int lk = tid % BK;
   int a_h[4], a_w[4];
@@ -816,7 +816,9 @@ int lo_conv3x3(const void* x, const void* w, const float* bias, const void* mask
     return tc_conv3x3((const bf16*)x, (const bf16*)w, bias, (const bf16*)mask, (bf16*)y, N, H, W, Cin, Cout, pad, relu, st);
   }
   const int Ho = H + 2 * pad - 2, Wo = W + 2 * pad - 2;
-  dim3 grid(cdiv(Cout, 64), cdiv((int64_t)N * Ho * Wo, 64));
+  const int64_t mtiles = ((int64_t)N * Ho * Wo + 63) / 64;
+  LO_CHECK_ARG(mtiles <= INT32_MAX && Cout <= 64 * 65535, "shape (too many output positions or channels for the grid)");
+  dim3 grid((unsigned)mtiles, cdiv(Cout, 64));
   LO_DISPATCH_DT(dt, T, (conv3x3_igemm_kernel<T><<<grid, 256, 0, st>>>((const T*)x, (const T*)w, bias, (const T*)mask, (T*)y,
                                                                        N, H, W, Cin, Cout, pad, relu)));
   LO_LAUNCH_OK();
@@ -836,10 +838,13 @@ int lo_conv3x3_wgrad(const void* x, const void* dy, float* dw, float* db, int dt
     if (db) LO_TRY(colsum(dy, dt, db, (int)P, Cout, Cout, 0, st));
     return LO_OK;
   }
+  // the splits add onto the zeroed dw with fp32 atomics.  Option "deterministic": at most two splits — two addends onto 0 sum
+  // the same in either order (the rule of lo_gemm's split-K)
   const int tiles = 9 * cdiv(Cin, 64) * cdiv(Cout, 64);
   int splits = cdiv(LO_NUM_SMS * 4, tiles);
   const int maxs = (int)((P + 511) / 512);
   if (splits > maxs) splits = maxs;
+  if (g_opt_det && splits > 2) splits = 2;
   if (splits < 1) splits = 1;
   dim3 grid(cdiv(Cin, 64), cdiv(Cout, 64), 9 * splits);
   LO_DISPATCH_DT(dt, T, (conv3x3_wgrad_kernel<T><<<grid, 256, 0, st>>>((const T*)x, (const T*)dy, dw, N, H, W, Cin, Cout, pad, splits)));

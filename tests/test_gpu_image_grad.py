@@ -276,12 +276,10 @@ def test_image_grad_changes_nothing_else_and_works_on_a_frozen_model(precision):
         out1, grads1 = step(x)
         assert torch.equal(out1, want_out) and torch.equal(out0, want_out)
         names = [n for mod in ("encoder", "decoder") for n, _ in getattr(m, mod).named_parameters()]
-        # gradients that the step itself does not reproduce bit for bit, even with "deterministic": in fp32 the CUDA-core weight
-        # gradient of cnn.3 (measured: 4e-9 apart between two identical steps); those are held to 1e-6 of max-abs instead
-        unstable = {n for n, a, b in zip(names, grads0, again) if not torch.equal(a, b)}
-        assert unstable <= ({"cnn.3.weight"} if precision == "fp32" else set()), unstable
-        differ = [(n, (a - b).abs().max().item()) for n, a, b in zip(names, grads0, grads1)
-                  if not torch.equal(a, b) and (n not in unstable or _err(b, a) > 1e-6)]
+        # with "deterministic" every gradient of the step is reproduced bit for bit, in fp32 (CUDA cores) as in bf16
+        unstable = [n for n, a, b in zip(names, grads0, again) if not torch.equal(a, b)]
+        assert not unstable, unstable
+        differ = [(n, (a - b).abs().max().item()) for n, a, b in zip(names, grads0, grads1) if not torch.equal(a, b)]
         assert not differ, differ
         dimg = x.grad.clone()
         assert dimg.abs().max() > 0

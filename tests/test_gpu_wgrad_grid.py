@@ -2,7 +2,8 @@
 bf16 inputs.  Default mode: whole-wave grids, one split or several, the last one ragged.  Option "deterministic": the ordered
 cluster sum of up to 8 splits, bit-identical from call to call.  Convolutions with Cin of 256 and 512 run the 128 x 256 tiles on
 64-position K blocks, and so does the TN GEMM with N % 256 == 0 under option wgrad256; the others run 128 x 128 / 128 x 64
-tiles on 128-position blocks."""
+tiles on 128-position blocks.  The convolution cases also run the CUDA-core kernel (fp32 storage, and bf16 with
+conv_impl="simt"), whose position splits must be just as reproducible under "deterministic"."""
 import pytest
 import torch
 import torch.nn.functional as F
@@ -27,21 +28,29 @@ CONVS = [(1, 6, 30, 64, 128, 1), (4, 16, 64, 64, 128, 1), (2, 16, 64, 128, 256, 
          (2, 10, 34, 512, 256, 0), (2, 4, 140, 512, 128, 1)]
 
 
+# impl: the tensor-core kernel (bf16), or the CUDA-core kernel (conv3x3_wgrad_kernel) at fp32 and at bf16.  The CUDA-core kernel
+# cuts the positions into up to cdiv(528, 9 cdiv(Cin, 64) cdiv(Cout, 64)) splits of at least 512 positions each, added with
+# atomics; under "deterministic" at most two, whose two addends onto the zeroed dw sum the same in either order.
+IMPLS = [("tc", "bf16"), ("simt", "fp32"), ("simt", "bf16")]
+
+
+@pytest.mark.parametrize("impl,precision", IMPLS, ids=["%s_%s" % i for i in IMPLS])
 @pytest.mark.parametrize("N,H,W,Cin,Cout,pad", CONVS)
-def test_conv3x3_wgrad_splits_against_float64(N, H, W, Cin, Cout, pad):
+def test_conv3x3_wgrad_splits_against_float64(N, H, W, Cin, Cout, pad, impl, precision):
     _lib, L = _L()
     g = torch.Generator(device="cuda").manual_seed(5)
     Ho, Wo = H + 2 * pad - 2, W + 2 * pad - 2
-    x = torch.randn(N, H, W, Cin, device="cuda", generator=g).bfloat16()
-    dy = torch.randn(N, Ho, Wo, Cout, device="cuda", generator=g).bfloat16()
+    dtype = torch.bfloat16 if precision == "bf16" else torch.float32
+    x = torch.randn(N, H, W, Cin, device="cuda", generator=g).bfloat16().to(dtype)
+    dy = torch.randn(N, Ho, Wo, Cout, device="cuda", generator=g).bfloat16().to(dtype)
     w = torch.zeros(Cout, Cin, 3, 3, device="cuda", dtype=torch.float64, requires_grad=True)
     F.conv2d(x.permute(0, 3, 1, 2).double(), w, None, padding=pad).backward(dy.permute(0, 3, 1, 2).double())
     ref = w.grad.permute(0, 2, 3, 1)
 
     def run():
         dw = torch.full((Cout, 3, 3, Cin), 7.0, device="cuda")      # the call clears it
-        _lib.check(L.lo_conv3x3_wgrad(_lib.ptr(x), _lib.ptr(dy), _lib.ptr(dw), None, _lib.LO_BF16, N, H, W, Cin, Cout, pad,
-                                      _lib.LO_IMPL_TC, _lib.stream_ptr()))
+        _lib.check(L.lo_conv3x3_wgrad(_lib.ptr(x), _lib.ptr(dy), _lib.ptr(dw), None, _lib.dt_of(x), N, H, W, Cin, Cout, pad,
+                                      _lib.impl_code(impl, precision), _lib.stream_ptr()))
         torch.cuda.synchronize()
         return dw
 

@@ -411,7 +411,7 @@ int lo_decoder_greedy_hist(const lo_decoder_args* a, int64_t start_id, int64_t e
 
 /* beam search on the same step kernels: beam_search_decoder_cell.py:98-187 (log-softmax, finished mask with
  * dtype.min, only beam 0 at time 0, top-k over beam*V with the lower index winning ties, state gather by parents;
- * no length normalisation, diversity penalty off as in configs/model.json:15-16).  a->B = n_img*beam rows,
+ * no length normalisation (lo_decoder_beam_pen adds it), diversity penalty off as in configs/model.json:15-16).  a->B = n_img*beam rows,
  * a->rows_per_img = beam, a->enc holds n_img images.  ids/parents out [n_img][max_steps][beam] int64,
  * fin_hist [n_img][max_steps][beam] int32 (finished flags after each step), logp [n_img][beam] final scores. */
 int lo_decoder_beam(const lo_decoder_args* a, int64_t start_id, int64_t end_id, int max_steps, int64_t* ids,
@@ -424,6 +424,39 @@ int lo_decoder_beam(const lo_decoder_args* a, int64_t start_id, int64_t end_id, 
 int lo_decoder_beam_div(const lo_decoder_args* a, int64_t start_id, int64_t end_id, int max_steps, int64_t* ids,
                         int64_t* parents, int32_t* fin_hist, float* logp, float div_gamma, float div_prob,
                         const float* div_u, const uint64_t* div_state, void* stream);
+
+/* Length and coverage penalties of beam search (lo_decoder_beam_pen, lo_tfdec_beam_pen): the penalties of GNMT (Wu et al. 2016,
+ * eq. 14) in the form of TF's BeamSearchDecoder(length_penalty_weight=alpha).  Every rule of the beam step above stays; per row k
+ * the search also keeps len[k], the tokens other than END its hypothesis has emitted (grows only while the row is unfinished),
+ * and cov[k][r], the sum over the unfinished steps of the row's attention weights, following the hypothesis's lineage, over the
+ * image's own regions r.  Candidate (k, v) at step t, with carried = logp[k] + log-softmax (+ diversity penalty) as today:
+ *   new_len = len[k] + (finished[k] || v == END ? 0 : 1)
+ *   cov'    = finished[k] ? cov[k] : cov[k] + alpha_t[k]             (alpha_t[k]: the attention row step t wrote for row k)
+ *   score   = carried / len_pen[new_len] + beta * sum_r ln(min(max(cov'_r, 1e-30), 1))
+ * A finished row's non-END candidates keep dtype.min as their score.  The top-k ranks by score; each winner carries its raw
+ * `carried` as the new logp (logp keeps its meaning), its new_len and cov' follow it to its slot.  With alpha = beta = 0 the call
+ * is lo_*_beam_div bit for bit (and scores == logp).
+ *   alpha, beta  weights, finite and >= 0; alpha = 0: no length penalty, beta = 0: no coverage penalty
+ *   len_pen      device fp32 [max_steps + 1], len_pen[l] = ((5 + l) / 6)^alpha computed by the caller (needed when alpha != 0)
+ *   cov          device fp32 scratch of 2 * B * R + B floats: the coverage [2][B][R] (read and written alternately, step by step)
+ *                then the coverage term of every row [B] (needed when beta > 0; R: the args' region capacity)
+ *   len          device int32 scratch [2][B] (always needed)
+ *   scores       optional device fp32 out [n_img][beam]: the winners' score after the last step
+ * Refused (LO_EINVAL) before any GPU work: a null struct, a negative or non-finite alpha or beta, alpha != 0 without len_pen,
+ * beta > 0 without cov, a null len, and beam * V * 8 bytes (the totals and the scores) above 200 kB when a penalty is on. */
+typedef struct lo_beam_penalty {
+  float alpha;
+  float beta;
+  const float* len_pen;
+  float* cov;
+  int32_t* len;
+  float* scores;
+} lo_beam_penalty;
+int64_t lo_sizeof_beam_penalty(void);
+/* lo_decoder_beam_div with the penalties of *pen */
+int lo_decoder_beam_pen(const lo_decoder_args* a, int64_t start_id, int64_t end_id, int max_steps, int64_t* ids,
+                        int64_t* parents, int32_t* fin_hist, float* logp, float div_gamma, float div_prob,
+                        const float* div_u, const uint64_t* div_state, const lo_beam_penalty* pen, void* stream);
 
 /* The hypotheses of a finished beam search of either flavour (lo_decoder_beam[_div], lo_tfdec_beam[_div]) and the attention weights
  * under which their tokens were chosen.  ids / parents: that call's outputs, [n_img][ids_stride_steps][beam] int64 (ids_stride_steps =
@@ -604,6 +637,10 @@ int lo_tfdec_beam(const lo_tfdec_args* a, int64_t end_id, int max_steps, int64_t
 /* with the diversity penalty (see lo_decoder_beam_div) */
 int lo_tfdec_beam_div(const lo_tfdec_args* a, int64_t end_id, int max_steps, int64_t* ids, int64_t* parents, int32_t* fin_hist,
                       float* logp, float div_gamma, float div_prob, const float* div_u, const uint64_t* div_state, void* stream);
+/* with the diversity penalty and the length and coverage penalties of *pen (see lo_beam_penalty) */
+int lo_tfdec_beam_pen(const lo_tfdec_args* a, int64_t end_id, int max_steps, int64_t* ids, int64_t* parents, int32_t* fin_hist,
+                      float* logp, float div_gamma, float div_prob, const float* div_u, const uint64_t* div_state,
+                      const lo_beam_penalty* pen, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * EXTENSION (not in the reference; BASELINE.json configs[3]): generic sequence LSTM with nn.LSTM semantics (gate order i,f,g,o,

@@ -904,9 +904,43 @@ __global__ void argmax_kernel(const float* __restrict__ logits, int V, int64_t* 
 
 
 // ------------------------------------------------------------------------------------------------
+// coverage of the beam rows (lo_beam_penalty, GNMT's coverage penalty, Wu et al. 2016 eq. 14): one warp per row b.  The hypothesis
+// in slot b continues the one of row parent_rows[b] (step t-1's selection), so cov_out[b] = cov_in[parent_rows[b]] (0 at t = 0),
+// plus this step's attention row alpha_t[b] when the hypothesis is unfinished; then term[b] = beta * sum_r ln(min(max(cov_r,
+// 1e-30), 1)) over the image's own regions (reg_off), each lane summing its regions in order and the warp in a fixed tree.
+// cov_in / cov_out are the two halves of the caller's [2][B][R] scratch, swapped every step: the gather needs no copy.
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) beam_coverage_kernel(const float* __restrict__ alpha_t, int64_t alpha_row_stride,
+                                                            const float* __restrict__ cov_in, float* __restrict__ cov_out,
+                                                            const int32_t* __restrict__ parent_rows,
+                                                            const int32_t* __restrict__ finished, const int32_t* __restrict__ reg_off,
+                                                            int B, int R, int beam, int t, float beta, float* __restrict__ term) {
+  const int b = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (b >= B) return;
+  const int img = b / beam;
+  const int Ri = reg_off ? reg_off[img + 1] - reg_off[img] : R;
+  const float* src = t > 0 ? cov_in + (int64_t)parent_rows[b] * R : nullptr;
+  const float* al = alpha_t + (int64_t)b * alpha_row_stride;
+  float* dst = cov_out + (int64_t)b * R;
+  const bool add = !finished[b];
+  float s = 0.f;
+  for (int r = lane; r < Ri; r += 32) {
+    const float c = (src ? src[r] : 0.f) + (add ? al[r] : 0.f);
+    dst[r] = c;
+    s += logf(fminf(fmaxf(c, 1e-30f), 1.f));
+  }
+  s = warp_sum(s);
+  if (lane == 0) term[b] = beta * s;
+}
+
+// ------------------------------------------------------------------------------------------------
 // beam search step (beam_search_decoder_cell.py:123-187): one block per image.
 //   lp = log_softmax(logits) ; finished beams -> [END: 0, else: dtype.min] ; total = prev + lp ;
 //   time 0: beam 0 only ; top-k(beam) over beam*V (lower flat index wins ties) ; id = idx % V ; parent = idx / V
+// With the penalties of lo_beam_penalty (len_in set) the top-k ranks candidate (k, v) by
+//   score = total / len_pen[len_in[k] + (finished[k] || v == END ? 0 : 1)] + cov_term[k]      (no division without len_pen,
+// no term without cov_term; a finished row's non-END candidates keep dtype.min) and each winner carries its raw total as logp; its
+// length goes to len_out by parent.  scores (optional): the winners' ranking values (== logp without penalties).
 // ------------------------------------------------------------------------------------------------
 #define LO_BEAM_MAX 16
 __global__ void __launch_bounds__(256) beam_step_kernel(const float* __restrict__ logits, int V, int beam, int t, int64_t end_id,
@@ -915,15 +949,22 @@ __global__ void __launch_bounds__(256) beam_step_kernel(const float* __restrict_
                                                         int32_t* __restrict__ fin_hist, int64_t* __restrict__ next_tok,
                                                         int32_t* __restrict__ parent_rows, int max_steps, float div_log_gamma,
                                                         float div_prob, const float* __restrict__ div_u,
-                                                        const unsigned long long* __restrict__ div_state) {
-  extern __shared__ float s_tot[];            // [beam*V] (+ [beam*V] penalties when the diversity penalty is on)
+                                                        const unsigned long long* __restrict__ div_state,
+                                                        const float* __restrict__ len_pen, const float* __restrict__ cov_term,
+                                                        const int32_t* __restrict__ len_in, int32_t* __restrict__ len_out,
+                                                        float* __restrict__ scores) {
+  extern __shared__ float s_tot[];            // [beam*V] (+ [beam*V] diversity penalties, then the penalised scores)
   __shared__ float s_red[8];
   __shared__ int s_redi[8];
   __shared__ float s_lse[LO_BEAM_MAX];
   __shared__ float s_newp[LO_BEAM_MAX];
+  __shared__ float s_newc[LO_BEAM_MAX];
   __shared__ int s_newi[LO_BEAM_MAX];
+  __shared__ int s_len[LO_BEAM_MAX];
   const int img = blockIdx.x, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
   const int row0 = img * beam;
+  const bool pen = len_in != nullptr;
+  if (pen && tid < beam) s_len[tid] = t == 0 ? 0 : len_in[row0 + tid];
   // log-sum-exp per beam row (warp w handles rows w, w+8, ...)
   for (int k = wid; k < beam; k += 8) {
     const float* lg = logits + (int64_t)(row0 + k) * V;
@@ -972,11 +1013,30 @@ __global__ void __launch_bounds__(256) beam_step_kernel(const float* __restrict_
     for (int i = tid; i < total; i += 256) s_tot[i] += s_pen[i];
     __syncthreads();
   }
+  float* s_key = s_tot;                       // what the top-k ranks
+  if (pen) {
+    // length penalty (GNMT eq. 14; TF BeamSearchDecoder's length_penalty_weight) and the coverage term, into the second array
+    s_key = s_tot + beam * V;
+    for (int i = tid; i < total; i += 256) {
+      const int k = i / V, v = i % V;
+      const int fin = finished[row0 + k];
+      float s;
+      if (fin && v != (int)end_id) {
+        s = -3.4028234663852886e38f;
+      } else {
+        s = s_tot[i];
+        if (len_pen) s = s / len_pen[s_len[k] + (fin || v == (int)end_id ? 0 : 1)];
+        if (cov_term) s += cov_term[row0 + k];
+      }
+      s_key[i] = s;
+    }
+    __syncthreads();
+  }
   for (int j = 0; j < beam; j++) {
     float best = -INFINITY;
     int bi = 0x7fffffff;
     for (int i = tid; i < total; i += 256) {
-      const float x = s_tot[i];
+      const float x = s_key[i];
       if (x > best || (x == best && i < bi)) { best = x; bi = i; }
     }
 #pragma unroll
@@ -994,22 +1054,26 @@ __global__ void __launch_bounds__(256) beam_step_kernel(const float* __restrict_
         if (s_red[w] > b2 || (s_red[w] == b2 && s_redi[w] < i2)) { b2 = s_red[w]; i2 = s_redi[w]; }
       if (i2 == 0x7fffffff) i2 = 0;          // fewer candidates than beams (beam*V < beam): cannot happen for V >= beam
       s_newp[j] = b2;
+      s_newc[j] = pen ? s_tot[i2] : b2;
       s_newi[j] = i2;
-      s_tot[i2] = -INFINITY;                  // remove from the candidate set
+      s_key[i2] = -INFINITY;                  // remove from the candidate set
     }
     __syncthreads();
   }
   if (tid < beam) {
     const int idx = s_newi[tid];
     const int id = idx % V, par = idx / V;
-    const int fin = finished[row0 + par] | (id == (int)end_id ? 1 : 0);
+    const int fin_par = finished[row0 + par];
+    const int fin = fin_par | (id == (int)end_id ? 1 : 0);
     const int64_t o = ((int64_t)img * max_steps + t) * beam + tid;
     ids[o] = id;
     parents[o] = par;
     fin_hist[o] = fin;
     next_tok[row0 + tid] = id;
     parent_rows[row0 + tid] = row0 + par;
-    logp[row0 + tid] = s_newp[tid];           // (every read of the old logp happened before the top-k loop)
+    logp[row0 + tid] = s_newc[tid];           // (every read of the old logp happened before the top-k loop)
+    if (pen) len_out[row0 + tid] = s_len[par] + (fin_par || id == (int)end_id ? 0 : 1);
+    if (scores) scores[row0 + tid] = s_newp[tid];
   }
   __syncthreads();                            // finished[] of the parents is read above, overwritten below
   if (tid < beam) {
@@ -1395,20 +1459,35 @@ static int backward_step(const lo_decoder_args* a, const Dims& d, int t, int nro
   return LO_OK;
 }
 
+// shared memory of beam_step_kernel: the beam x V totals, and a second such array for the diversity penalties and / or the
+// penalised scores (lo_beam_penalty)
+static size_t beam_step_smem(int beam, int V, bool second) { return (size_t)beam * V * 4 * (second ? 2 : 1); }
+
+// the penalty operands of one beam step (all NULL: no penalty)
+struct BeamPenStep {
+  const float* len_pen;
+  const float* cov_term;
+  const int32_t* len_in;
+  int32_t* len_out;
+  float* scores;
+};
+
 // one beam-search step of either decoder flavour (beam_step_kernel, one CTA per image): the top-k over beam x V log-probs in shared
-// memory, twice that with the diversity penalty (div_on)
+// memory, twice that with the diversity penalty (div_on) or the penalties of lo_beam_penalty (ps.len_in set)
 static int beam_select(const float* logits, int V, int beam, int n_img, int t, int max_steps, int64_t end_id, float* logp,
                        int32_t* finished, int64_t* ids, int64_t* parents, int32_t* fin_hist, int64_t* next_tok, int32_t* parent_rows,
-                       bool div_on, float div_gamma, float div_prob, const float* div_u_t, const uint64_t* div_state, cudaStream_t st) {
+                       bool div_on, float div_gamma, float div_prob, const float* div_u_t, const uint64_t* div_state,
+                       const BeamPenStep& ps, cudaStream_t st) {
   static bool smem_attr = false;      // the 200 kB opt-in, once per process
-  const size_t smem = (size_t)beam * V * 4 * (div_on ? 2 : 1);
+  const size_t smem = beam_step_smem(beam, V, div_on || ps.len_in);
   if (!smem_attr && smem > 48 * 1024) {
     LO_CUDA(cudaFuncSetAttribute(beam_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     smem_attr = true;
   }
   beam_step_kernel<<<n_img, 256, smem, st>>>(logits, V, beam, t, end_id, logp, finished, ids, parents, fin_hist, next_tok, parent_rows,
                                              max_steps, div_on ? logf(div_gamma) : 0.f, div_on ? div_prob : 0.f, div_u_t,
-                                             (const unsigned long long*)div_state);
+                                             (const unsigned long long*)div_state, ps.len_pen, ps.cov_term, ps.len_in, ps.len_out,
+                                             ps.scores);
   LO_LAUNCH_OK();
   return LO_OK;
 }
@@ -1480,12 +1559,16 @@ __global__ void __launch_bounds__(256) beam_backtrack_kernel(const int64_t* __re
 // A flavour F hands the loops F::c: the step's logits [B][V], device scratch of B rows each and the ragged attention state
 // (rg.reg_off NULL: every image has R regions) of rpi rows per image; F::prologue(st); F::step(t, st): the cell step fed next_tok
 // (or the start token), then the head into logits; and for beam search F::reorder(t, st): the state of step t gathered by parent_rows.
+// The step writes its attention rows of R regions: row b of step t at alphas + b * alpha_row_stride + t * R.
 struct DecodeCtx {
   int B, T, V, rpi;
   const float* logits;
   int64_t* next_tok;
   int32_t *finished, *parent_rows;
   AttRagged rg;
+  int R;
+  const float* alphas;
+  int64_t alpha_row_stride;
   const AttRagged* ragged() const { return rg.reg_off ? &rg : nullptr; }
 };
 
@@ -1494,8 +1577,24 @@ struct BeamArgs {
   float div_gamma, div_prob;
   const float* div_u;            // [max_steps][B][V] injected uniforms, or NULL (Philox from div_state)
   const uint64_t* div_state;
+  const lo_beam_penalty* pen;    // NULL: no penalty (checked by check_beam_penalty otherwise)
   bool div_on() const { return !(div_gamma == 1.f || div_prob == 0.f); }        // beam_search_decoder_cell.py:270-273
+  bool pen_on() const { return pen && (pen->alpha != 0.f || pen->beta > 0.f); }
 };
+
+// the refusals of lo_decoder_beam_pen / lo_tfdec_beam_pen, before any GPU work (beam, V: the args' rows_per_img and V)
+static int check_beam_penalty(const lo_beam_penalty* p, int beam, int V, bool div_on) {
+  LO_CHECK_ARG(p, "null lo_beam_penalty");
+  LO_CHECK_ARG(std::isfinite(p->alpha) && p->alpha >= 0.f && std::isfinite(p->beta) && p->beta >= 0.f,
+               "penalty weights alpha and beta must be finite and >= 0");
+  LO_CHECK_ARG(p->alpha == 0.f || p->len_pen, "length penalty (alpha != 0) needs the len_pen table");
+  LO_CHECK_ARG(!(p->beta > 0.f) || p->cov, "coverage penalty (beta > 0) needs the cov scratch");
+  LO_CHECK_ARG(p->len, "null len scratch");
+  const bool on = p->alpha != 0.f || p->beta > 0.f;
+  LO_CHECK_ARG(beam_step_smem(beam < 1 ? 1 : beam, V, div_on || on) <= 200 * 1024,
+               "beam*V too large for the shared-memory top-k");
+  return LO_OK;
+}
 
 // the decode arguments both flavours check alike (bm NULL: greedy decode), before anything is enqueued; then everything before
 // step 0: finished = 0, log-probs = 0 (beam search, :106-107), the prologue, the ragged CTA map
@@ -1507,7 +1606,7 @@ static int decode_begin(F& f, int max_steps, bool outputs, const BeamArgs* bm, f
     LO_CHECK_ARG(!bm->div_on() || (bm->div_gamma > 0.f && (bm->div_u || bm->div_state)),
                  "diversity penalty needs gamma > 0 and div_u or div_state");
     LO_CHECK_ARG(bm->beam >= 1 && bm->beam <= LO_BEAM_MAX && c.B % bm->beam == 0, "1 <= beam (rows_per_img) <= 16, B % beam == 0");
-    LO_CHECK_ARG((size_t)bm->beam * c.V * 4 * (bm->div_on() ? 2 : 1) <= 200 * 1024, "beam*V too large for the shared-memory top-k");
+    LO_CHECK_ARG(beam_step_smem(bm->beam, c.V, bm->div_on() || bm->pen_on()) <= 200 * 1024, "beam*V too large for the shared-memory top-k");
   }
   LO_CUDA(cudaMemsetAsync(c.finished, 0, (size_t)c.B * 4, st));
   if (logp) LO_CUDA(cudaMemsetAsync(logp, 0, (size_t)c.B * 4, st));
@@ -1538,11 +1637,30 @@ static int beam_loop(F& f, const BeamArgs& bm, int64_t end_id, int max_steps, in
                      float* logp, cudaStream_t st) {
   const DecodeCtx& c = f.c;
   LO_TRY(decode_begin(f, max_steps, ids && parents && fin_hist && logp, &bm, logp, st));
+  const bool pen = bm.pen_on(), cov = pen && bm.pen->beta > 0.f;
+  const int64_t nc = (int64_t)c.B * c.R;          // one half of the [2][B][R] coverage, then the [B] coverage terms
   for (int t = 0; t < max_steps; t++) {
     LO_TRY(f.step(t, st));
+    BeamPenStep ps{};
+    if (bm.pen) ps.scores = bm.pen->scores;
+    if (pen) {
+      // step t reads the lengths and coverage of step t-1 from one half of the scratch and writes its own to the other
+      const int h = t & 1;
+      ps.len_pen = bm.pen->alpha != 0.f ? bm.pen->len_pen : nullptr;
+      ps.len_in = bm.pen->len + (int64_t)(1 - h) * c.B;
+      ps.len_out = bm.pen->len + (int64_t)h * c.B;
+      if (cov) {
+        float* term = bm.pen->cov + 2 * nc;
+        beam_coverage_kernel<<<cdiv(c.B, 8), 256, 0, st>>>(c.alphas + (int64_t)t * c.R, c.alpha_row_stride, bm.pen->cov + (1 - h) * nc,
+                                                           bm.pen->cov + h * nc, c.parent_rows, c.finished, c.rg.reg_off, c.B, c.R,
+                                                           bm.beam, t, bm.pen->beta, term);
+        LO_LAUNCH_OK();
+        ps.cov_term = term;
+      }
+    }
     LO_TRY(beam_select(c.logits, c.V, bm.beam, c.B / bm.beam, t, max_steps, end_id, logp, c.finished, ids, parents, fin_hist,
                        c.next_tok, c.parent_rows, bm.div_on(), bm.div_gamma, bm.div_prob,
-                       bm.div_u ? bm.div_u + (int64_t)t * c.B * c.V : nullptr, bm.div_state, st));
+                       bm.div_u ? bm.div_u + (int64_t)t * c.B * c.V : nullptr, bm.div_state, ps, st));
     LO_TRY(f.reorder(t, st));
   }
   return LO_OK;
@@ -1559,7 +1677,7 @@ struct TorchDecode {
   TorchDecode(const lo_decoder_args* a_, int64_t start, int32_t* finished, int32_t* parent_rows)
       : a(a_), start_id(start), d(dims(a_)), bv(bf_views(a_, d)),
         c{d.B, d.T, d.V, a_->rows_per_img > 1 ? a_->rows_per_img : 1, a_->logits, (int64_t*)a_->sreg, finished, parent_rows,
-          ragged_of(a_)} {}
+          ragged_of(a_), d.R, a_->alphas, (int64_t)d.T * d.R} {}
   int prologue(cudaStream_t st) {
     fill_i64_kernel<<<cdiv(d.B, 128), 128, 0, st>>>(c.next_tok, start_id, d.B);
     LO_LAUNCH_OK();
@@ -1586,6 +1704,19 @@ struct TorchDecode {
     return LO_OK;
   }
 };
+
+// both beam entry points of the torch flavour (bm.beam is set here from rows_per_img)
+static int decoder_beam(const lo_decoder_args* a, int64_t start_id, int64_t end_id, int max_steps, int64_t* ids, int64_t* parents,
+                        int32_t* fin_hist, float* logp, BeamArgs bm, void* stream) {
+  LO_TRY(check_args(a));
+  LO_TRY(check_reg_off(a, true));
+  LO_CHECK_ARG(!a->ss_prob, "scheduled sampling (ss_prob) is a training mode: not available in beam search");
+  LO_CHECK_ARG((int64_t)a->B * a->T >= 2 * a->B, "row_loss scratch too small");
+  int32_t* finished = (int32_t*)a->row_loss;
+  TorchDecode f(a, start_id, finished, finished + a->B);
+  bm.beam = a->rows_per_img;
+  return beam_loop(f, bm, end_id, max_steps, ids, parents, fin_hist, logp, (cudaStream_t)stream);
+}
 
 }  // namespace lo
 
@@ -2046,15 +2177,20 @@ int lo_decoder_beam(const lo_decoder_args* a, int64_t start_id, int64_t end_id, 
 int lo_decoder_beam_div(const lo_decoder_args* a, int64_t start_id, int64_t end_id, int max_steps, int64_t* ids, int64_t* parents,
                         int32_t* fin_hist, float* logp, float div_gamma, float div_prob, const float* div_u,
                         const uint64_t* div_state, void* stream) {
-  LO_TRY(check_args(a));
-  LO_TRY(check_reg_off(a, true));
-  LO_CHECK_ARG(!a->ss_prob, "scheduled sampling (ss_prob) is a training mode: not available in beam search");
-  LO_CHECK_ARG((int64_t)a->B * a->T >= 2 * a->B, "row_loss scratch too small");
-  int32_t* finished = (int32_t*)a->row_loss;
-  TorchDecode f(a, start_id, finished, finished + a->B);
-  return beam_loop(f, BeamArgs{a->rows_per_img, div_gamma, div_prob, div_u, div_state}, end_id, max_steps, ids, parents, fin_hist, logp,
-                   (cudaStream_t)stream);
+  return decoder_beam(a, start_id, end_id, max_steps, ids, parents, fin_hist, logp, BeamArgs{0, div_gamma, div_prob, div_u, div_state,
+                                                                                             nullptr}, stream);
 }
+
+int lo_decoder_beam_pen(const lo_decoder_args* a, int64_t start_id, int64_t end_id, int max_steps, int64_t* ids, int64_t* parents,
+                        int32_t* fin_hist, float* logp, float div_gamma, float div_prob, const float* div_u,
+                        const uint64_t* div_state, const lo_beam_penalty* pen, void* stream) {
+  const BeamArgs bm{0, div_gamma, div_prob, div_u, div_state, pen};
+  LO_CHECK_ARG(a, "null args");
+  LO_TRY(check_beam_penalty(pen, a->rows_per_img, a->V, bm.div_on()));
+  return decoder_beam(a, start_id, end_id, max_steps, ids, parents, fin_hist, logp, bm, stream);
+}
+
+int64_t lo_sizeof_beam_penalty(void) { return (int64_t)sizeof(lo_beam_penalty); }
 
 int lo_beam_backtrack(const int64_t* ids, const int64_t* parents, int64_t ids_stride_steps, int n_img, int beam, int n,
                       const float* alphas, int64_t alpha_row_stride, int R, const int32_t* reg_off, const int32_t* reg_off_host,

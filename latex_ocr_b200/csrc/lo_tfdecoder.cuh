@@ -554,7 +554,7 @@ struct TfDecode {
   explicit TfDecode(const lo_tfdec_args* a_)
       : a(a_), d(tf_dims(a_)), w(tf_carve(a_)),
         c{d.B, d.T, d.V, d.rpi, a_->logits, w.next_tok, w.finished, w.parent_rows,
-          AttRagged{a_->reg_off, a_->reg_off_host, w.ragmap, 0}} {}
+          AttRagged{a_->reg_off, a_->reg_off_host, w.ragmap, 0}, d.R, a_->alphas, (int64_t)d.T * d.R} {}
   int prologue(cudaStream_t st) { return tf_prologue(a, d, w, st); }
   // step 0 is fed tok = NULL: the start-token row V of the token table
   int step(int t, cudaStream_t st) {
@@ -786,7 +786,19 @@ int lo_tfdec_beam_div(const lo_tfdec_args* a, int64_t end_id, int max_steps, int
                       float* logp, float div_gamma, float div_prob, const float* div_u, const uint64_t* div_state, void* stream) {
   LO_TRY(tf_check(a, true));
   TfDecode f(a);
-  return beam_loop(f, BeamArgs{f.d.rpi, div_gamma, div_prob, div_u, div_state}, end_id, max_steps, ids, parents, fin_hist, logp,
+  return beam_loop(f, BeamArgs{f.d.rpi, div_gamma, div_prob, div_u, div_state, nullptr}, end_id, max_steps, ids, parents, fin_hist,
+                   logp, (cudaStream_t)stream);
+}
+
+int lo_tfdec_beam_pen(const lo_tfdec_args* a, int64_t end_id, int max_steps, int64_t* ids, int64_t* parents, int32_t* fin_hist,
+                      float* logp, float div_gamma, float div_prob, const float* div_u, const uint64_t* div_state,
+                      const lo_beam_penalty* pen, void* stream) {
+  LO_CHECK_ARG(a, "null args");
+  const BeamArgs bm0{0, div_gamma, div_prob, div_u, div_state, pen};
+  LO_TRY(check_beam_penalty(pen, a->rows_per_img, a->V, bm0.div_on()));
+  LO_TRY(tf_check(a, true));
+  TfDecode f(a);
+  return beam_loop(f, BeamArgs{f.d.rpi, div_gamma, div_prob, div_u, div_state, pen}, end_id, max_steps, ids, parents, fin_hist, logp,
                    (cudaStream_t)stream);
 }
 

@@ -19,6 +19,7 @@ greedy / beam calls with their outputs trimmed to the steps the reference would 
 import collections
 import ctypes
 import itertools
+import math
 
 import torch
 
@@ -93,6 +94,39 @@ def run_beam(call, N, beam, steps, V, device, div_u=None, order=None):
     check(call(ids.data_ptr(), parents.data_ptr(), hist.data_ptr(), logp.data_ptr(), div_u.data_ptr() if div_u is not None else None))
     n = _n_steps(hist)
     return ids[:, :n], parents[:, :n], logp
+
+
+def penalty_weights(length_penalty, coverage_penalty):
+    """(alpha, beta) of the length and coverage penalties of beam search as floats; a negative or non-finite weight is refused."""
+    alpha, beta = float(length_penalty), float(coverage_penalty)
+    for name, v in (("length_penalty", alpha), ("coverage_penalty", beta)):
+        if not math.isfinite(v) or v < 0:
+            raise ValueError("%s must be a finite number >= 0 (got %r)" % (name, v))
+    return alpha, beta
+
+
+def length_penalty_table(alpha, steps):
+    """LP[l] = ((5 + l) / 6) ** alpha for l = 0..steps: the length penalty of GNMT (Wu et al. 2016, eq. 14) as TF's
+    BeamSearchDecoder computes it (length_penalty_weight = alpha), in float64 and rounded once to fp32, so that the kernel and the
+    CPU reference divide by the same numbers.  All ones for alpha = 0."""
+    return (((5.0 + torch.arange(steps + 1, dtype=torch.float64)) / 6.0) ** float(alpha)).float()
+
+
+def beam_penalty(alpha, beta, B, R, steps, beam, device):
+    """The lo_beam_penalty of a beam search of B rows (B / beam images) over at most R regions and ``steps`` steps, and the tensors
+    it points at, which must outlive the call: the length-penalty table, the coverage and length scratch, and ``scores`` [B / beam,
+    beam], the winners' penalised scores after the last step."""
+    t = {"len": torch.empty(2 * B, dtype=torch.int32, device=device),
+         "scores": torch.zeros(B // beam, beam, dtype=torch.float32, device=device)}
+    if alpha != 0:
+        t["len_pen"] = length_penalty_table(alpha, steps).to(device)
+    if beta > 0:
+        t["cov"] = torch.empty(2 * B * R + B, dtype=torch.float32, device=device)     # [2][B][R] coverage, then [B] terms
+    p = _lib.BeamPenalty()
+    p.alpha, p.beta = alpha, beta
+    for k in ("len_pen", "cov", "len", "scores"):
+        setattr(p, k, t[k].data_ptr() if k in t else None)
+    return p, t
 
 
 def beam_hypotheses(ids, parents, finalize, a=None, alphas=None):
@@ -228,7 +262,8 @@ def attention_maps(alphas, att_h, att_w):
 
 
 def beam_decode(model, img, start_id, end_id, beam_size=5, max_length_formula=150, finalize="reference",
-                div_gamma=1, div_prob=0, div_u=None, div_seed=None, return_attention=False):
+                div_gamma=1, div_prob=0, div_u=None, div_seed=None, return_attention=False, length_penalty=0.0,
+                coverage_penalty=0.0, return_scores=False):
     """Returns (ids [N, beam, steps], log_probs [N, beam]) on the CPU; hypothesis 0 is the one the reference scores
     (img2seq.py:210).  ``div_gamma`` / ``div_prob``: the diversity penalty of beam_search_decoder_cell.py:258-287 (off when
     gamma == 1 or prob == 0, as in configs/model.json:15-16); its Bernoulli draws come from the in-kernel Philox stream seeded
@@ -238,9 +273,16 @@ def beam_decode(model, img, start_id, end_id, beam_size=5, max_length_formula=15
     ``return_attention=True`` also returns the attention weights of every hypothesis, [N, beam, steps, R] fp32 on the CPU (a list
     of [beam, steps, R_i] for a list of images): under ``finalize='reference'`` the rows slot s computed at each step, what the
     reference's attention_mechanism.ctx_vector holds and visualize_attention.py draws for s = 0; under ``'backtrack'`` the
-    attention under which each token of the hypothesis was chosen (the rows of a teacher-forced pass over its tokens)."""
+    attention under which each token of the hypothesis was chosen (the rows of a teacher-forced pass over its tokens).
+
+    ``length_penalty`` (alpha) / ``coverage_penalty`` (beta): the penalties of GNMT (Wu et al. 2016) that lo_beam_penalty
+    documents — the search ranks hypotheses by log_probs / ((5 + length) / 6) ** alpha + beta * sum_r ln(min(coverage_r, 1)), the
+    coverage being the attention summed along the hypothesis.  Both default to 0, the reference's search.  The log-probs returned
+    stay the raw sums; ``return_scores=True`` also returns the ranking scores [N, beam] (CPU), after the log-probs and before the
+    attention weights."""
     if finalize not in ("reference", "backtrack"):
         raise NotImplementedError("finalize must be 'reference' or 'backtrack'")
+    alpha, beta = penalty_weights(length_penalty, coverage_penalty)
     L = _lib.lib()
     max_steps = max_length_formula + 2
     with torch.no_grad():
@@ -252,12 +294,19 @@ def beam_decode(model, img, start_id, end_id, beam_size=5, max_length_formula=15
             seed = torch.initial_seed() if div_seed is None else int(div_seed)
             state = torch.tensor([seed & 0x7FFFFFFFFFFFFFFF, 0], dtype=torch.int64, device=dev)
 
+        pen = None
+        if alpha != 0 or beta > 0 or return_scores:
+            pen, pen_t = beam_penalty(alpha, beta, a.B, a.R, max_steps, beam_size, dev)
+
         def call(ids, parents, hist, logp, u):
-            return L.lo_decoder_beam_div(ctypes.byref(a), int(start_id), int(end_id), max_steps, ids, parents, hist, logp,
-                                         float(div_gamma), float(div_prob), u, state.data_ptr() if state is not None else None,
-                                         stream_ptr())
+            args = (ctypes.byref(a), int(start_id), int(end_id), max_steps, ids, parents, hist, logp, float(div_gamma), float(div_prob), u,
+                    state.data_ptr() if state is not None else None)
+            if pen is not None:
+                return L.lo_decoder_beam_pen(*args, ctypes.byref(pen), stream_ptr())
+            return L.lo_decoder_beam_div(*args, stream_ptr())
         ids, parents, logp = run_beam(call, N, beam_size, max_steps, a.V, dev, div_u if div_on else None,
                                       lay.order if lay else None)
+        scores = pen_t["scores"].cpu() if return_scores else None
         att = None
         if return_attention or finalize == "backtrack":
             alphas = ws["t"]["alphas"].view(-1)[:a.B * a.T * a.R].view(a.B, a.T, a.R) if return_attention else None
@@ -269,9 +318,11 @@ def beam_decode(model, img, start_id, end_id, beam_size=5, max_length_formula=15
         if lay is not None:
             inv = _inverse(lay.order)
             ids, logp = ids[inv], logp[inv]
+            if scores is not None:
+                scores = scores[inv]
             if att is not None:
                 att = [att[j, :, :, :lay.counts[j]].clone() for j in inv.tolist()]
-        return (ids, logp, att) if return_attention else (ids, logp)
+        return (ids, logp) + ((scores,) if return_scores else ()) + ((att,) if return_attention else ())
 
 
 def truncate_end(list_of_ids, id_end):

@@ -390,7 +390,9 @@ class Img2SeqModel:
         beam = int(beam_size or getattr(self._config, "beam_size", 5))
         ids, _ = decode.beam_decode(self, images, start_id, end_id, beam, L,
                                     div_gamma=float(getattr(self._config, "div_gamma", 1)),
-                                    div_prob=float(getattr(self._config, "div_prob", 0)))
+                                    div_prob=float(getattr(self._config, "div_prob", 0)),
+                                    length_penalty=getattr(self._config, "length_penalty", 0) or 0,
+                                    coverage_penalty=getattr(self._config, "coverage_penalty", 0) or 0)
         return [ids[:, k].tolist() for k in range(beam)], end_id
 
     def predict_batch(self, images, start_id=None, decoding=None, beam_size=None):

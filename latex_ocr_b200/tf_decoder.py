@@ -69,6 +69,9 @@ class Decoder(nn.Module):
         # diversity penalty of beam_search_decoder_cell.py:258-287 (off in the shipped config: model.json:15-16 -> gamma 1, prob 0)
         self.div_gamma = float(getattr(config, "div_gamma", 1) or 1)
         self.div_prob = float(getattr(config, "div_prob", 0) or 0)
+        # length and coverage penalties of GNMT (lo_beam_penalty); 0, the reference's search, when the config has none
+        self.length_penalty, self.coverage_penalty = decode.penalty_weights(getattr(config, "length_penalty", 0) or 0,
+                                                                            getattr(config, "coverage_penalty", 0) or 0)
         self._div_state = None
         self.max_length_formula = int(getattr(config, "max_length_formula", 150))
         self.precision = precision or getattr(config, "precision", "bf16")
@@ -351,7 +354,8 @@ class Decoder(nn.Module):
         ws["counts"], ws["off"] = [int(n) for n in counts], off
         return ws
 
-    def decode_packed(self, ws, steps, div_u=None, return_attention=False, return_log_probs=False, finalize="reference"):
+    def decode_packed(self, ws, steps, div_u=None, return_attention=False, return_log_probs=False, finalize="reference",
+                      return_scores=False):
         """decode() over the images packed in ``ws`` by packed_workspace: every image attends over its own regions only."""
         if finalize not in ("reference", "backtrack"):
             raise NotImplementedError("finalize must be 'reference' or 'backtrack'")
@@ -363,7 +367,7 @@ class Decoder(nn.Module):
             L, ws, a = self._args(ws["enc"], N * beam, steps, R, rows_per_img=beam, ws=ws)
             decode.set_region_offsets(a, ws["reg_off_host"], ws["reg_off"], ws["off"])
             alphas = ws["alphas"][:N * beam * steps * R].view(N * beam, steps, R) if return_attention else None
-            out = self._run_decode(L, a, N, steps, div_u, alphas, return_log_probs, finalize)
+            out = self._run_decode(L, a, N, steps, div_u, alphas, return_log_probs, finalize, return_scores)
             if alphas is None:
                 return out
             att = out[-1]
@@ -371,7 +375,8 @@ class Decoder(nn.Module):
                 return out[:-1] + ([att[i, :, :counts[i]].clone() for i in range(N)],)
             return out[:-1] + ([att[i, :, :, :counts[i]].clone() for i in range(N)],)
 
-    def decode(self, enc, max_steps=None, div_u=None, return_attention=False, return_log_probs=False, finalize="reference"):
+    def decode(self, enc, max_steps=None, div_u=None, return_attention=False, return_log_probs=False, finalize="reference",
+               return_scores=False):
         """dynamic_decode(decoder_cell, max_length_formula + 1) (decoder.py:70): at most max_length_formula + 2 steps, stops when
         every row / beam has emitted END.  Returns DecoderOutput(logits=None, ids).  ``div_u`` (tests): injected uniforms
         [steps, N*beam, V] for the diversity penalty; ``return_log_probs`` (beam search): also the log-probs of the hypotheses
@@ -381,6 +386,9 @@ class Decoder(nn.Module):
         t) and the rows slot s computed, what visualize_attention.py draws for s = 0; 'backtrack' returns lineage-consistent
         hypotheses, ids [N, steps, beam] followed back from each final slot, and the attention under which each of their tokens
         was chosen (the rows of a teacher-forced pass over the hypothesis).
+        The search ranks hypotheses with the length and coverage penalties of the config's ``length_penalty`` /
+        ``coverage_penalty`` (lo_beam_penalty; 0: the reference's search); the log-probs stay the raw sums, and
+        ``return_scores`` (beam search) also returns the ranking scores [N, beam], after the log-probs.
 
         ``enc`` [N,R,C] / [N,H,W,C], or a list of the encoder outputs of images of different sizes, each [H_i,W_i,C] or [R_i,C]:
         the list is decoded in one time loop in which every image attends over its own regions only (lo_tfdec_args.reg_off), so
@@ -396,14 +404,15 @@ class Decoder(nn.Module):
             off = ws["off"]
             for i, e in enumerate(encs):
                 ws["enc"][off[i]:off[i + 1]].copy_(e)
-            return self.decode_packed(ws, steps, div_u, return_attention, return_log_probs, finalize)
+            return self.decode_packed(ws, steps, div_u, return_attention, return_log_probs, finalize, return_scores)
         enc = self._enc(enc)
         N, R, _ = enc.shape
         self.store.refresh_shadow()
         with torch.no_grad():
             L, ws, a = self._args(enc, N * self._tiles, steps, R, rows_per_img=self._tiles, decode=True)
             ws["enc"] = enc
-            return self._run_decode(L, a, N, steps, div_u, ws["alphas"] if return_attention else None, return_log_probs, finalize)
+            return self._run_decode(L, a, N, steps, div_u, ws["alphas"] if return_attention else None, return_log_probs, finalize,
+                                    return_scores)
 
     def _enc_regions(self, e):
         """one image's encoder output of a list -> [R_i, C] on the device"""
@@ -415,7 +424,7 @@ class Decoder(nn.Module):
             raise ValueError("each image's encoder output must be [H,W,%d] or [R,%d] (got shape %s)" % (self.C, self.C, tuple(e.shape)))
         return e
 
-    def _run_decode(self, L, a, N, steps, div_u, alphas, return_log_probs, finalize="reference"):
+    def _run_decode(self, L, a, N, steps, div_u, alphas, return_log_probs, finalize="reference", return_scores=False):
         """The greedy or beam decode of the filled args ``a`` (N images); ``alphas``: the attention rows [B, steps, R] of the call
         (attention export) or None."""
         dev = self.store.device
@@ -433,9 +442,16 @@ class Decoder(nn.Module):
             self._div_state[1] += 1                                  # a new Philox stream per decode call
             state = self._div_state.data_ptr()
 
+        alpha, beta = self.length_penalty, self.coverage_penalty
+        pen = None
+        if alpha != 0 or beta > 0 or return_scores:
+            pen, pen_t = decode.beam_penalty(alpha, beta, a.B, a.R, steps, self._tiles, dev)
+
         def call(ids, parents, fin, logp, u):
-            return L.lo_tfdec_beam_div(ctypes.byref(a), self._id_end, steps, ids, parents, fin, logp, self.div_gamma, self.div_prob, u,
-                                       state, stream_ptr())
+            args = (ctypes.byref(a), self._id_end, steps, ids, parents, fin, logp, self.div_gamma, self.div_prob, u, state)
+            if pen is not None:
+                return L.lo_tfdec_beam_pen(*args, ctypes.byref(pen), stream_ptr())
+            return L.lo_tfdec_beam_div(*args, stream_ptr())
         ids, parents, logp = decode.run_beam(call, N, self._tiles, steps, self.V, dev, div_u if div_on else None)
         # finalize (beam_search_decoder_cell.py:189-250) gathers with the unchanged initial parents -> identity (SURVEY §8-A.3)
         att = None
@@ -443,7 +459,8 @@ class Decoder(nn.Module):
             hyp, att = decode.beam_hypotheses(ids, parents, finalize, a, alphas)
             if finalize == "backtrack":
                 ids = hyp.permute(0, 2, 1).contiguous()
-        out = (DecoderOutput(None, ids),) + ((logp,) if return_log_probs else ()) + ((att,) if alphas is not None else ())
+        out = ((DecoderOutput(None, ids),) + ((logp,) if return_log_probs else ()) + ((pen_t["scores"],) if return_scores else ())
+               + ((att,) if alphas is not None else ()))
         return out if len(out) > 1 else out[0]
 
     def forward(self, img, formula=None, dropout=1.0):

@@ -69,8 +69,6 @@ int64_t lo_launch_count(void);
  *   skinny_mma       1 [p]    decoder per-step GEMMs (M <= 64) on mma.sync; 0: on wgmma
  *   skinny_tma       1 [p]    1: their operands by cp.async.bulk, one copy per row; 0: 16-byte cp.async
  *   skinny8          1        1: 8-stage (198 KB shared memory) wgmma config for GEMMs with M <= 128
- *   conv_persist     1 [p]    1: persistent double-accumulator convolution kernel; 0: one tile per CTA
- *   conv_mt2         1 [p]    1: layers with <= 128 output channels: two 128-position sub-tiles per CTA share each weight stage
  *   conv_mc          1        1: cluster-of-2 multicast of the A tile in the wgmma GEMM
  *   wgrad256         0 [p]    1: the TN weight-gradient GEMMs also run 128 x 256 tiles when N % 256 == 0 (the conv weight gradient
  *                             always does when Cin % 256 == 0); off: slower on two of the decoder backward's four such GEMMs

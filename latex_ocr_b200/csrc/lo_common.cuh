@@ -68,8 +68,6 @@ constexpr int LO_NUM_SMS = 132;
   X(g_opt_skinny_mma, "skinny_mma", 1)            /* per-step GEMMs on mma.sync; 0: wgmma */                   \
   X(g_opt_skinny_tma, "skinny_tma", 1)            /* their operands by cp.async.bulk */                        \
   X(g_opt_skinny8, "skinny8", 1)                  /* 8-stage wgmma config for M <= 128 */                      \
-  X(g_opt_conv_persist, "conv_persist", 1)        /* persistent double-accumulator conv kernel */              \
-  X(g_opt_conv_mt2, "conv_mt2", 1)                /* two position sub-tiles share a weight stage */            \
   X(g_opt_conv_mc, "conv_mc", 1)                  /* cluster-of-2 multicast of the A tile */                   \
   X(g_opt_wgrad256, "wgrad256", 0)                /* 128 x 256 tiles also for the TN weight-gradient GEMMs */  \
   X(g_opt_det, "deterministic", 0)                /* fixed-order cross-CTA sums */                             \

@@ -1,13 +1,18 @@
-// wgmma + TMA kernels (sm_90a): NHWC 3x3 implicit-GEMM convolution and the K-major "NT" GEMM.
+// wgmma + TMA kernels (sm_90a): the K-major "NT" GEMM, the persistent NHWC 3x3 implicit-GEMM convolution (forward and
+// data gradient) and the weight gradient / "TN" GEMM.
 //
-//   D[128 x NT] (registers, fp32) += A[128 x 64] (smem, bf16, K-major, SWIZZLE_128B) * B[NT x 64]^T (smem, bf16, K-major)
+//   D[128 x NT] (registers, fp32) += A[128 x 64] (smem, bf16, SWIZZLE_128B) * B[NT x 64]^T (smem, bf16, SWIZZLE_128B)
 //
-// A tiles come from TMA: for the convolution a 4-D tiled map over the NHWC feature map {C, W, H, N} with box
-// {64, BW, BH, 1} (BW*BH = 128 output positions); tap (r,s) is just a coordinate shift and the halo / zero padding
-// falls out of TMA's out-of-bounds zero fill — no im2col buffer, no predicates.  B tiles are rows of the
-// [Cout][9*Cin] weight matrix.  Warp roles: warps 0..7 = two consumer warpgroups (warpgroup g owns rows [64g, 64g+64)
-// of the tile: wgmma into registers, then the epilogue straight from the accumulators), warp 8 = A-tile TMA producer,
-// warp 9 = B-tile TMA producer.  3-8 stage mbarrier ring.
+// Warp roles, all three kernels: warps 0..7 = two consumer warpgroups (warpgroup g owns rows [64g, 64g+64) of the tile:
+// wgmma into registers, then the epilogue straight from the accumulators), warp 8 = A-tile TMA producer, warp 9 = B-tile
+// TMA producer, over a 3-8 stage mbarrier ring.
+//   tc_gemm_kernel    C = A W^T (+ bias, ReLU, accumulate, split-K atomics): one 128 x NT tile per CTA; 2-D maps over the
+//                     K-major rows of A and W.  Option conv_mc: a CTA pair shares the A tile by multicast.
+//   tc_conv_p_kernel  one CTA per SM walks over output tiles.  A tiles: a 4-D map over the NHWC feature map {C, W, H, N}
+//                     with box {64, BW, BH, 1} (BW*BH = 128 output positions); tap (r,s) is a coordinate shift and the
+//                     halo / zero padding falls out of TMA's out-of-bounds zero fill — no im2col buffer, no predicates.
+//                     B tiles are rows of the [Cout][9*Cin] weight matrix.
+//   tc_wgrad_kernel   dW = dY^T (*) X and the TN GEMMs, both operands MN-major.
 #include <cuda.h>
 
 #include <mutex>
@@ -49,20 +54,12 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* map, u
       "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
-// multicast variants: the box lands at the same CTA-relative offset in every CTA of `mask` and completes on each one's mbarrier
+// multicast variant: the box lands at the same CTA-relative offset in every CTA of `mask` and completes on each one's mbarrier
 __device__ __forceinline__ void tma_load_2d_mc(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, uint16_t mask) {
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%4, %5}], [%2], %3;" ::"r"(
           smem_u32(dst)),
       "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "h"(mask), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_mc(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, int c3,
-                                               uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%4, %5, %6, %7}], [%2], %3;" ::"r"(
-          smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "h"(mask), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
 // arrive on the mbarrier at the same shared-memory offset in CTA `cta` of the cluster (may be this CTA)
@@ -94,22 +91,29 @@ __device__ __forceinline__ uint64_t make_kmajor_sw128_desc(uint32_t saddr) {
   return d;
 }
 
+// the NT GEMM C[M][N] = A[M][K] W[N][K]^T
 struct TcParams {
-  // problem
-  int M, N, K;            // GEMM view: M rows (positions), N = Cout, K = 9*Cin (conv) or K (gemm)
-  int conv;               // 0: plain NT GEMM ; 1: 3x3 conv
-  int Ho, Wo, Cin, pad;   // conv geometry (output H, W)
-  int BW, BH, tiles_w, tiles_h;
+  int M, N, K;
   // epilogue
   const float* bias;
-  const bf16* mask;
   void* out;
   int64_t ldc;
   int out_f32, accumulate, relu;
   int kb_per_split, atomic;   // split-K over gridDim.z: fp32 atomics onto `out` (bias added by split 0)
   int w_evict_last;           // keep the B (weight) tiles in L2: the per-step decoder GEMMs re-read them every step
-  int half_w, half_h;         // MC=1 conv: box offset of the second half of the A tile (one of them is 0)
   long long* dbg;             // optional: clock64 stamps of CTA (0,0,0) at the pipeline milestones (lo_debug_buffer)
+};
+
+// the 3x3 convolution: GEMM view M = output positions, N = Cout, K = 9 * Cin
+struct ConvParams {
+  int N, K;
+  int Cin, pad, Ho, Wo;                 // output H, W
+  int BW, BH, tiles_w, tiles_h;         // position box (BW * BH = 128) and boxes per output row / column
+  const float* bias;
+  const bf16* mask;                     // optional: outputs where mask <= 0 are 0 (the data gradient's ReLU mask)
+  bf16* out;
+  int64_t ldc;
+  int relu;
 };
 
 constexpr int TC_BM = 128, TC_BK = 64;
@@ -134,9 +138,9 @@ __device__ __forceinline__ void tc_mma_kblock(float* acc, uint32_t sa, uint32_t 
     Wgmma<NT, 0, 0>::mma(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (first && k == 0) ? 0u : 1u);
 }
 
-// bias (+ReLU) (+bf16 mask) epilogue of two adjacent accumulator columns of one output row, written to bf16 or fp32;
+// bias (+ReLU) epilogue of two adjacent accumulator columns of one output row, written to bf16 or fp32;
 // `atomic` adds onto fp32 (split-K partial sums)
-__device__ __forceinline__ void tc_store_pair(const TcParams& p, int64_t off, float f0, float f1, bool use_mask) {
+__device__ __forceinline__ void tc_store_pair(const TcParams& p, int64_t off, float f0, float f1) {
   if (p.atomic) {
     float* o = reinterpret_cast<float*>(p.out) + off;
     atomicAdd(o, f0);
@@ -150,21 +154,16 @@ __device__ __forceinline__ void tc_store_pair(const TcParams& p, int64_t off, fl
     uint32_t* o = reinterpret_cast<uint32_t*>(reinterpret_cast<bf16*>(p.out) + off);
     if (p.accumulate) { const uint32_t old = *o; f0 += __uint_as_float(old << 16); f1 += __uint_as_float(old & 0xffff0000u); }
     if (p.relu) { f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f); }
-    if (use_mask) {
-      const uint32_t w = *reinterpret_cast<const uint32_t*>(p.mask + off);
-      if (!(__uint_as_float(w << 16) > 0.f)) f0 = 0.f;
-      if (!(__uint_as_float(w & 0xffff0000u) > 0.f)) f1 = 0.f;
-    }
     __nv_bfloat162 h = __floats2bfloat162_rn(f0, f1);
     *o = *reinterpret_cast<uint32_t*>(&h);
   }
 }
 
 // MC = 1: the two CTAs of a (2,1,1) cluster compute neighbouring N tiles of the SAME 128-row A tile; each loads one
-// 64-row half of A and multicasts it to both (halves the L2 -> SM traffic of A).  mapA then describes HALF boxes.
+// 64-row half of A and multicasts it to both (halves the L2 -> SM traffic of A).  mapA then describes 64-row boxes.
 template <int NT, int STAGES, int MC>
-__global__ void __launch_bounds__(TC_THREADS, 1) tc_gemm_conv_kernel(const __grid_constant__ CUtensorMap mapA,
-                                                                      const __grid_constant__ CUtensorMap mapB, TcParams p) {
+__global__ void __launch_bounds__(TC_THREADS, 1) tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA,
+                                                                 const __grid_constant__ CUtensorMap mapB, TcParams p) {
   using SM = TcSmem<NT, STAGES>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -174,20 +173,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_gemm_conv_kernel(const __gri
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n0 = blockIdx.x * NT;
-  const int mt = blockIdx.y;
+  const int m0 = blockIdx.y * TC_BM;
   const int KB_all = p.K / TC_BK;
   const int kb0 = blockIdx.z * p.kb_per_split;
   const int KB = min(KB_all, kb0 + p.kb_per_split) - kb0;      // K blocks of this split
-
-  // tile origin
-  int img = 0, h0 = 0, w0 = 0, m0 = mt * TC_BM;
-  if (p.conv) {
-    const int per_img = p.tiles_w * p.tiles_h;
-    img = mt / per_img;
-    const int rem = mt % per_img;
-    h0 = (rem / p.tiles_w) * p.BH;
-    w0 = (rem % p.tiles_w) * p.BW;
-  }
 
   const bool dbg = p.dbg && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0;
   if (dbg && threadIdx.x == 0) p.dbg[0] = clock64();
@@ -209,7 +198,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_gemm_conv_kernel(const __gri
   if (warp == TC_CWARPS) {
     if (lane == 0) {
       // ===== TMA producer, A tiles =====
-      const int cpb = p.conv ? p.Cin / TC_BK : 1;
       for (int kb = 0; kb < KB; kb++) {
         const int s = kb % STAGES;
         const uint32_t ph = (kb / STAGES) & 1;
@@ -217,23 +205,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_gemm_conv_kernel(const __gri
         uint8_t* sa = smem + s * SM::STAGE_BYTES;
         mbar_expect_tx(full_bar + s, SM::A_BYTES);
         const int kg = kb0 + kb;
-        if (MC) {
-          uint8_t* sh = sa + crank * (SM::A_BYTES / 2);        // my half of the tile, delivered to both CTAs
-          if (p.conv) {
-            const int tap = kg / cpb, cb = kg % cpb;
-            const int r = tap / 3, q = tap % 3;
-            tma_load_4d_mc(sh, &mapA, full_bar + s, cb * TC_BK, w0 + (int)crank * p.half_w + q - p.pad,
-                           h0 + (int)crank * p.half_h + r - p.pad, img, (uint16_t)3);
-          } else {
-            tma_load_2d_mc(sh, &mapA, full_bar + s, kg * TC_BK, m0 + (int)crank * (TC_BM / 2), (uint16_t)3);
-          }
-        } else if (p.conv) {
-          const int tap = kg / cpb, cb = kg % cpb;
-          const int r = tap / 3, q = tap % 3;
-          tma_load_4d(sa, &mapA, full_bar + s, cb * TC_BK, w0 + q - p.pad, h0 + r - p.pad, img);
-        } else {
+        if (MC)        // my half of the tile, delivered to both CTAs
+          tma_load_2d_mc(sa + crank * (SM::A_BYTES / 2), &mapA, full_bar + s, kg * TC_BK, m0 + (int)crank * (TC_BM / 2), (uint16_t)3);
+        else
           tma_load_2d(sa, &mapA, full_bar + s, kg * TC_BK, m0);
-        }
         if (dbg && kb == 0) p.dbg[2] = clock64();
         if (dbg && kb < 40) p.dbg[64 + kb] = clock64();          // A-producer: TMA of K block kb issued
       }
@@ -283,26 +258,16 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_gemm_conv_kernel(const __gri
     // ===== epilogue from the accumulators (layout: lo_wgmma.cuh) =====
     const int rbase = wg * 64 + (warp & 3) * 16 + (lane >> 2);
     const int cq = 2 * (lane & 3);
-    const bool use_mask = p.mask && !p.out_f32 && !p.atomic;
 #pragma unroll
     for (int h = 0; h < 2; h++) {
       const int row = rbase + 8 * h;
-      bool row_ok;
-      int64_t row_off;
-      if (p.conv) {
-        const int hh = h0 + row / p.BW, ww = w0 + row % p.BW;
-        row_ok = (hh < p.Ho) && (ww < p.Wo);
-        row_off = (((int64_t)img * p.Ho + hh) * p.Wo + ww) * p.ldc;
-      } else {
-        row_ok = (m0 + row) < p.M;
-        row_off = (int64_t)(m0 + row) * p.ldc;
-      }
-      if (!row_ok) continue;
+      if (m0 + row >= p.M) continue;
+      const int64_t row_off = (int64_t)(m0 + row) * p.ldc;
 #pragma unroll
       for (int i = 0; i < NT / 8; i++) {
         if (n0 + 8 * i >= p.N) continue;       // 8-column groups: columns up to roundup8(N) are written (ldc allows it)
         const int c = 8 * i + cq;
-        tc_store_pair(p, row_off + n0 + c, acc[4 * i + 2 * h] + s_bias[c], acc[4 * i + 2 * h + 1] + s_bias[c + 1], use_mask);
+        tc_store_pair(p, row_off + n0 + c, acc[4 * i + 2 * h] + s_bias[c], acc[4 * i + 2 * h + 1] + s_bias[c + 1]);
       }
     }
     if (dbg && threadIdx.x == 0) p.dbg[6] = clock64();
@@ -330,7 +295,7 @@ struct TcPSmem {
 // raises the FLOP per L2 byte from 64 to 87 (N = 128) / 43 to 52 (N = 64).
 template <int NT, int STAGES, int MT>
 __global__ void __launch_bounds__(TC_THREADS, 1) tc_conv_p_kernel(const __grid_constant__ CUtensorMap mapA,
-                                                                 const __grid_constant__ CUtensorMap mapB, TcParams p, int ntiles_n,
+                                                                 const __grid_constant__ CUtensorMap mapB, ConvParams p, int ntiles_n,
                                                                  int total_tiles, int mtiles) {
   using SM = TcPSmem<NT, STAGES, MT>;
   static_assert(MT * NT <= 256, "accumulator registers");
@@ -463,7 +428,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_conv_p_kernel(const __grid_c
               if (!(__uint_as_float(w & 0xffff0000u) > 0.f)) f1 = 0.f;
             }
             __nv_bfloat162 hv = __floats2bfloat162_rn(f0, f1);
-            *reinterpret_cast<__nv_bfloat162*>(reinterpret_cast<bf16*>(p.out) + row_off + n0 + c) = hv;
+            *reinterpret_cast<__nv_bfloat162*>(p.out + row_off + n0 + c) = hv;
           }
         }
       }
@@ -705,7 +670,7 @@ static int launch_tc(const CUtensorMap& mA, const CUtensorMap& mB, const TcParam
   using SM = TcSmem<NT, STAGES>;
   static bool attr_set = false;
   if (!attr_set) {
-    LO_CUDA(cudaFuncSetAttribute(tc_gemm_conv_kernel<NT, STAGES, MC>, cudaFuncAttributeMaxDynamicSharedMemorySize, SM::TOTAL));
+    LO_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<NT, STAGES, MC>, cudaFuncAttributeMaxDynamicSharedMemorySize, SM::TOTAL));
     attr_set = true;
   }
   dim3 grid(cdiv(p.N, NT), mtiles, splits);
@@ -730,7 +695,7 @@ static int launch_tc(const CUtensorMap& mA, const CUtensorMap& mB, const TcParam
   }
   cfg.attrs = attr;
   cfg.numAttrs = n;
-  LO_CUDA(cudaLaunchKernelEx(&cfg, tc_gemm_conv_kernel<NT, STAGES, MC>, mA, mB, p));
+  LO_CUDA(cudaLaunchKernelEx(&cfg, tc_gemm_kernel<NT, STAGES, MC>, mA, mB, p));
   LO_LAUNCH_OK();
   return LO_OK;
 }
@@ -772,8 +737,8 @@ int tc_gemm_nt_ex(const bf16* A, int64_t lda, const bf16* W, int64_t ldw, void* 
   }
   LO_CHECK_ARG(!(splits > 1 || atomic_acc) || (dtC == LO_F32 && !relu), "split-K needs fp32 output without ReLU");
   TcParams p{};
-  p.M = M; p.N = N; p.K = K; p.conv = 0;
-  p.bias = bias; p.mask = nullptr; p.out = C; p.ldc = ldc;
+  p.M = M; p.N = N; p.K = K;
+  p.bias = bias; p.out = C; p.ldc = ldc;
   p.out_f32 = (dtC == LO_F32); p.accumulate = accumulate; p.relu = relu; p.atomic = atomic_acc;
   p.w_evict_last = (M <= 128) ? 1 : 0;
   p.dbg = g_tc_dbg;
@@ -786,7 +751,7 @@ int tc_gemm_nt(const bf16* A, int64_t lda, const bf16* W, int64_t ldw, void* C, 
 }
 
 template <int NT, int STAGES, int MT>
-static int launch_conv_p(const CUtensorMap& mA, const CUtensorMap& mB, const TcParams& p, int mtiles, cudaStream_t st) {
+static int launch_conv_p(const CUtensorMap& mA, const CUtensorMap& mB, const ConvParams& p, int mtiles, cudaStream_t st) {
   using SM = TcPSmem<NT, STAGES, MT>;
   static bool attr_set = false;
   static int n_sm = 0;
@@ -813,40 +778,12 @@ int tc_conv3x3(const bf16* x, const bf16* w, const float* bias, const bf16* mask
   int BW = 128;
   while (BW > 8 && BW / 2 >= Wo) BW /= 2;     // smallest power of two >= Wo (capped at 128)
   const int BH = 128 / BW;
-  if (g_opt_conv_persist) {
-    const int NTp = Cout % 256 == 0 ? 256 : (Cout > 64 ? 128 : 64);
-    CUtensorMap mA, mB;
-    {
-      cuuint64_t dims[4] = {(cuuint64_t)Cin, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
-      cuuint64_t str[3] = {(cuuint64_t)Cin * 2, (cuuint64_t)W * Cin * 2, (cuuint64_t)H * W * Cin * 2};
-      cuuint32_t box[4] = {64, (cuuint32_t)BW, (cuuint32_t)BH, 1};
-      LO_TRY(make_map(&mA, x, 4, dims, str, box));
-    }
-    {
-      cuuint64_t dims[2] = {(cuuint64_t)9 * Cin, (cuuint64_t)Cout};
-      cuuint64_t str[1] = {(cuuint64_t)9 * Cin * 2};
-      cuuint32_t box[2] = {64, (cuuint32_t)NTp};
-      LO_TRY(make_map(&mB, w, 2, dims, str, box));
-    }
-    TcParams p{};
-    p.M = N * Ho * Wo; p.N = Cout; p.K = 9 * Cin; p.conv = 1;
-    p.Ho = Ho; p.Wo = Wo; p.Cin = Cin; p.pad = pad;
-    p.BW = BW; p.BH = BH; p.tiles_w = cdiv(Wo, BW); p.tiles_h = cdiv(Ho, BH);
-    p.bias = bias; p.mask = mask; p.out = y; p.ldc = Cout; p.relu = relu;
-    const int mtiles = N * p.tiles_w * p.tiles_h;
-    if (NTp == 256) return launch_conv_p<256, 4, 1>(mA, mB, p, mtiles, st);
-    if (NTp == 128) return g_opt_conv_mt2 ? launch_conv_p<128, 4, 2>(mA, mB, p, mtiles, st) : launch_conv_p<128, 6, 1>(mA, mB, p, mtiles, st);
-    return g_opt_conv_mt2 ? launch_conv_p<64, 4, 2>(mA, mB, p, mtiles, st) : launch_conv_p<64, 8, 1>(mA, mB, p, mtiles, st);
-  }
+  const int NT = Cout % 256 == 0 ? 256 : (Cout > 64 ? 128 : 64);
   CUtensorMap mA, mB;
-  const int NT = Cout <= 64 ? 64 : 128;
-  const int mc = (g_opt_conv_mc && NT == 128 && cdiv(Cout, 128) % 2 == 0) ? 1 : 0;
-  // MC: each CTA of the pair loads one 64-position half of the tile (the first BH/2 rows, or the first BW/2 columns when BH == 1)
-  const int hbw = mc ? (BH >= 2 ? BW : BW / 2) : BW, hbh = mc ? (BH >= 2 ? BH / 2 : 1) : BH;
   {
     cuuint64_t dims[4] = {(cuuint64_t)Cin, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
     cuuint64_t str[3] = {(cuuint64_t)Cin * 2, (cuuint64_t)W * Cin * 2, (cuuint64_t)H * W * Cin * 2};
-    cuuint32_t box[4] = {64, (cuuint32_t)hbw, (cuuint32_t)hbh, 1};
+    cuuint32_t box[4] = {64, (cuuint32_t)BW, (cuuint32_t)BH, 1};
     LO_TRY(make_map(&mA, x, 4, dims, str, box));
   }
   {
@@ -855,18 +792,15 @@ int tc_conv3x3(const bf16* x, const bf16* w, const float* bias, const bf16* mask
     cuuint32_t box[2] = {64, (cuuint32_t)NT};
     LO_TRY(make_map(&mB, w, 2, dims, str, box));
   }
-  TcParams p{};
-  p.M = N * Ho * Wo; p.N = Cout; p.K = 9 * Cin; p.conv = 1;
-  p.Ho = Ho; p.Wo = Wo; p.Cin = Cin; p.pad = pad;
+  ConvParams p{};
+  p.N = Cout; p.K = 9 * Cin;
+  p.Cin = Cin; p.pad = pad; p.Ho = Ho; p.Wo = Wo;
   p.BW = BW; p.BH = BH; p.tiles_w = cdiv(Wo, BW); p.tiles_h = cdiv(Ho, BH);
-  p.bias = bias; p.mask = mask; p.out = y; p.ldc = Cout;
-  p.out_f32 = 0; p.accumulate = 0; p.relu = relu;
-  p.dbg = g_tc_dbg;
-  p.half_w = (mc && BH < 2) ? BW / 2 : 0;
-  p.half_h = (mc && BH >= 2) ? BH / 2 : 0;
+  p.bias = bias; p.mask = mask; p.out = y; p.ldc = Cout; p.relu = relu;
   const int mtiles = N * p.tiles_w * p.tiles_h;
-  LO_CHECK_ARG(mtiles <= 65535, "too many M tiles for grid.y");
-  return launch_tc_any(mA, mB, p, mtiles, 1, NT, st, mc);
+  if (NT == 256) return launch_conv_p<256, 4, 1>(mA, mB, p, mtiles, st);
+  if (NT == 128) return launch_conv_p<128, 4, 2>(mA, mB, p, mtiles, st);
+  return launch_conv_p<64, 4, 2>(mA, mB, p, mtiles, st);
 }
 
 

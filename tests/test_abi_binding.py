@@ -66,7 +66,7 @@ for n in names:
         out["roundtrip"].setdefault(n, []).append([L.lo_set_option(n.encode(), v), get(n)])
     L.lo_set_option(n.encode(), out["defaults"][n])
 out["unknown"] = {}
-for n in ("no_such_option", "fuse_lstm", "dec_streams"):
+for n in ("no_such_option", "fuse_lstm", "dec_streams", "conv_persist", "conv_mt2"):
     rc = L.lo_set_option(n.encode(), 1)
     out["unknown"][n] = [rc, L.lo_last_error().decode(), get(n)]
 print(json.dumps(out))
@@ -85,7 +85,7 @@ def probe():
 
 def test_the_library_has_exactly_the_documented_options(probe):
     documented = _documented_options()
-    assert len(documented) >= 18
+    assert len(documented) >= 16
     assert probe["names"] == list(documented)
     assert probe["defaults"] == documented
 
@@ -97,8 +97,9 @@ def test_every_stored_option_reads_back_what_was_set(probe):
 
 
 def test_unknown_option_is_refused(probe):
-    # fuse_lstm and dec_streams were options until their schedules were removed: an LO_OPTS that still names one fails on load
-    assert sorted(probe["unknown"]) == ["dec_streams", "fuse_lstm", "no_such_option"]
+    # fuse_lstm, dec_streams, conv_persist and conv_mt2 were options until their schedules were removed: an LO_OPTS that still
+    # names one fails on load
+    assert sorted(probe["unknown"]) == ["conv_mt2", "conv_persist", "dec_streams", "fuse_lstm", "no_such_option"]
     for name, (rc, err, got) in probe["unknown"].items():
         assert rc == -1, name                                          # LO_EINVAL
         assert name in err

@@ -99,8 +99,8 @@ def test_tc_conv3x3_wgrad(N, H, W, Cin, Cout, pad):
     assert relerr(db, dy.double().sum(dim=(0, 2, 3)).float()) < 1e-5
 
 
-_SCHEDULE_OPTS = {"skinny_mma": (1, 0), "att_maskbits": (1, 0), "conv_persist": (1, 0), "wgrad256": (0, 1), "conv_mt2": (1, 0),
-                  "conv_mc": (1, 0), "att_bwd_mma": (1, 0), "skinny_tma": (1, 0)}
+_SCHEDULE_OPTS = {"skinny_mma": (1, 0), "att_maskbits": (1, 0), "wgrad256": (0, 1), "conv_mc": (1, 0), "att_bwd_mma": (1, 0),
+                  "skinny_tma": (1, 0)}
 
 
 @pytest.mark.parametrize("opt", sorted(_SCHEDULE_OPTS))

@@ -676,6 +676,33 @@ int64_t lo_lstm_seq_workspace_bytes(const lo_lstm_seq_args* a);
 int lo_lstm_seq_forward(const lo_lstm_seq_args* a, void* stream);
 int lo_lstm_seq_backward(const lo_lstm_seq_args* a, void* stream);
 
+/* EXTENSION: greedy and beam decode of the two-layer decoder (oracle/ref_ext.py decoder2_forward, no dropout at decode time).
+ * Layer 1 is the attention LSTM of lo_decoder_args, started from init_hidden_state of enc; layer 2 is nn.LSTMCell(D, D) over
+ * h1_t from a zero state (h2 = c2 = 0); logits_t = fc(h2_t).  The token and finish rules, the outputs, images of different sizes
+ * (reg_off / reg_off_host), the diversity penalty and the penalties of lo_beam_penalty are those of lo_decoder_greedy_hist and
+ * lo_decoder_beam_pen; lo_beam_backtrack reads the results unchanged (attention rows in a->alphas).  Layer 2 runs per step as
+ * two GEMMs on the step-GEMM dispatcher of layer 1 (one K slice each: a bf16 decode repeats its bits), one cell launch and the
+ * head on h2.  Its state lives in `scratch` (two slots of h2 / c2, their bf16 mirror, the gate pre-activations).
+ *   w_ih, w_hh   [4D][D] in the args' storage dtype `dt` (gate order i, f, g, o)
+ *   b_ih, b_hh   fp32 [4D]
+ *   scratch      device, lo_decoder2_scratch_bytes(a) bytes (depends on a->B and a->D only)
+ * Refused (LO_EINVAL) before any GPU work: a null layer, a null weight, bias or scratch, phase != 0, ss_prob, and every refusal
+ * of lo_decoder_greedy_hist / lo_decoder_beam_pen (pen NULL: no penalty, as lo_decoder_beam_div). */
+typedef struct lo_decoder2_layer {
+  const void* w_ih;
+  const void* w_hh;
+  const float* b_ih;
+  const float* b_hh;
+  void* scratch;
+} lo_decoder2_layer;
+int64_t lo_sizeof_decoder2_layer(void);
+int64_t lo_decoder2_scratch_bytes(const lo_decoder_args* a);
+int lo_decoder2_greedy(const lo_decoder_args* a, const lo_decoder2_layer* l2, int64_t start_id, int64_t end_id, int max_steps,
+                       int64_t* tokens, int32_t* finished, int32_t* fin_hist, void* stream);
+int lo_decoder2_beam(const lo_decoder_args* a, const lo_decoder2_layer* l2, int64_t start_id, int64_t end_id, int max_steps,
+                     int64_t* ids, int64_t* parents, int32_t* fin_hist, float* logp, float div_gamma, float div_prob,
+                     const float* div_u, const uint64_t* div_state, const lo_beam_penalty* pen, void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Optimiser: torch.optim.Adam defaults (img2seq_torch.py:86-87, :168-170) on one flat buffer.
  * state_dev: float[2] = {step (as float), lr}; step is incremented on the device so the call is

@@ -1705,15 +1705,17 @@ struct TorchDecode {
   }
 };
 
-// both beam entry points of the torch flavour (bm.beam is set here from rows_per_img)
+// the beam entry points of the torch flavour and of the two-layer decoder (F: TorchDecode or TwoLayerDecode, built with `extra`
+// after its TorchDecode arguments; bm.beam is set here from rows_per_img)
+template <class F = TorchDecode, class... X>
 static int decoder_beam(const lo_decoder_args* a, int64_t start_id, int64_t end_id, int max_steps, int64_t* ids, int64_t* parents,
-                        int32_t* fin_hist, float* logp, BeamArgs bm, void* stream) {
+                        int32_t* fin_hist, float* logp, BeamArgs bm, void* stream, X... extra) {
   LO_TRY(check_args(a));
   LO_TRY(check_reg_off(a, true));
   LO_CHECK_ARG(!a->ss_prob, "scheduled sampling (ss_prob) is a training mode: not available in beam search");
   LO_CHECK_ARG((int64_t)a->B * a->T >= 2 * a->B, "row_loss scratch too small");
   int32_t* finished = (int32_t*)a->row_loss;
-  TorchDecode f(a, start_id, finished, finished + a->B);
+  F f(a, start_id, finished, finished + a->B, extra...);
   bm.beam = a->rows_per_img;
   return beam_loop(f, bm, end_id, max_steps, ids, parents, fin_hist, logp, (cudaStream_t)stream);
 }
@@ -2232,3 +2234,5 @@ int lo_beam_backtrack(const int64_t* ids, const int64_t* parents, int64_t ids_st
 #include "lo_tfdecoder.cuh"
 // generic sequence LSTM (extension: row-encoder biLSTM, second decoder layer)
 #include "lo_lstmseq.cuh"
+// greedy / beam decode of the two-layer decoder (extension): a third flavour of the decode loops above
+#include "lo_decoder2.cuh"

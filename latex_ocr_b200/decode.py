@@ -185,19 +185,22 @@ def ragged_layout(images, out_hw):
     return RaggedLayout(imgs, order, groups, counts, region_offsets(counts))
 
 
-def encode_packed(encoder, lay, enc, device):
+def encode_packed(encoder, lay, enc, device, encode=None):
     """Runs ``encoder`` once per shape group of ``lay`` and writes its output into the packed ``enc`` [regions, C] in decode
-    order."""
+    order.  ``encode(encoder_out)``: optional, applied to each group's encoder output [n, H', W', C] before it is packed (the row
+    encoder of ext.Img2SeqRowModel); its result has the same shape."""
     imgs, order, off = lay.imgs, lay.order, lay.off
     for j0, j1 in lay.groups:
         batch = torch.stack([imgs[order[j]] for j in range(j0, j1)]).to(device)
         e = encoder.forward_raw(batch if batch.dtype == torch.uint8 else batch.float(), need_grad=False)
+        if encode is not None:
+            e = encode(e)
         enc[off[j0]:off[j1]].copy_(e.reshape(off[j1] - off[j0], e.shape[3]))
 
 
-def _prepare(model, img, rows_per_img, max_steps):
+def _prepare(model, img, rows_per_img, max_steps, encode=None):
     """Encoder output and the argument block of a decode of ``img``: a batch tensor, or a list of images of different sizes packed
-    by ragged_layout.  Returns (args, workspace, N, the RaggedLayout of a list or None)."""
+    by ragged_layout.  ``encode``: as in encode_packed.  Returns (args, workspace, N, the RaggedLayout of a list or None)."""
     dec = model.decoder
     lay = None
     if isinstance(img, (list, tuple)):
@@ -205,9 +208,11 @@ def _prepare(model, img, rows_per_img, max_steps):
         N, R = len(lay.order), max(lay.counts)
         ws = dec.ragged_workspace(N * rows_per_img, max_steps, R, lay.off[-1])
         enc = ws["t"]["enc"]
-        encode_packed(model.encoder, lay, enc, model.device)
+        encode_packed(model.encoder, lay, enc, model.device, encode)
     else:
         enc = model.encoder.forward_raw(img.to(model.device).float(), need_grad=False)
+        if encode is not None:
+            enc = encode(enc)
         N, R = enc.shape[0], enc.shape[1] * enc.shape[2]
         enc = enc.view(N, R, enc.shape[3])
         ws = dec.workspace(N * rows_per_img, max_steps, R, need_grad=False)
@@ -229,18 +234,31 @@ def _inverse(order):
     return torch.tensor(inv, dtype=torch.int64)
 
 
-def greedy_decode(model, img, start_id, end_id, max_length_formula=150, return_attention=False):
+def _greedy_entry(a, *args):
+    return _lib.lib().lo_decoder_greedy_hist(ctypes.byref(a), *args)
+
+
+def _beam_entry(a, pen, *args):
+    L = _lib.lib()
+    if pen is not None:
+        return L.lo_decoder_beam_pen(ctypes.byref(a), *args[:-1], ctypes.byref(pen), args[-1])
+    return L.lo_decoder_beam_div(ctypes.byref(a), *args)
+
+
+def greedy_decode(model, img, start_id, end_id, max_length_formula=150, return_attention=False, _encode=None, _entry=_greedy_entry):
     """Returns token ids [N, steps] (CPU int64), steps as the reference's loop would have run.  ``return_attention=True`` also
     returns the attention weights of every step, [N, steps, R] fp32 on the CPU — what the reference collects in
     ``attention_mechanism.ctx_vector`` for visualize_attention.py (attention_mechanism.py:96-121).  For a list of images the ids
-    are in input order and the attention weights are a list of [steps, R_i] tensors, R_i the image's own region count."""
-    L = _lib.lib()
+    are in input order and the attention weights are a list of [steps, R_i] tensors, R_i the image's own region count.
+
+    ``_encode`` (see encode_packed) and ``_entry(args, start_id, end_id, max_steps, tokens, finished, fin_hist, stream)``, the
+    library call, let ext.greedy_decode run the two-layer decoder through this body."""
     max_steps = max_length_formula + 2
     with torch.no_grad():
-        a, ws, N, lay = _prepare(model, img, 1, max_steps)
+        a, ws, N, lay = _prepare(model, img, 1, max_steps, _encode)
         finished = torch.zeros(N, dtype=torch.int32, device=model.device)
-        ids = run_greedy(lambda tokens, hist: L.lo_decoder_greedy_hist(ctypes.byref(a), int(start_id), int(end_id), max_steps, tokens,
-                                                                      finished.data_ptr(), hist, stream_ptr()),
+        ids = run_greedy(lambda tokens, hist: _entry(a, int(start_id), int(end_id), max_steps, tokens, finished.data_ptr(), hist,
+                                                     stream_ptr()),
                          N, max_steps, model.device).cpu()
         n = ids.shape[1]
         if lay is None:
@@ -263,7 +281,7 @@ def attention_maps(alphas, att_h, att_w):
 
 def beam_decode(model, img, start_id, end_id, beam_size=5, max_length_formula=150, finalize="reference",
                 div_gamma=1, div_prob=0, div_u=None, div_seed=None, return_attention=False, length_penalty=0.0,
-                coverage_penalty=0.0, return_scores=False):
+                coverage_penalty=0.0, return_scores=False, _encode=None, _entry=_beam_entry):
     """Returns (ids [N, beam, steps], log_probs [N, beam]) on the CPU; hypothesis 0 is the one the reference scores
     (img2seq.py:210).  ``div_gamma`` / ``div_prob``: the diversity penalty of beam_search_decoder_cell.py:258-287 (off when
     gamma == 1 or prob == 0, as in configs/model.json:15-16); its Bernoulli draws come from the in-kernel Philox stream seeded
@@ -279,14 +297,17 @@ def beam_decode(model, img, start_id, end_id, beam_size=5, max_length_formula=15
     documents — the search ranks hypotheses by log_probs / ((5 + length) / 6) ** alpha + beta * sum_r ln(min(coverage_r, 1)), the
     coverage being the attention summed along the hypothesis.  Both default to 0, the reference's search.  The log-probs returned
     stay the raw sums; ``return_scores=True`` also returns the ranking scores [N, beam] (CPU), after the log-probs and before the
-    attention weights."""
+    attention weights.
+
+    ``_encode`` (see encode_packed) and ``_entry(args, penalty or None, start_id, end_id, max_steps, ids, parents, fin_hist, logp,
+    div_gamma, div_prob, div_u, div_state, stream)``, the library call, let ext.beam_decode run the two-layer decoder through this
+    body."""
     if finalize not in ("reference", "backtrack"):
         raise NotImplementedError("finalize must be 'reference' or 'backtrack'")
     alpha, beta = penalty_weights(length_penalty, coverage_penalty)
-    L = _lib.lib()
     max_steps = max_length_formula + 2
     with torch.no_grad():
-        a, ws, N, lay = _prepare(model, img, beam_size, max_steps)
+        a, ws, N, lay = _prepare(model, img, beam_size, max_steps, _encode)
         dev = model.device
         div_on = not (div_gamma == 1 or div_prob == 0)
         state = None
@@ -299,11 +320,8 @@ def beam_decode(model, img, start_id, end_id, beam_size=5, max_length_formula=15
             pen, pen_t = beam_penalty(alpha, beta, a.B, a.R, max_steps, beam_size, dev)
 
         def call(ids, parents, hist, logp, u):
-            args = (ctypes.byref(a), int(start_id), int(end_id), max_steps, ids, parents, hist, logp, float(div_gamma), float(div_prob), u,
-                    state.data_ptr() if state is not None else None)
-            if pen is not None:
-                return L.lo_decoder_beam_pen(*args, ctypes.byref(pen), stream_ptr())
-            return L.lo_decoder_beam_div(*args, stream_ptr())
+            return _entry(a, pen, int(start_id), int(end_id), max_steps, ids, parents, hist, logp, float(div_gamma), float(div_prob), u,
+                          state.data_ptr() if state is not None else None, stream_ptr())
         ids, parents, logp = run_beam(call, N, beam_size, max_steps, a.V, dev, div_u if div_on else None,
                                       lay.order if lay else None)
         scores = pen_t["scores"].cpu() if return_scores else None

@@ -14,6 +14,9 @@ is no reference code to restate; semantics are defined HERE and checked against 
 Both LSTMs run on ``lo_lstm_seq_forward/backward`` (csrc/lo_lstmseq.cuh): hoisted input projection, one recurrent GEMM + one cell
 kernel per step, hand-derived backward with hoisted weight gradients.
 
+Decoding: ``greedy_decode`` / ``beam_decode`` below run CNN -> RowEncoder -> both decoder layers in one CUDA time loop
+(``lo_decoder2_greedy`` / ``lo_decoder2_beam``, csrc/lo_decoder2.cuh) through the bodies of decode.greedy_decode / beam_decode.
+
 Autograd: ``RowEncoder.forward`` and ``TwoLayerDecoder.forward`` (``Img2SeqRowModel.decoder2``) record a graph when grad mode is on
 and an input or a parameter requires grad, so the whole extension trains through ``loss.backward()`` and ``torch.optim`` with any
 loss of the predictions and alphas; the fused ``Img2SeqRowModel.train_step`` is unchanged.
@@ -24,7 +27,7 @@ import math
 import torch
 import torch.nn as nn
 
-from . import _lib
+from . import _lib, decode
 from ._lib import LstmSeqArgs, check, dtype_code, impl_code, stream_ptr
 from .img2seq import Img2SeqModel
 from .kernel_module import kernel_forward, stamp
@@ -185,6 +188,22 @@ class DecoderLayer2(nn.Module):
             for p_ in self.cell.parameters():
                 p_.uniform_(-b, b)
         self._x = LRUCache()
+        self._scratch = LRUCache()
+
+    def decode_layer(self, a):
+        """The lo_decoder2_layer of a decode with the decoder args ``a``: the weights in storage dtype (bf16 shadow refreshed), the
+        fp32 biases and a scratch buffer of lo_decoder2_scratch_bytes(a) bytes, cached per size.  The struct points at the store and
+        the cache: it is valid until the next call that changes either."""
+        self.store.refresh_shadow()
+        nbytes = int(_lib.lib().lo_decoder2_scratch_bytes(ctypes.byref(a)))
+        scratch = self._scratch.get(nbytes)
+        if scratch is None:
+            scratch = self._scratch[nbytes] = torch.empty(nbytes, dtype=torch.uint8, device=self.store.device)
+        l2 = _lib.Decoder2Layer()
+        l2.w_ih, l2.w_hh = self.store.w("cell.weight_ih").data_ptr(), self.store.w("cell.weight_hh").data_ptr()
+        l2.b_ih, l2.b_hh = self.store.f32("cell.bias_ih").data_ptr(), self.store.f32("cell.bias_hh").data_ptr()
+        l2.scratch = scratch.data_ptr()
+        return l2
 
     def forward_inplace(self, hd):
         """hd: fp32 [B,T,D] (dropout(h1), batch-major) — replaced IN PLACE by h2.  Returns the cache entries it wrote (layer
@@ -274,7 +293,8 @@ class TwoLayerDecoder(nn.Module):
 
 class Img2SeqRowModel(Img2SeqModel):
     """EncoderCNN -> RowEncoder -> attention decoder with a second LSTM layer (extension).  Same trainer surface as
-    Img2SeqModel (getLoss / train_step / train / ...); decoding (predict_batch) is not offered for this variant.  Through
+    Img2SeqModel (getLoss / train_step / train / ...); predict_batch is not offered for this variant: it decodes through
+    ext.greedy_decode / ext.beam_decode.  Through
     autograd: ``decoder2(row_encoder(encoder(img)), formula, lengths)`` -> any loss -> ``backward()``."""
 
     def getModel(self, model_name="Img2Seq"):
@@ -355,3 +375,31 @@ class Img2SeqRowModel(Img2SeqModel):
         super().load_state_dict(sd)
         self.row_encoder.load_state_dict(sd["row_encoder"])
         self.layer2.load_state_dict(sd["layer2"])
+
+
+# ------------------------------------------------------------------------------------------------ decoding
+def _row_encode(model):
+    """The row encoder as decode.encode_packed's ``encode``: CNN output [n,H',W',512] -> row encoding of the same shape."""
+    return model.row_encoder.forward_raw
+
+
+def greedy_decode(model, img, start_id, end_id, max_length_formula=150, return_attention=False):
+    """Greedy decode of an Img2SeqRowModel: CNN -> row encoder -> two-layer decoder (layer 2 over h1_t, logits = fc(h2_t)) in one
+    CUDA time loop (lo_decoder2_greedy).  Arguments, outputs and loop rules are those of decode.greedy_decode: ``img`` a batch
+    tensor or a list of images of different sizes, the attention weights of layer 1 with ``return_attention``."""
+    def entry(a, *args):
+        l2 = model.layer2.decode_layer(a)
+        return _lib.lib().lo_decoder2_greedy(ctypes.byref(a), ctypes.byref(l2), *args)
+    return decode.greedy_decode(model, img, start_id, end_id, max_length_formula, return_attention, _encode=_row_encode(model),
+                                _entry=entry)
+
+
+def beam_decode(model, img, start_id, end_id, beam_size=5, **kw):
+    """Beam search of an Img2SeqRowModel through the row encoder and the two-layer decoder (lo_decoder2_beam).  Keywords and return
+    values are those of decode.beam_decode: max_length_formula, finalize, div_gamma / div_prob / div_u / div_seed,
+    length_penalty / coverage_penalty, return_scores, return_attention."""
+    def entry(a, pen, *args):
+        l2 = model.layer2.decode_layer(a)
+        return _lib.lib().lo_decoder2_beam(ctypes.byref(a), ctypes.byref(l2), *args[:-1],
+                                           ctypes.byref(pen) if pen is not None else None, args[-1])
+    return decode.beam_decode(model, img, start_id, end_id, beam_size, _encode=_row_encode(model), _entry=entry, **kw)

@@ -407,6 +407,42 @@ int lo_decoder_greedy(const lo_decoder_args* a, int64_t start_id, int64_t end_id
 int lo_decoder_greedy_hist(const lo_decoder_args* a, int64_t start_id, int64_t end_id, int max_steps,
                            int64_t* tokens, int32_t* finished, int32_t* fin_hist, void* stream);
 
+/* Sampling decode (lo_decoder_sample, lo_tfdec_sample, lo_decoder2_sample): the greedy loop of the flavour with every step's token
+ * drawn instead of taken as the argmax, rows_per_img = n consecutive rows (n samples) sharing one image.  Row b of step t, with
+ * logits x [V]:
+ *   q = softmax(x / tau); the tokens in the order (q descending, index ascending)
+ *   top_k >= 1 keeps the first top_k tokens of that order (0: off); top_p < 1 keeps token v iff the mass of the tokens before v
+ *   is < top_p (1: off), so the most probable token is always kept; with both set a token must pass both
+ *   token = argmax over the kept v of (x_v / tau + g_v), g_v = -log(-log u_v), the lowest index among equals: one draw from q
+ *   renormalised over the kept set (Gumbel-max).  u_v: u[t][b][v] when u is given, else ((w >> 8) + 0.5) * 2^-24, w word
+ *   (v & 3) of Philox4x32-10(counter = (0x80000000 | v >> 2, t, b, call), key = seed) of the device state {seed, call} — the
+ *   stream of lo_decoder_args.ss_gu's Philox uniforms (host mirror: philox.gumbel_uniforms).
+ * The token goes to tokens[b][t] and is fed to step t + 1; a row is finished after its first end_id, and from then on emits end_id
+ * and adds nothing.  logp[b] = the sum over the row's tokens through its first end_id of log_softmax(x)[token] at temperature 1,
+ * unfiltered: the model's log-likelihood of the sample, comparable with beam search's logp.  fin_hist, finished, images of
+ * different sizes (reg_off) and the outputs are those of the flavour's greedy entry point.  With `state`, the call adds 1 to
+ * state[1] after its last step, so the next call draws new uniforms.
+ *   tau      temperature, finite and > 0
+ *   top_k    0..V
+ *   top_p    (0, 1]
+ *   u        optional device fp32 [max_steps][B][V] in (0, 1) (tests); NULL: Philox from state
+ *   state    device {seed, call} (needed without u)
+ *   logp     device fp32 out [B]
+ * Refused (LO_EINVAL) before any GPU work: a null struct, tau not finite or <= 0, top_k outside 0..V, top_p outside (0, 1], neither
+ * u nor state, a null logp, rows_per_img outside 1..16, V above 2048 (the shared-memory sort of a row, 12 bytes per entry), any
+ * ss_* field of the args, and every refusal of the flavour's greedy entry point. */
+typedef struct lo_sample_args {
+  float tau;
+  int32_t top_k;
+  float top_p;
+  const float* u;
+  uint64_t* state;
+  float* logp;
+} lo_sample_args;
+int64_t lo_sizeof_sample_args(void);
+int lo_decoder_sample(const lo_decoder_args* a, const lo_sample_args* s, int64_t start_id, int64_t end_id, int max_steps,
+                      int64_t* tokens, int32_t* finished, int32_t* fin_hist, void* stream);
+
 /* beam search on the same step kernels: beam_search_decoder_cell.py:98-187 (log-softmax, finished mask with
  * dtype.min, only beam 0 at time 0, top-k over beam*V with the lower index winning ties, state gather by parents;
  * no length normalisation (lo_decoder_beam_pen adds it), diversity penalty off as in configs/model.json:15-16).  a->B = n_img*beam rows,
@@ -628,6 +664,9 @@ int lo_tfdec_backward(const lo_tfdec_args* a, void* stream);
 /* greedy decode (greedy_decoder_cell.py:38-66 + dynamic_decode.py:38-61): tokens [B][max_steps], fin_hist (optional)
  * [B][max_steps] finished flags after each step; max_steps <= T */
 int lo_tfdec_greedy(const lo_tfdec_args* a, int64_t end_id, int max_steps, int64_t* tokens, int32_t* fin_hist, void* stream);
+/* sampling decode (see lo_sample_args): tokens [B][max_steps], fin_hist (optional) as lo_tfdec_greedy */
+int lo_tfdec_sample(const lo_tfdec_args* a, const lo_sample_args* s, int64_t end_id, int max_steps, int64_t* tokens, int32_t* fin_hist,
+                    void* stream);
 /* beam search (beam_search_decoder_cell.py:98-187): B = n_img*beam rows, rows_per_img = beam; ids/parents/fin_hist
  * [n_img][max_steps][beam], logp [n_img][beam] */
 int lo_tfdec_beam(const lo_tfdec_args* a, int64_t end_id, int max_steps, int64_t* ids, int64_t* parents, int32_t* fin_hist,
@@ -699,6 +738,9 @@ int64_t lo_sizeof_decoder2_layer(void);
 int64_t lo_decoder2_scratch_bytes(const lo_decoder_args* a);
 int lo_decoder2_greedy(const lo_decoder_args* a, const lo_decoder2_layer* l2, int64_t start_id, int64_t end_id, int max_steps,
                        int64_t* tokens, int32_t* finished, int32_t* fin_hist, void* stream);
+/* sampling decode of the two-layer decoder (see lo_sample_args), with the refusals of lo_decoder2_greedy */
+int lo_decoder2_sample(const lo_decoder_args* a, const lo_decoder2_layer* l2, const lo_sample_args* s, int64_t start_id, int64_t end_id,
+                       int max_steps, int64_t* tokens, int32_t* finished, int32_t* fin_hist, void* stream);
 int lo_decoder2_beam(const lo_decoder_args* a, const lo_decoder2_layer* l2, int64_t start_id, int64_t end_id, int max_steps,
                      int64_t* ids, int64_t* parents, int32_t* fin_hist, float* logp, float div_gamma, float div_prob,
                      const float* div_u, const uint64_t* div_state, const lo_beam_penalty* pen, void* stream);

@@ -457,6 +457,17 @@ __device__ __forceinline__ float neg_log_u24(uint32_t x) {
   return -log1pf(-(((float)((1u << 24) - 1u - m) + 0.5f) * (1.0f / 16777216.0f)));
 }
 
+// The Gumbel-max draw of scheduled sampling with a temperature (ss_block_tokens) and of sampling decode (sample_step_kernel):
+// argmax_v (x_v / tau + g_v), g_v = -log(-log u_v).  Philox uniforms: u_v from word v & 3 of gumbel_words(v >> 2, t, b) under the
+// device state {seed, call}, counter (0x80000000 | v >> 2, t, b, call): a first counter word neither the dropout stream
+// (j >> 2 < 2^31) nor the coin (0xFFFFFFFF) uses.  Host mirror: philox.gumbel_uniforms.
+__device__ __forceinline__ uint4 gumbel_words(int v4, int t, int b, unsigned long long seed, unsigned long long call) {
+  return philox4x32_10(make_uint4(0x80000000u | (uint32_t)v4, (uint32_t)t, (uint32_t)b, (uint32_t)call),
+                       make_uint2((uint32_t)seed, (uint32_t)(seed >> 32)));
+}
+// the score of logit x for Philox word w (an injected uniform u scores x / tau - log(-log u))
+__device__ __forceinline__ float gumbel_score(float x, float tau, uint32_t w) { return x / tau - logf(neg_log_u24(w)); }
+
 // Scheduled sampling (lo_decoder_args.ss_prob, lo_tfdec_args.ss_prob), shared by the pointwise LSTM kernels of both decoder
 // flavours: the token each row of a 256-thread block of a [nrows][D] launch feeds at this step, chosen and recorded once per row by
 // one warp and handed to the row's threads through shared memory.  tok: the teacher tokens (rows tok_stride apart).  Where the coin
@@ -496,18 +507,15 @@ __device__ __forceinline__ void ss_block_tokens(const int64_t* __restrict__ tok,
               if (x > best) { best = x; bi = v; }
             }
           } else {
-            // u_v from word v & 3 of Philox4x32-10(counter = (0x80000000 | v >> 2, t, b, call)): a first counter word neither
-            // the dropout stream (j >> 2 < 2^31) nor the coin (0xFFFFFFFF) uses
             const unsigned long long seed = ss.coin_state[0], call = ss.coin_state[1];
             for (int v4 = lane; v4 * 4 < V; v4 += 32) {
-              const uint4 w = philox4x32_10(make_uint4(0x80000000u | (uint32_t)v4, (uint32_t)t_idx, (uint32_t)(row0 + r), (uint32_t)call),
-                                            make_uint2((uint32_t)seed, (uint32_t)(seed >> 32)));
+              const uint4 w = gumbel_words(v4, t_idx, row0 + r, seed, call);
               const uint32_t ws[4] = {w.x, w.y, w.z, w.w};
 #pragma unroll
               for (int q = 0; q < 4; q++) {
                 const int v = v4 * 4 + q;
                 if (v < V) {
-                  const float x = lg[v] / tau - logf(neg_log_u24(ws[q]));
+                  const float x = gumbel_score(lg[v], tau, ws[q]);
                   if (x > best) { best = x; bi = v; }
                 }
               }
@@ -899,6 +907,187 @@ __global__ void argmax_kernel(const float* __restrict__ logits, int V, int64_t* 
     tokens[(int64_t)b * tok_stride] = bi;
     next_tok[b] = bi;
     if (bi == end_id) finished[b] = 1;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// sampling decode (lo_sample_args): one CTA per row b of step t over the row's V logits x.  q = softmax(x / tau); the tokens in the
+// order (q descending, index ascending), which the kernel takes from the logits (q is increasing in x, and comparing x avoids the
+// ties exp's rounding could make); top-k keeps the first k, top-p each token whose predecessors' mass is < p.  The kept set is a
+// prefix of that order, so with a filter on the CTA sorts the (logit, index) keys in shared memory (bitonic, padded to P = the
+// power of two >= V) and cuts at the first position either filter drops (the top-p mass scanned in that order).  The token is the
+// argmax over the kept v of x_v / tau + g_v (u_t [B][V] injected, or gumbel_score of the Philox words of state), ties to the lowest index, and
+// logp[b] += log_softmax(x)[token] at temperature 1.  A finished row writes end_id and adds nothing.
+// ------------------------------------------------------------------------------------------------
+#define LO_SAMPLE_THREADS 256
+#define LO_SAMPLE_MAX_V 2048                 // P * 12 bytes of shared memory: 24 kB at most
+static inline int sample_pad(int V) {
+  int P = 1;
+  while (P < V) P <<= 1;
+  return P;
+}
+// shared memory of sample_step_kernel with a filter on: P sort keys and P Gumbel scores
+static size_t sample_step_smem(int V) { return (size_t)sample_pad(V) * 12; }
+
+// sort key of (logit x, token v): a larger x first, then the lower v; every key is > 0, the padding's
+__device__ __forceinline__ unsigned long long sample_key(float x, int v) {
+  const uint32_t u = __float_as_uint(x);
+  const uint32_t o = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+  return ((unsigned long long)o << 32) | (0xFFFFFFFFu - (uint32_t)v);
+}
+__device__ __forceinline__ int sample_key_token(unsigned long long k) { return (int)(0xFFFFFFFFu - (uint32_t)k); }
+
+// the sum / max of v over the 256 threads, the same value in every thread in a fixed order (sh: 8 floats)
+__device__ __forceinline__ float sample_block_sum(float v, float* sh) {
+  v = warp_sum(v);
+  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
+  __syncthreads();
+  float r = 0.f;
+#pragma unroll
+  for (int w = 0; w < LO_SAMPLE_THREADS / 32; w++) r += sh[w];
+  __syncthreads();
+  return r;
+}
+__device__ __forceinline__ float sample_block_max(float v, float* sh) {
+  v = warp_max(v);
+  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
+  __syncthreads();
+  float r = -INFINITY;
+#pragma unroll
+  for (int w = 0; w < LO_SAMPLE_THREADS / 32; w++) r = fmaxf(r, sh[w]);
+  __syncthreads();
+  return r;
+}
+
+__global__ void __launch_bounds__(LO_SAMPLE_THREADS) sample_step_kernel(
+    const float* __restrict__ logits, int V, int P, int t, float tau, int top_k, float top_p, const float* __restrict__ u_t,
+    const unsigned long long* __restrict__ state, int64_t* __restrict__ tokens, int64_t tok_stride, int64_t* __restrict__ next_tok,
+    int32_t* __restrict__ finished, float* __restrict__ logp, int64_t end_id) {
+  extern __shared__ unsigned long long s_key[];   // [P] sort keys, then
+  float* s_sc = (float*)(s_key + P);              // [P] Gumbel scores by token (both with a filter on)
+  __shared__ float s_red[LO_SAMPLE_THREADS / 32];
+  __shared__ float s_best[LO_SAMPLE_THREADS / 32];
+  __shared__ int s_bi[LO_SAMPLE_THREADS / 32];
+  __shared__ int s_cut;
+  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  if (finished[b]) {                              // CTA-uniform
+    if (tid == 0) {
+      tokens[(int64_t)b * tok_stride] = end_id;
+      next_tok[b] = end_id;
+    }
+    return;
+  }
+  const float* lg = logits + (int64_t)b * V;
+  const bool by_k = top_k > 0 && top_k < V, by_p = top_p < 1.f, filter = by_k || by_p;
+  float m = -INFINITY;
+  for (int v = tid; v < V; v += LO_SAMPLE_THREADS) m = fmaxf(m, lg[v]);
+  m = sample_block_max(m, s_red);
+  unsigned long long seed = 0, call = 0;
+  if (!u_t) {
+    seed = state[0];
+    call = state[1];
+  }
+  // the softmax sums at temperature 1 and tau and every token's score; without a filter the thread's first maximum (its v rise)
+  float s1 = 0.f, sq = 0.f, best = -INFINITY;
+  int bi = V;
+  for (int v4 = tid; v4 * 4 < V; v4 += LO_SAMPLE_THREADS) {
+    uint4 w = make_uint4(0u, 0u, 0u, 0u);
+    if (!u_t) w = gumbel_words(v4, t, b, seed, call);
+    const uint32_t ws[4] = {w.x, w.y, w.z, w.w};
+#pragma unroll
+    for (int q = 0; q < 4; q++) {
+      const int v = v4 * 4 + q;
+      if (v < V) {
+        const float x = lg[v];
+        s1 += expf(x - m);
+        sq += expf((x - m) / tau);
+        const float sc = u_t ? x / tau - logf(-logf(u_t[(int64_t)b * V + v])) : gumbel_score(x, tau, ws[q]);
+        if (filter) {
+          s_sc[v] = sc;
+          s_key[v] = sample_key(x, v);
+        } else if (sc > best) {
+          best = sc;
+          bi = v;
+        }
+      }
+    }
+  }
+  s1 = sample_block_sum(s1, s_red);
+  sq = sample_block_sum(sq, s_red);
+  if (filter) {
+    for (int i = V + tid; i < P; i += LO_SAMPLE_THREADS) s_key[i] = 0ull;
+    if (tid == 0) s_cut = by_k ? top_k : V;
+    __syncthreads();
+    for (int k = 2; k <= P; k <<= 1)              // bitonic sort, descending
+      for (int j = k >> 1; j > 0; j >>= 1) {
+        for (int i = tid; i < P; i += LO_SAMPLE_THREADS) {
+          const int l = i ^ j;
+          if (l > i) {
+            const unsigned long long a = s_key[i], c = s_key[l];
+            if (((i & k) == 0) == (a < c)) {
+              s_key[i] = c;
+              s_key[l] = a;
+            }
+          }
+        }
+        __syncthreads();
+      }
+    if (by_p) {
+      // thread tid owns the positions [tid * per, (tid + 1) * per); the exclusive scan of the runs' unnormalised mass gives each
+      // position the mass before it
+      const int per = P > LO_SAMPLE_THREADS ? P / LO_SAMPLE_THREADS : 1, i0 = tid * per, i1 = min(i0 + per, V);
+      float run = 0.f;
+      for (int i = i0; i < i1; i++) run += expf((lg[sample_key_token(s_key[i])] - m) / tau);
+      float incl = run;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const float y = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += y;
+      }
+      float excl = __shfl_up_sync(0xffffffffu, incl, 1);
+      if (lane == 0) excl = 0.f;
+      if (lane == 31) s_red[warp] = incl;
+      __syncthreads();
+      float e = excl;
+      for (int w = 0; w < warp; w++) e += s_red[w];
+      for (int i = i0; i < i1; i++) {
+        if (e / sq >= top_p) {
+          atomicMin(&s_cut, i);
+          break;
+        }
+        e += expf((lg[sample_key_token(s_key[i])] - m) / tau);
+      }
+      __syncthreads();
+    }
+    const int cut = s_cut;
+    for (int i = tid; i < cut; i += LO_SAMPLE_THREADS) {
+      const int v = sample_key_token(s_key[i]);
+      const float sc = s_sc[v];
+      if (sc > best || (sc == best && v < bi)) {
+        best = sc;
+        bi = v;
+      }
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+    if (ob > best || (ob == best && oi < bi)) { best = ob; bi = oi; }
+  }
+  if (lane == 0) {
+    s_best[warp] = best;
+    s_bi[warp] = bi;
+  }
+  __syncthreads();
+  if (tid == 0) {
+    for (int w = 1; w < LO_SAMPLE_THREADS / 32; w++)
+      if (s_best[w] > best || (s_best[w] == best && s_bi[w] < bi)) { best = s_best[w]; bi = s_bi[w]; }
+    const int tok = bi < V ? bi : 0;
+    tokens[(int64_t)b * tok_stride] = tok;
+    next_tok[b] = tok;
+    logp[b] += lg[tok] - m - logf(s1);
+    if (tok == end_id) finished[b] = 1;
   }
 }
 
@@ -1615,18 +1804,69 @@ static int decode_begin(F& f, int max_steps, bool outputs, const BeamArgs* bm, f
   return LO_OK;
 }
 
-template <class F>
-static int greedy_loop(F& f, int64_t end_id, int max_steps, int64_t* tokens, int32_t* fin_hist, cudaStream_t st) {
+// the token choice of greedy decode: the lowest-index argmax of the step's logits
+struct ArgmaxChoice {
+  float* logp() const { return nullptr; }
+  int operator()(const DecodeCtx& c, int t, int64_t* tok_t, int64_t tok_stride, int64_t end_id, cudaStream_t st) const {
+    argmax_kernel<<<cdiv(c.B, 8), 256, 0, st>>>(c.logits, c.V, tok_t, tok_stride, c.next_tok, c.finished, end_id, c.B);
+    LO_LAUNCH_OK();
+    return LO_OK;
+  }
+};
+
+// the token choice of sampling decode (lo_sample_args, checked by check_sample): one filtered Gumbel-max draw per row
+struct SampleChoice {
+  const lo_sample_args* s;
+  float* logp() const { return s->logp; }
+  int operator()(const DecodeCtx& c, int t, int64_t* tok_t, int64_t tok_stride, int64_t end_id, cudaStream_t st) const {
+    const bool filter = (s->top_k > 0 && s->top_k < c.V) || s->top_p < 1.f;
+    sample_step_kernel<<<c.B, LO_SAMPLE_THREADS, filter ? sample_step_smem(c.V) : 0, st>>>(
+        c.logits, c.V, sample_pad(c.V), t, s->tau, s->top_k, s->top_p, s->u ? s->u + (int64_t)t * c.B * c.V : nullptr,
+        (const unsigned long long*)s->state, tok_t, tok_stride, c.next_tok, c.finished, s->logp, end_id);
+    LO_LAUNCH_OK();
+    return LO_OK;
+  }
+};
+
+// greedy decode and, with SampleChoice, sampling decode: per step the flavour's step, then `choose` writes the step's tokens, the
+// next tokens and the finished flags
+template <class F, class Choice = ArgmaxChoice>
+static int greedy_loop(F& f, int64_t end_id, int max_steps, int64_t* tokens, int32_t* fin_hist, cudaStream_t st,
+                       const Choice& choose = Choice{}) {
   const DecodeCtx& c = f.c;
-  LO_TRY(decode_begin(f, max_steps, tokens && c.finished, nullptr, nullptr, st));
+  LO_TRY(decode_begin(f, max_steps, tokens && c.finished, nullptr, choose.logp(), st));
   for (int t = 0; t < max_steps; t++) {
     LO_TRY(f.step(t, st));
-    argmax_kernel<<<cdiv(c.B, 8), 256, 0, st>>>(c.logits, c.V, tokens + t, max_steps, c.next_tok, c.finished, end_id, c.B);
-    LO_LAUNCH_OK();
+    LO_TRY(choose(c, t, tokens + t, max_steps, end_id, st));
     if (fin_hist) {
       fin_hist_kernel<<<cdiv(c.B, 128), 128, 0, st>>>(c.finished, fin_hist + t, max_steps, c.B);
       LO_LAUNCH_OK();
     }
+  }
+  return LO_OK;
+}
+
+// the refusals of the sampling entry points that concern *s, V and rows_per_img, before any GPU work
+static int check_sample(const lo_sample_args* s, int V, int rows_per_img) {
+  LO_CHECK_ARG(s, "null lo_sample_args");
+  LO_CHECK_ARG(std::isfinite(s->tau) && s->tau > 0.f, "temperature tau must be finite and > 0");
+  LO_CHECK_ARG(s->top_k >= 0 && s->top_k <= V, "top_k in 0..V (0: off)");
+  LO_CHECK_ARG(s->top_p > 0.f && s->top_p <= 1.f, "top_p in (0, 1] (1: off)");
+  LO_CHECK_ARG(s->u || s->state, "sampling needs injected uniforms u or the Philox state");
+  LO_CHECK_ARG(s->logp, "null logp");
+  LO_CHECK_ARG(rows_per_img >= 1 && rows_per_img <= LO_BEAM_MAX, "1 <= rows_per_img (samples per image) <= 16");
+  LO_CHECK_ARG(V <= LO_SAMPLE_MAX_V, "V above 2048: too large for the shared-memory sort of sampling");
+  return LO_OK;
+}
+
+// sampling decode of any flavour; the Philox state's call counter moves on after the last step, so the next call draws anew
+template <class F>
+static int sample_loop(F& f, const lo_sample_args* s, int64_t end_id, int max_steps, int64_t* tokens, int32_t* fin_hist,
+                       cudaStream_t st) {
+  LO_TRY(greedy_loop(f, end_id, max_steps, tokens, fin_hist, st, SampleChoice{s}));
+  if (s->state) {
+    bump_counter_kernel<<<1, 1, 0, st>>>((unsigned long long*)s->state + 1);
+    LO_LAUNCH_OK();
   }
   return LO_OK;
 }
@@ -1718,6 +1958,17 @@ static int decoder_beam(const lo_decoder_args* a, int64_t start_id, int64_t end_
   F f(a, start_id, finished, finished + a->B, extra...);
   bm.beam = a->rows_per_img;
   return beam_loop(f, bm, end_id, max_steps, ids, parents, fin_hist, logp, (cudaStream_t)stream);
+}
+
+// the refusals of the sampling entry points of the torch flavour and of the two-layer decoder
+static int check_decoder_sample(const lo_decoder_args* a, const lo_sample_args* s) {
+  LO_CHECK_ARG(a, "null args");
+  LO_TRY(check_args(a));
+  LO_TRY(check_sample(s, a->V, a->rows_per_img));
+  LO_TRY(check_reg_off(a, true));
+  LO_CHECK_ARG(!a->ss_prob && !a->ss_u && !a->ss_temp && !a->ss_gu,
+               "scheduled sampling (ss_prob, ss_u, ss_temp, ss_gu) is a training mode: not available in sampling decode");
+  return LO_OK;
 }
 
 }  // namespace lo
@@ -2170,6 +2421,15 @@ int lo_decoder_greedy(const lo_decoder_args* a, int64_t start_id, int64_t end_id
                       int32_t* finished, void* stream) {
   return lo_decoder_greedy_hist(a, start_id, end_id, max_steps, tokens, finished, nullptr, stream);
 }
+
+int lo_decoder_sample(const lo_decoder_args* a, const lo_sample_args* s, int64_t start_id, int64_t end_id, int max_steps,
+                      int64_t* tokens, int32_t* finished, int32_t* fin_hist, void* stream) {
+  LO_TRY(check_decoder_sample(a, s));
+  TorchDecode f(a, start_id, finished, nullptr);
+  return sample_loop(f, s, end_id, max_steps, tokens, fin_hist, (cudaStream_t)stream);
+}
+
+int64_t lo_sizeof_sample_args(void) { return (int64_t)sizeof(lo_sample_args); }
 
 int lo_decoder_beam(const lo_decoder_args* a, int64_t start_id, int64_t end_id, int max_steps, int64_t* ids, int64_t* parents,
                     int32_t* fin_hist, float* logp, void* stream) {

@@ -110,6 +110,14 @@ int lo_decoder2_greedy(const lo_decoder_args* a, const lo_decoder2_layer* l2, in
   return greedy_loop(f, end_id, max_steps, tokens, fin_hist, (cudaStream_t)stream);
 }
 
+int lo_decoder2_sample(const lo_decoder_args* a, const lo_decoder2_layer* l2, const lo_sample_args* s, int64_t start_id, int64_t end_id,
+                       int max_steps, int64_t* tokens, int32_t* finished, int32_t* fin_hist, void* stream) {
+  LO_TRY(check_decoder2(a, l2));
+  LO_TRY(check_decoder_sample(a, s));
+  TwoLayerDecode f(a, start_id, finished, nullptr, l2);
+  return sample_loop(f, s, end_id, max_steps, tokens, fin_hist, (cudaStream_t)stream);
+}
+
 int lo_decoder2_beam(const lo_decoder_args* a, const lo_decoder2_layer* l2, int64_t start_id, int64_t end_id, int max_steps,
                      int64_t* ids, int64_t* parents, int32_t* fin_hist, float* logp, float div_gamma, float div_prob,
                      const float* div_u, const uint64_t* div_state, const lo_beam_penalty* pen, void* stream) {

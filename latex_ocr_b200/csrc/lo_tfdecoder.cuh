@@ -777,6 +777,15 @@ int lo_tfdec_greedy(const lo_tfdec_args* a, int64_t end_id, int max_steps, int64
   return greedy_loop(f, end_id, max_steps, tokens, fin_hist, (cudaStream_t)stream);
 }
 
+int lo_tfdec_sample(const lo_tfdec_args* a, const lo_sample_args* s, int64_t end_id, int max_steps, int64_t* tokens, int32_t* fin_hist,
+                    void* stream) {
+  LO_CHECK_ARG(a, "null args");
+  LO_TRY(check_sample(s, a->V, a->rows_per_img));
+  LO_TRY(tf_check(a, true));
+  TfDecode f(a);
+  return sample_loop(f, s, end_id, max_steps, tokens, fin_hist, (cudaStream_t)stream);
+}
+
 int lo_tfdec_beam(const lo_tfdec_args* a, int64_t end_id, int max_steps, int64_t* ids, int64_t* parents, int32_t* fin_hist, float* logp,
                   void* stream) {
   return lo_tfdec_beam_div(a, end_id, max_steps, ids, parents, fin_hist, logp, 1.f, 0.f, nullptr, nullptr, stream);

@@ -343,6 +343,126 @@ def beam_decode(model, img, start_id, end_id, beam_size=5, max_length_formula=15
         return (ids, logp) + ((scores,) if return_scores else ()) + ((att,) if return_attention else ())
 
 
+def sampling_settings(n_samples, temperature, top_k, top_p, V):
+    """(n, tau, k, p) of a sampling decode as ints and floats; out-of-range values raise ValueError (lo_sample_args refuses the
+    same, but only after the encoder has run)."""
+    n, tau, k, p = int(n_samples), float(temperature), int(top_k), float(top_p)
+    if not 1 <= n <= 16:
+        raise ValueError("n_samples must lie in 1..16 (got %r)" % (n_samples,))
+    if not (math.isfinite(tau) and tau > 0):
+        raise ValueError("temperature must be finite and > 0 (got %r)" % (temperature,))
+    if not 0 <= k <= V:
+        raise ValueError("top_k must lie in 0..%d, 0 = off (got %r)" % (V, top_k))
+    if not 0 < p <= 1:
+        raise ValueError("top_p must lie in (0, 1], 1 = off (got %r)" % (top_p,))
+    return n, tau, k, p
+
+
+def sample_state(holder, seed, device):
+    """The Philox {seed, call} device state of one sampling decode: a new one at call 0 for a given ``seed`` (the same seed repeats
+    the draws), else ``holder``'s own, seeded from torch's initial seed on first use, whose call counter every decode advances."""
+    if seed is not None:
+        return torch.tensor([int(seed) & 0x7FFFFFFFFFFFFFFF, 0], dtype=torch.int64, device=device)
+    if getattr(holder, "_sample_state", None) is None:
+        holder._sample_state = torch.tensor([torch.initial_seed() & 0x7FFFFFFFFFFFFFFF, 0], dtype=torch.int64, device=device)
+    return holder._sample_state
+
+
+def run_sample(call, N, n, steps, tau, top_k, top_p, V, state, device, u=None, order=None):
+    """Sampling decode of N images x n samples: ``call(args, tokens, fin_hist)`` runs the flavour's entry point with the
+    lo_sample_args ``args`` and the device pointers of the outputs.  ``u``: None (Philox from ``state``) or injected uniforms
+    [steps, N * n, V] in input order (``order``: the input index of each decode image).  Returns (ids [N, n, k], log-probs [N, n]) on
+    the device in decode order, k the steps the reference's loop would have run."""
+    s = _lib.SampleArgs()
+    s.tau, s.top_k, s.top_p = tau, top_k, top_p
+    logp = torch.zeros(N * n, dtype=torch.float32, device=device)
+    s.logp = logp.data_ptr()
+    if u is not None:
+        u = torch.as_tensor(u, dtype=torch.float32).to(device).contiguous()
+        if tuple(u.shape) != (steps, N * n, V):
+            raise ValueError("u must be [steps, N * n_samples, V] = [%d, %d, %d]" % (steps, N * n, V))
+        if order is not None:
+            u = u.view(steps, N, n, V)[:, torch.tensor(order, device=device)].reshape(steps, N * n, V).contiguous()
+        s.u = u.data_ptr()
+    else:
+        s.state = state.data_ptr()
+    ids = run_greedy(lambda tokens, hist: call(s, tokens, hist), N * n, steps, device)
+    return ids.reshape(N, n, -1), logp.view(N, n)
+
+
+def _sample_entry(a, s, *args):
+    return _lib.lib().lo_decoder_sample(ctypes.byref(a), ctypes.byref(s), *args)
+
+
+def sample_decode(model, img, start_id, end_id, n_samples=8, temperature=1.0, top_k=0, top_p=1.0, max_length_formula=150,
+                  seed=None, u=None, return_attention=False, _encode=None, _entry=_sample_entry):
+    """Draws ``n_samples`` formulas per image (lo_decoder_sample): every step's token is a draw from softmax(logits /
+    ``temperature``), restricted to the ``top_k`` most probable tokens (0: all) and to the smallest prefix of them, by probability,
+    whose mass reaches ``top_p`` (1: all).  ``top_k = 1`` is greedy decode.  A sample ends at its first END (later positions hold
+    END); the loop runs as long as greedy decode's, until every sample has ended.
+
+    Returns (ids [N, n_samples, steps], log_probs [N, n_samples]) on the CPU; log_probs is each sample's log-likelihood under the
+    model (temperature 1, no filter) through its first END, comparable with beam_decode's.  ``return_attention=True`` also returns
+    the attention weights [N, n_samples, steps, R] fp32 (for a list of images, a list of [n_samples, steps, R_i]).  ``img``: a batch
+    tensor or a list of images of different sizes, results in input order.
+
+    The uniforms of the draws come from the in-kernel Philox stream: with ``seed``, a new stream at that seed (the same seed gives
+    the same samples); without, the model's own stream, which every call advances.  ``u`` (tests): injected uniforms [steps, N *
+    n_samples, V] in (0, 1), image i drawing the rows [i * n_samples, (i + 1) * n_samples).  ``mbr_select`` picks one sample per
+    image from the result.
+
+    ``_encode`` (see encode_packed) and ``_entry(args, sample_args, start_id, end_id, max_steps, tokens, finished, fin_hist,
+    stream)``, the library call, let ext.sample_decode run the two-layer decoder through this body."""
+    n, tau, k, p = sampling_settings(n_samples, temperature, top_k, top_p, model.decoder.vocab_size)
+    max_steps = max_length_formula + 2
+    with torch.no_grad():
+        dev = model.device
+        state = sample_state(model, seed, dev) if u is None else None
+        a, ws, N, lay = _prepare(model, img, n, max_steps, _encode)
+        finished = torch.zeros(a.B, dtype=torch.int32, device=dev)
+
+        def call(s, tokens, hist):
+            return _entry(a, s, int(start_id), int(end_id), max_steps, tokens, finished.data_ptr(), hist, stream_ptr())
+        ids, logp = run_sample(call, N, n, max_steps, tau, k, p, a.V, state, dev, u, lay.order if lay else None)
+        ids, logp = ids.cpu(), logp.cpu()
+        steps = ids.shape[2]
+        att = None
+        if return_attention:
+            att = ws["t"]["alphas"].view(-1)[:a.B * max_steps * a.R].view(N, n, max_steps, a.R)[:, :, :steps].cpu()
+        if lay is not None:
+            inv = _inverse(lay.order)
+            ids, logp = ids[inv], logp[inv]
+            if att is not None:
+                att = [att[j, :, :, :lay.counts[j]].clone() for j in inv.tolist()]
+        return (ids, logp) + ((att,) if return_attention else ())
+
+
+def mbr_select(ids, end_id):
+    """Minimum-Bayes-risk choice among the samples of each image: ids [N, n, steps] (sample_decode) -> (choice [N] int64,
+    agreement [N] fp32).  Every pair of samples of an image is scored with the edit-distance similarity of scst.rewards
+    (layout="tf": 1 - lev / max length, each truncated at its first ``end_id``), all pairs of all images in one
+    lo_scst_edit_reward launch; choice[i] is the sample with the highest mean similarity to the other samples (the lowest index
+    among equals) and agreement[i] that mean, a confidence for the image.  With one sample: choice 0, agreement 1."""
+    from . import scst
+    ids = torch.as_tensor(ids)
+    if ids.dim() != 3:
+        raise ValueError("ids must be [N, n, steps] (got shape %s)" % (tuple(ids.shape),))
+    N, n, _ = ids.shape
+    if n == 1:
+        return torch.zeros(N, dtype=torch.int64), torch.ones(N, dtype=torch.float32)
+    i, j = torch.triu_indices(n, n, 1)                        # the similarity is symmetric: each unordered pair once
+    dev = ids.device if ids.is_cuda else torch.device("cuda")
+    x = ids.to(dev, torch.int64)
+    r = scst.rewards(x[:, i].reshape(-1, x.shape[2]), x[:, j].reshape(-1, x.shape[2]), end_id, layout="tf")[0]
+    r = r.view(N, -1).double().cpu()
+    sim = torch.zeros(N, n, n, dtype=torch.float64)
+    sim[:, i, j] = r
+    sim[:, j, i] = r
+    mean = sim.sum(dim=2) / (n - 1)
+    choice = torch.argmax(mean, dim=1)                        # the first maximum
+    return choice, mean.gather(1, choice.unsqueeze(1)).squeeze(1).float()
+
+
 def truncate_end(list_of_ids, id_end):
     """model/evaluation/text.py:95-104."""
     out = []

@@ -403,3 +403,12 @@ def beam_decode(model, img, start_id, end_id, beam_size=5, **kw):
         return _lib.lib().lo_decoder2_beam(ctypes.byref(a), ctypes.byref(l2), *args[:-1],
                                            ctypes.byref(pen) if pen is not None else None, args[-1])
     return decode.beam_decode(model, img, start_id, end_id, beam_size, _encode=_row_encode(model), _entry=entry, **kw)
+
+
+def sample_decode(model, img, start_id, end_id, n_samples=8, **kw):
+    """Sampling decode of an Img2SeqRowModel through the row encoder and the two-layer decoder (lo_decoder2_sample).  Keywords and
+    return values are those of decode.sample_decode: temperature, top_k, top_p, max_length_formula, seed, u, return_attention."""
+    def entry(a, s, *args):
+        l2 = model.layer2.decode_layer(a)
+        return _lib.lib().lo_decoder2_sample(ctypes.byref(a), ctypes.byref(l2), ctypes.byref(s), *args)
+    return decode.sample_decode(model, img, start_id, end_id, n_samples, _encode=_row_encode(model), _entry=entry, **kw)

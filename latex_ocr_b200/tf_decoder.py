@@ -339,18 +339,21 @@ class Decoder(nn.Module):
             return ws
         return decode.ragged_cache(self._ws, (B, T, R, n_regions), build)
 
-    def packed_workspace(self, counts, steps):
+    def packed_workspace(self, counts, steps, rows_per_img=None):
         """The ragged workspace of one decode call over images of ``counts`` regions (in the order they are decoded).  The caller
-        writes image i's encoder output into ``ws["enc"][off[i]:off[i+1]]`` (``ws["off"]``) and then calls decode_packed."""
+        writes image i's encoder output into ``ws["enc"][off[i]:off[i+1]]`` (``ws["off"]``) and then calls decode_packed.
+        ``rows_per_img``: the rows of each image (default: the beam size; sample() passes its sample count)."""
         N = len(counts)
+        rpi = self._tiles if rows_per_img is None else int(rows_per_img)
         if N == 0:
             raise ValueError("no images")
         if min(counts) < 1:
             raise ValueError("an image has no encoder region")
-        if N * self._tiles > MAX_ROWS:
-            raise ValueError("%d images x beam %d exceed the %d rows of one decode call" % (N, self._tiles, MAX_ROWS))
+        if N * rpi > MAX_ROWS:
+            raise ValueError("%d images x %d rows exceed the %d rows of one decode call" % (N, rpi, MAX_ROWS))
         off = decode.region_offsets(counts)
-        ws = self.ragged_workspace(N * self._tiles, steps, max(counts), off[-1])
+        # the kernel workspace is sized for B / beam images, so a call of fewer rows per image asks for that many more rows
+        ws = self.ragged_workspace(N * max(rpi, self._tiles), steps, max(counts), off[-1])
         ws["counts"], ws["off"] = [int(n) for n in counts], off
         return ws
 
@@ -413,6 +416,51 @@ class Decoder(nn.Module):
             ws["enc"] = enc
             return self._run_decode(L, a, N, steps, div_u, ws["alphas"] if return_attention else None, return_log_probs, finalize,
                                     return_scores)
+
+    def sample(self, enc, n_samples=8, temperature=1.0, top_k=0, top_p=1.0, max_steps=None, u=None, seed=None,
+               return_attention=False):
+        """Sampling decode (lo_tfdec_sample): ``n_samples`` formulas per image, each step's token drawn from softmax(logits /
+        ``temperature``) restricted by ``top_k`` / ``top_p``, as decode.sample_decode documents.  ``enc`` as in decode(): a batch
+        [N,R,C] / [N,H,W,C] or a list of the encoder outputs of images of different sizes.  Returns (ids [N, n_samples, steps],
+        log_probs [N, n_samples]) on the device, ids in input order, and with ``return_attention`` the attention weights [N,
+        n_samples, steps, R] (a list of [n_samples, steps, R_i] for a list).  ``seed``: a new Philox stream at that seed, else the
+        decoder's own, which every call advances; ``u`` (tests): injected uniforms [steps, N * n_samples, V], image i drawing the
+        rows [i * n_samples, (i + 1) * n_samples)."""
+        n, tau, k, p = decode.sampling_settings(n_samples, temperature, top_k, top_p, self.V)
+        steps = int(max_steps) if max_steps is not None else self.max_length_formula + 2
+        dev = self.store.device
+        self.store.refresh_shadow()
+        counts = None
+        if isinstance(enc, (list, tuple)):
+            encs = [self._enc_regions(e) for e in enc]
+            counts = [e.shape[0] for e in encs]
+            ws = self.packed_workspace(counts, steps, n)
+            off = ws["off"]
+            for i, e in enumerate(encs):
+                ws["enc"][off[i]:off[i + 1]].copy_(e)
+            N, R = len(encs), max(counts)
+        else:
+            enc = self._enc(enc)
+            N, R, _ = enc.shape
+            ws = None
+        with torch.no_grad():
+            state = decode.sample_state(self, seed, dev) if u is None else None
+            if counts is None:
+                L, ws, a = self._args(enc, N * n, steps, R, rows_per_img=n, decode=True)
+                ws["enc"] = enc
+            else:
+                L, ws, a = self._args(ws["enc"], N * n, steps, R, rows_per_img=n, ws=ws)
+                decode.set_region_offsets(a, ws["reg_off_host"], ws["reg_off"], ws["off"])
+
+            def call(s, tokens, fin):
+                return L.lo_tfdec_sample(ctypes.byref(a), ctypes.byref(s), self._id_end, steps, tokens, fin, stream_ptr())
+            ids, logp = decode.run_sample(call, N, n, steps, tau, k, p, self.V, state, dev, u)
+            if not return_attention:
+                return ids, logp
+            att = ws["alphas"].view(-1)[:N * n * steps * R].view(N, n, steps, R)[:, :, :ids.shape[2]].clone()
+            if counts is not None:
+                att = [att[i, :, :, :counts[i]].clone() for i in range(N)]
+            return ids, logp, att
 
     def _enc_regions(self, e):
         """one image's encoder output of a list -> [R_i, C] on the device"""

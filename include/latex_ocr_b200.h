@@ -447,7 +447,8 @@ int lo_decoder_sample(const lo_decoder_args* a, const lo_sample_args* s, int64_t
  * dtype.min, only beam 0 at time 0, top-k over beam*V with the lower index winning ties, state gather by parents;
  * no length normalisation (lo_decoder_beam_pen adds it), diversity penalty off as in configs/model.json:15-16).  a->B = n_img*beam rows,
  * a->rows_per_img = beam, a->enc holds n_img images.  ids/parents out [n_img][max_steps][beam] int64,
- * fin_hist [n_img][max_steps][beam] int32 (finished flags after each step), logp [n_img][beam] final scores. */
+ * fin_hist [n_img][max_steps][beam] int32 (finished flags after each step), logp [n_img][beam] final scores.  beam above 16 or
+ * above V (time 0 ranks beam 0's V tokens alone) is refused (LO_EINVAL) before any GPU work, in every flavour's beam search. */
 int lo_decoder_beam(const lo_decoder_args* a, int64_t start_id, int64_t end_id, int max_steps, int64_t* ids,
                     int64_t* parents, int32_t* fin_hist, float* logp, void* stream);
 /* the same with the diversity penalty of beam_search_decoder_cell.py:258-287 (Li et al. 2016; configs/model.json:15-16

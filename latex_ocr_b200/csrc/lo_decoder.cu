@@ -1241,7 +1241,7 @@ __global__ void __launch_bounds__(256) beam_step_kernel(const float* __restrict_
       int i2 = s_redi[0];
       for (int w = 1; w < 8; w++)
         if (s_red[w] > b2 || (s_red[w] == b2 && s_redi[w] < i2)) { b2 = s_red[w]; i2 = s_redi[w]; }
-      if (i2 == 0x7fffffff) i2 = 0;          // fewer candidates than beams (beam*V < beam): cannot happen for V >= beam
+      if (i2 == 0x7fffffff) i2 = 0;          // fewer candidates than beams: decode_begin refuses V < beam
       s_newp[j] = b2;
       s_newc[j] = pen ? s_tot[i2] : b2;
       s_newi[j] = i2;
@@ -1795,6 +1795,8 @@ static int decode_begin(F& f, int max_steps, bool outputs, const BeamArgs* bm, f
     LO_CHECK_ARG(!bm->div_on() || (bm->div_gamma > 0.f && (bm->div_u || bm->div_state)),
                  "diversity penalty needs gamma > 0 and div_u or div_state");
     LO_CHECK_ARG(bm->beam >= 1 && bm->beam <= LO_BEAM_MAX && c.B % bm->beam == 0, "1 <= beam (rows_per_img) <= 16, B % beam == 0");
+    // step 0 ranks beam 0's V candidates alone: with fewer than beam of them the top-k would repeat a hypothesis
+    LO_CHECK_ARG(bm->beam <= c.V, "beam (rows_per_img) <= V: step 0 needs a distinct token per beam");
     LO_CHECK_ARG(beam_step_smem(bm->beam, c.V, bm->div_on() || bm->pen_on()) <= 200 * 1024, "beam*V too large for the shared-memory top-k");
   }
   LO_CUDA(cudaMemsetAsync(c.finished, 0, (size_t)c.B * 4, st));

@@ -206,7 +206,7 @@ def _prepare(model, img, rows_per_img, max_steps, encode=None):
     if isinstance(img, (list, tuple)):
         lay = ragged_layout(img, model.encoder.out_hw)
         N, R = len(lay.order), max(lay.counts)
-        ws = dec.ragged_workspace(N * rows_per_img, max_steps, R, lay.off[-1])
+        ws = decode_workspace(dec, N, R, rows_per_img, max_steps, lay.off)
         enc = ws["t"]["enc"]
         encode_packed(model.encoder, lay, enc, model.device, encode)
     else:
@@ -215,16 +215,32 @@ def _prepare(model, img, rows_per_img, max_steps, encode=None):
             enc = encode(enc)
         N, R = enc.shape[0], enc.shape[1] * enc.shape[2]
         enc = enc.view(N, R, enc.shape[3])
-        ws = dec.workspace(N * rows_per_img, max_steps, R, need_grad=False)
+        ws = decode_workspace(dec, N, R, rows_per_img, max_steps)
+    a = decode_args(dec, ws, enc, N, R, rows_per_img, max_steps, lay.off if lay is not None else None)
+    return a, ws, N, lay
+
+
+def decode_workspace(dec, N, R, rows_per_img, max_steps, off=None):
+    """The workspace of a decode of N images x rows_per_img rows over at most R regions: for images of different sizes (``off``,
+    their region offsets) the ragged one, whose packed encoder output ``ws["t"]["enc"]`` the caller fills; else the one of the
+    shape, for an encoder output [N, R, C] of the caller's."""
+    if off is not None:
+        return dec.ragged_workspace(N * rows_per_img, max_steps, R, off[-1])
+    return dec.workspace(N * rows_per_img, max_steps, R, need_grad=False)
+
+
+def decode_args(dec, ws, enc, N, R, rows_per_img, max_steps, off=None):
+    """The lo_decoder_args of a decode on ``ws`` (decode_workspace) once the encoder output ``enc`` is in place: every step runs
+    all N * rows_per_img rows, the bf16 shadow refreshed, and with ``off`` the images' own region counts."""
     B = N * rows_per_img
     dec.store.refresh_shadow()
     for t in range(max_steps):
         ws["bt"][t] = B
     a = dec.fill_args(ws, enc, B, max_steps, R, has_dropout=False)
     a.rows_per_img = rows_per_img
-    if lay is not None:
-        set_region_offsets(a, ws["reg_off_host"], ws["t"]["reg_off"], lay.off)
-    return a, ws, N, lay
+    if off is not None:
+        set_region_offsets(a, ws["reg_off_host"], ws["t"]["reg_off"], off)
+    return a
 
 
 def _inverse(order):

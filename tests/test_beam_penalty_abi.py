@@ -129,6 +129,25 @@ def test_the_shared_memory_limit_counts_the_score_array(L, flavour):
     assert rc == -1 and b"reg_off_host[0] must be 0" in err
 
 
+@pytest.mark.parametrize("flavour", ["torch", "tf"])
+def test_beam_above_V_is_refused(L, flavour):
+    """time 0 ranks beam 0's V tokens alone: a beam wider than V would repeat a hypothesis, so it is refused, with and without a
+    penalty; beam == V passes on to the next check (the deliberately bad region offsets)"""
+    for pen in (ctypes.byref(_penalty(alpha=0.0, beta=0.0)), ctypes.byref(_penalty())):
+        for beam, V in ((4, 3), (16, 15), (3, 2)):
+            rc, err = _call(L, flavour, pen, V=V, beam=beam)
+            assert rc == -1 and b"beam (rows_per_img) <= V" in err, (beam, V, err)
+        rc, err = _call(L, flavour, pen, V=3, beam=3, off=[1, 3, 5, 8])
+        assert rc == -1 and b"reg_off_host[0] must be 0" in err, err
+    # the entry points without penalties share the check
+    o = [ctypes.c_void_p(_FAKE)] * 4
+    if flavour == "torch":
+        rc = L.lo_decoder_beam_div(ctypes.byref(_args(3, 4, None)), 0, 1, 3, *o, 1.0, 0.0, None, None, None)
+    else:
+        rc = L.lo_tfdec_beam_div(ctypes.byref(_tf_args(3, 4, None)), 1, 3, *o, 1.0, 0.0, None, None, None)
+    assert rc == -1 and b"beam (rows_per_img) <= V" in L.lo_last_error()
+
+
 def test_python_refuses_negative_weights():
     for a, b in ((-0.1, 0.0), (0.0, -0.5), (math.nan, 0.0), (0.0, math.inf)):
         with pytest.raises(ValueError):

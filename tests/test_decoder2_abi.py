@@ -138,6 +138,8 @@ BEAM_BAD = [
     ("null len", dict(pen=dict(len=None)), b"null len scratch"),
     ("diversity without a source", dict(div=(0.5, 0.7, None, None)), b"diversity penalty needs"),
     ("beam above 16", dict(beam=17), b"1 <= beam"),
+    ("beam above V", dict(beam=4, V=3), b"beam (rows_per_img) <= V"),
+    ("beam above V with a penalty", dict(beam=16, V=15, pen={}), b"beam (rows_per_img) <= V"),
     ("beam*V too large", dict(beam=16, V=2000, pen={}), b"beam*V too large"),
 ]
 

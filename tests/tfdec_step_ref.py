@@ -284,15 +284,18 @@ def attention_workspace_bytes(B, C):
     return 4096 + B * 16 * (C + 2) * 4
 
 
-def carve(B, T, R, C, A, D, O, E, V, ldl, bf16):
+def carve(B, T, R, C, A, D, O, E, V, ldl, bf16, rows_per_img=1):
     """(views, end): name -> (byte offset, dtype, shape) of every region of the workspace up to ``sreg``, and the offset where the
-    next region (the ragged decode's CTA map, which depends on B only) starts.  Training layout: rows_per_img = 1."""
+    next region (the ragged decode's CTA map, which depends on B only) starts.  Training runs rows_per_img = 1; a decode of
+    rows_per_img rows per image keeps att_img / datt_img per image, [B / rows_per_img][R][A] (a ragged decode packs each image's
+    own regions there, [regions][A])."""
     es = 2 if bf16 else 4
     XH, G, N2 = O + D, 4 * D, A + O
     Vl = ldl or V
     TB, T1B = T * B, (T + 1) * B
     f32, b16, wdt = torch.float32, torch.bfloat16, (torch.bfloat16 if bf16 else torch.float32)
-    plan = [("att_img", wdt, (B, R, A)), ("datt_img", wdt, (B, R, A)), ("dbeta_acc", f32, (B, A)),
+    nimg = B // rows_per_img
+    plan = [("att_img", wdt, (nimg, R, A)), ("datt_img", wdt, (nimg, R, A)), ("dbeta_acc", f32, (B, A)),
             ("ptab", f32, (V + 1, G)), ("dptab", f32, (V + 1, G)), ("xh", f32, (T + 1, B, XH)), ("call", f32, (T + 1, B, D)),
             ("gates", f32, (T, B, G)), ("ztmp", f32, (B, G)), ("out2", f32, (T, B, N2)), ("ctx", f32, (T, B, C)), ("oc", f32, (B, O)),
             ("dologit", f32, (T, B, O)), ("dout2", f32, (T, B, N2)), ("dhc", f32, (B, D + C)), ("dz", f32, (T, B, G)),

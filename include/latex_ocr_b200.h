@@ -746,6 +746,69 @@ int lo_decoder2_beam(const lo_decoder_args* a, const lo_decoder2_layer* l2, int6
                      int64_t* ids, int64_t* parents, int32_t* fin_hist, float* logp, float div_gamma, float div_prob,
                      const float* div_u, const uint64_t* div_state, const lo_beam_penalty* pen, void* stream);
 
+/* EXTENSION: balanced brackets in greedy, beam and sampling decode of every flavour (the *_brackets entry points).  A rule gives
+ * every token a role: 0 neutral, +k opens kind k, -k closes kind k (1 <= k <= n_kinds).  Every decode row keeps a stack of kinds.
+ * At step t of a call of max_steps steps, with d the row's depth and r = max_steps - 1 - t the steps left after this one, the row
+ * may take token v only if
+ *   close of kind k:   d > 0 and kind k on top of the stack
+ *   open:              d < max_depth and d + 1 <= r
+ *   neutral, not END:  d <= r
+ *   END:               d == 0
+ * so d <= r + 1 holds at every step, the close of the top kind is always allowed and a row never runs out of tokens.  The excluded
+ * tokens get logit -inf before the token choice: greedy takes the argmax over the allowed tokens, beam search's log-softmax runs
+ * over them alone (the finished mask, diversity rank and lo_beam_penalty act on those totals unchanged, logp sums restricted
+ * log-probs), and sampling filters and draws from the restricted distribution (its logp at temperature 1 is the restricted one).
+ * The chosen token then pushes or pops the row's stack; finished rows keep theirs; in beam search the stacks follow the hypotheses
+ * by parent, as the coverage of lo_beam_penalty does.  Every greedy and sampled row, and every beam hypothesis followed by
+ * lineage (lo_beam_backtrack LO_BEAM_LINEAGE), cut at its first END or ending at max_steps, nests properly and leaves no bracket
+ * open; slot-wise hypotheses (LO_BEAM_SLOTS) are not lineages and carry no such guarantee.  One launch per step (one warp per
+ * row, the role table in shared memory), between the flavour's head and the token choice; the other launches are those of the
+ * entry point without the rule.
+ *   role       device int32 [V]; a precondition the kernel does not check: every |role| <= n_kinds, end_id neutral, every kind
+ *              with an opening and a closing token (the kernel reads role[0..V) and nothing else, whatever the contents)
+ *   n_kinds    1..255
+ *   max_depth  1..32
+ *   state      device scratch of lo_bracket_state_bytes(B, max_depth) bytes: [2][B] int32 depths, then [2][B][max_depth] uint8
+ *              kinds (read and written alternately, step by step; zeroed by the call)
+ * Refused (LO_EINVAL) before any GPU work: a null rule, role or state, n_kinds outside 1..255, max_depth outside 1..32, V above
+ * 24576 (the role table as int16 in shared memory), and every refusal of the entry point without the rule.  Beam search ranks
+ * beam distinct tokens at step 0: the caller makes sure at least beam tokens are allowed at depth 0. */
+typedef struct lo_bracket_rule {
+  const int32_t* role;
+  int n_kinds;
+  int max_depth;
+  void* state;
+} lo_bracket_rule;
+int64_t lo_sizeof_bracket_rule(void);
+/* bytes of lo_bracket_rule.state for B rows (0 for B < 1 or max_depth outside 1..32) */
+int64_t lo_bracket_state_bytes(int B, int max_depth);
+/* lo_decoder_greedy_hist, lo_decoder_sample and lo_decoder_beam_pen (pen NULL: no penalty) under the rule *br */
+int lo_decoder_greedy_brackets(const lo_decoder_args* a, int64_t start_id, int64_t end_id, int max_steps, int64_t* tokens,
+                               int32_t* finished, int32_t* fin_hist, const lo_bracket_rule* br, void* stream);
+int lo_decoder_sample_brackets(const lo_decoder_args* a, const lo_sample_args* s, int64_t start_id, int64_t end_id, int max_steps,
+                               int64_t* tokens, int32_t* finished, int32_t* fin_hist, const lo_bracket_rule* br, void* stream);
+int lo_decoder_beam_brackets(const lo_decoder_args* a, int64_t start_id, int64_t end_id, int max_steps, int64_t* ids, int64_t* parents,
+                             int32_t* fin_hist, float* logp, float div_gamma, float div_prob, const float* div_u,
+                             const uint64_t* div_state, const lo_beam_penalty* pen, const lo_bracket_rule* br, void* stream);
+/* lo_tfdec_greedy, lo_tfdec_sample and lo_tfdec_beam_pen (pen NULL: no penalty) under the rule *br */
+int lo_tfdec_greedy_brackets(const lo_tfdec_args* a, int64_t end_id, int max_steps, int64_t* tokens, int32_t* fin_hist,
+                             const lo_bracket_rule* br, void* stream);
+int lo_tfdec_sample_brackets(const lo_tfdec_args* a, const lo_sample_args* s, int64_t end_id, int max_steps, int64_t* tokens,
+                             int32_t* fin_hist, const lo_bracket_rule* br, void* stream);
+int lo_tfdec_beam_brackets(const lo_tfdec_args* a, int64_t end_id, int max_steps, int64_t* ids, int64_t* parents, int32_t* fin_hist,
+                           float* logp, float div_gamma, float div_prob, const float* div_u, const uint64_t* div_state,
+                           const lo_beam_penalty* pen, const lo_bracket_rule* br, void* stream);
+/* lo_decoder2_greedy, lo_decoder2_sample and lo_decoder2_beam under the rule *br */
+int lo_decoder2_greedy_brackets(const lo_decoder_args* a, const lo_decoder2_layer* l2, int64_t start_id, int64_t end_id, int max_steps,
+                                int64_t* tokens, int32_t* finished, int32_t* fin_hist, const lo_bracket_rule* br, void* stream);
+int lo_decoder2_sample_brackets(const lo_decoder_args* a, const lo_decoder2_layer* l2, const lo_sample_args* s, int64_t start_id,
+                                int64_t end_id, int max_steps, int64_t* tokens, int32_t* finished, int32_t* fin_hist,
+                                const lo_bracket_rule* br, void* stream);
+int lo_decoder2_beam_brackets(const lo_decoder_args* a, const lo_decoder2_layer* l2, int64_t start_id, int64_t end_id, int max_steps,
+                              int64_t* ids, int64_t* parents, int32_t* fin_hist, float* logp, float div_gamma, float div_prob,
+                              const float* div_u, const uint64_t* div_state, const lo_beam_penalty* pen, const lo_bracket_rule* br,
+                              void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Optimiser: torch.optim.Adam defaults (img2seq_torch.py:86-87, :168-170) on one flat buffer.
  * state_dev: float[2] = {step (as float), lr}; step is incremented on the device so the call is

@@ -1123,6 +1123,62 @@ __global__ void __launch_bounds__(256) beam_coverage_kernel(const float* __restr
 }
 
 // ------------------------------------------------------------------------------------------------
+// balanced brackets (lo_bracket_rule): one warp per row b, after the step's logits [B][V] are written and before the token
+// choice.  First the row's stack of kinds catches up with the token it took at step t-1 (t > 0): the stack of row parent_rows[b]
+// (beam search; b itself otherwise) is read from one half of the [2] state and written to the other, then pushed (role +k) or
+// popped (role -k) by prev_tok[b] unless the row is finished (a row finishing at t-1 took END, a neutral token).  Lane i holds
+// stack entry i.  Then every token the row may not take gets logit -inf, in place: with d the depth and r = max_steps - 1 - t the
+// steps left after this one, a close of kind k needs d > 0 and kind k on top, an open d < max_depth and d + 1 <= r, a neutral
+// token d <= r and END d == 0.  The role table is loop-invariant: it goes to shared memory (int16, |role| <= 255) before
+// griddepcontrol.wait.  A token outside [0, V) or a push past max_depth or a pop at depth 0 (impossible for a token the mask
+// allowed) leaves the stack as it is: no access outside the table or the state.
+// ------------------------------------------------------------------------------------------------
+#define LO_BRACKET_MAX_V 24576               // the role table as int16 in 48 kB of shared memory
+__global__ void __launch_bounds__(256) bracket_mask_kernel(float* __restrict__ logits, int V, const int32_t* __restrict__ role,
+                                                           const int32_t* __restrict__ depth_in, const uint8_t* __restrict__ kind_in,
+                                                           int32_t* __restrict__ depth_out, uint8_t* __restrict__ kind_out,
+                                                           const int32_t* __restrict__ parent_rows,
+                                                           const int32_t* __restrict__ finished, const int64_t* __restrict__ prev_tok,
+                                                           int B, int max_depth, int t, int max_steps, int64_t end_id) {
+  extern __shared__ int16_t s_role[];
+  for (int v = threadIdx.x; v < V; v += blockDim.x) s_role[v] = (int16_t)max(-255, min(255, role[v]));
+  __syncthreads();
+  pdl_wait();
+  pdl_trigger();
+  const int b = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (b >= B) return;
+  int d = 0, k = 0;
+  if (t > 0) {
+    const int src = parent_rows ? parent_rows[b] : b;
+    d = depth_in[src];
+    if (lane < max_depth) k = kind_in[(int64_t)src * max_depth + lane];
+    if (!finished[b]) {
+      const int64_t tok = prev_tok[b];
+      const int ro = (tok >= 0 && tok < V) ? s_role[tok] : 0;
+      if (ro > 0 && d < max_depth) {
+        if (lane == d) k = ro;
+        d++;
+      } else if (ro < 0 && d > 0) {
+        d--;
+      }
+    }
+    if (lane == 0) depth_out[b] = d;
+    if (lane < max_depth) kind_out[(int64_t)b * max_depth + lane] = (uint8_t)k;
+  }
+  const int top = __shfl_sync(0xffffffffu, k, d > 0 ? d - 1 : 0);
+  const int r = max_steps - 1 - t;
+  float* lg = logits + (int64_t)b * V;
+  for (int v = lane; v < V; v += 32) {
+    const int ro = s_role[v];
+    bool ok;
+    if (ro < 0) ok = d > 0 && top == -ro;
+    else if (ro > 0) ok = d < max_depth && d + 1 <= r;
+    else ok = v == end_id ? d == 0 : d <= r;
+    if (!ok) lg[v] = -INFINITY;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
 // beam search step (beam_search_decoder_cell.py:123-187): one block per image.
 //   lp = log_softmax(logits) ; finished beams -> [END: 0, else: dtype.min] ; total = prev + lp ;
 //   time 0: beam 0 only ; top-k(beam) over beam*V (lower flat index wins ties) ; id = idx % V ; parent = idx / V
@@ -1751,7 +1807,7 @@ __global__ void __launch_bounds__(256) beam_backtrack_kernel(const int64_t* __re
 // The step writes its attention rows of R regions: row b of step t at alphas + b * alpha_row_stride + t * R.
 struct DecodeCtx {
   int B, T, V, rpi;
-  const float* logits;
+  float* logits;
   int64_t* next_tok;
   int32_t *finished, *parent_rows;
   AttRagged rg;
@@ -1785,10 +1841,38 @@ static int check_beam_penalty(const lo_beam_penalty* p, int beam, int V, bool di
   return LO_OK;
 }
 
+// the refusals of the *_brackets entry points that concern *br and V, before any GPU work (the table's contents are the caller's
+// precondition: the kernel reads role[0..V) and nothing else of it)
+static int check_bracket_rule(const lo_bracket_rule* br, int V) {
+  LO_CHECK_ARG(br, "null lo_bracket_rule");
+  LO_CHECK_ARG(br->role && br->state, "null role table or state");
+  LO_CHECK_ARG(br->n_kinds >= 1 && br->n_kinds <= 255, "n_kinds in 1..255");
+  LO_CHECK_ARG(br->max_depth >= 1 && br->max_depth <= 32, "max_depth in 1..32");
+  LO_CHECK_ARG(V <= LO_BRACKET_MAX_V, "V above 24576: too large for the shared-memory role table of the bracket rule");
+  return LO_OK;
+}
+
+static int64_t bracket_state_bytes(int B, int max_depth) { return ((int64_t)B * 8 + (int64_t)2 * B * max_depth + 15) / 16 * 16; }
+
+// one step of the bracket rule (bracket_mask_kernel): the state of step t in half t & 1 of br->state, that of step t-1 in the
+// other; parent_rows NULL outside beam search
+static int bracket_step(const DecodeCtx& c, const lo_bracket_rule* br, const int32_t* parent_rows, int t, int max_steps,
+                        int64_t end_id, cudaStream_t st) {
+  const int h = t & 1;
+  int32_t* depth = (int32_t*)br->state;
+  uint8_t* kind = (uint8_t*)(depth + 2 * (int64_t)c.B);
+  const int64_t nk = (int64_t)c.B * br->max_depth;
+  LO_CUDA(launch_pdl(bracket_mask_kernel, dim3(cdiv(c.B, 8)), dim3(256), (size_t)c.V * sizeof(int16_t), st, c.logits, c.V,
+                     br->role, depth + (1 - h) * c.B, kind + (1 - h) * nk, depth + h * c.B, kind + h * nk, parent_rows,
+                     (const int32_t*)c.finished, (const int64_t*)c.next_tok, c.B, br->max_depth, t, max_steps, end_id));
+  return LO_OK;
+}
+
 // the decode arguments both flavours check alike (bm NULL: greedy decode), before anything is enqueued; then everything before
-// step 0: finished = 0, log-probs = 0 (beam search, :106-107), the prologue, the ragged CTA map
+// step 0: finished = 0, log-probs = 0 (beam search, :106-107), every row's bracket stack empty (br), the prologue, the ragged CTA map
 template <class F>
-static int decode_begin(F& f, int max_steps, bool outputs, const BeamArgs* bm, float* logp, cudaStream_t st) {
+static int decode_begin(F& f, int max_steps, bool outputs, const BeamArgs* bm, float* logp, cudaStream_t st,
+                        const lo_bracket_rule* br = nullptr) {
   DecodeCtx& c = f.c;
   LO_CHECK_ARG(outputs && max_steps > 0 && max_steps <= c.T, "outputs / max_steps (<= T capacity)");
   if (bm) {
@@ -1799,8 +1883,10 @@ static int decode_begin(F& f, int max_steps, bool outputs, const BeamArgs* bm, f
     LO_CHECK_ARG(bm->beam <= c.V, "beam (rows_per_img) <= V: step 0 needs a distinct token per beam");
     LO_CHECK_ARG(beam_step_smem(bm->beam, c.V, bm->div_on() || bm->pen_on()) <= 200 * 1024, "beam*V too large for the shared-memory top-k");
   }
+  if (br) LO_TRY(check_bracket_rule(br, c.V));
   LO_CUDA(cudaMemsetAsync(c.finished, 0, (size_t)c.B * 4, st));
   if (logp) LO_CUDA(cudaMemsetAsync(logp, 0, (size_t)c.B * 4, st));
+  if (br) LO_CUDA(cudaMemsetAsync(br->state, 0, (size_t)bracket_state_bytes(c.B, br->max_depth), st));
   LO_TRY(f.prologue(st));
   if (c.rg.reg_off) LO_TRY(attention_ragged_prepare(c.rg, c.B, c.rpi, st));
   return LO_OK;
@@ -1834,11 +1920,12 @@ struct SampleChoice {
 // next tokens and the finished flags
 template <class F, class Choice = ArgmaxChoice>
 static int greedy_loop(F& f, int64_t end_id, int max_steps, int64_t* tokens, int32_t* fin_hist, cudaStream_t st,
-                       const Choice& choose = Choice{}) {
+                       const Choice& choose = Choice{}, const lo_bracket_rule* br = nullptr) {
   const DecodeCtx& c = f.c;
-  LO_TRY(decode_begin(f, max_steps, tokens && c.finished, nullptr, choose.logp(), st));
+  LO_TRY(decode_begin(f, max_steps, tokens && c.finished, nullptr, choose.logp(), st, br));
   for (int t = 0; t < max_steps; t++) {
     LO_TRY(f.step(t, st));
+    if (br) LO_TRY(bracket_step(c, br, nullptr, t, max_steps, end_id, st));
     LO_TRY(choose(c, t, tokens + t, max_steps, end_id, st));
     if (fin_hist) {
       fin_hist_kernel<<<cdiv(c.B, 128), 128, 0, st>>>(c.finished, fin_hist + t, max_steps, c.B);
@@ -1864,8 +1951,8 @@ static int check_sample(const lo_sample_args* s, int V, int rows_per_img) {
 // sampling decode of any flavour; the Philox state's call counter moves on after the last step, so the next call draws anew
 template <class F>
 static int sample_loop(F& f, const lo_sample_args* s, int64_t end_id, int max_steps, int64_t* tokens, int32_t* fin_hist,
-                       cudaStream_t st) {
-  LO_TRY(greedy_loop(f, end_id, max_steps, tokens, fin_hist, st, SampleChoice{s}));
+                       cudaStream_t st, const lo_bracket_rule* br = nullptr) {
+  LO_TRY(greedy_loop(f, end_id, max_steps, tokens, fin_hist, st, SampleChoice{s}, br));
   if (s->state) {
     bump_counter_kernel<<<1, 1, 0, st>>>((unsigned long long*)s->state + 1);
     LO_LAUNCH_OK();
@@ -1876,13 +1963,15 @@ static int sample_loop(F& f, const lo_sample_args* s, int64_t end_id, int max_st
 // bm.beam == c.rpi once decode_begin has checked it
 template <class F>
 static int beam_loop(F& f, const BeamArgs& bm, int64_t end_id, int max_steps, int64_t* ids, int64_t* parents, int32_t* fin_hist,
-                     float* logp, cudaStream_t st) {
+                     float* logp, cudaStream_t st, const lo_bracket_rule* br = nullptr) {
   const DecodeCtx& c = f.c;
-  LO_TRY(decode_begin(f, max_steps, ids && parents && fin_hist && logp, &bm, logp, st));
+  LO_TRY(decode_begin(f, max_steps, ids && parents && fin_hist && logp, &bm, logp, st, br));
   const bool pen = bm.pen_on(), cov = pen && bm.pen->beta > 0.f;
   const int64_t nc = (int64_t)c.B * c.R;          // one half of the [2][B][R] coverage, then the [B] coverage terms
   for (int t = 0; t < max_steps; t++) {
     LO_TRY(f.step(t, st));
+    // the rule's stacks follow the hypotheses by parent_rows, as the coverage does; excluded tokens leave the log-softmax
+    if (br) LO_TRY(bracket_step(c, br, c.parent_rows, t, max_steps, end_id, st));
     BeamPenStep ps{};
     if (bm.pen) ps.scores = bm.pen->scores;
     if (pen) {
@@ -1951,7 +2040,7 @@ struct TorchDecode {
 // after its TorchDecode arguments; bm.beam is set here from rows_per_img)
 template <class F = TorchDecode, class... X>
 static int decoder_beam(const lo_decoder_args* a, int64_t start_id, int64_t end_id, int max_steps, int64_t* ids, int64_t* parents,
-                        int32_t* fin_hist, float* logp, BeamArgs bm, void* stream, X... extra) {
+                        int32_t* fin_hist, float* logp, BeamArgs bm, const lo_bracket_rule* br, void* stream, X... extra) {
   LO_TRY(check_args(a));
   LO_TRY(check_reg_off(a, true));
   LO_CHECK_ARG(!a->ss_prob, "scheduled sampling (ss_prob) is a training mode: not available in beam search");
@@ -1959,7 +2048,7 @@ static int decoder_beam(const lo_decoder_args* a, int64_t start_id, int64_t end_
   int32_t* finished = (int32_t*)a->row_loss;
   F f(a, start_id, finished, finished + a->B, extra...);
   bm.beam = a->rows_per_img;
-  return beam_loop(f, bm, end_id, max_steps, ids, parents, fin_hist, logp, (cudaStream_t)stream);
+  return beam_loop(f, bm, end_id, max_steps, ids, parents, fin_hist, logp, (cudaStream_t)stream, br);
 }
 
 // the refusals of the sampling entry points of the torch flavour and of the two-layer decoder
@@ -2442,7 +2531,7 @@ int lo_decoder_beam_div(const lo_decoder_args* a, int64_t start_id, int64_t end_
                         int32_t* fin_hist, float* logp, float div_gamma, float div_prob, const float* div_u,
                         const uint64_t* div_state, void* stream) {
   return decoder_beam(a, start_id, end_id, max_steps, ids, parents, fin_hist, logp, BeamArgs{0, div_gamma, div_prob, div_u, div_state,
-                                                                                             nullptr}, stream);
+                                                                                             nullptr}, nullptr, stream);
 }
 
 int lo_decoder_beam_pen(const lo_decoder_args* a, int64_t start_id, int64_t end_id, int max_steps, int64_t* ids, int64_t* parents,
@@ -2451,10 +2540,45 @@ int lo_decoder_beam_pen(const lo_decoder_args* a, int64_t start_id, int64_t end_
   const BeamArgs bm{0, div_gamma, div_prob, div_u, div_state, pen};
   LO_CHECK_ARG(a, "null args");
   LO_TRY(check_beam_penalty(pen, a->rows_per_img, a->V, bm.div_on()));
-  return decoder_beam(a, start_id, end_id, max_steps, ids, parents, fin_hist, logp, bm, stream);
+  return decoder_beam(a, start_id, end_id, max_steps, ids, parents, fin_hist, logp, bm, nullptr, stream);
 }
 
 int64_t lo_sizeof_beam_penalty(void) { return (int64_t)sizeof(lo_beam_penalty); }
+
+int64_t lo_sizeof_bracket_rule(void) { return (int64_t)sizeof(lo_bracket_rule); }
+
+int64_t lo_bracket_state_bytes(int B, int max_depth) {
+  if (B < 1 || max_depth < 1 || max_depth > 32) return 0;
+  return bracket_state_bytes(B, max_depth);
+}
+
+int lo_decoder_greedy_brackets(const lo_decoder_args* a, int64_t start_id, int64_t end_id, int max_steps, int64_t* tokens,
+                               int32_t* finished, int32_t* fin_hist, const lo_bracket_rule* br, void* stream) {
+  LO_TRY(check_args(a));
+  LO_TRY(check_bracket_rule(br, a->V));
+  LO_TRY(check_reg_off(a, true));
+  LO_CHECK_ARG(!a->ss_prob, "scheduled sampling (ss_prob) is a training mode: greedy decode feeds its own argmax already");
+  TorchDecode f(a, start_id, finished, nullptr);
+  return greedy_loop(f, end_id, max_steps, tokens, fin_hist, (cudaStream_t)stream, ArgmaxChoice{}, br);
+}
+
+int lo_decoder_sample_brackets(const lo_decoder_args* a, const lo_sample_args* s, int64_t start_id, int64_t end_id, int max_steps,
+                               int64_t* tokens, int32_t* finished, int32_t* fin_hist, const lo_bracket_rule* br, void* stream) {
+  LO_TRY(check_decoder_sample(a, s));
+  LO_TRY(check_bracket_rule(br, a->V));
+  TorchDecode f(a, start_id, finished, nullptr);
+  return sample_loop(f, s, end_id, max_steps, tokens, fin_hist, (cudaStream_t)stream, br);
+}
+
+int lo_decoder_beam_brackets(const lo_decoder_args* a, int64_t start_id, int64_t end_id, int max_steps, int64_t* ids, int64_t* parents,
+                             int32_t* fin_hist, float* logp, float div_gamma, float div_prob, const float* div_u,
+                             const uint64_t* div_state, const lo_beam_penalty* pen, const lo_bracket_rule* br, void* stream) {
+  const BeamArgs bm{0, div_gamma, div_prob, div_u, div_state, pen};
+  LO_CHECK_ARG(a, "null args");
+  LO_TRY(check_bracket_rule(br, a->V));
+  if (pen) LO_TRY(check_beam_penalty(pen, a->rows_per_img, a->V, bm.div_on()));
+  return decoder_beam(a, start_id, end_id, max_steps, ids, parents, fin_hist, logp, bm, br, stream);
+}
 
 int lo_beam_backtrack(const int64_t* ids, const int64_t* parents, int64_t ids_stride_steps, int n_img, int beam, int n,
                       const float* alphas, int64_t alpha_row_stride, int R, const int32_t* reg_off, const int32_t* reg_off_host,

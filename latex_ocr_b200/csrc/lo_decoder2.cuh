@@ -124,7 +124,38 @@ int lo_decoder2_beam(const lo_decoder_args* a, const lo_decoder2_layer* l2, int6
   const BeamArgs bm{0, div_gamma, div_prob, div_u, div_state, pen};
   LO_TRY(check_decoder2(a, l2));
   if (pen) LO_TRY(check_beam_penalty(pen, a->rows_per_img, a->V, bm.div_on()));
-  return decoder_beam<TwoLayerDecode>(a, start_id, end_id, max_steps, ids, parents, fin_hist, logp, bm, stream, l2);
+  return decoder_beam<TwoLayerDecode>(a, start_id, end_id, max_steps, ids, parents, fin_hist, logp, bm, nullptr, stream, l2);
+}
+
+int lo_decoder2_greedy_brackets(const lo_decoder_args* a, const lo_decoder2_layer* l2, int64_t start_id, int64_t end_id, int max_steps,
+                                int64_t* tokens, int32_t* finished, int32_t* fin_hist, const lo_bracket_rule* br, void* stream) {
+  LO_TRY(check_decoder2(a, l2));
+  LO_TRY(check_args(a));
+  LO_TRY(check_bracket_rule(br, a->V));
+  LO_TRY(check_reg_off(a, true));
+  TwoLayerDecode f(a, start_id, finished, nullptr, l2);
+  return greedy_loop(f, end_id, max_steps, tokens, fin_hist, (cudaStream_t)stream, ArgmaxChoice{}, br);
+}
+
+int lo_decoder2_sample_brackets(const lo_decoder_args* a, const lo_decoder2_layer* l2, const lo_sample_args* s, int64_t start_id,
+                                int64_t end_id, int max_steps, int64_t* tokens, int32_t* finished, int32_t* fin_hist,
+                                const lo_bracket_rule* br, void* stream) {
+  LO_TRY(check_decoder2(a, l2));
+  LO_TRY(check_decoder_sample(a, s));
+  LO_TRY(check_bracket_rule(br, a->V));
+  TwoLayerDecode f(a, start_id, finished, nullptr, l2);
+  return sample_loop(f, s, end_id, max_steps, tokens, fin_hist, (cudaStream_t)stream, br);
+}
+
+int lo_decoder2_beam_brackets(const lo_decoder_args* a, const lo_decoder2_layer* l2, int64_t start_id, int64_t end_id, int max_steps,
+                              int64_t* ids, int64_t* parents, int32_t* fin_hist, float* logp, float div_gamma, float div_prob,
+                              const float* div_u, const uint64_t* div_state, const lo_beam_penalty* pen, const lo_bracket_rule* br,
+                              void* stream) {
+  const BeamArgs bm{0, div_gamma, div_prob, div_u, div_state, pen};
+  LO_TRY(check_decoder2(a, l2));
+  LO_TRY(check_bracket_rule(br, a->V));
+  if (pen) LO_TRY(check_beam_penalty(pen, a->rows_per_img, a->V, bm.div_on()));
+  return decoder_beam<TwoLayerDecode>(a, start_id, end_id, max_steps, ids, parents, fin_hist, logp, bm, br, stream, l2);
 }
 
 }  // extern "C"

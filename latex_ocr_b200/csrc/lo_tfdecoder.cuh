@@ -811,4 +811,36 @@ int lo_tfdec_beam_pen(const lo_tfdec_args* a, int64_t end_id, int max_steps, int
                    (cudaStream_t)stream);
 }
 
+int lo_tfdec_greedy_brackets(const lo_tfdec_args* a, int64_t end_id, int max_steps, int64_t* tokens, int32_t* fin_hist,
+                             const lo_bracket_rule* br, void* stream) {
+  LO_CHECK_ARG(a, "null args");
+  LO_TRY(check_bracket_rule(br, a->V));
+  LO_TRY(tf_check(a, true));
+  TfDecode f(a);
+  return greedy_loop(f, end_id, max_steps, tokens, fin_hist, (cudaStream_t)stream, ArgmaxChoice{}, br);
+}
+
+int lo_tfdec_sample_brackets(const lo_tfdec_args* a, const lo_sample_args* s, int64_t end_id, int max_steps, int64_t* tokens,
+                             int32_t* fin_hist, const lo_bracket_rule* br, void* stream) {
+  LO_CHECK_ARG(a, "null args");
+  LO_TRY(check_sample(s, a->V, a->rows_per_img));
+  LO_TRY(check_bracket_rule(br, a->V));
+  LO_TRY(tf_check(a, true));
+  TfDecode f(a);
+  return sample_loop(f, s, end_id, max_steps, tokens, fin_hist, (cudaStream_t)stream, br);
+}
+
+int lo_tfdec_beam_brackets(const lo_tfdec_args* a, int64_t end_id, int max_steps, int64_t* ids, int64_t* parents, int32_t* fin_hist,
+                           float* logp, float div_gamma, float div_prob, const float* div_u, const uint64_t* div_state,
+                           const lo_beam_penalty* pen, const lo_bracket_rule* br, void* stream) {
+  LO_CHECK_ARG(a, "null args");
+  const BeamArgs bm0{0, div_gamma, div_prob, div_u, div_state, pen};
+  LO_TRY(check_bracket_rule(br, a->V));
+  if (pen) LO_TRY(check_beam_penalty(pen, a->rows_per_img, a->V, bm0.div_on()));
+  LO_TRY(tf_check(a, true));
+  TfDecode f(a);
+  return beam_loop(f, BeamArgs{f.d.rpi, div_gamma, div_prob, div_u, div_state, pen}, end_id, max_steps, ids, parents, fin_hist, logp,
+                   (cudaStream_t)stream, br);
+}
+
 }  // extern "C"

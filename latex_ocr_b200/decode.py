@@ -149,6 +149,120 @@ def beam_hypotheses(ids, parents, finalize, a=None, alphas=None):
     return out, att
 
 
+class BracketRule:
+    """Balanced brackets in decode (lo_bracket_rule): ``role[v]`` is 0 for a neutral token, +k for a token that opens kind k and
+    -k for one that closes it.  Under a rule every greedy and sampled formula, and every beam hypothesis under
+    ``finalize='backtrack'``, cut at its first END, nests the kinds properly, at most ``max_depth`` deep, and leaves none open
+    (``check`` tells whether a sequence does).  The decode masks on the device, between the head and the token choice; the
+    probabilities are the model's restricted to the allowed tokens.
+
+    ``role``: V ints, each kind 1..n_kinds with at least one opening and one closing token (n_kinds = max |role|, at most 255);
+    ``max_depth``: 1..32.  A table without kinds (all neutral) is accepted and changes nothing."""
+
+    def __init__(self, role, max_depth=16):
+        role = [int(r) for r in role]
+        if not role:
+            raise ValueError("empty role table")
+        if not 1 <= int(max_depth) <= 32:
+            raise ValueError("max_depth must lie in 1..32 (got %r)" % (max_depth,))
+        bad = [v for v, r in enumerate(role) if not -255 <= r <= 255]
+        if bad:
+            raise ValueError("role of token %d out of range -255..255 (got %d)" % (bad[0], role[bad[0]]))
+        self.n_kinds = max(abs(r) for r in role)
+        for k in range(1, self.n_kinds + 1):
+            if k not in role or -k not in role:
+                raise ValueError("kind %d has no %s token" % (k, "opening" if k not in role else "closing"))
+        self.role = role
+        self.max_depth = int(max_depth)
+        self._dev = {}
+
+    @classmethod
+    def latex(cls, id_to_tok, max_depth=16):
+        """The rule of LaTeX formulas over a vocabulary (``id_to_tok``: a dict id -> token or a list): ``{`` / ``}`` are kind 1;
+        every ``\\left`` + delimiter token (the character after ``\\left`` is not a letter, so ``\\leftarrow`` stays neutral) opens
+        kind 2 and every ``\\right`` + delimiter token closes it, in any pairing (``\\left( ... \\right.`` is valid LaTeX); each
+        ``\\begin{X}`` / ``\\end{X}`` pair of the vocabulary is a kind of its own (either without the other stays neutral).
+        Everything else is neutral, ``\\{``, ``\\}``, parentheses and square brackets included."""
+        toks = dict(id_to_tok) if isinstance(id_to_tok, dict) else dict(enumerate(id_to_tok))
+        role = [0] * (max(toks) + 1)
+
+        def delim(tok, cmd):
+            return tok.startswith(cmd) and len(tok) > len(cmd) and not tok[len(cmd)].isalpha()
+
+        def env(tok, cmd):
+            return tok[len(cmd):-1] if tok.startswith(cmd) and tok.endswith("}") else None
+        pairs = [([i for i, t in toks.items() if t == "{"], [i for i, t in toks.items() if t == "}"]),
+                 ([i for i, t in toks.items() if delim(t, "\\left")], [i for i, t in toks.items() if delim(t, "\\right")])]
+        for name in sorted({env(t, "\\begin{") for t in toks.values()} - {None}):
+            pairs.append(([i for i, t in toks.items() if env(t, "\\begin{") == name],
+                          [i for i, t in toks.items() if env(t, "\\end{") == name]))
+        kind = 0
+        for opens, closes in pairs:            # kinds in this order, a pair missing either side stays neutral
+            if opens and closes:
+                kind += 1
+                for i in opens:
+                    role[i] = kind
+                for i in closes:
+                    role[i] = -kind
+        return cls(role, max_depth)
+
+    def check(self, ids, end_id):
+        """For every sequence of ``ids`` (a [..., steps] tensor or array, or a list of sequences), cut at its first ``end_id``:
+        whether it nests properly, at most max_depth deep, and leaves no bracket open.  Returns a list of bools."""
+        if torch.is_tensor(ids) or hasattr(ids, "shape"):
+            t = torch.as_tensor(ids)
+            seqs = t.reshape(-1, t.shape[-1]).tolist() if t.dim() >= 1 and t.numel() else []
+        else:
+            seqs = [list(s) for s in ids]
+        end_id, V = int(end_id), len(self.role)
+        out = []
+        for seq in seqs:
+            stack, ok = [], True
+            for tok in seq:
+                tok = int(tok)
+                if tok == end_id:
+                    break
+                r = self.role[tok] if 0 <= tok < V else 0
+                if r > 0:
+                    stack.append(r)
+                    ok = len(stack) <= self.max_depth
+                elif r < 0:
+                    ok = bool(stack) and stack.pop() == -r
+                if not ok:
+                    break
+            out.append(ok and not stack)
+        return out
+
+    def device_role(self, device):
+        """The role table as an int32 tensor on ``device``, copied once per device."""
+        device = torch.device(device)
+        if device not in self._dev:
+            self._dev[device] = torch.tensor(self.role, dtype=torch.int32, device=device)
+        return self._dev[device]
+
+    def allowed_at_start(self, end_id, max_steps):
+        """The tokens a row may take at step 0 of a call of ``max_steps`` steps (depth 0): END, neutral tokens and, with a step
+        left to close them, opening ones."""
+        return sum(1 for v, r in enumerate(self.role) if v == end_id or r == 0 or (r > 0 and max_steps >= 2))
+
+    def args(self, end_id, V, B, max_steps, device, beam=1):
+        """The lo_bracket_rule of a decode of B rows over V tokens and the tensors it points at, which must outlive the call.
+        Refuses (ValueError) a table of another size than V, a non-neutral END and, for beam search, fewer tokens allowed at step 0
+        than ``beam``."""
+        if len(self.role) != V:
+            raise ValueError("the rule's role table has %d entries, the model %d tokens" % (len(self.role), V))
+        if not 0 <= int(end_id) < V or self.role[int(end_id)] != 0:
+            raise ValueError("END (id %d) must be a neutral token of the rule" % int(end_id))
+        if self.allowed_at_start(int(end_id), max_steps) < beam:
+            raise ValueError("only %d tokens are allowed at step 0 under the rule: fewer than beam_size %d"
+                             % (self.allowed_at_start(int(end_id), max_steps), beam))
+        role = self.device_role(device)
+        state = torch.empty(int(_lib.lib().lo_bracket_state_bytes(B, self.max_depth)), dtype=torch.uint8, device=device)
+        br = _lib.BracketRule()
+        br.role, br.n_kinds, br.max_depth, br.state = role.data_ptr(), max(self.n_kinds, 1), self.max_depth, state.data_ptr()
+        return br, (role, state)
+
+
 def _image(x):
     """one image of a list: [1,H,W] tensor (uint8 or float) on the CPU or the GPU"""
     t = x if torch.is_tensor(x) else torch.from_numpy(x).permute(2, 0, 1)      # HxWx1 array -> [1,H,W]
@@ -250,31 +364,57 @@ def _inverse(order):
     return torch.tensor(inv, dtype=torch.int64)
 
 
-def _greedy_entry(a, *args):
+def _greedy_entry(a, *args, br=None):
+    if br is not None:
+        return _lib.lib().lo_decoder_greedy_brackets(ctypes.byref(a), *args[:-1], ctypes.byref(br), args[-1])
     return _lib.lib().lo_decoder_greedy_hist(ctypes.byref(a), *args)
 
 
-def _beam_entry(a, pen, *args):
+def _beam_entry(a, pen, *args, br=None):
     L = _lib.lib()
+    if br is not None:
+        return L.lo_decoder_beam_brackets(ctypes.byref(a), *args[:-1], ctypes.byref(pen) if pen is not None else None,
+                                          ctypes.byref(br), args[-1])
     if pen is not None:
         return L.lo_decoder_beam_pen(ctypes.byref(a), *args[:-1], ctypes.byref(pen), args[-1])
     return L.lo_decoder_beam_div(ctypes.byref(a), *args)
 
 
-def greedy_decode(model, img, start_id, end_id, max_length_formula=150, return_attention=False, _encode=None, _entry=_greedy_entry):
+def bracket_args(brackets, end_id, V, B, max_steps, device, beam=1):
+    """(lo_bracket_rule or None, tensors to keep alive) of a decode under ``brackets`` (a BracketRule or None)."""
+    if brackets is None:
+        return None, None
+    if not isinstance(brackets, BracketRule):
+        raise TypeError("brackets must be a decode.BracketRule (got %s)" % type(brackets).__name__)
+    return brackets.args(end_id, V, B, max_steps, device, beam)
+
+
+def refuse_reference_finalize(brackets, finalize):
+    """A bracket rule holds along hypothesis lineages only: 'reference' finalize (slot s of every step) is refused with it."""
+    if brackets is not None and finalize != "backtrack":
+        raise ValueError("a bracket rule needs finalize='backtrack': 'reference' returns slot s of every step, not a hypothesis's "
+                         "lineage, so its sequences need not nest")
+
+
+def greedy_decode(model, img, start_id, end_id, max_length_formula=150, return_attention=False, brackets=None, _encode=None,
+                  _entry=_greedy_entry):
     """Returns token ids [N, steps] (CPU int64), steps as the reference's loop would have run.  ``return_attention=True`` also
     returns the attention weights of every step, [N, steps, R] fp32 on the CPU — what the reference collects in
     ``attention_mechanism.ctx_vector`` for visualize_attention.py (attention_mechanism.py:96-121).  For a list of images the ids
     are in input order and the attention weights are a list of [steps, R_i] tensors, R_i the image's own region count.
 
-    ``_encode`` (see encode_packed) and ``_entry(args, start_id, end_id, max_steps, tokens, finished, fin_hist, stream)``, the
-    library call, let ext.greedy_decode run the two-layer decoder through this body."""
+    ``brackets``: a BracketRule, under which every formula nests its brackets and closes them (lo_decoder_greedy_brackets).
+
+    ``_encode`` (see encode_packed) and ``_entry(args, start_id, end_id, max_steps, tokens, finished, fin_hist, stream, br=None)``,
+    the library call, let ext.greedy_decode run the two-layer decoder through this body."""
     max_steps = max_length_formula + 2
     with torch.no_grad():
         a, ws, N, lay = _prepare(model, img, 1, max_steps, _encode)
         finished = torch.zeros(N, dtype=torch.int32, device=model.device)
+        br, keep = bracket_args(brackets, end_id, a.V, a.B, max_steps, model.device)
+        kw = {"br": br} if br is not None else {}
         ids = run_greedy(lambda tokens, hist: _entry(a, int(start_id), int(end_id), max_steps, tokens, finished.data_ptr(), hist,
-                                                     stream_ptr()),
+                                                     stream_ptr(), **kw),
                          N, max_steps, model.device).cpu()
         n = ids.shape[1]
         if lay is None:
@@ -297,7 +437,7 @@ def attention_maps(alphas, att_h, att_w):
 
 def beam_decode(model, img, start_id, end_id, beam_size=5, max_length_formula=150, finalize="reference",
                 div_gamma=1, div_prob=0, div_u=None, div_seed=None, return_attention=False, length_penalty=0.0,
-                coverage_penalty=0.0, return_scores=False, _encode=None, _entry=_beam_entry):
+                coverage_penalty=0.0, return_scores=False, brackets=None, _encode=None, _entry=_beam_entry):
     """Returns (ids [N, beam, steps], log_probs [N, beam]) on the CPU; hypothesis 0 is the one the reference scores
     (img2seq.py:210).  ``div_gamma`` / ``div_prob``: the diversity penalty of beam_search_decoder_cell.py:258-287 (off when
     gamma == 1 or prob == 0, as in configs/model.json:15-16); its Bernoulli draws come from the in-kernel Philox stream seeded
@@ -315,11 +455,15 @@ def beam_decode(model, img, start_id, end_id, beam_size=5, max_length_formula=15
     stay the raw sums; ``return_scores=True`` also returns the ranking scores [N, beam] (CPU), after the log-probs and before the
     attention weights.
 
+    ``brackets``: a BracketRule (lo_decoder_beam_brackets): the search runs on the log-probs restricted to the tokens the rule
+    allows, and every hypothesis nests its brackets and closes them.  It needs ``finalize='backtrack'`` (ValueError otherwise).
+
     ``_encode`` (see encode_packed) and ``_entry(args, penalty or None, start_id, end_id, max_steps, ids, parents, fin_hist, logp,
-    div_gamma, div_prob, div_u, div_state, stream)``, the library call, let ext.beam_decode run the two-layer decoder through this
-    body."""
+    div_gamma, div_prob, div_u, div_state, stream, br=None)``, the library call, let ext.beam_decode run the two-layer decoder
+    through this body."""
     if finalize not in ("reference", "backtrack"):
         raise NotImplementedError("finalize must be 'reference' or 'backtrack'")
+    refuse_reference_finalize(brackets, finalize)
     alpha, beta = penalty_weights(length_penalty, coverage_penalty)
     max_steps = max_length_formula + 2
     with torch.no_grad():
@@ -334,10 +478,12 @@ def beam_decode(model, img, start_id, end_id, beam_size=5, max_length_formula=15
         pen = None
         if alpha != 0 or beta > 0 or return_scores:
             pen, pen_t = beam_penalty(alpha, beta, a.B, a.R, max_steps, beam_size, dev)
+        br, keep = bracket_args(brackets, end_id, a.V, a.B, max_steps, dev, beam_size)
+        kw = {"br": br} if br is not None else {}
 
         def call(ids, parents, hist, logp, u):
             return _entry(a, pen, int(start_id), int(end_id), max_steps, ids, parents, hist, logp, float(div_gamma), float(div_prob), u,
-                          state.data_ptr() if state is not None else None, stream_ptr())
+                          state.data_ptr() if state is not None else None, stream_ptr(), **kw)
         ids, parents, logp = run_beam(call, N, beam_size, max_steps, a.V, dev, div_u if div_on else None,
                                       lay.order if lay else None)
         scores = pen_t["scores"].cpu() if return_scores else None
@@ -406,12 +552,14 @@ def run_sample(call, N, n, steps, tau, top_k, top_p, V, state, device, u=None, o
     return ids.reshape(N, n, -1), logp.view(N, n)
 
 
-def _sample_entry(a, s, *args):
+def _sample_entry(a, s, *args, br=None):
+    if br is not None:
+        return _lib.lib().lo_decoder_sample_brackets(ctypes.byref(a), ctypes.byref(s), *args[:-1], ctypes.byref(br), args[-1])
     return _lib.lib().lo_decoder_sample(ctypes.byref(a), ctypes.byref(s), *args)
 
 
 def sample_decode(model, img, start_id, end_id, n_samples=8, temperature=1.0, top_k=0, top_p=1.0, max_length_formula=150,
-                  seed=None, u=None, return_attention=False, _encode=None, _entry=_sample_entry):
+                  seed=None, u=None, return_attention=False, brackets=None, _encode=None, _entry=_sample_entry):
     """Draws ``n_samples`` formulas per image (lo_decoder_sample): every step's token is a draw from softmax(logits /
     ``temperature``), restricted to the ``top_k`` most probable tokens (0: all) and to the smallest prefix of them, by probability,
     whose mass reaches ``top_p`` (1: all).  ``top_k = 1`` is greedy decode.  A sample ends at its first END (later positions hold
@@ -427,8 +575,12 @@ def sample_decode(model, img, start_id, end_id, n_samples=8, temperature=1.0, to
     n_samples, V] in (0, 1), image i drawing the rows [i * n_samples, (i + 1) * n_samples).  ``mbr_select`` picks one sample per
     image from the result.
 
+    ``brackets``: a BracketRule (lo_decoder_sample_brackets): the draws come from the model's distribution restricted to the
+    tokens the rule allows (temperature, top_k and top_p act on it, and log_probs are restricted log-likelihoods), and every sample
+    nests its brackets and closes them.
+
     ``_encode`` (see encode_packed) and ``_entry(args, sample_args, start_id, end_id, max_steps, tokens, finished, fin_hist,
-    stream)``, the library call, let ext.sample_decode run the two-layer decoder through this body."""
+    stream, br=None)``, the library call, let ext.sample_decode run the two-layer decoder through this body."""
     n, tau, k, p = sampling_settings(n_samples, temperature, top_k, top_p, model.decoder.vocab_size)
     max_steps = max_length_formula + 2
     with torch.no_grad():
@@ -436,9 +588,11 @@ def sample_decode(model, img, start_id, end_id, n_samples=8, temperature=1.0, to
         state = sample_state(model, seed, dev) if u is None else None
         a, ws, N, lay = _prepare(model, img, n, max_steps, _encode)
         finished = torch.zeros(a.B, dtype=torch.int32, device=dev)
+        br, keep = bracket_args(brackets, end_id, a.V, a.B, max_steps, dev)
+        kw = {"br": br} if br is not None else {}
 
         def call(s, tokens, hist):
-            return _entry(a, s, int(start_id), int(end_id), max_steps, tokens, finished.data_ptr(), hist, stream_ptr())
+            return _entry(a, s, int(start_id), int(end_id), max_steps, tokens, finished.data_ptr(), hist, stream_ptr(), **kw)
         ids, logp = run_sample(call, N, n, max_steps, tau, k, p, a.V, state, dev, u, lay.order if lay else None)
         ids, logp = ids.cpu(), logp.cpu()
         steps = ids.shape[2]

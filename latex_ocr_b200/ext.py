@@ -383,32 +383,41 @@ def _row_encode(model):
     return model.row_encoder.forward_raw
 
 
-def greedy_decode(model, img, start_id, end_id, max_length_formula=150, return_attention=False):
+def greedy_decode(model, img, start_id, end_id, max_length_formula=150, return_attention=False, brackets=None):
     """Greedy decode of an Img2SeqRowModel: CNN -> row encoder -> two-layer decoder (layer 2 over h1_t, logits = fc(h2_t)) in one
     CUDA time loop (lo_decoder2_greedy).  Arguments, outputs and loop rules are those of decode.greedy_decode: ``img`` a batch
-    tensor or a list of images of different sizes, the attention weights of layer 1 with ``return_attention``."""
-    def entry(a, *args):
+    tensor or a list of images of different sizes, the attention weights of layer 1 with ``return_attention``, a
+    decode.BracketRule with ``brackets`` (lo_decoder2_greedy_brackets)."""
+    def entry(a, *args, br=None):
         l2 = model.layer2.decode_layer(a)
+        if br is not None:
+            return _lib.lib().lo_decoder2_greedy_brackets(ctypes.byref(a), ctypes.byref(l2), *args[:-1], ctypes.byref(br), args[-1])
         return _lib.lib().lo_decoder2_greedy(ctypes.byref(a), ctypes.byref(l2), *args)
-    return decode.greedy_decode(model, img, start_id, end_id, max_length_formula, return_attention, _encode=_row_encode(model),
-                                _entry=entry)
+    return decode.greedy_decode(model, img, start_id, end_id, max_length_formula, return_attention, brackets,
+                                _encode=_row_encode(model), _entry=entry)
 
 
 def beam_decode(model, img, start_id, end_id, beam_size=5, **kw):
     """Beam search of an Img2SeqRowModel through the row encoder and the two-layer decoder (lo_decoder2_beam).  Keywords and return
     values are those of decode.beam_decode: max_length_formula, finalize, div_gamma / div_prob / div_u / div_seed,
-    length_penalty / coverage_penalty, return_scores, return_attention."""
-    def entry(a, pen, *args):
+    length_penalty / coverage_penalty, return_scores, return_attention, brackets (lo_decoder2_beam_brackets)."""
+    def entry(a, pen, *args, br=None):
         l2 = model.layer2.decode_layer(a)
-        return _lib.lib().lo_decoder2_beam(ctypes.byref(a), ctypes.byref(l2), *args[:-1],
-                                           ctypes.byref(pen) if pen is not None else None, args[-1])
+        p = ctypes.byref(pen) if pen is not None else None
+        if br is not None:
+            return _lib.lib().lo_decoder2_beam_brackets(ctypes.byref(a), ctypes.byref(l2), *args[:-1], p, ctypes.byref(br), args[-1])
+        return _lib.lib().lo_decoder2_beam(ctypes.byref(a), ctypes.byref(l2), *args[:-1], p, args[-1])
     return decode.beam_decode(model, img, start_id, end_id, beam_size, _encode=_row_encode(model), _entry=entry, **kw)
 
 
 def sample_decode(model, img, start_id, end_id, n_samples=8, **kw):
     """Sampling decode of an Img2SeqRowModel through the row encoder and the two-layer decoder (lo_decoder2_sample).  Keywords and
-    return values are those of decode.sample_decode: temperature, top_k, top_p, max_length_formula, seed, u, return_attention."""
-    def entry(a, s, *args):
+    return values are those of decode.sample_decode: temperature, top_k, top_p, max_length_formula, seed, u, return_attention,
+    brackets (lo_decoder2_sample_brackets)."""
+    def entry(a, s, *args, br=None):
         l2 = model.layer2.decode_layer(a)
+        if br is not None:
+            return _lib.lib().lo_decoder2_sample_brackets(ctypes.byref(a), ctypes.byref(l2), ctypes.byref(s), *args[:-1],
+                                                          ctypes.byref(br), args[-1])
         return _lib.lib().lo_decoder2_sample(ctypes.byref(a), ctypes.byref(l2), ctypes.byref(s), *args)
     return decode.sample_decode(model, img, start_id, end_id, n_samples, _encode=_row_encode(model), _entry=entry, **kw)

@@ -22,6 +22,21 @@ from .encoder import EncoderCNN
 from .params import LRUCache, bind_grads
 
 
+def bracket_rule(config, vocab):
+    """The decode.BracketRule of ``config.balanced_brackets`` (default off: None), built once per vocabulary from its id_to_tok
+    table with BracketRule.latex and kept on the vocabulary."""
+    if not getattr(config, "balanced_brackets", False):
+        return None
+    from . import decode
+    if vocab is None or getattr(vocab, "id_to_tok", None) is None:
+        raise ValueError("balanced_brackets needs a vocabulary with an id_to_tok table")
+    rule = getattr(vocab, "_bracket_rule", None)
+    if rule is None:
+        rule = decode.BracketRule.latex(vocab.id_to_tok)
+        vocab._bracket_rule = rule
+    return rule
+
+
 class Img2SeqModel:
     def __init__(self, config, dir_output=None, vocab=None, device=None, precision=None, impl=None, n_tok=None):
         self._config = config
@@ -383,16 +398,19 @@ class Img2SeqModel:
         start_id = end_id - 1 if start_id is None else start_id          # default: the PAD id (no START in the torch flavour)
         L = int(getattr(self._config, "max_length_formula", 150))
         self.train_mode(False)
+        br = bracket_rule(self._config, self._vocab)
         if decoding == "greedy":
-            return [decode.greedy_decode(self, images, start_id, end_id, L).tolist()], end_id
+            return [decode.greedy_decode(self, images, start_id, end_id, L, brackets=br).tolist()], end_id
         if decoding != "beam_search" and decoding != "beam":
             raise NotImplementedError("decoding=%r: 'greedy' or 'beam_search' (model.json:13)" % (decoding,))
         beam = int(beam_size or getattr(self._config, "beam_size", 5))
+        # a bracket rule holds along lineages: with it on, the hypotheses are followed back from their final slots
+        kw = {"brackets": br, "finalize": "backtrack"} if br is not None else {}
         ids, _ = decode.beam_decode(self, images, start_id, end_id, beam, L,
                                     div_gamma=float(getattr(self._config, "div_gamma", 1)),
                                     div_prob=float(getattr(self._config, "div_prob", 0)),
                                     length_penalty=getattr(self._config, "length_penalty", 0) or 0,
-                                    coverage_penalty=getattr(self._config, "coverage_penalty", 0) or 0)
+                                    coverage_penalty=getattr(self._config, "coverage_penalty", 0) or 0, **kw)
         return [ids[:, k].tolist() for k in range(beam)], end_id
 
     def predict_batch(self, images, start_id=None, decoding=None, beam_size=None):

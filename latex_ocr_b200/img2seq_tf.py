@@ -285,7 +285,7 @@ class Img2SeqModel:
             l = ws["loss"].tolist()
             ce_words += l[0] * l[3]
             n_words += l[3]
-            ids = self.decoder.decode(enc).ids
+            ids = self.decoder.decode(enc, **self._decode_kw()).ids
             hyp0 = ids if ids.dim() == 2 else ids[:, :, 0]
             hyps += decode.truncate_end(hyp0.tolist(), self._vocab.id_end)
             refs += [list(map(int, f)) for f in formulas]
@@ -296,7 +296,14 @@ class Img2SeqModel:
     def predict_batch(self, images):
         """img2seq.py:256-275: list over hypotheses (1 for greedy, beam_size for beam search) of N token-id lists, truncated at END."""
         enc = self.encoder.forward_raw(self._to_device_images(images))
-        return self._format(self.decoder.decode(enc).ids)
+        return self._format(self.decoder.decode(enc, **self._decode_kw()).ids)
+
+    def _decode_kw(self):
+        """The decode keywords of ``config.balanced_brackets``: none when off; else the LaTeX bracket rule of the vocabulary and
+        lineage-consistent beam hypotheses (the rule holds along lineages)."""
+        from .img2seq import bracket_rule
+        br = bracket_rule(self._config, self._vocab)
+        return {} if br is None else {"brackets": br, "finalize": "backtrack"}
 
     def predict_images(self, images):
         """``predict_batch`` for a list of images of different sizes (HxWx1 uint8 arrays or [1,H,W] tensors), each decoded at its
@@ -322,7 +329,7 @@ class Img2SeqModel:
         steps = dec.max_length_formula + 2
         ws = dec.packed_workspace(lay.counts, steps)               # decode order: sorted by shape
         decode.encode_packed(self.encoder, lay, ws["enc"], self.device)
-        ids = dec.decode_packed(ws, steps).ids
+        ids = dec.decode_packed(ws, steps, **self._decode_kw()).ids
         return self._format(ids[decode._inverse(lay.order).to(ids.device)])
 
     def _format(self, ids):

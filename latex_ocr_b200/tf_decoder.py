@@ -358,10 +358,12 @@ class Decoder(nn.Module):
         return ws
 
     def decode_packed(self, ws, steps, div_u=None, return_attention=False, return_log_probs=False, finalize="reference",
-                      return_scores=False):
+                      return_scores=False, brackets=None):
         """decode() over the images packed in ``ws`` by packed_workspace: every image attends over its own regions only."""
         if finalize not in ("reference", "backtrack"):
             raise NotImplementedError("finalize must be 'reference' or 'backtrack'")
+        if self.decoding != "greedy":
+            decode.refuse_reference_finalize(brackets, finalize)
         counts = ws["counts"]
         N, beam = len(counts), self._tiles
         R = max(counts)
@@ -370,7 +372,7 @@ class Decoder(nn.Module):
             L, ws, a = self._args(ws["enc"], N * beam, steps, R, rows_per_img=beam, ws=ws)
             decode.set_region_offsets(a, ws["reg_off_host"], ws["reg_off"], ws["off"])
             alphas = ws["alphas"][:N * beam * steps * R].view(N * beam, steps, R) if return_attention else None
-            out = self._run_decode(L, a, N, steps, div_u, alphas, return_log_probs, finalize, return_scores)
+            out = self._run_decode(L, a, N, steps, div_u, alphas, return_log_probs, finalize, return_scores, brackets)
             if alphas is None:
                 return out
             att = out[-1]
@@ -379,7 +381,7 @@ class Decoder(nn.Module):
             return out[:-1] + ([att[i, :, :, :counts[i]].clone() for i in range(N)],)
 
     def decode(self, enc, max_steps=None, div_u=None, return_attention=False, return_log_probs=False, finalize="reference",
-               return_scores=False):
+               return_scores=False, brackets=None):
         """dynamic_decode(decoder_cell, max_length_formula + 1) (decoder.py:70): at most max_length_formula + 2 steps, stops when
         every row / beam has emitted END.  Returns DecoderOutput(logits=None, ids).  ``div_u`` (tests): injected uniforms
         [steps, N*beam, V] for the diversity penalty; ``return_log_probs`` (beam search): also the log-probs of the hypotheses
@@ -397,9 +399,14 @@ class Decoder(nn.Module):
         the list is decoded in one time loop in which every image attends over its own regions only (lo_tfdec_args.reg_off), so
         an image's ids do not depend on the other images of the call.  Ids come back in input order, image i draws the rows
         [i*beam, (i+1)*beam) of ``div_u``, and ``return_attention`` gives a list of [steps, R_i] (greedy) or [beam, steps, R_i]
-        tensors."""
+        tensors.
+
+        ``brackets``: a decode.BracketRule (lo_tfdec_greedy_brackets / lo_tfdec_beam_brackets): every formula, and every beam
+        hypothesis under ``finalize='backtrack'``, nests its brackets and closes them; beam search refuses it with 'reference'."""
         if finalize not in ("reference", "backtrack"):
             raise NotImplementedError("finalize must be 'reference' or 'backtrack'")
+        if self.decoding != "greedy":
+            decode.refuse_reference_finalize(brackets, finalize)
         steps = int(max_steps) if max_steps is not None else self.max_length_formula + 2
         if isinstance(enc, (list, tuple)):
             encs = [self._enc_regions(e) for e in enc]
@@ -407,7 +414,7 @@ class Decoder(nn.Module):
             off = ws["off"]
             for i, e in enumerate(encs):
                 ws["enc"][off[i]:off[i + 1]].copy_(e)
-            return self.decode_packed(ws, steps, div_u, return_attention, return_log_probs, finalize, return_scores)
+            return self.decode_packed(ws, steps, div_u, return_attention, return_log_probs, finalize, return_scores, brackets)
         enc = self._enc(enc)
         N, R, _ = enc.shape
         self.store.refresh_shadow()
@@ -415,17 +422,18 @@ class Decoder(nn.Module):
             L, ws, a = self._args(enc, N * self._tiles, steps, R, rows_per_img=self._tiles, decode=True)
             ws["enc"] = enc
             return self._run_decode(L, a, N, steps, div_u, ws["alphas"] if return_attention else None, return_log_probs, finalize,
-                                    return_scores)
+                                    return_scores, brackets)
 
     def sample(self, enc, n_samples=8, temperature=1.0, top_k=0, top_p=1.0, max_steps=None, u=None, seed=None,
-               return_attention=False):
+               return_attention=False, brackets=None):
         """Sampling decode (lo_tfdec_sample): ``n_samples`` formulas per image, each step's token drawn from softmax(logits /
         ``temperature``) restricted by ``top_k`` / ``top_p``, as decode.sample_decode documents.  ``enc`` as in decode(): a batch
         [N,R,C] / [N,H,W,C] or a list of the encoder outputs of images of different sizes.  Returns (ids [N, n_samples, steps],
         log_probs [N, n_samples]) on the device, ids in input order, and with ``return_attention`` the attention weights [N,
         n_samples, steps, R] (a list of [n_samples, steps, R_i] for a list).  ``seed``: a new Philox stream at that seed, else the
         decoder's own, which every call advances; ``u`` (tests): injected uniforms [steps, N * n_samples, V], image i drawing the
-        rows [i * n_samples, (i + 1) * n_samples)."""
+        rows [i * n_samples, (i + 1) * n_samples).  ``brackets``: a decode.BracketRule (lo_tfdec_sample_brackets), as
+        decode.sample_decode documents."""
         n, tau, k, p = decode.sampling_settings(n_samples, temperature, top_k, top_p, self.V)
         steps = int(max_steps) if max_steps is not None else self.max_length_formula + 2
         dev = self.store.device
@@ -452,7 +460,12 @@ class Decoder(nn.Module):
                 L, ws, a = self._args(ws["enc"], N * n, steps, R, rows_per_img=n, ws=ws)
                 decode.set_region_offsets(a, ws["reg_off_host"], ws["reg_off"], ws["off"])
 
+            br, keep = decode.bracket_args(brackets, self._id_end, self.V, a.B, steps, dev)
+
             def call(s, tokens, fin):
+                if br is not None:
+                    return L.lo_tfdec_sample_brackets(ctypes.byref(a), ctypes.byref(s), self._id_end, steps, tokens, fin,
+                                                      ctypes.byref(br), stream_ptr())
                 return L.lo_tfdec_sample(ctypes.byref(a), ctypes.byref(s), self._id_end, steps, tokens, fin, stream_ptr())
             ids, logp = decode.run_sample(call, N, n, steps, tau, k, p, self.V, state, dev, u)
             if not return_attention:
@@ -472,13 +485,18 @@ class Decoder(nn.Module):
             raise ValueError("each image's encoder output must be [H,W,%d] or [R,%d] (got shape %s)" % (self.C, self.C, tuple(e.shape)))
         return e
 
-    def _run_decode(self, L, a, N, steps, div_u, alphas, return_log_probs, finalize="reference", return_scores=False):
+    def _run_decode(self, L, a, N, steps, div_u, alphas, return_log_probs, finalize="reference", return_scores=False,
+                    brackets=None):
         """The greedy or beam decode of the filled args ``a`` (N images); ``alphas``: the attention rows [B, steps, R] of the call
-        (attention export) or None."""
+        (attention export) or None; ``brackets``: a decode.BracketRule or None."""
         dev = self.store.device
+        br, keep = decode.bracket_args(brackets, self._id_end, self.V, a.B, steps, dev, self._tiles)
         if self.decoding == "greedy":
-            ids = decode.run_greedy(lambda tokens, fin: L.lo_tfdec_greedy(ctypes.byref(a), self._id_end, steps, tokens, fin,
-                                                                          stream_ptr()), N, steps, dev)
+            def greedy(tokens, fin):
+                if br is not None:
+                    return L.lo_tfdec_greedy_brackets(ctypes.byref(a), self._id_end, steps, tokens, fin, ctypes.byref(br), stream_ptr())
+                return L.lo_tfdec_greedy(ctypes.byref(a), self._id_end, steps, tokens, fin, stream_ptr())
+            ids = decode.run_greedy(greedy, N, steps, dev)
             if alphas is not None:
                 return DecoderOutput(None, ids), alphas[:, :ids.shape[1]].float().clone()
             return DecoderOutput(None, ids)
@@ -497,6 +515,8 @@ class Decoder(nn.Module):
 
         def call(ids, parents, fin, logp, u):
             args = (ctypes.byref(a), self._id_end, steps, ids, parents, fin, logp, self.div_gamma, self.div_prob, u, state)
+            if br is not None:
+                return L.lo_tfdec_beam_brackets(*args, ctypes.byref(pen) if pen is not None else None, ctypes.byref(br), stream_ptr())
             if pen is not None:
                 return L.lo_tfdec_beam_pen(*args, ctypes.byref(pen), stream_ptr())
             return L.lo_tfdec_beam_div(*args, stream_ptr())
